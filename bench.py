@@ -2,6 +2,7 @@
 """bench.py -- FNO rollout steps/sec on 64x64 cavity fields (BASELINE.json metric).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--batch B] [--act bf16|f32]
+                    [--dump-outputs DIR]
 
 One "step" = one `generate()` of the whole per-GPU batch (one autoregressive rollout step,
 SURVEY.md 8d).  N=1 workload = BASELINE.json configs[1]: cavity (p=5), batch 256, hidden activations
@@ -11,9 +12,14 @@ data-path collective ("weak" scaling); value = N*K / max-over-ranks time.
 
 The printed JSON line carries, besides the contract keys: "e2e" (public API, HOST buffers, H2D+D2H inside
 the timed region every step), "roofline" (dominant kernel, algorithmic bytes / CUDA-event duration /
-measured HBM peak), "kernels" (per-kernel mean durations from a second, event-bracketed pass),
+HBM data-sheet peak), "kernels" (per-kernel mean durations from a second, event-bracketed pass),
 "cpu_baseline" (oracle torch port = the reference's own library calls, timed on this host's cores),
 "rel_l2" (per-step relative L2 vs the fp32 CPU oracle on identical inputs) and "clocks".
+
+--dump-outputs DIR writes, after the timed steps, the predictions of the last timed step of each storage mode (what
+generate_many returned for it) as DIR/<name>.npy (float32, 8 MB each at B=256).  Both files together stay within 64 MB:
+from B=1024 on, each holds a fixed sample of the batch (the same seeded choice of samples in every run, in batch order).
+Inputs and weights are seeded, so two builds run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -37,34 +43,23 @@ sys.path.insert(0, ROOT)
 
 from cfdbench_b200 import dp, synth  # noqa: E402
 
-# roofline.traffic = dram__bytes_read.sum + dram__bytes_write.sum of ONE launch of the dominant kernel, read at run
-# time from the committed summary of the `ncu --set full` capture (profiles/ncu_traffic.json, written by
-# tools/summarize_profiles.py from the .ncu-rep).  Keyed by kernel name, activation storage and batch: if the kernel was
-# renamed / the workload changed since the capture, the lookup fails and traffic is reported as null with the reason.
-def ncu_traffic(kernel: str, act: str, batch: int):
-    path = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-    try:
-        with open(path) as f:
-            table = json.load(f)
-    except Exception as e:  # noqa: BLE001
-        return None, f"profiles/ncu_traffic.json unreadable ({type(e).__name__})"
-    ent = table.get(f"{kernel}|{act}|{batch}")
-    if ent is None:
-        return None, f"no ncu capture of {kernel} at act={act}, B={batch} in profiles/ncu_traffic.json"
-    return int(ent["dram_bytes"]), ent.get("source", "")
-
 METRIC = "fno_rollout_steps_per_sec"
 UNIT = "steps/s"
 HW = 64 * 64
+DUMP_LIMIT_BYTES = 64 << 20   # --dump-outputs: all files of one run together
 
 
-def measured_hbm_peak():
-    path = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    try:
-        with open(path) as f:
-            return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    except Exception:  # noqa: BLE001
-        return 6650.0, "fallback (B200_PROFILING.md)"
+def dump_rows(batch: int, n_files: int) -> np.ndarray:
+    """Samples of the batch that --dump-outputs stores: all of them, or a fixed seeded sample (sorted) when n_files
+    float32 frames of the whole batch would exceed DUMP_LIMIT_BYTES."""
+    keep = min(batch, (DUMP_LIMIT_BYTES - n_files * 4096) // (n_files * 2 * HW * 4))   # 4 KB per file: .npy header
+    if keep == batch:
+        return np.arange(batch)
+    return np.sort(np.random.default_rng(0).choice(batch, keep, replace=False))
+
+
+# HBM3 bandwidth of the H100 SXM (NVIDIA data sheet): the denominator of the roofline fractions, not a reached figure
+HBM_PEAK_GBS = 3350.0
 
 
 class ClockSampler:
@@ -309,10 +304,10 @@ def host_cpu():
 
 def reference_impl(sd):
     """The CPU implementation `cpu_baseline` / `--impl reference` time, as (kind, forward, train_step_factory).
-    kind "reference": the UNMODIFIED reference module, installed by __graft_entry__.build() from /root/reference/src into
-    the git-ignored baseline/_ref/ (it travels to the GPU box with the snapshot); kind "port": oracle/fno_torch_port.py,
-    verified bit-identical to it by oracle/make_golden.py, when baseline/_ref is absent."""
-    ref_src = os.path.join(ROOT, "baseline", "_ref", "src")
+    kind "reference": the UNMODIFIED reference module, installed by __graft_entry__.build() into the git-ignored
+    oracle/_ref/ (oracle/install_reference.py); kind "port": oracle/fno_torch_port.py, verified bit-identical to it by
+    oracle/make_golden.py, when oracle/_ref is absent."""
+    ref_src = os.path.join(ROOT, "oracle", "_ref", "src")
     if os.path.isdir(os.path.join(ref_src, "models", "fno")):
         try:
             sys.path.insert(0, ref_src)
@@ -344,7 +339,7 @@ def reference_impl(sd):
                 return step
             return "reference", fwd, many, make_train
         except Exception as e:  # noqa: BLE001
-            sys.stderr.write(f"bench.py: baseline/_ref unusable ({type(e).__name__}: {e}); timing the oracle port\n")
+            sys.stderr.write(f"bench.py: oracle/_ref unusable ({type(e).__name__}: {e}); timing the oracle port\n")
         finally:
             if sys.path and sys.path[0] == ref_src:
                 sys.path.pop(0)
@@ -422,7 +417,7 @@ def workload_name(batch: int) -> str:
 
 
 def run_reference(args, rank: int, world: int):
-    """--impl reference: the reference's own CPU implementation of the path (the unmodified module from baseline/_ref when
+    """--impl reference: the reference's own CPU implementation of the path (the unmodified module from oracle/_ref when
     build() could install it, else the verified port) on ALL physical cores of this host -- also under torchrun, where
     OMP_NUM_THREADS=1 would otherwise leave it single-threaded.  Rank 0 only; the other ranks exit."""
     if rank != 0:
@@ -451,7 +446,7 @@ def run_reference(args, rank: int, world: int):
         # same workload as the GPU arm; one step = one pass over one batch of `batch_per_gpu` cases
         "config": {"workload": workload_name(args.batch), "batch_per_gpu": args.batch, "global_batch": args.batch,
                    "act_storage": "f32", "arithmetic": "fp32",
-                   "implementation": (f"reference CPU path ({'unmodified src/models/fno/fno2d.py from baseline/_ref' if kind == 'reference' else 'torch port of src/models/fno/fno2d.py'}), "
+                   "implementation": (f"reference CPU path ({'unmodified src/models/fno/fno2d.py from oracle/_ref' if kind == 'reference' else 'torch port of src/models/fno/fno2d.py'}), "
                                       f"{threads} threads on {cpu_model} ({phys} cores), rank 0 only")},
         "sample_steps_per_s": val * args.batch,
         "cpu_baseline": {"value": val, "unit": UNIT, "cores": threads, "kind": kind, "cpu_model": cpu_model,
@@ -471,6 +466,8 @@ def main():
     ap.add_argument("--batch", type=int, default=256, help="cases per GPU")
     ap.add_argument("--act", default="bf16", choices=["bf16", "f32"], help="headline activation storage")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's predictions of each storage mode to DIR/<name>.npy")
     ap.add_argument("--no-graph", action="store_true",
                     help="launch every kernel on the stream instead of replaying the rollout from a CUDA graph")
     args = ap.parse_args()
@@ -499,7 +496,12 @@ def main():
         headline = act == args.act
         if headline and rank == 0:
             sampler.start()
-        ts, _ = timed_rollout(model, inp, cp, mk, args.steps, args.warmup, reps=5 if headline else 3)
+        ts, seq = timed_rollout(model, inp, cp, mk, args.steps, args.warmup, reps=5 if headline else 3)
+        if args.dump_outputs and rank == 0:
+            os.makedirs(args.dump_outputs, exist_ok=True)
+            rows = torch.from_numpy(dump_rows(args.batch, 2)).to(seq[-1].device)
+            np.save(os.path.join(args.dump_outputs, f"preds_last_step_{act}.npy"),
+                    seq[-1].index_select(0, rows).float().cpu().numpy().astype(np.float32))
         if headline and rank == 0:
             clocks = sampler.stop()
         ts_max = [dp.max_over_ranks(t, dev) for t in ts]   # max over ranks of every repetition
@@ -527,7 +529,7 @@ def main():
             torch.distributed.destroy_process_group()
         return
 
-    peak, peak_src = measured_hbm_peak()
+    peak, peak_src = HBM_PEAK_GBS, "H100 SXM data sheet (HBM3 3.35 TB/s)"
 
     def summarize(act):
         r = results[act]
@@ -545,13 +547,11 @@ def main():
         step_alg = args.batch * (3 * HW * 2 + 32 * HW * elt + 4 * 32 * HW * 2 * elt + 32 * HW * elt + 2 * HW * 4) if act == "f32" \
             else args.batch * 2662400
         ms = 1e3 * r["t"] / args.steps
-        traffic, traffic_src = ncu_traffic(dom_kernel, act, args.batch)
         return {
             "value": world * args.steps / r["t"], "ms_per_step": ms, "ms_per_step_min": 1e3 * r["t_min"] / args.steps,
             "reps_ms_per_step": [1e3 * t / args.steps for t in r["t_all"]],
             "roofline": {"bound": "hbm", "kernel": dom_kernel, "achieved": alg / k3 / 1e9, "peak": peak,
-                         "unit": "GB/s", "frac": alg / k3 / 1e9 / peak, "traffic": traffic, "traffic_source": traffic_src,
-                         "algorithmic_bytes_per_launch": alg, "peak_source": peak_src,
+                         "unit": "GB/s", "frac": alg / k3 / 1e9 / peak, "algorithmic_bytes_per_launch": alg, "peak_source": peak_src,
                          "share_of_step": k[dom]["mean_us"] * k[dom]["launches_per_step"] / step_us,
                          "fourier_layer_frac": alg / blk / 1e9 / peak, "fourier_layer_us": blk * 1e6,
                          "step_frac": step_alg / (ms * 1e-3) / 1e9 / peak, "step_algorithmic_bytes": step_alg},
@@ -574,7 +574,7 @@ def main():
             "arithmetic": "fp32-grade: tensor-core products as 3xTF32 / bf16x3 (24-bit operands), fp32 accumulation",
             "parallelism": f"dp{world} (independent case shards, no data-path collective)",
             "l2": "inputs larger than L2: per-step working set (2 activation buffers + modes) = "
-                  f"{(2 * args.batch * 32 * HW * (2 if args.act == 'bf16' else 4) + 2 * args.batch * 288 * 32 * 8) / 1e6:.0f} MB > 126 MB",
+                  f"{(2 * args.batch * 32 * HW * (2 if args.act == 'bf16' else 4) + 2 * args.batch * 288 * 32 * 8) / 1e6:.0f} MB > 50 MB",
             "cuda_graph": not args.no_graph,
             "timing": "median of 5 repetitions of K steps each (CUDA events, max over ranks per repetition); "
                       "ms_per_step_min / reps_ms_per_step alongside",

@@ -1,4 +1,4 @@
-"""cfdbench_b200 -- B200-native (sm_100a) FNO hot path for CFDBench.
+"""cfdbench_b200 -- H100-native (sm_90a) FNO hot path for CFDBench.
 
 Public surface mirrors the reference's for this path:
     Fno2d, SpectralConv2d_fast, FnoBlock   (reference src/models/fno/fno2d.py)

@@ -3,7 +3,7 @@
 When the reference's `src/` directory is on sys.path (i.e. when `train_auto.py` / `test_multistep.py`
 drive this package through `cfdbench_b200.runner`), the drop-in model must subclass the *reference's*
 class, because `test_multistep.py:109` checks `isinstance(model, AutoCfdModel)`.  Stand-alone (tests,
-bench, the GPU box, where /root/reference does not exist) a mirror with the same three abstract
+bench, or wherever the reference is not importable) a mirror with the same three abstract
 methods is used (reference src/models/base_model.py:41-81).
 """
 from __future__ import annotations

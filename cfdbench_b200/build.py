@@ -1,8 +1,8 @@
-"""Build libcfdbench_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build libcfdbench_b200.so in-tree with nvcc for sm_90a (cross-compiles without a GPU).
 
     python -m cfdbench_b200.build [--force] [--verbose]
 
-The .so is git-ignored but travels to the GPU box with the repo snapshot.  The product path never
+The .so and the object files are git-ignored build products.  The product path never
 JIT-compiles and never falls back: if the library is missing, `cfdbench_b200._lib` raises.
 """
 from __future__ import annotations
@@ -17,9 +17,9 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libcfdbench_b200.so")
 STAMP = os.path.join(HERE, ".build_stamp")
-SOURCES = ["fno_abi.cu", "fno_dft_fwd.cu", "fno_dft_fwd_tc.cu", "fno_mode_mix.cu", "fno_block_tc.cu", "fno_block_fused.cu", "fno_pointwise.cu", "fno_project_tc.cu", "fno_project_ws.cu", "fno_project_bwd_tc.cu",
+SOURCES = ["fno_abi.cu", "fno_dft_fwd.cu", "fno_dft_fwd_tc.cu", "fno_mode_mix.cu", "fno_block_tc.cu", "fno_block_fused.cu", "fno_pointwise.cu", "fno_project_tc.cu", "fno_project_bwd_tc.cu",
            "fno_backward.cu", "fno_metrics.cu", "fno_train_step.cu"]
-NVCC_FLAGS = ["-std=c++17", "-O3", "-lineinfo", "-gencode", "arch=compute_100a,code=sm_100a",
+NVCC_FLAGS = ["-std=c++17", "-O3", "-lineinfo", "-gencode", "arch=compute_90a,code=sm_90a",
               "-Xcompiler", "-fPIC"]
 
 

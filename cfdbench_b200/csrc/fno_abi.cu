@@ -12,8 +12,6 @@ cudaError_t launch_dft_fwd(const void*, void*, int, float, float, cudaStream_t);
 cudaError_t launch_mode_mix(const void*, const void*, void*, void*, int, cudaStream_t);
 cudaError_t launch_block_fused(const void*, const void*, const float*, const float*, void*, int, cudaStream_t);
 size_t ym_image_bytes(int);
-cudaError_t launch_project_ws(const void*, const float*, const float*, const float*, const float*, const float*, float*, int,
-                              cudaStream_t);
 cudaError_t launch_pack_spectral(const void*, const void*, void*, int, cudaStream_t);
 cudaError_t launch_unpack_spectral(const void*, void*, void*, cudaStream_t);
 cudaError_t launch_dft_fwd_tc(const void*, void*, int, float, float, cudaStream_t);
@@ -242,7 +240,7 @@ int fno_project_fwd(const void* act_in, const float* mask, const fno_weights* w,
   cudaError_t e =
       act_dtype == FNO_ACT_F32
           ? launch_project_tc<float>(act_in, w->fc1_w, w->fc1_b, w->fc2_w, w->fc2_b, mask, preds, batch, S(stream))
-          : launch_project_ws(act_in, w->fc1_w, w->fc1_b, w->fc2_w, w->fc2_b, mask, preds, batch, S(stream));
+          : launch_project_tc<__nv_bfloat16>(act_in, w->fc1_w, w->fc1_b, w->fc2_w, w->fc2_b, mask, preds, batch, S(stream));
   FNO_CUDA(e, "project_kernel");
   return kOk;
 }

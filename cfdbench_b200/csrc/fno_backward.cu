@@ -162,8 +162,8 @@ __global__ void __launch_bounds__(kPbThreads)
     float2 z0 = make_float2(bj, bj), z1 = make_float2(0.f, 0.f);
 #pragma unroll
     for (int i = 0; i < kC; i += 2) {
-      z0 = __ffma2_rn(x[i], make_float2(wr[i], wr[i]), z0);
-      z1 = __ffma2_rn(x[i + 1], make_float2(wr[i + 1], wr[i + 1]), z1);
+      z0 = ffma2(x[i], make_float2(wr[i], wr[i]), z0);
+      z1 = ffma2(x[i + 1], make_float2(wr[i + 1], wr[i + 1]), z1);
     }
     const float2 z = make_float2(z0.x + z1.x, z0.y + z1.y);
     float gx_, gy_, dgx, dgy;
@@ -172,7 +172,7 @@ __global__ void __launch_bounds__(kPbThreads)
     const float w20 = sm.w2[0][j], w21 = sm.w2[1][j];
     const float2 dz = make_float2((w20 * d0.x + w21 * d1.x) * dgx, (w20 * d0.y + w21 * d1.y) * dgy);
 #pragma unroll
-    for (int i = 0; i < kC; ++i) da[i] = __ffma2_rn(make_float2(wr[i], wr[i]), dz, da[i]);
+    for (int i = 0; i < kC; ++i) da[i] = ffma2(make_float2(wr[i], wr[i]), dz, da[i]);
     *reinterpret_cast<float2*>(dz_b + static_cast<size_t>(j) * kHW) = dz;
     // fc2 weight gradient and fc1 bias gradient: warp partials -> smem accumulators
     const float p0 = warp_sum(d0.x * gx_ + d0.y * gy_);
@@ -439,10 +439,10 @@ __global__ void __launch_bounds__(kSwWarps * 32)
 #pragma unroll
     for (int i = 0; i < kC; i += 2) {
       const float4 v = *reinterpret_cast<const float4*>(&xs[warp][i]);
-      acc_a[i] = __ffma2_rn(make_float2(v.x, v.x), g, acc_a[i]);
-      acc_b[i] = __ffma2_rn(make_float2(v.y, v.y), g, acc_b[i]);
-      acc_a[i + 1] = __ffma2_rn(make_float2(v.z, v.z), g, acc_a[i + 1]);
-      acc_b[i + 1] = __ffma2_rn(make_float2(v.w, v.w), g, acc_b[i + 1]);
+      acc_a[i] = ffma2(make_float2(v.x, v.x), g, acc_a[i]);
+      acc_b[i] = ffma2(make_float2(v.y, v.y), g, acc_b[i]);
+      acc_a[i + 1] = ffma2(make_float2(v.z, v.z), g, acc_a[i + 1]);
+      acc_b[i + 1] = ffma2(make_float2(v.w, v.w), g, acc_b[i + 1]);
     }
   }
 #pragma unroll

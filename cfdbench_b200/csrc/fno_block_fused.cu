@@ -1,510 +1,247 @@
-// Fused Fourier-block output stage for bf16 activation storage: ONE kernel replaces inv_kx_kernel + block_tc_kernel
-//   out[b][o][h][w] = GELU( irfft2(pad(Y))[b][o][h][w] + sum_i W0[o][i] x[b][i][h][w] + bias[o] )      (bf16 in, bf16 out)
-// i.e. irfft2 + Conv2d(32,32,1) + add + GELU of the reference FnoBlock (src/models/fno/fno2d.py:65-72,81,104-111).
-// The half-inverted spectrum Z never leaves the SM (it used to be written and re-read through HBM, 50 MB per layer at
-// B = 256) and no operand is staged through registers on the load side:
+// Fused Fourier-block output stage for bf16 activation storage (inference):
+//   out[b][o][h][w] = GELU( irfft2(pad(Y))[b][o][h][w] + sum_i W0[o][i] x[b][i][h][w] + bias[o] )       (bf16 in, bf16 out)
+// replacing irfft2 + Conv2d(32,32,1) + add + GELU of the reference FnoBlock (src/models/fno/fno2d.py:65-72,81,104-111)
+// with one kernel in which the half-inverted spectrum Z never leaves the SM.
 //
-//   work unit  = (sample, half image of 32 rows) = 16 tiles of 128 pixels; units are dealt round-robin to the CTAs.
-//   GEMM1      inverse DFT along kx of the unit's 32 rows, on the tensor cores, 3xTF32:
-//                  D1[(ky,o) 3 x 128 lanes][(h',re|im) 64 cols] = Y^T[(ky,o)][(kx,re|im) 48] * F[(kx,re|im)][(h',re|im)]
-//              A = the mixed modes of the sample exactly as mode_mix_tc_kernel's epilogue wrote them: tf32 hi/lo images,
-//                  MN-major, 128B/32B-base swizzle (the only MN-major form kind::tf32 accepts: tools/tc_probe5.cu), bulk-copied
-//                  24 KB at a time;   B = constant twiddles (K-major), second half image = first with odd kx negated
-//                  (a_negate bit of the instruction descriptor).
-//   converters 12 warps, thread = (ky, o): pull D1 out of tensor memory (tcgen05.ld), split into tf32 hi/lo and write
-//              the per-tile B operand  Zt[(j,ky,re|im) 48][o 32]  (MN-major: a warp writes whole 128-byte rows).
-//   tile MMA   D2[128 px][32 o] = X[128 px][32 i] W0^T          kind::f16: x tile arrives by TMA (tensor map, 128B swizzle)
-//                                                               straight from the NCHW bf16 activation (bf16 is exact),
-//                                                               W0 as three bf16 pieces (24 significant bits)
-//                               + (E (+) E)[128 px][48] Zt       kind::tf32, 3xTF32; E = C2R stage (cos,-sin)(2 pi ky w/64)
-//                                                               c_ky/HW folded in, resident in TENSOR MEMORY as the A operand;
-//                                                               its (ky=0, Im) column is 1 and the matching Zt row = bias.
-//   epilogue   8 warps: TMEM -> registers -> exact-erf GELU -> bf16 -> global.
-// Warp roles (768 threads): 0-11 converters, 12-19 epilogue, 20/21 tile MMA issue (even / odd tiles, one elected lane
-// each), 22 GEMM1 issue, 23 producers (lane 0: x tiles by TMA, lane 1: mode images by bulk copy).  All hand-offs are
-// mbarriers.  The dependent chain per tile is what limits the kernel (no pipe is saturated: DESIGN.md 4.1), so a tile's three
-// inputs -- x tile, Zt operand, drained accumulator -- share ONE ring of 3 super-slots (2 tiles each) and ONE "ready"
-// barrier (TMA bytes + 12 converter arrivals + 4 epilogue arrivals), three threads issue MMAs, and the next unit's GEMM1 is
-// paced behind the current unit's super-tiles in the in-order tensor queue.
+// Work unit = (sample, chunk of 16 image rows); a CTA always works on the same chunk (blockIdx.x % 4), so its inverse-kx
+// constant is loaded once.  Per unit:
+//   GEMM1 (inverse DFT along kx, 3xTF32):  Z1[(ky, o) 384][(h', re|im) 32] = Y^T[(ky, o)][(kx, re|im) 48] * F[(h', ri)][.]^T
+//          six m64n32k8 chains, one per ky pair; A = the mode image of the sample (fno_mode_mix.cu writes it with the
+//          tf32 hi/lo split done), loaded from shared memory into A-fragment registers -- the image's 32-byte chunk
+//          swizzle makes those loads conflict-free -- and B = the constant F (K-major); Z1 -> tf32 hi/lo -> Zt, the
+//          K-major B operand of GEMM2 per image row (96 KB for 16 rows).  Bias rides in the row that irfft2's C2R stage
+//          ignores (Im of ky = 0).
+//   GEMM2 per image row h:  D[64 w][32 o] = E[w][(ky, ri) 24] Zt_h + X_h[w][32 i] W0^T   (m64n32k8, 3xTF32 / 2 passes)
+//          E = C2R stage with c_ky/HW folded in (fno_block_tc.cu builds it); X_h staged through registers (bf16 values
+//          are exact in tf32); epilogue exact-erf GELU, bf16 pairs exchanged between neighbouring lanes, 4-byte stores.
+// Roles: warp 8 lanes 0/1 -- producers of the two image slots (24 KB = one ky pair, hi + lo, two bulk copies each);
+// warpgroups 0 / 1 -- the even / odd ky pairs of GEMM1 and the even / odd rows of GEMM2.
 #include "fno_common.cuh"
 #include "tc_common.cuh"
-#include "tc_tma.cuh"
 #include <math.h>
 #include <string.h>
 
 namespace fno {
 
-constexpr int kFzThreads = 768;
-constexpr int kFzConvWarps = 12, kFzEpiWarps = 8;
-constexpr int kFzMmaWarp = 20;    // 20: tiles T even, 21: tiles T odd (one elected lane each)
-constexpr int kFzG1Warp = 22;     // GEMM1 (inverse DFT along kx) issue
-constexpr int kFzProdWarp = 23;
-constexpr int kFzTilesPerUnit = 16;         // 32 rows / 2
-constexpr int kFzTS = 2;   // tiles per hand-off ("super-tile" = 4 image rows): every barrier wait / fence is paid once per 2 tiles
-constexpr int kFzSPU = kFzTilesPerUnit / kFzTS;   // 8 super-tiles per unit
-constexpr int kFzR = 3;    // ONE ring of super-slots for x tiles, Zt operands and accumulators: a single "ready" barrier
-constexpr int kFzNY = 3;   // mode-image stages
-constexpr uint32_t kFzXBytes = 8192;        // 2 boxes x (32 ch x 128 B)
-constexpr uint32_t kFzBtBytes = 12288;      // hi + lo, 48 rows x 128 B each
-constexpr uint32_t kFzYStage = 24576;       // (M-tile, kx parity): hi + lo, 4 ky groups x 24 rows x 128 B
-constexpr uint32_t kFzFBytes = 24576;       // twiddle operand: hi + lo images of [64][48]
-constexpr uint32_t kFzWBytes = 3 * 2048;    // three bf16 pieces of W0
-// mode image of one sample (written by mode_mix_tc_kernel): [hi|lo][M-tile 3][ky group 4][48 rows][32 o] fp32
-constexpr size_t kYmImgPart = 73728, kYmImgMtile = 24576, kYmImgGroup = 6144;
-constexpr size_t kYmImgBytes = 2 * kYmImgPart;
-// tensor memory columns
-constexpr uint32_t kFzColE = 0;      // E hi (48) | E lo (48)
-constexpr uint32_t kFzColD1 = 96;    // 3 x 64
-constexpr uint32_t kFzColD2 = 288;   // kFzR x kFzTS x 32
-
-// Optional timeline trace (tools/trace_fused.py builds a -DFNO_FZ_TRACE variant of the library): CTA 0 records
-// clock64() at the hand-off points of every role: trace[(role * 256 + T) * 8 + event].
-#ifdef FNO_FZ_TRACE
-__device__ long long* g_fz_trace = nullptr;
-// The pointer is read ONCE per thread (fz_tr): re-reading the global for every stamp costs an L2 round trip (~450 cycles)
-// that the stamps of a single-thread role then mostly measure (tools/mbar_probe.cu: a completed mbarrier wait is 46 cycles).
-#define FZ_T(role, T, ev)                                                                          \
-  do {                                                                                             \
-    if (fz_tr != nullptr && blockIdx.x == 0 && (T) < 256) fz_tr[((role) * 256 + (T)) * 8 + (ev)] = clock64(); \
-  } while (0)
-// knock-out experiments (results are wrong): 1 no conv MMAs, 2 no E MMAs, 4 no GEMM1 MMAs, 8 no converter stores,
-// 16 no GELU, 32 no output stores
-__device__ int g_fz_knock = 0;
-#define FZ_KNOCK(bit) ((fz_knock & (bit)) != 0)
-#else
-#define FZ_T(role, T, ev) do { } while (0)
-#define FZ_KNOCK(bit) false
-#endif
+constexpr int kFzRows = 16;                            // image rows per unit
+constexpr int kFzChunks = kH / kFzRows;                // 4
+constexpr int kFzThreads = 9 * 32;                     // 2 warpgroups + producer warp
+constexpr int kFzProdWarp = 8;
+constexpr int kZK = 2 * kM2;                           // 24: (ky, re|im)
+constexpr int kImgK = 2 * kKX;                         // 48: (kx, re|im) image rows
+constexpr size_t kYmImgBytes = 147456;                 // per sample: [hi|lo][ky 12][48 rows][32 o] fp32
+constexpr uint32_t kFzStage = 4 * 6144;                // one ky pair: hi (2 x 6144 B) then lo
+constexpr int kFzFFloats = 2 * (2 * kFzRows) * kImgK;  // [n = 2 h' + ri (32)][48], hi | lo: per chunk
+constexpr int kFzEFloats = 2 * kW * kZK;               // [64 w][24] hi | lo
+constexpr uint32_t kFzZtFloats = kC * kZK;             // one image row, hi or lo: [32 o][24 k] K-major
+constexpr uint32_t kLboF = (2 * kFzRows / 8) * 128;    // 512
+constexpr uint32_t kLboE = (kW / 8) * 128;             // 1024
+constexpr uint32_t kLboO = (kC / 8) * 128;             // 512: B operands with 32 rows (o)
 
 struct FzSmem {
-  alignas(1024) unsigned char x[kFzR][kFzTS][kFzXBytes];
-  alignas(1024) unsigned char bt[kFzR][kFzTS][kFzBtBytes];
-  alignas(1024) unsigned char y[kFzNY][kFzYStage];
-  alignas(1024) unsigned char f[kFzFBytes];
-  alignas(1024) unsigned char w[kFzWBytes];
+  alignas(128) unsigned char y[2][kFzStage];           // image ring (slot = parity of the ky pair)
+  alignas(128) float zt[kFzRows][2][kFzZtFloats];      // GEMM2 B operand per row: hi, lo
+  alignas(128) float f_hi[kFzFFloats / 2];
+  alignas(128) float f_lo[kFzFFloats / 2];
+  alignas(128) float e_hi[kFzEFloats / 2];
+  alignas(128) float e_lo[kFzEFloats / 2];
+  alignas(128) float wb_hi[kC * kC];
+  alignas(128) float wb_lo[kC * kC];
+  alignas(128) float ax[2][kW * kC];                   // per warpgroup: conv A operand of the current row
   alignas(16) float bias[kC];
-  // ready[s]: slot s holds tile T's x tile (1 arrival + 8 KB of TMA bytes), its Zt operand (12 converter warps) and its
-  // accumulator is free again (the 4 epilogue warps that drained it; pre-arrived once in the prologue)  -> ONE wait per tile in the MMA thread.
-  // slot_free[s]: the tile's MMAs have completed (x tile and Zt operand may be overwritten); d2_full[s]: same event,
-  // consumed by the epilogue (two barriers so that neither waiter has to re-arm the other's phase bookkeeping).
-  // Indexed by fz_bar(S) = (slot, parity of the super-tile index S): the two MMA threads / epilogue groups take alternate
-  // super-tiles, and with an odd ring size a role would otherwise see only every other phase of a slot's barrier, which
-  // the one-bit phase parity cannot express (a wait could match the completion of three super-tiles earlier).
-  alignas(8) uint64_t ready[2 * kFzR], slot_free[2 * kFzR], d2_full[2 * kFzR];
-  // x_free[s]: the 1x1-convolution MMAs of the super-tile have completed: its x tiles may be refilled while its C2R MMAs
-  // still run (the TMA round trip of the slot's next user starts ~1,000 cycles earlier)
-  uint64_t x_free[2 * kFzR];
-  // pace[s]: the same completion event once more, consumed by the GEMM1 thread: it spreads the 54 MMAs of the NEXT unit's
-  // inverse-kx GEMM over the super-tiles of the current unit (one stage per super-tile) instead of queueing them in one
-  // ~3,200-cycle burst in front of the tile MMAs the three-slot ring is waiting for
-  uint64_t pace[2 * kFzR];
-  uint64_t y_full[kFzNY], y_empty[kFzNY];
-  uint64_t d1_full, d1_free, f_bar;
-  uint32_t tmem_base;
+  alignas(8) uint64_t y_full[2], y_free[2];
 };
-__device__ __forceinline__ int fz_bar(int S) { return (S % kFzR) * 2 + (S & 1); }   // barrier of super-tile S
-__device__ __forceinline__ uint32_t fz_phase(int S) { return static_cast<uint32_t>(S / (2 * kFzR)) & 1u; }
-constexpr uint32_t kFzReadyCount = kFzConvWarps + 1 + kFzEpiWarps / 2;   // 4 epilogue warps (one group) per tile
-
-__device__ __forceinline__ void fz_ld16(uint32_t taddr, float* v) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
 
 __global__ void __launch_bounds__(kFzThreads, 1)
-    block_fused_kernel(const __grid_constant__ CUtensorMap x_map, const unsigned char* __restrict__ ym_img,
+    block_fused_kernel(const unsigned char* __restrict__ img, const __nv_bfloat16* __restrict__ x,
                        const float* __restrict__ w0t, const float* __restrict__ bias, const float* __restrict__ etab,
-                       const float* __restrict__ ftab, __nv_bfloat16* __restrict__ out, int n_units) {
+                       const float* __restrict__ ftab, __nv_bfloat16* __restrict__ out, int batch) {
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   FzSmem& sm = *reinterpret_cast<FzSmem*>(smem_raw);
-  if ((smem_u32(smem_raw) & 1023u) != 0) __trap();
-#ifdef FNO_FZ_TRACE
-  long long* const fz_tr = g_fz_trace;
-  const int fz_knock = g_fz_knock;
-  if (fz_tr != nullptr && threadIdx.x == 0) fz_tr[4 * 256 * 8 + blockIdx.x * 4 + 0] = clock64();
-#endif
   const int tid = threadIdx.x, lane = tid & 31, warp = tc::warp_index_uniform();
+  const int chunk = blockIdx.x % kFzChunks, b0 = blockIdx.x / kFzChunks, bstride = gridDim.x / kFzChunks;
+  const int n_units = b0 < batch ? (batch - b0 + bstride - 1) / bstride : 0;
 
-  const int first = blockIdx.x, stride = gridDim.x;
-  // Work items of this CTA: `n_full` whole units (u = first + k * stride; unit u = 2 * sample + half image), then the units
-  // of the last, incomplete round.  When at most half of the CTAs would get one of those, each of them is SPLIT between two
-  // CTAs (rows 0-15 / 16-31 of the half image = super-tiles 0-3 / 4-7; both run the unit's GEMM1, on 32 columns only), so
-  // the makespan is 3.5 instead of 4 units at B = 256 (512 units on 148 SMs).
-  const int n_full = n_units / stride, n_rem = n_units % stride;
-  int ex_u = -1, ex_s0 = 0, ex_ns = 0;   // extra item: unit, first unit-local super-tile, number of super-tiles
-  if (n_rem > 0) {
-    if (2 * n_rem <= stride) {
-      if (first < 2 * n_rem) { ex_u = n_full * stride + first % n_rem; ex_s0 = (first / n_rem) * (kFzSPU / 2); ex_ns = kFzSPU / 2; }
-    } else if (first < n_rem) {
-      ex_u = n_full * stride + first;
-      ex_ns = kFzSPU;
-    }
-  }
-  const int n_mine = n_full + (ex_ns > 0 ? 1 : 0);        // items
-  const int n_super_all = n_full * kFzSPU + ex_ns;         // super-tiles of all items
-  auto unit_of = [&](int k) { return k < n_full ? first + k * stride : ex_u; };
-  auto item_s0 = [&](int k) { return k < n_full ? 0 : ex_s0; };
-  auto item_ns = [&](int k) { return k < n_full ? kFzSPU : ex_ns; };
-  // global super-tile S of this CTA -> (unit, unit-local super-tile)
-  auto super_unit = [&](int S) { return S < n_full * kFzSPU ? first + (S / kFzSPU) * stride : ex_u; };
-  auto super_local = [&](int S) { return S < n_full * kFzSPU ? S % kFzSPU : ex_s0 + (S - n_full * kFzSPU); };
-
-  // ---------------------------------------------------------------- prologue (weights / constant tables only)
+  // ---------------------------------------------------------------- prologue (constants and weights only)
   if (tid == 0) {
-    for (int i = 0; i < 2 * kFzR; ++i) {
-      mbar_init(&sm.ready[i], kFzReadyCount);
-      mbar_init(&sm.slot_free[i], 1);
-      mbar_init(&sm.x_free[i], 1);
-      mbar_init(&sm.d2_full[i], 1);
-      mbar_init(&sm.pace[i], 1);
+    for (int i = 0; i < 2; ++i) {
+      mbar_init(&sm.y_full[i], 1);
+      mbar_init(&sm.y_free[i], 4);   // the four warps of the warpgroup that reads the slot
     }
-    for (int i = 0; i < kFzNY; ++i) { mbar_init(&sm.y_full[i], 1); mbar_init(&sm.y_empty[i], 1); }
-    mbar_init(&sm.d1_full, 1);
-    mbar_init(&sm.d1_free, kFzConvWarps);
-    mbar_init(&sm.f_bar, 1);
     fence_mbar_init();
-    mbar_expect_tx(&sm.f_bar, kFzFBytes);
-    bulk_g2s(sm.f, ftab, kFzFBytes, &sm.f_bar);   // twiddle operand, already in its K-major tf32 hi|lo layout
   }
-  if (warp == kFzMmaWarp) tc::tmem_alloc<512>(&sm.tmem_base);
-  // The constant E operand goes to tensor memory below; its 48 values per thread are requested NOW, so that their L2
-  // round trip overlaps the TMEM allocation and the W0 conversion (loaded 16 at a time after the barrier, the three
-  // dependent round trips made this prologue 6,400 cycles per CTA).
-  const bool loads_e = warp >= kFzConvWarps && warp < kFzConvWarps + kFzEpiWarps;
-  float e_val[48];
-  if (loads_e) {
-    const int m = (warp & 3) * 32 + lane, cbase = ((warp - kFzConvWarps) >> 2) * 48;
-#pragma unroll
-    for (int j = 0; j < 48; ++j) e_val[j] = __ldg(etab + (cbase + j) * 128 + m);
+  for (int e = tid; e < kFzFFloats / 2; e += kFzThreads) {
+    sm.f_hi[e] = __ldg(ftab + chunk * kFzFFloats + e);
+    sm.f_lo[e] = __ldg(ftab + chunk * kFzFFloats + kFzFFloats / 2 + e);
   }
-  // W0 -> three bf16 pieces, B operand [n = o][k = i], K-major, no swizzle (8 x 16-byte core matrices)
-  float w_val[2];
-#pragma unroll
-  for (int it = 0; it < 2; ++it) w_val[it] = (tid + it * kFzThreads < kC * kC) ? w0t[tid + it * kFzThreads] : 0.f;
-  static_assert(2 * kFzThreads >= kC * kC, "two W0 elements per thread");
-#pragma unroll
-  for (int it = 0; it < 2; ++it) {
-    const int e = tid + it * kFzThreads;
-    if (e >= kC * kC) break;
-    const int i = e / kC, o = e % kC;   // w0t[i][o] = W0[o][i]
-    const float wv = w_val[it];
-    const __nv_bfloat16 p0 = __float2bfloat16_rn(wv);
-    const float r1 = wv - __bfloat162float(p0);
-    const __nv_bfloat16 p1 = __float2bfloat16_rn(r1);
-    const __nv_bfloat16 p2 = __float2bfloat16_rn(r1 - __bfloat162float(p1));
-    const uint32_t off = ((i >> 3) * 4 + (o >> 3)) * 128 + (o & 7) * 16 + (i & 7) * 2;
-    *reinterpret_cast<__nv_bfloat16*>(sm.w + off) = p0;
-    *reinterpret_cast<__nv_bfloat16*>(sm.w + 2048 + off) = p1;
-    *reinterpret_cast<__nv_bfloat16*>(sm.w + 4096 + off) = p2;
+  for (int e = tid; e < kFzEFloats / 2; e += kFzThreads) {
+    sm.e_hi[e] = __ldg(etab + e);
+    sm.e_lo[e] = __ldg(etab + kFzEFloats / 2 + e);
   }
-  if (tid < kC) sm.bias[tid] = bias ? bias[tid] : 0.f;
-  tc::fence_proxy_async_smem();
-  tc::fence_before_thread_sync();
+  for (int e = tid; e < kC * kC; e += kFzThreads) {  // B[n = o][k = i] = W0[o][i] = w0t[i][o]
+    const int i = e / kC, o = e % kC;
+    float hi, lo;
+    tc::split_tf32(w0t[e], hi, lo);
+    const uint32_t off = tc::kmajor_offset(o, i, kC) / 4;
+    sm.wb_hi[off] = hi;
+    sm.wb_lo[off] = lo;
+  }
+  if (tid < kC) sm.bias[tid] = bias != nullptr ? bias[tid] : 0.f;
+  tc::fence_proxy_async_smem();   // the constant operands above are read by the tensor cores
   __syncthreads();
-  tc::fence_after_thread_sync();
-  const uint32_t tmem = sm.tmem_base;
-  if (loads_e) {
-    // constant E operand -> tensor memory (row m in lane m).  The table is stored column-major (etab[c][m]) so that a warp
-    // reads 128 contiguous bytes per column; with the row-major table every load touched 32 lines and this prologue cost
-    // 17,000 cycles per CTA (a quarter of the kernel, FNO_FZ_TRACE).  Two warps per lane quadrant, 48 columns each.
-    const int cbase = ((warp - kFzConvWarps) >> 2) * 48;
-#pragma unroll
-    for (int c0 = 0; c0 < 48; c0 += 16)
-      tc::tmem_st16(tmem + kFzColE + cbase + c0 + (static_cast<uint32_t>((warp & 3) * 32) << 16), e_val + c0);
-    tc::tmem_wait_st();
-  }
-  tc::fence_before_thread_sync();
-  __syncthreads();   // (the twiddle operand's bulk copy is awaited by its only reader, the GEMM1 thread)
-  tc::fence_after_thread_sync();
-#ifdef FNO_FZ_TRACE
-  if (fz_tr != nullptr && threadIdx.x == 0) fz_tr[4 * 256 * 8 + blockIdx.x * 4 + 1] = clock64();
-#endif
-  pdl_wait();   // ym_img and x come from the previous kernels of the chain
+  pdl_wait();   // the image and x come from the previous kernels of the chain
   pdl_launch_dependents();
-  // all accumulators start out free: the epilogue warps' share of every ready barrier's first phase
-  if (warp >= kFzConvWarps && warp < kFzConvWarps + kFzEpiWarps / 2 && lane == 0)
-    for (int S = 0; S < kFzR; ++S) mbar_arrive(&sm.ready[fz_bar(S)]);
 
-  // ================================================================ converters
-  if (warp < kFzConvWarps) {
-    const int mt = warp >> 2, q = warp & 3, ky = 4 * mt + q, o = lane;
-    const float bias_o = sm.bias[o];
-    const uint32_t lane_base = static_cast<uint32_t>(q * 32) << 16;
-    // byte offsets of this thread's 4 operand rows (j, ky, ri) at column o; row k = 24 j + 2 ky + ri
-    uint32_t roff[4];
-#pragma unroll
-    for (int r = 0; r < 4; ++r) {
-      const int k = 24 * (r >> 1) + 2 * ky + (r & 1);
-      roff[r] = k * 128 + ((((o >> 3) ^ (k & 3)) & 3) << 5) + (o & 7) * 4;
-    }
-    for (int k = 0; k < n_mine; ++k) {
-      if (tid == 0) FZ_T(0, k * kFzSPU, 0);
-      mbar_wait(&sm.d1_full, k & 1);
-      tc::fence_after_thread_sync();
-      if (tid == 0) FZ_T(0, k * kFzSPU, 1);
-      const int hh_begin = item_s0(k) / 4, hh_end = (item_s0(k) + item_ns(k)) / 4;
-#pragma unroll 1
-      for (int hh = hh_begin; hh < hh_end; ++hh) {
-        float v[32];
-        tc::tmem_ld32(tmem + kFzColD1 + mt * 64 + hh * 32 + lane_base, v);
-        if (tid == 0) FZ_T(0, k * kFzSPU + (hh - hh_begin) * 4, 2);
-        if (hh == hh_end - 1) {   // D1 fully read: the next item's GEMM1 may overwrite it
-          tc::fence_before_thread_sync();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&sm.d1_free);
-        }
-#pragma unroll
-        for (int s4 = 0; s4 < 4; ++s4) {
-          const int S = k * kFzSPU + (hh - hh_begin) * 4 + s4;   // all items but the last have kFzSPU super-tiles
-          const int ss = S % kFzR;
-          if (tid == 0) FZ_T(0, S, 3);
-          if (S >= kFzR) mbar_wait(&sm.slot_free[fz_bar(S - kFzR)], fz_phase(S - kFzR));   // previous user of the slot
-          if (tid == 0) FZ_T(0, S, 4);
-#pragma unroll
-          for (int i = 0; i < kFzTS; ++i) {
-            unsigned char* slot = sm.bt[ss][i];
-#pragma unroll
-            for (int r = 0; r < 4; ++r) {
-              float z = v[(s4 * kFzTS + i) * 4 + r];
-              if ((r & 1) && ky == 0) z = bias_o;   // Im of the ky = 0 column is dropped by C2R; the row carries the bias
-              float hi, lo;
-              tc::split_tf32(z, hi, lo);
-              if (FZ_KNOCK(8)) continue;
-              *reinterpret_cast<float*>(slot + roff[r]) = hi;
-              *reinterpret_cast<float*>(slot + 6144 + roff[r]) = lo;
-            }
-          }
-          tc::fence_proxy_async_smem();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&sm.ready[fz_bar(S)]);
-          if (tid == 0) FZ_T(0, S, 5);
+  // ================================================================ producers: lane s fills image slot s
+  if (warp == kFzProdWarp) {
+    if (lane < 2) {
+      const int s = lane;
+      for (int u = 0; u < n_units; ++u) {
+        const unsigned char* src = img + static_cast<size_t>(b0 + u * bstride) * kYmImgBytes;
+        for (int pi = 0; pi < 3; ++pi) {
+          const int p = s + 2 * pi, f = 3 * u + pi;   // ky pair p, fill number f of the slot
+          if (f >= 1) mbar_wait(&sm.y_free[s], (f - 1) & 1);
+          mbar_expect_tx(&sm.y_full[s], kFzStage);
+          bulk_g2s(sm.y[s], src + p * (kFzStage / 2), kFzStage / 2, &sm.y_full[s]);
+          bulk_g2s(sm.y[s] + kFzStage / 2, src + kYmImgBytes / 2 + p * (kFzStage / 2), kFzStage / 2, &sm.y_full[s]);
         }
       }
     }
-  }
-  // ================================================================ epilogue
-  // Two groups of four warps (one warp per TMEM lane quadrant) take alternate super-tiles; a thread owns one pixel of each
-  // tile and all 32 output channels of it: one barrier wait per super-tile, one tcgen05.ld per tile, 16 independent GELU
-  // pairs per tile (the fixed latencies -- barrier wake-up, ~270 cycles per TMEM read -- dominate the epilogue otherwise).
-  else if (warp < kFzConvWarps + kFzEpiWarps) {
-    const int q = warp & 3, grp = (warp - kFzConvWarps) >> 2;
-    const uint32_t lane_base = static_cast<uint32_t>(q * 32) << 16;
-    const int n_super = n_super_all;
-    const bool odd = lane & 1;
-    for (int S = grp; S < n_super; S += 2) {
-      const int ss = S % kFzR;
-      const int u = super_unit(S), t0 = super_local(S) * kFzTS;
-      if ((warp & 3) == 0 && lane == 0) FZ_T(1, S, 0);
-      mbar_wait(&sm.d2_full[fz_bar(S)], fz_phase(S));
-      tc::fence_after_thread_sync();
-      if ((warp & 3) == 0 && lane == 0) FZ_T(1, S, 1);
-#pragma unroll 1
-      for (int i = 0; i < kFzTS; ++i) {
-        float v[32];
-        tc::tmem_ld32(tmem + kFzColD2 + (ss * kFzTS + i) * 32 + lane_base, v);
-        if (i == kFzTS - 1) {   // both accumulators of the slot are in registers: the slot may be reused
-          tc::fence_before_thread_sync();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&sm.ready[fz_bar(S + kFzR)]);   // next user of the slot
-          if ((warp & 3) == 0 && lane == 0) FZ_T(1, S, 2);
-        }
-        // lanes 2i / 2i+1 hold adjacent pixels: exchange halves so that the even lane stores the pixel PAIR of channel c
-        // and the odd lane the pair of channel c+1 (one 4-byte store per two values instead of two 2-byte stores)
-        const int b = u >> 1, px = (u & 1) * 2048 + (t0 + i) * 128 + q * 32 + (lane & ~1);
-        __nv_bfloat16* dst = out + (static_cast<size_t>(b) * kC + (odd ? 1 : 0)) * kHW + px;
-#pragma unroll
-        for (int c = 0; c < 32; c += 2) {
-          const float2 g = FZ_KNOCK(16) ? make_float2(v[c], v[c + 1]) : gelu_erf2(make_float2(v[c], v[c + 1]));
-          const __nv_bfloat162 pk = __float22bfloat162_rn(g);                    // (channel c, channel c+1) of my pixel
-          const uint32_t mine = *reinterpret_cast<const uint32_t*>(&pk);
-          const uint32_t other = __shfl_xor_sync(0xffffffffu, mine, 1);
-          // even lane: (my c, neighbour's c);  odd lane: (neighbour's c+1, my c+1)
-          const uint32_t pair = odd ? __byte_perm(other, mine, 0x7632) : __byte_perm(mine, other, 0x5410);
-          if (!FZ_KNOCK(32)) *reinterpret_cast<uint32_t*>(dst + static_cast<size_t>(c) * kHW) = pair;
-        }
-      }
-      if ((warp & 3) == 0 && lane == 0) FZ_T(1, S, 3);
-    }
-  }
-  // ================================================================ MMA issue: tiles
-  // Two issuing threads (warps 20 / 21) take alternate super-tiles, so that one can wait for its super-tile's inputs while
-  // the other's MMAs are being queued.  Each thread commits only its own
-  // super-tile's barriers (tcgen05.commit tracks the MMAs of the executing thread).
-  else if (warp == kFzMmaWarp || warp == kFzMmaWarp + 1) {
-    if (tc::elect_one()) {
-      const uint32_t w_s = tc::smem_addr(sm.w);
-      constexpr uint32_t idesc_e = tc::make_idesc_tf32(128, 32) | kBMajorMN;
-      constexpr uint32_t idesc_c = fz_idesc_bf16(128, 32) | kAMajorMN;
-      const int n_super = n_super_all;
-#pragma unroll 1
-      for (int S = warp - kFzMmaWarp; S < n_super; S += 2) {
-        const int ss = S % kFzR;
-        FZ_T(2, S, 0);
-        mbar_wait(&sm.ready[fz_bar(S)], fz_phase(S));   // x tiles landed, Zt operands written, accumulators drained
-        tc::fence_after_thread_sync();
-        FZ_T(2, S, 2);
-#pragma unroll
-        for (int i = 0; i < kFzTS; ++i) {   // 1x1 convolution: per tile (the x tiles differ)
-          const uint32_t d = tmem + kFzColD2 + (ss * kFzTS + i) * 32;
-          const uint32_t x_s = tc::smem_addr(sm.x[ss][i]);
-#pragma unroll
-          for (int pc = 0; pc < 3; ++pc)
-#pragma unroll
-            for (int ks = 0; ks < 2; ++ks)
-              if (!FZ_KNOCK(1) || (pc | ks) == 0)
-              fz_mma_f16_ss(d, fz_desc_sw128(x_s + ks * 2048, 4096, 1024),
-                            tc::make_smem_desc(w_s + pc * 2048 + ks * 1024, 512, 128), idesc_c, (pc | ks) ? 1u : 0u);
-        }
-        tc::mma_commit(&sm.x_free[fz_bar(S)]);
-        {
-          // C2R stage: the constant E is the same for every tile, so BOTH tiles of the super-slot go through one N = 64
-          // instruction per K step -- their Zt operands are two 128-byte column blocks kFzBtBytes apart (the descriptor's
-          // MN-direction stride), their accumulators two adjacent 32-column blocks: 18 MMAs instead of 36.
-          static_assert(kFzTS == 2, "the C2R MMAs cover exactly two tiles");
-          constexpr uint32_t idesc_e2 = tc::make_idesc_tf32(128, 64) | kBMajorMN;
-          const uint32_t d = tmem + kFzColD2 + (ss * kFzTS) * 32;
-          const uint32_t z_hi = tc::smem_addr(sm.bt[ss][0]), z_lo = z_hi + 6144;
-#pragma unroll
-          for (int pass = 0; pass < 3; ++pass) {
-            const uint32_t a_t = tmem + kFzColE + ((pass == 1) ? 48u : 0u);
-            const uint32_t b_s = (pass == 2) ? z_lo : z_hi;
-#pragma unroll
-            for (int ks = 0; ks < 6; ++ks)
-              if (!FZ_KNOCK(2))
-              fz_mma_tf32_ts(d, a_t + ks * 8, fz_desc_sw128_32(b_s + ks * 1024, kFzBtBytes, 512), idesc_e2, 1u);
-          }
-        }
-        tc::mma_commit(&sm.slot_free[fz_bar(S)]);
-        tc::mma_commit(&sm.d2_full[fz_bar(S)]);
-        tc::mma_commit(&sm.pace[fz_bar(S)]);
-        FZ_T(2, S, 5);
-      }
-    }
-    __syncwarp();
-  }
-  // ================================================================ MMA issue: GEMM1 (its own thread: a 24 KB stage load
-  // takes ~1300 cycles from DRAM, which must not hold up the tile MMAs; the tensor pipe interleaves the two streams)
-  else if (warp == kFzG1Warp) {
-    if (tc::elect_one()) {
-      const uint32_t f_hi = tc::smem_addr(sm.f), f_lo = f_hi + kFzFBytes / 2;
-      int pace_next = 0;   // first super-tile whose completion this thread has not consumed yet
-      mbar_wait(&sm.f_bar, 0);   // twiddle operand (prologue bulk copy)
-      constexpr uint32_t idesc_g64 = tc::make_idesc_tf32(128, 64) | kAMajorMN;
-      constexpr uint32_t idesc_g32 = tc::make_idesc_tf32(128, 32) | kAMajorMN;
-#pragma unroll 1
-      for (int k = 0; k < n_mine; ++k) {
-        const uint32_t neg = (unit_of(k) & 1) ? kANegate : 0u;   // second half image: odd kx change sign
-        // a split item needs only the 32 columns (16 rows x re|im) of its rows: N = 32 at column / B-row offset 32 hh
-        const bool half_item = item_ns(k) < kFzSPU;
-        const uint32_t col0 = half_item ? static_cast<uint32_t>(item_s0(k) / 4) * 32u : 0u;
-        const uint32_t idesc_g1 = half_item ? idesc_g32 : idesc_g64;
-        if (k >= 1) {   // the converters have pulled the previous unit's D1 out of tensor memory (at their tile 8)
-          mbar_wait(&sm.d1_free, (k - 1) & 1);
-          tc::fence_after_thread_sync();
-        }
-#pragma unroll 1
-        for (int st = 0; st < 6; ++st) {
-          // pacing: the stages of unit k >= 1 go behind super-tiles 1..6 of unit k-1 -- after the converters have released
-          // D1 (d1_free, around super-tile 1) and before they want the new D1 (three super-tiles ahead of the MMAs).  This
-          // thread observes EVERY phase of the pace barriers, in order, and never falls 6 super-tiles (one barrier period) behind
-          // the MMAs: it resumes at super-tile 7 of unit k-1 when d1_free(k) arrives, i.e. while the MMAs are at super-tiles 1..3
-          // of unit k.  (Schedules that stop consuming earlier -- two stages per super-tile behind super-tiles 0..3 -- fall
-          // behind by a full period, alias the one-bit parity and hang; measured gain of the tighter safe schedule: 0.25 %.)
-          if (k >= 1) {
-            const int s_hi = (k - 1) * kFzSPU + 1 + st;   // one stage behind each of super-tiles 1..6 (A/B on one box: 2..5 0.4 % slower)
-            for (; pace_next <= s_hi && pace_next < n_super_all; ++pace_next)
-              mbar_wait(&sm.pace[fz_bar(pace_next)], fz_phase(pace_next));
-          }
-          const int c = k * 6 + st, slot = c % kFzNY;
-          const int mt = st >> 1, par = st & 1;
-          FZ_T(3, k * 8 + st, 0);
-          mbar_wait(&sm.y_full[slot], (c / kFzNY) & 1);
-          tc::fence_after_thread_sync();
-          FZ_T(3, k * 8 + st, 1);
-          const uint32_t a_hi = tc::smem_addr(sm.y[slot]), a_lo = a_hi + kFzYStage / 2;
-          const uint32_t d = tmem + kFzColD1 + mt * 64 + col0;
-          const uint32_t idesc = idesc_g1 | (par ? neg : 0u);
-#pragma unroll
-          for (int pass = 0; pass < 3; ++pass) {
-            const uint32_t a_s = (pass == 1) ? a_lo : a_hi;
-            const uint32_t b_s = (pass == 2) ? f_lo : f_hi;
-#pragma unroll
-            for (int ks = 0; ks < 3; ++ks) {
-              const uint64_t da = fz_desc_sw128_32(a_s + ks * 1024, 3072, 512);
-              const uint64_t db = tc::make_smem_desc(b_s + (3 * par + ks) * 2048 + (col0 >> 3) * 128, 1024, 128);
-              if (!FZ_KNOCK(4)) fz_mma_tf32_ss(d, da, db, idesc, (par | pass | ks) ? 1u : 0u);
-            }
-          }
-          tc::mma_commit(&sm.y_empty[slot]);
-          FZ_T(3, k * 8 + st, 2);
-        }
-        tc::mma_commit(&sm.d1_full);
-      }
-    }
-    __syncwarp();
-  }
-  // ================================================================ producers
-  else if (warp == kFzProdWarp) {
-    if (lane == 0) {          // x tiles: two {64 px, 32 ch} boxes per tile, kFzTS tiles per super-slot
-      const int n_super = n_super_all;
-      for (int S = 0; S < n_super; ++S) {
-        const int ss = S % kFzR;
-        const int u = super_unit(S), t0 = super_local(S) * kFzTS;
-        const int b = u >> 1;
-        if (S >= kFzR) mbar_wait(&sm.x_free[fz_bar(S - kFzR)], fz_phase(S - kFzR));
-        uint64_t* rdy = &sm.ready[fz_bar(S)];
-        mbar_expect_tx(rdy, kFzTS * kFzXBytes);
-#pragma unroll
-        for (int i = 0; i < kFzTS; ++i) {
-          const int px0 = (u & 1) * 2048 + (t0 + i) * 128;
-          fz_tma_load_2d(sm.x[ss][i], &x_map, px0, b * kC, rdy);
-          fz_tma_load_2d(sm.x[ss][i] + 4096, &x_map, px0 + 64, b * kC, rdy);
-        }
-      }
-    } else if (lane == 1) {   // mode images: per (M-tile, kx parity) 8 runs of 24 rows x 128 B
-      for (int k = 0; k < n_mine; ++k) {
-        const unsigned char* img = ym_img + static_cast<size_t>(unit_of(k) >> 1) * kYmImgBytes;
-        for (int st = 0; st < 6; ++st) {
-          const int c = k * 6 + st, slot = c % kFzNY;
-          const int mt = st >> 1, par = st & 1;
-          mbar_wait(&sm.y_empty[slot], ((c / kFzNY) & 1) ^ 1);
-          mbar_expect_tx(&sm.y_full[slot], kFzYStage);
-#pragma unroll
-          for (int part = 0; part < 2; ++part)
-#pragma unroll
-            for (int g = 0; g < 4; ++g)
-              bulk_g2s(sm.y[slot] + part * (kFzYStage / 2) + g * 3072,
-                       img + part * kYmImgPart + mt * kYmImgMtile + g * kYmImgGroup + par * 3072, 3072, &sm.y_full[slot]);
-        }
-      }
-    }
-    __syncwarp();
+    return;
   }
 
-  tc::fence_before_thread_sync();
-  __syncthreads();
-#ifdef FNO_FZ_TRACE
-  if (fz_tr != nullptr && threadIdx.x == 0) fz_tr[4 * 256 * 8 + blockIdx.x * 4 + 2] = clock64();
-#endif
-  if (warp == kFzMmaWarp) tc::tmem_dealloc<512>(tmem);
+  // ================================================================ consumers
+  const int g = warp >> 2, wq = warp & 3, q = lane & 3, t = tid & 127;
+  const int m0 = 16 * wq + (lane >> 2);   // fragment rows m0, m0 + 8
+  for (int u = 0; u < n_units; ++u) {
+    const int b = b0 + u * bstride;
+    // ---------------------------------------------------------------- GEMM1: ky pairs g, g + 2, g + 4
+    for (int pi = 0; pi < 3; ++pi) {
+      const int p = g + 2 * pi, f = 3 * u + pi;
+      mbar_wait(&sm.y_full[g], f & 1);
+      // A[m = (ky - 2p) * 32 + o][kk] = image[ky][kk][o]: line kk, 32-byte chunk (o / 8) ^ (kk & 3)
+      uint32_t a_hi[6][4], a_lo[6][4];
+#pragma unroll
+      for (int ks = 0; ks < kImgK / 8; ++ks)
+#pragma unroll
+        for (int r = 0; r < 4; ++r) {
+          const int m = m0 + 8 * (r & 1), kk = 8 * ks + q + 4 * (r >> 1), o = m & 31;
+          const uint32_t off = (m >> 5) * 6144 + kk * 128 + (((o >> 3) ^ (kk & 3)) << 5) + (o & 7) * 4;
+          a_hi[ks][r] = *reinterpret_cast<const uint32_t*>(sm.y[g] + off);
+          a_lo[ks][r] = *reinterpret_cast<const uint32_t*>(sm.y[g] + kFzStage / 2 + off);
+        }
+      float acc[16];
+      tc::wg_fence();
+#pragma unroll
+      for (int pass = 0; pass < 3; ++pass) {   // Y_hi F_hi + Y_lo F_hi + Y_hi F_lo
+        const uint32_t fb = tc::smem_addr(pass == 2 ? sm.f_lo : sm.f_hi);
+#pragma unroll
+        for (int ks = 0; ks < kImgK / 8; ++ks)
+          tc::wg_tf32_rs_n32(acc, pass == 1 ? a_lo[ks] : a_hi[ks], tc::make_smem_desc(fb + ks * 2 * kLboF, kLboF, 128),
+                             (pass | ks) ? 1u : 0u);
+      }
+      tc::wg_commit();
+      tc::wg_wait<0>();
+      tc::wg_fence_acc(acc);
+      // the MMAs have consumed the fragments loaded from the stage: the producer may refill it
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&sm.y_free[g]);
+      if (pi == 0) tc::named_barrier(1, 256);   // both warpgroups are done with the previous unit's Zt
+      // acc[4 i + 2 hh + e] = Z1[m0 + 8 hh][n = 8 i + 2 q + e]: row h' = 4 i + q, re|im = e
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const int m = m0 + 8 * hh, ky = 2 * p + (m >> 5), o = m & 31;
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            float v = acc[4 * i + 2 * hh + e];
+            if (ky == 0 && e == 1) v = sm.bias[o];   // Im of ky = 0: C2R ignores it, the E column there is 1
+            float hi, lo;
+            tc::split_tf32(v, hi, lo);
+            const uint32_t off = tc::kmajor_offset(o, 2 * ky + e, kC) / 4;
+            sm.zt[4 * i + q][0][off] = hi;
+            sm.zt[4 * i + q][1][off] = lo;
+          }
+      }
+    }
+    tc::fence_proxy_async_smem();
+    tc::named_barrier(1, 256);   // Zt of all 16 rows is complete
+
+    // ---------------------------------------------------------------- GEMM2: rows g, g + 2, ..., 14 + g
+    __nv_bfloat16 xr[4][4];   // task = rep * 128 + t -> (pixel w = task & 63, channel quad = task >> 6)
+    auto x_prefetch = [&](int h) {
+#pragma unroll
+      for (int rep = 0; rep < 4; ++rep) {
+        const int task = rep * 128 + t, w = task & 63, kq = task >> 6;
+        const __nv_bfloat16* src = x + (static_cast<size_t>(b) * kC + 4 * kq) * kHW + h * kW + w;
+#pragma unroll
+        for (int c = 0; c < 4; ++c) xr[rep][c] = src[static_cast<size_t>(c) * kHW];
+      }
+    };
+    x_prefetch(kFzRows * chunk + g);
+    for (int r = 0; r < kFzRows / 2; ++r) {
+      const int hl = g + 2 * r, h = kFzRows * chunk + hl;
+#pragma unroll
+      for (int rep = 0; rep < 4; ++rep) {
+        const int task = rep * 128 + t, w = task & 63, kq = task >> 6;
+        *reinterpret_cast<float4*>(sm.ax[g] + tc::kmajor_offset(w, 4 * kq, kW) / 4) =
+            make_float4(__bfloat162float(xr[rep][0]), __bfloat162float(xr[rep][1]), __bfloat162float(xr[rep][2]),
+                        __bfloat162float(xr[rep][3]));
+      }
+      tc::fence_proxy_async_smem();
+      tc::named_barrier(2 + g, 128);
+      if (r + 1 < kFzRows / 2) x_prefetch(h + 2);
+      float acc[16];
+      tc::wg_fence();
+      {
+        const uint32_t a_e[3] = {tc::smem_addr(sm.e_hi), tc::smem_addr(sm.e_lo), tc::smem_addr(sm.e_hi)};
+        const uint32_t b_z[3] = {tc::smem_addr(sm.zt[hl][0]), tc::smem_addr(sm.zt[hl][0]), tc::smem_addr(sm.zt[hl][1])};
+#pragma unroll
+        for (int pass = 0; pass < 3; ++pass)
+#pragma unroll
+          for (int ks = 0; ks < kZK / 8; ++ks)
+            tc::wg_tf32_ss_n32(acc, tc::make_smem_desc(a_e[pass] + ks * 2 * kLboE, kLboE, 128),
+                               tc::make_smem_desc(b_z[pass] + ks * 2 * kLboO, kLboO, 128), (pass | ks) ? 1u : 0u);
+        const uint32_t a_x = tc::smem_addr(sm.ax[g]);
+#pragma unroll
+        for (int pass = 0; pass < 2; ++pass) {
+          const uint32_t b_w = tc::smem_addr(pass ? sm.wb_lo : sm.wb_hi);
+#pragma unroll
+          for (int ks = 0; ks < kC / 8; ++ks)
+            tc::wg_tf32_ss_n32(acc, tc::make_smem_desc(a_x + ks * 2 * kLboE, kLboE, 128),
+                               tc::make_smem_desc(b_w + ks * 2 * kLboO, kLboO, 128), 1u);
+        }
+      }
+      tc::wg_commit();
+      tc::wg_wait<0>();
+      tc::wg_fence_acc(acc);
+      // acc[4 i + 2 hh + e] = D[w = m0 + 8 hh][o = 8 i + 2 q + e].  Lane ^ 4 holds pixel w ^ 1: the even pixel's lane stores
+      // channel o of both pixels, the odd one channel o + 1, as bf16x2.
+      const bool odd = (lane >> 2) & 1;
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+          const float2 v = gelu_erf2(make_float2(acc[4 * i + 2 * hh], acc[4 * i + 2 * hh + 1]));
+          const float recv = __shfl_xor_sync(0xffffffffu, odd ? v.x : v.y, 4);
+          const int w = m0 + 8 * hh, o = 8 * i + 2 * q + (odd ? 1 : 0);
+          const __nv_bfloat162 pair = odd ? __floats2bfloat162_rn(recv, v.y) : __floats2bfloat162_rn(v.x, recv);
+          *reinterpret_cast<__nv_bfloat162*>(out + (static_cast<size_t>(b) * kC + o) * kHW + h * kW + (w & ~1)) = pair;
+        }
+    }
+  }
 }
 
 // ------------------------------------------------------------------------------------------------
 // Constant tables, built once per device in float64 and split into tf32 hi/lo (round to nearest).
-//   etab[96][128] (column-major): row m = 64 j + w of the A operand (E (+) E): columns 0..47 hi, 48..95 lo; column k = 24 j' + 2 ky + ri:
-//                c_ky/4096 * cos(2 pi ky w/64) (ri = 0), -c_ky/4096 * sin(..) (ri = 1), 0 for j != j';
-//                the (ky = 0, ri = 1) column is 1 (bias row of the B operand).   c_0 = 1, c_ky = 2 (Hermitian fold).
-//   ftab: B operand of GEMM1, [n = 2 h' + ri (64)][k = 24 p + 2 q + ri' (48)], kxi = 2 q + p, kx = kxi (< 12) or kxi + 40:
-//         (ri,ri') = (0,0): cos t, (0,1): -sin t, (1,0): sin t, (1,1): cos t,  t = 2 pi kx h'/64;  K-major hi image | lo image.
+//   etab: the C2R operand of fno_block_tc.cu with c_ky/HW folded in (c_0 = 1, c_ky = 2: Hermitian fold).
+//   ftab: per chunk c, B operand of GEMM1 [n = 2 h' + ri (32)][k = 24 (kxi & 1) + 2 (kxi >> 1) + ri' (48)], h = 16 c + h',
+//         kx = kxi (< 12) or kxi + 40: (ri,ri') = (0,0): cos t, (0,1): -sin t, (1,0): sin t, (1,1): cos t,
+//         t = 2 pi kx h/64;  K-major hi image | lo image.
 // ------------------------------------------------------------------------------------------------
+void c2r_operand_table(float* host, double s0, double s1);
+
 static float fz_round_tf32_host(double v) {
   float f = static_cast<float>(v);
   uint32_t u;
@@ -526,35 +263,22 @@ static cudaError_t fz_ensure(int dev, cudaStream_t stream) {
   FzTables& t = g_fz[dev];
   if (t.configured) return cudaSuccess;
   const double two_pi = 6.283185307179586476925286766559;
-  static float h_e[128 * 96];
-  static float h_f[2 * 64 * 48];
-  for (int m = 0; m < 128; ++m) {
-    const int j = m >> 6, w = m & 63;
-    for (int k = 0; k < 48; ++k) {
-      const int jj = k / 24, ky = (k % 24) >> 1, ri = k & 1;
-      double val = 0.0;
-      if (jj == j) {
-        const double c = (ky == 0 ? 1.0 : 2.0) / 4096.0, ang = two_pi * ((ky * w) % 64) / 64.0;
-        val = ri == 0 ? c * cos(ang) : (ky == 0 ? 1.0 : -c * sin(ang));
+  static float h_e[kFzEFloats];
+  static float h_f[kFzChunks * kFzFFloats];
+  c2r_operand_table(h_e, 1.0 / kHW, 2.0 / kHW);
+  for (int c = 0; c < kFzChunks; ++c)
+    for (int n = 0; n < 2 * kFzRows; ++n) {
+      const int h = kFzRows * c + (n >> 1), ri = n & 1;
+      for (int k = 0; k < kImgK; ++k) {
+        const int rip = k & 1, kxi = 2 * ((k % 24) >> 1) + k / 24, kx = kxi < kM1 ? kxi : kxi + (kH - kKX);
+        const double ang = two_pi * ((kx * h) % 64) / 64.0;
+        const double val = (ri == rip) ? cos(ang) : (ri == 0 ? -sin(ang) : sin(ang));
+        const float hi = fz_round_tf32_host(val);
+        const uint32_t off = tc::kmajor_offset(n, k, 2 * kFzRows) / 4;
+        h_f[c * kFzFFloats + off] = hi;
+        h_f[c * kFzFFloats + kFzFFloats / 2 + off] = fz_round_tf32_host(val - static_cast<double>(hi));
       }
-      const float hi = fz_round_tf32_host(val);
-      h_e[k * 128 + m] = hi;                                                        // column-major: [column][row]
-      h_e[(48 + k) * 128 + m] = fz_round_tf32_host(val - static_cast<double>(hi));
     }
-  }
-  for (int n = 0; n < 64; ++n) {
-    const int hp = n >> 1, ri = n & 1;
-    for (int k = 0; k < 48; ++k) {
-      const int p = k / 24, q = (k % 24) >> 1, rip = k & 1;
-      const int kxi = 2 * q + p, kx = kxi < 12 ? kxi : kxi + 40;
-      const double ang = two_pi * ((kx * hp) % 64) / 64.0;
-      const double val = (ri == rip) ? cos(ang) : (ri == 0 ? -sin(ang) : sin(ang));
-      const float hi = fz_round_tf32_host(val);
-      const uint32_t off = tc::kmajor_offset(n, k, 64) / 4;
-      h_f[off] = hi;
-      h_f[64 * 48 + off] = fz_round_tf32_host(val - static_cast<double>(hi));
-    }
-  }
   cudaError_t e = cudaMalloc(&t.etab, sizeof(h_e));
   if (e != cudaSuccess) return e;
   e = cudaMalloc(&t.ftab, sizeof(h_f));
@@ -573,14 +297,6 @@ static cudaError_t fz_ensure(int dev, cudaStream_t stream) {
   return cudaSuccess;
 }
 
-#ifdef FNO_FZ_TRACE
-extern "C" int fno_debug_fused_knock(int bits) { return cudaMemcpyToSymbol(g_fz_knock, &bits, sizeof(bits)) == cudaSuccess ? 0 : 2; }
-extern "C" int fno_debug_fused_trace(void* p) {
-  long long* q = static_cast<long long*>(p);
-  return cudaMemcpyToSymbol(g_fz_trace, &q, sizeof(q)) == cudaSuccess ? 0 : 2;
-}
-#endif
-
 void block_fused_release(int dev) {
   if (dev < 0 || dev >= 64) return;
   FzTables& t = g_fz[dev];
@@ -588,8 +304,6 @@ void block_fused_release(int dev) {
   if (t.ftab) cudaFree(t.ftab);
   t = FzTables();
 }
-
-size_t ym_image_bytes(int batch) { return static_cast<size_t>(batch) * kYmImgBytes; }
 
 cudaError_t launch_block_fused(const void* ym_img, const void* x, const float* w0t, const float* bias, void* out, int batch,
                                cudaStream_t stream) {
@@ -599,17 +313,16 @@ cudaError_t launch_block_fused(const void* ym_img, const void* x, const float* w
   if (dev < 0 || dev >= 64) return cudaErrorInvalidDevice;
   e = fz_ensure(dev, stream);
   if (e != cudaSuccess) return e;
-  if ((reinterpret_cast<uintptr_t>(x) & 15) || (reinterpret_cast<uintptr_t>(ym_img) & 15)) return cudaErrorMisalignedAddress;
-  CUtensorMap map;
-  e = fz_make_map(x, batch, &map);
-  if (e != cudaSuccess) return e;
-  const int n_units = 2 * batch;
-  // few units: two CTAs per unit (the kernel splits a unit's rows between them)
-  const int n_sm = g_fz[dev].n_sm;
-  const int grid = 2 * n_units <= n_sm ? 2 * n_units : (n_units < n_sm ? n_units : n_sm);
-  return launch_chained(block_fused_kernel, dim3(grid), dim3(kFzThreads), sizeof(FzSmem), stream, map,
-                        static_cast<const unsigned char*>(ym_img), w0t, bias, static_cast<const float*>(g_fz[dev].etab),
-                        static_cast<const float*>(g_fz[dev].ftab), static_cast<__nv_bfloat16*>(out), n_units);
+  if ((reinterpret_cast<uintptr_t>(x) & 15) || (reinterpret_cast<uintptr_t>(ym_img) & 15) ||
+      (reinterpret_cast<uintptr_t>(out) & 3))
+    return cudaErrorMisalignedAddress;
+  // four CTAs (one per chunk of rows) per sample slot; the slots stride over the batch
+  const int slots_max = g_fz[dev].n_sm / kFzChunks;
+  const int slots = batch < slots_max ? batch : slots_max;
+  return launch_chained(block_fused_kernel, dim3(kFzChunks * slots), dim3(kFzThreads), sizeof(FzSmem), stream,
+                        static_cast<const unsigned char*>(ym_img), static_cast<const __nv_bfloat16*>(x), w0t, bias,
+                        static_cast<const float*>(g_fz[dev].etab), static_cast<const float*>(g_fz[dev].ftab),
+                        static_cast<__nv_bfloat16*>(out), batch);
 }
 
 }  // namespace fno

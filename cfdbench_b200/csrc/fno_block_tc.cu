@@ -5,15 +5,8 @@
 //
 // K3a  inv_kx_kernel   inverse DFT along kx of the 24 kept rows (codelet icfft64_in24_full, one thread per
 //                      (ky, o)), scaled by c_ky/HW, written as Z[b][h][k][o], k = 2 ky + (re|im): 196 KB/sample.
-// K3b  block_tc_kernel per tile of 128 consecutive pixels (2 image rows) one accumulation chain of UMMAs
-//          D[128 px][32 o] = [E (+) E | X] * [Z_h ; Z_h+1 ; W0^T]      K = 24 + 24 + 32, kind::tf32, 3xTF32
-//      E[w][k] = (cos, -sin)(2 pi ky w/64) is the C2R stage of the inverse transform as a constant matrix (its
-//      ky=0 imaginary column would be zero -- irfft2 drops Im of the DC column -- and carries the bias instead:
-//      E = 1 there, the B row = bias), block-diagonal over the two rows.
-//      Persistent CTA of two independent 256-thread pipelines; operands are prefetched into registers one tile
-//      ahead (coalesced), split into tf32 hi/lo (round-to-nearest) and written as K-major UMMA operands; the
-//      accumulator lives in TMEM (double buffered) and the epilogue (thread = pixel) applies the
-//      exact GELU (or the backward epilogues) and stores coalesced along w.
+// K3b  block_tc_kernel per image row: the C2R stage along w and the 1x1 convolution as one wgmma accumulation chain
+//                      (below), epilogue GELU (or the backward epilogues) from the accumulator registers.
 #include "fft_codelets.cuh"
 #include "fno_common.cuh"
 #include "tc_common.cuh"
@@ -62,42 +55,35 @@ cudaError_t launch_inv_kx(const void* ym, void* z, int batch, float s0, float s1
 }
 
 // ------------------------------------------------------------------------------------------------ K3b
-constexpr int kBtThreads = 512;  // two independent 256-thread tile pipelines
-constexpr int kBtGroup = 256;
-constexpr int kBtM = 128;        // pixels per tile (2 image rows)
-constexpr int kKE = 2 * kZK;     // 48: E-part K
-constexpr int kKConv = kC;       // 32: conv-part K
-constexpr uint32_t kLboA = (kBtM / 8) * 128;  // 2048
-constexpr uint32_t kLboB = (kC / 8) * 128;    // 512
-constexpr int kBtTilesPerSample = kHW / kBtM;  // 32
-constexpr int kETabFloats = 2 * kBtM * kKE;
-// Operand staging is done by warps 1..7 of a pipeline only: warp 0 issues the tile's ~30 MMAs in that time, so all
-// eight warps reach the group barrier together.
-constexpr int kBtWorkers = kBtGroup - 32;
-constexpr int kBtXTasks = kBtM * (kKConv / 4);               // 1024
-constexpr int kBtZTasks = kC * (kKE / 4);                    // 384
-constexpr int kBtXReps = (kBtXTasks + kBtWorkers - 1) / kBtWorkers;  // 5
-static_assert(2 * kBtWorkers >= kBtZTasks, "two z reps must cover the tile");
+constexpr int kBtWG = 4;                       // independent warpgroup pipelines per CTA
+constexpr int kBtThreads = 128 * kBtWG;
+constexpr int kBtM = kW;                       // pixels per tile: one image row
+constexpr int kKE = kZK;                       // 24: E-part K
+constexpr int kKConv = kC;                     // 32: conv-part K
+constexpr uint32_t kLboA = (kBtM / 8) * 128;   // 1024
+constexpr uint32_t kLboB = (kC / 8) * 128;     // 512
+constexpr int kBtTilesPerSample = kH;          // 64
+constexpr int kETabFloats = 2 * kBtM * kKE;    // hi image, then lo image
+constexpr int kBtXReps = kBtM * (kKConv / 4) / 128;   // 4 x-tasks per thread
+constexpr int kBtZTasks = kC * (kKE / 4);             // 192
+static_assert(2 * 128 >= kBtZTasks, "two z reps must cover the tile");
 
 struct BtSmem {
-  alignas(128) float e_hi[kBtM * kKE];        // A operand, E part (constant)            24,576 B
+  alignas(128) float e_hi[kBtM * kKE];              // A operand, E part (constant)       6,144 B
   alignas(128) float e_lo[kBtM * kKE];
-  alignas(128) float ax_hi[2][kBtM * kKConv]; // A operand, conv part, per pipeline      2 x 16,384 B
-  alignas(128) float ax_lo[2][kBtM * kKConv];
-  alignas(128) float bz_hi[2][kC * kKE];      // B operand, E part, per pipeline         2 x 6,144 B
-  alignas(128) float bz_lo[2][kC * kKE];
-  alignas(128) float wb_hi[kC * kKConv];      // B operand, conv part                    4,096 B
+  alignas(128) float wb_hi[kC * kKConv];            // B operand, conv part               4,096 B
   alignas(128) float wb_lo[kC * kKConv];
+  alignas(128) float ax_hi[kBtWG][kBtM * kKConv];   // A operand, conv part, per pipeline 8,192 B
+  alignas(128) float ax_lo[kBtWG][kBtM * kKConv];
+  alignas(128) float bz_hi[kBtWG][kC * kKE];        // B operand, E part, per pipeline    3,072 B
+  alignas(128) float bz_lo[kBtWG][kC * kKE];
   alignas(16) float bias[kC];
-  alignas(8) uint64_t mma_bar[2][2];
-  alignas(8) uint64_t etab_bar;
-  uint32_t tmem_base;
 };
 
 template <typename TAct>
 struct BtRegs {
-  TAct x[kBtXReps][4];  // task = rep*224 + wtid (< 1024) -> (pixel m = task & 127, channel quad = task >> 7)
-  float z[2][4];        // task = rep*224 + wtid (< 384)  -> (o = task & 31, k quad = task >> 5)
+  TAct x[kBtXReps][4];  // task = rep*128 + t -> (pixel m = task & 63, channel quad = task >> 6)
+  float z[2][4];        // task = rep*128 + t (< 192) -> (o = task & 31, k quad = task >> 5)
 };
 
 __device__ __forceinline__ float bt_to_float(float v) { return v; }
@@ -107,26 +93,22 @@ __device__ __forceinline__ void bt_store(__nv_bfloat16* p, float v) { *p = __flo
 
 template <typename TAct>
 __device__ __forceinline__ void bt_prefetch(BtRegs<TAct>& r, const TAct* __restrict__ x, const float* __restrict__ z,
-                                            int tile, int wtid) {
-  if (wtid < 0) return;
-  const int b = tile / kBtTilesPerSample, tt = tile % kBtTilesPerSample;
+                                            int tile, int t) {
+  const int b = tile / kBtTilesPerSample, h = tile % kBtTilesPerSample;
 #pragma unroll
   for (int rep = 0; rep < kBtXReps; ++rep) {
-    const int task = rep * kBtWorkers + wtid;
-    if (task < kBtXTasks) {
-      const int m = task & (kBtM - 1), kq = task >> 7;
-      const TAct* src = x + (static_cast<size_t>(b) * kC + 4 * kq) * kHW + tt * kBtM + m;
+    const int task = rep * 128 + t;
+    const int m = task & (kBtM - 1), kq = task >> 6;
+    const TAct* src = x + (static_cast<size_t>(b) * kC + 4 * kq) * kHW + h * kW + m;
 #pragma unroll
-      for (int c = 0; c < 4; ++c) r.x[rep][c] = __ldg(src + static_cast<size_t>(c) * kHW);
-    }
+    for (int c = 0; c < 4; ++c) r.x[rep][c] = __ldg(src + static_cast<size_t>(c) * kHW);
   }
 #pragma unroll
   for (int rep = 0; rep < 2; ++rep) {
-    const int task = rep * kBtWorkers + wtid;
+    const int task = rep * 128 + t;
     if (task < kBtZTasks) {
-      const int o = task & 31, kq = task >> 5;           // kq 0..11: row j = kq / 6, column quad (kq % 6)
-      const int j = kq / 6, kk0 = (kq % 6) * 4;
-      const float* src = z + ((static_cast<size_t>(b) * kH + 2 * tt + j) * kZK + kk0) * kC + o;
+      const int o = task & 31, kq = task >> 5;
+      const float* src = z + ((static_cast<size_t>(b) * kH + h) * kZK + 4 * kq) * kC + o;
 #pragma unroll
       for (int c = 0; c < 4; ++c) r.z[rep][c] = __ldg(src + c * kC);
     }
@@ -135,37 +117,34 @@ __device__ __forceinline__ void bt_prefetch(BtRegs<TAct>& r, const TAct* __restr
 
 template <typename TAct>
 __device__ __forceinline__ void bt_split_store(const BtRegs<TAct>& r, float* ax_hi, float* ax_lo, float* bz_hi,
-                                               float* bz_lo, const float* bias_s, int wtid) {
-  if (wtid < 0) return;
+                                               float* bz_lo, const float* bias_s, int t) {
 #pragma unroll
   for (int rep = 0; rep < kBtXReps; ++rep) {
-    const int task = rep * kBtWorkers + wtid;
-    if (task < kBtXTasks) {
-      const int m = task & (kBtM - 1), kq = task >> 7;
-      float hi[4], lo[4];
+    const int task = rep * 128 + t;
+    const int m = task & (kBtM - 1), kq = task >> 6;
+    float hi[4], lo[4];
 #pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        const float v = bt_to_float(r.x[rep][c]);
-        if constexpr (sizeof(TAct) == 4) tc::split_tf32(v, hi[c], lo[c]);
-        else hi[c] = v;  // bf16 is tf32-exact: no lo part
-      }
-      const uint32_t off = tc::kmajor_offset(m, 4 * kq, kBtM) / 4;
-      *reinterpret_cast<float4*>(ax_hi + off) = make_float4(hi[0], hi[1], hi[2], hi[3]);
-      if constexpr (sizeof(TAct) == 4) *reinterpret_cast<float4*>(ax_lo + off) = make_float4(lo[0], lo[1], lo[2], lo[3]);
+    for (int c = 0; c < 4; ++c) {
+      const float v = bt_to_float(r.x[rep][c]);
+      if constexpr (sizeof(TAct) == 4) tc::split_tf32(v, hi[c], lo[c]);
+      else hi[c] = v;  // bf16 is tf32-exact: no lo part
     }
+    const uint32_t off = tc::kmajor_offset(m, 4 * kq, kBtM) / 4;
+    *reinterpret_cast<float4*>(ax_hi + off) = make_float4(hi[0], hi[1], hi[2], hi[3]);
+    if constexpr (sizeof(TAct) == 4) *reinterpret_cast<float4*>(ax_lo + off) = make_float4(lo[0], lo[1], lo[2], lo[3]);
   }
 #pragma unroll
   for (int rep = 0; rep < 2; ++rep) {
-    const int task = rep * kBtWorkers + wtid;
+    const int task = rep * 128 + t;
     if (task < kBtZTasks) {
       const int o = task & 31, kq = task >> 5;
       float hi[4], lo[4];
 #pragma unroll
       for (int c = 0; c < 4; ++c) {
         float v = r.z[rep][c];
-        // K columns 1 and 25 (Im of the ky = 0 column, which the C2R stage ignores) carry the bias instead: the E
-        // table holds 1 there for the rows of the matching image row, so the MMA adds bias[o] to every pixel.
-        if (c == 1 && (kq == 0 || kq == 6)) v = bias_s[o];
+        // K column 1 (Im of the ky = 0 column, which the C2R stage ignores) carries the bias instead: the E table holds 1
+        // there, so the MMA adds bias[o] to every pixel.
+        if (c == 1 && kq == 0) v = bias_s[o];
         tc::split_tf32(v, hi[c], lo[c]);
       }
       const uint32_t off = tc::kmajor_offset(o, 4 * kq, kC) / 4;
@@ -175,142 +154,25 @@ __device__ __forceinline__ void bt_split_store(const BtRegs<TAct>& r, float* ax_
   }
 }
 
-template <int GRP>
-__device__ __forceinline__ void bt_group_barrier() {
-  asm volatile("bar.sync %0, %1;" ::"n"(GRP + 1), "n"(kBtGroup) : "memory");
-}
-
-template <typename TAct, int EPI, int GRP>
-__device__ __forceinline__ void bt_pipeline(BtSmem& sm, const float* __restrict__ z, const TAct* __restrict__ x,
-                                            TAct* __restrict__ out, float* __restrict__ pre_out,
-                                            const float* __restrict__ pre_in, int n_tiles) {
-  constexpr bool kBf16 = sizeof(TAct) == 2;
-  const int tid = threadIdx.x, lane = tid & 31;
-  const int gtid = tid & (kBtGroup - 1), gwarp = tc::warp_index_uniform() & 7;
-  const int wtid = gtid - 32;  // staging worker index; negative for the MMA-issuing warp
-  const uint32_t tmem_base = sm.tmem_base + GRP * (2 * kC);
-  constexpr uint32_t idesc = tc::make_idesc_tf32(kBtM, kC);
-
-  const int first = blockIdx.x, stride = gridDim.x;
-  const int n_cta = (first < n_tiles) ? (n_tiles - first + stride - 1) / stride : 0;
-  const int n_mine = (n_cta + 1 - GRP) / 2;
-  auto tile_of = [&](int it) { return first + (2 * it + GRP) * stride; };
-
-  // epilogue of local tile `it`: TMEM -> registers -> global.  Warps w and w+4 of the pipeline share TMEM lane
-  // quadrant w & 3 (pixels 32(w&3)..+31 of the tile) and take output channels 0..15 / 16..31.
-  auto epilogue = [&](int it) {
-    const int buf = it & 1;
-    mbar_wait(&sm.mma_bar[GRP][buf], (it >> 1) & 1);
-    tc::fence_after_thread_sync();
-    const int quad = gwarp & 3, half = gwarp >> 2;
-    const int tile = tile_of(it);
-    const int b = tile / kBtTilesPerSample, pix = (tile % kBtTilesPerSample) * kBtM + quad * 32 + lane;
-    float v[16];
-    {
-      uint32_t rr[16];
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(quad * 32) << 16) + buf * kC + half * 16;
-      asm volatile(
-          "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-          : "=r"(rr[0]), "=r"(rr[1]), "=r"(rr[2]), "=r"(rr[3]), "=r"(rr[4]), "=r"(rr[5]), "=r"(rr[6]), "=r"(rr[7]),
-            "=r"(rr[8]), "=r"(rr[9]), "=r"(rr[10]), "=r"(rr[11]), "=r"(rr[12]), "=r"(rr[13]), "=r"(rr[14]), "=r"(rr[15])
-          : "r"(taddr)
-          : "memory");
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-      for (int c = 0; c < 16; ++c) v[c] = __uint_as_float(rr[c]);
-    }
-    tc::fence_before_thread_sync();
-    const size_t base = (static_cast<size_t>(b) * kC + half * 16) * kHW + pix;
-#pragma unroll
-    for (int c = 0; c < 16; c += 2) {
-      float2 p = make_float2(v[c], v[c + 1]);
-      const size_t o0 = base + static_cast<size_t>(c) * kHW, o1 = o0 + kHW;
-      if constexpr (EPI == kEpiGelu || EPI == kEpiGeluSavePre) {  // the accumulator already includes the bias
-        if constexpr (EPI == kEpiGeluSavePre) {
-          pre_out[o0] = p.x;
-          pre_out[o1] = p.y;
-        }
-        p = gelu_erf2(p);
-      } else if constexpr (EPI == kEpiMulDgelu) {
-        p.x *= dgelu_erf(__ldg(pre_in + o0));
-        p.y *= dgelu_erf(__ldg(pre_in + o1));
-      }
-      bt_store(out + o0, p.x);
-      bt_store(out + o1, p.y);
-    }
-  };
-
-  BtRegs<TAct> regs;
-  if (n_mine > 0) bt_prefetch<TAct>(regs, x, z, tile_of(0), wtid);
-
-  for (int it = 0; it < n_mine; ++it) {
-    const int buf = it & 1;
-    // the single-buffered operands were last read by the MMAs of tile it-1: wait for them (normally long done)
-    if (it >= 1) mbar_wait(&sm.mma_bar[GRP][(it - 1) & 1], ((it - 1) >> 1) & 1);
-    bt_split_store<TAct>(regs, sm.ax_hi[GRP], sm.ax_lo[GRP], sm.bz_hi[GRP], sm.bz_lo[GRP], sm.bias, wtid);
-    tc::fence_proxy_async_smem();
-    tc::fence_before_thread_sync();
-    bt_group_barrier<GRP>();
-    tc::fence_after_thread_sync();
-    // prefetch AFTER the fence: the membar inside fence.proxy.async would otherwise wait for these loads
-    if (it + 1 < n_mine) bt_prefetch<TAct>(regs, x, z, tile_of(it + 1), wtid);
-    if (gwarp == 0) {
-      if (tc::elect_one()) {
-        // 3xTF32: pass 0 = hi*hi, pass 1 = lo*hi, pass 2 = hi*lo (A part, B part); all warp-uniform -> UR operands
-        const uint32_t d_tmem = tmem_base + buf * kC;
-        const uint32_t a_e[3] = {tc::smem_addr(sm.e_hi), tc::smem_addr(sm.e_lo), tc::smem_addr(sm.e_hi)};
-        const uint32_t b_z[3] = {tc::smem_addr(sm.bz_hi[GRP]), tc::smem_addr(sm.bz_hi[GRP]), tc::smem_addr(sm.bz_lo[GRP])};
-        const uint32_t a_x[3] = {tc::smem_addr(sm.ax_hi[GRP]), tc::smem_addr(sm.ax_lo[GRP]), tc::smem_addr(sm.ax_hi[GRP])};
-        const uint32_t b_w[3] = {tc::smem_addr(sm.wb_hi), tc::smem_addr(sm.wb_hi), tc::smem_addr(sm.wb_lo)};
-#pragma unroll
-        for (int pass = 0; pass < 3; ++pass) {
-          const uint64_t da0 = tc::make_smem_desc(a_e[pass], kLboA, 128);
-          const uint64_t db0 = tc::make_smem_desc(b_z[pass], kLboB, 128);
-#pragma unroll
-          for (int ks = 0; ks < kKE / 8; ++ks) {
-            const uint64_t da = da0 + ((ks * 2 * kLboA) >> 4), db = db0 + ((ks * 2 * kLboB) >> 4);
-            if (pass == 0 && ks == 0) tc::mma_tf32_imm<false>(d_tmem, da, db, idesc);
-            else tc::mma_tf32_imm<true>(d_tmem, da, db, idesc);
-          }
-          if (kBf16 && pass == 1) continue;  // conv-part A has no lo component
-          const uint64_t dx0 = tc::make_smem_desc(a_x[pass], kLboA, 128);
-          const uint64_t dw0 = tc::make_smem_desc(b_w[pass], kLboB, 128);
-#pragma unroll
-          for (int ks = 0; ks < kKConv / 8; ++ks)
-            tc::mma_tf32_imm<true>(d_tmem, dx0 + ((ks * 2 * kLboA) >> 4), dw0 + ((ks * 2 * kLboB) >> 4), idesc);
-        }
-        tc::mma_commit(&sm.mma_bar[GRP][buf]);
-      }
-      __syncwarp();
-    }
-    if (it >= 1) epilogue(it - 1);
-  }
-  if (n_mine >= 1) epilogue(n_mine - 1);
-}
-
+// K3b: per tile (one image row of one sample, 64 pixels) one warpgroup runs the accumulation chain
+//     D[64 px][32 o] = [E | X] * [Z_h ; W0^T]        K = 24 + 32, wgmma m64n32k8 tf32, 3xTF32
+// E[w][k] = (cos, -sin)(2 pi ky w/64) is the C2R stage of the inverse transform as a constant matrix (its ky=0 imaginary
+// column would be zero -- irfft2 drops Im of the DC column -- and carries the bias instead: E = 1 there, the B row = bias).
+// Four independent warpgroup pipelines per CTA; a pipeline prefetches the next tile's operands into registers while the
+// current tile's MMAs and epilogue run, splits them into tf32 hi/lo (round-to-nearest) and writes them as K-major operands.
 template <typename TAct, int EPI>
 __global__ void __launch_bounds__(kBtThreads, 1)
     block_tc_kernel(const float* __restrict__ z, const TAct* __restrict__ x, const float* __restrict__ w0t,
                     const float* __restrict__ bias, const float* __restrict__ etab, TAct* __restrict__ out,
                     float* __restrict__ pre_out, const float* __restrict__ pre_in, int n_tiles) {
+  constexpr bool kBf16 = sizeof(TAct) == 2;
   extern __shared__ __align__(1024) unsigned char smem_raw[];  // no pointer arithmetic: keeps LDS/STS addressing
   BtSmem& sm = *reinterpret_cast<BtSmem*>(smem_raw);
-  if ((smem_u32(smem_raw) & 127u) != 0) __trap();
-  const int tid = threadIdx.x, warp = tc::warp_index_uniform();
-  const int grp = warp >> 3;
+  const int tid = threadIdx.x, lane = tid & 31;
+  const int wg = tc::warp_index_uniform() >> 2, t = tid & 127, wq = (tid >> 5) & 3;
 
-  if (tid == 0) {
-#pragma unroll
-    for (int i = 0; i < 4; ++i) mbar_init(&sm.mma_bar[i >> 1][i & 1], 1);
-    mbar_init(&sm.etab_bar, 1);
-    fence_mbar_init();
-    // constant E operand (hi image then lo image, 48 KB): one TMA bulk copy straight into its UMMA layout
-    constexpr uint32_t kETabBytes = kETabFloats * sizeof(float);
-    static_assert(offsetof(BtSmem, e_lo) == offsetof(BtSmem, e_hi) + kETabBytes / 2, "e_hi / e_lo must be contiguous");
-    mbar_expect_tx(&sm.etab_bar, kETabBytes);
-    bulk_g2s(sm.e_hi, etab, kETabBytes, &sm.etab_bar);
-  }
-  if (warp == 0) tc::tmem_alloc<4 * kC>(&sm.tmem_base);
+  static_assert(offsetof(BtSmem, e_lo) == offsetof(BtSmem, e_hi) + kETabFloats * 2, "e_hi / e_lo must be contiguous");
+  for (int e = tid; e < kETabFloats; e += kBtThreads) sm.e_hi[e] = __ldg(etab + e);   // runs on into e_lo
   for (int e = tid; e < kC * kKConv; e += kBtThreads) {  // B[n = o][k = i] = W0[o][i] = w0t[i][o]
     const int i = e / kC, o = e % kC;
     float hi, lo;
@@ -321,26 +183,80 @@ __global__ void __launch_bounds__(kBtThreads, 1)
   }
   constexpr bool kHasBias = EPI == kEpiGelu || EPI == kEpiGeluSavePre;  // the adjoint epilogues take none
   if (tid < kC) sm.bias[tid] = (kHasBias && bias != nullptr) ? bias[tid] : 0.f;
-  tc::fence_proxy_async_smem();
-  tc::fence_before_thread_sync();
+  tc::fence_proxy_async_smem();   // the constant operands above are read by the tensor cores
   __syncthreads();
-  tc::fence_after_thread_sync();
-  mbar_wait(&sm.etab_bar, 0);
   pdl_wait();  // everything above touched only weights / the constant E table; z and x come from the chain
   pdl_launch_dependents();
-  if (grp == 0) bt_pipeline<TAct, EPI, 0>(sm, z, x, out, pre_out, pre_in, n_tiles);
-  else bt_pipeline<TAct, EPI, 1>(sm, z, x, out, pre_out, pre_in, n_tiles);
-  tc::fence_before_thread_sync();
-  __syncthreads();
-  if (warp == 0) tc::tmem_dealloc<4 * kC>(sm.tmem_base);
+
+  const int first = blockIdx.x * kBtWG + wg, stride = gridDim.x * kBtWG;
+  float* ax_hi = sm.ax_hi[wg];
+  float* ax_lo = sm.ax_lo[wg];
+  float* bz_hi = sm.bz_hi[wg];
+  float* bz_lo = sm.bz_lo[wg];
+  BtRegs<TAct> regs;
+  if (first < n_tiles) bt_prefetch<TAct>(regs, x, z, first, t);
+  for (int tile = first; tile < n_tiles; tile += stride) {
+    // this pipeline's operands were last read by the MMAs of its previous tile, which every thread waited for
+    bt_split_store<TAct>(regs, ax_hi, ax_lo, bz_hi, bz_lo, sm.bias, t);
+    tc::fence_proxy_async_smem();
+    tc::named_barrier(1 + wg, 128);
+    // prefetch AFTER the fence: the membar inside fence.proxy.async would otherwise wait for these loads
+    if (tile + stride < n_tiles) bt_prefetch<TAct>(regs, x, z, tile + stride, t);
+    float acc[16];
+    tc::wg_fence();
+    {
+      // 3xTF32: pass 0 = hi*hi, pass 1 = lo*hi, pass 2 = hi*lo (A part, B part)
+      const uint32_t a_e[3] = {tc::smem_addr(sm.e_hi), tc::smem_addr(sm.e_lo), tc::smem_addr(sm.e_hi)};
+      const uint32_t b_z[3] = {tc::smem_addr(bz_hi), tc::smem_addr(bz_hi), tc::smem_addr(bz_lo)};
+      const uint32_t a_x[3] = {tc::smem_addr(ax_hi), tc::smem_addr(ax_lo), tc::smem_addr(ax_hi)};
+      const uint32_t b_w[3] = {tc::smem_addr(sm.wb_hi), tc::smem_addr(sm.wb_hi), tc::smem_addr(sm.wb_lo)};
+#pragma unroll
+      for (int pass = 0; pass < 3; ++pass) {
+#pragma unroll
+        for (int ks = 0; ks < kKE / 8; ++ks)
+          tc::wg_tf32_ss_n32(acc, tc::make_smem_desc(a_e[pass] + ks * 2 * kLboA, kLboA, 128),
+                             tc::make_smem_desc(b_z[pass] + ks * 2 * kLboB, kLboB, 128), (pass | ks) ? 1u : 0u);
+        if (kBf16 && pass == 1) continue;  // conv-part A has no lo component
+#pragma unroll
+        for (int ks = 0; ks < kKConv / 8; ++ks)
+          tc::wg_tf32_ss_n32(acc, tc::make_smem_desc(a_x[pass] + ks * 2 * kLboA, kLboA, 128),
+                             tc::make_smem_desc(b_w[pass] + ks * 2 * kLboB, kLboB, 128), 1u);
+      }
+    }
+    tc::wg_commit();
+    tc::wg_wait<0>();
+    tc::wg_fence_acc(acc);
+    // epilogue: acc[4 i + 2 hh + e] = D[px = 16 wq + lane/4 + 8 hh][o = 8 i + 2 (lane%4) + e]
+    const int b = tile / kBtTilesPerSample, h = tile % kBtTilesPerSample;
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const int px = 16 * wq + (lane >> 2) + 8 * hh, o = 8 * i + 2 * (lane & 3);
+        float2 p = make_float2(acc[4 * i + 2 * hh], acc[4 * i + 2 * hh + 1]);
+        const size_t o0 = (static_cast<size_t>(b) * kC + o) * kHW + h * kW + px, o1 = o0 + kHW;
+        if constexpr (EPI == kEpiGelu || EPI == kEpiGeluSavePre) {  // the accumulator already includes the bias
+          if constexpr (EPI == kEpiGeluSavePre) {
+            pre_out[o0] = p.x;
+            pre_out[o1] = p.y;
+          }
+          p = gelu_erf2(p);
+        } else if constexpr (EPI == kEpiMulDgelu) {
+          p.x *= dgelu_erf(__ldg(pre_in + o0));
+          p.y *= dgelu_erf(__ldg(pre_in + o1));
+        }
+        bt_store(out + o0, p.x);
+        bt_store(out + o1, p.y);
+      }
+  }
 }
 
 // ------------------------------------------------------------------------------------------------
-// Constant A-operand image of the C2R stage: rows m = 64 j + w (j = row of the tile), columns
-// k = 24 j' + 2 ky + ri;  E = cos(2 pi ky w/64) (ri=0), -sin(2 pi ky w/64) (ri=1), zero for j != j'.  The
-// (ky=0, ri=1) column would be identically zero (C2R drops Im of the ky=0 column); it holds 1 instead and the
-// matching B row holds the conv bias, which folds the bias add into the MMA.
-// Built once per device in float64, split into tf32 hi/lo (round-to-nearest), laid out K-major.
+// Constant A-operand image of the C2R stage: rows m = w (one image row), columns k = 2 ky + ri;
+// E = c_ky cos(2 pi ky w/64) (ri=0), -c_ky sin(2 pi ky w/64) (ri=1), c_0 = s0, c_ky = s1 otherwise.  The (ky=0, ri=1)
+// column would be identically zero (C2R drops Im of the ky=0 column); it holds 1 instead and the matching B row holds
+// the conv bias, which folds the bias add into the MMA.  Built in float64, split into tf32 hi/lo (round-to-nearest),
+// laid out K-major: hi image then lo image.  Also the constant of block_fused_kernel (with s0 = 1/HW, s1 = 2/HW).
 // ------------------------------------------------------------------------------------------------
 static float round_tf32_host(double v) {
   float f = static_cast<float>(v);
@@ -349,6 +265,23 @@ static float round_tf32_host(double v) {
   u = (u + 0x1000u) & 0xffffe000u;  // round half away from zero on the magnitude (cvt.rna)
   memcpy(&f, &u, 4);
   return f;
+}
+
+void c2r_operand_table(float* host, double s0, double s1) {
+  for (int i = 0; i < kETabFloats; ++i) host[i] = 0.f;
+  for (int w = 0; w < kBtM; ++w)
+    for (int ky = 0; ky < kM2; ++ky) {
+      const double ang = 2.0 * 3.14159265358979323846 * ((ky * w) % 64) / 64.0;
+      const double c = ky == 0 ? s0 : s1;
+      const double val[2] = {c * cos(ang), ky == 0 ? 1.0 : -c * sin(ang)};  // ky = 0, ri = 1: the bias column
+      for (int ri = 0; ri < 2; ++ri) {
+        const float hi = round_tf32_host(val[ri]);
+        const float lo = round_tf32_host(val[ri] - static_cast<double>(hi));
+        const uint32_t off = tc::kmajor_offset(w, 2 * ky + ri, kBtM) / 4;
+        host[off] = hi;
+        host[kBtM * kKE + off] = lo;
+      }
+    }
 }
 
 static float* g_etab[64] = {nullptr};
@@ -360,22 +293,7 @@ static cudaError_t ensure_etab(const float** out, cudaStream_t stream) {
   if (dev < 0 || dev >= 64) return cudaErrorInvalidDevice;
   if (g_etab[dev] == nullptr) {
     static float host[kETabFloats];
-    for (int i = 0; i < kETabFloats; ++i) host[i] = 0.f;
-    for (int m = 0; m < kBtM; ++m) {
-      const int j = m >> 6, w = m & 63;
-      for (int ky = 0; ky < kM2; ++ky) {
-        const double ang = 2.0 * 3.14159265358979323846 * ((ky * w) % 64) / 64.0;
-        const double val[2] = {cos(ang), ky == 0 ? 1.0 : -sin(ang)};  // ky = 0, ri = 1: the bias column (B row = bias)
-        for (int ri = 0; ri < 2; ++ri) {
-          const int k = kZK * j + 2 * ky + ri;
-          const float hi = round_tf32_host(val[ri]);
-          const float lo = round_tf32_host(val[ri] - static_cast<double>(hi));
-          const uint32_t off = tc::kmajor_offset(m, k, kBtM) / 4;
-          host[off] = hi;
-          host[kBtM * kKE + off] = lo;
-        }
-      }
-    }
+    c2r_operand_table(host, 1.0, 1.0);   // Z arrives scaled by inv_kx
     float* d = nullptr;
     e = cudaMalloc(&d, sizeof(host));
     if (e != cudaSuccess) return e;
@@ -409,7 +327,8 @@ static cudaError_t launch_one(const void* z, const void* x, const float* w0t, co
   e = ensure_etab(&etab, stream);
   if (e != cudaSuccess) return e;
   const int n_tiles = batch * kBtTilesPerSample;
-  const int grid = n_tiles < 2 * n_sm ? (n_tiles + 1) / 2 : n_sm;
+  const int want = (n_tiles + kBtWG - 1) / kBtWG;
+  const int grid = want < n_sm ? want : n_sm;
   return launch_chained(kern, dim3(grid), dim3(kBtThreads), smem, stream, static_cast<const float*>(z),
                         static_cast<const TAct*>(x), w0t, bias, etab, static_cast<TAct*>(out), pre_out, pre_in, n_tiles);
 }

@@ -1,4 +1,4 @@
-// Shared definitions for the sm_100a FNO kernels (cfdbench_b200).
+// Shared definitions for the sm_90a FNO kernels (cfdbench_b200).
 //
 // Problem constants are the reference's FNO configuration (reference src/args.py:99-103,187-197:
 // 64x64 grid, fno_hidden_dim=32, fno_modes_x=fno_modes_y=12); the Python wrapper rejects anything
@@ -72,7 +72,7 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 // ------------------------------------------------------------------------------------------------
 // Programmatic dependent launch.  The six kernels of a rollout step form one dependency chain on one
 // stream; each is launched with cudaLaunchAttributeProgrammaticStreamSerialization so that its CTAs
-// may become resident -- and run their prologue: barrier init, TMEM allocation, weight staging --
+// may become resident -- and run their prologue: barrier init, constant tables, weight staging --
 // while the previous kernel drains.  Rules every chained kernel follows:
 //   * pdl_wait() (griddepcontrol.wait: the previous grid has completed and its writes are visible)
 //     comes before the first access to anything a kernel of the chain writes, and every CTA executes it;
@@ -80,10 +80,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 //     next kernel's prologue may read anything written two or more launches earlier (packed weights);
 //   * the prologue before pdl_wait() reads only weights / constant tables and writes only shared memory.
 // Without the launch attribute both instructions are no-ops, so the same kernels serve the training path.
-// Measured (B200, B=256, tools/pdl_sweep.py in the round-1 history): every kernel of the step carrying the
-// attribute is SLOWER (590 us/step) than none (556 us): the triple mode_mix -> inv_kx -> block_tc launched
-// early back to back costs ~10 us per layer.  With inv_kx launched normally (kEarly = false; it has no
-// prologue to overlap anyway) the step is 544 us, so that is the configuration shipped.
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
@@ -148,12 +144,18 @@ struct Act<__nv_bfloat16> {
   static __device__ __forceinline__ void st(__nv_bfloat16* p, float v) { *p = __float2bfloat16_rn(v); }
 };
 
+// Fused multiply-add on a pair of floats: two correctly rounded FFMA, so the pair form of the GELU / fc2 code gives
+// the same bits as the scalar form.
+__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
+  return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y));
+}
+
 // ------------------------------------------------------------------------------------------------
 // Exact (erf) GELU, nn.GELU() default (reference fno2d.py:147), evaluated without erff():
 //   GELU(x) = max(x,0) - 0.5|x| * erfc(|x|/sqrt2),   erfc(z) = 2^{p(z)}, p = degree-8 minimax fit
 // |exp2(p)-erfc| <= 1.5e-8 on [0,4.5]; beyond that erfc < 2e-10 and p keeps decreasing (no clamp needed).  In fp32 the result
 // is within 2.7e-7 abs of the float64 GELU (torch's own fp32 GELU: 1.3e-6), see tests/test_gelu.py.
-// One MUFU.EX2 + 8 FFMA per element, branch-free, and vectorises to FFMA2 on float2.
+// One MUFU.EX2 + 8 FFMA per element, branch-free.
 // ------------------------------------------------------------------------------------------------
 #define FNO_GELU_C0 2.1715042208825253e-08f
 #define FNO_GELU_C1 -1.6279093256885822f
@@ -200,11 +202,11 @@ __device__ __forceinline__ float dgelu_erf(float x) {
   return fmaf(x, pdf, cdf);
 }
 
-// Packed pair version (FFMA2 on sm_100).  The same polynomial re-expressed in a = |x| with the 1/2 folded into the
+// Pair version.  The same polynomial re-expressed in a = |x| with the 1/2 folded into the
 // exponent:  q(a) = p(a / sqrt2) - 1,  D_k = C_k 2^{-k/2} (D_0 = C_0 - 1),  so  2^{q(|x|)} = erfc(|x|/sqrt2) / 2  and
 //   GELU(x) = max(x,0) - |x| 2^{q(|x|)}.
-// Per pair: 9 FFMA2 on the fma pipe (the version in z = |x|/sqrt2 needed 12: two scalar FMULs for z, one FMUL2 for
-// -|x|/2), 2 MUFU, and |x| / max(x,0) on the alu pipe.  Accuracy is unchanged (2.7e-7 max abs, tests/test_host.py).
+// Per pair: 9 fma pairs (the version in z = |x|/sqrt2 needs 12), 2 MUFU, and |x| / max(x,0).  Accuracy is unchanged
+// (2.7e-7 max abs, tests/test_host.py).
 #define FNO_GELU_D0 -0.9999999782849578f
 #define FNO_GELU_D1 -1.1511057233512165f
 #define FNO_GELU_D2 -0.4592049091239145f
@@ -217,21 +219,20 @@ __device__ __forceinline__ float dgelu_erf(float x) {
 __device__ __forceinline__ float2 gelu_erf2(float2 x) {
   const float2 a = make_float2(fabsf(x.x), fabsf(x.y));
   float2 p = make_float2(FNO_GELU_D8, FNO_GELU_D8);
-  p = __ffma2_rn(p, a, make_float2(FNO_GELU_D7, FNO_GELU_D7));
-  p = __ffma2_rn(p, a, make_float2(FNO_GELU_D6, FNO_GELU_D6));
-  p = __ffma2_rn(p, a, make_float2(FNO_GELU_D5, FNO_GELU_D5));
-  p = __ffma2_rn(p, a, make_float2(FNO_GELU_D4, FNO_GELU_D4));
-  p = __ffma2_rn(p, a, make_float2(FNO_GELU_D3, FNO_GELU_D3));
-  p = __ffma2_rn(p, a, make_float2(FNO_GELU_D2, FNO_GELU_D2));
-  p = __ffma2_rn(p, a, make_float2(FNO_GELU_D1, FNO_GELU_D1));
-  p = __ffma2_rn(p, a, make_float2(FNO_GELU_D0, FNO_GELU_D0));
+  p = ffma2(p, a, make_float2(FNO_GELU_D7, FNO_GELU_D7));
+  p = ffma2(p, a, make_float2(FNO_GELU_D6, FNO_GELU_D6));
+  p = ffma2(p, a, make_float2(FNO_GELU_D5, FNO_GELU_D5));
+  p = ffma2(p, a, make_float2(FNO_GELU_D4, FNO_GELU_D4));
+  p = ffma2(p, a, make_float2(FNO_GELU_D3, FNO_GELU_D3));
+  p = ffma2(p, a, make_float2(FNO_GELU_D2, FNO_GELU_D2));
+  p = ffma2(p, a, make_float2(FNO_GELU_D1, FNO_GELU_D1));
+  p = ffma2(p, a, make_float2(FNO_GELU_D0, FNO_GELU_D0));
   const float2 h = make_float2(ex2_approx(p.x), ex2_approx(p.y));  // erfc(|x|/sqrt2) / 2
-  return __ffma2_rn(make_float2(-a.x, -a.y), h, make_float2(fmaxf(x.x, 0.f), fmaxf(x.y, 0.f)));
+  return ffma2(make_float2(-a.x, -a.y), h, make_float2(fmaxf(x.x, 0.f), fmaxf(x.y, 0.f)));
 }
 
-// Degree-5 variant of the packed GELU for the project kernel in bf16 storage mode (project_ws_kernel), whose epilogue -- 134 M
-// GELUs per launch at B=256 -- is bound by the fma pipe: a 3-register FFMA2 occupies it for 4 cycles, an immediate-operand
-// one for 2, and neither warp specialisation nor more instruction-level parallelism changed its 85 us (profiles/README.md).
+// Degree-5 variant of the pair GELU for the project kernel in bf16 storage mode (project_tc_kernel<bf16>), whose epilogue
+// -- 134 M GELUs per launch at B=256 -- is bound by the fma pipe; three fewer fma per element.
 // q(a) ~ log2(erfc(a/sqrt2)/2), weighted minimax fit of the GELU error on [0, 8], negative leading coefficient (2^q underflows
 // beyond the fit range, no clamp).  fp32 result within 6.4e-7 abs of the float64 GELU -- torch's own fp32 nn.GELU() is at
 // 1.3e-6 -- checked by tests/test_host.py.  Used ONLY where the output is not fed back through further layers in fp32
@@ -250,17 +251,17 @@ __device__ __forceinline__ void gelu_erf2_deg5_batch(float2 (&x)[N]) {
   constexpr float kE[6] = {FNO_GELU_E0, FNO_GELU_E1, FNO_GELU_E2, FNO_GELU_E3, FNO_GELU_E4, FNO_GELU_E5};
 #pragma unroll
   for (int i = 0; i < N; ++i)
-    p[i] = __ffma2_rn(make_float2(kE[5], kE[5]), make_float2(fabsf(x[i].x), fabsf(x[i].y)), make_float2(kE[4], kE[4]));
+    p[i] = ffma2(make_float2(kE[5], kE[5]), make_float2(fabsf(x[i].x), fabsf(x[i].y)), make_float2(kE[4], kE[4]));
 #pragma unroll
   for (int k = 3; k >= 0; --k)
 #pragma unroll
     for (int i = 0; i < N; ++i)
-      p[i] = __ffma2_rn(p[i], make_float2(fabsf(x[i].x), fabsf(x[i].y)), make_float2(kE[k], kE[k]));
+      p[i] = ffma2(p[i], make_float2(fabsf(x[i].x), fabsf(x[i].y)), make_float2(kE[k], kE[k]));
 #pragma unroll
   for (int i = 0; i < N; ++i) p[i] = make_float2(ex2_approx(p[i].x), ex2_approx(p[i].y));   // erfc(|x|/sqrt2) / 2
 #pragma unroll
   for (int i = 0; i < N; ++i)
-    x[i] = __ffma2_rn(make_float2(-fabsf(x[i].x), -fabsf(x[i].y)), p[i], make_float2(fmaxf(x[i].x, 0.f), fmaxf(x[i].y, 0.f)));
+    x[i] = ffma2(make_float2(-fabsf(x[i].x), -fabsf(x[i].y)), p[i], make_float2(fmaxf(x[i].x, 0.f), fmaxf(x[i].y, 0.f)));
 }
 
 // status codes of the C ABI

@@ -2,34 +2,21 @@
 //     x[b][c][64][64] (bf16)  ->  Xm[k][b][c]  (288 kept modes, complex64, mode-major).
 //
 // Replaces torch.fft.rfft2 + the two corner slices of the reference (src/models/fno/fno2d.py:62,73-78).
-// Both 1-D transforms are GEMMs against constant twiddle matrices, on a batch of 4 planes:
+// Both 1-D transforms are GEMMs against constant twiddle matrices, on a pair of planes (one sample, two channels):
 //
-//  stage A (along w):  G[(p,h)][(q,ri)] = sum_w x_p[h][w] * TA[(q,ri)][w],  q = 0..11,  TA = (cos, -sin)(2 pi q w/64)
-//      tcgen05.mma kind::f16, M = 128 (2 planes x 64 rows), K = 64.  The A operand IS the bf16 plane: one TMA box
-//      {64 w, 256 rows} with the 128-byte swizzle lands 4 planes as two K-major operands, no register pass, exact.
-//      TA is split into three bf16 terms (t1 + t2 + t3 carries 24 mantissa bits); the three terms are three column
-//      blocks of ONE N = 80 operand (72 used), so a plane pair costs 4 MMAs and the terms are added when the
-//      accumulator is read.
+//  stage A (along w):  G_p[h][(q,ri)] = sum_w x_p[h][w] * TA[(q,ri)][w],  q = 0..11,  TA = (cos, -sin)(2 pi q w/64)
+//      wgmma m64n72k16 bf16 per plane, K = 64.  The A operand IS the bf16 plane: one TMA box {64 w, 128 rows} with the
+//      128-byte swizzle lands both planes as K-major operands, no register pass, exact.  TA is split into three bf16 terms
+//      (t1 + t2 + t3 carries 24 mantissa bits); the terms are column blocks of ONE N = 72 operand, ordered so that the
+//      three terms of a column land in the same thread's accumulator registers, where they are added.
 //  stage B (along h):  F[(kxi,part)][(q,p)] = sum_{(ri,h)} A2[(kxi,part)][(ri,h)] * G_p[h][q][ri],  kxi = 0..23
-//      tcgen05.mma kind::tf32 as 3xTF32, N = 48 (12 q x 4 planes), K = 128.  A2 = (c, s | -s, c) is a constant that lives
-//      in TENSOR MEMORY for the whole kernel with its tf32 hi and lo parts STACKED IN M (lanes 0-15 / 16-31 of three lane
-//      quadrants hold 16 rows of A2_hi / the same rows of A2_lo): two passes over the B operand (G_hi, G_lo) of 16 MMAs each
-//      give all four hi/lo products, and a stage-B MMA reads only its 1.5 KB B operand from shared memory.  The B operand
-//      is stage A's accumulator, read from TMEM by the thread that owns row (p,h), split into tf32 hi (truncated) / lo
-//      (exact residual, rounded) and scattered K-major (4-byte stores, conflict-free through a skewed K stride).  Because
-//      x is real, G[h][-q] = conj(G[h][q]): only q >= 0 is computed and stage B produces all 24 kept kx rows
-//      (kx = 0..11 and 52..63) of the 12 kept columns directly.
-//  epilogue: drains the accumulator into registers at once (single D_B buffer, released immediately), adds the hi / lo
-//      row blocks (lane ^ 16), pairs the (kxi,re) / (kxi,im) lanes (lane ^ 1) and writes 16 bytes per lane and column.
+//      wgmma m64n24k8 tf32 as 3xTF32, K = 128; A2 = (c, s | -s, c) is a constant (48 rows, padded to 64) kept in shared
+//      memory for the whole kernel; the B operand is stage A's result, summed over the terms, split into tf32 hi / lo and
+//      written K-major.  Because x is real, G[h][-q] = conj(G[h][q]): only q >= 0 is computed and stage B produces all
+//      24 kept kx rows (kx = 0..11 and 52..63) of the 12 kept columns directly.
+//  epilogue: pairs the (kxi,re) / (kxi,im) rows (lane ^ 4) and writes (re, im) of one plane per lane.
 //
-// Warp-specialised, one persistent 832-thread CTA per SM, every hand-off an mbarrier (round 1's version of this kernel
-// ran the same two GEMMs from 16 worker warps that fetched, split and stored in turn: 43 us, latency-serial):
-//   warp 25 lane 0        producer: one 32 KB TMA per batch into a 3-slot ring (released when stage A has completed)
-//   warp 19               issues stage A (8 MMAs per batch) into one of two D_A buffers
-//   warps 0..15           converters: D_A -> registers (36 columns each) -> sum of terms -> tf32 hi/lo -> B2 (double buffered)
-//   warps 23, 24          issue stage B (32 MMAs per batch) for even / odd batches
-//   warps 16-18 / 20-22   two epilogue groups (lane quadrants 0..2 hold the 96 stacked result rows), alternate batches
-// Tensor time per batch ~ 8 x 55 + 32 x 26 cycles; 13.8 batches per SM at B = 256; 25 us per launch (DESIGN.md 4.2).
+// Persistent CTA of two independent warpgroup pipelines, each with a two-slot TMA ring of plane pairs.
 // The register-FFT kernel (fno_dft_fwd.cu) remains for fp32 storage and the fp32 gradients of the backward pass.
 #include "fno_common.cuh"
 #include "tc_common.cuh"
@@ -40,358 +27,152 @@
 
 namespace fno {
 
-constexpr int kTdThreads = 832;
-constexpr int kTdConvWarps = 16;
-constexpr int kTdEpiWarp0 = 16;      // group 0: warps 16, 17, 18; group 1: warps 20, 21, 22 (lane quadrants 0, 1, 2)
-constexpr int kTdMmaAWarp = 19, kTdMmaBWarp = 23 /* and 24: even / odd batches */, kTdProdWarp = 25;
-constexpr int kTdPlanes = 4;                               // planes per batch
-constexpr int kTdR = 3;                                    // x ring slots
-constexpr uint32_t kTdXBytes = kTdPlanes * kHW * 2;        // 32,768 B per batch
-constexpr int kTdNA = 80;                                  // stage A N: 3 terms x 24, padded to a multiple of 16
-constexpr uint32_t kTdLboTA = (kTdNA / 8) * 128;           // 1280: K stride of the TA operand (8-element chunks)
-constexpr uint32_t kTdTABytes = 8 * kTdLboTA;              // 10,240 B
-constexpr int kTdK2 = 128, kTdN2 = kTdPlanes * kM2;        // stage B: K = (ri, h), N = 48, column n2 = 4 q + p
-constexpr uint32_t kTdLboB2 = (kTdN2 / 8) * 128 + 16;      // 784: skewed so that lanes running along h do not collide
-constexpr uint32_t kTdB2Bytes = (kTdK2 / 4) * kTdLboB2;    // 25,088 B per image
-constexpr int kTdA2Rows = 96;                              // lanes of the A2 operand that are loaded (3 quadrants)
-// tensor memory columns
-constexpr uint32_t kTdColA2 = 0;      // A2: 128 columns (k2); hi and lo parts are stacked in M (see td_a2_lane)
-constexpr uint32_t kTdColDA = 128;    // 2 buffers x 2 plane pairs x 80
-constexpr uint32_t kTdColDB = 448;    // 48 (single: the epilogue drains it into registers while stage A of the next batch runs)
-constexpr int kTdTmemCols = 512;
-
-// Optional timeline trace (tools/trace_dft.py builds a -DFNO_FZ_TRACE variant of the library): CTA 0 records clock64() at
-// the hand-off points of every role: trace[(role * 64 + batch) * 8 + event]; per-CTA stamps follow at 5 * 64 * 8.
-#ifdef FNO_FZ_TRACE
-__device__ long long* g_td_trace = nullptr;
-// the pointer is read ONCE per thread (td_tr): re-reading the global for every stamp costs an L2 round trip (~450 cycles),
-// which is what the stamps of a single-thread role would then mostly measure
-#define TD_T(role, T, ev)                                                                          \
-  do {                                                                                             \
-    if (td_tr != nullptr && blockIdx.x == 0 && (T) < 64) td_tr[((role) * 64 + (T)) * 8 + (ev)] = clock64(); \
-  } while (0)
-#define TD_CTA(ev)                                                                                 \
-  do {                                                                                             \
-    if (td_tr != nullptr && threadIdx.x == 0) {                                                    \
-      td_tr[5 * 64 * 8 + blockIdx.x * 4 + (ev)] = clock64();                                       \
-      long long gt_;                                                                               \
-      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(gt_));                                      \
-      td_tr[5 * 64 * 8 + 148 * 4 + blockIdx.x * 4 + (ev)] = gt_;                                   \
-    }                                                                                              \
-  } while (0)
-__device__ int g_td_knock = 0;   // knock-out experiments (results are wrong): 1 no stage-B MMAs, 2 no converter stores, 4 no mode stores, 8 no stage-A MMAs
-#define TD_KNOCK(bit) ((td_knock & (bit)) != 0)
-#else
-#define TD_T(role, T, ev) do { } while (0)
-#define TD_CTA(ev) do { } while (0)
-#define TD_KNOCK(bit) false
-#endif
+constexpr int kTdWG = 2;
+constexpr int kTdThreads = 128 * kTdWG;
+constexpr int kTdPlanes = 2;                               // planes per unit
+constexpr uint32_t kTdPlaneBytes = kHW * 2;                // 8,192 B
+constexpr uint32_t kTdXBytes = kTdPlanes * kTdPlaneBytes;  // 16,384 B per unit
+constexpr int kTdNA = 72;                                  // stage A N: 3 terms x 24
+constexpr uint32_t kTdLboTA = (kTdNA / 8) * 128;           // 1152: K stride of the TA operand (8-element chunks)
+constexpr uint32_t kTdTABytes = 8 * kTdLboTA;              // 9,216 B
+constexpr int kTdK2 = 128, kTdN2 = kTdPlanes * kM2;        // stage B: K = (ri, h), N = 24, column n2 = 2 q + p
+constexpr int kTdM2 = 64;                                  // stage B rows (48 used)
+constexpr uint32_t kTdLboA2 = (kTdM2 / 8) * 128;           // 1024
+constexpr uint32_t kTdLboB2 = (kTdN2 / 8) * 128;           // 384
+constexpr int kTdA2Floats = kTdM2 * kTdK2;                 // per image (hi or lo)
 
 struct TdSmem {
-  alignas(1024) unsigned char x[kTdR][kTdXBytes];       // stage-A A operands (TMA, 128B swizzle)
+  alignas(1024) unsigned char x[kTdWG][2][kTdXBytes];   // stage-A A operands (TMA, 128B swizzle): [pipeline][slot]
   alignas(128) unsigned char ta[kTdTABytes];            // stage-A B operand: three bf16 terms, K-major
-  alignas(128) unsigned char b2[2][2][kTdB2Bytes];      // stage-B B operand: [buffer][tf32 hi, lo]
-  alignas(8) uint64_t x_full[kTdR], x_free[kTdR];
-  uint64_t da_full[2], da_free[2];
-  uint64_t b2_ready[2], b2_free[2];
-  uint64_t db_full[2], db_free[2];
-  uint64_t ta_bar;
-  uint32_t tmem_base;
+  alignas(128) float a2_hi[kTdA2Floats];                // stage-B A operand, K-major
+  alignas(128) float a2_lo[kTdA2Floats];
+  alignas(128) float b2[kTdWG][2][kTdN2 * kTdK2];       // stage-B B operand: [pipeline][tf32 hi, lo]
+  alignas(8) uint64_t x_full[kTdWG][2];
 };
-
-__device__ __forceinline__ void td_ld4(uint32_t taddr, float* v) {   // 32 lanes x 4 columns, waits
-  uint32_t r0, r1, r2, r3;
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0, %1, %2, %3}, [%4];"
-               : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(taddr) : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-  v[0] = __uint_as_float(r0);
-  v[1] = __uint_as_float(r1);
-  v[2] = __uint_as_float(r2);
-  v[3] = __uint_as_float(r3);
-}
-__device__ __forceinline__ void td_ld16(uint32_t taddr, float* v) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
 
 __global__ void __launch_bounds__(kTdThreads, 1)
     dft_fwd_tc_kernel(const __grid_constant__ CUtensorMap x_map, float2* __restrict__ xm,
-                      const unsigned char* __restrict__ ta_tab, const float* __restrict__ a2_tab, int n_batches, int batch,
+                      const unsigned char* __restrict__ ta_tab, const float* __restrict__ a2_tab, int n_units, int batch,
                       float s0, float s1) {
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   TdSmem& sm = *reinterpret_cast<TdSmem*>(smem_raw);
   if ((smem_u32(smem_raw) & 1023u) != 0) __trap();
-  const int tid = threadIdx.x, lane = tid & 31, warp = tc::warp_index_uniform();
-#ifdef FNO_FZ_TRACE
-  long long* const td_tr = g_td_trace;
-  const int td_knock = g_td_knock;
-#endif
-  TD_CTA(0);
-
-  const int first = blockIdx.x, stride = gridDim.x;
-  const int n_mine = (first < n_batches) ? (n_batches - first + stride - 1) / stride : 0;
+  const int tid = threadIdx.x, lane = tid & 31;
+  const int wg = tc::warp_index_uniform() >> 2, wq = (tid >> 5) & 3, t = tid & 127, q = lane & 3;
+  const int first = blockIdx.x * kTdWG + wg, stride = gridDim.x * kTdWG;
+  const int n_mine = first < n_units ? (n_units - first + stride - 1) / stride : 0;
 
   // ---------------------------------------------------------------- prologue (constant tables only)
   if (tid == 0) {
-    for (int i = 0; i < kTdR; ++i) { mbar_init(&sm.x_full[i], 1); mbar_init(&sm.x_free[i], 1); }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&sm.da_full[i], 1);
-      mbar_init(&sm.da_free[i], kTdConvWarps);
-      mbar_init(&sm.b2_ready[i], kTdConvWarps);
-      mbar_init(&sm.b2_free[i], 1);
-      mbar_init(&sm.db_full[i], 1);
-      mbar_init(&sm.db_free[i], 3);
-    }
-    mbar_init(&sm.ta_bar, 1);
+    for (int i = 0; i < kTdWG; ++i) { mbar_init(&sm.x_full[i][0], 1); mbar_init(&sm.x_full[i][1], 1); }
     fence_mbar_init();
-    mbar_expect_tx(&sm.ta_bar, kTdTABytes);
-    bulk_g2s(sm.ta, ta_tab, kTdTABytes, &sm.ta_bar);
   }
-  if (warp == kTdMmaAWarp) tc::tmem_alloc<kTdTmemCols>(&sm.tmem_base);
-  // the A2 values of this thread are requested before the barrier: their L2 round trip overlaps the TMEM allocation
-  const bool loads_a2 = warp < kTdConvWarps && (warp & 3) < 3;
-  float a2v[32];
-  if (loads_a2) {
-    const int m = (warp & 3) * 32 + lane, cbase = (warp >> 2) * 32;
-#pragma unroll
-    for (int j = 0; j < 32; ++j) a2v[j] = __ldg(a2_tab + (cbase + j) * kTdA2Rows + m);
+  for (int e = tid; e < static_cast<int>(kTdTABytes / 16); e += kTdThreads)
+    reinterpret_cast<uint4*>(sm.ta)[e] = __ldg(reinterpret_cast<const uint4*>(ta_tab) + e);
+  for (int e = tid; e < kTdA2Floats / 4; e += kTdThreads) {
+    reinterpret_cast<float4*>(sm.a2_hi)[e] = __ldg(reinterpret_cast<const float4*>(a2_tab) + e);
+    reinterpret_cast<float4*>(sm.a2_lo)[e] = __ldg(reinterpret_cast<const float4*>(a2_tab + kTdA2Floats) + e);
   }
-  tc::fence_before_thread_sync();
+  tc::fence_proxy_async_smem();
   __syncthreads();
-  tc::fence_after_thread_sync();
-  const uint32_t tmem = sm.tmem_base;
-  if (loads_a2) {
-    // constant A2 operand -> tensor memory (lanes 96..127 of the M = 128 operand are never written: their products land
-    // in accumulator rows nobody reads).  The table is stored column-major in LANE order, so that a warp reads 128
-    // contiguous bytes per column; 4 warps per lane quadrant, 32 columns each.
-    const int cbase = (warp >> 2) * 32;
-#pragma unroll
-    for (int c0 = 0; c0 < 32; c0 += 16)
-      tc::tmem_st16(tmem + kTdColA2 + cbase + c0 + (static_cast<uint32_t>((warp & 3) * 32) << 16), a2v + c0);
-    tc::tmem_wait_st();
-  }
-  tc::fence_before_thread_sync();
-  __syncthreads();
-  tc::fence_after_thread_sync();
-  TD_CTA(1);
   pdl_wait();   // x comes from the previous kernel of the chain
   pdl_launch_dependents();
 
-  // ================================================================ converters
-  if (warp < kTdConvWarps) {
-    // thread = row (p, h) of stage A's result and 12 of its 24 columns (q = 6 hf + jj / 2, ri = jj & 1), three terms each.
-    // B2 element (n2 = 4 q + p, k2 = 64 ri + h): the byte offset is a per-thread constant plus a compile-time function of jj.
-    const int quad = warp & 3, g = (warp >> 2) & 1, hf = warp >> 3;
-    const int p = 2 * g + (quad >> 1), h = (quad & 1) * 32 + lane;
-    const uint32_t t_src0 = tmem + kTdColDA + g * kTdNA + hf * 36 + (static_cast<uint32_t>(quad * 32) << 16);
-    unsigned char* dst0 = sm.b2[0][0] + (h >> 2) * kTdLboB2 + (h & 3) * 4 + (3 * hf) * 128 + p * 16;
-    for (int i = 0; i < n_mine; ++i) {
-      if (tid == 0) TD_T(0, i, 0);
-      mbar_wait(&sm.da_full[i & 1], (i >> 1) & 1);
-      tc::fence_after_thread_sync();
-      if (tid == 0) TD_T(0, i, 1);
-      float v[36];
-      const uint32_t t_src = t_src0 + (i & 1) * (2 * kTdNA);
-      tc::tmem_ld32(t_src, v);
-      td_ld4(t_src + 32, v + 32);
-      tc::fence_before_thread_sync();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&sm.da_free[i & 1]);   // D_A drained: stage A of batch i + 2 may overwrite it
-      if (tid == 0) TD_T(0, i, 2);
-      // sum of the three terms and the tf32 split happen BEFORE the wait for the operand buffer: only the stores need it
-      // tf32 split with a truncated hi (one LOP; the residual is exact) and a rounded lo whose low bits the tensor core
-      // drops itself: 3 instructions per element instead of 5, |g - hi - lo| <= 2^-22 |g| as before
-      float hi[12], lo[12];
-#pragma unroll
-      for (int jj = 0; jj < 12; ++jj) {
-        const float gsum = (v[24 + jj] + v[12 + jj]) + v[jj];
-        hi[jj] = __uint_as_float(__float_as_uint(gsum) & 0xffffe000u);
-        lo[jj] = __uint_as_float(__float_as_uint(gsum - hi[jj]) + 0x1000u);
-      }
-      if (i >= 2) mbar_wait(&sm.b2_free[i & 1], ((i >> 1) - 1) & 1);   // stage B of batch i-2 has consumed this buffer
-      if (tid == 0) TD_T(0, i, 3);
-      unsigned char* hi_p = dst0 + (i & 1) * 2 * kTdB2Bytes;
-#pragma unroll
-      for (int jj = 0; jj < 12; ++jj) {
-        constexpr uint32_t kRiStep = 16 * kTdLboB2;  // k2 += 64
-        const uint32_t off = (jj & 1) * kRiStep + (jj >> 2) * 128 + ((jj >> 1) & 1) * 64;
-        if (TD_KNOCK(2)) continue;
-        *reinterpret_cast<float*>(hi_p + off) = hi[jj];
-        *reinterpret_cast<float*>(hi_p + kTdB2Bytes + off) = lo[jj];
-      }
-      tc::fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&sm.b2_ready[i & 1]);
-      if (tid == 0) TD_T(0, i, 4);
-    }
+  auto load = [&](int i) {   // unit i of this pipeline -> slot i & 1
+    mbar_expect_tx(&sm.x_full[wg][i & 1], kTdXBytes);
+    tma_load_2d(sm.x[wg][i & 1], &x_map, 0, (first + i * stride) * (kTdPlanes * kH), &sm.x_full[wg][i & 1]);
+  };
+  if (t == 0) {
+    if (n_mine > 0) load(0);
+    if (n_mine > 1) load(1);
   }
-  // ================================================================ epilogue
-  else if (warp >= kTdEpiWarp0 && warp < kTdEpiWarp0 + 8 && (warp & 3) < 3) {
-    // lane = 16 * part_of_A2 + r: lanes 0..15 hold rows m2 = 16 quad + r of A2_hi x G, lanes 16..31 the same rows of A2_lo x G
-    const int grp = (warp - kTdEpiWarp0) >> 2, quad = warp & 3;
-    const int m2 = quad * 16 + (lane & 15), kxi = m2 >> 1, part = m2 & 1, half = lane >> 4;
-    const uint32_t t_src = tmem + kTdColDB + (static_cast<uint32_t>(quad * 32) << 16);
-    const size_t q_stride = static_cast<size_t>(batch) * kC;
-    for (int i = grp; i < n_mine; i += 2) {
-      if (lane == 0 && quad == 0) TD_T(1, i, 0);
-      mbar_wait(&sm.db_full[grp], (i >> 1) & 1);
-      tc::fence_after_thread_sync();
-      if (lane == 0 && quad == 0) TD_T(1, i, 1);
-      // drain the accumulator first: (A2_hi + A2_lo) x G = this lane's value + the partner lane's (lane ^ 16); lanes 0..15
-      // keep the even columns q, lanes 16..31 the odd ones -> 24 values per lane
-      float keep[24];
-      {
-        uint32_t r[48];
-        asm volatile(
-            "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-            "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-            : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-              "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-              "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-              "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-            : "r"(t_src)
-            : "memory");
-        asm volatile(
-            "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-            : "=r"(r[32]), "=r"(r[33]), "=r"(r[34]), "=r"(r[35]), "=r"(r[36]), "=r"(r[37]), "=r"(r[38]), "=r"(r[39]),
-              "=r"(r[40]), "=r"(r[41]), "=r"(r[42]), "=r"(r[43]), "=r"(r[44]), "=r"(r[45]), "=r"(r[46]), "=r"(r[47])
-            : "r"(t_src + 32)
-            : "memory");
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        tc::fence_before_thread_sync();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&sm.db_free[grp]);   // the accumulator is in registers: stage B of the next batch may start
-#pragma unroll
-        for (int q = 0; q < kM2; ++q)
-#pragma unroll
-          for (int pl = 0; pl < 4; ++pl) {
-            const float fv = __uint_as_float(r[4 * q + pl]);
-            const float sum = fv + __shfl_xor_sync(0xffffffffu, fv, 16);
-            if ((q & 1) == 0) { if (!half) keep[4 * (q >> 1) + pl] = sum; } else { if (half) keep[4 * (q >> 1) + pl] = sum; }
-          }
-      }
-      if (lane == 0 && quad == 0) TD_T(1, i, 2);
-      const size_t plane0 = static_cast<size_t>(first + i * stride) * kTdPlanes;
-      const int b = static_cast<int>(plane0 / kC), c0 = static_cast<int>(plane0 % kC);
-      float2* dst = xm + ((static_cast<size_t>(kxi) * kM2 + half) * batch + b) * kC + c0 + 2 * part;
-#pragma unroll
-      for (int j = 0; j < 6; ++j) {   // column q = 2 j + half
-        const float s = (j == 0 && half == 0) ? s0 : s1;
-        const float w0 = keep[4 * j] * s, w1 = keep[4 * j + 1] * s, w2 = keep[4 * j + 2] * s, w3 = keep[4 * j + 3] * s;
-        // even lane (re row) keeps planes 0,1 and needs their im; odd lane (im row) keeps planes 2,3 and needs their re
-        const float got0 = __shfl_xor_sync(0xffffffffu, part ? w0 : w2, 1);
-        const float got1 = __shfl_xor_sync(0xffffffffu, part ? w1 : w3, 1);
-        const float4 o = part ? make_float4(got0, w2, got1, w3)    // (re2, im2, re3, im3)
-                              : make_float4(w0, got0, w1, got1);   // (re0, im0, re1, im1)
-        if (!TD_KNOCK(4)) *reinterpret_cast<float4*>(dst + (2 * j) * q_stride) = o;
-      }
-      if (lane == 0 && quad == 0) TD_T(1, i, 3);
-    }
-  }
-  // ================================================================ MMA issue: stage A
-  else if (warp == kTdMmaAWarp) {
-    if (tc::elect_one()) {
-      constexpr uint32_t idesc = fz_idesc_bf16(128, kTdNA);
-      const uint32_t ta_s = tc::smem_addr(sm.ta);
-      mbar_wait(&sm.ta_bar, 0);
+  const int m0 = 16 * wq + (lane >> 2);   // accumulator rows m0, m0 + 8
+  const uint32_t ta_s = tc::smem_addr(sm.ta);
+  float* b2_hi = sm.b2[wg][0];
+  float* b2_lo = sm.b2[wg][1];
 #pragma unroll 1
-      for (int i = 0; i < n_mine; ++i) {
-        const int s = i % kTdR;
-        TD_T(2, i, 0);
-        mbar_wait(&sm.x_full[s], (i / kTdR) & 1);
-        TD_T(2, i, 1);
-        if (i >= 2) mbar_wait(&sm.da_free[i & 1], ((i >> 1) - 1) & 1);
-        tc::fence_after_thread_sync();
-        TD_T(2, i, 2);
-        const uint32_t x_s = tc::smem_addr(sm.x[s]);
+  for (int i = 0; i < n_mine; ++i) {
+    const int s = i & 1;
+    mbar_wait(&sm.x_full[wg][s], (i >> 1) & 1);
+    // ---------------------------------------------------------------- stage A
+    float ga[kTdPlanes][36];
+    tc::wg_fence();
+    const uint32_t x_s = tc::smem_addr(sm.x[wg][s]);
 #pragma unroll
-        for (int g = 0; g < 2; ++g) {
-          if (TD_KNOCK(8)) break;
-          const uint32_t d = tmem + kTdColDA + (i & 1) * (2 * kTdNA) + g * kTdNA;
+    for (int p = 0; p < kTdPlanes; ++p)
 #pragma unroll
-          for (int ks = 0; ks < 4; ++ks) {   // K = 16 per MMA: 32 bytes inside the 128-byte swizzle row / two 8-element chunks
-            const uint64_t da = fz_desc_sw128(x_s + g * (2 * kHW * 2) + ks * 32, 0, 1024);
-            const uint64_t db = tc::make_smem_desc(ta_s + ks * 2 * kTdLboTA, kTdLboTA, 128);
-            fz_mma_f16_ss(d, da, db, idesc, ks ? 1u : 0u);
+      for (int ks = 0; ks < kW / 16; ++ks)   // K = 16 per MMA: 32 bytes inside the 128-byte swizzle row
+        tc::wg_bf16_ss_n72(ga[p], tc::make_smem_desc_sw128(x_s + p * kTdPlaneBytes + ks * 32),
+                           tc::make_smem_desc(ta_s + ks * 2 * kTdLboTA, kTdLboTA, 128), ks ? 1u : 0u);
+    tc::wg_commit();
+    tc::wg_wait<0>();
+    tc::wg_fence_acc(ga[0]);
+    tc::wg_fence_acc(ga[1]);
+    if (t == 0 && i + 2 < n_mine) load(i + 2);   // stage A has read the slot
+    // ga[p][4 (3 g + term) + 2 hh + ri] = G_p[h = m0 + 8 hh][q = 4 g + lane % 4][ri], term 0..2 (TA row order, see td_ensure)
+    // -> B2[n2 = 2 q + p][k2 = 64 ri + h], tf32 hi / lo.  Stage B of the previous unit is complete (waited for below).
+#pragma unroll
+    for (int p = 0; p < kTdPlanes; ++p)
+#pragma unroll
+      for (int g3 = 0; g3 < 3; ++g3)
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+          for (int ri = 0; ri < 2; ++ri) {
+            const int c = 4 * (3 * g3) + 2 * hh + ri;
+            const float gsum = (ga[p][c + 8] + ga[p][c + 4]) + ga[p][c];
+            float hi, lo;
+            tc::split_tf32(gsum, hi, lo);
+            const uint32_t off = tc::kmajor_offset(2 * (4 * g3 + q) + p, 64 * ri + m0 + 8 * hh, kTdN2) / 4;
+            b2_hi[off] = hi;
+            b2_lo[off] = lo;
           }
-        }
-        tc::mma_commit(&sm.x_free[s]);
-        tc::mma_commit(&sm.da_full[i & 1]);
-        TD_T(2, i, 3);
-      }
-    }
-    __syncwarp();
-  }
-  // ================================================================ MMA issue: stage B
-  // two issuing threads (even / odd batches, each with its own accumulator and operand buffer): one waits for its
-  // operands while the other's MMAs are being queued
-  else if (warp == kTdMmaBWarp || warp == kTdMmaBWarp + 1) {
-    if (tc::elect_one()) {
-      constexpr uint32_t idesc = tc::make_idesc_tf32(128, kTdN2);
-#pragma unroll 1
-      for (int i = warp - kTdMmaBWarp; i < n_mine; i += 2) {
-        const int bf = i & 1;
-        TD_T(3, i, 0);
-        mbar_wait(&sm.b2_ready[bf], (i >> 1) & 1);
-        TD_T(3, i, 1);
-        if (i >= 1) mbar_wait(&sm.db_free[bf ^ 1], ((i - 1) >> 1) & 1);   // the previous batch has left the accumulator
-        tc::fence_after_thread_sync();
-        TD_T(3, i, 2);
-        const uint32_t d = tmem + kTdColDB;
-        const uint32_t b_hi = tc::smem_addr(sm.b2[bf][0]), b_lo = b_hi + kTdB2Bytes;
+    tc::fence_proxy_async_smem();
+    tc::named_barrier(1 + wg, 128);
+    // ---------------------------------------------------------------- stage B
+    float fb[12];
+    tc::wg_fence();
+    {
+      const uint32_t a_s[3] = {tc::smem_addr(sm.a2_hi), tc::smem_addr(sm.a2_lo), tc::smem_addr(sm.a2_hi)};
+      const uint32_t b_s[3] = {tc::smem_addr(b2_hi), tc::smem_addr(b2_hi), tc::smem_addr(b2_lo)};
 #pragma unroll
-        for (int pass = 0; pass < 2; ++pass) {
-          if (TD_KNOCK(1)) break;   // [A2_hi; A2_lo] x G_hi, then [A2_hi; A2_lo] x G_lo (the epilogue adds the two row blocks)
-          const uint32_t b_s = pass ? b_lo : b_hi;
+      for (int pass = 0; pass < 3; ++pass)
 #pragma unroll
-          for (int ks = 0; ks < kTdK2 / 8; ++ks)
-            fz_mma_tf32_ts(d, tmem + kTdColA2 + ks * 8, tc::make_smem_desc(b_s + ks * 2 * kTdLboB2, kTdLboB2, 128), idesc,
-                           (pass | ks) ? 1u : 0u);
+        for (int ks = 0; ks < kTdK2 / 8; ++ks)
+          tc::wg_tf32_ss_n24(fb, tc::make_smem_desc(a_s[pass] + ks * 2 * kTdLboA2, kTdLboA2, 128),
+                             tc::make_smem_desc(b_s[pass] + ks * 2 * kTdLboB2, kTdLboB2, 128), (pass | ks) ? 1u : 0u);
+    }
+    tc::wg_commit();
+    tc::wg_wait<0>();
+    tc::wg_fence_acc(fb);
+    // ---------------------------------------------------------------- epilogue
+    // fb[4 j + 2 hh + p] = F[m2 = m0 + 8 hh = 2 kxi + part][q = 4 j + lane % 4][plane p]; lane ^ 4 holds the other part
+    const int part = (lane >> 2) & 1;
+    const int plane0 = (first + i * stride) * kTdPlanes;
+    const int b = plane0 / kC, c0 = plane0 % kC;
+#pragma unroll
+    for (int j = 0; j < 3; ++j)
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const int qq = 4 * j + q, m2 = m0 + 8 * hh, kxi = m2 >> 1;
+        const float sc = qq == 0 ? s0 : s1;
+        const float v0 = fb[4 * j + 2 * hh] * sc, v1 = fb[4 * j + 2 * hh + 1] * sc;
+        // the re lane keeps plane 0 and needs its im; the im lane keeps plane 1 and needs its re
+        const float got = __shfl_xor_sync(0xffffffffu, part ? v0 : v1, 4);
+        if (m2 < 2 * kKX) {
+          float2* dst = xm + (static_cast<size_t>(kxi * kM2 + qq) * batch + b) * kC + c0 + part;
+          *dst = part ? make_float2(got, v1) : make_float2(v0, got);
         }
-        tc::mma_commit(&sm.b2_free[bf]);
-        tc::mma_commit(&sm.db_full[bf]);
-        TD_T(3, i, 3);
       }
-    }
-    __syncwarp();
   }
-  // ================================================================ producer
-  else if (warp == kTdProdWarp) {
-    if (lane == 0) {
-      for (int i = 0; i < n_mine; ++i) {
-        const int s = i % kTdR;
-        TD_T(4, i, 0);
-        if (i >= kTdR) mbar_wait(&sm.x_free[s], ((i / kTdR) - 1) & 1);
-        TD_T(4, i, 1);
-        mbar_expect_tx(&sm.x_full[s], kTdXBytes);
-        fz_tma_load_2d(sm.x[s], &x_map, 0, (first + i * stride) * (kTdPlanes * kH), &sm.x_full[s]);
-      }
-    }
-    __syncwarp();
-  }
-
-  tc::fence_before_thread_sync();
-  __syncthreads();
-  TD_CTA(2);
-  if (warp == kTdMmaAWarp) tc::tmem_dealloc<kTdTmemCols>(tmem);
 }
 
 // ------------------------------------------------------------------------------------------------
 // Constant tables, built once per device from float64:
-//   TA  -- three bf16 terms of (cos, -sin)(2 pi q w / 64) as ONE K-major operand of 80 rows: row = 36 hf + 12 t + jj
-//          holds term t of column n = 12 hf + jj = 2 q + ri (so that a converter thread's 36 values are contiguous
-//          accumulator columns); rows 72..79 are zero.
-//   A2  -- [m2 = 2 kxi + part][k2 = ri*64 + h] as tf32 hi | lo, column-major [256][64] (rows 48..63 zero): it is
-//          copied into tensor memory lane by lane.
+//   TA  -- three bf16 terms of (cos, -sin)(2 pi q w / 64) as ONE K-major operand of 72 rows: term t of column (q, ri) is
+//          row 8 (3 (q / 4) + t) + 2 (q % 4) + ri, i.e. the accumulator registers 4 (3 (q / 4) + t) + 2 hh + ri of the
+//          thread with lane % 4 = q % 4 (fragment layout in tc_common.cuh).
+//   A2  -- [m2 = 2 kxi + part (64, rows 48..63 zero)][k2 = ri*64 + h] as tf32 hi image | lo image, K-major.
 // ------------------------------------------------------------------------------------------------
 static uint16_t td_bf16_bits(double v) {  // round to nearest even
   float f = static_cast<float>(v);
@@ -427,7 +208,7 @@ static cudaError_t td_ensure(int dev, cudaStream_t stream) {
   TdTables& t = g_td[dev];
   if (t.configured) return cudaSuccess;
   static unsigned char h_ta[kTdTABytes];
-  static float h_a2[kTdK2 * kTdA2Rows];
+  static float h_a2[2 * kTdA2Floats];
   memset(h_ta, 0, sizeof(h_ta));
   memset(h_a2, 0, sizeof(h_a2));
   const double two_pi = 2.0 * 3.14159265358979323846;
@@ -436,9 +217,8 @@ static cudaError_t td_ensure(int dev, cudaStream_t stream) {
       for (int w = 0; w < 64; ++w) {
         const double ang = two_pi * ((q * w) % 64) / 64.0;
         double rest = ri ? -sin(ang) : cos(ang);
-        const int n = 2 * q + ri, hf = n / 12, jj = n % 12;
         for (int t3 = 0; t3 < 3; ++t3) {
-          const int row = 36 * hf + 12 * t3 + jj;
+          const int row = 8 * (3 * (q >> 2) + t3) + 2 * (q & 3) + ri;
           const size_t off = static_cast<size_t>(w >> 3) * kTdLboTA + (row >> 3) * 128 + (row & 7) * 16 + (w & 7) * 2;
           const uint16_t bits = td_bf16_bits(rest);
           memcpy(h_ta + off, &bits, 2);
@@ -454,11 +234,10 @@ static cudaError_t td_ensure(int dev, cudaStream_t stream) {
           const double c = cos(ang), s = sin(ang);
           // Fre = sum c Gre + s Gim;  Fim = sum -s Gre + c Gim
           const double val = part == 0 ? (ri == 0 ? c : s) : (ri == 0 ? -s : c);
-          const int m2 = 2 * kxi + part, k2 = ri * 64 + h;
+          const uint32_t off = tc::kmajor_offset(2 * kxi + part, ri * 64 + h, kTdM2) / 4;
           const float hi = td_round_tf32(val);
-          const int lane_hi = 32 * (m2 >> 4) + (m2 & 15);   // quadrant m2 / 16: lanes 0..15 hi part, 16..31 lo part
-          h_a2[k2 * kTdA2Rows + lane_hi] = hi;
-          h_a2[k2 * kTdA2Rows + lane_hi + 16] = td_round_tf32(val - static_cast<double>(hi));
+          h_a2[off] = hi;
+          h_a2[kTdA2Floats + off] = td_round_tf32(val - static_cast<double>(hi));
         }
   }
   cudaError_t e = cudaMalloc(&t.ta, sizeof(h_ta));
@@ -479,40 +258,12 @@ static cudaError_t td_ensure(int dev, cudaStream_t stream) {
   return cudaSuccess;
 }
 
-#ifdef FNO_FZ_TRACE
-extern "C" int fno_debug_dft_knock(int bits) { return cudaMemcpyToSymbol(g_td_knock, &bits, sizeof(bits)) == cudaSuccess ? 0 : 2; }
-extern "C" int fno_debug_dft_trace(void* p) {
-  long long* q = static_cast<long long*>(p);
-  return cudaMemcpyToSymbol(g_td_trace, &q, sizeof(q)) == cudaSuccess ? 0 : 2;
-}
-#endif
-
 void dft_fwd_tc_release(int dev) {
   if (dev < 0 || dev >= 64) return;
   TdTables& t = g_td[dev];
   if (t.ta) cudaFree(t.ta);
   if (t.a2) cudaFree(t.a2);
   t = TdTables();
-}
-
-// tensor map of a bf16 activation seen as rows of one image row each: [batch * 32 * 64 rows][64 w], box {64, 256}
-static cudaError_t td_make_map(const void* act, int batch, CUtensorMap* out) {
-  static FzEncodeFn fn = nullptr;
-  if (!fn) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    cudaError_t e = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q);
-    if (e != cudaSuccess) return e;
-    if (!p) return cudaErrorNotSupported;
-    fn = reinterpret_cast<FzEncodeFn>(p);
-  }
-  const cuuint64_t gdim[2] = {static_cast<cuuint64_t>(kW), static_cast<cuuint64_t>(batch) * kC * kH};
-  const cuuint64_t gstride[1] = {static_cast<cuuint64_t>(kW) * 2};
-  const cuuint32_t box[2] = {static_cast<cuuint32_t>(kW), static_cast<cuuint32_t>(kTdPlanes * kH)}, estr[2] = {1, 1};
-  const CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(act), gdim, gstride, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS ? cudaSuccess : cudaErrorInvalidValue;
 }
 
 cudaError_t launch_dft_fwd_tc(const void* x, void* xm, int batch, float s0, float s1, cudaStream_t stream) {
@@ -523,14 +274,17 @@ cudaError_t launch_dft_fwd_tc(const void* x, void* xm, int batch, float s0, floa
   e = td_ensure(dev, stream);
   if (e != cudaSuccess) return e;
   if ((reinterpret_cast<uintptr_t>(x) & 15) || (reinterpret_cast<uintptr_t>(xm) & 15)) return cudaErrorMisalignedAddress;
+  // a bf16 activation seen as rows of one image row each: [batch * 32 * 64 rows][64 w], box {64, 128} = two planes
   CUtensorMap map;
-  e = td_make_map(x, batch, &map);
+  e = make_tma_map_2d(&map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, x, kW, static_cast<uint64_t>(batch) * kC * kH, kW,
+                      kTdPlanes * kH);
   if (e != cudaSuccess) return e;
-  const int n_batches = batch * kC / kTdPlanes;
-  const int grid = n_batches < g_td[dev].n_sm ? n_batches : g_td[dev].n_sm;
+  const int n_units = batch * kC / kTdPlanes;
+  const int want = (n_units + kTdWG - 1) / kTdWG;
+  const int grid = want < g_td[dev].n_sm ? want : g_td[dev].n_sm;
   return launch_chained(dft_fwd_tc_kernel, dim3(grid), dim3(kTdThreads), sizeof(TdSmem), stream, map,
                         static_cast<float2*>(xm), static_cast<const unsigned char*>(g_td[dev].ta),
-                        static_cast<const float*>(g_td[dev].a2), n_batches, batch, s0, s1);
+                        static_cast<const float*>(g_td[dev].a2), n_units, batch, s0, s1);
 }
 
 }  // namespace fno

@@ -6,26 +6,20 @@
 // Modes are stored mode-major (xm[k][b][c], written that way by the forward DFT kernels), so the 128 rows of a tile are
 // one contiguous 32 KB block.  For one mode k the mix over a tile of 128 samples is a real GEMM on the interleaved
 // complex64 rows exactly as they sit in memory:
-//     D[128 samples][64 = (o, re|im)] = A[128][64 = (i, re|im)] * B_k^T         (tcgen05.mma kind::tf32, K = 64)
+//     D[128 samples][64 = (o, re|im)] = A[128][64 = (i, re|im)] * B_k^T         (wgmma m64n64k8 tf32, K = 64)
 //     B_k[(o,re)][(i,re)] = Wre,  B_k[(o,re)][(i,im)] = -Wim,  B_k[(o,im)][(i,re)] = Wim,  B_k[(o,im)][(i,im)] = Wre
 // run as 3xTF32.  The B operand of every mode is prepared once per weight update (pack_mix_operand_*_kernel:
-// real-expanded, split into tf32 hi/lo, laid out as the K-major UMMA image) and arrives with ONE 32 KB bulk copy per mode.
+// real-expanded, split into tf32 hi/lo, laid out as the K-major operand image) and arrives with ONE 32 KB bulk copy per mode.
 //
-// Warp-specialised (round 2; round 1's version staged A through registers in two 256-thread pipelines and was
-// latency-bound at ~2 tiles per pipeline: 19 us against the ~10 us its 66 MB need):
-//   * work item = one MODE (all its sample tiles): B_k is fetched once per mode, 288 items on 148 persistent CTAs;
-//   * warp 16 lane 0 -- producer: the A tile is the raw fp32 block itself, dropped by TMA (two {32 floats, 128 rows}
-//     boxes, 128-byte swizzle) into a 4-slot ring as a K-major operand.  At B = 256 the ring holds ALL the tiles of a CTA,
-//     so every load of the kernel is in flight from the first microsecond;
-//   * the tensor core truncates what it reads to tf32, so the raw tile IS the hi operand; warps 0-7 compute the lo part
-//     (x - trunc(x), exact, then rounded) as soon as a tile lands and put it into TENSOR MEMORY (thread = sample row =
-//     TMEM lane; one 64-column block per ring slot), where it is the A operand of the third pass.  (A first version kept
-//     one lo buffer in shared memory, refilled per tile: the refill's LDS/STS then ran concurrently with the previous
-//     tile's 64 KB of global stores and took ~4,000 cycles instead of ~300, serialising the tiles -- tools/trace_mix.py.)
-//   * warp 17 -- MMA issue: A_raw x B_hi, A_raw x B_lo (16 MMAs, need only the TMA data) then A_lo x B_hi (8, A in TMEM);
-//     4 accumulators of 64 columns, so the epilogue of a tile never holds up the next tile's MMAs;
-//   * warps 8-15 -- epilogue: mode-major ym rows (fp32 path / backward) or the per-sample operand image of
-//     block_fused_kernel's GEMM1 (tf32 hi/lo split here, 256-bit stores).
+//   * work item = one MODE (all its sample tiles): B_k is fetched once per mode, 288 items on the persistent CTAs;
+//   * warp 8 lane 0 -- producer: the A tile is the raw fp32 block itself, dropped by TMA (two {32 floats, 128 rows}
+//     boxes, 128-byte swizzle) into a 4-slot ring.  At B = 256 (two tiles per mode, two or three modes per CTA) the
+//     ring holds all or most of the tiles of a CTA, so nearly every load is in flight from the start;
+//   * warpgroups 0 and 1 -- rows 0..63 / 64..127 of every tile: each thread reads its A fragments out of the swizzled
+//     tile (conflict-free) and splits them into tf32 hi / lo in registers; then A_hi x B_hi, A_hi x B_lo, A_lo x B_hi
+//     (24 register-A MMAs), after which the slot is released, and the epilogue from the accumulator registers: mode-major
+//     ym rows (fp32 path / backward) or the per-sample operand image of block_fused_kernel's inverse-kx GEMM (tf32 hi/lo
+//     split).
 // With the conj-transposed pack the same kernel is the adjoint mix of the backward pass
 // (Xbar[b,i,k] = sum_o G[b,o,k] conj(W[i,o,k]), SURVEY.md 8a).
 #include "fno_common.cuh"
@@ -40,80 +34,41 @@ constexpr int kMxN = 2 * kC;     // 64 real (o, re|im)
 constexpr uint32_t kMxLboB = (kMxN / 8) * 128;       // 1024
 constexpr int kMxBFloats = kMxN * kMxK;              // 4096 per image (hi or lo)
 constexpr int kMxOperandFloats = 2 * kMxBFloats;     // per mode: hi image then lo image (32 KB)
-constexpr int kMxConvWarps = 8, kMxEpiWarps = 8;
-constexpr int kMxProdWarp = 16, kMxMmaWarp = 17;
-constexpr int kMxThreads = 18 * 32;
-constexpr int kMxRing = 4;                           // A slots (and accumulators)
+constexpr int kMxConsumerWarps = 8;
+constexpr int kMxProdWarp = 8;
+constexpr int kMxThreads = 9 * 32;
+constexpr int kMxRing = 4;                           // A slots
 constexpr uint32_t kMxABytes = kMxM * kMxK * 4;      // 32,768 B per tile: two K halves of 128 rows x 128 B
 constexpr uint32_t kMxBBytes = kMxOperandFloats * 4; // 32,768 B per mode
-
-// Optional timeline trace (-DFNO_FZ_TRACE build, tools/trace_mix.py): CTA 0 stamps clock64() at the hand-off points,
-// trace[(role * 16 + tile) * 8 + event]; per-CTA clock / globaltimer stamps follow at 4 * 16 * 8.
-#ifdef FNO_FZ_TRACE
-__device__ long long* g_mx_trace = nullptr;
-#define MX_T(role, T, ev)                                                                          \
-  do {                                                                                             \
-    if (mx_tr != nullptr && blockIdx.x == 0 && (T) < 16) mx_tr[((role) * 16 + (T)) * 8 + (ev)] = clock64(); \
-  } while (0)
-#define MX_CTA(ev)                                                                                 \
-  do {                                                                                             \
-    if (mx_tr != nullptr && threadIdx.x == 0) {                                                    \
-      mx_tr[4 * 16 * 8 + blockIdx.x * 4 + (ev)] = clock64();                                       \
-      long long gt_;                                                                               \
-      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(gt_));                                      \
-      mx_tr[4 * 16 * 8 + 148 * 4 + blockIdx.x * 4 + (ev)] = gt_;                                   \
-    }                                                                                              \
-  } while (0)
-#else
-#define MX_T(role, T, ev) do { } while (0)
-#define MX_CTA(ev) do { } while (0)
-#endif
+constexpr size_t kMxImageBytes = 147456;             // per sample: [hi|lo][ky 12][48 rows][32 o] fp32
+constexpr int kMxStageLd = kMxN + 1;                 // padded row of the staged result tile
 
 struct MxSmem {
-  alignas(1024) unsigned char a[kMxRing][kMxABytes];   // raw fp32 tiles (TMA, 128B swizzle): the hi operand
+  alignas(1024) unsigned char a[kMxRing][kMxABytes];   // raw fp32 tiles (TMA, 128B swizzle)
   alignas(1024) float b[2][kMxOperandFloats];          // [mode parity] hi | lo images
-  alignas(8) uint64_t a_full[kMxRing], a_free[kMxRing], d_full[kMxRing], d_free[kMxRing], lo_ready[kMxRing];
+  float stage[2][64 * kMxStageLd];                      // per warpgroup: its 64 x 64 result tile (image epilogue)
+  alignas(8) uint64_t a_full[kMxRing], a_free[kMxRing];
   uint64_t b_full[2], b_free[2];
-  uint32_t tmem_base;
 };
-constexpr uint32_t kMxColD = 0, kMxColLo = kMxRing * kMxN;   // tensor memory: 4 accumulators, then 4 lo operands
-constexpr int kMxTmemCols = 2 * kMxRing * kMxN;              // 512
-
-// 256-bit global store (sm_100: st.global.v8): the image epilogue writes 32-byte chunks of 32 different samples per warp
-// instruction, so the instruction count -- not the bytes -- is what the LSU queue sees (lg_throttle 5.0 per issue with
-// 16-byte stores, profiles/ncu_r02*.md).
-__device__ __forceinline__ void mx_store32(void* dst, const float* v) {
-  asm volatile("st.global.v8.f32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(dst), "f"(v[0]), "f"(v[1]), "f"(v[2]), "f"(v[3]),
-               "f"(v[4]), "f"(v[5]), "f"(v[6]), "f"(v[7])
-               : "memory");
-}
 
 __global__ void __launch_bounds__(kMxThreads, 1)
-    mode_mix_tc_kernel(const __grid_constant__ CUtensorMap x_map, const float* __restrict__ wop, float4* __restrict__ ym,
+    mode_mix_tc_kernel(const __grid_constant__ CUtensorMap x_map, const float* __restrict__ wop, float2* __restrict__ ym,
                        unsigned char* __restrict__ ym_img, int batch, int n_btiles) {
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   MxSmem& sm = *reinterpret_cast<MxSmem*>(smem_raw);
   if ((smem_u32(smem_raw) & 1023u) != 0) __trap();
   const int tid = threadIdx.x, lane = tid & 31, warp = tc::warp_index_uniform();
-#ifdef FNO_FZ_TRACE
-  long long* const mx_tr = g_mx_trace;
-#endif
-  MX_CTA(0);
 
   // modes of this CTA: k = first + j * stride; tiles are numbered t = j * n_btiles + bt in processing order
   const int first = blockIdx.x, stride = gridDim.x;
   const int n_modes = (first < kModes) ? (kModes - first + stride - 1) / stride : 0;
-  const int n_tiles = n_modes * n_btiles;
 
   if (tid == 0) {
     for (int i = 0; i < kMxRing; ++i) {
       mbar_init(&sm.a_full[i], 1);
-      mbar_init(&sm.a_free[i], 1);
-      mbar_init(&sm.d_full[i], 1);
-      mbar_init(&sm.d_free[i], kMxEpiWarps);
-      mbar_init(&sm.lo_ready[i], kMxConvWarps);
+      mbar_init(&sm.a_free[i], kMxConsumerWarps);
     }
-    for (int i = 0; i < 2; ++i) { mbar_init(&sm.b_full[i], 1); mbar_init(&sm.b_free[i], 1); }
+    for (int i = 0; i < 2; ++i) { mbar_init(&sm.b_full[i], 1); mbar_init(&sm.b_free[i], kMxConsumerWarps); }
     fence_mbar_init();
     // the weights of the first two modes do not depend on the previous kernel of the chain: fetch them now
     for (int j = 0; j < 2 && j < n_modes; ++j) {
@@ -121,192 +76,126 @@ __global__ void __launch_bounds__(kMxThreads, 1)
       bulk_g2s(sm.b[j], wop + static_cast<size_t>(first + j * stride) * kMxOperandFloats, kMxBBytes, &sm.b_full[j]);
     }
   }
-  if (warp == kMxMmaWarp) tc::tmem_alloc<kMxTmemCols>(&sm.tmem_base);
-  tc::fence_before_thread_sync();
   __syncthreads();
-  tc::fence_after_thread_sync();
-  const uint32_t tmem = sm.tmem_base;
-  MX_CTA(1);
   pdl_wait();  // xm comes from the previous kernel of the chain
   pdl_launch_dependents();
 
-  // ================================================================ lo-part converters
-  if (warp < kMxConvWarps) {
-    // thread = sample row m = 32 quad + lane (its TMEM lane) and one K half (32 floats = one swizzled 128-byte segment)
-    const int quad = warp & 3, kh = warp >> 2, m = quad * 32 + lane;
-    const uint32_t t_dst0 = tmem + kMxColLo + kh * 32 + (static_cast<uint32_t>(quad * 32) << 16);
-    for (int t = 0; t < n_tiles; ++t) {
-      const int s = t % kMxRing;
-      if (tid == 0) MX_T(0, t, 0);
-      mbar_wait(&sm.a_full[s], (t / kMxRing) & 1);
-      if (tid == 0) MX_T(0, t, 1);
-      // the lo block of this slot was last read by the MMAs of tile t - kMxRing, whose completion released the slot to the
-      // producer (a_free) before this tile could land: no separate barrier
-      if (tid == 0) MX_T(0, t, 2);
-      const unsigned char* row = sm.a[s] + kh * (kMxABytes / 2) + m * 128;
-      float lo[32];
-#pragma unroll
-      for (int c = 0; c < 8; ++c) {   // logical 16-byte chunk c of the row sits at position c ^ (m & 7)
-        const float4 x = *reinterpret_cast<const float4*>(row + ((c ^ (m & 7)) << 4));
-        // x - trunc_tf32(x) is exact; +0x1000 rounds what the tensor core then truncates
-        lo[4 * c + 0] = __uint_as_float(__float_as_uint(x.x - __uint_as_float(__float_as_uint(x.x) & 0xffffe000u)) + 0x1000u);
-        lo[4 * c + 1] = __uint_as_float(__float_as_uint(x.y - __uint_as_float(__float_as_uint(x.y) & 0xffffe000u)) + 0x1000u);
-        lo[4 * c + 2] = __uint_as_float(__float_as_uint(x.z - __uint_as_float(__float_as_uint(x.z) & 0xffffe000u)) + 0x1000u);
-        lo[4 * c + 3] = __uint_as_float(__float_as_uint(x.w - __uint_as_float(__float_as_uint(x.w) & 0xffffe000u)) + 0x1000u);
-      }
-      tc::tmem_st16(t_dst0 + s * kMxN, lo);
-      tc::tmem_st16(t_dst0 + s * kMxN + 16, lo + 16);
-      tc::tmem_wait_st();
-      tc::fence_before_thread_sync();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&sm.lo_ready[s]);
-      if (tid == 0) MX_T(0, t, 3);
-    }
-  }
-  // ================================================================ epilogue
-  // warps w and w+4 share TMEM lane quadrant w & 3 (rows 32 (w&3) .. +31 of the tile) and take the 32-float column halves
-  else if (warp < kMxConvWarps + kMxEpiWarps) {
-    const int quad = warp & 3, half = (warp >> 2) & 1;
-    for (int t = 0; t < n_tiles; ++t) {
-      const int s = t % kMxRing;
-      const int k = first + (t / n_btiles) * stride, b = (t % n_btiles) * kMxM + quad * 32 + lane;
-      if (warp == kMxConvWarps && lane == 0) MX_T(1, t, 0);
-      mbar_wait(&sm.d_full[s], (t / kMxRing) & 1);
-      tc::fence_after_thread_sync();
-      if (warp == kMxConvWarps && lane == 0) MX_T(1, t, 1);
-      float v[32];
-      tc::tmem_ld32(tmem + kMxColD + (static_cast<uint32_t>(quad * 32) << 16) + s * kMxN + half * 32, v);
-      tc::fence_before_thread_sync();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&sm.d_free[s]);
-      if (b < batch && ym_img == nullptr) {
-        float4* dst = ym + (static_cast<size_t>(k) * batch + b) * (kC / 2) + half * 8;
-#pragma unroll
-        for (int c = 0; c < 8; ++c) dst[c] = make_float4(v[4 * c], v[4 * c + 1], v[4 * c + 2], v[4 * c + 3]);
-      } else if (b < batch) {
-        // Operand image of block_fused_kernel's GEMM1 (fno_block_fused.cu): per sample [hi|lo][ky/4][ky%4][48 rows][32 o]
-        // fp32, row = 24 (kxi & 1) + 2 (kxi >> 1) + (re|im), 32-byte chunks XOR-swizzled with (row & 3); tf32 hi / lo
-        // split here so the consumer is pure bulk copy + MMA.  This thread holds o = 16 half .. 16 half + 15, (re, im).
-        const int kxi = k / kM2, ky = k % kM2;
-        unsigned char* img = ym_img + static_cast<size_t>(b) * 147456 + (ky >> 2) * 24576 + (ky & 3) * 6144;
-#pragma unroll
-        for (int ri = 0; ri < 2; ++ri) {
-          const int row = 24 * (kxi & 1) + 2 * (kxi >> 1) + ri;
-#pragma unroll
-          for (int c = 0; c < 2; ++c) {
-            float hi[8], lo[8];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) tc::split_tf32(v[2 * (8 * c + j) + ri], hi[j], lo[j]);
-            unsigned char* dst = img + row * 128 + (((2 * half + c) ^ (row & 3)) << 5);
-            mx_store32(dst, hi);            // one 32-byte chunk = one full sector per store instruction
-            mx_store32(dst + 73728, lo);
-          }
-        }
-      }
-      if (warp == kMxConvWarps && lane == 0) MX_T(1, t, 2);
-    }
-  }
-  // ================================================================ producer
-  else if (warp == kMxProdWarp) {
-    if (lane == 0) {
-      int t = 0;
-      for (int j = 0; j < n_modes; ++j) {
-        const int k = first + j * stride;
-        if (j >= 2) {   // modes 0 and 1 were requested in the prologue
-          mbar_wait(&sm.b_free[j & 1], ((j >> 1) - 1) & 1);
-          mbar_expect_tx(&sm.b_full[j & 1], kMxBBytes);
-          bulk_g2s(sm.b[j & 1], wop + static_cast<size_t>(k) * kMxOperandFloats, kMxBBytes, &sm.b_full[j & 1]);
-        }
-        for (int bt = 0; bt < n_btiles; ++bt, ++t) {
-          const int s = t % kMxRing;
-          if (t >= kMxRing) mbar_wait(&sm.a_free[s], ((t / kMxRing) - 1) & 1);
-          MX_T(2, t, 0);
-          mbar_expect_tx(&sm.a_full[s], kMxABytes);
-          const int row0 = k * batch + bt * kMxM;   // rows past this mode's samples are never stored by the epilogue
-          fz_tma_load_2d(sm.a[s], &x_map, 0, row0, &sm.a_full[s]);
-          fz_tma_load_2d(sm.a[s] + kMxABytes / 2, &x_map, 32, row0, &sm.a_full[s]);
-        }
-      }
-    }
-    __syncwarp();
-  }
-  // ================================================================ MMA issue
-  else if (warp == kMxMmaWarp) {
-    if (tc::elect_one()) {
-      constexpr uint32_t idesc = tc::make_idesc_tf32(kMxM, kMxN);
-      int t = 0;
+  if (warp < kMxConsumerWarps) {
+    const int wg = warp >> 2, wq = warp & 3, q = lane & 3;
+    const int m0 = 64 * wg + 16 * wq + (lane >> 2);   // fragment rows m0, m0 + 8 of the tile
+    int t = 0;
 #pragma unroll 1
-      for (int j = 0; j < n_modes; ++j) {
-        mbar_wait(&sm.b_full[j & 1], (j >> 1) & 1);
-        const uint32_t b_hi = tc::smem_addr(sm.b[j & 1]), b_lo = b_hi + kMxBFloats * 4;
+    for (int j = 0; j < n_modes; ++j) {
+      const int k = first + j * stride;
+      mbar_wait(&sm.b_full[j & 1], (j >> 1) & 1);
+      const uint32_t b_hi = tc::smem_addr(sm.b[j & 1]), b_lo = b_hi + kMxBFloats * 4;
 #pragma unroll 1
-        for (int bt = 0; bt < n_btiles; ++bt, ++t) {
-          const int s = t % kMxRing;
-          MX_T(3, t, 0);
-          mbar_wait(&sm.a_full[s], (t / kMxRing) & 1);
-          if (t >= kMxRing) mbar_wait(&sm.d_free[s], ((t / kMxRing) - 1) & 1);
-          tc::fence_after_thread_sync();
-          MX_T(3, t, 1);
-          const uint32_t d = tmem + kMxColD + s * kMxN, a_s = tc::smem_addr(sm.a[s]);
+      for (int bt = 0; bt < n_btiles; ++bt, ++t) {
+        const int s = t % kMxRing;
+        mbar_wait(&sm.a_full[s], (t / kMxRing) & 1);
+        // A fragments: element (m, k) of the tile sits in K half k / 32, line m, 16-byte chunk ((k % 32) / 4) ^ (m & 7)
+        uint32_t a_hi[8][4], a_lo[8][4];
 #pragma unroll
-          for (int pass = 0; pass < 2; ++pass) {   // A_raw x B_hi, A_raw x B_lo
-            const uint32_t pb = pass ? b_lo : b_hi;
+        for (int ks = 0; ks < kMxK / 8; ++ks)
 #pragma unroll
-            for (int ks = 0; ks < kMxK / 8; ++ks)   // K = 8 per MMA: 32 bytes inside the 128-byte swizzle row of a K half
-              fz_mma_tf32_ss(d, fz_desc_sw128(a_s + (ks >> 2) * (kMxABytes / 2) + (ks & 3) * 32, 0, 1024),
-                             tc::make_smem_desc(pb + ks * 2 * kMxLboB, kMxLboB, 128), idesc, (pass | ks) ? 1u : 0u);
+          for (int r = 0; r < 4; ++r) {
+            const int m = m0 + 8 * (r & 1), chunk = 2 * (ks & 3) + (r >> 1);
+            const float x = *reinterpret_cast<const float*>(sm.a[s] + (ks >> 2) * (kMxABytes / 2) + m * 128 +
+                                                            ((chunk ^ (m & 7)) << 4) + q * 4);
+            float hi, lo;
+            tc::split_tf32(x, hi, lo);
+            a_hi[ks][r] = __float_as_uint(hi);
+            a_lo[ks][r] = __float_as_uint(lo);
           }
-          MX_T(3, t, 2);
-          mbar_wait(&sm.lo_ready[s], (t / kMxRing) & 1);
-          tc::fence_after_thread_sync();
-          MX_T(3, t, 3);
+        float acc[32];
+        tc::wg_fence();
 #pragma unroll
-          for (int ks = 0; ks < kMxK / 8; ++ks)   // A_lo (tensor memory) x B_hi
-            fz_mma_tf32_ts(d, tmem + kMxColLo + s * kMxN + ks * 8, tc::make_smem_desc(b_hi + ks * 2 * kMxLboB, kMxLboB, 128), idesc, 1u);
-          tc::mma_commit(&sm.a_free[s]);
-          tc::mma_commit(&sm.d_full[s]);
-          if (bt == n_btiles - 1) tc::mma_commit(&sm.b_free[j & 1]);
-          MX_T(3, t, 4);
+        for (int pass = 0; pass < 3; ++pass) {   // A_hi x B_hi, A_hi x B_lo, A_lo x B_hi
+          const uint32_t pb = pass == 1 ? b_lo : b_hi;
+#pragma unroll
+          for (int ks = 0; ks < kMxK / 8; ++ks)
+            tc::wg_tf32_rs_n64(acc, pass == 2 ? a_lo[ks] : a_hi[ks], tc::make_smem_desc(pb + ks * 2 * kMxLboB, kMxLboB, 128),
+                               (pass | ks) ? 1u : 0u);
+        }
+        tc::wg_commit();
+        tc::wg_wait<0>();
+        tc::wg_fence_acc(acc);
+        // the MMAs have consumed the fragments loaded from the A slot (and, after the last tile of the mode, the B slot):
+        // the producer may refill them
+        __syncwarp();
+        if (lane == 0) {
+          mbar_arrive(&sm.a_free[s]);
+          if (bt == n_btiles - 1) mbar_arrive(&sm.b_free[j & 1]);
+        }
+        // acc[4 i + 2 hh + e] = D[m0 + 8 hh][8 i + 2 q + e]: output channel o = 4 i + q, e = re | im
+        if (ym_img == nullptr) {
+#pragma unroll
+          for (int hh = 0; hh < 2; ++hh) {
+            const int b = bt * kMxM + m0 + 8 * hh;
+            if (b >= batch) continue;
+            float2* dst = ym + (static_cast<size_t>(k) * batch + b) * kC + q;
+#pragma unroll
+            for (int i = 0; i < 8; ++i) dst[4 * i] = make_float2(acc[4 * i + 2 * hh], acc[4 * i + 2 * hh + 1]);
+          }
+        } else {
+          // Operand image of block_fused_kernel's inverse-kx GEMM (fno_block_fused.cu): per sample
+          // [hi|lo][ky][48 rows][32 o] fp32, row = 24 (kxi & 1) + 2 (kxi >> 1) + (re|im), 32-byte chunks XOR-swizzled
+          // with (row & 3); tf32 hi / lo split here so the consumer only copies and multiplies.  A sample's (re|im) row of
+          // this mode is one 128-byte line: the tile goes through shared memory so that a warp stores whole lines
+          // (lane = o).
+          float* stg = sm.stage[wg];
+#pragma unroll
+          for (int i = 0; i < 8; ++i)
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh) {
+              stg[(m0 - 64 * wg + 8 * hh) * kMxStageLd + 8 * i + 2 * q] = acc[4 * i + 2 * hh];
+              stg[(m0 - 64 * wg + 8 * hh) * kMxStageLd + 8 * i + 2 * q + 1] = acc[4 * i + 2 * hh + 1];
+            }
+          tc::named_barrier(1 + wg, 128);
+          const int kxi = k / kM2, ky = k % kM2;
+#pragma unroll 4
+          for (int rr = 0; rr < 16; ++rr) {
+            const int r = 16 * wq + rr, b = bt * kMxM + 64 * wg + r;
+            if (b >= batch) break;
+            unsigned char* img = ym_img + static_cast<size_t>(b) * kMxImageBytes + ky * 6144;
+#pragma unroll
+            for (int ri = 0; ri < 2; ++ri) {
+              const int row = 24 * (kxi & 1) + 2 * (kxi >> 1) + ri;
+              float hi, lo;
+              tc::split_tf32(stg[r * kMxStageLd + 2 * lane + ri], hi, lo);
+              unsigned char* dst = img + row * 128 + (((lane >> 3) ^ (row & 3)) << 5) + (lane & 7) * 4;
+              *reinterpret_cast<float*>(dst) = hi;
+              *reinterpret_cast<float*>(dst + kMxImageBytes / 2) = lo;
+            }
+          }
+          tc::named_barrier(1 + wg, 128);   // the tile buffer is free for the next tile
         }
       }
     }
-    __syncwarp();
+  } else if (warp == kMxProdWarp && lane == 0) {
+    int t = 0;
+    for (int j = 0; j < n_modes; ++j) {
+      const int k = first + j * stride;
+      if (j >= 2) {   // modes 0 and 1 were requested in the prologue
+        mbar_wait(&sm.b_free[j & 1], ((j >> 1) - 1) & 1);
+        mbar_expect_tx(&sm.b_full[j & 1], kMxBBytes);
+        bulk_g2s(sm.b[j & 1], wop + static_cast<size_t>(k) * kMxOperandFloats, kMxBBytes, &sm.b_full[j & 1]);
+      }
+      for (int bt = 0; bt < n_btiles; ++bt, ++t) {
+        const int s = t % kMxRing;
+        if (t >= kMxRing) mbar_wait(&sm.a_free[s], ((t / kMxRing) - 1) & 1);
+        mbar_expect_tx(&sm.a_full[s], kMxABytes);
+        const int row0 = k * batch + bt * kMxM;   // rows past this mode's samples are never stored by the epilogue
+        tma_load_2d(sm.a[s], &x_map, 0, row0, &sm.a_full[s]);
+        tma_load_2d(sm.a[s] + kMxABytes / 2, &x_map, 32, row0, &sm.a_full[s]);
+      }
+    }
   }
-
-  tc::fence_before_thread_sync();
-  __syncthreads();
-  MX_CTA(2);
-  if (warp == kMxMmaWarp) tc::tmem_dealloc<kMxTmemCols>(tmem);
 }
 
-#ifdef FNO_FZ_TRACE
-extern "C" int fno_debug_mix_trace(void* p) {
-  long long* q = static_cast<long long*>(p);
-  return cudaMemcpyToSymbol(g_mx_trace, &q, sizeof(q)) == cudaSuccess ? 0 : 2;
-}
-#endif
+size_t ym_image_bytes(int batch) { return static_cast<size_t>(batch) * kMxImageBytes; }
 
-// tensor map of the mode-major spectrum as rows of 64 floats: [288 * batch rows][64], box {32 floats, 128 rows}
-static cudaError_t mx_make_map(const void* xm, int batch, CUtensorMap* out) {
-  static FzEncodeFn fn = nullptr;
-  if (!fn) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    cudaError_t e = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q);
-    if (e != cudaSuccess) return e;
-    if (!p) return cudaErrorNotSupported;
-    fn = reinterpret_cast<FzEncodeFn>(p);
-  }
-  const cuuint64_t gdim[2] = {static_cast<cuuint64_t>(kMxK), static_cast<cuuint64_t>(kModes) * batch};
-  const cuuint64_t gstride[1] = {static_cast<cuuint64_t>(kMxK) * 4};
-  const cuuint32_t box[2] = {32, static_cast<cuuint32_t>(kMxM)}, estr[2] = {1, 1};
-  const CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void*>(xm), gdim, gstride, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS ? cudaSuccess : cudaErrorInvalidValue;
-}
-
-// ym_img != nullptr: write the per-sample GEMM1 operand image (see the epilogue) instead of the mode-major ym.
+// ym_img != nullptr: write the per-sample inverse-kx operand image (see the epilogue) instead of the mode-major ym.
 cudaError_t launch_mode_mix(const void* xm, const void* wop, void* ym, void* ym_img, int batch, cudaStream_t stream) {
   auto kern = mode_mix_tc_kernel;
   constexpr size_t smem = sizeof(MxSmem);
@@ -315,13 +204,14 @@ cudaError_t launch_mode_mix(const void* xm, const void* wop, void* ym, void* ym_
   cudaError_t e0 = per_device_setup(kern, smem, pd, &n_sm);
   if (e0 != cudaSuccess) return e0;
   if (reinterpret_cast<uintptr_t>(xm) & 15) return cudaErrorMisalignedAddress;
+  // the mode-major spectrum as rows of 64 floats: [288 * batch rows][64], box {32 floats, 128 rows}
   CUtensorMap map;
-  e0 = mx_make_map(xm, batch, &map);
+  e0 = make_tma_map_2d(&map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, xm, kMxK, static_cast<uint64_t>(kModes) * batch, 32, kMxM);
   if (e0 != cudaSuccess) return e0;
   const int n_btiles = (batch + kMxM - 1) / kMxM;
   const int grid = kModes < n_sm ? kModes : n_sm;
   return launch_chained(kern, dim3(grid), dim3(kMxThreads), smem, stream, map, static_cast<const float*>(wop),
-                        static_cast<float4*>(ym), static_cast<unsigned char*>(ym_img), batch, n_btiles);
+                        static_cast<float2*>(ym), static_cast<unsigned char*>(ym_img), batch, n_btiles);
 }
 
 // ------------------------------------------------------------------------------------------------

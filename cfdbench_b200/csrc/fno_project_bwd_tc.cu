@@ -1,76 +1,51 @@
 // Backward of the project stage (fc1 -> GELU -> fc2 -> mask; reference src/models/fno/fno2d.py:228-233 under autograd,
 // src/train_auto.py:255) on the tensor cores, both activation storage types.
 //
-// Per tile of 128 pixels (thread = pixel x 32 hidden units, 16 warps = 4 TMEM lane quadrants x 4 column groups):
-//   1. x tile ([32 ch][128 px]) -> three bf16 pieces (24 significant bits; bf16 storage: the plane itself, one piece) in the
-//      MN-major 128B-swizzled operand layout; the loads of the NEXT tile are issued before this tile's arithmetic.
-//   2. GEMM1  z[128 px][128] = X W1^T           kind::f16, 6 piece products x 2 K steps, accumulator in tensor memory
-//   3. epilogue A: z + b1 -> GELU and GELU' sharing one erfc;  dz = (w2[0] d0 + w2[1] d1) GELU'(z)  (d = dpreds * mask);
-//      dz goes to global memory (the fc1 weight gradient is chan_outer's job) AND back into tensor memory as tf32 hi / lo;
-//      the pixel sums for the fc2 weight / fc1 bias gradients use a halving transpose-reduction (48 values per lane ->
-//      3 per lane in 45 shuffles instead of 240), then fixed-order adds across the four quadrant warps and across tiles.
-//   4. GEMM2  da[128 px][32] = dz W1             kind::tf32 as 3xTF32, A = dz in tensor memory, 48 MMAs
+// Per tile of 64 pixels (one image row), one warpgroup:
+//   1. x tile -> tf32 hi / lo (bf16 storage: hi only, exact), K-major A operand; the loads of the NEXT tile are issued
+//      before this tile's arithmetic.
+//   2. GEMM1  z[64 px][128] = X W1^T           wgmma m64n128k8 tf32, 3xTF32 (2 passes in bf16 storage)
+//   3. epilogue A (from the accumulator registers): z + b1 -> GELU and GELU' sharing one erfc;
+//      dz = (w2[0] d0 + w2[1] d1) GELU'(z)  (d = dpreds * mask); dz goes to global memory (the fc1 weight gradient is
+//      chan_outer's job) and, split into tf32 hi / lo, stays in registers as the A operand of GEMM2: the accumulator
+//      fragment of a column pair (2 q, 2 q + 1) of a K = 8 block is exactly the A fragment of K positions (q, q + 4),
+//      so the B operand of GEMM2 is stored with its K order permuted accordingly.  The pixel sums for the fc2 weight /
+//      fc1 bias gradients use a halving transpose-reduction over the 8 lanes of a column, then fixed-order adds across
+//      the four warps and across tiles.
+//   4. GEMM2  da[64 px][32] = dz W1            wgmma m64n32k8 tf32 (register A), 3xTF32
 //   5. epilogue B: da (x GELU'(pre) of the last Fourier block) -> d_out.
-// The phases of a tile run one after the other (one CTA per SM, __syncthreads between phases): even so the tile costs
-// ~8k cycles against ~35k for the CUDA-core kernel it replaces (project_bwd_kernel: both GEMMs as register-operand
-// FFMA2, fma-pipe bound at half rate; kept behind FNO_PBWD_TC=0).
-// Deterministic: per-CTA partial row [g_w2 256 | g_b1 128 | g_b2 2], reduced by reduce_partials in CTA order.
+// Two warpgroup pipelines per CTA.  Deterministic: per-pipeline partial row [g_w2 256 | g_b1 128 | g_b2 2], reduced by
+// reduce_partials in row order.
+#include "../../include/cfdbench_b200.h"
 #include "fno_common.cuh"
 #include "tc_common.cuh"
-#include "tc_tma.cuh"
 
 namespace fno {
 
-constexpr int kQbThreads = 512;
-constexpr int kQbM = 128;                       // pixels per tile
-constexpr int kQbTilesPerSample = kHW / kQbM;   // 32
+constexpr int kQbWG = 2;
+constexpr int kQbThreads = 128 * kQbWG;
+constexpr int kQbM = kW;                        // pixels per tile
+constexpr int kQbTilesPerSample = kH;           // 64
 constexpr int kQbOut = 3 * kProj + 2;           // partial row, same layout as project_bwd_kernel's
-constexpr uint32_t kQbColZ = 0, kQbColHi = 128, kQbColLo = 256, kQbColDa = 384;
+constexpr int kQbReps = kQbM * (kC / 4) / 128;  // 4 activation tasks per thread
+constexpr uint32_t kQbLboA = (kQbM / 8) * 128;  // 1024
+constexpr uint32_t kQbLboW1 = (kProj / 8) * 128;   // 2048
+constexpr uint32_t kQbLboW1t = (kC / 8) * 128;     // 512
 
 struct QbSmem {
-  alignas(1024) unsigned char xp[3][8192];     // x pieces, bf16 MN-major (two 64-pixel halves of 32 rows x 128 B, 128B swizzle)
-  alignas(1024) unsigned char w1p[3][8192];    // W1 pieces, bf16 K-major [n = hidden j][k = channel i]
-  alignas(1024) float w1t[2][kProj * kC];      // GEMM2 B operand: [n = channel i][k = hidden j] K-major, tf32 hi | lo
+  alignas(128) float w1_hi[kProj * kC];        // GEMM1 B operand: [n = hidden j][k = channel i] K-major
+  alignas(128) float w1_lo[kProj * kC];
+  alignas(128) float w1t_hi[kC * kProj];       // GEMM2 B operand: [n = channel i][k = hidden j, permuted] K-major
+  alignas(128) float w1t_lo[kC * kProj];
+  alignas(128) float x_hi[kQbWG][kQbM * kC];   // per pipeline
+  alignas(128) float x_lo[kQbWG][kQbM * kC];
   alignas(16) float b1[kProj];
   alignas(16) float w2[2][kProj];
-  alignas(16) float red[16][48];               // per-warp column sums of a 16-column sub-batch
-  alignas(16) float acc[kQbOut];               // running totals of this CTA (fixed order: tile by tile)
-  alignas(16) float red_b2[16][2];
-  alignas(8) uint64_t bar_g1, bar_g2;
-  uint32_t tmem_base;
+  alignas(16) float red[kQbWG][4][4][96];      // [pipeline][warp][lane % 4][kind * 32 + column]: per-warp pixel sums
+  alignas(16) float acc[kQbWG][3 * kProj];     // running totals of a pipeline (fixed order: tile by tile)
+  alignas(16) float red_b2[kQbWG][4][2];
 };
 
-__device__ __forceinline__ void qb_split3(float v, __nv_bfloat16& p0, __nv_bfloat16& p1, __nv_bfloat16& p2) {
-  p0 = __float2bfloat16_rn(v);
-  const float r1 = v - __bfloat162float(p0);
-  p1 = __float2bfloat16_rn(r1);
-  p2 = __float2bfloat16_rn(r1 - __bfloat162float(p1));
-}
-__host__ __device__ constexpr uint32_t qb_kmajor16(int row, int k, int rows) {   // bf16 K-major, 8 x 16-byte core matrices
-  return static_cast<uint32_t>(((k >> 3) * (rows >> 3) + (row >> 3)) * 128 + (row & 7) * 16 + (k & 7) * 2);
-}
-__device__ __forceinline__ void qb_ld8(uint32_t taddr, float* v) {
-  uint32_t r[8];
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr)
-               : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 8; ++i) v[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ void qb_ld16(uint32_t taddr, float* v) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
 __device__ __forceinline__ float qb_warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -95,235 +70,212 @@ __global__ void __launch_bounds__(kQbThreads, 1)
                           const float* __restrict__ w1, const float* __restrict__ b1, const float* __restrict__ w2,
                           float* __restrict__ d_out,          // [B][32][4096]: dpre_{L-1} (pre != null) or d a_L
                           float* __restrict__ dz1,            // [B][128][4096]
-                          float* __restrict__ partial,        // [CTA][kQbOut]
+                          float* __restrict__ partial,        // [pipeline][kQbOut]
                           int n_tiles) {
+  constexpr bool kBf = sizeof(TAct) == 2;
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   QbSmem& sm = *reinterpret_cast<QbSmem*>(smem_raw);
-  if ((smem_u32(smem_raw) & 1023u) != 0) __trap();
-  const int tid = threadIdx.x, lane = tid & 31, warp = tc::warp_index_uniform();
-  const int q = warp & 3, cg = warp >> 2;   // TMEM lane quadrant (pixels 32 q ..), hidden-unit group (32 cg ..)
-  const uint32_t lane_base = static_cast<uint32_t>(q * 32) << 16;
+  const int tid = threadIdx.x, lane = tid & 31;
+  const int wg = tc::warp_index_uniform() >> 2, wq = (tid >> 5) & 3, t = tid & 127, q = lane & 3;
 
   // ---------------------------------------------------------------- prologue
-  if (tid == 0) {
-    mbar_init(&sm.bar_g1, 1);
-    mbar_init(&sm.bar_g2, 1);
-    fence_mbar_init();
-  }
-  if (warp == 0) tc::tmem_alloc<512>(&sm.tmem_base);
-  constexpr int kW1PerThread = kProj * kC / kQbThreads;   // 8: all loads first (one L2 round trip), then the conversions
-  float w1v[kW1PerThread];
-#pragma unroll
-  for (int it = 0; it < kW1PerThread; ++it) w1v[it] = __ldg(w1 + tid + it * kQbThreads);
-#pragma unroll
-  for (int it = 0; it < kW1PerThread; ++it) {   // w1[j][i]
-    const int e = tid + it * kQbThreads;
+  for (int e = tid; e < kProj * kC; e += kQbThreads) {   // w1[j][i]
     const int j = e / kC, i = e % kC;
-    const float wv = w1v[it];
-    __nv_bfloat16 p0, p1, p2;
-    qb_split3(wv, p0, p1, p2);
-    const uint32_t off = qb_kmajor16(j, i, kProj);
-    *reinterpret_cast<__nv_bfloat16*>(sm.w1p[0] + off) = p0;
-    *reinterpret_cast<__nv_bfloat16*>(sm.w1p[1] + off) = p1;
-    *reinterpret_cast<__nv_bfloat16*>(sm.w1p[2] + off) = p2;
     float hi, lo;
-    tc::split_tf32(wv, hi, lo);
-    const uint32_t o2 = tc::kmajor_offset(i, j, kC) / 4;   // B[n = i][k = j]
-    sm.w1t[0][o2] = hi;
-    sm.w1t[1][o2] = lo;
+    tc::split_tf32(w1[e], hi, lo);
+    const uint32_t o1 = tc::kmajor_offset(j, i, kProj) / 4;
+    sm.w1_hi[o1] = hi;
+    sm.w1_lo[o1] = lo;
+    // K position of hidden unit j in GEMM2: block j / 8, position (j % 8) / 2 for even j, 4 + (j % 8) / 2 for odd j
+    const int kk = (j & ~7) + ((j & 1) ? 4 + ((j & 7) >> 1) : ((j & 7) >> 1));
+    const uint32_t o2 = tc::kmajor_offset(i, kk, kC) / 4;
+    sm.w1t_hi[o2] = hi;
+    sm.w1t_lo[o2] = lo;
   }
   for (int j = tid; j < kProj; j += kQbThreads) {
     sm.b1[j] = b1[j];
     sm.w2[0][j] = w2[j];
     sm.w2[1][j] = w2[kProj + j];
   }
-  for (int e = tid; e < kQbOut; e += kQbThreads) sm.acc[e] = 0.f;
-  tc::fence_proxy_async_smem();
-  tc::fence_before_thread_sync();
+  for (int e = tid; e < kQbWG * 3 * kProj; e += kQbThreads) (&sm.acc[0][0])[e] = 0.f;
+  tc::fence_proxy_async_smem();   // the constant operands above are read by the tensor cores
   __syncthreads();
-  tc::fence_after_thread_sync();
-  const uint32_t tmem = sm.tmem_base;
 
-  const int first = blockIdx.x, stride = gridDim.x;
-  // x piece conversion: thread = (channel c, group of 8 pixels)
-  const int xc = tid >> 4, xg = tid & 15;
-  const uint32_t x_dst = (xg >> 3) * 4096 + xc * 128 + (((xg & 7) ^ (xc & 7)) << 4);
-  constexpr bool kBf = sizeof(TAct) == 2;   // bf16 storage: the plane IS the first piece, the other two are zero
-  auto x_load = [&](int tile, float4& va, float4& vb) {   // 8 consecutive pixels of channel xc (fp32: 32 B, bf16: 16 B in va)
-    const int b = tile / kQbTilesPerSample, px0 = (tile % kQbTilesPerSample) * kQbM;
-    const TAct* src = a + (static_cast<size_t>(b) * kC + xc) * kHW + px0 + xg * 8;
-    va = __ldg(reinterpret_cast<const float4*>(src));
-    if constexpr (!kBf) vb = __ldg(reinterpret_cast<const float4*>(src) + 1);
+  const int first = blockIdx.x * kQbWG + wg, stride = gridDim.x * kQbWG;
+  float* x_hi = sm.x_hi[wg];
+  float* x_lo = sm.x_lo[wg];
+  const int m0 = 16 * wq + (lane >> 2);   // fragment rows m0, m0 + 8
+  TAct xr[kQbReps][4];   // task = rep * 128 + t -> (pixel m = task & 63, channel quad = task >> 6)
+  auto x_load = [&](int tile) {
+    const int b = tile / kQbTilesPerSample, p0 = (tile % kQbTilesPerSample) * kQbM;
+#pragma unroll
+    for (int rep = 0; rep < kQbReps; ++rep) {
+      const int task = rep * 128 + t, m = task & (kQbM - 1), kq = task >> 6;
+      const TAct* src = a + (static_cast<size_t>(b) * kC + 4 * kq) * kHW + p0 + m;
+#pragma unroll
+      for (int c = 0; c < 4; ++c) xr[rep][c] = __ldg(src + static_cast<size_t>(c) * kHW);
+    }
   };
-  float4 xa = make_float4(0.f, 0.f, 0.f, 0.f), xb = xa;
-  if (first < n_tiles) x_load(first, xa, xb);
-  float acc_b2[2] = {0.f, 0.f};   // sum over this thread's pixels of d0, d1 (warps with cg == 0 only)
+  if (first < n_tiles) x_load(first);
+  float acc_b2[2] = {0.f, 0.f};   // sum over this thread's pixels of d0, d1 (lanes with lane % 4 == 0)
 
-  int it = 0;
-  for (int tile = first; tile < n_tiles; tile += stride, ++it) {
-    const int b = tile / kQbTilesPerSample, pix = (tile % kQbTilesPerSample) * kQbM + q * 32 + lane;
-    // ---- phase 1: x pieces of this tile -> shared memory (the registers were loaded one tile ago)
-    if constexpr (kBf) {
-      *reinterpret_cast<float4*>(sm.xp[0] + x_dst) = xa;
-    } else {
-      const float xv[8] = {xa.x, xa.y, xa.z, xa.w, xb.x, xb.y, xb.z, xb.w};
-      uint32_t pk[3][4];
+  for (int tile = first; tile < n_tiles; tile += stride) {
+    const int b = tile / kQbTilesPerSample, p0 = (tile % kQbTilesPerSample) * kQbM;
+    // ---- phase 1: x of this tile -> shared memory (the registers were loaded one tile ago)
 #pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        __nv_bfloat16 p0a, p1a, p2a, p0b, p1b, p2b;
-        qb_split3(xv[2 * e], p0a, p1a, p2a);
-        qb_split3(xv[2 * e + 1], p0b, p1b, p2b);
-        pk[0][e] = static_cast<uint32_t>(__bfloat16_as_ushort(p0a)) | (static_cast<uint32_t>(__bfloat16_as_ushort(p0b)) << 16);
-        pk[1][e] = static_cast<uint32_t>(__bfloat16_as_ushort(p1a)) | (static_cast<uint32_t>(__bfloat16_as_ushort(p1b)) << 16);
-        pk[2][e] = static_cast<uint32_t>(__bfloat16_as_ushort(p2a)) | (static_cast<uint32_t>(__bfloat16_as_ushort(p2b)) << 16);
+    for (int rep = 0; rep < kQbReps; ++rep) {
+      const int task = rep * 128 + t, m = task & (kQbM - 1), kq = task >> 6;
+      float hi[4], lo[4];
+#pragma unroll
+      for (int c = 0; c < 4; ++c) {
+        const float v = kBf ? __bfloat162float(xr[rep][c]) : static_cast<float>(xr[rep][c]);
+        if constexpr (kBf) hi[c] = v;
+        else tc::split_tf32(v, hi[c], lo[c]);
       }
-#pragma unroll
-      for (int pc = 0; pc < 3; ++pc)
-        *reinterpret_cast<uint4*>(sm.xp[pc] + x_dst) = make_uint4(pk[pc][0], pk[pc][1], pk[pc][2], pk[pc][3]);
+      const uint32_t off = tc::kmajor_offset(m, 4 * kq, kQbM) / 4;
+      *reinterpret_cast<float4*>(x_hi + off) = make_float4(hi[0], hi[1], hi[2], hi[3]);
+      if constexpr (!kBf) *reinterpret_cast<float4*>(x_lo + off) = make_float4(lo[0], lo[1], lo[2], lo[3]);
     }
     tc::fence_proxy_async_smem();
-    tc::fence_before_thread_sync();
-    __syncthreads();
-    tc::fence_after_thread_sync();
-    // ---- phase 2: GEMM1 (one elected thread), everybody else fetches the next tile's x and this tile's per-pixel inputs
-    if (warp == 0 && tc::elect_one()) {
-      constexpr uint32_t idesc = fz_idesc_bf16(kQbM, kProj) | kAMajorMN;
-      // x piece, W piece: all products down to 2^-24 (bf16 storage: x has one piece)
-      constexpr int pa[6] = {0, 0, 0, 1, 1, 2}, pb[6] = {0, 1, 2, 0, 1, 0};
-      constexpr int n_prod = kBf ? 3 : 6;
+    tc::named_barrier(1 + wg, 128);
+    // ---- phase 2: GEMM1
+    float z[64];
+    tc::wg_fence();
+    {
+      const uint32_t a_s[3] = {tc::smem_addr(x_hi), tc::smem_addr(x_lo), tc::smem_addr(x_hi)};
+      const uint32_t b_s[3] = {tc::smem_addr(sm.w1_hi), tc::smem_addr(sm.w1_hi), tc::smem_addr(sm.w1_lo)};
 #pragma unroll
-      for (int t = 0; t < n_prod; ++t) {
-        const uint32_t x_s = tc::smem_addr(sm.xp[pa[t]]), w_s = tc::smem_addr(sm.w1p[pb[t]]);
+      for (int pass = 0; pass < 3; ++pass) {
+        if (kBf && pass == 1) continue;
 #pragma unroll
-        for (int ks = 0; ks < 2; ++ks)
-          fz_mma_f16_ss(tmem + kQbColZ, fz_desc_sw128(x_s + ks * 2048, 4096, 1024), tc::make_smem_desc(w_s + ks * 4096, 2048, 128),
-                        idesc, (t | ks) ? 1u : 0u);
+        for (int ks = 0; ks < kC / 8; ++ks)
+          tc::wg_tf32_ss_n128(z, tc::make_smem_desc(a_s[pass] + ks * 2 * kQbLboA, kQbLboA, 128),
+                              tc::make_smem_desc(b_s[pass] + ks * 2 * kQbLboW1, kQbLboW1, 128), (pass | ks) ? 1u : 0u);
       }
-      tc::mma_commit(&sm.bar_g1);
     }
-    __syncwarp();
-    if (tile + stride < n_tiles) x_load(tile + stride, xa, xb);
-    const float mk = __ldg(mask + static_cast<size_t>(b) * kHW + pix);
-    const float d0 = __ldg(dpreds + (static_cast<size_t>(b) * 2 + 0) * kHW + pix) * mk;
-    const float d1 = __ldg(dpreds + (static_cast<size_t>(b) * 2 + 1) * kHW + pix) * mk;
-    if (cg == 0) { acc_b2[0] += d0; acc_b2[1] += d1; }
-    mbar_wait(&sm.bar_g1, it & 1);
-    tc::fence_after_thread_sync();
-    // ---- phase 3: epilogue A, two sub-batches of 16 hidden units
-    float* dz_b = dz1 + static_cast<size_t>(b) * kProj * kHW + pix;
-#pragma unroll 1
-    for (int sb = 0; sb < 2; ++sb) {
-      const int j0 = cg * 32 + sb * 16;
-      float z[16];
-      qb_ld16(tmem + kQbColZ + j0 + lane_base, z);
-      float hi[16], lo[16], v[48];   // v: [p0 | p1 | pb] x 16 columns, to be summed over the pixels
+    tc::wg_commit();
+    if (tile + stride < n_tiles) x_load(tile + stride);
+    float d[2][2];   // [row hh][out channel]
 #pragma unroll
-      for (int jj = 0; jj < 16; ++jj) {
-        float g, dg;
-        qb_gelu_both(z[jj] + sm.b1[j0 + jj], g, dg);
-        const float dz = (sm.w2[0][j0 + jj] * d0 + sm.w2[1][j0 + jj] * d1) * dg;
-        dz_b[static_cast<size_t>(j0 + jj) * kHW] = dz;
-        tc::split_tf32(dz, hi[jj], lo[jj]);
-        v[jj] = d0 * g;
-        v[16 + jj] = d1 * g;
-        v[32 + jj] = dz;
-      }
-      tc::tmem_st16(tmem + kQbColHi + j0 + lane_base, hi);
-      tc::tmem_st16(tmem + kQbColLo + j0 + lane_base, lo);
-      // halving transpose-reduction over the 32 lanes: 48 -> 24 -> 12 -> 6 -> 3 values per lane, then lane pairs
+    for (int hh = 0; hh < 2; ++hh) {
+      const int pix = p0 + m0 + 8 * hh;
+      const float mk = __ldg(mask + static_cast<size_t>(b) * kHW + pix);
+      d[hh][0] = __ldg(dpreds + (static_cast<size_t>(b) * 2 + 0) * kHW + pix) * mk;
+      d[hh][1] = __ldg(dpreds + (static_cast<size_t>(b) * 2 + 1) * kHW + pix) * mk;
+      if (q == 0) { acc_b2[0] += d[hh][0]; acc_b2[1] += d[hh][1]; }
+    }
+    tc::wg_wait<0>();
+    tc::wg_fence_acc(z);
+    // ---- phase 3: epilogue A.  z[4 i + 2 hh + e] = z[px = m0 + 8 hh][j = 8 i + 2 q + e], in four chunks of 4 i
+    uint32_t dz_hi[16][4], dz_lo[16][4];   // GEMM2 A fragments: K block i, positions (q, q + 4) <-> j = 8 i + 2 q + (0, 1)
+    float* dz_b = dz1 + static_cast<size_t>(b) * kProj * kHW + p0;
 #pragma unroll
-      for (int i = 0; i < 24; ++i) {
+    for (int ic = 0; ic < 4; ++ic) {
+      float v[24];   // [kind: d0 g | d1 g | dz][column c = 2 (i - 4 ic) + e], summed over the two rows
+#pragma unroll
+      for (int i = 4 * ic; i < 4 * ic + 4; ++i)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int j = 8 * i + 2 * q + e, c = 2 * (i - 4 * ic) + e;
+          v[c] = v[8 + c] = v[16 + c] = 0.f;
+#pragma unroll
+          for (int hh = 0; hh < 2; ++hh) {
+            float g, dg;
+            qb_gelu_both(z[4 * i + 2 * hh + e] + sm.b1[j], g, dg);
+            const float dz = (sm.w2[0][j] * d[hh][0] + sm.w2[1][j] * d[hh][1]) * dg;
+            dz_b[static_cast<size_t>(j) * kHW + m0 + 8 * hh] = dz;
+            float hi, lo;
+            tc::split_tf32(dz, hi, lo);
+            dz_hi[i][hh + 2 * e] = __float_as_uint(hi);   // a[0] = (r, q), a[1] = (r + 8, q), a[2] = (r, q + 4), a[3] = (r + 8, q + 4)
+            dz_lo[i][hh + 2 * e] = __float_as_uint(lo);
+            v[c] += d[hh][0] * g;
+            v[8 + c] += d[hh][1] * g;
+            v[16 + c] += dz;
+          }
+        }
+      // halving transpose-reduction over the 8 lanes of a column (lane bits 4, 3, 2): 24 -> 12 -> 6 -> 3 values per lane
+#pragma unroll
+      for (int i = 0; i < 12; ++i) {
         const bool up = lane & 16;
-        const float send = up ? v[i] : v[i + 24], keep = up ? v[i + 24] : v[i];
+        const float send = up ? v[i] : v[i + 12], keep = up ? v[i + 12] : v[i];
         v[i] = keep + __shfl_xor_sync(0xffffffffu, send, 16);
       }
 #pragma unroll
-      for (int i = 0; i < 12; ++i) {
+      for (int i = 0; i < 6; ++i) {
         const bool up = lane & 8;
-        const float send = up ? v[i] : v[i + 12], keep = up ? v[i + 12] : v[i];
+        const float send = up ? v[i] : v[i + 6], keep = up ? v[i + 6] : v[i];
         v[i] = keep + __shfl_xor_sync(0xffffffffu, send, 8);
       }
 #pragma unroll
-      for (int i = 0; i < 6; ++i) {
+      for (int i = 0; i < 3; ++i) {
         const bool up = lane & 4;
-        const float send = up ? v[i] : v[i + 6], keep = up ? v[i + 6] : v[i];
+        const float send = up ? v[i] : v[i + 3], keep = up ? v[i + 3] : v[i];
         v[i] = keep + __shfl_xor_sync(0xffffffffu, send, 4);
       }
+      const int off = ((lane >> 4) & 1) * 12 + ((lane >> 3) & 1) * 6 + ((lane >> 2) & 1) * 3;
 #pragma unroll
-      for (int i = 0; i < 3; ++i) {
-        const bool up = lane & 2;
-        const float send = up ? v[i] : v[i + 3], keep = up ? v[i + 3] : v[i];
-        v[i] = keep + __shfl_xor_sync(0xffffffffu, send, 2);
-      }
-#pragma unroll
-      for (int i = 0; i < 3; ++i) v[i] += __shfl_xor_sync(0xffffffffu, v[i], 1);
-      if ((lane & 1) == 0) {
-        const int off = ((lane >> 4) & 1) * 24 + ((lane >> 3) & 1) * 12 + ((lane >> 2) & 1) * 6 + ((lane >> 1) & 1) * 3;
-#pragma unroll
-        for (int i = 0; i < 3; ++i) sm.red[warp][off + i] = v[i];
-      }
-      __syncthreads();
-      // running totals: entry (quantity t, column j0' + jj) of column group c' = sum over the four quadrant warps, in order
-      if (tid < 4 * 48) {
-        const int c2 = tid / 48, e = tid % 48, t = e >> 4, jj = e & 15;
-        const float s = ((sm.red[c2 * 4 + 0][e] + sm.red[c2 * 4 + 1][e]) + sm.red[c2 * 4 + 2][e]) + sm.red[c2 * 4 + 3][e];
-        sm.acc[t * kProj + c2 * 32 + sb * 16 + jj] += s;
-      }
-      __syncthreads();
+      for (int i = 0; i < 3; ++i) sm.red[wg][wq][q][24 * ic + off + i] = v[i];
     }
-    tc::tmem_wait_st();
-    tc::fence_before_thread_sync();
-    __syncthreads();
-    tc::fence_after_thread_sync();
-    // ---- phase 4: GEMM2, da = dz W1 (A in tensor memory)
-    if (warp == 0 && tc::elect_one()) {
-      constexpr uint32_t idesc = tc::make_idesc_tf32(kQbM, kC);
-      const uint32_t b_hi = tc::smem_addr(sm.w1t[0]), b_lo = tc::smem_addr(sm.w1t[1]);
+    // ---- phase 4: GEMM2, da = dz W1 (A from registers); the pixel sums are added up while it runs
+    float da[16];
+    tc::wg_fence();
+    {
+      const uint32_t b_s[3] = {tc::smem_addr(sm.w1t_hi), tc::smem_addr(sm.w1t_hi), tc::smem_addr(sm.w1t_lo)};
 #pragma unroll
-      for (int pass = 0; pass < 3; ++pass) {
-        const uint32_t a_t = tmem + ((pass == 1) ? kQbColLo : kQbColHi);
-        const uint32_t b_s = (pass == 2) ? b_lo : b_hi;
+      for (int pass = 0; pass < 3; ++pass)
 #pragma unroll
         for (int ks = 0; ks < kProj / 8; ++ks)
-          fz_mma_tf32_ts(tmem + kQbColDa, a_t + ks * 8, tc::make_smem_desc(b_s + ks * 1024, 512, 128), idesc, (pass | ks) ? 1u : 0u);
-      }
-      tc::mma_commit(&sm.bar_g2);
+          tc::wg_tf32_rs_n32(da, pass == 1 ? dz_lo[ks] : dz_hi[ks],
+                             tc::make_smem_desc(b_s[pass] + ks * 2 * kQbLboW1t, kQbLboW1t, 128), (pass | ks) ? 1u : 0u);
     }
-    __syncwarp();
-    // ---- phase 5: epilogue B: 8 channels per thread
-    float pv[8];
-    const size_t base = (static_cast<size_t>(b) * kC + cg * 8) * kHW + pix;
+    tc::wg_commit();
+    tc::named_barrier(1 + wg, 128);
+    // running totals: entry (kind, hidden unit j) = sum over the four warps, in order
+#pragma unroll
+    for (int r = 0; r < 3; ++r) {
+      const int ent = r * 128 + t, kind = ent >> 7, j = ent & 127, i = j >> 3;
+      const int qq = (j >> 1) & 3, idx = 24 * (i >> 2) + 8 * kind + 2 * (i & 3) + (j & 1);
+      const float s = ((sm.red[wg][0][qq][idx] + sm.red[wg][1][qq][idx]) + sm.red[wg][2][qq][idx]) + sm.red[wg][3][qq][idx];
+      sm.acc[wg][ent] += s;
+    }
+    // ---- phase 5: epilogue B.  da[4 i + 2 hh + e] = da[px = m0 + 8 hh][channel 8 i + 2 q + e]
+    float pv[16];
     if (pre != nullptr) {
 #pragma unroll
-      for (int i = 0; i < 8; ++i) pv[i] = __ldg(pre + base + static_cast<size_t>(i) * kHW);
-    }
-    mbar_wait(&sm.bar_g2, it & 1);
-    tc::fence_after_thread_sync();
-    float da[8];
-    qb_ld8(tmem + kQbColDa + cg * 8 + lane_base, da);
+      for (int i = 0; i < 4; ++i)
 #pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      float o = da[i];
-      if (pre != nullptr) o *= dgelu_erf(pv[i]);
-      d_out[base + static_cast<size_t>(i) * kHW] = o;
+        for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+          for (int e = 0; e < 2; ++e)
+            pv[4 * i + 2 * hh + e] =
+                __ldg(pre + (static_cast<size_t>(b) * kC + 8 * i + 2 * q + e) * kHW + p0 + m0 + 8 * hh);
     }
-    tc::fence_before_thread_sync();
-    __syncthreads();   // the accumulators and the x piece buffers are free again
-    tc::fence_after_thread_sync();
+    tc::wg_wait<0>();
+    tc::wg_fence_acc(da);
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          float o = da[4 * i + 2 * hh + e];
+          if (pre != nullptr) o *= dgelu_erf(pv[4 * i + 2 * hh + e]);
+          d_out[(static_cast<size_t>(b) * kC + 8 * i + 2 * q + e) * kHW + p0 + m0 + 8 * hh] = o;
+        }
   }
-  // ---- the CTA's partial row: [g_w2[0][j] | g_w2[1][j] | g_b1[j] | g_b2]
-  if (cg == 0) {
+  // ---- the pipeline's partial row: [g_w2[0][j] | g_w2[1][j] | g_b1[j] | g_b2]
+  {
     const float s0 = qb_warp_sum(acc_b2[0]), s1 = qb_warp_sum(acc_b2[1]);
-    if (lane == 0) { sm.red_b2[q][0] = s0; sm.red_b2[q][1] = s1; }
+    if (lane == 0) { sm.red_b2[wg][wq][0] = s0; sm.red_b2[wg][wq][1] = s1; }
   }
-  __syncthreads();
-  float* prow = partial + static_cast<size_t>(blockIdx.x) * kQbOut;
-  for (int e = tid; e < 3 * kProj; e += kQbThreads) prow[e] = sm.acc[e];
-  if (tid < 2) prow[3 * kProj + tid] = ((sm.red_b2[0][tid] + sm.red_b2[1][tid]) + sm.red_b2[2][tid]) + sm.red_b2[3][tid];
-  tc::fence_before_thread_sync();
-  __syncthreads();
-  if (warp == 0) tc::tmem_dealloc<512>(tmem);
+  tc::named_barrier(1 + wg, 128);
+  float* prow = partial + static_cast<size_t>(blockIdx.x * kQbWG + wg) * kQbOut;
+  for (int e = t; e < 3 * kProj; e += 128) prow[e] = sm.acc[wg][e];
+  if (t < 2)
+    prow[3 * kProj + t] = ((sm.red_b2[wg][0][t] + sm.red_b2[wg][1][t]) + sm.red_b2[wg][2][t]) + sm.red_b2[wg][3][t];
 }
+
+int project_bwd_parts(int);
 
 // returns the number of partial rows written through *n_parts
 template <typename TAct>
@@ -337,9 +289,12 @@ cudaError_t launch_project_bwd_tc(const void* a, const float* dpreds, const floa
   cudaError_t e0 = per_device_setup(kern, smem, pd, &n_sm);
   if (e0 != cudaSuccess) return e0;
   const int n_tiles = batch * kQbTilesPerSample;
-  const int grid = n_tiles < n_sm ? n_tiles : n_sm;
+  int grid = (n_tiles + kQbWG - 1) / kQbWG;
+  if (grid > n_sm) grid = n_sm;
+  const int rows_max = project_bwd_parts(FNO_BWD_CHUNK) / kQbWG;   // the partial rows fit the caller's buffer
+  if (grid > rows_max) grid = rows_max;
   kern<<<grid, kQbThreads, smem, stream>>>(static_cast<const TAct*>(a), dpreds, mask, pre, w1, b1, w2, d_out, dz1, partial, n_tiles);
-  *n_parts = grid;
+  *n_parts = grid * kQbWG;
   return cudaGetLastError();
 }
 template cudaError_t launch_project_bwd_tc<float>(const void*, const float*, const float*, const float*, const float*, const float*,

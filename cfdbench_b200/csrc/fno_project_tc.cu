@@ -1,59 +1,54 @@
 // Project kernel on the tensor cores: preds = (fc2 . GELU . fc1)(a_L) * mask
 // replacing Conv2d(32,128,1) + GELU + Conv2d(128,2,1) + "* mask" (reference src/models/fno/fno2d.py:228-233).
 //
-// fc1 is the one genuinely dense GEMM of the model (16.8 MFMA per sample): per tile of 128 pixels
-//     D[128 px][128 hidden] = A[128 px][32 ch] * W1^T         (tcgen05.mma kind::tf32, M=128, N=128, K=32)
-// run as 3xTF32 (hi*hi + lo*hi + hi*lo, round-to-nearest split) so the result stays within 1e-6 of fp32.
-// The (B,128,64,64) hidden tensor of the reference (537 MB at B=256) lives only in TMEM: the epilogue reads
-// it back (thread = pixel, 32 hidden units per warp group), applies the exact GELU (the bias arrives through one
-// extra K = 8 MMA step: a constant ones column times a B block holding b1), contracts
-// with fc2 in registers; the four column groups are summed in a fixed order (deterministic results).
+// fc1 is the one genuinely dense GEMM of the model (16.8 MFMA per sample): per tile of 64 pixels (one image row)
+//     D[64 px][128 hidden] = A[64 px][32 ch] * W1^T         (wgmma m64n128k8 tf32, K = 32)
+// run as 3xTF32 (hi*hi + lo*hi + hi*lo, round-to-nearest split) so the result stays within 1e-6 of fp32; bf16 activations
+// are exact in tf32, so that storage mode needs two passes (x*W1_hi + x*W1_lo).  The (B,128,64,64) hidden tensor of the
+// reference (537 MB at B=256) exists only in the accumulator registers: the epilogue adds b1, applies the GELU (degree-8
+// erfc fit; the degree-5 fit in bf16 storage mode, fno_common.cuh), contracts with fc2 and sums the partial sums of the
+// four lanes that share a pixel in a fixed order (deterministic results).
 //
-// Persistent CTA (512 threads) per SM.  Per tile: the activation values prefetched into registers one tile
-// ahead (coalesced 16-byte loads) are split into tf32 hi/lo and written as the K-major A operand (double
-// buffered); one elected thread issues the 14 MMAs (12 + 2 bias steps; 10 with bf16 storage) into one of two 128-column TMEM accumulators; the epilogue
-// of the previous tile overlaps them.
+// Persistent CTA of four independent warpgroup pipelines.  Per tile: the activation values prefetched into registers one
+// tile ahead (coalesced loads) are split into tf32 hi/lo and written as the K-major A operand; the warpgroup issues the
+// MMAs, waits for them and runs the epilogue while the other pipelines of the SM load, multiply or compute their GELUs.
 #include "fno_common.cuh"
 #include "tc_common.cuh"
 
 namespace fno {
 
-constexpr int kPtThreads = 512;                            // two independent 256-thread tile pipelines
-constexpr int kPtGroup = 256;
-constexpr int kPtM = 128;                                  // pixels per tile (2 image rows)
-constexpr uint32_t kPtLboA = (kPtM / 8) * 128;             // 2048
+constexpr int kPtWG = 4;
+constexpr int kPtThreads = 128 * kPtWG;
+constexpr int kPtM = kW;                                   // pixels per tile (one image row)
+constexpr uint32_t kPtLboA = (kPtM / 8) * 128;             // 1024
 constexpr uint32_t kPtLboB = (kProj / 8) * 128;            // 2048 (B operand has 128 rows = hidden units)
-constexpr int kPtTilesPerSample = kHW / kPtM;              // 32
+constexpr int kPtTilesPerSample = kH;                      // 64
+constexpr int kPtReps = kPtM * (kC / 4) / 128;             // 4 activation tasks per thread
 
 struct PtSmem {
-  alignas(128) float a_hi[2][2][kPtM * kC];  // [group][buffer] 4 x 16 KB
-  alignas(128) float a_lo[2][2][kPtM * kC];  // 4 x 16 KB
   alignas(128) float w_hi[kProj * kC];       // 16 KB   B operand: [n = hidden j][k = channel i]
   alignas(128) float w_lo[kProj * kC];       // 16 KB
-  alignas(128) float ones[kPtM * 8];         // 4 KB    A operand of the bias step: column 0 = 1, columns 1..7 = 0
-  alignas(128) float bb_hi[kProj * 8];       // 4 KB    B operand of the bias step: column 0 = b1[j] (tf32 hi / lo)
-  alignas(128) float bb_lo[kProj * 8];
+  alignas(128) float a_hi[kPtWG][kPtM * kC]; // 4 x 8 KB
+  alignas(128) float a_lo[kPtWG][kPtM * kC]; // 4 x 8 KB
   alignas(16) float4 w2q[kProj / 2];         // (w2[0][j], w2[1][j], w2[0][j+1], w2[1][j+1])
-  alignas(16) float2 opart[2][2][2][kPtM];   // [group][buffer][column half][pixel] fc2 partial sums
-  alignas(8) uint64_t mma_bar[2][2];
-  uint32_t tmem_base;
+  alignas(16) float2 b1p[kProj / 2];         // (b1[j], b1[j+1])
 };
 
 // Activation values of one tile held by a thread between the prefetch and the split pass.
-// task = rep*256 + gtid -> (pixel m = task & 127, channel quad kq = task >> 7): lanes run over consecutive pixels,
-// so the global loads coalesce (128 B per channel per warp) and the 16-byte operand stores are conflict-free.
+// task = rep*128 + t -> (pixel m = task & 63, channel quad kq = task >> 6): lanes run over consecutive pixels,
+// so the global loads coalesce and the 16-byte operand stores are conflict-free.
 template <typename TAct>
 struct PtRegs {
-  TAct v[4][4];
+  TAct v[kPtReps][4];
 };
 
 template <typename TAct>
-__device__ __forceinline__ void pt_prefetch(PtRegs<TAct>& r, const TAct* __restrict__ a, int tile, int tid) {
+__device__ __forceinline__ void pt_prefetch(PtRegs<TAct>& r, const TAct* __restrict__ a, int tile, int t) {
   const int b = tile / kPtTilesPerSample, p0 = (tile % kPtTilesPerSample) * kPtM;
 #pragma unroll
-  for (int rep = 0; rep < 4; ++rep) {
-    const int task = rep * kPtGroup + tid;
-    const int m = task & (kPtM - 1), kq = task >> 7;
+  for (int rep = 0; rep < kPtReps; ++rep) {
+    const int task = rep * 128 + t;
+    const int m = task & (kPtM - 1), kq = task >> 6;
     const TAct* src = a + (static_cast<size_t>(b) * kC + 4 * kq) * kHW + p0 + m;
 #pragma unroll
     for (int c = 0; c < 4; ++c) r.v[rep][c] = __ldg(src + static_cast<size_t>(c) * kHW);
@@ -64,11 +59,11 @@ __device__ __forceinline__ float pt_to_float(float v) { return v; }
 __device__ __forceinline__ float pt_to_float(__nv_bfloat16 v) { return __bfloat162float(v); }
 
 template <typename TAct>
-__device__ __forceinline__ void pt_split_store(const PtRegs<TAct>& r, float* a_hi, float* a_lo, int tid) {
+__device__ __forceinline__ void pt_split_store(const PtRegs<TAct>& r, float* a_hi, float* a_lo, int t) {
 #pragma unroll
-  for (int rep = 0; rep < 4; ++rep) {
-    const int task = rep * kPtGroup + tid;
-    const int m = task & (kPtM - 1), kq = task >> 7;
+  for (int rep = 0; rep < kPtReps; ++rep) {
+    const int task = rep * 128 + t;
+    const int m = task & (kPtM - 1), kq = task >> 6;
     float hi[4], lo[4];
 #pragma unroll
     for (int c = 0; c < 4; ++c) {
@@ -82,129 +77,17 @@ __device__ __forceinline__ void pt_split_store(const PtRegs<TAct>& r, float* a_h
   }
 }
 
-template <int GRP>
-__device__ __forceinline__ void group_barrier() {  // named barrier of one 256-thread pipeline
-  asm volatile("bar.sync %0, %1;" ::"n"(GRP + 1), "n"(kPtGroup) : "memory");
-}
-
-template <typename TAct, int GRP>
-__device__ __forceinline__ void pt_pipeline(PtSmem& sm, const TAct* __restrict__ a, const float* __restrict__ mask,
-                                            float* __restrict__ preds, int n_tiles, float b2x, float b2y) {
-  constexpr bool kBf16 = sizeof(TAct) == 2;
-  const int tid = threadIdx.x, lane = tid & 31;
-  const int gtid = tid & (kPtGroup - 1), gwarp = tc::warp_index_uniform() & 7;
-  const uint32_t tmem_base = sm.tmem_base + GRP * (2 * kProj);
-  constexpr uint32_t idesc = tc::make_idesc_tf32(kPtM, kProj);
-
-  // tiles of this CTA: first, first+stride, ...; pipeline g takes every other one
-  const int first = blockIdx.x, stride = gridDim.x;
-  const int n_cta = (first < n_tiles) ? (n_tiles - first + stride - 1) / stride : 0;
-  const int n_mine = (n_cta + 1 - GRP) / 2;
-  auto tile_of = [&](int it) { return first + (2 * it + GRP) * stride; };
-
-  // epilogue of local tile `it`: TMEM accumulator -> +bias -> GELU -> fc2 partial sums (two 32-column chunks)
-  auto epilogue = [&](int it) {
-    const int buf = it & 1;
-    mbar_wait(&sm.mma_bar[GRP][buf], (it >> 1) & 1);
-    tc::fence_after_thread_sync();
-    const int quad = gwarp & 3, half = gwarp >> 2;  // TMEM lane quadrant / 64-column half
-    float2 acc = make_float2(0.f, 0.f);             // (out channel 0, out channel 1)
-#pragma unroll
-    for (int chunk = 0; chunk < 2; ++chunk) {
-      float v[32];
-      const int j0 = half * 64 + chunk * 32;
-      tc::tmem_ld32(tmem_base + (static_cast<uint32_t>(quad * 32) << 16) + buf * kProj + j0, v);
-#pragma unroll
-      for (int c = 0; c < 32; c += 2) {
-        const int j = j0 + c;
-        const float2 g = gelu_erf2(make_float2(v[c], v[c + 1]));  // the accumulator already includes b1
-        const float4 wq = sm.w2q[j >> 1];
-        acc = __ffma2_rn(make_float2(g.x, g.x), make_float2(wq.x, wq.y), acc);
-        acc = __ffma2_rn(make_float2(g.y, g.y), make_float2(wq.z, wq.w), acc);
-      }
-    }
-    sm.opart[GRP][buf][half][quad * 32 + lane] = acc;  // summed in a fixed order by finalize(): deterministic
-    tc::fence_before_thread_sync();
-  };
-  // after the group barrier that follows epilogue(it): write tile `it`'s predictions
-  auto finalize = [&](int it) {
-    if (gtid < kPtM) {
-      const int buf = it & 1;
-      const int tile = tile_of(it);
-      const int b = tile / kPtTilesPerSample, pix = (tile % kPtTilesPerSample) * kPtM + gtid;
-      const float2 p0 = sm.opart[GRP][buf][0][gtid], p1 = sm.opart[GRP][buf][1][gtid];
-      const float mk = __ldg(mask + static_cast<size_t>(b) * kHW + pix);
-      preds[(static_cast<size_t>(b) * 2 + 0) * kHW + pix] = ((b2x + p0.x) + p1.x) * mk;
-      preds[(static_cast<size_t>(b) * 2 + 1) * kHW + pix] = ((b2y + p0.y) + p1.y) * mk;
-    }
-  };
-
-  PtRegs<TAct> regs;
-  if (n_mine > 0) pt_prefetch<TAct>(regs, a, tile_of(0), gtid);
-
-  for (int it = 0; it < n_mine; ++it) {
-    const int buf = it & 1;
-    // A[buf] was last read by the MMAs of tile it-2, whose completion epilogue(it-2) waited for
-    pt_split_store<TAct>(regs, sm.a_hi[GRP][buf], sm.a_lo[GRP][buf], gtid);
-    tc::fence_proxy_async_smem();
-    tc::fence_before_thread_sync();
-    group_barrier<GRP>();
-    tc::fence_after_thread_sync();
-    // prefetch AFTER the fence: the membar inside fence.proxy.async would otherwise wait for these loads
-    if (it + 1 < n_mine) pt_prefetch<TAct>(regs, a, tile_of(it + 1), gtid);
-    if (it >= 2) finalize(it - 2);
-    if (gwarp == 0) {
-      if (tc::elect_one()) {
-        const uint32_t d_tmem = tmem_base + buf * kProj;
-        const uint32_t a_s[3] = {tc::smem_addr(sm.a_hi[GRP][buf]), tc::smem_addr(sm.a_lo[GRP][buf]),
-                                 tc::smem_addr(sm.a_hi[GRP][buf])};
-        const uint32_t b_s[3] = {tc::smem_addr(sm.w_hi), tc::smem_addr(sm.w_hi), tc::smem_addr(sm.w_lo)};
-#pragma unroll
-        for (int pass = 0; pass < 3; ++pass) {
-          if (kBf16 && pass == 1) continue;
-          const uint64_t da0 = tc::make_smem_desc(a_s[pass], kPtLboA, 128);
-          const uint64_t db0 = tc::make_smem_desc(b_s[pass], kPtLboB, 128);
-#pragma unroll
-          for (int ks = 0; ks < kC / 8; ++ks) {
-            const uint64_t da = da0 + ((ks * 2 * kPtLboA) >> 4), db = db0 + ((ks * 2 * kPtLboB) >> 4);
-            if (pass == 0 && ks == 0) tc::mma_tf32_imm<false>(d_tmem, da, db, idesc);
-            else tc::mma_tf32_imm<true>(d_tmem, da, db, idesc);
-          }
-          if (pass != 1)  // bias step: ones (exact in tf32, no lo part) x b1 hi (pass 0) / b1 lo (pass 2)
-            tc::mma_tf32_imm<true>(d_tmem, tc::make_smem_desc(tc::smem_addr(sm.ones), kPtLboA, 128),
-                                   tc::make_smem_desc(tc::smem_addr(pass == 0 ? sm.bb_hi : sm.bb_lo), kPtLboB, 128), idesc);
-        }
-        tc::mma_commit(&sm.mma_bar[GRP][buf]);
-      }
-      __syncwarp();
-    }
-    if (it >= 1) epilogue(it - 1);
-  }
-  if (n_mine >= 1) epilogue(n_mine - 1);
-  tc::fence_before_thread_sync();
-  group_barrier<GRP>();
-  tc::fence_after_thread_sync();
-  if (n_mine >= 2) finalize(n_mine - 2);
-  if (n_mine >= 1) finalize(n_mine - 1);
-}
-
 template <typename TAct>
 __global__ void __launch_bounds__(kPtThreads, 1)
     project_tc_kernel(const TAct* __restrict__ a, const float* __restrict__ w1, const float* __restrict__ b1,
                       const float* __restrict__ w2, const float* __restrict__ b2, const float* __restrict__ mask,
                       float* __restrict__ preds, int n_tiles) {
+  constexpr bool kBf16 = sizeof(TAct) == 2;
   extern __shared__ __align__(1024) unsigned char smem_raw[];  // no pointer arithmetic: keeps LDS/STS addressing
   PtSmem& sm = *reinterpret_cast<PtSmem*>(smem_raw);
-  if ((smem_u32(smem_raw) & 127u) != 0) __trap();
-  const int tid = threadIdx.x, warp = tc::warp_index_uniform();
-  const int grp = warp >> 3;          // pipeline 0 / 1
+  const int tid = threadIdx.x, lane = tid & 31;
+  const int wg = tc::warp_index_uniform() >> 2, t = tid & 127, wq = (tid >> 5) & 3;
 
-  if (tid == 0) {
-#pragma unroll
-    for (int i = 0; i < 4; ++i) mbar_init(&sm.mma_bar[i >> 1][i & 1], 1);
-    fence_mbar_init();
-  }
-  if (warp == 0) tc::tmem_alloc<4 * kProj>(&sm.tmem_base);
   for (int e = tid; e < kProj * kC; e += kPtThreads) {  // w1[j][i] -> B[n = j][k = i]
     const int j = e / kC, i = e % kC;
     float hi, lo;
@@ -213,41 +96,98 @@ __global__ void __launch_bounds__(kPtThreads, 1)
     sm.w_hi[off] = hi;
     sm.w_lo[off] = lo;
   }
-  if (tid < kProj / 2) sm.w2q[tid] = make_float4(w2[2 * tid], w2[kProj + 2 * tid], w2[2 * tid + 1], w2[kProj + 2 * tid + 1]);
-  for (int e = tid; e < kPtM * 8; e += kPtThreads)  // e = flat index of the K-major [128][8] tile: k = column
-    sm.ones[tc::kmajor_offset(e >> 3, e & 7, kPtM) / 4] = (e & 7) == 0 ? 1.f : 0.f;
-  for (int e = tid; e < kProj * 8; e += kPtThreads) {
-    float hi = 0.f, lo = 0.f;
-    if ((e & 7) == 0) tc::split_tf32(b1[e >> 3], hi, lo);
-    const uint32_t off = tc::kmajor_offset(e >> 3, e & 7, kProj) / 4;
-    sm.bb_hi[off] = hi;
-    sm.bb_lo[off] = lo;
+  if (tid < kProj / 2) {
+    sm.w2q[tid] = make_float4(w2[2 * tid], w2[kProj + 2 * tid], w2[2 * tid + 1], w2[kProj + 2 * tid + 1]);
+    sm.b1p[tid] = make_float2(b1[2 * tid], b1[2 * tid + 1]);
   }
   const float b2x = b2[0], b2y = b2[1];
-  tc::fence_proxy_async_smem();
-  tc::fence_before_thread_sync();
+  tc::fence_proxy_async_smem();   // the constant operands above are read by the tensor cores
   __syncthreads();
-  tc::fence_after_thread_sync();
   pdl_wait();  // fc1 / fc2 weights above are not produced by the chain; the activations are
   pdl_launch_dependents();
-  if (grp == 0) pt_pipeline<TAct, 0>(sm, a, mask, preds, n_tiles, b2x, b2y);
-  else pt_pipeline<TAct, 1>(sm, a, mask, preds, n_tiles, b2x, b2y);
-  tc::fence_before_thread_sync();
-  __syncthreads();
-  if (warp == 0) tc::tmem_dealloc<4 * kProj>(sm.tmem_base);
+
+  const int first = blockIdx.x * kPtWG + wg, stride = gridDim.x * kPtWG;
+  float* a_hi = sm.a_hi[wg];
+  float* a_lo = sm.a_lo[wg];
+  PtRegs<TAct> regs;
+  if (first < n_tiles) pt_prefetch<TAct>(regs, a, first, t);
+  for (int tile = first; tile < n_tiles; tile += stride) {
+    // the A operand was last read by this pipeline's previous MMAs, which every thread waited for
+    pt_split_store<TAct>(regs, a_hi, a_lo, t);
+    tc::fence_proxy_async_smem();
+    tc::named_barrier(1 + wg, 128);
+    // prefetch AFTER the fence: the membar inside fence.proxy.async would otherwise wait for these loads
+    if (tile + stride < n_tiles) pt_prefetch<TAct>(regs, a, tile + stride, t);
+    float acc[64];
+    tc::wg_fence();
+    {
+      const uint32_t a_s[3] = {tc::smem_addr(a_hi), tc::smem_addr(a_lo), tc::smem_addr(a_hi)};
+      const uint32_t b_s[3] = {tc::smem_addr(sm.w_hi), tc::smem_addr(sm.w_hi), tc::smem_addr(sm.w_lo)};
+#pragma unroll
+      for (int pass = 0; pass < 3; ++pass) {
+        if (kBf16 && pass == 1) continue;
+#pragma unroll
+        for (int ks = 0; ks < kC / 8; ++ks)
+          tc::wg_tf32_ss_n128(acc, tc::make_smem_desc(a_s[pass] + ks * 2 * kPtLboA, kPtLboA, 128),
+                              tc::make_smem_desc(b_s[pass] + ks * 2 * kPtLboB, kPtLboB, 128), (pass | ks) ? 1u : 0u);
+      }
+    }
+    tc::wg_commit();
+    tc::wg_wait<0>();
+    tc::wg_fence_acc(acc);
+    // epilogue: acc[4 i + 2 hh + e] = D[px = 16 wq + lane/4 + 8 hh][j = 8 i + 2 (lane%4) + e]
+    const int b = tile / kPtTilesPerSample, p0 = (tile % kPtTilesPerSample) * kPtM;
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      float2 out = make_float2(0.f, 0.f);   // (out channel 0, out channel 1)
+#pragma unroll
+      for (int i0 = 0; i0 < 16; i0 += 8) {  // 8 pairs at a time: 8 independent polynomial chains in flight
+        float2 g[8];
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          const float2 bb = sm.b1p[4 * (i0 + i) + (lane & 3)];
+          g[i] = make_float2(acc[4 * (i0 + i) + 2 * hh] + bb.x, acc[4 * (i0 + i) + 2 * hh + 1] + bb.y);
+        }
+        if constexpr (kBf16) {
+          gelu_erf2_deg5_batch<8>(g);
+        } else {
+#pragma unroll
+          for (int i = 0; i < 8; ++i) g[i] = gelu_erf2(g[i]);
+        }
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          const float4 wq4 = sm.w2q[4 * (i0 + i) + (lane & 3)];
+          out = ffma2(make_float2(g[i].x, g[i].x), make_float2(wq4.x, wq4.y), out);
+          out = ffma2(make_float2(g[i].y, g[i].y), make_float2(wq4.z, wq4.w), out);
+        }
+      }
+      // the four lanes of a pixel hold disjoint hidden units: fixed-order butterfly sum
+      out.x += __shfl_xor_sync(0xffffffffu, out.x, 1);
+      out.y += __shfl_xor_sync(0xffffffffu, out.y, 1);
+      out.x += __shfl_xor_sync(0xffffffffu, out.x, 2);
+      out.y += __shfl_xor_sync(0xffffffffu, out.y, 2);
+      if ((lane & 3) == 0) {
+        const int pix = p0 + 16 * wq + (lane >> 2) + 8 * hh;
+        const float mk = __ldg(mask + static_cast<size_t>(b) * kHW + pix);
+        preds[(static_cast<size_t>(b) * 2 + 0) * kHW + pix] = (b2x + out.x) * mk;
+        preds[(static_cast<size_t>(b) * 2 + 1) * kHW + pix] = (b2y + out.y) * mk;
+      }
+    }
+  }
 }
 
 template <typename TAct>
 cudaError_t launch_project_tc(const void* a, const float* w1, const float* b1, const float* w2, const float* b2,
                               const float* mask, float* preds, int batch, cudaStream_t stream) {
   auto kern = project_tc_kernel<TAct>;
-  constexpr size_t smem = sizeof(PtSmem) + 128;
+  constexpr size_t smem = sizeof(PtSmem);
   static PerDeviceLaunch pd;
   int n_sm = 0;
   cudaError_t e0 = per_device_setup(kern, smem, pd, &n_sm);
   if (e0 != cudaSuccess) return e0;
   const int n_tiles = batch * kPtTilesPerSample;
-  const int grid = n_tiles < n_sm ? n_tiles : n_sm;
+  const int want = (n_tiles + kPtWG - 1) / kPtWG;
+  const int grid = want < n_sm ? want : n_sm;
   return launch_chained(kern, dim3(grid), dim3(kPtThreads), smem, stream, static_cast<const TAct*>(a), w1, b1, w2, b2,
                         mask, preds, n_tiles);
 }

@@ -1,10 +1,14 @@
-// tcgen05 / TMEM primitives (sm_100a) used by the tensor-core kernels: raw PTX wrappers and the
-// shared-memory / instruction descriptor encodings for kind::tf32 with un-swizzled K-major operands.
+// Hopper (sm_90a) tensor-core primitives used by the wgmma kernels: shared-memory matrix descriptors, warpgroup MMA
+// (wgmma.mma_async) wrappers for the shapes the kernels issue, and the tf32 hi/lo split of 3xTF32.
 //
-// Operand layout ("canonical K-major, SWIZZLE_NONE"): the matrix is tiled in core matrices of
-// 8 rows (M or N) x 16 bytes (4 tf32 along K), each stored as 128 contiguous bytes (row r at r*16 B).
-// SBO = byte distance between core matrices adjacent along M/N, LBO = along K.  One MMA consumes
-// K = 8 (two core matrices, LBO apart); advancing K by 8 adds 2*LBO to the descriptor start address.
+// Operand layout ("canonical K-major, no swizzle"): the matrix is tiled in core matrices of 8 rows (M or N) x 16 bytes
+// (4 tf32 / 8 bf16 along K), each stored as 128 contiguous bytes (row r at r*16 B).  SBO = byte distance between core
+// matrices adjacent along M/N, LBO = along K.  One tf32 MMA consumes K = 8 (two core matrices, LBO apart); advancing K
+// by 8 adds 2*LBO to the descriptor start address.
+//
+// Accumulator fragment of an m64nN wgmma (f32): warp w of the warpgroup, lane l, r = 16 w + l / 4, q = l % 4:
+//   d[4 i + 2 h + e] = D[r + 8 h][8 i + 2 q + e]      (i < N / 8, h, e in {0, 1})
+// tf32 A fragment from registers (m64k8): a[0] = A[r][q], a[1] = A[r + 8][q], a[2] = A[r][q + 4], a[3] = A[r + 8][q + 4].
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -16,153 +20,101 @@ __device__ __forceinline__ uint32_t smem_addr(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
 
-// ---- TMEM allocation (one full warp executes these) -------------------------------------------------
-template <int kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst) {
-  static_assert(kCols >= 32 && kCols <= 512 && (kCols & (kCols - 1)) == 0, "TMEM columns: power of two in [32,512]");
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_addr(smem_dst)), "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int kCols>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols) : "memory");
+// Warp index broadcast from lane 0: tells the compiler the value is warp-uniform, so branches on it are uniform
+// branches and the code under them may use the uniform datapath.
+__device__ __forceinline__ int warp_index_uniform() {
+  return __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);
 }
 
-__device__ __forceinline__ void fence_before_thread_sync() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+// named barrier of `count` threads (ids 1..15; 0 is __syncthreads)
+__device__ __forceinline__ void named_barrier(int id, int count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
-__device__ __forceinline__ void fence_after_thread_sync() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// generic-proxy smem writes -> visible to the async proxy (tensor core operand fetch)
+
+// generic-proxy smem writes -> visible to the async proxy (wgmma operand fetch, TMA)
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
 
 // ---- descriptors ----------------------------------------------------------------------------------
-// 64-bit shared-memory matrix descriptor, SWIZZLE_NONE, Blackwell version field = 1.
+// 64-bit shared-memory matrix descriptor, no swizzle (layout type 0, base offset 0).
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((saddr & 0x3FFFFu) >> 4);              // bits [0,14)  start address >> 4
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;     // bits [16,30) leading byte offset >> 4
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;     // bits [32,46) stride byte offset >> 4
-  d |= static_cast<uint64_t>(1) << 46;                              // bits [46,48) descriptor version (sm_100)
-  return d;                                                         // base_offset 0, lbo_mode 0, layout NONE
+  return d;
 }
-// 32-bit instruction descriptor: D f32, A/B tf32, both K-major, dense, no negate.
-__host__ __device__ constexpr uint32_t make_idesc_tf32(int m, int n) {
-  return (1u << 4)                 // c_format = F32
-         | (2u << 7)               // a_format = TF32
-         | (2u << 10)              // b_format = TF32
-         | (static_cast<uint32_t>(n >> 3) << 17)   // n_dim
-         | (static_cast<uint32_t>(m >> 4) << 24);  // m_dim
+// K-major operand written by TMA with the 128-byte swizzle (rows of 128 B, 8-row atoms of 1024 B, 1024-byte aligned
+// atoms).  A K step inside the 128-byte row advances the start address by its byte width; SBO = 1024.
+__device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t saddr) {
+  return make_smem_desc(saddr, 16, 1024) | (static_cast<uint64_t>(1) << 62);
 }
 
-// Warp index broadcast from lane 0: tells the compiler the value is warp-uniform, so branches on it are uniform
-// branches and the code under them may use the uniform datapath (UR address math, ULDC descriptors) instead of
-// re-deriving every uniform operand with R2UR (14 % of block_tc's executed instructions before this).
-__device__ __forceinline__ int warp_index_uniform() {
-  return __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);
-}
-
-// One elected lane of a converged warp.  Code guarded by this (and fed with warp-uniform values) is compiled
-// to the uniform datapath: back-to-back UTCHMMA with UR operands instead of an R2UR + ELECT loop per MMA.
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "elect.sync _|p, 0xffffffff;\n"
-      "selp.u32 %0, 1, 0, p;\n"
-      "}\n"
-      : "=r"(pred));
-  return pred != 0;
-}
-// compile-time accumulate flag variants (keep the predicate an immediate)
-template <bool kAccumulate>
-__device__ __forceinline__ void mma_tf32_imm(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc) {
-  if constexpr (kAccumulate) {
-    asm volatile(
-        "{\n.reg .pred p;\nsetp.ne.b32 p, 1, 0;\ntcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n}\n" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc)
-        : "memory");
-  } else {
-    asm volatile(
-        "{\n.reg .pred p;\nsetp.ne.b32 p, 0, 0;\ntcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n}\n" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc)
-        : "memory");
-  }
-}
-
-// Same with the A operand in TENSOR MEMORY (row m in lane m, 8 consecutive 32-bit columns per K = 8 step; M = 64 uses
-// the same 16-lanes-per-quadrant placement as the accumulator, tools/tc_probe4.cu).  An MMA whose two operands
-// come from shared memory is bound by their fetch -- (M + N) * 32 B at ~128 B/clk: 45.6 cycles for M=128, N=32 --
-// whereas this form fetches only B: 22.7 cycles (tools/tc_latency.cu, tools/tc_probe3.cu).
-template <bool kAccumulate>
-__device__ __forceinline__ void mma_tf32_tmem_a_imm(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc) {
-  if constexpr (kAccumulate) {
-    asm volatile(
-        "{\n.reg .pred p;\nsetp.ne.b32 p, 1, 0;\ntcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n}\n" ::"r"(d_tmem),
-        "r"(a_tmem), "l"(b_desc), "r"(idesc)
-        : "memory");
-  } else {
-    asm volatile(
-        "{\n.reg .pred p;\nsetp.ne.b32 p, 0, 0;\ntcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n}\n" ::"r"(d_tmem),
-        "r"(a_tmem), "l"(b_desc), "r"(idesc)
-        : "memory");
-  }
-}
-// registers -> TMEM: 32 lanes x 16 consecutive 32-bit columns per warp (its own lane quadrant)
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const float* v) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-      "r"(__float_as_uint(v[0])), "r"(__float_as_uint(v[1])), "r"(__float_as_uint(v[2])), "r"(__float_as_uint(v[3])),
-      "r"(__float_as_uint(v[4])), "r"(__float_as_uint(v[5])), "r"(__float_as_uint(v[6])), "r"(__float_as_uint(v[7])),
-      "r"(__float_as_uint(v[8])), "r"(__float_as_uint(v[9])), "r"(__float_as_uint(v[10])), "r"(__float_as_uint(v[11])),
-      "r"(__float_as_uint(v[12])), "r"(__float_as_uint(v[13])), "r"(__float_as_uint(v[14])), "r"(__float_as_uint(v[15]))
-      : "memory");
-}
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem] * B[smem]^T ; issued by ONE thread
-__device__ __forceinline__ void mma_tf32(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                         bool accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(static_cast<uint32_t>(accumulate))
-      : "memory");
-}
-// arrive on an mbarrier once all previously issued MMAs of this thread have completed
-__device__ __forceinline__ void mma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_addr(bar))
-               : "memory");
-}
-
-// ---- TMEM -> registers: 32 lanes x 32 consecutive fp32 columns per warp ------------------------------
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float* v) {
-  uint32_t r[32];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// ---- warpgroup MMA ----------------------------------------------------------------------------------
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int kPending>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(kPending) : "memory"); }
+// Keeps the compiler from touching accumulator registers across wg_wait (the MMA writes them asynchronously).
+template <int N>
+__device__ __forceinline__ void wg_fence_acc(float (&d)[N]) {
 #pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// D (+)= A * B^T.  _ss: both operands by descriptor; _rs: A from registers (tf32 fragment above).  acc = 0 overwrites D.
+__device__ __forceinline__ void wg_tf32_ss_n24(float* d, uint64_t a, uint64_t b, uint32_t acc) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %14, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n24k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11}, %12, %13, p, 1, 1;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11])
+      : "l"(a), "l"(b), "r"(acc)
+      : "memory");
+}
+__device__ __forceinline__ void wg_tf32_ss_n32(float* d, uint64_t a, uint64_t b, uint32_t acc) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(a), "l"(b), "r"(acc)
+      : "memory");
+}
+__device__ __forceinline__ void wg_tf32_ss_n128(float* d, uint64_t a, uint64_t b, uint32_t acc) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(a), "l"(b), "r"(acc)
+      : "memory");
+}
+__device__ __forceinline__ void wg_bf16_ss_n72(float* d, uint64_t a, uint64_t b, uint32_t acc) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %38, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n72k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35}, %36, %37, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35])
+      : "l"(a), "l"(b), "r"(acc)
+      : "memory");
+}
+__device__ __forceinline__ void wg_tf32_rs_n32(float* d, const uint32_t* a, uint64_t b, uint32_t acc) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %21, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p, 1, 1;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(acc)
+      : "memory");
+}
+__device__ __forceinline__ void wg_tf32_rs_n64(float* d, const uint32_t* a, uint64_t b, uint32_t acc) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %37, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(acc)
+      : "memory");
 }
 
 // ---- operand staging helpers -------------------------------------------------------------------------
-// byte offset of element (row, k) inside a K-major un-swizzled operand tile with `rows` rows:
+// byte offset of element (row, k) inside a K-major un-swizzled tf32 operand tile with `rows` rows:
 // core matrix (row/8, k/4) at ((k/4) * (rows/8) + row/8) * 128
 __host__ __device__ constexpr uint32_t kmajor_offset(int row, int k, int rows) {
   return static_cast<uint32_t>(((k >> 2) * (rows >> 3) + (row >> 3)) * 128 + (row & 7) * 16 + (k & 3) * 4);

@@ -1,64 +1,40 @@
-// Pieces shared by the warp-specialised tcgen05 kernels (fno_block_fused.cu, fno_project_ws.cu): MN-major / swizzled
-// shared-memory descriptors, kind::f16 / kind::tf32 MMA wrappers with a run-time accumulate flag, the 2-D TMA tensor load
-// and the tensor map of a bf16 activation.  Operand forms verified on B200 by tools/tc_probe5.cu.
+// 2-D TMA tensor loads (cp.async.bulk.tensor, completion on an mbarrier) and the encoding of their tensor maps, shared
+// by the TMA-fed kernels (fno_mode_mix.cu, fno_dft_fwd_tc.cu).
 #pragma once
 #include "fno_common.cuh"
-#include "tc_common.cuh"
 #include <cuda.h>
 
 namespace fno {
 
-constexpr uint32_t kAMajorMN = 1u << 15, kBMajorMN = 1u << 16, kANegate = 1u << 13;
-__host__ __device__ constexpr uint32_t fz_idesc_bf16(int m, int n) {  // D f32, A/B bf16
-  return (1u << 4) | (1u << 7) | (1u << 10) | (static_cast<uint32_t>(n >> 3) << 17) | (static_cast<uint32_t>(m >> 4) << 24);
-}
-__device__ __forceinline__ uint64_t fz_desc_sw128(uint32_t saddr, uint32_t lbo, uint32_t sbo) {      // 16-bit MN-major
-  return tc::make_smem_desc(saddr, lbo, sbo) | (static_cast<uint64_t>(2) << 61);
-}
-__device__ __forceinline__ uint64_t fz_desc_sw128_32(uint32_t saddr, uint32_t lbo, uint32_t sbo) {   // 32-bit MN-major
-  return tc::make_smem_desc(saddr, lbo, sbo) | (static_cast<uint64_t>(1) << 61);
-}
-__device__ __forceinline__ void fz_mma_tf32_ss(uint32_t d, uint64_t a, uint64_t b, uint32_t idesc, uint32_t acc) {
-  asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\ntcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n}\n" ::"r"(d),
-               "l"(a), "l"(b), "r"(idesc), "r"(acc) : "memory");
-}
-__device__ __forceinline__ void fz_mma_tf32_ts(uint32_t d, uint32_t a_tmem, uint64_t b, uint32_t idesc, uint32_t acc) {
-  asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\ntcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n}\n" ::"r"(d),
-               "r"(a_tmem), "l"(b), "r"(idesc), "r"(acc) : "memory");
-}
-__device__ __forceinline__ void fz_mma_f16_ss(uint32_t d, uint64_t a, uint64_t b, uint32_t idesc, uint32_t acc) {
-  asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\ntcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n}\n" ::"r"(d),
-               "l"(a), "l"(b), "r"(idesc), "r"(acc) : "memory");
-}
-__device__ __forceinline__ void fz_tma_load_2d(void* dst, const CUtensorMap* tm, int c0, int c1, uint64_t* bar) {
+__device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* tm, int c0, int c1, uint64_t* bar) {
   asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(
                    smem_u32(dst)),
                "l"(tm), "r"(c0), "r"(c1), "r"(smem_u32(bar))
                : "memory");
 }
 
-// tensor map of a bf16 activation [batch * 32 rows][4096 px], box {64 px, 32 rows}, 128B swizzle
-typedef CUresult (*FzEncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                               const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                               CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-inline cudaError_t fz_make_map(const void* act, int batch, CUtensorMap* out) {
-  static FzEncodeFn fn = nullptr;
+// Row-major 2-D tensor [rows][inner] (row pitch = inner elements), box {box_inner, box_rows}, 128-byte swizzle: every
+// box row is one 128-byte line, and the 16-byte chunk c of line r lands at chunk position c ^ (r & 7).
+typedef CUresult (*TmaEncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
+                                const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
+                                CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+inline cudaError_t make_tma_map_2d(CUtensorMap* out, CUtensorMapDataType dtype, size_t elt_bytes, const void* base,
+                                   uint64_t inner, uint64_t rows, uint32_t box_inner, uint32_t box_rows) {
+  static TmaEncodeFn fn = nullptr;
   if (!fn) {
     void* p = nullptr;
     cudaDriverEntryPointQueryResult q;
     cudaError_t e = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q);
     if (e != cudaSuccess) return e;
     if (!p) return cudaErrorNotSupported;
-    fn = reinterpret_cast<FzEncodeFn>(p);
+    fn = reinterpret_cast<TmaEncodeFn>(p);
   }
-  const cuuint64_t gdim[2] = {static_cast<cuuint64_t>(kHW), static_cast<cuuint64_t>(batch) * kC};
-  const cuuint64_t gstride[1] = {static_cast<cuuint64_t>(kHW) * 2};
-  const cuuint32_t box[2] = {64, static_cast<cuuint32_t>(kC)}, estr[2] = {1, 1};
-  const CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(act), gdim, gstride, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  const cuuint64_t gdim[2] = {static_cast<cuuint64_t>(inner), static_cast<cuuint64_t>(rows)};
+  const cuuint64_t gstride[1] = {static_cast<cuuint64_t>(inner * elt_bytes)};
+  const cuuint32_t box[2] = {box_inner, box_rows}, estr[2] = {1, 1};
+  const CUresult r = fn(out, dtype, 2, const_cast<void*>(base), gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                        CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return r == CUDA_SUCCESS ? cudaSuccess : cudaErrorInvalidValue;
 }
-
 
 }  // namespace fno

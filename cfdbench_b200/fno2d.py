@@ -1,4 +1,4 @@
-"""Drop-in `Fno2d` for CFDBench backed by the sm_100a kernels in libcfdbench_b200.so.
+"""Drop-in `Fno2d` for CFDBench backed by the sm_90a kernels in libcfdbench_b200.so.
 
 Mirrors the reference module's public surface (reference src/models/fno/fno2d.py:115-295):
 same constructor keywords as `utils/autoregressive.py:114-125` passes, same parameter names /
@@ -157,7 +157,7 @@ class Fno2d(AutoCfdModel):
         self._dp_events = None
         self._dp_stream = None
         # how the flat gradient buffer is all-reduced: "one" collective after backward, "two" (upper half of the network
-        # while the lower half is still in backward) or "all" (one per gradient group); measured in profiles/README.md
+        # while the lower half is still in backward) or "all" (one per gradient group); tools/time_train_dp.py compares them
         self.dp_segments = os.environ.get("FNO_DP_SEGMENTS", "one")
         # CUDA-graph replay of device-resident rollouts: one capture per (batch, steps), the 18 launches of every
         # step replayed as one graph (B=256: 591 -> 544 us/step, B=1: 2.09 -> 1.48 ms per 20 steps).  False = launch
@@ -398,9 +398,8 @@ class Fno2d(AutoCfdModel):
         # Optional: reduce the flat buffer segment by segment, each as soon as its gradients are final -- the native
         # backward records one event per segment (fc1/fc2, block L-1 .. block 0, fc0) and a side stream starts the NCCL
         # all-reduce (ReduceOp.AVG) of that slice while the remaining backward kernels still run on the main stream.
-        # Measured on 2 x B200 (tools/time_train_dp.py): no gain -- cylinder B=256/GPU 4.89 ms in every mode (4.83 ms on one
-        # GPU), cavity B=64/GPU 1.83 ("one") / 1.87 ("two") / 2.04 ms ("all"): the 9.5 MB collective costs less than the
-        # extra launches and the SM contention between NCCL's kernels and the persistent backward kernels.
+        # tools/time_train_dp.py compares the modes; the 9.5 MB collective is small next to the extra launches and the SM
+        # contention between NCCL's kernels and the persistent backward kernels, so "one" is the default.
         from .dp import allreduce_mean_async
         ends = {name: off + n for name, _p, off, n in layout}
         starts = {name: off for name, _p, off, n in layout}

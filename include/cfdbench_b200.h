@@ -1,4 +1,4 @@
-/* cfdbench_b200 -- C ABI of the B200-native FNO hot path for CFDBench.
+/* cfdbench_b200 -- C ABI of the H100-native FNO hot path for CFDBench.
  *
  * The reference (luo-yining/CFDBench @ 6c30c62) is pure Python/PyTorch: its "FFI" for this path is the
  * set of ATen calls made by src/models/fno/fno2d.py.  Each entry point below replaces the calls cited

@@ -1,6 +1,6 @@
 """TEST INFRASTRUCTURE -- generate tests/golden/*.npz from the UNMODIFIED reference module.
 
-Run in the build container only (needs /root/reference):
+Needs the reference tree that `oracle/install_reference.py` places in the git-ignored oracle/_ref/src:
 
     PYTHONDONTWRITEBYTECODE=1 python oracle/make_golden.py
 
@@ -20,7 +20,7 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, "/root/reference/src")
+sys.path.insert(0, os.path.join(ROOT, "oracle", "_ref", "src"))
 sys.dont_write_bytecode = True
 
 from models.fno.fno2d import Fno2d, SpectralConv2d_fast  # noqa: E402  (the reference)
@@ -109,8 +109,9 @@ def main() -> None:
             preds=out["preds"].detach().numpy(),
             loss=np.array([out["loss"][k].item() for k in ("mse", "rmse", "mae", "nmse")], dtype=np.float64),
             rollout=np.stack([r.numpy() for r in roll]),
-            act0_b0=acts[0][:1], act1_b0=acts[1][:1], act4_b0=acts[-1][:1],
-            spectral0_b0=spec[:1],
+            # hidden tensors of sample 0 on every 8th channel (0, 8, 16, 24): keeps each fixture below 1 MB
+            act0_b0=acts[0][:1, ::8], act1_b0=acts[1][:1, ::8], act4_b0=acts[-1][:1, ::8],
+            spectral0_b0=spec[:1, ::8],
         )
         for k in ("fc0.weight", "fc0.bias", "fc1.weight", "fc1.bias", "fc2.weight", "fc2.bias",
                   "blocks.0.w0.weight", "blocks.0.w0.bias", "blocks.3.w0.weight", "blocks.3.w0.bias"):

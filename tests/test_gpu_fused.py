@@ -130,8 +130,8 @@ def test_mode_mix_image_kernel(lib):
 
 
 def test_mode_mix_ring_recycling_large_batch(lib):
-    """700 samples = 6 sample tiles per mode, 12 tiles per CTA: the 4-slot A ring, the 4 accumulators and the 4 lo-operand
-    blocks in tensor memory are each reused three times, the B ring's two slots hold the CTA's two modes (ragged last tile).
+    """700 samples = 6 sample tiles per mode, 12 or 18 tiles per CTA: the 4-slot A ring is reused three or more times, the B
+    ring's two slots hold the CTA's first two modes and are refilled for a third (ragged last tile).
     Both outputs (mode-major ym, per-sample operand image) against float64 on a sample of modes."""
     from cfdbench_b200 import _lib
     rng = np.random.default_rng(12)
@@ -145,7 +145,7 @@ def test_mode_mix_ring_recycling_large_batch(lib):
     ym = torch.zeros(288, batch, 32, dtype=torch.complex64, device="cuda")
     _lib.check(lib.fno_mode_mix(xmd.data_ptr(), wop.data_ptr(), ym.data_ptr(), batch, stream()), "mix")
     wt = onp.stack_weights(w1, w2).reshape(32, 32, 288)
-    modes = [0, 1, 147, 148, 149, 200, 286, 287]   # first / second round of the 148 CTAs, last modes
+    modes = [0, 1, 131, 132, 133, 147, 200, 286, 287]   # first / second / third round of the 132 CTAs, last modes
     ref = np.einsum("kbi,iok->kbo", xm[modes].astype(np.complex128), wt[:, :, modes])
     got = ym.cpu().numpy()
     assert np.linalg.norm(got[modes] - ref) / np.linalg.norm(ref) < 2e-6
@@ -159,7 +159,7 @@ def test_mode_mix_ring_recycling_large_batch(lib):
 @pytest.mark.parametrize("batch", [1, 3, 80])
 def test_block_fused_kernel(lib, batch):
     """irfft2 (both stages on tensor cores, Z kept on chip) + 1x1 conv + bias + GELU, bf16 in / bf16 out.
-    80 samples = 160 work units > 148 CTAs: some CTAs run two units (D1 / ring phase wrap-around)."""
+    80 samples = 320 work units on 132 CTAs: every CTA runs two or three units (image ring phase wrap-around)."""
     from cfdbench_b200 import _lib
     rng = np.random.default_rng(20 + batch)
     ym = (rng.standard_normal((batch, 32, 24, 12)) + 1j * rng.standard_normal((batch, 32, 24, 12))) * 40.0
@@ -212,9 +212,9 @@ def test_block_fused_equals_unfused_path(lib):
 
 @pytest.mark.parametrize("batch,problem", [(1, "cavity"), (5, "cylinder"), (40, "cavity")])
 def test_project_ws_kernel_bf16(lib, batch, problem):
-    """fc1 + GELU + fc2 + mask on bf16 activations (project_ws_kernel: TMA-fed kind::f16 MMAs, W1 / b1 as three bf16
-    pieces): the inputs are bf16-exact, so the comparison with the float64 oracle measures the arithmetic only.
-    40 samples = 1280 tiles > 148 CTAs x 4 slots: every ring slot wraps several times."""
+    """fc1 + GELU + fc2 + mask on bf16 activations (project_tc_kernel<bf16>: wgmma with W1 as tf32 hi / lo): the inputs
+    are bf16-exact, so the comparison with the float64 oracle measures the arithmetic only.
+    40 samples = 2560 tiles > 132 CTAs x 4 pipelines: every pipeline runs several tiles."""
     from cfdbench_b200 import _lib
     p = synth.n_case_params(problem)
     sd = synth.make_state_dict(5, n_params=p)

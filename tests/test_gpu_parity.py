@@ -1,4 +1,4 @@
-"""GPU parity tests (run with `-m gpu` on a B200): every CUDA kernel and the whole model, called
+"""GPU parity tests (run with `-m gpu` on an H100): every CUDA kernel and the whole model, called
 through the C ABI / the drop-in module, against the oracles and the golden vectors generated from
 the reference module.  Tolerance for fp32-storage mode is BASELINE.json's 1e-5 relative L2."""
 import ctypes as C
@@ -147,7 +147,7 @@ def test_mode_mix_and_pack_kernels(lib):
 
 @pytest.mark.parametrize("batch", [1, 3, 41])
 def test_dft_fwd_tensor_core_kernel_bf16_storage(lib, batch):
-    """bf16 planes through dft_fwd_tc_kernel (two chained UMMA GEMMs; the forward path of bf16 storage) by its own entry
+    """bf16 planes through dft_fwd_tc_kernel (two chained wgmma GEMMs; the forward path of bf16 storage) by its own entry
     point and through fno_spectral_dft_fwd (which routes bf16 planes to it unless FNO_DFT_TC=0 selects the register-FFT
     kernel); 41 samples = 328 plane batches, i.e. up to three per persistent CTA (pipeline steady state + ragged tail).
     The inputs are bf16-exact, so the comparison with the float64 oracle measures the arithmetic only."""

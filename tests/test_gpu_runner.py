@@ -1,7 +1,7 @@
 """The reference's own scripts, UNCHANGED, on the drop-in (north_star: "train_auto.py and test_multistep.py run unchanged").
 
-`baseline/_ref/src` is the unmodified reference tree copied by `__graft_entry__.build()` (git-ignored, travels to the GPU
-box with the snapshot).  `python -m cfdbench_b200.runner <src> <script> --stub-missing ...` rebinds the plug-in seam
+`oracle/_ref/src` is the unmodified reference tree copied by `__graft_entry__.build()` (git-ignored;
+oracle/install_reference.py).  `python -m cfdbench_b200.runner <src> <script> --stub-missing ...` rebinds the plug-in seam
 (reference src/utils/autoregressive.py:10) and runs the script as `__main__`; stand-ins are installed only for packages
 this image lacks (tap, matplotlib, diffusers, ...).  Data: a tiny on-disk cavity set in the reference's format
 (tools/make_tiny_cavity.py; reference src/dataset/cavity.py:15-34).
@@ -11,6 +11,7 @@ StepLR :214-216,280, checkpoint save :301), :126-152 (test) and src/test_multist
 per-step metrics, load_best_ckpt)."""
 import json
 import os
+import shutil
 import subprocess
 import sys
 
@@ -19,17 +20,29 @@ import pytest
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF_SRC = os.path.join(ROOT, "baseline", "_ref", "src")
+REF_SRC = os.path.join(ROOT, "oracle", "_ref", "src")
 
 pytestmark = [pytest.mark.gpu,
               pytest.mark.skipif(not os.path.isdir(os.path.join(REF_SRC, "models", "fno")),
-                                 reason="baseline/_ref/src (installed by __graft_entry__.build()) is not present")]
+                                 reason="oracle/_ref/src (installed by __graft_entry__.build()) is not present")]
 
 COMMON = ["--model", "fno", "--data_name", "cavity_prop_bc_geo", "--loss_name", "nmse", "--lr", "0.001"]
 
 
-def run_script(script, data_dir, out_dir, extra, act=None):
-    cmd = [sys.executable, "-m", "cfdbench_b200.runner", REF_SRC, script, "--stub-missing"]
+@pytest.fixture(scope="module")
+def ref_src(tmp_path_factory):
+    """A private copy of the reference tree: its scripts write next to themselves, and the repository may be read-only."""
+    d = str(tmp_path_factory.mktemp("ref") / "src")
+    shutil.copytree(REF_SRC, d)
+    for root, dirs, files in os.walk(d):   # the copy keeps the source's modes
+        os.chmod(root, 0o755)
+        for f in files:
+            os.chmod(os.path.join(root, f), 0o644)
+    return d
+
+
+def run_script(src, script, data_dir, out_dir, extra, act=None):
+    cmd = [sys.executable, "-m", "cfdbench_b200.runner", src, script, "--stub-missing"]
     if act:
         cmd += ["--act-dtype", act]
     cmd += COMMON + ["--data_dir", data_dir, "--output_dir", out_dir] + extra
@@ -47,9 +60,9 @@ def tiny(tmp_path_factory):
 
 
 @pytest.mark.parametrize("act", [None, "bfloat16"])
-def test_train_auto_and_test_multistep_run_unchanged(tiny, tmp_path, act):
+def test_train_auto_and_test_multistep_run_unchanged(ref_src, tiny, tmp_path, act):
     out = str(tmp_path / "result")
-    r = run_script("train_auto.py", tiny, out, ["--num_epochs", "2", "--batch_size", "4", "--eval_batch_size", "2",
+    r = run_script(ref_src, "train_auto.py", tiny, out, ["--num_epochs", "2", "--batch_size", "4", "--eval_batch_size", "2",
                                                 "--eval_interval", "1", "--log_interval", "2", "--mode", "train_test"], act)
     assert r.returncode == 0, (r.stdout[-1500:], r.stderr[-3000:])
     assert "====== Training done ======" in r.stdout and "=== Testing done ===" in r.stdout
@@ -74,7 +87,7 @@ def test_train_auto_and_test_multistep_run_unchanged(tiny, tmp_path, act):
     ckpt = os.path.join(run_dir, "ckpt-1", "model.pt")
     code = f"""
 import sys, json, torch, numpy as np
-sys.path.insert(0, {REF_SRC!r}); sys.path.insert(0, {ROOT!r})
+sys.path.insert(0, {ref_src!r}); sys.path.insert(0, {ROOT!r})
 from models.fno.fno2d import Fno2d as Ref
 from models.loss import loss_name_to_fn
 sd = torch.load({ckpt!r}, map_location="cpu")
@@ -94,7 +107,7 @@ print(json.dumps(dict(rel=float((a - b).norm() / a.norm()))))
     assert r2.returncode == 0, r2.stderr[-2000:]
     assert json.loads(r2.stdout.strip().splitlines()[-1])["rel"] < 1e-5
 
-    r3 = run_script("test_multistep.py", tiny, out, [], act)
+    r3 = run_script(ref_src, "test_multistep.py", tiny, out, [], act)
     assert r3.returncode == 0, (r3.stdout[-1500:], r3.stderr[-3000:])
     metrics = json.load(open(os.path.join(run_dir, "multistep_metrics.json")))
     assert len(metrics) == 20 and all(np.isfinite(m_["nmse"]) and np.isfinite(m_["mse"]) for m_ in metrics)

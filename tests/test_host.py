@@ -315,7 +315,7 @@ def test_bench_reference_arm_prints_one_contract_line():
         assert key in d, key
     assert d["impl"] == "reference" and d["metric"] == "fno_rollout_steps_per_sec" and d["unit"] == "steps/s"
     assert d["higher_is_better"] is True and d["gpu_launches"] == 0 and d["value"] > 0
-    ref_installed = os.path.isdir(os.path.join(ROOT, "baseline", "_ref", "src", "models", "fno"))
+    ref_installed = os.path.isdir(os.path.join(ROOT, "oracle", "_ref", "src", "models", "fno"))
     assert d["cpu_baseline"]["kind"] == ("reference" if ref_installed else "port") and d["cpu_baseline"]["cores"] >= 1
     assert d["cpu_baseline"]["cpu_model"]
     assert d["e2e"]["h2d_bytes_per_step"] == 0 and d["e2e"]["d2h_bytes_per_step"] == 0

@@ -41,9 +41,10 @@ def test_torch_port_matches_reference_golden(name):
     assert onp.rel_l2(out["preds"].detach().numpy(), g["preds"].astype(np.float64)) < 1e-6
     loss = np.array([out["loss"][k].item() for k in ("mse", "rmse", "mae", "nmse")])
     np.testing.assert_allclose(loss, g["loss"], rtol=1e-5)
-    assert onp.rel_l2(out["acts"][0][:1].detach().numpy(), g["act0_b0"].astype(np.float64)) < 1e-6
-    assert onp.rel_l2(out["acts"][1][:1].detach().numpy(), g["act1_b0"].astype(np.float64)) < 1e-6
-    assert onp.rel_l2(out["acts"][-1][:1].detach().numpy(), g["act4_b0"].astype(np.float64)) < 1e-6
+    # the hidden-tensor fixtures hold sample 0 on every 8th channel
+    assert onp.rel_l2(out["acts"][0][:1, ::8].detach().numpy(), g["act0_b0"].astype(np.float64)) < 1e-6
+    assert onp.rel_l2(out["acts"][1][:1, ::8].detach().numpy(), g["act1_b0"].astype(np.float64)) < 1e-6
+    assert onp.rel_l2(out["acts"][-1][:1, ::8].detach().numpy(), g["act4_b0"].astype(np.float64)) < 1e-6
     out["loss"]["nmse"].backward()
     for key in g.files:
         if key.startswith("grad::"):
@@ -63,11 +64,12 @@ def test_numpy_oracle_matches_reference_golden(name):
     out = onp.fno_forward(sd, batch["inputs"], batch["case_params"], batch["mask"], batch["label"],
                           return_acts=True)
     assert onp.rel_l2(g["preds"], out["preds"]) < 2e-6
-    assert onp.rel_l2(g["act1_b0"], out["acts"][1][:1]) < 2e-6
+    assert onp.rel_l2(g["act0_b0"], out["acts"][0][:1, ::8]) < 2e-6   # sample 0, every 8th channel
+    assert onp.rel_l2(g["act1_b0"], out["acts"][1][:1, ::8]) < 2e-6
     for i, k in enumerate(("mse", "rmse", "mae", "nmse")):
         assert abs(out["loss"][k] - g["loss"][i]) <= 2e-6 * abs(g["loss"][i])
-    spec = onp.spectral_conv(g["act0_b0"], sd["blocks.0.conv0.weights1"], sd["blocks.0.conv0.weights2"])
-    assert onp.rel_l2(g["spectral0_b0"], spec) < 2e-6
+    spec = onp.spectral_conv(out["acts"][0][:1], sd["blocks.0.conv0.weights1"], sd["blocks.0.conv0.weights2"])
+    assert onp.rel_l2(g["spectral0_b0"], spec[:, ::8]) < 2e-6
 
 
 def test_numpy_oracle_gradients_match_reference_golden():
