@@ -130,6 +130,9 @@ SIGNATURES = {
     "fno_backward": (C.c_int, [C.POINTER(FnoWeights), C.POINTER(FnoWeightsBwd), _P, _P, _P, _P,
                                C.POINTER(FnoTrainSaved), C.POINTER(FnoGrads), C.POINTER(FnoBwdScratch),
                                C.POINTER(FnoWorkspace), _I, _I, _P]),
+    "fno_backward_inputs": (C.c_int, [C.POINTER(FnoWeights), C.POINTER(FnoWeightsBwd), _P, _P, _P, _P,
+                                      C.POINTER(FnoTrainSaved), C.POINTER(FnoGrads), C.POINTER(FnoBwdScratch),
+                                      C.POINTER(FnoWorkspace), _P, _P, _I, _I, _P, C.POINTER(C.c_void_p)]),
 }
 
 _lib = None

@@ -49,6 +49,7 @@ cudaError_t launch_multistep_metrics(const float*, const float*, const float*, f
 cudaError_t launch_spectral_wgrad(const void*, const void*, void*, int, cudaStream_t);
 cudaError_t launch_lift_bwd(const float*, const float*, const float*, const float*, const float*, const float*,
                             float*, float*, float*, int, int, cudaStream_t);
+cudaError_t launch_lift_bwd_data(const float*, const float*, float*, float*, int, int, cudaStream_t);
 }  // namespace fno
 
 using namespace fno;
@@ -371,21 +372,24 @@ int fno_forward_train(const fno_weights* w, const float* inputs, const float* ma
   return fno_project_fwd(saved->act[w->n_layers], mask, w, preds, batch, act_dtype, stream);
 }
 
-int fno_backward(const fno_weights* w, const fno_weights_bwd* wb, const float* inputs, const float* mask,
-                 const float* case_params, const float* dpreds, const fno_train_saved* saved,
-                 const fno_grads* g, const fno_bwd_scratch* sc, const fno_workspace* ws, int batch,
-                 int act_dtype, void* stream) {
-  return fno_backward_ex(w, wb, inputs, mask, case_params, dpreds, saved, g, sc, ws, batch, act_dtype, stream, nullptr);
-}
-
-int fno_backward_ex(const fno_weights* w, const fno_weights_bwd* wb, const float* inputs, const float* mask,
-                    const float* case_params, const float* dpreds, const fno_train_saved* saved,
-                    const fno_grads* g, const fno_bwd_scratch* sc, const fno_workspace* ws, int batch,
-                    int act_dtype, void* stream, void* const* seg_events) {
-  if (!w || !wb || !inputs || !mask || !dpreds || !saved || !g || !sc || !ws || batch <= 0 || bad_dtype(act_dtype))
-    return fail(kErrArg, "fno_backward: bad argument");
-  if (!sc->d[0] || !sc->d[1] || !sc->dz1 || !sc->gm || !sc->gwk || !sc->partials || !ws->ym || !ws->z)
-    return fail(kErrArg, "fno_backward: null scratch buffer");
+// The backward pass behind fno_backward, fno_backward_ex and fno_backward_inputs.  g == NULL: no parameter gradients --
+// every weight-gradient launch (the reduce_partials / chan_outer of fc1, fc2 and w0, spectral_wgrad,
+// unpack_spectral_grads, lift_bwd) is skipped and only the data path runs.  d_inputs / d_case_params (either may be NULL)
+// receive the lift's data adjoint of dL/da0 (lift_bwd_data_kernel); with both NULL and g set, the launches are exactly
+// those of the parameter-only backward.
+static int backward_impl(const char* what, const fno_weights* w, const fno_weights_bwd* wb, const float* inputs,
+                         const float* mask, const float* case_params, const float* dpreds, const fno_train_saved* saved,
+                         const fno_grads* g, const fno_bwd_scratch* sc, const fno_workspace* ws, int batch, int act_dtype,
+                         void* stream, void* const* seg_events, float* d_inputs, float* d_case_params) {
+  char msg[128];
+  if (!w || !wb || !inputs || !mask || !dpreds || !saved || !sc || !ws || batch <= 0 || bad_dtype(act_dtype)) {
+    snprintf(msg, sizeof(msg), "%s: bad argument", what);
+    return fail(kErrArg, msg);
+  }
+  if (!sc->d[0] || !sc->d[1] || !sc->dz1 || !sc->gm || !sc->gwk || !sc->partials || !ws->ym || !ws->z) {
+    snprintf(msg, sizeof(msg), "%s: null scratch buffer", what);
+    return fail(kErrArg, msg);
+  }
   cudaStream_t st = S(stream);
   const int L = w->n_layers, p = w->n_case_params;
   const bool bf = act_dtype == FNO_ACT_BF16;
@@ -419,6 +423,7 @@ int fno_backward_ex(const fno_weights* w, const fno_weights_bwd* wb, const float
              : launch_project_bwd<float>(a_l, dp, mk, pre, w->fc1_w, w->fc1_b, w->fc2_w, dout, sc->dz1, part_pb, nb, st);
     }
     FNO_CUDA(e, "project_bwd_kernel");
+    if (!g) continue;   // data-only: the partial rows just written are never reduced
     const int accum = b0 > 0 ? 1 : 0;
     FNO_CUDA(launch_reduce_partials(part_pb, rows, rs, g->fc2_w, 2 * kProj, g->fc1_b, kProj, g->fc2_b, 2, accum, st),
              "reduce(fc2.weight | fc1.bias | fc2.bias)");
@@ -440,15 +445,19 @@ int fno_backward_ex(const fno_weights* w, const fno_weights_bwd* wb, const float
   for (int l = L - 1; l >= 0; --l) {
     float* dpre = sc->d[cur];
     float* dnext = sc->d[cur ^ 1];
-    int n_co = 0;
-    cudaError_t e = bf ? launch_chan_outer<float, __nv_bfloat16, 32, 32>(dpre, saved->act[l], part_co, &n_co, batch, st)
-                       : launch_chan_outer<float, float, 32, 32>(dpre, saved->act[l], part_co, &n_co, batch, st);
-    FNO_CUDA(e, "chan_outer_kernel(w0)");
-    FNO_CUDA(launch_reduce_partials(part_co, n_co, kC * kC + kC, g->w0_w[l], kC * kC, g->w0_b[l], kC, nullptr, 0, 0, st),
-             "reduce(w0.weight | w0.bias)");
+    if (g) {
+      int n_co = 0;
+      cudaError_t e = bf ? launch_chan_outer<float, __nv_bfloat16, 32, 32>(dpre, saved->act[l], part_co, &n_co, batch, st)
+                         : launch_chan_outer<float, float, 32, 32>(dpre, saved->act[l], part_co, &n_co, batch, st);
+      FNO_CUDA(e, "chan_outer_kernel(w0)");
+      FNO_CUDA(launch_reduce_partials(part_co, n_co, kC * kC + kC, g->w0_w[l], kC * kC, g->w0_b[l], kC, nullptr, 0, 0, st),
+               "reduce(w0.weight | w0.bias)");
+    }
     FNO_TRY(fno_spectral_dft_fwd(dpre, sc->gm, batch, FNO_ACT_F32, inv, 2.f * inv, stream));
-    FNO_CUDA(launch_spectral_wgrad(saved->xm[l], sc->gm, sc->gwk, batch, st), "spectral_wgrad_kernel");
-    FNO_TRY(fno_unpack_spectral_grads(sc->gwk, g->spec_w1[l], g->spec_w2[l], stream));
+    if (g) {
+      FNO_CUDA(launch_spectral_wgrad(saved->xm[l], sc->gm, sc->gwk, batch, st), "spectral_wgrad_kernel");
+      FNO_TRY(fno_unpack_spectral_grads(sc->gwk, g->spec_w1[l], g->spec_w2[l], stream));
+    }
     FNO_CUDA(mark(1 + (L - 1 - l)), "cudaEventRecord(block gradients)");
     FNO_TRY(fno_mode_mix(sc->gm, wb->spec_wkT[l], ws->ym, batch, stream));
     FNO_TRY(fno_spectral_inv_kx(ws->ym, ws->z, batch, 1.f, 1.f, stream));
@@ -456,10 +465,44 @@ int fno_backward_ex(const fno_weights* w, const fno_weights_bwd* wb, const float
                           l > 0 ? saved->pre[l - 1] : nullptr, batch, FNO_ACT_F32, stream));
     cur ^= 1;
   }
-  FNO_CUDA(launch_lift_bwd(sc->d[cur], inputs, mask, case_params, w->gx, w->gy, g->fc0_w, g->fc0_b, part_lb, batch, p, st),
-           "lift_bwd_kernel");
+  // sc->d[cur] = dL/da0, the gradient at the lift output (a bf16-stored a0 is differentiated straight through)
+  if (g)
+    FNO_CUDA(launch_lift_bwd(sc->d[cur], inputs, mask, case_params, w->gx, w->gy, g->fc0_w, g->fc0_b, part_lb, batch, p, st),
+             "lift_bwd_kernel");
   FNO_CUDA(mark(L + 1), "cudaEventRecord(fc0 gradients)");
+  if (d_inputs || d_case_params)
+    FNO_CUDA(launch_lift_bwd_data(sc->d[cur], w->fc0_w, d_inputs, d_case_params, batch, p, st), "lift_bwd_data_kernel");
   return kOk;
+}
+
+int fno_backward(const fno_weights* w, const fno_weights_bwd* wb, const float* inputs, const float* mask,
+                 const float* case_params, const float* dpreds, const fno_train_saved* saved,
+                 const fno_grads* g, const fno_bwd_scratch* sc, const fno_workspace* ws, int batch,
+                 int act_dtype, void* stream) {
+  return fno_backward_ex(w, wb, inputs, mask, case_params, dpreds, saved, g, sc, ws, batch, act_dtype, stream, nullptr);
+}
+
+int fno_backward_ex(const fno_weights* w, const fno_weights_bwd* wb, const float* inputs, const float* mask,
+                    const float* case_params, const float* dpreds, const fno_train_saved* saved,
+                    const fno_grads* g, const fno_bwd_scratch* sc, const fno_workspace* ws, int batch,
+                    int act_dtype, void* stream, void* const* seg_events) {
+  if (!g) return fail(kErrArg, "fno_backward: bad argument");
+  return backward_impl("fno_backward", w, wb, inputs, mask, case_params, dpreds, saved, g, sc, ws, batch, act_dtype, stream,
+                       seg_events, nullptr, nullptr);
+}
+
+int fno_backward_inputs(const fno_weights* w, const fno_weights_bwd* wb, const float* inputs, const float* mask,
+                        const float* case_params, const float* dpreds, const fno_train_saved* saved,
+                        const fno_grads* grads, const fno_bwd_scratch* scratch, const fno_workspace* ws,
+                        float* d_inputs, float* d_case_params, int batch, int act_dtype, void* stream,
+                        void* const* seg_events) {
+  if (w && (w->n_case_params < 0 || w->n_case_params > kMaxCaseParams))
+    return fail(kErrArg, "fno_backward_inputs: n_case_params out of range");
+  if (w && w->n_case_params == 0) d_case_params = nullptr;   // nothing to write
+  if (!grads && !d_inputs && !d_case_params) return fail(kErrArg, "fno_backward_inputs: no output requested");
+  if ((reinterpret_cast<uintptr_t>(d_inputs) & 15) != 0) return fail(kErrArg, "fno_backward_inputs: d_inputs must be 16-byte aligned");
+  return backward_impl("fno_backward_inputs", w, wb, inputs, mask, case_params, dpreds, saved, grads, scratch, ws, batch,
+                       act_dtype, stream, seg_events, d_inputs, d_case_params);
 }
 
 int fno_multistep_metrics(const float* preds_seq, const float* label_u, const float* mask, float* sums, int steps,

@@ -9,6 +9,7 @@
 //   chan_outer_kernel    G[j][i] += sum_{b,pix} P[b][j][pix] Q[b][i][pix]  (1x1-conv weight gradients)
 //   spectral_wgrad_kernel  gWk[k][i][o] = sum_b conj(X[b][k][i]) G[b][k][o]   (SURVEY.md 8a)
 //   lift_bwd_kernel      gradients of fc0 (spatial feature columns + folded per-sample constants)
+//   lift_bwd_data_kernel gradients w.r.t. the input frame (u, v) and the case parameters
 #include "fno_common.cuh"
 
 namespace fno {
@@ -556,6 +557,107 @@ cudaError_t launch_lift_bwd(const float* da0, const float* inputs, const float* 
   if (e != cudaSuccess) return e;
   const int n = kC * (5 + p + 1);
   lift_bwd_reduce_kernel<<<(n + 127) / 128, 128, 0, stream>>>(partial, static_cast<int>(grid.y), 5 + p, g_w, g_b);
+  return cudaGetLastError();
+}
+
+// ---------------------------------------------------------------------------------- lift bwd (data)
+// The data adjoint of the lift (gradients w.r.t. the input frame and the case parameters):
+//   d_inputs[b][c][pix] = sum_o fc0_w[o][c] d_a0[b][o][pix]                  c = 0 (u), 1 (v)
+//   d_params[b][j]      = sum_o fc0_w[o][5 + j] sum_pix d_a0[b][o][pix]
+// One CTA owns one sample, so the plane sums are block reductions in a fixed order (warp butterflies, then warps in
+// index order): no atomics, bit-reproducible.  Thread = kLdVec groups of 4 consecutive pixels, 16-byte loads and stores;
+// the case-parameter weights are applied to each thread's per-channel pixel sum on the fly, so only p values per thread
+// are reduced at the end.  One pass over d_a0 (float32 in both storage modes, 134 MB at B = 256).
+constexpr int kLdThreads = 512;
+constexpr int kLdVec = kHW / (4 * kLdThreads);   // float4 groups per thread and channel
+
+__global__ void __launch_bounds__(kLdThreads)
+    lift_bwd_data_kernel(const float* __restrict__ da0,     // [B][32][4096]
+                         const float* __restrict__ fc0_w,   // [32][5+p]
+                         float* __restrict__ d_inputs,      // [B][2][4096] or null
+                         float* __restrict__ d_params,      // [B][p] or null
+                         int p) {
+  __shared__ float wu[kC], wv[kC];
+  __shared__ __align__(16) float wp[kC][kMaxCaseParams];   // columns 5..5+p, zero-padded to 16
+  __shared__ float red[kLdThreads / 32][kMaxCaseParams];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int b = blockIdx.x;
+  const int nin = 5 + p;
+  if (tid < kC) {
+    wu[tid] = fc0_w[tid * nin];
+    wv[tid] = fc0_w[tid * nin + 1];
+  }
+  for (int e = tid; e < kC * kMaxCaseParams; e += kLdThreads) {
+    const int o = e / kMaxCaseParams, j = e % kMaxCaseParams;
+    wp[o][j] = j < p ? fc0_w[o * nin + 5 + j] : 0.f;
+  }
+  __syncthreads();
+
+  const float4* d = reinterpret_cast<const float4*>(da0 + static_cast<size_t>(b) * kC * kHW);
+  const bool want_p = d_params != nullptr;
+  float4 du[kLdVec], dv[kLdVec];
+  float cp[kMaxCaseParams];
+#pragma unroll
+  for (int k = 0; k < kLdVec; ++k) du[k] = dv[k] = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+  for (int j = 0; j < kMaxCaseParams; ++j) cp[j] = 0.f;
+#pragma unroll 4
+  for (int o = 0; o < kC; ++o) {
+    const float a = wu[o], c = wv[o];
+    float s = 0.f;   // this thread's share of the plane sum of channel o
+#pragma unroll
+    for (int k = 0; k < kLdVec; ++k) {
+      const float4 x = __ldcs(d + o * (kHW / 4) + k * kLdThreads + tid);   // last use of d_a0: stream through L2
+      du[k].x = fmaf(a, x.x, du[k].x); du[k].y = fmaf(a, x.y, du[k].y);
+      du[k].z = fmaf(a, x.z, du[k].z); du[k].w = fmaf(a, x.w, du[k].w);
+      dv[k].x = fmaf(c, x.x, dv[k].x); dv[k].y = fmaf(c, x.y, dv[k].y);
+      dv[k].z = fmaf(c, x.z, dv[k].z); dv[k].w = fmaf(c, x.w, dv[k].w);
+      s += (x.x + x.y) + (x.z + x.w);
+    }
+    if (want_p) {
+      const float4* wrow = reinterpret_cast<const float4*>(&wp[o][0]);
+#pragma unroll
+      for (int q = 0; q < kMaxCaseParams / 4; ++q) {
+        const float4 t = wrow[q];
+        cp[4 * q] = fmaf(t.x, s, cp[4 * q]);
+        cp[4 * q + 1] = fmaf(t.y, s, cp[4 * q + 1]);
+        cp[4 * q + 2] = fmaf(t.z, s, cp[4 * q + 2]);
+        cp[4 * q + 3] = fmaf(t.w, s, cp[4 * q + 3]);
+      }
+    }
+  }
+  if (d_inputs != nullptr) {
+    float4* u_out = reinterpret_cast<float4*>(d_inputs + static_cast<size_t>(b) * 2 * kHW);
+    float4* v_out = u_out + kHW / 4;
+#pragma unroll
+    for (int k = 0; k < kLdVec; ++k) {
+      u_out[k * kLdThreads + tid] = du[k];
+      v_out[k * kLdThreads + tid] = dv[k];
+    }
+  }
+  if (want_p) {
+#pragma unroll
+    for (int j = 0; j < kMaxCaseParams; ++j) {
+      if (j < p) {
+        const float r = warp_sum(cp[j]);
+        if (lane == 0) red[warp][j] = r;
+      }
+    }
+    __syncthreads();
+    if (tid < p) {
+      float t = 0.f;
+      for (int w = 0; w < kLdThreads / 32; ++w) t += red[w][tid];   // warp order: fixed
+      d_params[static_cast<size_t>(b) * p + tid] = t;
+    }
+  }
+}
+
+cudaError_t launch_lift_bwd_data(const float* da0, const float* fc0_w, float* d_inputs, float* d_params, int batch, int p,
+                                 cudaStream_t stream) {
+  if (p < 0 || p > kMaxCaseParams) return cudaErrorInvalidValue;
+  if (p == 0) d_params = nullptr;
+  if (d_inputs == nullptr && d_params == nullptr) return cudaSuccess;
+  lift_bwd_data_kernel<<<batch, kLdThreads, 0, stream>>>(da0, fc0_w, d_inputs, d_params, p);
   return cudaGetLastError();
 }
 

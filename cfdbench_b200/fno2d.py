@@ -12,6 +12,8 @@ Extras that the reference does not have (all optional, defaults keep reference b
   * `generate_many(..)` runs the whole rollout in one native call; host tensors in -> host tensors out
     through `fno_rollout_host` (H2D + rollout + D2H on one stream).
   * `enable_data_parallel()`: all-reduce of one flat gradient buffer (NCCL) inside backward.
+Like the reference, `forward` / `generate` are differentiable w.r.t. `inputs` and `case_params` (not `mask`), also with
+every parameter frozen.
 """
 from __future__ import annotations
 
@@ -70,15 +72,17 @@ def _ptr(t: Optional[Tensor]) -> int:
 
 
 class _TrainFn(torch.autograd.Function):
-    """One autograd node for the whole network: forward = fno_forward_train, backward = fno_backward."""
+    """One autograd node for the whole network: forward = fno_forward_train, backward = fno_backward (parameter
+    gradients only) or fno_backward_inputs (also, or only, the gradients w.r.t. inputs / case_params).  Every call keeps
+    its own saved activations, so forward k+1 may run before backward k (unrolled training through rollouts)."""
 
     @staticmethod
     def forward(ctx, model: "Fno2d", inputs: Tensor, mask: Tensor, case_params: Tensor, *params: Tensor):
-        if inputs.requires_grad or case_params.requires_grad or mask.requires_grad:
-            # the reference propagates dL/dinputs; nothing on the hot path (train_auto.py) asks for it, so the native
-            # backward stops at the lift weights -- say so instead of silently returning None
-            raise NotImplementedError("cfdbench_b200.Fno2d: gradients w.r.t. inputs / case_params / mask are not "
-                                      "implemented (only parameter gradients are; reference train_auto.py:255)")
+        if mask.requires_grad:
+            # the masked projection keeps no unmasked output, so dL/dmask cannot be formed -- say so instead of
+            # silently returning None
+            raise NotImplementedError("cfdbench_b200.Fno2d: gradients w.r.t. the mask are not implemented (inputs, "
+                                      "case_params and parameters are differentiable)")
         preds, saved = model._native_forward_train(inputs, mask, case_params)
         ctx.model = model
         ctx.saved_native = saved
@@ -92,9 +96,15 @@ class _TrainFn(torch.autograd.Function):
         if ctx.saved_native is None:
             raise RuntimeError("cfdbench_b200.Fno2d: backward through the same forward a second time (the saved native "
                                "activations were released after the first backward; run forward again)")
-        grads = model._native_backward(inputs, mask, case_params, dpreds.contiguous().float(), ctx.saved_native)
+        need = ctx.needs_input_grad   # (model, inputs, mask, case_params, *params)
+        d_inputs = torch.empty_like(inputs) if need[1] else None
+        d_cp = torch.empty_like(case_params) if need[3] else None
+        grads = model._native_backward(inputs, mask, case_params, dpreds.contiguous().float(), ctx.saved_native,
+                                       any(need[4:]), d_inputs, d_cp)
         ctx.saved_native = None   # the saved activations (up to 1.2 GB at B=256) are released with the first backward
-        return (None, None, None, None, *grads)
+        if grads is None:
+            grads = [None] * (len(need) - 4)
+        return (None, d_inputs, None, d_cp, *grads)
 
 
 class Fno2d(AutoCfdModel):
@@ -355,27 +365,39 @@ class Fno2d(AutoCfdModel):
             off += n
         return out, off
 
-    def _native_backward(self, inputs, mask4, case_params, dpreds, saved_native):
+    def _native_backward(self, inputs, mask4, case_params, dpreds, saved_native, want_params: bool = True,
+                         d_inputs: Optional[Tensor] = None, d_cp: Optional[Tensor] = None):
+        """Parameter gradients in parameter order (None when `want_params` is false).  Without `d_inputs` / `d_cp` this is
+        fno_backward / fno_backward_ex, the training step of train_auto.py; otherwise fno_backward_inputs also writes
+        dL/dinputs into `d_inputs` and dL/dcase_params into `d_cp`.  Those are per sample: with data parallel enabled
+        only the parameter gradients are all-reduced."""
+        if self.n_case_params == 0:
+            d_cp = None   # a (B, 0) gradient: nothing to write
+        with_data = d_inputs is not None or d_cp is not None
+        if not want_params and not with_data:
+            return None
         lib = _lib.load()
         sv, acts, pres, xms = saved_native
         b, L, dev = inputs.shape[0], self.num_layers, self.device
         pk = self._pack(need_bwd=True)
         ws, _ = self._workspace(b)
         layout, total = self._grad_layout()
-        flat = torch.empty(total, dtype=torch.float32, device=dev)
-        views: Dict[str, Tensor] = {}
-        for name, p, off, n in layout:
-            seg = flat[off:off + n]
-            views[name] = torch.view_as_complex(seg.view(*p.shape, 2)) if p.is_complex() else seg.view(p.shape)
-        g = _lib.FnoGrads()
-        g.fc0_w, g.fc0_b = views["fc0.weight"].data_ptr(), views["fc0.bias"].data_ptr()
-        for l in range(L):
-            g.spec_w1[l] = views[f"blocks.{l}.conv0.weights1"].data_ptr()
-            g.spec_w2[l] = views[f"blocks.{l}.conv0.weights2"].data_ptr()
-            g.w0_w[l] = views[f"blocks.{l}.w0.weight"].data_ptr()
-            g.w0_b[l] = views[f"blocks.{l}.w0.bias"].data_ptr()
-        g.fc1_w, g.fc1_b = views["fc1.weight"].data_ptr(), views["fc1.bias"].data_ptr()
-        g.fc2_w, g.fc2_b = views["fc2.weight"].data_ptr(), views["fc2.bias"].data_ptr()
+        g = None
+        if want_params:
+            flat = torch.empty(total, dtype=torch.float32, device=dev)
+            views: Dict[str, Tensor] = {}
+            for name, p, off, n in layout:
+                seg = flat[off:off + n]
+                views[name] = torch.view_as_complex(seg.view(*p.shape, 2)) if p.is_complex() else seg.view(p.shape)
+            g = _lib.FnoGrads()
+            g.fc0_w, g.fc0_b = views["fc0.weight"].data_ptr(), views["fc0.bias"].data_ptr()
+            for l in range(L):
+                g.spec_w1[l] = views[f"blocks.{l}.conv0.weights1"].data_ptr()
+                g.spec_w2[l] = views[f"blocks.{l}.conv0.weights2"].data_ptr()
+                g.w0_w[l] = views[f"blocks.{l}.w0.weight"].data_ptr()
+                g.w0_b[l] = views[f"blocks.{l}.w0.bias"].data_ptr()
+            g.fc1_w, g.fc1_b = views["fc1.weight"].data_ptr(), views["fc1.bias"].data_ptr()
+            g.fc2_w, g.fc2_b = views["fc2.weight"].data_ptr(), views["fc2.bias"].data_ptr()
         d0 = torch.empty(b, HIDDEN, H, W, dtype=torch.float32, device=dev)
         d1 = torch.empty(b, HIDDEN, H, W, dtype=torch.float32, device=dev)
         dz1 = torch.empty(min(b, _lib.BWD_CHUNK), PROJ, H, W, dtype=torch.float32, device=dev)
@@ -386,11 +408,30 @@ class Fno2d(AutoCfdModel):
         sc.dz1, sc.gm, sc.gwk = dz1.data_ptr(), gm.data_ptr(), gwk.data_ptr()
         partials = torch.empty(lib.fno_bwd_partials_bytes(), dtype=torch.uint8, device=dev)
         sc.partials = partials.data_ptr()
+
+        def run(events=None):
+            if with_data:
+                _lib.check(lib.fno_backward_inputs(C.byref(pk["struct"]), C.byref(pk["struct_bwd"]), inputs.data_ptr(),
+                                                   mask4.data_ptr(), case_params.data_ptr(), dpreds.data_ptr(),
+                                                   C.byref(sv), C.byref(g) if g is not None else None, C.byref(sc),
+                                                   C.byref(ws), _ptr(d_inputs), _ptr(d_cp), b, self._act_code(),
+                                                   self._stream(), events), "fno_backward_inputs")
+            elif events is None:
+                _lib.check(lib.fno_backward(C.byref(pk["struct"]), C.byref(pk["struct_bwd"]), inputs.data_ptr(),
+                                            mask4.data_ptr(), case_params.data_ptr(), dpreds.data_ptr(), C.byref(sv),
+                                            C.byref(g), C.byref(sc), C.byref(ws), b, self._act_code(), self._stream()),
+                           "fno_backward")
+            else:
+                _lib.check(lib.fno_backward_ex(C.byref(pk["struct"]), C.byref(pk["struct_bwd"]), inputs.data_ptr(),
+                                               mask4.data_ptr(), case_params.data_ptr(), dpreds.data_ptr(), C.byref(sv),
+                                               C.byref(g), C.byref(sc), C.byref(ws), b, self._act_code(), self._stream(),
+                                               events), "fno_backward_ex")
+
+        if not want_params:   # data-only backward: no parameter gradients, nothing to all-reduce
+            run()
+            return None
         if not self._dp_enabled or self.dp_segments == "one":
-            _lib.check(lib.fno_backward(C.byref(pk["struct"]), C.byref(pk["struct_bwd"]), inputs.data_ptr(),
-                                        mask4.data_ptr(), case_params.data_ptr(), dpreds.data_ptr(), C.byref(sv),
-                                        C.byref(g), C.byref(sc), C.byref(ws), b, self._act_code(), self._stream()),
-                       "fno_backward")
+            run()
             if self._dp_enabled:   # one all-reduce (NCCL: ReduceOp.AVG, no division kernel) of the whole flat buffer
                 from .dp import allreduce_mean_
                 allreduce_mean_(flat, self._dp_group)
@@ -424,10 +465,7 @@ class Fno2d(AutoCfdModel):
                 ev.record()   # creates the underlying cudaEvent_t
         handles = (C.c_void_p * (L + 2))(*[ev.cuda_event for ev in self._dp_events])
         main = torch.cuda.current_stream(dev)
-        _lib.check(lib.fno_backward_ex(C.byref(pk["struct"]), C.byref(pk["struct_bwd"]), inputs.data_ptr(),
-                                       mask4.data_ptr(), case_params.data_ptr(), dpreds.data_ptr(), C.byref(sv),
-                                       C.byref(g), C.byref(sc), C.byref(ws), b, self._act_code(), self._stream(), handles),
-                   "fno_backward_ex")
+        run(handles)
         works = []
         flat.record_stream(self._dp_stream)
         with torch.cuda.stream(self._dp_stream):
@@ -452,10 +490,13 @@ class Fno2d(AutoCfdModel):
     def forward(self, inputs: Tensor, case_params: Tensor, mask: Optional[Tensor] = None,
                 label: Optional[Tensor] = None) -> Dict:
         """Same contract as reference fno2d.py:178-242: returns {"preds": (B,2,H,W) float32 masked}
-        plus {"loss": dict} when `label` is given."""
+        plus {"loss": dict} when `label` is given.  With grad mode on, `preds` is differentiable w.r.t. the parameters,
+        `inputs` and `case_params` (whichever require grad; `mask` does not take gradients), so a frozen model still
+        gives d(preds)/d(inputs) and `generate` can be chained for unrolled training."""
         self._require_cuda()
         inputs, case_params, mask4 = self._prep_inputs(inputs, case_params, mask)
-        needs_grad = torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters())
+        needs_grad = torch.is_grad_enabled() and (inputs.requires_grad or case_params.requires_grad or mask4.requires_grad
+                                                  or any(p.requires_grad for p in self.parameters()))
         with torch.cuda.device(self.device):
             if needs_grad:
                 preds = _TrainFn.apply(self, inputs, mask4, case_params, *self.parameters())
@@ -471,7 +512,8 @@ class Fno2d(AutoCfdModel):
 
     def generate_many(self, inputs: Tensor, case_params: Tensor, mask: Tensor, steps: int) -> List[Tensor]:
         """reference fno2d.py:269-295.  Returns a list of `steps` tensors (B,c,h,w); tensors live where
-        `inputs` lives (host tensors take the H2D -> rollout -> D2H path in one native call)."""
+        `inputs` lives (host tensors take the H2D -> rollout -> D2H path in one native call).  Always runs without
+        autograd (the graph-replayed inference rollout); to train through a rollout, chain `generate` calls."""
         self._require_cuda()
         assert len(inputs.shape) == len(case_params.shape) + 2
         if inputs.dim() == 3:

@@ -216,6 +216,22 @@ int fno_backward_ex(const fno_weights* w, const fno_weights_bwd* wb, const float
                  const float* case_params, const float* dpreds, const fno_train_saved* saved,
                  const fno_grads* grads, const fno_bwd_scratch* scratch, const fno_workspace* ws, int batch,
                  int act_dtype, void* stream, void* const* seg_events);
+/* Same backward, also differentiating w.r.t. the input frame and the case parameters (unrolled training through
+ * rollouts, sensitivities / inverse problems with a frozen model; what autograd gives the reference when `inputs` or
+ * `case_params` require grad, fno2d.py:195-217):
+ *   d_inputs[b][c][h][w] = sum_o fc0_w[o][c] dL/da0[b][o][h][w]               c = 0 (u), 1 (v)
+ *   d_case_params[b][j]  = sum_o fc0_w[o][5+j] sum_{h,w} dL/da0[b][o][h][w]
+ * where a0 is the lift output (a bf16-stored a0 is differentiated straight through).  Both are overwritten and
+ * bit-reproducible (fixed-order reductions, no atomics).  grads = NULL skips every parameter-gradient launch (data-only
+ * backward, e.g. a frozen model); otherwise `grads` and `seg_events` are filled / recorded as by fno_backward_ex.
+ * At least one of grads, d_inputs, d_case_params must be non-NULL; d_inputs must be 16-byte aligned. */
+int fno_backward_inputs(const fno_weights* w, const fno_weights_bwd* wb, const float* inputs, const float* mask,
+                        const float* case_params, const float* dpreds, const fno_train_saved* saved,
+                        const fno_grads* grads,        /* NULL: no parameter gradients (data-only backward) */
+                        const fno_bwd_scratch* scratch, const fno_workspace* ws,
+                        float* d_inputs,               /* [B][2][64][64] or NULL */
+                        float* d_case_params,          /* [B][p] or NULL (must be NULL or unused when p == 0) */
+                        int batch, int act_dtype, void* stream, void* const* seg_events);
 
 /* Rollout evaluation on the device (SURVEY.md 8f.1; reference src/test_multistep.py:73-83,153-177 get_metrics on the
  * masked u channel, three .item() syncs per step and case there).  preds_seq [S][B][2][64][64], label_u and mask
