@@ -133,7 +133,26 @@ SIGNATURES = {
     "fno_backward_inputs": (C.c_int, [C.POINTER(FnoWeights), C.POINTER(FnoWeightsBwd), _P, _P, _P, _P,
                                       C.POINTER(FnoTrainSaved), C.POINTER(FnoGrads), C.POINTER(FnoBwdScratch),
                                       C.POINTER(FnoWorkspace), _P, _P, _I, _I, _P, C.POINTER(C.c_void_p)]),
+    # grid-generic fp32 path (H, W in 24..128)
+    "fno_grid_act_bytes": (C.c_size_t, [_I, _I, _I]),
+    "fno_grid_z_bytes": (C.c_size_t, [_I, _I]),
+    "fno_grid_bwd_partials_bytes": (C.c_size_t, [_I, _I]),
+    "fno_grid_lift_fwd": (C.c_int, [_P, _P, _P, C.POINTER(FnoWeights), _P, _I, _I, _I, _P]),
+    "fno_grid_spectral_dft_fwd": (C.c_int, [_P, _P, _I, _I, _I, _F, _F, _P]),
+    "fno_grid_spectral_inv_kx": (C.c_int, [_P, _P, _I, _I, _I, _F, _F, _P]),
+    "fno_grid_block_out": (C.c_int, [_I, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _P]),
+    "fno_grid_project_fwd": (C.c_int, [_P, _P, C.POINTER(FnoWeights), _P, _I, _I, _I, _P]),
+    "fno_grid_project_bwd": (C.c_int, [_P, _P, _P, _P, C.POINTER(FnoWeights), _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _P]),
+    "fno_grid_forward": (C.c_int, [C.POINTER(FnoWeights), _P, _P, _P, _P, C.POINTER(FnoWorkspace), _I, _I, _I, _P]),
+    "fno_grid_rollout": (C.c_int, [C.POINTER(FnoWeights), _P, _P, _P, _P, _I, C.POINTER(FnoWorkspace), _I, _I, _I, _P]),
+    "fno_grid_forward_train": (C.c_int, [C.POINTER(FnoWeights), _P, _P, _P, _P, C.POINTER(FnoTrainSaved),
+                                         C.POINTER(FnoWorkspace), _I, _I, _I, _P]),
+    "fno_grid_backward": (C.c_int, [C.POINTER(FnoWeights), C.POINTER(FnoWeightsBwd), _P, _P, _P, _P,
+                                    C.POINTER(FnoTrainSaved), C.POINTER(FnoGrads), C.POINTER(FnoBwdScratch),
+                                    C.POINTER(FnoWorkspace), _P, _P, _I, _I, _I, _P, C.POINTER(C.c_void_p)]),
 }
+
+GRID_MIN, GRID_MAX = 24, 128
 
 _lib = None
 

@@ -18,7 +18,7 @@ CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libcfdbench_b200.so")
 STAMP = os.path.join(HERE, ".build_stamp")
 SOURCES = ["fno_abi.cu", "fno_dft_fwd.cu", "fno_dft_fwd_tc.cu", "fno_mode_mix.cu", "fno_block_tc.cu", "fno_block_fused.cu", "fno_pointwise.cu", "fno_project_tc.cu", "fno_project_bwd_tc.cu",
-           "fno_backward.cu", "fno_metrics.cu", "fno_train_step.cu"]
+           "fno_backward.cu", "fno_metrics.cu", "fno_train_step.cu", "fno_grid.cu"]
 NVCC_FLAGS = ["-std=c++17", "-O3", "-lineinfo", "-gencode", "arch=compute_90a,code=sm_90a",
               "-Xcompiler", "-fPIC"]
 

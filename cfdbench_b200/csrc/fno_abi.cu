@@ -50,6 +50,30 @@ cudaError_t launch_spectral_wgrad(const void*, const void*, void*, int, cudaStre
 cudaError_t launch_lift_bwd(const float*, const float*, const float*, const float*, const float*, const float*,
                             float*, float*, float*, int, int, cudaStream_t);
 cudaError_t launch_lift_bwd_data(const float*, const float*, float*, float*, int, int, cudaStream_t);
+// grid-generic fp32 path (fno_grid.cu)
+bool grid_ok(int, int);
+void grid_tables_release(int);
+cudaError_t launch_grid_lift(const float*, const float*, const float*, const float*, const float*, const float*,
+                             const float*, float*, int, int, int, int, cudaStream_t);
+cudaError_t launch_grid_dft(const float*, void*, int, int, int, float, float, cudaStream_t);
+cudaError_t launch_grid_inv_kx(const void*, float*, int, int, int, float, float, cudaStream_t);
+cudaError_t launch_grid_block_out(int, const float*, const float*, const float*, const float*, float*, float*, const float*,
+                                  int, int, int, cudaStream_t);
+cudaError_t launch_grid_project(const float*, const float*, const float*, const float*, const float*, const float*, float*,
+                                int, int, cudaStream_t);
+cudaError_t launch_grid_project_bwd(const float*, const float*, const float*, const float*, const float*, const float*,
+                                    const float*, float*, float*, float*, int, int, cudaStream_t);
+int grid_project_bwd_parts(int, int);
+int grid_project_bwd_row();
+template <int NJ, int NI>
+cudaError_t launch_grid_chan_outer(const float*, const float*, float*, int*, int, int, cudaStream_t);
+cudaError_t launch_grid_lift_bwd(const float*, const float*, const float*, const float*, const float*, const float*,
+                                 const float*, float*, float*, float*, int, int, int, int, cudaStream_t);
+int grid_lift_bwd_parts(int);
+int grid_lift_bwd_row();
+size_t grid_bwd_partials_floats();
+size_t grid_partials_offset_co();
+size_t grid_partials_offset_lb();
 }  // namespace fno
 
 using namespace fno;
@@ -96,6 +120,7 @@ int fno_destroy(void) {
   block_tc_release(dev);
   block_fused_release(dev);
   dft_fwd_tc_release(dev);
+  grid_tables_release(dev);
   for (int k = 0; k < 2; ++k)
     for (int c = 0; c < 16; ++c)
       if (g_chunk_events[dev][k][c]) {
@@ -551,6 +576,233 @@ int fno_adam_step(const fno_adam_tensors* t, float lr, float beta1, float beta2,
     if (!t->param[i] || !t->grad[i] || !t->exp_avg[i] || !t->exp_avg_sq[i] || t->n[i] <= 0)
       return fail(kErrArg, "fno_adam_step: null tensor or empty size");
   FNO_CUDA(launch_adam_step(t, lr, beta1, beta2, eps, weight_decay, step, S(stream)), "adam_step_kernel");
+  return kOk;
+}
+
+// ------------------------------------------------------------------------------------------------ grid-generic fp32 path
+static int grid_arg(const char* what, int h, int w) {
+  char msg[160];
+  if (!grid_ok(h, w)) {
+    snprintf(msg, sizeof(msg), "%s: grid %dx%d outside the supported range 24..128 x 24..128", what, h, w);
+    return fail(kErrUnsupported, msg);
+  }
+  return kOk;
+}
+
+size_t fno_grid_act_bytes(int batch, int h, int w) {
+  return static_cast<size_t>(batch) * kC * h * w * sizeof(float);
+}
+size_t fno_grid_z_bytes(int batch, int h) { return static_cast<size_t>(batch) * h * 2 * kM2 * kC * sizeof(float); }
+size_t fno_grid_bwd_partials_bytes(int h, int w) {
+  (void)h;
+  (void)w;   // the partial rows come from a fixed number of CTAs: the size does not depend on the grid
+  return grid_bwd_partials_floats() * sizeof(float);
+}
+
+int fno_grid_lift_fwd(const float* inputs, const float* mask, const float* case_params, const fno_weights* w,
+                      float* act_out, int batch, int h, int wd, void* stream) {
+  FNO_TRY(grid_arg("fno_grid_lift_fwd", h, wd));
+  if (!inputs || !mask || !w || !act_out || batch <= 0 || !w->gx || !w->gy) return fail(kErrArg, "fno_grid_lift_fwd: bad argument");
+  if (w->n_case_params > 0 && !case_params) return fail(kErrArg, "fno_grid_lift_fwd: case_params is null");
+  FNO_CUDA(launch_grid_lift(inputs, mask, case_params, w->fc0_w, w->fc0_b, w->gx, w->gy, act_out, batch, w->n_case_params, h,
+                            wd, S(stream)),
+           "grid_lift_kernel");
+  return kOk;
+}
+
+int fno_grid_spectral_dft_fwd(const float* act_in, void* xm, int batch, int h, int wd, float s0, float s1, void* stream) {
+  FNO_TRY(grid_arg("fno_grid_spectral_dft_fwd", h, wd));
+  if (!act_in || !xm || batch <= 0) return fail(kErrArg, "fno_grid_spectral_dft_fwd: bad argument");
+  FNO_CUDA(launch_grid_dft(act_in, xm, batch, h, wd, s0, s1, S(stream)), "grid_dft_kernel");
+  return kOk;
+}
+
+int fno_grid_spectral_inv_kx(const void* ym, float* z, int batch, int h, int wd, float s0, float s1, void* stream) {
+  FNO_TRY(grid_arg("fno_grid_spectral_inv_kx", h, wd));
+  if (!ym || !z || batch <= 0) return fail(kErrArg, "fno_grid_spectral_inv_kx: bad argument");
+  FNO_CUDA(launch_grid_inv_kx(ym, z, batch, h, wd, s0, s1, S(stream)), "grid_inv_kx_kernel");
+  return kOk;
+}
+
+int fno_grid_block_out(int epilogue, const float* z, const float* act_in, const float* w0t, const float* bias, float* act_out,
+                       float* pre_out, const float* pre_in, int batch, int h, int wd, void* stream) {
+  FNO_TRY(grid_arg("fno_grid_block_out", h, wd));
+  if (!z || !act_in || !w0t || !act_out || batch <= 0 || epilogue < FNO_EPI_GELU || epilogue > FNO_EPI_PLAIN)
+    return fail(kErrArg, "fno_grid_block_out: bad argument");
+  if (epilogue == FNO_EPI_GELU_SAVE_PRE && !pre_out) return fail(kErrArg, "fno_grid_block_out: pre_out is null");
+  if (epilogue == FNO_EPI_MUL_DGELU && !pre_in) return fail(kErrArg, "fno_grid_block_out: pre_in is null");
+  FNO_CUDA(launch_grid_block_out(epilogue, z, act_in, w0t, bias, act_out, pre_out, pre_in, batch, h, wd, S(stream)),
+           "grid_block_out_kernel");
+  return kOk;
+}
+
+int fno_grid_project_fwd(const float* act_in, const float* mask, const fno_weights* w, float* preds, int batch, int h, int wd,
+                         void* stream) {
+  FNO_TRY(grid_arg("fno_grid_project_fwd", h, wd));
+  if (!act_in || !mask || !w || !preds || batch <= 0) return fail(kErrArg, "fno_grid_project_fwd: bad argument");
+  FNO_CUDA(launch_grid_project(act_in, w->fc1_w, w->fc1_b, w->fc2_w, w->fc2_b, mask, preds, batch, h * wd, S(stream)),
+           "grid_project_kernel");
+  return kOk;
+}
+
+// project backward over batch chunks of FNO_BWD_CHUNK (dz1 holds one chunk); gradients written when g_fc1_w is set
+static int grid_project_bwd_impl(const float* act, const float* dpreds, const float* mask, const float* pre,
+                                 const fno_weights* w, float* dpre_out, float* dz1, float* partials, float* g_fc1_w,
+                                 float* g_fc1_b, float* g_fc2_w, float* g_fc2_b, int batch, int h, int wd, cudaStream_t st) {
+  const int hw = h * wd;
+  float* part_pb = partials;
+  float* part_co = partials + grid_partials_offset_co();
+  const bool grads = g_fc1_w != nullptr;
+  for (int b0 = 0; b0 < batch; b0 += FNO_BWD_CHUNK) {
+    const int nb = (batch - b0 < FNO_BWD_CHUNK) ? batch - b0 : FNO_BWD_CHUNK;
+    const size_t act_off = static_cast<size_t>(b0) * kC * hw;
+    FNO_CUDA(launch_grid_project_bwd(act + act_off, dpreds + static_cast<size_t>(b0) * 2 * hw, mask + static_cast<size_t>(b0) * hw,
+                                     pre + act_off, w->fc1_w, w->fc1_b, w->fc2_w, dpre_out + act_off, dz1,
+                                     grads ? part_pb : nullptr, nb, hw, st),
+             "grid_project_bwd_kernel");
+    if (!grads) continue;
+    const int accum = b0 > 0 ? 1 : 0;
+    FNO_CUDA(launch_reduce_partials(part_pb, grid_project_bwd_parts(nb, hw), grid_project_bwd_row(), g_fc2_w, 2 * kProj,
+                                    g_fc1_b, kProj, g_fc2_b, 2, accum, st),
+             "reduce(fc2.weight | fc1.bias | fc2.bias)");
+    int n_co = 0;
+    FNO_CUDA((launch_grid_chan_outer<kProj, kC>(dz1, act + act_off, part_co, &n_co, nb, hw, st)), "grid_chan_outer_kernel(fc1)");
+    FNO_CUDA(launch_reduce_partials(part_co, n_co, kProj * kC + kProj, g_fc1_w, kProj * kC, nullptr, 0, nullptr, 0, accum, st),
+             "reduce(fc1.weight)");
+  }
+  return kOk;
+}
+
+int fno_grid_project_bwd(const float* act_in, const float* dpreds, const float* mask, const float* pre, const fno_weights* w,
+                         float* dpre_out, float* dz1, float* partials, float* g_fc1_w, float* g_fc1_b, float* g_fc2_w,
+                         float* g_fc2_b, int batch, int h, int wd, void* stream) {
+  FNO_TRY(grid_arg("fno_grid_project_bwd", h, wd));
+  if (!act_in || !dpreds || !mask || !pre || !w || !dpre_out || !dz1 || !partials || batch <= 0)
+    return fail(kErrArg, "fno_grid_project_bwd: bad argument");
+  const bool any = g_fc1_w || g_fc1_b || g_fc2_w || g_fc2_b, all = g_fc1_w && g_fc1_b && g_fc2_w && g_fc2_b;
+  if (any && !all) return fail(kErrArg, "fno_grid_project_bwd: pass all four gradient pointers or none");
+  return grid_project_bwd_impl(act_in, dpreds, mask, pre, w, dpre_out, dz1, partials, g_fc1_w, g_fc1_b, g_fc2_w, g_fc2_b,
+                               batch, h, wd, S(stream));
+}
+
+static int grid_block(const fno_weights* w, int l, const float* act_in, float* act_out, float* pre_out, void* xm,
+                      const fno_workspace* ws, int batch, int h, int wd, void* stream) {
+  const float inv = 1.f / static_cast<float>(h * wd);
+  FNO_TRY(fno_grid_spectral_dft_fwd(act_in, xm, batch, h, wd, 1.f, 1.f, stream));
+  FNO_TRY(fno_mode_mix(xm, w->spec_wk[l], ws->ym, batch, stream));
+  FNO_TRY(fno_grid_spectral_inv_kx(ws->ym, static_cast<float*>(ws->z), batch, h, wd, inv, 2.f * inv, stream));
+  return fno_grid_block_out(pre_out ? FNO_EPI_GELU_SAVE_PRE : FNO_EPI_GELU, static_cast<const float*>(ws->z), act_in,
+                            w->w0t[l], w->w0_b[l], act_out, pre_out, nullptr, batch, h, wd, stream);
+}
+
+int fno_grid_forward(const fno_weights* w, const float* inputs, const float* mask, const float* case_params, float* preds,
+                     const fno_workspace* ws, int batch, int h, int wd, void* stream) {
+  FNO_TRY(grid_arg("fno_grid_forward", h, wd));
+  if (!w || !ws || !ws->act[0] || !ws->act[1] || !ws->xm || !ws->ym || !ws->z) return fail(kErrArg, "fno_grid_forward: bad workspace");
+  if (w->n_layers < 1 || w->n_layers > FNO_MAX_LAYERS) return fail(kErrUnsupported, "fno_grid_forward: n_layers out of range");
+  float* act[2] = {static_cast<float*>(ws->act[0]), static_cast<float*>(ws->act[1])};
+  FNO_TRY(fno_grid_lift_fwd(inputs, mask, case_params, w, act[0], batch, h, wd, stream));
+  int cur = 0;
+  for (int l = 0; l < w->n_layers; ++l) {
+    FNO_TRY(grid_block(w, l, act[cur], act[cur ^ 1], nullptr, ws->xm, ws, batch, h, wd, stream));
+    cur ^= 1;
+  }
+  return fno_grid_project_fwd(act[cur], mask, w, preds, batch, h, wd, stream);
+}
+
+int fno_grid_rollout(const fno_weights* w, const float* inputs, const float* mask, const float* case_params, float* preds_seq,
+                     int steps, const fno_workspace* ws, int batch, int h, int wd, void* stream) {
+  FNO_TRY(grid_arg("fno_grid_rollout", h, wd));
+  if (steps < 0 || !preds_seq || batch <= 0) return fail(kErrArg, "fno_grid_rollout: bad argument");
+  const size_t frame = static_cast<size_t>(batch) * 2 * h * wd;
+  const float* cur = inputs;
+  for (int s = 0; s < steps; ++s) {
+    float* nxt = preds_seq + static_cast<size_t>(s) * frame;
+    FNO_TRY(fno_grid_forward(w, cur, mask, case_params, nxt, ws, batch, h, wd, stream));
+    cur = nxt;
+  }
+  return kOk;
+}
+
+int fno_grid_forward_train(const fno_weights* w, const float* inputs, const float* mask, const float* case_params,
+                           float* preds, const fno_train_saved* saved, const fno_workspace* ws, int batch, int h, int wd,
+                           void* stream) {
+  FNO_TRY(grid_arg("fno_grid_forward_train", h, wd));
+  if (!w || !saved || !ws || !ws->ym || !ws->z || !saved->act[0]) return fail(kErrArg, "fno_grid_forward_train: bad argument");
+  if (w->n_layers < 1 || w->n_layers > FNO_MAX_LAYERS) return fail(kErrUnsupported, "fno_grid_forward_train: n_layers");
+  FNO_TRY(fno_grid_lift_fwd(inputs, mask, case_params, w, static_cast<float*>(saved->act[0]), batch, h, wd, stream));
+  for (int l = 0; l < w->n_layers; ++l) {
+    if (!saved->act[l + 1] || !saved->pre[l] || !saved->xm[l])
+      return fail(kErrArg, "fno_grid_forward_train: null saved buffer");
+    FNO_TRY(grid_block(w, l, static_cast<const float*>(saved->act[l]), static_cast<float*>(saved->act[l + 1]), saved->pre[l],
+                       saved->xm[l], ws, batch, h, wd, stream));
+  }
+  return fno_grid_project_fwd(static_cast<const float*>(saved->act[w->n_layers]), mask, w, preds, batch, h, wd, stream);
+}
+
+int fno_grid_backward(const fno_weights* w, const fno_weights_bwd* wb, const float* inputs, const float* mask,
+                      const float* case_params, const float* dpreds, const fno_train_saved* saved, const fno_grads* g,
+                      const fno_bwd_scratch* sc, const fno_workspace* ws, float* d_inputs, float* d_case_params, int batch,
+                      int h, int wd, void* stream, void* const* seg_events) {
+  FNO_TRY(grid_arg("fno_grid_backward", h, wd));
+  if (!w || !wb || !inputs || !mask || !dpreds || !saved || !sc || !ws || batch <= 0)
+    return fail(kErrArg, "fno_grid_backward: bad argument");
+  if (w->n_layers < 1 || w->n_layers > FNO_MAX_LAYERS) return fail(kErrUnsupported, "fno_grid_backward: n_layers");
+  if (w->n_case_params < 0 || w->n_case_params > kMaxCaseParams)
+    return fail(kErrArg, "fno_grid_backward: n_case_params out of range");
+  if (w->n_case_params == 0) d_case_params = nullptr;   // nothing to write
+  if (!g && !d_inputs && !d_case_params) return fail(kErrArg, "fno_grid_backward: no output requested");
+  if (!sc->d[0] || !sc->d[1] || !sc->dz1 || !sc->gm || !sc->gwk || !sc->partials || !ws->ym || !ws->z)
+    return fail(kErrArg, "fno_grid_backward: null scratch buffer");
+  cudaStream_t st = S(stream);
+  const int L = w->n_layers, p = w->n_case_params;
+  auto mark = [&](int seg) -> cudaError_t {
+    if (seg_events == nullptr || seg_events[seg] == nullptr) return cudaSuccess;
+    return cudaEventRecord(static_cast<cudaEvent_t>(seg_events[seg]), st);
+  };
+  // ---- projection -> d[0] = dpre_{L-1}
+  FNO_TRY(grid_project_bwd_impl(static_cast<const float*>(saved->act[L]), dpreds, mask, saved->pre[L - 1], w, sc->d[0], sc->dz1,
+                                sc->partials, g ? g->fc1_w : nullptr, g ? g->fc1_b : nullptr, g ? g->fc2_w : nullptr,
+                                g ? g->fc2_b : nullptr, batch, h, wd, st));
+  FNO_CUDA(mark(0), "cudaEventRecord(fc1/fc2 gradients)");
+  // ---- Fourier blocks, last to first
+  float* part_co = sc->partials + grid_partials_offset_co();
+  const float inv = 1.f / static_cast<float>(h * wd);
+  int cur = 0;
+  for (int l = L - 1; l >= 0; --l) {
+    float* dpre = sc->d[cur];
+    float* dnext = sc->d[cur ^ 1];
+    const float* act_l = static_cast<const float*>(saved->act[l]);
+    if (g) {
+      int n_co = 0;
+      FNO_CUDA((launch_grid_chan_outer<kC, kC>(dpre, act_l, part_co, &n_co, batch, h * wd, st)), "grid_chan_outer_kernel(w0)");
+      FNO_CUDA(launch_reduce_partials(part_co, n_co, kC * kC + kC, g->w0_w[l], kC * kC, g->w0_b[l], kC, nullptr, 0, 0, st),
+               "reduce(w0.weight | w0.bias)");
+    }
+    FNO_TRY(fno_grid_spectral_dft_fwd(dpre, sc->gm, batch, h, wd, inv, 2.f * inv, stream));
+    if (g) {
+      FNO_CUDA(launch_spectral_wgrad(saved->xm[l], sc->gm, sc->gwk, batch, st), "spectral_wgrad_kernel");
+      FNO_TRY(fno_unpack_spectral_grads(sc->gwk, g->spec_w1[l], g->spec_w2[l], stream));
+    }
+    FNO_CUDA(mark(1 + (L - 1 - l)), "cudaEventRecord(block gradients)");
+    FNO_TRY(fno_mode_mix(sc->gm, wb->spec_wkT[l], ws->ym, batch, stream));
+    FNO_TRY(fno_grid_spectral_inv_kx(ws->ym, static_cast<float*>(ws->z), batch, h, wd, 1.f, 1.f, stream));
+    FNO_TRY(fno_grid_block_out(l > 0 ? FNO_EPI_MUL_DGELU : FNO_EPI_PLAIN, static_cast<const float*>(ws->z), dpre, wb->w0[l],
+                               nullptr, dnext, nullptr, l > 0 ? saved->pre[l - 1] : nullptr, batch, h, wd, stream));
+    cur ^= 1;
+  }
+  // ---- lift: fc0 gradients and the data adjoint of dL/da0 = d[cur]
+  float* part_lb = g ? sc->partials + grid_partials_offset_lb() : nullptr;
+  if (g || d_inputs || d_case_params) {
+    FNO_CUDA(launch_grid_lift_bwd(sc->d[cur], inputs, mask, case_params, w->gx, w->gy, w->fc0_w, part_lb, d_inputs,
+                                  d_case_params, batch, p, h, wd, st),
+             "grid_lift_bwd_kernel");
+  }
+  if (g)
+    FNO_CUDA(launch_reduce_partials(part_lb, grid_lift_bwd_parts(batch), grid_lift_bwd_row(), g->fc0_w, kC * (5 + p), g->fc0_b,
+                                    kC, nullptr, 0, 0, st),
+             "reduce(fc0.weight | fc0.bias)");
+  FNO_CUDA(mark(L + 1), "cudaEventRecord(fc0 gradients)");
   return kOk;
 }
 

@@ -1,8 +1,8 @@
 // Shared definitions for the sm_90a FNO kernels (cfdbench_b200).
 //
 // Problem constants are the reference's FNO configuration (reference src/args.py:99-103,187-197:
-// 64x64 grid, fno_hidden_dim=32, fno_modes_x=fno_modes_y=12); the Python wrapper rejects anything
-// else, there is no generic / CPU fallback.
+// 64x64 grid, fno_hidden_dim=32, fno_modes_x=fno_modes_y=12).  Other grids run the runtime-(H, W) kernels of
+// fno_grid.cu; the Python wrapper rejects anything else, there is no CPU fallback.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>

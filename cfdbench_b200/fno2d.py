@@ -12,6 +12,8 @@ Extras that the reference does not have (all optional, defaults keep reference b
   * `generate_many(..)` runs the whole rollout in one native call; host tensors in -> host tensors out
     through `fno_rollout_host` (H2D + rollout + D2H on one stream).
   * `enable_data_parallel()`: all-reduce of one flat gradient buffer (NCCL) inside backward.
+Frames: 64x64 runs the 64x64 kernels (either storage mode); any other H x W with 24 <= H, W <= 128 (CFDBench's tube
+and dam problems: 66x65) runs the grid-generic fp32 kernels (fno_grid_* in the C ABI), routed by `inputs.shape[-2:]`.
 Like the reference, `forward` / `generate` are differentiable w.r.t. `inputs` and `case_params` (not `mask`), also with
 every parameter frozen.
 """
@@ -183,6 +185,9 @@ class Fno2d(AutoCfdModel):
         self.host_zero_copy = False  # opt-in: lift reads the pinned frame, project writes the pinned result directly
         self.zero_copy_chunks = 2
         self._graphs: dict = {}
+        # True: 64x64 frames in float32 storage also run the grid-generic kernels (fno_grid_*), which cross-checks the two
+        # paths; False (default): 64x64 frames run the 64x64 kernels
+        self.generic_grid_at_64 = False
 
     # ------------------------------------------------------------------------------------ plumbing
     def invalidate_packed(self) -> None:
@@ -307,9 +312,25 @@ class Fno2d(AutoCfdModel):
             self._ws_cache[key] = ws
         return ws
 
+    def _check_grid(self, shape) -> tuple:
+        """(H, W) of an input frame: 64x64 runs the 64x64 kernels in either storage mode, any other grid with
+        24 <= H, W <= 128 the grid-generic fp32 kernels."""
+        gh, gw = int(shape[-2]), int(shape[-1])
+        if (gh, gw) == (H, W):
+            return gh, gw
+        if not (_lib.GRID_MIN <= gh <= _lib.GRID_MAX and _lib.GRID_MIN <= gw <= _lib.GRID_MAX):
+            raise ValueError(f"cfdbench_b200.Fno2d supports {H}x{W} frames and grids with {_lib.GRID_MIN} <= H, W <= "
+                             f"{_lib.GRID_MAX}; got {gh}x{gw}")
+        if self.act_dtype != "float32":
+            raise ValueError(f"cfdbench_b200.Fno2d: act_dtype={self.act_dtype!r} is supported on {H}x{W} frames only; "
+                             f"the {gh}x{gw} grid runs with act_dtype='float32'")
+        return gh, gw
+
     def _prep_inputs(self, inputs: Tensor, case_params: Tensor, mask: Optional[Tensor]):
-        if inputs.dim() != 4 or inputs.shape[1] != self.in_chan or tuple(inputs.shape[-2:]) != (H, W):
-            raise ValueError(f"inputs must be (B,{self.in_chan},{H},{W}); got {tuple(inputs.shape)}")
+        if inputs.dim() != 4 or inputs.shape[1] != self.in_chan:
+            raise ValueError(f"inputs must be (B,{self.in_chan},H,W); got {tuple(inputs.shape)}")
+        if tuple(inputs.shape[-2:]) != (H, W):
+            return self._prep_inputs_grid(inputs, case_params, mask)
         b = inputs.shape[0]
         dev = self.device
         inputs = inputs.to(device=dev, dtype=torch.float32, non_blocking=True).contiguous()
@@ -325,11 +346,81 @@ class Fno2d(AutoCfdModel):
             mask4 = mask4.to(device=dev, dtype=torch.float32, non_blocking=True).contiguous()
         return inputs, case_params, mask4
 
+    def _prep_inputs_grid(self, inputs: Tensor, case_params: Tensor, mask: Optional[Tensor]):
+        """_prep_inputs for a non-64x64 frame: the mask follows the input's grid."""
+        gh, gw = self._check_grid(inputs.shape)
+        b = inputs.shape[0]
+        dev = self.device
+        inputs = inputs.to(device=dev, dtype=torch.float32, non_blocking=True).contiguous()
+        if case_params.shape != (b, self.n_case_params):
+            raise ValueError(f"case_params must be ({b},{self.n_case_params}); got {tuple(case_params.shape)}")
+        case_params = case_params.to(device=dev, dtype=torch.float32, non_blocking=True).contiguous()
+        if mask is None:
+            mask4 = torch.ones((b, 1, gh, gw), device=dev)
+        else:
+            mask4 = mask.unsqueeze(1) if mask.dim() == 3 else mask
+            if tuple(mask4.shape) != (b, 1, gh, gw):
+                raise ValueError(f"mask must be (B,{gh},{gw}) or (B,1,{gh},{gw}); got {tuple(mask.shape)}")
+            mask4 = mask4.to(device=dev, dtype=torch.float32, non_blocking=True).contiguous()
+        return inputs, case_params, mask4
+
+    # ------------------------------------------------------------------------ grid-generic path
+    # Frames other than 64x64 (CFDBench's tube and dam problems: 66x65) run the grid-generic fp32 kernels
+    # (fno_grid_* in the C ABI).  Coordinate tables, workspaces and graphs are keyed by (H, W).
+    def _on_grid_path(self, gh: int, gw: int) -> bool:
+        if (gh, gw) != (H, W):
+            return True
+        if self.generic_grid_at_64 and self.act_dtype != "float32":
+            raise ValueError("generic_grid_at_64 needs act_dtype='float32'")
+        return self.generic_grid_at_64
+
+    def _grid_struct(self, pk: dict, gh: int, gw: int) -> "_lib.FnoWeights":
+        """The packed weight struct with the (gh, gw) coordinate tables (float32(np.linspace(0, 1, n)))."""
+        grids = pk.setdefault("grid", {})
+        ent = grids.get((gh, gw))
+        if ent is None:
+            gx = torch.tensor(np.linspace(0, 1, gh), dtype=torch.float).to(self.device)
+            gy = torch.tensor(np.linspace(0, 1, gw), dtype=torch.float).to(self.device)
+            st = _lib.FnoWeights.from_buffer_copy(pk["struct"])
+            st.gx, st.gy = gx.data_ptr(), gy.data_ptr()
+            ent = (st, gx, gy)
+            grids[(gh, gw)] = ent
+        return ent[0]
+
+    def _grid_workspace(self, batch: int, gh: int, gw: int):
+        key = ("grid", batch, gh, gw, self.device)
+        ws = self._ws_cache.get(key)
+        if ws is None:
+            dev = self.device
+            bufs = dict(
+                act0=torch.empty(batch, HIDDEN, gh, gw, dtype=torch.float32, device=dev),
+                act1=torch.empty(batch, HIDDEN, gh, gw, dtype=torch.float32, device=dev),
+                xm=torch.empty(NMODES, batch, HIDDEN, dtype=torch.complex64, device=dev),
+                ym=torch.empty(NMODES, batch, HIDDEN, dtype=torch.complex64, device=dev),
+                z=torch.empty(batch, gh, 2 * MODES, HIDDEN, dtype=torch.float32, device=dev),
+            )
+            st = _lib.FnoWorkspace()
+            st.act[0], st.act[1] = bufs["act0"].data_ptr(), bufs["act1"].data_ptr()
+            st.xm, st.ym, st.z = bufs["xm"].data_ptr(), bufs["ym"].data_ptr(), bufs["z"].data_ptr()
+            ws = (st, bufs)
+            if len(self._ws_cache) > 16:
+                self._ws_cache.clear()
+            self._ws_cache[key] = ws
+        return ws
+
     # ------------------------------------------------------------------------------ native calls
     def _native_forward(self, inputs: Tensor, mask4: Tensor, case_params: Tensor) -> Tensor:
         lib = _lib.load()
         b = inputs.shape[0]
         pk = self._pack()
+        gh, gw = inputs.shape[-2:]
+        if self._on_grid_path(gh, gw):
+            ws, _ = self._grid_workspace(b, gh, gw)
+            preds = torch.empty(b, self.out_chan, gh, gw, dtype=torch.float32, device=self.device)
+            _lib.check(lib.fno_grid_forward(C.byref(self._grid_struct(pk, gh, gw)), inputs.data_ptr(), mask4.data_ptr(),
+                                            case_params.data_ptr(), preds.data_ptr(), C.byref(ws), b, gh, gw,
+                                            self._stream()), "fno_grid_forward")
+            return preds
         ws, _ = self._workspace(b)
         preds = torch.empty(b, self.out_chan, H, W, dtype=torch.float32, device=self.device)
         _lib.check(lib.fno_forward(C.byref(pk["struct"]), inputs.data_ptr(), mask4.data_ptr(), case_params.data_ptr(),
@@ -340,6 +431,22 @@ class Fno2d(AutoCfdModel):
         lib = _lib.load()
         b, L, dev = inputs.shape[0], self.num_layers, self.device
         pk = self._pack(need_bwd=True)
+        gh, gw = inputs.shape[-2:]
+        if self._on_grid_path(gh, gw):
+            ws, _ = self._grid_workspace(b, gh, gw)
+            acts = [torch.empty(b, HIDDEN, gh, gw, dtype=torch.float32, device=dev) for _ in range(L + 1)]
+            pres = [torch.empty(b, HIDDEN, gh, gw, dtype=torch.float32, device=dev) for _ in range(L)]
+            xms = [torch.empty(NMODES, b, HIDDEN, dtype=torch.complex64, device=dev) for _ in range(L)]
+            sv = _lib.FnoTrainSaved()
+            for l in range(L + 1):
+                sv.act[l] = acts[l].data_ptr()
+            for l in range(L):
+                sv.pre[l], sv.xm[l] = pres[l].data_ptr(), xms[l].data_ptr()
+            preds = torch.empty(b, self.out_chan, gh, gw, dtype=torch.float32, device=dev)
+            _lib.check(lib.fno_grid_forward_train(C.byref(self._grid_struct(pk, gh, gw)), inputs.data_ptr(),
+                                                  mask4.data_ptr(), case_params.data_ptr(), preds.data_ptr(), C.byref(sv),
+                                                  C.byref(ws), b, gh, gw, self._stream()), "fno_grid_forward_train")
+            return preds, (sv, acts, pres, xms)
         ws, _ = self._workspace(b)
         adt = self._act_torch_dtype()
         acts = [torch.empty(b, HIDDEN, H, W, dtype=adt, device=dev) for _ in range(L + 1)]
@@ -380,7 +487,9 @@ class Fno2d(AutoCfdModel):
         sv, acts, pres, xms = saved_native
         b, L, dev = inputs.shape[0], self.num_layers, self.device
         pk = self._pack(need_bwd=True)
-        ws, _ = self._workspace(b)
+        gh, gw = inputs.shape[-2:]
+        grid = self._on_grid_path(gh, gw)
+        ws, _ = self._grid_workspace(b, gh, gw) if grid else self._workspace(b)
         layout, total = self._grad_layout()
         g = None
         if want_params:
@@ -398,19 +507,26 @@ class Fno2d(AutoCfdModel):
                 g.w0_b[l] = views[f"blocks.{l}.w0.bias"].data_ptr()
             g.fc1_w, g.fc1_b = views["fc1.weight"].data_ptr(), views["fc1.bias"].data_ptr()
             g.fc2_w, g.fc2_b = views["fc2.weight"].data_ptr(), views["fc2.bias"].data_ptr()
-        d0 = torch.empty(b, HIDDEN, H, W, dtype=torch.float32, device=dev)
-        d1 = torch.empty(b, HIDDEN, H, W, dtype=torch.float32, device=dev)
-        dz1 = torch.empty(min(b, _lib.BWD_CHUNK), PROJ, H, W, dtype=torch.float32, device=dev)
+        d0 = torch.empty(b, HIDDEN, gh, gw, dtype=torch.float32, device=dev)
+        d1 = torch.empty(b, HIDDEN, gh, gw, dtype=torch.float32, device=dev)
+        dz1 = torch.empty(min(b, _lib.BWD_CHUNK), PROJ, gh, gw, dtype=torch.float32, device=dev)
         gm = torch.empty(NMODES, b, HIDDEN, dtype=torch.complex64, device=dev)
         gwk = torch.empty(NMODES, HIDDEN, HIDDEN, dtype=torch.complex64, device=dev)
         sc = _lib.FnoBwdScratch()
         sc.d[0], sc.d[1] = d0.data_ptr(), d1.data_ptr()
         sc.dz1, sc.gm, sc.gwk = dz1.data_ptr(), gm.data_ptr(), gwk.data_ptr()
-        partials = torch.empty(lib.fno_bwd_partials_bytes(), dtype=torch.uint8, device=dev)
+        nbytes = lib.fno_grid_bwd_partials_bytes(gh, gw) if grid else lib.fno_bwd_partials_bytes()
+        partials = torch.empty(nbytes, dtype=torch.uint8, device=dev)
         sc.partials = partials.data_ptr()
 
         def run(events=None):
-            if with_data:
+            if grid:
+                _lib.check(lib.fno_grid_backward(C.byref(self._grid_struct(pk, gh, gw)), C.byref(pk["struct_bwd"]),
+                                                 inputs.data_ptr(), mask4.data_ptr(), case_params.data_ptr(),
+                                                 dpreds.data_ptr(), C.byref(sv), C.byref(g) if g is not None else None,
+                                                 C.byref(sc), C.byref(ws), _ptr(d_inputs), _ptr(d_cp), b, gh, gw,
+                                                 self._stream(), events), "fno_grid_backward")
+            elif with_data:
                 _lib.check(lib.fno_backward_inputs(C.byref(pk["struct"]), C.byref(pk["struct_bwd"]), inputs.data_ptr(),
                                                    mask4.data_ptr(), case_params.data_ptr(), dpreds.data_ptr(),
                                                    C.byref(sv), C.byref(g) if g is not None else None, C.byref(sc),
@@ -534,24 +650,32 @@ class Fno2d(AutoCfdModel):
         lib = _lib.load()
         b = inputs.shape[0]
         pk = self._pack()
-        ws, ws_bufs = self._workspace(b)
-        seq = torch.empty(steps, b, self.out_chan, H, W, dtype=torch.float32, device=self.device)
+        gh, gw = inputs.shape[-2:]
+        grid = self._on_grid_path(gh, gw)
+        ws, ws_bufs = self._grid_workspace(b, gh, gw) if grid else self._workspace(b)
+        seq = torch.empty(steps, b, self.out_chan, gh, gw, dtype=torch.float32, device=self.device)
+
+        def rollout(x, mk, cp, out):
+            if grid:
+                _lib.check(lib.fno_grid_rollout(C.byref(self._grid_struct(pk, gh, gw)), x.data_ptr(), mk.data_ptr(),
+                                                cp.data_ptr(), out.data_ptr(), steps, C.byref(ws), b, gh, gw,
+                                                self._stream()), "fno_grid_rollout")
+            else:
+                _lib.check(lib.fno_rollout(C.byref(pk["struct"]), x.data_ptr(), mk.data_ptr(), cp.data_ptr(),
+                                           out.data_ptr(), steps, C.byref(ws), b, self._act_code(), self._stream()),
+                           "fno_rollout")
         if not self.graph_rollout:
-            _lib.check(lib.fno_rollout(C.byref(pk["struct"]), inputs.data_ptr(), mask4.data_ptr(),
-                                       case_params.data_ptr(), seq.data_ptr(), steps, C.byref(ws), b,
-                                       self._act_code(), self._stream()), "fno_rollout")
+            rollout(inputs, mask4, case_params, seq)
             return seq
-        # CUDA-graph replay: static buffers, one capture per (batch, steps)
-        key = (b, steps, self.act_dtype)
+        # CUDA-graph replay: static buffers, one capture per (batch, steps[, grid])
+        key = (b, steps, "grid", gh, gw) if grid else (b, steps, self.act_dtype)
         ent = self._graphs.get(key)
         if ent is None:
             s_in, s_cp, s_mk = inputs.clone(), case_params.clone(), mask4.clone()
             s_seq = torch.empty_like(seq)
 
             def run():
-                _lib.check(lib.fno_rollout(C.byref(pk["struct"]), s_in.data_ptr(), s_mk.data_ptr(), s_cp.data_ptr(),
-                                           s_seq.data_ptr(), steps, C.byref(ws), b, self._act_code(),
-                                           self._stream()), "fno_rollout")
+                rollout(s_in, s_mk, s_cp, s_seq)
             side = torch.cuda.Stream(device=self.device)
             side.wait_stream(torch.cuda.current_stream(self.device))
             graph = torch.cuda.CUDAGraph()
@@ -627,6 +751,8 @@ class Fno2d(AutoCfdModel):
         calls: they are uploaded again only when the caller's tensors change (pointer / version / shape)."""
         lib = _lib.load()
         b = inputs.shape[0]
+        if inputs.dim() == 4 and inputs.shape[1] == self.in_chan and tuple(inputs.shape[-2:]) != (H, W):
+            return self._rollout_host_grid(inputs, case_params, mask, steps)
         if tuple(inputs.shape[1:]) != (self.in_chan, H, W):
             raise ValueError(f"inputs must be (B,{self.in_chan},{H},{W})")
         mask3 = mask.reshape(b, H, W)
@@ -733,4 +859,16 @@ class Fno2d(AutoCfdModel):
             with torch.cuda.stream(s_out):
                 out2[offs[c]:offs[c] + sizes[c]].copy_(ent["d_out"][c], non_blocking=True)
         s_out.synchronize()
+        return out
+
+    def _rollout_host_grid(self, inputs: Tensor, case_params: Tensor, mask: Tensor, steps: int) -> Tensor:
+        """Host tensors on a non-64x64 grid: upload, device rollout (graph-replayed like device tensors), and a copy into
+        a fresh pinned tensor the caller owns."""
+        b = inputs.shape[0]
+        gh, gw = self._check_grid(inputs.shape)
+        d_in, d_cp, mask4 = self._prep_inputs_grid(inputs, case_params, mask.reshape(b, gh, gw))
+        seq = self._rollout_device(d_in, d_cp, mask4, steps)
+        out = torch.empty(steps, b, self.out_chan, gh, gw, dtype=torch.float32, pin_memory=True)
+        out.copy_(seq, non_blocking=True)
+        torch.cuda.current_stream(self.device).synchronize()
         return out

@@ -11,7 +11,9 @@ seed, not 9.5 MB of spectral weights.  Distributions follow the reference's init
 * inputs: N(0,1) clipped to +-3 (fields are O(1) after the dataset's BC normalisation,
   reference ``src/dataset/utils.py:24-28``); case params N(0,1) (``dataset/utils.py:8-21``);
 * masks: cavity all ones (``src/dataset/cavity.py:31``); cylinder ones with a zeroed disc of
-  radius 4..8 px plus zeroed rows 0/63 and column 0 (``src/dataset/cylinder.py:249-275``).
+  radius 4..8 px plus zeroed rows 0/63 and column 0 (``src/dataset/cylinder.py:249-275``);
+  tube and dam ones on the 66x65 grid with the padded inlet column and the top / bottom wall rows
+  zeroed (``src/dataset/tube.py:34-50``, ``src/dataset/dam.py:87-105``).
 """
 from __future__ import annotations
 
@@ -26,8 +28,14 @@ PROJ = 128
 
 
 def n_case_params(problem: str) -> int:
-    """cavity -> 5, cylinder -> 8 (reference src/utils/autoregressive.py:31-37)."""
-    return {"cavity": 5, "cylinder": 8}[problem]
+    """cavity, tube, dam -> 5, cylinder -> 8 (reference src/utils/autoregressive.py:31-37)."""
+    return {"cavity": 5, "cylinder": 8, "tube": 5, "dam": 5}[problem]
+
+
+def grid(problem: str) -> tuple[int, int]:
+    """Frame size: 64x64 for cavity and cylinder as stored here; (64 + 2) x (64 + 1) for tube and dam, whose loaders pad
+    one inlet column and two wall rows (reference src/utils/autoregressive.py:24-26)."""
+    return (H + 2, W + 1) if problem in ("tube", "dam") else (H, W)
 
 
 def make_state_dict(seed: int, n_params: int = 5, in_chan: int = 2, out_chan: int = 2,
@@ -61,6 +69,13 @@ def make_state_dict(seed: int, n_params: int = 5, in_chan: int = 2, out_chan: in
 
 
 def make_mask(rng: np.random.Generator, batch: int, problem: str) -> np.ndarray:
+    if problem in ("tube", "dam"):
+        gh, gw = grid(problem)
+        mask = np.ones((batch, 1, gh, gw), dtype=np.float32)
+        mask[:, :, :, 0] = 0.0
+        mask[:, :, 0, :] = 0.0
+        mask[:, :, gh - 1, :] = 0.0
+        return mask
     mask = np.ones((batch, 1, H, W), dtype=np.float32)
     if problem == "cylinder":
         hh, ww = np.meshgrid(np.arange(H), np.arange(W), indexing="ij")
@@ -79,14 +94,15 @@ def make_batch(seed: int, batch: int, problem: str = "cavity", in_chan: int = 2,
                with_label: bool = True) -> dict[str, np.ndarray]:
     """One synthetic batch with the keys ``collate_fn`` produces (reference
     src/train_auto.py:53-58): inputs (B,2,H,W), label (B,2,H,W), mask (B,1,H,W),
-    case_params (B,p); all float32."""
+    case_params (B,p); all float32.  (H, W) = ``grid(problem)``."""
     rng = np.random.default_rng(seed)
     p = n_case_params(problem)
+    gh, gw = grid(problem)
     out = {
-        "inputs": np.clip(rng.standard_normal((batch, in_chan, H, W)), -3, 3).astype(np.float32),
+        "inputs": np.clip(rng.standard_normal((batch, in_chan, gh, gw)), -3, 3).astype(np.float32),
         "case_params": rng.standard_normal((batch, p)).astype(np.float32),
         "mask": make_mask(rng, batch, problem),
     }
     if with_label:
-        out["label"] = np.clip(rng.standard_normal((batch, in_chan, H, W)), -3, 3).astype(np.float32)
+        out["label"] = np.clip(rng.standard_normal((batch, in_chan, gh, gw)), -3, 3).astype(np.float32)
     return out

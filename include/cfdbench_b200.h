@@ -8,7 +8,8 @@
  * (fno_last_error() gives the message).  No entry point synchronises the device, none falls back to CPU.
  *
  * Fixed configuration (the reference's FNO config, src/args.py:99-103,187-197): H=W=64, hidden=32,
- * modes 12x12, fc1 width 128, out_chan=2, in_chan=2.  Activation storage `act_dtype`:
+ * modes 12x12, fc1 width 128, out_chan=2, in_chan=2.  Other grids (24 <= H, W <= 128, e.g. the 66x65 tube and dam
+ * frames) go through the fno_grid_* entry points at the end of this header (fp32 storage only).  Activation storage `act_dtype`:
  * FNO_ACT_F32 (parity mode) or FNO_ACT_BF16 (hidden activations stored as bf16 between kernels);
  * arithmetic is fp32 in both.
  *
@@ -274,6 +275,54 @@ typedef struct fno_adam_tensors {
 } fno_adam_tensors;
 int fno_adam_step(const fno_adam_tensors* t, float lr, float beta1, float beta2, float eps, float weight_decay,
                   int64_t step, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------
+ * Grid-generic path: the same network on H x W frames with 24 <= H <= 128 and 24 <= W <= 128, e.g. CFDBench's
+ * tube and dam problems (66 x 65, reference src/utils/autoregressive.py:24-26).  fp32 activation storage only (there is
+ * no act_dtype argument); hidden 32, modes 12 x 12, in/out 2 channels and p <= 16 as above.  With H = W = 64 these entry
+ * points run the generic kernels, not the 64 x 64 kernels above.  A grid outside the range returns FNO_ERR_UNSUPPORTED
+ * (3) with a message.  They take the structs above with these layouts:
+ *   frames / preds / d_inputs [B][2][H][W], mask [B][H][W]    float32, caller tensors: no alignment beyond 4 bytes needed
+ *   activations, pre, d[]     [B][32][H*W]                     float32, fno_grid_act_bytes(B, H, W)
+ *   modes (xm, ym, gm)        [288][B][32] complex64           as above; kxi 12..23 <-> kx H-12..H-1
+ *   z                         [B][H][24][32] float32           fno_grid_z_bytes(B, H)
+ *   dz1                       [min(B, FNO_BWD_CHUNK)][128][H*W] float32
+ *   partials                  fno_grid_bwd_partials_bytes(H, W)
+ *   fno_weights.gx / gy       H / W entries: float32(np.linspace(0, 1, n))
+ * Twiddle tables are built in float64 on the host once per (device, H, W) on first use; fno_destroy releases them.
+ * Gradients are bit-reproducible (per-CTA partial rows from a fixed number of CTAs, fixed-order reductions).
+ * ------------------------------------------------------------------------------------------------- */
+size_t fno_grid_act_bytes(int batch, int h, int w);
+size_t fno_grid_z_bytes(int batch, int h);
+size_t fno_grid_bwd_partials_bytes(int h, int w);
+/* the stages, one launch each (same meaning as fno_lift_fwd .. fno_project_fwd) */
+int fno_grid_lift_fwd(const float* inputs, const float* mask, const float* case_params, const fno_weights* w,
+                      float* act_out, int batch, int h, int w_, void* stream);
+int fno_grid_spectral_dft_fwd(const float* act_in, void* xm, int batch, int h, int w, float s0, float s1, void* stream);
+int fno_grid_spectral_inv_kx(const void* ym, float* z, int batch, int h, int w, float s0, float s1, void* stream);
+int fno_grid_block_out(int epilogue, const float* z, const float* act_in, const float* w0t, const float* bias, float* act_out,
+                       float* pre_out, const float* pre_in, int batch, int h, int w, void* stream);
+int fno_grid_project_fwd(const float* act_in, const float* mask, const fno_weights* w, float* preds, int batch, int h, int w_,
+                         void* stream);
+/* backward of fno_grid_project_fwd given dL/dpreds: dpre_out = dL/dpre of the last block (pre = its pre-activation),
+ * and, when the four gradient pointers are set (all or none), the fc1 / fc2 gradients (overwritten).  dz1 and partials:
+ * scratch as above. */
+int fno_grid_project_bwd(const float* act_in, const float* dpreds, const float* mask, const float* pre, const fno_weights* w,
+                         float* dpre_out, float* dz1, float* partials, float* g_fc1_w, float* g_fc1_b, float* g_fc2_w,
+                         float* g_fc2_b, int batch, int h, int w_, void* stream);
+/* fno_forward / fno_rollout / fno_forward_train on an H x W grid */
+int fno_grid_forward(const fno_weights* w, const float* inputs, const float* mask, const float* case_params, float* preds,
+                     const fno_workspace* ws, int batch, int h, int w_, void* stream);
+int fno_grid_rollout(const fno_weights* w, const float* inputs, const float* mask, const float* case_params, float* preds_seq,
+                     int steps, const fno_workspace* ws, int batch, int h, int w_, void* stream);
+int fno_grid_forward_train(const fno_weights* w, const float* inputs, const float* mask, const float* case_params,
+                           float* preds, const fno_train_saved* saved, const fno_workspace* ws, int batch, int h, int w_,
+                           void* stream);
+/* fno_backward_inputs on an H x W grid: grads = NULL gives the data-only backward; seg_events as fno_backward_ex */
+int fno_grid_backward(const fno_weights* w, const fno_weights_bwd* wb, const float* inputs, const float* mask,
+                      const float* case_params, const float* dpreds, const fno_train_saved* saved, const fno_grads* grads,
+                      const fno_bwd_scratch* scratch, const fno_workspace* ws, float* d_inputs, float* d_case_params,
+                      int batch, int h, int w_, void* stream, void* const* seg_events);
 
 #ifdef __cplusplus
 }
