@@ -11,13 +11,19 @@
 //          swizzle makes those loads conflict-free -- and B = the constant F (K-major); Z1 -> tf32 hi/lo -> Zt, the
 //          K-major B operand of GEMM2 per image row (96 KB for 16 rows).  Bias rides in the row that irfft2's C2R stage
 //          ignores (Im of ky = 0).
-//   GEMM2 per image row h:  D[64 w][32 o] = E[w][(ky, ri) 24] Zt_h + X_h[w][32 i] W0^T   (m64n32k8, 3xTF32 / 2 passes)
-//          E = C2R stage with c_ky/HW folded in (fno_block_tc.cu builds it); X_h staged through registers (bf16 values
-//          are exact in tf32); epilogue exact-erf GELU, bf16 pairs exchanged between neighbouring lanes, 4-byte stores.
+//   GEMM2 per image row h:  D[64 w][32 o] = E[w][(ky, ri) 24] Zt_h + X_h[w][32 i] W0^T
+//          E Zt_h: m64n32k8 tf32, 3xTF32 (E = C2R stage with c_ky/HW folded in, fno_block_tc.cu builds it).
+//          X_h W0^T: m64n32k16 bf16 straight from the TMA slot that holds the row as [i][w] (the M-major A operand), W0 as
+//          three bf16 terms (24 mantissa bits), accumulated into the same fp32 registers.  x is exact in bf16.
+//          Epilogue exact-erf GELU -> bf16 -> swizzled [o][w] staging tile -> one TMA store per row.
 // Roles: warp 8 lanes 0/1 -- producers of the two image slots (24 KB = one ky pair, hi + lo, two bulk copies each);
-// warpgroups 0 / 1 -- the even / odd ky pairs of GEMM1 and the even / odd rows of GEMM2.
+// warpgroups 0 / 1 -- the even / odd ky pairs of GEMM1 and the even / odd rows of GEMM2.  Each warpgroup owns a ring of
+// kFzXSlots activation rows; its thread 0 refills a slot as soon as the MMAs that read it have completed, so the ring
+// runs up to kFzXSlots rows ahead, across GEMM1 and across unit boundaries.  GEMM2 keeps two accumulator sets: the MMAs of
+// row r + 1 run while row r's epilogue does.
 #include "fno_common.cuh"
 #include "tc_common.cuh"
+#include "tc_tma.cuh"
 #include <math.h>
 #include <string.h>
 
@@ -25,6 +31,7 @@ namespace fno {
 
 constexpr int kFzRows = 16;                            // image rows per unit
 constexpr int kFzChunks = kH / kFzRows;                // 4
+constexpr int kFzWgRows = kFzRows / 2;                 // GEMM2 rows per warpgroup and unit
 constexpr int kFzThreads = 9 * 32;                     // 2 warpgroups + producer warp
 constexpr int kFzProdWarp = 8;
 constexpr int kZK = 2 * kM2;                           // 24: (ky, re|im)
@@ -37,27 +44,47 @@ constexpr uint32_t kFzZtFloats = kC * kZK;             // one image row, hi or l
 constexpr uint32_t kLboF = (2 * kFzRows / 8) * 128;    // 512
 constexpr uint32_t kLboE = (kW / 8) * 128;             // 1024
 constexpr uint32_t kLboO = (kC / 8) * 128;             // 512: B operands with 32 rows (o)
+// One image row of all 32 channels of a bf16 activation: TMA box {w 64, h 1, (b, c) 32}, [c][w] with the 128-byte swizzle.
+// The same box is the load of x and the store of out.
+constexpr uint32_t kFzBoxW = kW, kFzBoxH = 1, kFzBoxC = kC;
+constexpr uint32_t kFzRowBytes = kFzBoxW * kFzBoxH * kFzBoxC * 2;   // 4096 = expect_tx of one fill
+constexpr int kFzXSlots = 4;                                         // activation rows in flight per warpgroup
+constexpr uint32_t kFzW0Bytes = kC * kC * 2;                         // one bf16 term of W0, K-major
+
+// Activation ring of a warpgroup: fill n (n = kFzWgRows * unit + r, r-th GEMM2 row of the unit) goes to slot n % S and
+// completes phase n / S of that slot's barrier.  The same two functions are used where a fill is issued and waited for.
+__host__ __device__ constexpr int fz_x_slot(int n) { return n % kFzXSlots; }
+__host__ __device__ constexpr uint32_t fz_x_parity(int n) { return static_cast<uint32_t>(n / kFzXSlots) & 1u; }
 
 struct FzSmem {
+  alignas(1024) unsigned char x[2][kFzXSlots][kFzRowBytes];   // per warpgroup: activation ring (TMA, 128B swizzle)
+  alignas(1024) unsigned char st[2][2][kFzRowBytes];          // per warpgroup: double-buffered output staging tile
   alignas(128) unsigned char y[2][kFzStage];           // image ring (slot = parity of the ky pair)
   alignas(128) float zt[kFzRows][2][kFzZtFloats];      // GEMM2 B operand per row: hi, lo
   alignas(128) float f_hi[kFzFFloats / 2];
   alignas(128) float f_lo[kFzFFloats / 2];
   alignas(128) float e_hi[kFzEFloats / 2];
   alignas(128) float e_lo[kFzEFloats / 2];
-  alignas(128) float wb_hi[kC * kC];
-  alignas(128) float wb_lo[kC * kC];
-  alignas(128) float ax[2][kW * kC];                   // per warpgroup: conv A operand of the current row
+  alignas(128) unsigned char w0[3][kFzW0Bytes];        // B[n = o][k = i] = W0[o][i] = t1 + t2 + t3 (bf16 terms)
   alignas(16) float bias[kC];
   alignas(8) uint64_t y_full[2], y_free[2];
+  alignas(8) uint64_t x_full[2][kFzXSlots];
 };
+static_assert(sizeof(FzSmem) <= 232448, "block_fused_kernel: shared memory over the per-block opt-in limit");
+
+// byte offset of (line, element e) in a 128-byte-swizzled image of 128-byte lines of bf16 (what TMA writes / reads)
+__device__ __forceinline__ uint32_t sw128_bf16_offset(int line, int e) {
+  return static_cast<uint32_t>(line * 128 + ((((e >> 3) ^ line) & 7) << 4) + (e & 7) * 2);
+}
 
 __global__ void __launch_bounds__(kFzThreads, 1)
-    block_fused_kernel(const unsigned char* __restrict__ img, const __nv_bfloat16* __restrict__ x,
-                       const float* __restrict__ w0t, const float* __restrict__ bias, const float* __restrict__ etab,
-                       const float* __restrict__ ftab, __nv_bfloat16* __restrict__ out, int batch) {
+    block_fused_kernel(const __grid_constant__ CUtensorMap x_map, const __grid_constant__ CUtensorMap out_map,
+                       const unsigned char* __restrict__ img, const float* __restrict__ w0t,
+                       const float* __restrict__ bias, const float* __restrict__ etab, const float* __restrict__ ftab,
+                       int batch) {
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   FzSmem& sm = *reinterpret_cast<FzSmem*>(smem_raw);
+  if ((smem_u32(smem_raw) & 1023u) != 0) __trap();   // the TMA swizzle atoms need 1024-byte alignment
   const int tid = threadIdx.x, lane = tid & 31, warp = tc::warp_index_uniform();
   const int chunk = blockIdx.x % kFzChunks, b0 = blockIdx.x / kFzChunks, bstride = gridDim.x / kFzChunks;
   const int n_units = b0 < batch ? (batch - b0 + bstride - 1) / bstride : 0;
@@ -67,6 +94,7 @@ __global__ void __launch_bounds__(kFzThreads, 1)
     for (int i = 0; i < 2; ++i) {
       mbar_init(&sm.y_full[i], 1);
       mbar_init(&sm.y_free[i], 4);   // the four warps of the warpgroup that reads the slot
+      for (int s = 0; s < kFzXSlots; ++s) mbar_init(&sm.x_full[i][s], 1);   // thread 0 of the warpgroup: expect_tx
     }
     fence_mbar_init();
   }
@@ -78,13 +106,17 @@ __global__ void __launch_bounds__(kFzThreads, 1)
     sm.e_hi[e] = __ldg(etab + e);
     sm.e_lo[e] = __ldg(etab + kFzEFloats / 2 + e);
   }
-  for (int e = tid; e < kC * kC; e += kFzThreads) {  // B[n = o][k = i] = W0[o][i] = w0t[i][o]
+  for (int e = tid; e < kC * kC; e += kFzThreads) {  // B[n = o][k = i] = W0[o][i] = w0t[i][o]: three bf16 terms
     const int i = e / kC, o = e % kC;
-    float hi, lo;
-    tc::split_tf32(w0t[e], hi, lo);
-    const uint32_t off = tc::kmajor_offset(o, i, kC) / 4;
-    sm.wb_hi[off] = hi;
-    sm.wb_lo[off] = lo;
+    const float w = w0t[e];
+    const __nv_bfloat16 t1 = __float2bfloat16_rn(w);
+    const float r1 = w - __bfloat162float(t1);
+    const __nv_bfloat16 t2 = __float2bfloat16_rn(r1);
+    const __nv_bfloat16 t3 = __float2bfloat16_rn(r1 - __bfloat162float(t2));
+    const uint32_t off = static_cast<uint32_t>(((i >> 3) * (kC / 8) + (o >> 3)) * 128 + (o & 7) * 16 + (i & 7) * 2);
+    *reinterpret_cast<__nv_bfloat16*>(sm.w0[0] + off) = t1;
+    *reinterpret_cast<__nv_bfloat16*>(sm.w0[1] + off) = t2;
+    *reinterpret_cast<__nv_bfloat16*>(sm.w0[2] + off) = t3;
   }
   if (tid < kC) sm.bias[tid] = bias != nullptr ? bias[tid] : 0.f;
   tc::fence_proxy_async_smem();   // the constant operands above are read by the tensor cores
@@ -113,6 +145,17 @@ __global__ void __launch_bounds__(kFzThreads, 1)
   // ================================================================ consumers
   const int g = warp >> 2, wq = warp & 3, q = lane & 3, t = tid & 127;
   const int m0 = 16 * wq + (lane >> 2);   // fragment rows m0, m0 + 8
+  const int n_fills = kFzWgRows * n_units;
+  // fill n of this warpgroup's activation ring: row h = 16 chunk + g + 2 r of unit u, all 32 channels (thread t == 0)
+  auto x_fill = [&](int n) {
+    const int u = n / kFzWgRows, r = n % kFzWgRows, s = fz_x_slot(n);
+    mbar_expect_tx(&sm.x_full[g][s], kFzRowBytes);
+    tma_load_3d(sm.x[g][s], &x_map, 0, kFzRows * chunk + g + 2 * r, (b0 + u * bstride) * kC, &sm.x_full[g][s]);
+  };
+  if (t == 0)
+    for (int n = 0; n < kFzXSlots && n < n_fills; ++n) x_fill(n);
+  const uint32_t w0_s = tc::smem_addr(sm.w0[0]);
+
   for (int u = 0; u < n_units; ++u) {
     const int b = b0 + u * bstride;
     // ---------------------------------------------------------------- GEMM1: ky pairs g, g + 2, g + 4
@@ -141,11 +184,12 @@ __global__ void __launch_bounds__(kFzThreads, 1)
                              (pass | ks) ? 1u : 0u);
       }
       tc::wg_commit();
-      tc::wg_wait<0>();
-      tc::wg_fence_acc(acc);
-      // the MMAs have consumed the fragments loaded from the stage: the producer may refill it
+      // the MMAs above were issued, so the fragments they take from registers have been loaded from the stage: the
+      // producer may refill it while they run
       __syncwarp();
       if (lane == 0) mbar_arrive(&sm.y_free[g]);
+      tc::wg_wait<0>();
+      tc::wg_fence_acc(acc);
       if (pi == 0) tc::named_barrier(1, 256);   // both warpgroups are done with the previous unit's Zt
       // acc[4 i + 2 hh + e] = Z1[m0 + 8 hh][n = 8 i + 2 q + e]: row h' = 4 i + q, re|im = e
 #pragma unroll
@@ -169,68 +213,68 @@ __global__ void __launch_bounds__(kFzThreads, 1)
     tc::named_barrier(1, 256);   // Zt of all 16 rows is complete
 
     // ---------------------------------------------------------------- GEMM2: rows g, g + 2, ..., 14 + g
-    __nv_bfloat16 xr[4][4];   // task = rep * 128 + t -> (pixel w = task & 63, channel quad = task >> 6)
-    auto x_prefetch = [&](int h) {
+    // Iteration r issues row r's MMAs into acc[r & 1], then finishes row r - 1: wait for its MMAs (all but the newest
+    // group), GELU into staging tile (r - 1) & 1, one TMA store, and the refill of the activation slot it read.
+    float acc[2][16];
 #pragma unroll
-      for (int rep = 0; rep < 4; ++rep) {
-        const int task = rep * 128 + t, w = task & 63, kq = task >> 6;
-        const __nv_bfloat16* src = x + (static_cast<size_t>(b) * kC + 4 * kq) * kHW + h * kW + w;
-#pragma unroll
-        for (int c = 0; c < 4; ++c) xr[rep][c] = src[static_cast<size_t>(c) * kHW];
-      }
-    };
-    x_prefetch(kFzRows * chunk + g);
-    for (int r = 0; r < kFzRows / 2; ++r) {
-      const int hl = g + 2 * r, h = kFzRows * chunk + hl;
-#pragma unroll
-      for (int rep = 0; rep < 4; ++rep) {
-        const int task = rep * 128 + t, w = task & 63, kq = task >> 6;
-        *reinterpret_cast<float4*>(sm.ax[g] + tc::kmajor_offset(w, 4 * kq, kW) / 4) =
-            make_float4(__bfloat162float(xr[rep][0]), __bfloat162float(xr[rep][1]), __bfloat162float(xr[rep][2]),
-                        __bfloat162float(xr[rep][3]));
-      }
-      tc::fence_proxy_async_smem();
-      tc::named_barrier(2 + g, 128);
-      if (r + 1 < kFzRows / 2) x_prefetch(h + 2);
-      float acc[16];
-      tc::wg_fence();
-      {
+    for (int r = 0; r <= kFzWgRows; ++r) {
+      if (r < kFzWgRows) {
+        const int n = kFzWgRows * u + r, hl = g + 2 * r;
+        mbar_wait(&sm.x_full[g][fz_x_slot(n)], fz_x_parity(n));
+        tc::wg_fence();
         const uint32_t a_e[3] = {tc::smem_addr(sm.e_hi), tc::smem_addr(sm.e_lo), tc::smem_addr(sm.e_hi)};
         const uint32_t b_z[3] = {tc::smem_addr(sm.zt[hl][0]), tc::smem_addr(sm.zt[hl][0]), tc::smem_addr(sm.zt[hl][1])};
 #pragma unroll
         for (int pass = 0; pass < 3; ++pass)
 #pragma unroll
           for (int ks = 0; ks < kZK / 8; ++ks)
-            tc::wg_tf32_ss_n32(acc, tc::make_smem_desc(a_e[pass] + ks * 2 * kLboE, kLboE, 128),
+            tc::wg_tf32_ss_n32(acc[r & 1], tc::make_smem_desc(a_e[pass] + ks * 2 * kLboE, kLboE, 128),
                                tc::make_smem_desc(b_z[pass] + ks * 2 * kLboO, kLboO, 128), (pass | ks) ? 1u : 0u);
-        const uint32_t a_x = tc::smem_addr(sm.ax[g]);
+        tc::wg_fence();   // the bf16 MMAs below have another shape: order their accumulator accesses explicitly
+        const uint32_t a_x = tc::smem_addr(sm.x[g][fz_x_slot(n)]);
 #pragma unroll
-        for (int pass = 0; pass < 2; ++pass) {
-          const uint32_t b_w = tc::smem_addr(pass ? sm.wb_lo : sm.wb_hi);
+        for (int term = 0; term < 3; ++term)
 #pragma unroll
-          for (int ks = 0; ks < kC / 8; ++ks)
-            tc::wg_tf32_ss_n32(acc, tc::make_smem_desc(a_x + ks * 2 * kLboE, kLboE, 128),
-                               tc::make_smem_desc(b_w + ks * 2 * kLboO, kLboO, 128), 1u);
-        }
+          for (int ks = 0; ks < kC / 16; ++ks)   // K = 16 channels = 16 lines of 128 B
+            tc::wg_bf16_ss_n32_mn_a(acc[r & 1], tc::make_smem_desc_sw128_mn(a_x + ks * 2048),
+                                    tc::make_smem_desc(w0_s + term * kFzW0Bytes + ks * 2 * kLboO, kLboO, 128), 1u);
+        tc::wg_commit();
       }
-      tc::wg_commit();
-      tc::wg_wait<0>();
-      tc::wg_fence_acc(acc);
-      // acc[4 i + 2 hh + e] = D[w = m0 + 8 hh][o = 8 i + 2 q + e].  Lane ^ 4 holds pixel w ^ 1: the even pixel's lane stores
-      // channel o of both pixels, the odd one channel o + 1, as bf16x2.
-      const bool odd = (lane >> 2) & 1;
+      if (r == 0) continue;
+      const int rr = r - 1, h = kFzRows * chunk + g + 2 * rr;
+      float* d = acc[rr & 1];
+      if (r < kFzWgRows) {
+        tc::wg_wait<1>();
+      } else {
+        tc::wg_wait<0>();
+      }
+      tc::wg_fence_acc(acc[rr & 1]);
+      // d[4 i + 2 hh + e] = D[w = m0 + 8 hh][o = 8 i + 2 q + e] -> staging line o, element w.  Per store instruction a
+      // warp writes 8 consecutive pixels of 4 channels whose lines have distinct swizzle phases: no bank conflicts.
+      unsigned char* stile = sm.st[g][rr & 1];
 #pragma unroll
       for (int i = 0; i < 4; ++i)
 #pragma unroll
         for (int hh = 0; hh < 2; ++hh) {
-          const float2 v = gelu_erf2(make_float2(acc[4 * i + 2 * hh], acc[4 * i + 2 * hh + 1]));
-          const float recv = __shfl_xor_sync(0xffffffffu, odd ? v.x : v.y, 4);
-          const int w = m0 + 8 * hh, o = 8 * i + 2 * q + (odd ? 1 : 0);
-          const __nv_bfloat162 pair = odd ? __floats2bfloat162_rn(recv, v.y) : __floats2bfloat162_rn(v.x, recv);
-          *reinterpret_cast<__nv_bfloat162*>(out + (static_cast<size_t>(b) * kC + o) * kHW + h * kW + (w & ~1)) = pair;
+          const float2 v = gelu_erf2(make_float2(d[4 * i + 2 * hh], d[4 * i + 2 * hh + 1]));
+          const int w = m0 + 8 * hh, o = 8 * i + 2 * q;
+          *reinterpret_cast<__nv_bfloat16*>(stile + sw128_bf16_offset(o, w)) = __float2bfloat16_rn(v.x);
+          *reinterpret_cast<__nv_bfloat16*>(stile + sw128_bf16_offset(o + 1, w)) = __float2bfloat16_rn(v.y);
         }
+      tc::fence_proxy_async_smem();
+      // the store of the previous row has read its tile, which the next row's epilogue overwrites
+      if (t == 0) bulk_wait_group_read<0>();
+      // all 128 threads: tile written, and row rr's MMAs -- the last readers of its activation slot -- complete
+      tc::named_barrier(2 + g, 128);
+      if (t == 0) {
+        tma_store_3d(&out_map, stile, 0, h, b * kC);
+        bulk_commit_group();
+        const int nf = kFzWgRows * u + rr + kFzXSlots;
+        if (nf < n_fills) x_fill(nf);
+      }
     }
   }
+  if (t == 0) bulk_wait_group<0>();   // the staging tiles live in this CTA's shared memory
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -313,16 +357,24 @@ cudaError_t launch_block_fused(const void* ym_img, const void* x, const float* w
   if (dev < 0 || dev >= 64) return cudaErrorInvalidDevice;
   e = fz_ensure(dev, stream);
   if (e != cudaSuccess) return e;
+  // TMA needs 16-byte aligned global addresses
   if ((reinterpret_cast<uintptr_t>(x) & 15) || (reinterpret_cast<uintptr_t>(ym_img) & 15) ||
-      (reinterpret_cast<uintptr_t>(out) & 3))
+      (reinterpret_cast<uintptr_t>(out) & 15))
     return cudaErrorMisalignedAddress;
+  // x and out as [batch * 32 planes][64 h][64 w] bf16; box = one image row of the 32 channels of a sample.  The maps are
+  // kernel parameters, so a captured graph keeps the ones of its own buffers.
+  CUtensorMap x_map, out_map;
+  const uint64_t planes = static_cast<uint64_t>(batch) * kC;
+  e = make_tma_map_3d(&x_map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, x, kW, kH, planes, kFzBoxW, kFzBoxH, kFzBoxC);
+  if (e != cudaSuccess) return e;
+  e = make_tma_map_3d(&out_map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, out, kW, kH, planes, kFzBoxW, kFzBoxH, kFzBoxC);
+  if (e != cudaSuccess) return e;
   // four CTAs (one per chunk of rows) per sample slot; the slots stride over the batch
   const int slots_max = g_fz[dev].n_sm / kFzChunks;
   const int slots = batch < slots_max ? batch : slots_max;
-  return launch_chained(block_fused_kernel, dim3(kFzChunks * slots), dim3(kFzThreads), sizeof(FzSmem), stream,
-                        static_cast<const unsigned char*>(ym_img), static_cast<const __nv_bfloat16*>(x), w0t, bias,
-                        static_cast<const float*>(g_fz[dev].etab), static_cast<const float*>(g_fz[dev].ftab),
-                        static_cast<__nv_bfloat16*>(out), batch);
+  return launch_chained(block_fused_kernel, dim3(kFzChunks * slots), dim3(kFzThreads), sizeof(FzSmem), stream, x_map,
+                        out_map, static_cast<const unsigned char*>(ym_img), w0t, bias,
+                        static_cast<const float*>(g_fz[dev].etab), static_cast<const float*>(g_fz[dev].ftab), batch);
 }
 
 }  // namespace fno

@@ -50,6 +50,12 @@ __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_
 __device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t saddr) {
   return make_smem_desc(saddr, 16, 1024) | (static_cast<uint64_t>(1) << 62);
 }
+// M-major (MN-major) bf16 operand of 64 rows written by TMA with the 128-byte swizzle: line k holds the 64 M values of
+// K index k (128 B), 8-line atoms of 1024 B, 1024-byte aligned.  SBO = the K distance between 8-line groups (1024); LBO
+// would step to the next 64 M values, which a 64-row operand does not have.  A K step of 16 advances the start by 2048.
+__device__ __forceinline__ uint64_t make_smem_desc_sw128_mn(uint32_t saddr) {
+  return make_smem_desc(saddr, 16, 1024) | (static_cast<uint64_t>(1) << 62);
+}
 
 // ---- warpgroup MMA ----------------------------------------------------------------------------------
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
@@ -93,6 +99,15 @@ __device__ __forceinline__ void wg_bf16_ss_n72(float* d, uint64_t a, uint64_t b,
       "{\n.reg .pred p;\nsetp.ne.b32 p, %38, 0;\n"
       "wgmma.mma_async.sync.aligned.m64n72k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35}, %36, %37, p, 1, 1, 0, 0;\n}\n"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35])
+      : "l"(a), "l"(b), "r"(acc)
+      : "memory");
+}
+// A M-major (transpose bit set, descriptor above), B K-major.
+__device__ __forceinline__ void wg_bf16_ss_n32_mn_a(float* d, uint64_t a, uint64_t b, uint32_t acc) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 1, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
       : "l"(a), "l"(b), "r"(acc)
       : "memory");
 }

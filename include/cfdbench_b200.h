@@ -120,7 +120,8 @@ int fno_block_out(int epilogue, const void* z, const void* act_in, const float* 
  * reference src/models/fno/fno2d.py:81,104-111, without the Z round trip through HBM.
  *   fno_mode_mix_image: same product as fno_mode_mix, written as the per-sample tensor-core operand image the fused
  *     kernel bulk-copies (tf32 hi/lo split, fno_ym_image_bytes(B) bytes).
- *   fno_block_fused:    act_out = GELU(irfft2(pad(Y)) + W0 act_in + bias); act_in / act_out bf16 [B][32][64][64]. */
+ *   fno_block_fused:    act_out = GELU(irfft2(pad(Y)) + W0 act_in + bias); act_in / act_out bf16 [B][32][64][64],
+ *     16-byte aligned (they are read and written by TMA). */
 int fno_mode_mix_image(const void* xm, const void* wop, void* ym_img, int batch, void* stream);
 int fno_block_fused(const void* ym_img, const void* act_in_bf16, const float* w0t, const float* bias, void* act_out_bf16,
                     int batch, void* stream);
