@@ -11,7 +11,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libcfdbench_b200.so")
 
 FNO_MAX_LAYERS = 8
-ABI_VERSION = 3
+ABI_VERSION = 4
 ACT_F32, ACT_BF16 = 0, 1
 EPI_GELU, EPI_GELU_SAVE_PRE, EPI_MUL_DGELU, EPI_PLAIN = 0, 1, 2, 3
 
@@ -103,7 +103,6 @@ SIGNATURES = {
     "fno_pack_mix_operand_from_weights": (C.c_int, [_P, _P, _P, _I, _P]),
     "fno_lift_fwd": (C.c_int, [_P, _P, _P, C.POINTER(FnoWeights), _P, _I, _I, _P]),
     "fno_spectral_dft_fwd": (C.c_int, [_P, _P, _I, _I, _F, _F, _P]),
-    "fno_spectral_dft_fwd_tc": (C.c_int, [_P, _P, _I, _F, _F, _P]),
     "fno_mode_mix": (C.c_int, [_P, _P, _P, _I, _P]),
     "fno_spectral_inv_kx": (C.c_int, [_P, _P, _I, _F, _F, _P]),
     "fno_block_out": (C.c_int, [_I, _P, _P, _P, _P, _P, _P, _P, _I, _I, _P]),
@@ -112,8 +111,6 @@ SIGNATURES = {
     "fno_forward": (C.c_int, [C.POINTER(FnoWeights), _P, _P, _P, _P, C.POINTER(FnoWorkspace), _I, _I, _P]),
     "fno_rollout": (C.c_int, [C.POINTER(FnoWeights), _P, _P, _P, _P, _I, C.POINTER(FnoWorkspace), _I, _I, _P]),
     "fno_rollout_host": (C.c_int, [C.POINTER(FnoWeights), _P, _P, _P, _P, _I, C.POINTER(FnoWorkspace), _P, _I, _I, _P]),
-    "fno_rollout_host_chunked": (C.c_int, [C.POINTER(FnoWeights), _P, _P, _P, _P, C.POINTER(FnoWorkspace),
-                                           C.POINTER(C.c_void_p), _I, _I, _I, _P, _P, _P]),
     "fno_rollout_host_scratch_bytes": (C.c_size_t, [_I, _I, _I]),
     "fno_multistep_metrics": (C.c_int, [_P, _P, _P, _P, _I, _I, _P]),
     "fno_gather_batch": (C.c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _P, _P, _P, _P, _P]),
@@ -124,15 +121,12 @@ SIGNATURES = {
                                 C.c_int64, _P]),
     "fno_forward_train": (C.c_int, [C.POINTER(FnoWeights), _P, _P, _P, _P, C.POINTER(FnoTrainSaved),
                                     C.POINTER(FnoWorkspace), _I, _I, _P]),
-    "fno_backward_ex": (C.c_int, [C.POINTER(FnoWeights), C.POINTER(FnoWeightsBwd), _P, _P, _P, _P,
-                                  C.POINTER(FnoTrainSaved), C.POINTER(FnoGrads), C.POINTER(FnoBwdScratch),
-                                  C.POINTER(FnoWorkspace), _I, _I, _P, C.POINTER(C.c_void_p)]),
     "fno_backward": (C.c_int, [C.POINTER(FnoWeights), C.POINTER(FnoWeightsBwd), _P, _P, _P, _P,
                                C.POINTER(FnoTrainSaved), C.POINTER(FnoGrads), C.POINTER(FnoBwdScratch),
                                C.POINTER(FnoWorkspace), _I, _I, _P]),
     "fno_backward_inputs": (C.c_int, [C.POINTER(FnoWeights), C.POINTER(FnoWeightsBwd), _P, _P, _P, _P,
                                       C.POINTER(FnoTrainSaved), C.POINTER(FnoGrads), C.POINTER(FnoBwdScratch),
-                                      C.POINTER(FnoWorkspace), _P, _P, _I, _I, _P, C.POINTER(C.c_void_p)]),
+                                      C.POINTER(FnoWorkspace), _P, _P, _I, _I, _P]),
     # grid-generic fp32 path (H, W in 24..128)
     "fno_grid_act_bytes": (C.c_size_t, [_I, _I, _I]),
     "fno_grid_z_bytes": (C.c_size_t, [_I, _I]),
@@ -149,7 +143,7 @@ SIGNATURES = {
                                          C.POINTER(FnoWorkspace), _I, _I, _I, _P]),
     "fno_grid_backward": (C.c_int, [C.POINTER(FnoWeights), C.POINTER(FnoWeightsBwd), _P, _P, _P, _P,
                                     C.POINTER(FnoTrainSaved), C.POINTER(FnoGrads), C.POINTER(FnoBwdScratch),
-                                    C.POINTER(FnoWorkspace), _P, _P, _I, _I, _I, _P, C.POINTER(C.c_void_p)]),
+                                    C.POINTER(FnoWorkspace), _P, _P, _I, _I, _I, _P]),
 }
 
 GRID_MIN, GRID_MAX = 24, 128

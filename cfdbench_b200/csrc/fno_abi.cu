@@ -1,5 +1,4 @@
 // extern "C" surface of libcfdbench_b200.so (declared in include/cfdbench_b200.h).
-#include <stdlib.h>
 #include <stdio.h>
 #include <string.h>
 
@@ -7,7 +6,6 @@
 #include "fno_common.cuh"
 
 namespace fno {
-template <typename TAct>
 cudaError_t launch_dft_fwd(const void*, void*, int, float, float, cudaStream_t);
 cudaError_t launch_mode_mix(const void*, const void*, void*, void*, int, cudaStream_t);
 cudaError_t launch_block_fused(const void*, const void*, const float*, const float*, void*, int, cudaStream_t);
@@ -34,10 +32,7 @@ cudaError_t launch_lift(const float*, const float*, const float*, const float*, 
 template <typename TAct>
 cudaError_t launch_project_tc(const void*, const float*, const float*, const float*, const float*, const float*,
                               float*, int, cudaStream_t);
-template <typename TAct>
-cudaError_t launch_project_bwd(const void*, const float*, const float*, const float*, const float*, const float*,
-                               const float*, float*, float*, float*, int, cudaStream_t);
-int project_bwd_parts(int);
+int project_bwd_rows_max();
 int project_bwd_row();
 cudaError_t launch_reduce_partials(const float*, int, int, float*, int, float*, int, float*, int, int, cudaStream_t);
 template <typename TAct>
@@ -83,7 +78,6 @@ void block_tc_release(int);
 void block_fused_release(int);
 void dft_fwd_tc_release(int);
 }  // namespace fno
-static cudaEvent_t g_chunk_events[64][2][16] = {};   // fno_rollout_host_chunked: [device][upload|compute][chunk]
 
 static thread_local char g_err[512] = "";
 
@@ -121,12 +115,6 @@ int fno_destroy(void) {
   block_fused_release(dev);
   dft_fwd_tc_release(dev);
   grid_tables_release(dev);
-  for (int k = 0; k < 2; ++k)
-    for (int c = 0; c < 16; ++c)
-      if (g_chunk_events[dev][k][c]) {
-        cudaEventDestroy(g_chunk_events[dev][k][c]);
-        g_chunk_events[dev][k][c] = nullptr;
-      }
   return kOk;
 }
 const char* fno_last_error(void) { return g_err; }
@@ -138,7 +126,7 @@ size_t fno_modes_bytes(int batch) { return static_cast<size_t>(batch) * kModes *
 size_t fno_z_bytes(int batch) { return static_cast<size_t>(batch) * kH * 2 * kM2 * kC * sizeof(float); }
 size_t fno_ym_image_bytes(int batch) { return ym_image_bytes(batch); }
 size_t fno_bwd_partials_bytes(void) {
-  return (static_cast<size_t>(296) * (kProj * kC + kProj) + static_cast<size_t>(project_bwd_parts(FNO_BWD_CHUNK)) * project_bwd_row() +
+  return (static_cast<size_t>(296) * (kProj * kC + kProj) + static_cast<size_t>(project_bwd_rows_max()) * project_bwd_row() +
           static_cast<size_t>(16) * kC * (5 + kMaxCaseParams + 1)) * sizeof(float);
 }
 
@@ -184,24 +172,11 @@ int fno_lift_fwd(const float* inputs, const float* mask, const float* case_param
 
 int fno_spectral_dft_fwd(const void* act_in, void* xm, int batch, int act_dtype, float s0, float s1, void* stream) {
   if (!act_in || !xm || batch <= 0 || bad_dtype(act_dtype)) return fail(kErrArg, "fno_spectral_dft_fwd: bad argument");
-  if (act_dtype == FNO_ACT_BF16) {
-    // bf16 planes: the two-GEMM tensor-core kernel (fno_dft_fwd_tc.cu); FNO_DFT_TC=0 selects the register-FFT kernel
-    // (an A/B switch for measurements, read once)
-    static const bool use_tc = [] { const char* v = getenv("FNO_DFT_TC"); return !(v && v[0] == '0'); }();
-    if (use_tc) {
-      FNO_CUDA(launch_dft_fwd_tc(act_in, xm, batch, s0, s1, S(stream)), "dft_fwd_tc_kernel");
-      return kOk;
-    }
+  if (act_dtype == FNO_ACT_BF16) {   // bf16 planes: the two-GEMM tensor-core kernel (fno_dft_fwd_tc.cu)
+    FNO_CUDA(launch_dft_fwd_tc(act_in, xm, batch, s0, s1, S(stream)), "dft_fwd_tc_kernel");
+    return kOk;
   }
-  cudaError_t e = act_dtype == FNO_ACT_F32 ? launch_dft_fwd<float>(act_in, xm, batch, s0, s1, S(stream))
-                                           : launch_dft_fwd<__nv_bfloat16>(act_in, xm, batch, s0, s1, S(stream));
-  FNO_CUDA(e, "dft_fwd_kernel");
-  return kOk;
-}
-
-int fno_spectral_dft_fwd_tc(const void* act_in_bf16, void* xm, int batch, float s0, float s1, void* stream) {
-  if (!act_in_bf16 || !xm || batch <= 0) return fail(kErrArg, "fno_spectral_dft_fwd_tc: bad argument");
-  FNO_CUDA(launch_dft_fwd_tc(act_in_bf16, xm, batch, s0, s1, S(stream)), "dft_fwd_tc_kernel");
+  FNO_CUDA(launch_dft_fwd(act_in, xm, batch, s0, s1, S(stream)), "dft_fwd_kernel");
   return kOk;
 }
 
@@ -327,58 +302,6 @@ int fno_rollout_host(const fno_weights* w, const float* inputs_host, const float
   return kOk;
 }
 
-// One step for host buffers as a three-stage pipeline over batch chunks: all host->device copies go, in chunk order,
-// through ONE stream, the kernels of the chunks through a second one and the device->host copies through a third,
-// chained by events.  Copies of the same direction therefore never run concurrently, while chunk c+1's upload still
-// overlaps chunk c's kernels and chunk c-1's download (0.88 ms per step at B = 256 with two chunks, 0.97 ms unchunked).
-int fno_rollout_host_chunked(const fno_weights* w, const float* inputs_host, const float* mask_host,
-                             const float* case_params_host, float* preds_host, const fno_workspace* ws_chunks,
-                             void* const* dev_io_chunks, int batch, int n_chunks, int act_dtype, void* stream_in,
-                             void* stream_compute, void* stream_out) {
-  constexpr int kMaxChunks = 16;
-  if (!w || !inputs_host || !mask_host || !preds_host || !ws_chunks || !dev_io_chunks || batch <= 0 || n_chunks <= 0 ||
-      n_chunks > kMaxChunks || batch % n_chunks != 0)
-    return fail(kErrArg, "fno_rollout_host_chunked: bad argument");
-  auto& ev = g_chunk_events;
-  int dev = 0;
-  FNO_CUDA(cudaGetDevice(&dev), "cudaGetDevice");
-  if (dev < 0 || dev >= 64) return fail(kErrArg, "fno_rollout_host_chunked: device index");
-  for (int c = 0; c < n_chunks; ++c)
-    for (int k = 0; k < 2; ++k)
-      if (!ev[dev][k][c]) FNO_CUDA(cudaEventCreateWithFlags(&ev[dev][k][c], cudaEventDisableTiming), "cudaEventCreate");
-  const size_t cb = static_cast<size_t>(batch / n_chunks);
-  const int p = w->n_case_params;
-  cudaStream_t s_in = S(stream_in), s_cmp = S(stream_compute), s_out = S(stream_out);
-  auto d_in = [&](int c) { return static_cast<float*>(dev_io_chunks[c]); };
-  auto d_mask = [&](int c) { return d_in(c) + cb * 2 * kHW; };
-  auto d_seq = [&](int c) { return d_mask(c) + cb * kHW; };
-  auto d_params = [&](int c) { return d_seq(c) + cb * 2 * kHW; };
-  for (int c = 0; c < n_chunks; ++c) {
-    const size_t lo = c * cb;
-    FNO_CUDA(cudaMemcpyAsync(d_in(c), inputs_host + lo * 2 * kHW, cb * 2 * kHW * sizeof(float), cudaMemcpyHostToDevice, s_in),
-             "H2D inputs");
-    FNO_CUDA(cudaMemcpyAsync(d_mask(c), mask_host + lo * kHW, cb * kHW * sizeof(float), cudaMemcpyHostToDevice, s_in),
-             "H2D mask");
-    if (p > 0)
-      FNO_CUDA(cudaMemcpyAsync(d_params(c), case_params_host + lo * p, cb * p * sizeof(float), cudaMemcpyHostToDevice, s_in),
-               "H2D case_params");
-    FNO_CUDA(cudaEventRecord(ev[dev][0][c], s_in), "cudaEventRecord");
-  }
-  for (int c = 0; c < n_chunks; ++c) {
-    FNO_CUDA(cudaStreamWaitEvent(s_cmp, ev[dev][0][c], 0), "cudaStreamWaitEvent");
-    FNO_TRY(fno_rollout(w, d_in(c), d_mask(c), d_params(c), d_seq(c), 1, &ws_chunks[c], static_cast<int>(cb), act_dtype,
-                        stream_compute));
-    FNO_CUDA(cudaEventRecord(ev[dev][1][c], s_cmp), "cudaEventRecord");
-  }
-  for (int c = 0; c < n_chunks; ++c) {
-    FNO_CUDA(cudaStreamWaitEvent(s_out, ev[dev][1][c], 0), "cudaStreamWaitEvent");
-    FNO_CUDA(cudaMemcpyAsync(preds_host + c * cb * 2 * kHW, d_seq(c), cb * 2 * kHW * sizeof(float), cudaMemcpyDeviceToHost,
-                             s_out),
-             "D2H preds");
-  }
-  return kOk;
-}
-
 int fno_forward_train(const fno_weights* w, const float* inputs, const float* mask, const float* case_params,
                       float* preds, const fno_train_saved* saved, const fno_workspace* ws, int batch,
                       int act_dtype, void* stream) {
@@ -397,7 +320,7 @@ int fno_forward_train(const fno_weights* w, const float* inputs, const float* ma
   return fno_project_fwd(saved->act[w->n_layers], mask, w, preds, batch, act_dtype, stream);
 }
 
-// The backward pass behind fno_backward, fno_backward_ex and fno_backward_inputs.  g == NULL: no parameter gradients --
+// The backward pass behind fno_backward and fno_backward_inputs.  g == NULL: no parameter gradients --
 // every weight-gradient launch (the reduce_partials / chan_outer of fc1, fc2 and w0, spectral_wgrad,
 // unpack_spectral_grads, lift_bwd) is skipped and only the data path runs.  d_inputs / d_case_params (either may be NULL)
 // receive the lift's data adjoint of dL/da0 (lift_bwd_data_kernel); with both NULL and g set, the launches are exactly
@@ -405,7 +328,7 @@ int fno_forward_train(const fno_weights* w, const float* inputs, const float* ma
 static int backward_impl(const char* what, const fno_weights* w, const fno_weights_bwd* wb, const float* inputs,
                          const float* mask, const float* case_params, const float* dpreds, const fno_train_saved* saved,
                          const fno_grads* g, const fno_bwd_scratch* sc, const fno_workspace* ws, int batch, int act_dtype,
-                         void* stream, void* const* seg_events, float* d_inputs, float* d_case_params) {
+                         void* stream, float* d_inputs, float* d_case_params) {
   char msg[128];
   if (!w || !wb || !inputs || !mask || !dpreds || !saved || !sc || !ws || batch <= 0 || bad_dtype(act_dtype)) {
     snprintf(msg, sizeof(msg), "%s: bad argument", what);
@@ -423,7 +346,7 @@ static int backward_impl(const char* what, const fno_weights* w, const fno_weigh
   // over batch chunks / launches: clear them first.
   float* part_co = sc->partials;                                   // chan_outer: up to 296 rows x (128*32 + 128)
   float* part_pb = part_co + static_cast<size_t>(296) * (kProj * kC + kProj);   // project_bwd: 16 * chunk rows x 386
-  float* part_lb = part_pb + static_cast<size_t>(project_bwd_parts(FNO_BWD_CHUNK)) * project_bwd_row();   // lift_bwd
+  float* part_lb = part_pb + static_cast<size_t>(project_bwd_rows_max()) * project_bwd_row();   // lift_bwd
   // no memsets: every gradient is WRITTEN by its (first) reduction -- reduce_partials with accumulate = 0,
   // lift_bwd_reduce, unpack_spectral_grads -- and only further batch chunks of the project stage accumulate
   // ---- project backward (batch chunks bound the dz1 scratch) -> d[0] = dpre_{L-1}
@@ -435,22 +358,14 @@ static int backward_impl(const char* what, const fno_weights* w, const fno_weigh
     float* dout = sc->d[0] + static_cast<size_t>(b0) * kC * kHW;
     const float* dp = dpreds + static_cast<size_t>(b0) * 2 * kHW;
     const float* mk = mask + static_cast<size_t>(b0) * kHW;
-    // the tensor-core kernel (fno_project_bwd_tc.cu); FNO_PBWD_TC=0 selects the CUDA-core kernel (A/B measurements)
-    static const bool use_tc = [] { const char* v = getenv("FNO_PBWD_TC"); return !(v && v[0] == '0'); }();
-    int rows = project_bwd_parts(nb);
-    const int rs = project_bwd_row();
-    cudaError_t e;
-    if (use_tc) {
-      e = bf ? launch_project_bwd_tc<__nv_bfloat16>(a_l, dp, mk, pre, w->fc1_w, w->fc1_b, w->fc2_w, dout, sc->dz1, part_pb, &rows, nb, st)
-             : launch_project_bwd_tc<float>(a_l, dp, mk, pre, w->fc1_w, w->fc1_b, w->fc2_w, dout, sc->dz1, part_pb, &rows, nb, st);
-    } else {
-      e = bf ? launch_project_bwd<__nv_bfloat16>(a_l, dp, mk, pre, w->fc1_w, w->fc1_b, w->fc2_w, dout, sc->dz1, part_pb, nb, st)
-             : launch_project_bwd<float>(a_l, dp, mk, pre, w->fc1_w, w->fc1_b, w->fc2_w, dout, sc->dz1, part_pb, nb, st);
-    }
-    FNO_CUDA(e, "project_bwd_kernel");
+    int rows = 0;
+    cudaError_t e =
+        bf ? launch_project_bwd_tc<__nv_bfloat16>(a_l, dp, mk, pre, w->fc1_w, w->fc1_b, w->fc2_w, dout, sc->dz1, part_pb, &rows, nb, st)
+           : launch_project_bwd_tc<float>(a_l, dp, mk, pre, w->fc1_w, w->fc1_b, w->fc2_w, dout, sc->dz1, part_pb, &rows, nb, st);
+    FNO_CUDA(e, "project_bwd_tc_kernel");
     if (!g) continue;   // data-only: the partial rows just written are never reduced
     const int accum = b0 > 0 ? 1 : 0;
-    FNO_CUDA(launch_reduce_partials(part_pb, rows, rs, g->fc2_w, 2 * kProj, g->fc1_b, kProj, g->fc2_b, 2, accum, st),
+    FNO_CUDA(launch_reduce_partials(part_pb, rows, project_bwd_row(), g->fc2_w, 2 * kProj, g->fc1_b, kProj, g->fc2_b, 2, accum, st),
              "reduce(fc2.weight | fc1.bias | fc2.bias)");
     int n_co = 0;
     e = bf ? launch_chan_outer<float, __nv_bfloat16, 128, 32>(sc->dz1, a_l, part_co, &n_co, nb, st)
@@ -459,11 +374,6 @@ static int backward_impl(const char* what, const fno_weights* w, const fno_weigh
     FNO_CUDA(launch_reduce_partials(part_co, n_co, kProj * kC + kProj, g->fc1_w, kProj * kC, nullptr, 0, nullptr, 0, accum, st),
              "reduce(fc1.weight)");
   }
-  auto mark = [&](int seg) -> cudaError_t {   // the gradients of segment `seg` are final from here on (stream order)
-    if (seg_events == nullptr || seg_events[seg] == nullptr) return cudaSuccess;
-    return cudaEventRecord(static_cast<cudaEvent_t>(seg_events[seg]), st);
-  };
-  FNO_CUDA(mark(0), "cudaEventRecord(fc1/fc2 gradients)");
   // ---- Fourier blocks, last to first
   const float inv = 1.f / static_cast<float>(kHW);
   int cur = 0;
@@ -483,7 +393,6 @@ static int backward_impl(const char* what, const fno_weights* w, const fno_weigh
       FNO_CUDA(launch_spectral_wgrad(saved->xm[l], sc->gm, sc->gwk, batch, st), "spectral_wgrad_kernel");
       FNO_TRY(fno_unpack_spectral_grads(sc->gwk, g->spec_w1[l], g->spec_w2[l], stream));
     }
-    FNO_CUDA(mark(1 + (L - 1 - l)), "cudaEventRecord(block gradients)");
     FNO_TRY(fno_mode_mix(sc->gm, wb->spec_wkT[l], ws->ym, batch, stream));
     FNO_TRY(fno_spectral_inv_kx(ws->ym, ws->z, batch, 1.f, 1.f, stream));
     FNO_TRY(fno_block_out(l > 0 ? FNO_EPI_MUL_DGELU : FNO_EPI_PLAIN, ws->z, dpre, wb->w0[l], nullptr, dnext, nullptr,
@@ -494,7 +403,6 @@ static int backward_impl(const char* what, const fno_weights* w, const fno_weigh
   if (g)
     FNO_CUDA(launch_lift_bwd(sc->d[cur], inputs, mask, case_params, w->gx, w->gy, g->fc0_w, g->fc0_b, part_lb, batch, p, st),
              "lift_bwd_kernel");
-  FNO_CUDA(mark(L + 1), "cudaEventRecord(fc0 gradients)");
   if (d_inputs || d_case_params)
     FNO_CUDA(launch_lift_bwd_data(sc->d[cur], w->fc0_w, d_inputs, d_case_params, batch, p, st), "lift_bwd_data_kernel");
   return kOk;
@@ -504,30 +412,22 @@ int fno_backward(const fno_weights* w, const fno_weights_bwd* wb, const float* i
                  const float* case_params, const float* dpreds, const fno_train_saved* saved,
                  const fno_grads* g, const fno_bwd_scratch* sc, const fno_workspace* ws, int batch,
                  int act_dtype, void* stream) {
-  return fno_backward_ex(w, wb, inputs, mask, case_params, dpreds, saved, g, sc, ws, batch, act_dtype, stream, nullptr);
-}
-
-int fno_backward_ex(const fno_weights* w, const fno_weights_bwd* wb, const float* inputs, const float* mask,
-                    const float* case_params, const float* dpreds, const fno_train_saved* saved,
-                    const fno_grads* g, const fno_bwd_scratch* sc, const fno_workspace* ws, int batch,
-                    int act_dtype, void* stream, void* const* seg_events) {
   if (!g) return fail(kErrArg, "fno_backward: bad argument");
   return backward_impl("fno_backward", w, wb, inputs, mask, case_params, dpreds, saved, g, sc, ws, batch, act_dtype, stream,
-                       seg_events, nullptr, nullptr);
+                       nullptr, nullptr);
 }
 
 int fno_backward_inputs(const fno_weights* w, const fno_weights_bwd* wb, const float* inputs, const float* mask,
                         const float* case_params, const float* dpreds, const fno_train_saved* saved,
                         const fno_grads* grads, const fno_bwd_scratch* scratch, const fno_workspace* ws,
-                        float* d_inputs, float* d_case_params, int batch, int act_dtype, void* stream,
-                        void* const* seg_events) {
+                        float* d_inputs, float* d_case_params, int batch, int act_dtype, void* stream) {
   if (w && (w->n_case_params < 0 || w->n_case_params > kMaxCaseParams))
     return fail(kErrArg, "fno_backward_inputs: n_case_params out of range");
   if (w && w->n_case_params == 0) d_case_params = nullptr;   // nothing to write
   if (!grads && !d_inputs && !d_case_params) return fail(kErrArg, "fno_backward_inputs: no output requested");
   if ((reinterpret_cast<uintptr_t>(d_inputs) & 15) != 0) return fail(kErrArg, "fno_backward_inputs: d_inputs must be 16-byte aligned");
   return backward_impl("fno_backward_inputs", w, wb, inputs, mask, case_params, dpreds, saved, grads, scratch, ws, batch,
-                       act_dtype, stream, seg_events, d_inputs, d_case_params);
+                       act_dtype, stream, d_inputs, d_case_params);
 }
 
 int fno_multistep_metrics(const float* preds_seq, const float* label_u, const float* mask, float* sums, int steps,
@@ -743,7 +643,7 @@ int fno_grid_forward_train(const fno_weights* w, const float* inputs, const floa
 int fno_grid_backward(const fno_weights* w, const fno_weights_bwd* wb, const float* inputs, const float* mask,
                       const float* case_params, const float* dpreds, const fno_train_saved* saved, const fno_grads* g,
                       const fno_bwd_scratch* sc, const fno_workspace* ws, float* d_inputs, float* d_case_params, int batch,
-                      int h, int wd, void* stream, void* const* seg_events) {
+                      int h, int wd, void* stream) {
   FNO_TRY(grid_arg("fno_grid_backward", h, wd));
   if (!w || !wb || !inputs || !mask || !dpreds || !saved || !sc || !ws || batch <= 0)
     return fail(kErrArg, "fno_grid_backward: bad argument");
@@ -756,15 +656,10 @@ int fno_grid_backward(const fno_weights* w, const fno_weights_bwd* wb, const flo
     return fail(kErrArg, "fno_grid_backward: null scratch buffer");
   cudaStream_t st = S(stream);
   const int L = w->n_layers, p = w->n_case_params;
-  auto mark = [&](int seg) -> cudaError_t {
-    if (seg_events == nullptr || seg_events[seg] == nullptr) return cudaSuccess;
-    return cudaEventRecord(static_cast<cudaEvent_t>(seg_events[seg]), st);
-  };
   // ---- projection -> d[0] = dpre_{L-1}
   FNO_TRY(grid_project_bwd_impl(static_cast<const float*>(saved->act[L]), dpreds, mask, saved->pre[L - 1], w, sc->d[0], sc->dz1,
                                 sc->partials, g ? g->fc1_w : nullptr, g ? g->fc1_b : nullptr, g ? g->fc2_w : nullptr,
                                 g ? g->fc2_b : nullptr, batch, h, wd, st));
-  FNO_CUDA(mark(0), "cudaEventRecord(fc1/fc2 gradients)");
   // ---- Fourier blocks, last to first
   float* part_co = sc->partials + grid_partials_offset_co();
   const float inv = 1.f / static_cast<float>(h * wd);
@@ -784,7 +679,6 @@ int fno_grid_backward(const fno_weights* w, const fno_weights_bwd* wb, const flo
       FNO_CUDA(launch_spectral_wgrad(saved->xm[l], sc->gm, sc->gwk, batch, st), "spectral_wgrad_kernel");
       FNO_TRY(fno_unpack_spectral_grads(sc->gwk, g->spec_w1[l], g->spec_w2[l], stream));
     }
-    FNO_CUDA(mark(1 + (L - 1 - l)), "cudaEventRecord(block gradients)");
     FNO_TRY(fno_mode_mix(sc->gm, wb->spec_wkT[l], ws->ym, batch, stream));
     FNO_TRY(fno_grid_spectral_inv_kx(ws->ym, static_cast<float*>(ws->z), batch, h, wd, 1.f, 1.f, stream));
     FNO_TRY(fno_grid_block_out(l > 0 ? FNO_EPI_MUL_DGELU : FNO_EPI_PLAIN, static_cast<const float*>(ws->z), dpre, wb->w0[l],
@@ -802,7 +696,6 @@ int fno_grid_backward(const fno_weights* w, const fno_weights_bwd* wb, const flo
     FNO_CUDA(launch_reduce_partials(part_lb, grid_lift_bwd_parts(batch), grid_lift_bwd_row(), g->fc0_w, kC * (5 + p), g->fc0_b,
                                     kC, nullptr, 0, 0, st),
              "reduce(fc0.weight | fc0.bias)");
-  FNO_CUDA(mark(L + 1), "cudaEventRecord(fc0 gradients)");
   return kOk;
 }
 

@@ -2,10 +2,7 @@
 // Fno2d.forward when train_auto.py:255 calls loss["nmse"].backward()).  The data-gradient path of a
 // Fourier block reuses the forward kernels (K1 with the c_ky/4096 output scale, K2 with the
 // conj-transposed weight pack, K3 with W0 un-transposed and the MUL_DGELU / PLAIN epilogues); this
-// file holds what is new in the backward direction:
-//   project_bwd_kernel   d(fc1,GELU,fc2,mask): recomputes the 128-wide hidden layer per pixel, emits
-//                        dpre of the last block (or d a_L), dz1 for the fc1 weight gradient, and the
-//                        fc2 / bias gradients
+// file holds what is new in the backward direction besides the project stage's (fno_project_bwd_tc.cu):
 //   chan_outer_kernel    G[j][i] += sum_{b,pix} P[b][j][pix] Q[b][i][pix]  (1x1-conv weight gradients)
 //   spectral_wgrad_kernel  gWk[k][i][o] = sum_b conj(X[b][k][i]) G[b][k][o]   (SURVEY.md 8a)
 //   lift_bwd_kernel      gradients of fc0 (spatial feature columns + folded per-sample constants)
@@ -19,21 +16,6 @@ __device__ __forceinline__ float warp_sum(float v) {
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
 }
-
-// GELU and its derivative sharing one erfc evaluation
-__device__ __forceinline__ void gelu_both(float x, float& g, float& dg) {
-  const float ax = fabsf(x);
-  const float e = 0.5f * erfc_abs_scaled(ax);  // 0.5 erfc(|x|/sqrt2)
-  g = fmaxf(x, 0.f) - ax * e;
-  const float cdf = x >= 0.f ? 1.f - e : e;
-  const float pdf = 0.3989422804014327f * ex2_approx(-0.7213475204444817f * x * x);
-  dg = fmaf(x, pdf, cdf);
-}
-
-// ------------------------------------------------------------------------------------ project bwd
-constexpr int kPbThreads = 128;
-constexpr int kPbPix = 256;
-constexpr int kPbOut = 3 * kProj + 2;   // per-CTA partial row: g_w2 (2 x 128) | g_b1 (128) | g_b2 (2)
 
 // out[i] += sum over parts of partial[part][i] in a FIXED order: the second, deterministic half of every small-gradient
 // reduction (the first half = one plain store per CTA).  Replaces float atomics, whose summation order -- and therefore the
@@ -84,167 +66,6 @@ cudaError_t launch_reduce_partials(const float* partial, int n_parts, int row_st
   reduce_partials_kernel<<<(n_out + 31) / 32, 1024, 0, stream>>>(partial, n_parts, row_stride, seg);
   return cudaGetLastError();
 }
-
-template <typename TAct>
-struct PbSmem {
-  alignas(128) TAct xs[kC][kPbPix];
-  alignas(16) float w1[kProj][kC];
-  alignas(16) float b1[kProj];
-  alignas(16) float w2[2][kProj];
-  alignas(16) float acc[kPbThreads / 32][3][kProj];   // per-warp partials of (g_w2[0][j], g_w2[1][j], g_b1[j]): fixed order
-  alignas(16) float acc_b2[kPbThreads / 32][2];
-  alignas(8) uint64_t bar;
-};
-
-template <typename TAct>
-__global__ void __launch_bounds__(kPbThreads)
-    project_bwd_kernel(const TAct* __restrict__ a,        // [B][32][4096]  a_L
-                       const float* __restrict__ dpreds,  // [B][2][4096]
-                       const float* __restrict__ mask,    // [B][4096]
-                       const float* __restrict__ pre,     // [B][32][4096] pre-activation of the last block (or null)
-                       const float* __restrict__ w1, const float* __restrict__ b1, const float* __restrict__ w2,
-                       float* __restrict__ d_out,         // [B][32][4096]: dpre_{L-1} (pre != null) or d a_L
-                       float* __restrict__ dz1,           // [B][128][4096]
-                       float* __restrict__ partial) {   // [CTA][kPbOut]: (g_w2 256 | g_b1 128 | g_b2 2), reduced in CTA order
-  extern __shared__ __align__(128) unsigned char smem_raw[];
-  PbSmem<TAct>& sm = *reinterpret_cast<PbSmem<TAct>*>(smem_raw);
-  const int tid = threadIdx.x, lane = tid & 31;
-  const int b = blockIdx.y;
-  const int pix0 = blockIdx.x * kPbPix;
-
-  if (tid == 0) {
-    mbar_init(&sm.bar, 1);
-    fence_mbar_init();
-  }
-  __syncthreads();
-  if (tid < kC) {
-    constexpr uint32_t bytes = kPbPix * sizeof(TAct);
-    if (tid == 0) mbar_expect_tx(&sm.bar, kC * bytes);
-    __syncwarp();
-    bulk_g2s(&sm.xs[tid][0], a + (static_cast<size_t>(b) * kC + tid) * kHW + pix0, bytes, &sm.bar);
-  }
-  for (int i = tid; i < kProj * kC; i += kPbThreads) (&sm.w1[0][0])[i] = w1[i];
-  for (int j = tid; j < kProj; j += kPbThreads) {
-    sm.b1[j] = b1[j];
-    sm.w2[0][j] = w2[j];
-    sm.w2[1][j] = w2[kProj + j];
-  }
-  __syncthreads();
-  mbar_wait(&sm.bar, 0);
-
-  const int pix = pix0 + 2 * tid;
-  float2 x[kC], da[kC];
-#pragma unroll
-  for (int i = 0; i < kC; ++i) {
-    if constexpr (sizeof(TAct) == 4) {
-      x[i] = *reinterpret_cast<const float2*>(&sm.xs[i][2 * tid]);
-    } else {
-      const uint32_t v = *reinterpret_cast<const uint32_t*>(&sm.xs[i][2 * tid]);
-      x[i] = make_float2(__uint_as_float(v << 16), __uint_as_float(v & 0xffff0000u));
-    }
-    da[i] = make_float2(0.f, 0.f);
-  }
-  const float2 m = *reinterpret_cast<const float2*>(mask + static_cast<size_t>(b) * kHW + pix);
-  float2 d0 = *reinterpret_cast<const float2*>(dpreds + (static_cast<size_t>(b) * 2 + 0) * kHW + pix);
-  float2 d1 = *reinterpret_cast<const float2*>(dpreds + (static_cast<size_t>(b) * 2 + 1) * kHW + pix);
-  d0.x *= m.x; d0.y *= m.y; d1.x *= m.x; d1.y *= m.y;
-
-  float* dz_b = dz1 + static_cast<size_t>(b) * kProj * kHW + pix;
-#pragma unroll 1
-  for (int j = 0; j < kProj; ++j) {
-    float wr[kC];
-    const float4* wrow = reinterpret_cast<const float4*>(&sm.w1[j][0]);
-#pragma unroll
-    for (int q = 0; q < kC / 4; ++q) {
-      const float4 t = wrow[q];
-      wr[4 * q] = t.x; wr[4 * q + 1] = t.y; wr[4 * q + 2] = t.z; wr[4 * q + 3] = t.w;
-    }
-    const float bj = sm.b1[j];
-    float2 z0 = make_float2(bj, bj), z1 = make_float2(0.f, 0.f);
-#pragma unroll
-    for (int i = 0; i < kC; i += 2) {
-      z0 = ffma2(x[i], make_float2(wr[i], wr[i]), z0);
-      z1 = ffma2(x[i + 1], make_float2(wr[i + 1], wr[i + 1]), z1);
-    }
-    const float2 z = make_float2(z0.x + z1.x, z0.y + z1.y);
-    float gx_, gy_, dgx, dgy;
-    gelu_both(z.x, gx_, dgx);
-    gelu_both(z.y, gy_, dgy);
-    const float w20 = sm.w2[0][j], w21 = sm.w2[1][j];
-    const float2 dz = make_float2((w20 * d0.x + w21 * d1.x) * dgx, (w20 * d0.y + w21 * d1.y) * dgy);
-#pragma unroll
-    for (int i = 0; i < kC; ++i) da[i] = ffma2(make_float2(wr[i], wr[i]), dz, da[i]);
-    *reinterpret_cast<float2*>(dz_b + static_cast<size_t>(j) * kHW) = dz;
-    // fc2 weight gradient and fc1 bias gradient: warp partials -> smem accumulators
-    const float p0 = warp_sum(d0.x * gx_ + d0.y * gy_);
-    const float p1 = warp_sum(d1.x * gx_ + d1.y * gy_);
-    const float pb = warp_sum(dz.x + dz.y);
-    if (lane == 0) {   // no atomics anywhere in the gradient path: every slot has one writer, every sum a fixed order
-      sm.acc[tid >> 5][0][j] = p0;
-      sm.acc[tid >> 5][1][j] = p1;
-      sm.acc[tid >> 5][2][j] = pb;
-    }
-  }
-  // fc2 bias gradient
-  {
-    const float s0 = warp_sum(d0.x + d0.y), s1 = warp_sum(d1.x + d1.y);
-    if (lane == 0) {
-      sm.acc_b2[tid >> 5][0] = s0;
-      sm.acc_b2[tid >> 5][1] = s1;
-    }
-  }
-  // d a_L (optionally times GELU'(pre_{L-1}))
-  const size_t base = static_cast<size_t>(b) * kC * kHW + pix;
-#pragma unroll
-  for (int i = 0; i < kC; ++i) {
-    float2 v = da[i];
-    if (pre != nullptr) {
-      const float2 pv = *reinterpret_cast<const float2*>(pre + base + static_cast<size_t>(i) * kHW);
-      v.x *= dgelu_erf(pv.x);
-      v.y *= dgelu_erf(pv.y);
-    }
-    *reinterpret_cast<float2*>(d_out + base + static_cast<size_t>(i) * kHW) = v;
-  }
-  __syncthreads();
-  float* prow = partial + (static_cast<size_t>(blockIdx.y) * gridDim.x + blockIdx.x) * kPbOut;
-  for (int j = tid; j < kProj; j += kPbThreads) {
-    float t0 = 0.f, t1 = 0.f, t2 = 0.f;
-#pragma unroll
-    for (int w = 0; w < kPbThreads / 32; ++w) { t0 += sm.acc[w][0][j]; t1 += sm.acc[w][1][j]; t2 += sm.acc[w][2][j]; }
-    prow[j] = t0;
-    prow[kProj + j] = t1;
-    prow[2 * kProj + j] = t2;
-  }
-  if (tid < 2) {
-    float t = 0.f;
-#pragma unroll
-    for (int w = 0; w < kPbThreads / 32; ++w) t += sm.acc_b2[w][tid];
-    prow[3 * kProj + tid] = t;
-  }
-}
-
-template <typename TAct>
-cudaError_t launch_project_bwd(const void* a, const float* dpreds, const float* mask, const float* pre,
-                               const float* w1, const float* b1, const float* w2, float* d_out, float* dz1,
-                               float* partial, int batch, cudaStream_t stream) {
-  auto kern = project_bwd_kernel<TAct>;
-  constexpr size_t smem = sizeof(PbSmem<TAct>);
-  static PerDeviceLaunch pd;
-  cudaError_t e0 = per_device_setup(kern, smem, pd);
-  if (e0 != cudaSuccess) return e0;
-  dim3 grid(kHW / kPbPix, batch);
-  kern<<<grid, kPbThreads, smem, stream>>>(static_cast<const TAct*>(a), dpreds, mask, pre, w1, b1, w2, d_out, dz1,
-                                           partial);
-  return cudaGetLastError();
-}
-int project_bwd_parts(int batch) { return (kHW / kPbPix) * batch; }   // partial rows written by one launch
-int project_bwd_row() { return kPbOut; }
-template cudaError_t launch_project_bwd<float>(const void*, const float*, const float*, const float*, const float*,
-                                               const float*, const float*, float*, float*, float*,
-                                               int, cudaStream_t);
-template cudaError_t launch_project_bwd<__nv_bfloat16>(const void*, const float*, const float*, const float*,
-                                                       const float*, const float*, const float*, float*, float*,
-                                                       float*, int, cudaStream_t);
 
 // ------------------------------------------------------------------------------------- chan outer
 // out[j][i] += sum_{b,pix} P[b][j][pix] * Q[b][i][pix];   rowsum[j] += sum_{b,pix} P[b][j][pix]

@@ -1,4 +1,5 @@
-// K1 -- truncated forward 2-D DFT of activation planes: x[b][c][64][64] -> Xm[b][k][c] (288 modes).
+// K1 -- truncated forward 2-D DFT of fp32 planes: x[b][c][64][64] -> Xm[b][k][c] (288 modes).  Runs the fp32-storage
+// forward and every gradient plane of the backward; bf16 planes go through dft_fwd_tc_kernel (fno_dft_fwd_tc.cu).
 //
 // Replaces torch.fft.rfft2 + the two corner slices of the reference
 // (src/models/fno/fno2d.py:62,73-78): only kx in {0..11, 52..63} x ky in {0..11} is ever used, so
@@ -12,18 +13,17 @@
 // j is warp-uniform so the four codelets do not diverge.  X[64-kx', ky] = conj(F[kx'][-ky]).
 #include "fft_codelets.cuh"
 #include "fno_common.cuh"
-#include <stdlib.h>
 
 namespace fno {
 
 constexpr int kDftPlanes = 2;     // planes per CTA (small CTAs: 4-5 resident per SM hide each other's TMA wait)
+constexpr int kDftMinBlocks = 4;  // resident CTAs per SM the kernel is compiled for
 constexpr int kDftThreads = 128;  // 64 columns x 2 planes
 constexpr int kDftRows = kDftPlanes * 13;
 constexpr int kDftRowPitch = 65;  // float2 elements; +1 keeps stage-2 row gathers conflict-free
 
-template <typename TAct>
 struct DftSmem {
-  alignas(128) TAct xs[kDftPlanes * kHW];
+  alignas(128) float xs[kDftPlanes * kHW];
   alignas(16) float2 as[kDftRows * kDftRowPitch];
   alignas(8) uint64_t bar;
 };
@@ -72,11 +72,10 @@ __device__ __forceinline__ void row_transform_and_emit(const float2* __restrict_
   }
 }
 
-template <typename TAct, int MINB>
-__global__ void __launch_bounds__(kDftThreads, MINB)
-    dft_fwd_kernel(const TAct* __restrict__ x, float2* __restrict__ xm, float s0, float s1) {
+__global__ void __launch_bounds__(kDftThreads, kDftMinBlocks)
+    dft_fwd_kernel(const float* __restrict__ x, float2* __restrict__ xm, float s0, float s1) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
-  DftSmem<TAct>& sm = *reinterpret_cast<DftSmem<TAct>*>(smem_raw);
+  DftSmem& sm = *reinterpret_cast<DftSmem*>(smem_raw);
   const int tid = threadIdx.x;
   const int plane0 = blockIdx.x * kDftPlanes;  // global plane index = b*32 + c
   const int b = plane0 / kC;
@@ -90,7 +89,7 @@ __global__ void __launch_bounds__(kDftThreads, MINB)
   pdl_wait();
   pdl_launch_dependents();
   if (tid == 0) {
-    constexpr uint32_t bytes = kDftPlanes * kHW * sizeof(TAct);
+    constexpr uint32_t bytes = kDftPlanes * kHW * sizeof(float);
     mbar_expect_tx(&sm.bar, bytes);
     bulk_g2s(sm.xs, x + static_cast<size_t>(plane0) * kHW, bytes, &sm.bar);
   }
@@ -100,9 +99,9 @@ __global__ void __launch_bounds__(kDftThreads, MINB)
   {
     const int p = tid >> 6, w = tid & 63;
     float v[64], ore[13], oim[13];
-    const TAct* col = sm.xs + p * kHW + w;
+    const float* col = sm.xs + p * kHW + w;
 #pragma unroll
-    for (int h = 0; h < 64; ++h) v[h] = Act<TAct>::ld(col + h * kW);
+    for (int h = 0; h < 64; ++h) v[h] = col[h * kW];
     fno_codelets::rfft64_lo13<float>(v, ore, oim);
     float2* dst = sm.as + (p * 13) * kDftRowPitch + w;
 #pragma unroll
@@ -132,25 +131,14 @@ __global__ void __launch_bounds__(kDftThreads, MINB)
   }
 }
 
-template <typename TAct>
 cudaError_t launch_dft_fwd(const void* x, void* xm, int batch, float s0, float s1, cudaStream_t stream) {
-  static int minb = 0;
-  if (minb == 0) {
-    const char* ev = getenv("FNO_DFT_MINB");   // experiment knob: resident CTAs per SM the kernel is compiled for
-    minb = ev ? atoi(ev) : 4;
-    if (minb < 4 || minb > 6) minb = 4;
-  }
-  auto kern = minb == 4 ? dft_fwd_kernel<TAct, 4> : (minb == 5 ? dft_fwd_kernel<TAct, 5> : dft_fwd_kernel<TAct, 6>);
-  constexpr size_t smem = sizeof(DftSmem<TAct>);
-  static PerDeviceLaunch pd[3];  // per instantiation and compile-time occupancy variant
-  cudaError_t e0 = per_device_setup(kern, smem, pd[minb - 4]);
+  constexpr size_t smem = sizeof(DftSmem);
+  static PerDeviceLaunch pd;
+  cudaError_t e0 = per_device_setup(dft_fwd_kernel, smem, pd);
   if (e0 != cudaSuccess) return e0;
   const int n_ctas = batch * kC / kDftPlanes;
-  return launch_chained(kern, dim3(n_ctas), dim3(kDftThreads), smem, stream, static_cast<const TAct*>(x),
+  return launch_chained(dft_fwd_kernel, dim3(n_ctas), dim3(kDftThreads), smem, stream, static_cast<const float*>(x),
                         static_cast<float2*>(xm), s0, s1);
 }
-
-template cudaError_t launch_dft_fwd<float>(const void*, void*, int, float, float, cudaStream_t);
-template cudaError_t launch_dft_fwd<__nv_bfloat16>(const void*, void*, int, float, float, cudaStream_t);
 
 }  // namespace fno

@@ -26,7 +26,11 @@ constexpr int kQbWG = 2;
 constexpr int kQbThreads = 128 * kQbWG;
 constexpr int kQbM = kW;                        // pixels per tile
 constexpr int kQbTilesPerSample = kH;           // 64
-constexpr int kQbOut = 3 * kProj + 2;           // partial row, same layout as project_bwd_kernel's
+constexpr int kQbOut = 3 * kProj + 2;           // partial row: g_w2 (2 x 128) | g_b1 (128) | g_b2 (2)
+// Partial rows reserved for one launch: 16 per sample of a FNO_BWD_CHUNK batch chunk.  This sizes the caller's partial
+// buffer (fno_bwd_partials_bytes()) and caps the grid; a cap below the SM count would change how many rows
+// reduce_partials adds, and with it the last bits of the fc2.weight / fc1.bias / fc2.bias gradients.
+constexpr int kQbRowsMax = 16 * FNO_BWD_CHUNK;
 constexpr int kQbReps = kQbM * (kC / 4) / 128;  // 4 activation tasks per thread
 constexpr uint32_t kQbLboA = (kQbM / 8) * 128;  // 1024
 constexpr uint32_t kQbLboW1 = (kProj / 8) * 128;   // 2048
@@ -51,7 +55,7 @@ __device__ __forceinline__ float qb_warp_sum(float v) {
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
 }
-// GELU and its derivative sharing one erfc evaluation (same formulas as project_bwd_kernel)
+// GELU and its derivative sharing one erfc evaluation
 __device__ __forceinline__ void qb_gelu_both(float x, float& g, float& dg) {
   const float ax = fabsf(x);
   const float e = 0.5f * erfc_abs_scaled(ax);  // 0.5 erfc(|x|/sqrt2)
@@ -275,7 +279,8 @@ __global__ void __launch_bounds__(kQbThreads, 1)
     prow[3 * kProj + t] = ((sm.red_b2[wg][0][t] + sm.red_b2[wg][1][t]) + sm.red_b2[wg][2][t]) + sm.red_b2[wg][3][t];
 }
 
-int project_bwd_parts(int);
+int project_bwd_rows_max() { return kQbRowsMax; }
+int project_bwd_row() { return kQbOut; }
 
 // returns the number of partial rows written through *n_parts
 template <typename TAct>
@@ -291,8 +296,7 @@ cudaError_t launch_project_bwd_tc(const void* a, const float* dpreds, const floa
   const int n_tiles = batch * kQbTilesPerSample;
   int grid = (n_tiles + kQbWG - 1) / kQbWG;
   if (grid > n_sm) grid = n_sm;
-  const int rows_max = project_bwd_parts(FNO_BWD_CHUNK) / kQbWG;   // the partial rows fit the caller's buffer
-  if (grid > rows_max) grid = rows_max;
+  if (grid > kQbRowsMax / kQbWG) grid = kQbRowsMax / kQbWG;   // the partial rows fit the caller's buffer
   kern<<<grid, kQbThreads, smem, stream>>>(static_cast<const TAct*>(a), dpreds, mask, pre, w1, b1, w2, d_out, dz1, partial, n_tiles);
   *n_parts = grid * kQbWG;
   return cudaGetLastError();

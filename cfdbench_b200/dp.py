@@ -48,23 +48,6 @@ def allreduce_mean_(flat: torch.Tensor, group=None) -> torch.Tensor:
     return flat
 
 
-def allreduce_mean_async(seg: torch.Tensor, group=None):
-    """Start the mean all-reduce of one gradient segment on the CURRENT stream and return a handle whose .wait() makes the
-    then-current stream wait for it.  NCCL averages in the collective (ReduceOp.AVG: no separate division kernel); gloo
-    (CPU tests) has no AVG, so the sum is divided afterwards."""
-    if seg.is_complex():
-        raise TypeError("pass the real view of complex gradients")
-    if dist.get_backend(group) == "nccl":
-        return dist.all_reduce(seg, op=dist.ReduceOp.AVG, group=group, async_op=True)
-    work = dist.all_reduce(seg, op=dist.ReduceOp.SUM, group=group, async_op=True)
-
-    class _Div:
-        def wait(self_inner):
-            work.wait()
-            seg.div_(dist.get_world_size(group))
-    return _Div()
-
-
 def max_over_ranks(value: float, device=None) -> float:
     """Max of a host scalar over all ranks (used for the bench's max-over-ranks timing)."""
     if not dist.is_initialized():

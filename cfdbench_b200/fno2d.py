@@ -20,7 +20,6 @@ every parameter frozen.
 from __future__ import annotations
 
 import ctypes as C
-import os
 from typing import Dict, List, Optional
 
 import numpy as np
@@ -36,6 +35,9 @@ HIDDEN = 32
 MODES = 12
 NMODES = 2 * MODES * MODES  # 288
 PROJ = 128
+# A host-tensor single step of a large batch is cut into this many equal batch chunks, so that one chunk's copies overlap
+# another's kernels.  More chunks run the kernels at batch sizes where their fixed per-launch costs dominate.
+HOST_CHUNKS = 2
 
 
 class SpectralConv2d_fast(nn.Module):
@@ -74,9 +76,9 @@ def _ptr(t: Optional[Tensor]) -> int:
 
 
 class _TrainFn(torch.autograd.Function):
-    """One autograd node for the whole network: forward = fno_forward_train, backward = fno_backward (parameter
-    gradients only) or fno_backward_inputs (also, or only, the gradients w.r.t. inputs / case_params).  Every call keeps
-    its own saved activations, so forward k+1 may run before backward k (unrolled training through rollouts)."""
+    """One autograd node for the whole network: forward = fno_forward_train, backward = fno_backward_inputs (parameter
+    gradients and / or the gradients w.r.t. inputs / case_params).  Every call keeps its own saved activations, so
+    forward k+1 may run before backward k (unrolled training through rollouts)."""
 
     @staticmethod
     def forward(ctx, model: "Fno2d", inputs: Tensor, mask: Tensor, case_params: Tensor, *params: Tensor):
@@ -166,24 +168,12 @@ class Fno2d(AutoCfdModel):
         self._ws_cache: dict = {}
         self._dp_group = None
         self._dp_enabled = False
-        self._dp_events = None
-        self._dp_stream = None
-        # how the flat gradient buffer is all-reduced: "one" collective after backward, "two" (upper half of the network
-        # while the lower half is still in backward) or "all" (one per gradient group); tools/time_train_dp.py compares them
-        self.dp_segments = os.environ.get("FNO_DP_SEGMENTS", "one")
         # CUDA-graph replay of device-resident rollouts: one capture per (batch, steps), the 18 launches of every
         # step replayed as one graph (B=256: 591 -> 544 us/step, B=1: 2.09 -> 1.48 ms per 20 steps).  False = launch
         # every kernel on the stream.
         self.graph_rollout = True
         self.fused_block = True  # bf16 storage, inference: inv_kx + block_tc replaced by block_fused_kernel
         self.max_graphs = 8
-        # host-tensor single step (bench.py's e2e), measured at B=256 bf16 (tools/e2e_sweep.py): staged copies on three
-        # streams over 2 batch chunks 0.753 ms, over 4 chunks 0.842 ms (chunks of 64 run the 14 kernels at their fixed
-        # costs); kernels reading / writing the pinned host buffers directly 0.796 ms (1 chunk) / 0.815 / 0.881 ms
-        self.host_chunks = 2
-        self.host_chunk_plan = None   # e.g. (0.25, 0.75): uneven chunks (short exposed upload, see tools/e2e_sweep.py)
-        self.host_zero_copy = False  # opt-in: lift reads the pinned frame, project writes the pinned result directly
-        self.zero_copy_chunks = 2
         self._graphs: dict = {}
         # True: 64x64 frames in float32 storage also run the grid-generic kernels (fno_grid_*), which cross-checks the two
         # paths; False (default): 64x64 frames run the 64x64 kernels
@@ -474,14 +464,13 @@ class Fno2d(AutoCfdModel):
 
     def _native_backward(self, inputs, mask4, case_params, dpreds, saved_native, want_params: bool = True,
                          d_inputs: Optional[Tensor] = None, d_cp: Optional[Tensor] = None):
-        """Parameter gradients in parameter order (None when `want_params` is false).  Without `d_inputs` / `d_cp` this is
-        fno_backward / fno_backward_ex, the training step of train_auto.py; otherwise fno_backward_inputs also writes
-        dL/dinputs into `d_inputs` and dL/dcase_params into `d_cp`.  Those are per sample: with data parallel enabled
-        only the parameter gradients are all-reduced."""
+        """Parameter gradients in parameter order (None when `want_params` is false), from one native call:
+        fno_backward_inputs on 64x64 frames (with `d_inputs` and `d_cp` None it issues exactly fno_backward's launches),
+        fno_grid_backward on other grids.  It also writes dL/dinputs into `d_inputs` and dL/dcase_params into `d_cp` when
+        given.  Those are per sample: with data parallel enabled only the parameter gradients are all-reduced."""
         if self.n_case_params == 0:
             d_cp = None   # a (B, 0) gradient: nothing to write
-        with_data = d_inputs is not None or d_cp is not None
-        if not want_params and not with_data:
+        if not want_params and d_inputs is None and d_cp is None:
             return None
         lib = _lib.load()
         sv, acts, pres, xms = saved_native
@@ -490,9 +479,9 @@ class Fno2d(AutoCfdModel):
         gh, gw = inputs.shape[-2:]
         grid = self._on_grid_path(gh, gw)
         ws, _ = self._grid_workspace(b, gh, gw) if grid else self._workspace(b)
-        layout, total = self._grad_layout()
         g = None
         if want_params:
+            layout, total = self._grad_layout()
             flat = torch.empty(total, dtype=torch.float32, device=dev)
             views: Dict[str, Tensor] = {}
             for name, p, off, n in layout:
@@ -518,79 +507,22 @@ class Fno2d(AutoCfdModel):
         nbytes = lib.fno_grid_bwd_partials_bytes(gh, gw) if grid else lib.fno_bwd_partials_bytes()
         partials = torch.empty(nbytes, dtype=torch.uint8, device=dev)
         sc.partials = partials.data_ptr()
-
-        def run(events=None):
-            if grid:
-                _lib.check(lib.fno_grid_backward(C.byref(self._grid_struct(pk, gh, gw)), C.byref(pk["struct_bwd"]),
-                                                 inputs.data_ptr(), mask4.data_ptr(), case_params.data_ptr(),
-                                                 dpreds.data_ptr(), C.byref(sv), C.byref(g) if g is not None else None,
-                                                 C.byref(sc), C.byref(ws), _ptr(d_inputs), _ptr(d_cp), b, gh, gw,
-                                                 self._stream(), events), "fno_grid_backward")
-            elif with_data:
-                _lib.check(lib.fno_backward_inputs(C.byref(pk["struct"]), C.byref(pk["struct_bwd"]), inputs.data_ptr(),
-                                                   mask4.data_ptr(), case_params.data_ptr(), dpreds.data_ptr(),
-                                                   C.byref(sv), C.byref(g) if g is not None else None, C.byref(sc),
-                                                   C.byref(ws), _ptr(d_inputs), _ptr(d_cp), b, self._act_code(),
-                                                   self._stream(), events), "fno_backward_inputs")
-            elif events is None:
-                _lib.check(lib.fno_backward(C.byref(pk["struct"]), C.byref(pk["struct_bwd"]), inputs.data_ptr(),
-                                            mask4.data_ptr(), case_params.data_ptr(), dpreds.data_ptr(), C.byref(sv),
-                                            C.byref(g), C.byref(sc), C.byref(ws), b, self._act_code(), self._stream()),
-                           "fno_backward")
-            else:
-                _lib.check(lib.fno_backward_ex(C.byref(pk["struct"]), C.byref(pk["struct_bwd"]), inputs.data_ptr(),
+        g_arg = C.byref(g) if g is not None else None
+        if grid:
+            _lib.check(lib.fno_grid_backward(C.byref(self._grid_struct(pk, gh, gw)), C.byref(pk["struct_bwd"]),
+                                             inputs.data_ptr(), mask4.data_ptr(), case_params.data_ptr(), dpreds.data_ptr(),
+                                             C.byref(sv), g_arg, C.byref(sc), C.byref(ws), _ptr(d_inputs), _ptr(d_cp), b,
+                                             gh, gw, self._stream()), "fno_grid_backward")
+        else:
+            _lib.check(lib.fno_backward_inputs(C.byref(pk["struct"]), C.byref(pk["struct_bwd"]), inputs.data_ptr(),
                                                mask4.data_ptr(), case_params.data_ptr(), dpreds.data_ptr(), C.byref(sv),
-                                               C.byref(g), C.byref(sc), C.byref(ws), b, self._act_code(), self._stream(),
-                                               events), "fno_backward_ex")
-
-        if not want_params:   # data-only backward: no parameter gradients, nothing to all-reduce
-            run()
+                                               g_arg, C.byref(sc), C.byref(ws), _ptr(d_inputs), _ptr(d_cp), b,
+                                               self._act_code(), self._stream()), "fno_backward_inputs")
+        if g is None:   # data-only backward: no parameter gradients, nothing to all-reduce
             return None
-        if not self._dp_enabled or self.dp_segments == "one":
-            run()
-            if self._dp_enabled:   # one all-reduce (NCCL: ReduceOp.AVG, no division kernel) of the whole flat buffer
-                from .dp import allreduce_mean_
-                allreduce_mean_(flat, self._dp_group)
-            return [views[name] for name, _ in self.named_parameters()]
-        # Optional: reduce the flat buffer segment by segment, each as soon as its gradients are final -- the native
-        # backward records one event per segment (fc1/fc2, block L-1 .. block 0, fc0) and a side stream starts the NCCL
-        # all-reduce (ReduceOp.AVG) of that slice while the remaining backward kernels still run on the main stream.
-        # tools/time_train_dp.py compares the modes; the 9.5 MB collective is small next to the extra launches and the SM
-        # contention between NCCL's kernels and the persistent backward kernels, so "one" is the default.
-        from .dp import allreduce_mean_async
-        ends = {name: off + n for name, _p, off, n in layout}
-        starts = {name: off for name, _p, off, n in layout}
-        # (event index, begin, end): event k of fno_backward_ex = fc1/fc2 (0), block L-1 .. block 0 (1..L), fc0 (L+1)
-        mode = self.dp_segments
-        if mode == "all":      # one collective per gradient group, each as early as possible
-            segs = [(0, starts["fc1.weight"], ends["fc2.bias"])]
-            for l in range(L - 1, -1, -1):
-                segs.append((L - l, starts[f"blocks.{l}.conv0.weights1"], ends[f"blocks.{l}.w0.bias"]))
-            segs.append((L + 1, starts["fc0.weight"], ends["fc0.bias"]))
-        elif mode == "two":    # upper half of the network (contiguous tail of the buffer) early, the rest at the end
-            mid = L // 2
-            cut = starts[f"blocks.{mid}.conv0.weights1"]
-            segs = [(L - mid, cut, total), (L + 1, 0, cut)]
-        else:                  # "one": a single all-reduce of the whole buffer after the backward pass
-            segs = [(L + 1, 0, total)]
-        assert sum(e - s_ for _, s_, e in segs) == total   # the segments tile the buffer
-        if self._dp_events is None or len(self._dp_events) != L + 2:
-            self._dp_events = [torch.cuda.Event() for _ in range(L + 2)]
-            self._dp_stream = torch.cuda.Stream(device=dev)
-            for ev in self._dp_events:
-                ev.record()   # creates the underlying cudaEvent_t
-        handles = (C.c_void_p * (L + 2))(*[ev.cuda_event for ev in self._dp_events])
-        main = torch.cuda.current_stream(dev)
-        run(handles)
-        works = []
-        flat.record_stream(self._dp_stream)
-        with torch.cuda.stream(self._dp_stream):
-            for k, s_, e in segs:
-                self._dp_stream.wait_event(self._dp_events[k])
-                works.append(allreduce_mean_async(flat[s_:e], self._dp_group))
-        for wk in works:
-            wk.wait()   # the main stream waits for the collectives
-        main.wait_stream(self._dp_stream)
+        if self._dp_enabled:   # one all-reduce (NCCL: ReduceOp.AVG, no division kernel) of the whole flat buffer
+            from .dp import allreduce_mean_
+            allreduce_mean_(flat, self._dp_group)
         return [views[name] for name, _ in self.named_parameters()]
 
     # -------------------------------------------------------------------------------- public API
@@ -702,49 +634,12 @@ class Fno2d(AutoCfdModel):
         seq.copy_(s_seq)
         return seq
 
-    def _step_host_zero_copy(self, inputs, case_params, mask3, out, pk) -> Tensor:
-        """One step with PINNED host frames and no staging copies: the lift kernel reads the frame straight from host
-        memory and the project kernel writes the prediction straight into the caller's pinned result tensor (unified
-        addressing: a pinned allocation is device-accessible at the same address), so both transfers ride inside the
-        first / last kernel of the step instead of in front of / behind it.  The batch is cut into `zero_copy_chunks`
-        halves on two streams: while one half runs its Fourier blocks the other half's lift (PCIe-bound) runs.  Mask and
-        case parameters stay cached on the device between calls."""
-        lib = _lib.load()
-        b, dev = inputs.shape[0], self.device
-        cur = torch.cuda.current_stream(dev)
-        n_chunks = self.zero_copy_chunks if b % self.zero_copy_chunks == 0 and b // self.zero_copy_chunks >= 8 else 1
-        cb = b // n_chunks
-        key = ("host_zero_copy", b, n_chunks)
-        ent = self._ws_cache.get(key)
-        if ent is None:
-            ent = dict(d_mask=torch.empty(b, 1, H, W, dtype=torch.float32, device=dev),
-                       d_cp=torch.empty(b, max(self.n_case_params, 1), dtype=torch.float32, device=dev),
-                       streams=[torch.cuda.Stream(device=dev) for _ in range(n_chunks)], inv_key=None)
-            self._ws_cache[key] = ent
-        inv_key = (mask3.data_ptr(), mask3._version, case_params.data_ptr(), case_params._version, tuple(mask3.shape))
-        if ent["inv_key"] != inv_key:
-            ent["d_mask"].view(b, H, W).copy_(mask3, non_blocking=True)
-            if self.n_case_params > 0:
-                ent["d_cp"][:, :self.n_case_params].copy_(case_params, non_blocking=True)
-            ent["inv_key"] = inv_key
-        out2 = out.view(b, self.out_chan, H, W)
-        for c, st in enumerate(ent["streams"]):
-            st.wait_stream(cur)
-            ws, _ = self._workspace(cb, slot=1 + c)
-            lo = c * cb
-            _lib.check(lib.fno_forward(C.byref(pk["struct"]), inputs[lo:lo + cb].data_ptr(), ent["d_mask"][lo:lo + cb].data_ptr(),
-                                       ent["d_cp"][lo:lo + cb].data_ptr(), out2[lo:lo + cb].data_ptr(), C.byref(ws), cb,
-                                       self._act_code(), C.c_void_p(st.cuda_stream)), "fno_forward")
-        for st in ent["streams"]:
-            st.synchronize()
-        return out
-
     def _rollout_host(self, inputs: Tensor, case_params: Tensor, mask: Tensor, steps: int) -> Tensor:
         """Host tensors in -> host tensors out; the result is a tensor the caller OWNS (fresh pinned memory from torch's
         caching host allocator, never a view of a reused buffer -- the reference returns fresh tensors too).
 
         Multi-step rollouts run `fno_rollout_host` (H2D, rollout, D2H on one stream).  A single step of a large batch --
-        the per-step host round trip that `bench.py`'s e2e number times -- is cut into `host_chunks` batch chunks whose
+        the per-step host round trip that `bench.py`'s e2e number times -- is cut into HOST_CHUNKS equal batch chunks whose
         uploads, kernels and downloads go through three streams chained by events, so the copies of one chunk overlap the
         kernels of another (the cases are independent).  Each chunk's 14 kernel launches are replayed from a CUDA graph
         (one driver call), and the loop-invariant operands -- mask and case parameters -- stay on the device between
@@ -763,21 +658,7 @@ class Fno2d(AutoCfdModel):
         dev = self.device
         cur = torch.cuda.current_stream(dev)
         out = torch.empty(steps, b, self.out_chan, H, W, dtype=torch.float32, pin_memory=True)
-        if steps == 1 and self.host_zero_copy and inputs.is_pinned() and b >= 8:
-            return self._step_host_zero_copy(inputs, case_params, mask3, out, pk)
-        # chunk plan of a single large step: explicit fractions (host_chunk_plan, e.g. (0.25, 0.75)) or host_chunks equal parts
-        sizes = [b]
-        if steps == 1 and b >= 128:
-            if self.host_chunk_plan is not None:
-                sizes = [int(round(f * b)) for f in self.host_chunk_plan]
-                sizes[-1] = b - sum(sizes[:-1])
-                if min(sizes) < 8:
-                    sizes = [b]
-            elif b % self.host_chunks == 0:
-                sizes = [b // self.host_chunks] * self.host_chunks
-        n_chunks = len(sizes)
-        offs = [sum(sizes[:c]) for c in range(n_chunks)]
-        if n_chunks == 1:
+        if not (steps == 1 and b >= 128 and b % HOST_CHUNKS == 0):
             key = ("host_io", b, steps)
             ent = self._ws_cache.get(key)
             if ent is None:
@@ -792,17 +673,19 @@ class Fno2d(AutoCfdModel):
             cur.synchronize()
             return out
 
-        key = ("host_chunked", b, tuple(sizes), self.act_dtype, self.fused_block)
+        cb = b // HOST_CHUNKS
+        key = ("host_chunked", b, self.act_dtype, self.fused_block)
         ent = self._ws_cache.get(key)
         if ent is None or ent["pk"] is not pk:
             ent = dict(
                 pk=pk,
-                d_in=[torch.empty(cb, self.in_chan, H, W, dtype=torch.float32, device=dev) for cb in sizes],
+                d_in=[torch.empty(cb, self.in_chan, H, W, dtype=torch.float32, device=dev) for _ in range(HOST_CHUNKS)],
                 d_mask=torch.empty(b, 1, H, W, dtype=torch.float32, device=dev),
                 d_cp=torch.empty(b, max(self.n_case_params, 1), dtype=torch.float32, device=dev),
-                d_out=[torch.empty(cb, self.out_chan, H, W, dtype=torch.float32, device=dev) for cb in sizes],
+                d_out=[torch.empty(cb, self.out_chan, H, W, dtype=torch.float32, device=dev) for _ in range(HOST_CHUNKS)],
                 streams=[torch.cuda.Stream(device=dev) for _ in range(3)],
-                ev_in=[torch.cuda.Event() for _ in range(n_chunks)], ev_cmp=[torch.cuda.Event() for _ in range(n_chunks)],
+                ev_in=[torch.cuda.Event() for _ in range(HOST_CHUNKS)],
+                ev_cmp=[torch.cuda.Event() for _ in range(HOST_CHUNKS)],
                 graphs=None, inv_key=None,
             )
             self._ws_cache[key] = ent
@@ -820,15 +703,15 @@ class Fno2d(AutoCfdModel):
             graphs = []
             s_cmp.wait_stream(s_in)
             with torch.cuda.stream(s_cmp):
-                for c in range(n_chunks):
-                    cb, lo = sizes[c], offs[c]
+                for c in range(HOST_CHUNKS):
+                    lo = c * cb
                     ws, _ = self._workspace(cb, slot=1 + c)
                     cp_c = ent["d_cp"][lo:lo + cb]
                     assert cp_c.is_contiguous() or self.n_case_params == 0
                     if self.n_case_params not in (0, ent["d_cp"].shape[1]):
                         raise _lib.FnoNativeError("internal: case-parameter staging width")
 
-                    def run(c=c, ws=ws, cb=cb, lo=lo):
+                    def run(c=c, ws=ws, lo=lo):
                         _lib.check(lib.fno_forward(C.byref(pk["struct"]), ent["d_in"][c].data_ptr(),
                                                    ent["d_mask"][lo:lo + cb].data_ptr(),
                                                    ent["d_cp"][lo:lo + cb].data_ptr(), ent["d_out"][c].data_ptr(),
@@ -847,9 +730,9 @@ class Fno2d(AutoCfdModel):
         out2 = out.view(b, self.out_chan, H, W)
         # issue order = dependency order per chunk (upload, kernels, download): the first chunk's graph launch is already
         # queued when its upload lands (issuing all uploads first put ~20 us of host time on the step's critical path)
-        for c in range(n_chunks):
+        for c in range(HOST_CHUNKS):
             with torch.cuda.stream(s_in):
-                ent["d_in"][c].copy_(inputs[offs[c]:offs[c] + sizes[c]], non_blocking=True)
+                ent["d_in"][c].copy_(inputs[c * cb:(c + 1) * cb], non_blocking=True)
                 ent["ev_in"][c].record(s_in)
             s_cmp.wait_event(ent["ev_in"][c])
             with torch.cuda.stream(s_cmp):
@@ -857,7 +740,7 @@ class Fno2d(AutoCfdModel):
                 ent["ev_cmp"][c].record(s_cmp)
             s_out.wait_event(ent["ev_cmp"][c])
             with torch.cuda.stream(s_out):
-                out2[offs[c]:offs[c] + sizes[c]].copy_(ent["d_out"][c], non_blocking=True)
+                out2[c * cb:(c + 1) * cb].copy_(ent["d_out"][c], non_blocking=True)
         s_out.synchronize()
         return out
 

@@ -35,7 +35,7 @@
 extern "C" {
 #endif
 
-#define FNO_ABI_VERSION 3
+#define FNO_ABI_VERSION 4
 #define FNO_MAX_LAYERS 8
 
 enum { FNO_ACT_F32 = 0, FNO_ACT_BF16 = 1 };
@@ -70,8 +70,8 @@ typedef struct fno_workspace {
 } fno_workspace;
 
 int fno_version(void);
-/* Frees what the library itself owns on the CURRENT device (constant operand tables built on first use, events of the
- * chunked host path); they are rebuilt on demand.  Everything else is caller-owned.  Synchronises the device. */
+/* Frees what the library itself owns on the CURRENT device (constant operand tables built on first use); they are
+ * rebuilt on demand.  Everything else is caller-owned.  Synchronises the device. */
 int fno_destroy(void);
 const char* fno_last_error(void);
 /* bytes of one activation buffer / one mode buffer for batch B */
@@ -99,13 +99,11 @@ int fno_lift_fwd(const float* inputs, const float* mask, const float* case_param
                  void* act_out, int batch, int act_dtype, void* stream);
 
 /* The four phases of SpectralConv2d_fast + FnoBlock (reference fno2d.py:59-82, 106-112):            */
-/* (1) torch.fft.rfft2 restricted to the kept modes (fno2d.py:62,73-78); outputs scaled by s0 (ky=0), s1 (ky>0) */
+/* (1) torch.fft.rfft2 restricted to the kept modes (fno2d.py:62,73-78); outputs scaled by s0 (ky=0), s1 (ky>0).
+ *     fp32 planes: register FFT codelets (fno_dft_fwd.cu); bf16 planes: two chained tensor-core GEMMs
+ *     (fno_dft_fwd_tc.cu: 25 us per launch at B=256 against 35 us for the register-FFT kernel, same 2e-6 against
+ *     float64). */
 int fno_spectral_dft_fwd(const void* act_in, void* xm, int batch, int act_dtype, float s0, float s1, void* stream);
-/* (1') the same transform for bf16 planes as two chained tensor-core GEMMs (fno_dft_fwd_tc.cu, warp-specialised since
- *      round 2: 25 us per launch at B=256 against 35 us for the register-FFT kernel, same 2e-6 against float64).
- *      fno_spectral_dft_fwd(..., FNO_ACT_BF16, ...) routes here (environment FNO_DFT_TC=0 selects the register kernel for
- *      A/B measurements); this entry point calls it directly. */
-int fno_spectral_dft_fwd_tc(const void* act_in_bf16, void* xm, int batch, float s0, float s1, void* stream);
 /* (2) einsum("bixy,ioxy->boxy") on both corners (fno2d.py:54-57,73-78); wop = fno_pack_mix_operand image */
 int fno_mode_mix(const void* xm, const void* wop, void* ym, int batch, void* stream);
 /* (3) first half of irfft2 on the zero-padded spectrum (fno2d.py:65-72,81): inverse C2C along kx of the 24 kept
@@ -147,15 +145,6 @@ int fno_rollout(const fno_weights* w, const float* inputs, const float* mask, co
 int fno_rollout_host(const fno_weights* w, const float* inputs_host, const float* mask_host,
                      const float* case_params_host, float* preds_seq_host, int steps, const fno_workspace* ws,
                      void* dev_io, int batch, int act_dtype, void* stream);
-/* One step (steps = 1) for host buffers, pipelined over n_chunks equal batch chunks: uploads, kernels and downloads
- * run on three caller-provided streams chained by events, so chunk c+1's upload overlaps chunk c's kernels and
- * chunk c-1's download while copies of one direction stay serialised.  ws_chunks / dev_io_chunks: one workspace and
- * one fno_rollout_host_scratch_bytes(batch / n_chunks, p, 1) buffer per chunk.  The caller orders the three streams
- * after its own stream before the call and waits for stream_out afterwards. */
-int fno_rollout_host_chunked(const fno_weights* w, const float* inputs_host, const float* mask_host,
-                             const float* case_params_host, float* preds_host, const fno_workspace* ws_chunks,
-                             void* const* dev_io_chunks, int batch, int n_chunks, int act_dtype, void* stream_in,
-                             void* stream_compute, void* stream_out);
 size_t fno_rollout_host_scratch_bytes(int batch, int n_case_params, int steps);
 
 /* ---------------------------------------------------------------------------------------------------
@@ -210,14 +199,6 @@ int fno_backward(const fno_weights* w, const fno_weights_bwd* wb, const float* i
                  const float* case_params, const float* dpreds, const fno_train_saved* saved,
                  const fno_grads* grads, const fno_bwd_scratch* scratch, const fno_workspace* ws, int batch,
                  int act_dtype, void* stream);
-/* Same, recording CUDA events as gradient segments become final so that the caller can start their all-reduce while
- * the rest of the backward pass still runs (data-parallel training, SURVEY.md 8e): seg_events[0] after the fc1 / fc2
- * gradients, seg_events[1 + i] after the gradients of block (n_layers - 1 - i), seg_events[n_layers + 1] after the fc0
- * gradients.  seg_events = NULL or a NULL entry: nothing recorded there.  Entries are cudaEvent_t. */
-int fno_backward_ex(const fno_weights* w, const fno_weights_bwd* wb, const float* inputs, const float* mask,
-                 const float* case_params, const float* dpreds, const fno_train_saved* saved,
-                 const fno_grads* grads, const fno_bwd_scratch* scratch, const fno_workspace* ws, int batch,
-                 int act_dtype, void* stream, void* const* seg_events);
 /* Same backward, also differentiating w.r.t. the input frame and the case parameters (unrolled training through
  * rollouts, sensitivities / inverse problems with a frozen model; what autograd gives the reference when `inputs` or
  * `case_params` require grad, fno2d.py:195-217):
@@ -225,15 +206,16 @@ int fno_backward_ex(const fno_weights* w, const fno_weights_bwd* wb, const float
  *   d_case_params[b][j]  = sum_o fc0_w[o][5+j] sum_{h,w} dL/da0[b][o][h][w]
  * where a0 is the lift output (a bf16-stored a0 is differentiated straight through).  Both are overwritten and
  * bit-reproducible (fixed-order reductions, no atomics).  grads = NULL skips every parameter-gradient launch (data-only
- * backward, e.g. a frozen model); otherwise `grads` and `seg_events` are filled / recorded as by fno_backward_ex.
- * At least one of grads, d_inputs, d_case_params must be non-NULL; d_inputs must be 16-byte aligned. */
+ * backward, e.g. a frozen model); otherwise `grads` is filled as by fno_backward, and with d_inputs and d_case_params
+ * both NULL the launches are exactly fno_backward's.  At least one of grads, d_inputs, d_case_params must be non-NULL;
+ * d_inputs must be 16-byte aligned. */
 int fno_backward_inputs(const fno_weights* w, const fno_weights_bwd* wb, const float* inputs, const float* mask,
                         const float* case_params, const float* dpreds, const fno_train_saved* saved,
                         const fno_grads* grads,        /* NULL: no parameter gradients (data-only backward) */
                         const fno_bwd_scratch* scratch, const fno_workspace* ws,
                         float* d_inputs,               /* [B][2][64][64] or NULL */
                         float* d_case_params,          /* [B][p] or NULL (must be NULL or unused when p == 0) */
-                        int batch, int act_dtype, void* stream, void* const* seg_events);
+                        int batch, int act_dtype, void* stream);
 
 /* Rollout evaluation on the device (SURVEY.md 8f.1; reference src/test_multistep.py:73-83,153-177 get_metrics on the
  * masked u channel, three .item() syncs per step and case there).  preds_seq [S][B][2][64][64], label_u and mask
@@ -319,11 +301,11 @@ int fno_grid_rollout(const fno_weights* w, const float* inputs, const float* mas
 int fno_grid_forward_train(const fno_weights* w, const float* inputs, const float* mask, const float* case_params,
                            float* preds, const fno_train_saved* saved, const fno_workspace* ws, int batch, int h, int w_,
                            void* stream);
-/* fno_backward_inputs on an H x W grid: grads = NULL gives the data-only backward; seg_events as fno_backward_ex */
+/* fno_backward_inputs on an H x W grid: grads = NULL gives the data-only backward */
 int fno_grid_backward(const fno_weights* w, const fno_weights_bwd* wb, const float* inputs, const float* mask,
                       const float* case_params, const float* dpreds, const fno_train_saved* saved, const fno_grads* grads,
                       const fno_bwd_scratch* scratch, const fno_workspace* ws, float* d_inputs, float* d_case_params,
-                      int batch, int h, int w_, void* stream, void* const* seg_events);
+                      int batch, int h, int w_, void* stream);
 
 #ifdef __cplusplus
 }

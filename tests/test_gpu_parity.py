@@ -146,31 +146,32 @@ def test_mode_mix_and_pack_kernels(lib):
 
 
 @pytest.mark.parametrize("batch", [1, 3, 41])
-def test_dft_fwd_tensor_core_kernel_bf16_storage(lib, batch):
-    """bf16 planes through dft_fwd_tc_kernel (two chained wgmma GEMMs; the forward path of bf16 storage) by its own entry
-    point and through fno_spectral_dft_fwd (which routes bf16 planes to it unless FNO_DFT_TC=0 selects the register-FFT
-    kernel); 41 samples = 328 plane batches, i.e. up to three per persistent CTA (pipeline steady state + ragged tail).
+def test_spectral_dft_fwd_bf16_planes_tensor_core_kernel(lib, batch):
+    """bf16 planes through dft_fwd_tc_kernel (two chained wgmma GEMMs; the forward path of bf16 storage), which
+    fno_spectral_dft_fwd runs for every bf16 plane; 41 samples = 328 plane batches, i.e. up to three per persistent CTA
+    (pipeline steady state + ragged tail).
     The inputs are bf16-exact, so the comparison with the float64 oracle measures the arithmetic only."""
     from cfdbench_b200 import _lib
     rng = np.random.default_rng(10 + batch)
     x = torch.from_numpy(rng.standard_normal((batch, 32, 64, 64)).astype(np.float32)).to(torch.bfloat16)
     xd = x.cuda()
     xm = torch.zeros(288, batch, 32, dtype=torch.complex64, device="cuda")
-    _lib.check(lib.fno_spectral_dft_fwd_tc(xd.data_ptr(), xm.data_ptr(), batch, 1.0, 1.0, stream()), "dft tc")
+    _lib.check(lib.fno_spectral_dft_fwd(xd.data_ptr(), xm.data_ptr(), batch, _lib.ACT_BF16, 1.0, 1.0, stream()), "dft tc")
     xf = x.float().numpy()
     ref = onp.spectral_modes(xf, 12, 12).reshape(batch, 32, 288).transpose(2, 0, 1)
     err = np.linalg.norm(xm.cpu().numpy() - ref) / np.linalg.norm(ref)
     assert err < 2e-6, err
     assert np.abs(xm.cpu().numpy() - ref).max() < 2e-5 * np.abs(ref).max()
     xm2 = torch.zeros_like(xm)
-    _lib.check(lib.fno_spectral_dft_fwd_tc(xd.data_ptr(), xm2.data_ptr(), batch, 0.25, 0.5, stream()), "dft tc")
+    _lib.check(lib.fno_spectral_dft_fwd(xd.data_ptr(), xm2.data_ptr(), batch, _lib.ACT_BF16, 0.25, 0.5, stream()), "dft tc")
     c = np.full(12, 0.5)
     c[0] = 0.25
     ref2 = (onp.spectral_modes(xf, 12, 12) * c).reshape(batch, 32, 288).transpose(2, 0, 1)
     assert np.linalg.norm(xm2.cpu().numpy() - ref2) / np.linalg.norm(ref2) < 2e-6
-    xm3 = torch.zeros_like(xm)  # the kernel of the forward path on the same planes
+    xm3 = torch.zeros_like(xm)  # a second launch on the same planes: the same bits
     _lib.check(lib.fno_spectral_dft_fwd(xd.data_ptr(), xm3.data_ptr(), batch, _lib.ACT_BF16, 1.0, 1.0, stream()), "dft")
     assert np.linalg.norm(xm3.cpu().numpy() - ref) / np.linalg.norm(ref) < 2e-6
+    assert torch.equal(xm3, xm)
 
 
 @pytest.mark.parametrize("epi", ["gelu", "save_pre", "mul_dgelu", "plain"])
@@ -404,7 +405,8 @@ def test_full_batch_properties():
         perm = torch.randperm(256, device="cuda", generator=torch.Generator(device="cuda").manual_seed(0))
         yp = m.generate(inp[perm], cp[perm], mk[perm])
         assert torch.equal(yp, y1[perm])
-    # host tensors at this size take the chunked multi-stream path (4 x fno_rollout_host): identical result
+    # host tensors at this size take the chunked multi-stream path (graph-replayed fno_forward per batch chunk): identical
+    # result
     hseq = m.generate_many(inp.cpu(), cp.cpu(), mk.cpu(), 1)
     assert hseq[0].device.type == "cpu" and torch.equal(hseq[0], y1.cpu())
     hseq2 = m.generate_many(hseq[0], cp.cpu(), mk.cpu(), 1)  # feeding the returned (pinned) buffer back is safe

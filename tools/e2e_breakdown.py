@@ -34,11 +34,7 @@ for b in (32, 64, 128, 256):
     print(f"B={b}: device step {1e6*t/20:.1f} us  (graph {1e6*tg/20:.1f} us)  -> x{256//b} = {1e6*t/20*256/b:.0f} us")
     del m
 batch = synth.make_batch(1, 256, "cavity", with_label=False)
-for chunks in (1, 2, 4, 8):
-    m, _ = build_model("bf16", p)
-    m.host_chunks = chunks
-    timed_e2e(m, batch, 5, 2)
-    t, _, _ = timed_e2e(m, batch, 20, 2)
-    # host-side time of the call alone
-    print(f"chunks={chunks}: e2e {20 / t:.1f} steps/s ({1e3 * t / 20:.3f} ms/step)")
-    del m
+m, _ = build_model("bf16", p)
+timed_e2e(m, batch, 5, 2)
+t, _, _ = timed_e2e(m, batch, 20, 2)
+print(f"chunked e2e: {20 / t:.1f} steps/s ({1e3 * t / 20:.3f} ms/step)")

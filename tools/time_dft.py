@@ -1,5 +1,6 @@
-"""Standalone timing of fno_spectral_dft_fwd at B=256 (bf16 and fp32 planes): median of 30 event-bracketed launches,
-L2 flushed between launches by the 67 MB / 134 MB input itself being larger than what survives."""
+"""Standalone timing of fno_spectral_dft_fwd at B=256 (bf16 planes: dft_fwd_tc_kernel, fp32 planes: dft_fwd_kernel):
+median of 30 event-bracketed launches, L2 flushed between launches by the 67 MB / 134 MB input itself being larger
+than what survives."""
 import ctypes as C, os, sys
 import numpy as np, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -21,19 +22,4 @@ for name, dt, code in (("bf16", torch.bfloat16, _lib.ACT_BF16), ("f32", torch.fl
         torch.cuda.synchronize()
         if i >= 4:
             ts.append(a.elapsed_time(z) * 1e3)
-    print(f"dft_fwd {name} FNO_DFT_MINB={os.environ.get('FNO_DFT_MINB', '4')}: median {np.median(ts):.1f} us, min {min(ts):.1f} us")
-# tensor-core kernel (bf16 planes)
-x = torch.randn(b, 32, 64, 64, device="cuda").to(torch.bfloat16)
-x2 = torch.randn(b, 32, 64, 64, device="cuda").to(torch.bfloat16)
-xm = torch.empty(288, b, 32, dtype=torch.complex64, device="cuda")
-ts = []
-for i in range(34):
-    src = x if i % 2 == 0 else x2
-    a, z = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    _lib.check(lib.fno_spectral_dft_fwd_tc(src.data_ptr(), xm.data_ptr(), b, 1.0, 1.0, st), "dft tc")
-    z.record()
-    torch.cuda.synchronize()
-    if i >= 4:
-        ts.append(a.elapsed_time(z) * 1e3)
-print(f"dft_fwd_tc bf16: median {np.median(ts):.1f} us, min {min(ts):.1f} us")
+    print(f"dft_fwd {name}: median {np.median(ts):.1f} us, min {min(ts):.1f} us")
