@@ -4,11 +4,13 @@ Public surface mirrors the reference's for this path:
     Fno2d, SpectralConv2d_fast, FnoBlock   (reference src/models/fno/fno2d.py)
     AutoCfdModel                           (reference src/models/base_model.py)
     MseLoss, loss_name_to_fn               (reference src/models/loss.py)
+    infer_multistep                        (reference src/test_multistep.py infer, batched on the device)
 """
 from .base_model import AutoCfdModel
 from .loss import MseLoss, loss_name_to_fn
 
-__all__ = ["AutoCfdModel", "MseLoss", "loss_name_to_fn", "Fno2d", "FnoBlock", "SpectralConv2d_fast", "FusedAdam", "DeviceFrames"]
+__all__ = ["AutoCfdModel", "MseLoss", "loss_name_to_fn", "Fno2d", "FnoBlock", "SpectralConv2d_fast", "FusedAdam", "DeviceFrames",
+           "infer_multistep"]
 
 
 def __getattr__(name):  # lazy: importing the package must not require the native library
@@ -21,4 +23,7 @@ def __getattr__(name):  # lazy: importing the package must not require the nativ
     if name == "DeviceFrames":
         from .data import DeviceFrames
         return DeviceFrames
+    if name == "infer_multistep":
+        from .metrics import infer_multistep
+        return infer_multistep
     raise AttributeError(name)

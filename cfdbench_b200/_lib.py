@@ -144,6 +144,8 @@ SIGNATURES = {
     "fno_grid_backward": (C.c_int, [C.POINTER(FnoWeights), C.POINTER(FnoWeightsBwd), _P, _P, _P, _P,
                                     C.POINTER(FnoTrainSaved), C.POINTER(FnoGrads), C.POINTER(FnoBwdScratch),
                                     C.POINTER(FnoWorkspace), _P, _P, _I, _I, _I, _P]),
+    "fno_grid_multistep_metrics": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _P]),
+    "fno_grid_gather_batch": (C.c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _P, _P, _P, _P, _I, _I, _P]),
 }
 
 GRID_MIN, GRID_MAX = 24, 128

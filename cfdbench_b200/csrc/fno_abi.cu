@@ -69,6 +69,9 @@ int grid_lift_bwd_row();
 size_t grid_bwd_partials_floats();
 size_t grid_partials_offset_co();
 size_t grid_partials_offset_lb();
+cudaError_t launch_grid_multistep_metrics(const float*, const float*, const float*, float*, int, int, int, int, cudaStream_t);
+cudaError_t launch_grid_gather_batch(const void*, const void*, const float*, const int*, const long long*, int, int, int,
+                                     float*, float*, float*, float*, int, int, cudaStream_t);
 }  // namespace fno
 
 using namespace fno;
@@ -696,6 +699,30 @@ int fno_grid_backward(const fno_weights* w, const fno_weights_bwd* wb, const flo
     FNO_CUDA(launch_reduce_partials(part_lb, grid_lift_bwd_parts(batch), grid_lift_bwd_row(), g->fc0_w, kC * (5 + p), g->fc0_b,
                                     kC, nullptr, 0, 0, st),
              "reduce(fc0.weight | fc0.bias)");
+  return kOk;
+}
+
+int fno_grid_multistep_metrics(const float* preds_seq, const float* label_u, const float* mask, float* sums, int steps,
+                               int batch, int h, int wd, void* stream) {
+  FNO_TRY(grid_arg("fno_grid_multistep_metrics", h, wd));
+  if (!preds_seq || !label_u || !mask || !sums || steps <= 0 || steps > 65535 || batch <= 0)
+    return fail(kErrArg, "fno_grid_multistep_metrics: bad argument");
+  FNO_CUDA(launch_grid_multistep_metrics(preds_seq, label_u, mask, sums, steps, batch, h, wd, S(stream)),
+           "grid_multistep_metrics_kernel");
+  return kOk;
+}
+
+int fno_grid_gather_batch(const void* frames_in, const void* frames_out, const float* case_table, const int32_t* case_ids,
+                          const int64_t* idx, int n_idx, int n_case_params, int frame_dtype, float* inputs, float* label,
+                          float* mask, float* case_params, int h, int wd, void* stream) {
+  FNO_TRY(grid_arg("fno_grid_gather_batch", h, wd));
+  if (!frames_in || !frames_out || !case_ids || !idx || !inputs || !label || !mask || n_idx <= 0 || n_case_params < 0 ||
+      n_case_params > kMaxCaseParams || bad_dtype(frame_dtype) || (n_case_params > 0 && (!case_table || !case_params)))
+    return fail(kErrArg, "fno_grid_gather_batch: bad argument");
+  FNO_CUDA(launch_grid_gather_batch(frames_in, frames_out, case_table, reinterpret_cast<const int*>(case_ids),
+                                    reinterpret_cast<const long long*>(idx), n_idx, n_case_params,
+                                    frame_dtype == FNO_ACT_BF16, inputs, label, mask, case_params, h, wd, S(stream)),
+           "grid_gather_batch_kernel");
   return kOk;
 }
 

@@ -122,3 +122,101 @@ cudaError_t launch_gather_batch(const void* frames_in, const void* frames_out, c
 }
 
 }  // namespace fno
+
+// ------------------------------------------------------------------------------------------------
+// Grid-generic versions of the two kernels above, for any H x W the grid path runs (24..128 each; the tube and dam
+// problems' 66x65).  A plane of H*W floats (or bf16) need not start on more than an element boundary -- a 66x65 fp32
+// plane is 17,160 B, so every odd plane of label_u / mask is only 8-byte aligned, and at odd H*W (25x127) only 4-byte
+// aligned -- so both kernels use scalar loads and stores.  They move a few MB per call; the loads are not the limit.
+// ------------------------------------------------------------------------------------------------
+namespace fno {
+
+// Same layouts and sums as multistep_metrics_kernel with hw = H*W in place of 4096.  grid (B, S): one CTA per
+// (step, case) plane.  Each thread's pixels, the shuffle tree and the warp order are fixed, so a repeated launch is
+// bit-identical (no atomics).
+__global__ void __launch_bounds__(kMtThreads)
+    grid_multistep_metrics_kernel(const float* __restrict__ preds_seq, const float* __restrict__ label_u,
+                                  const float* __restrict__ mask, float* __restrict__ out, int batch, int hw) {
+  __shared__ float red[kMtThreads / 32][3];
+  const int b = blockIdx.x, s = blockIdx.y;
+  const size_t plane = static_cast<size_t>(s) * batch + b;
+  const float* p = preds_seq + plane * 2 * hw;   // channel 0 = u
+  const float* l = label_u + plane * hw;
+  const float* m = mask + plane * hw;
+  float se = 0.f, sl = 0.f, sa = 0.f;
+  for (int i = threadIdx.x; i < hw; i += kMtThreads) {
+    const float mv = __ldg(m + i);
+    const float pp = __ldg(p + i) * mv, ll = __ldg(l + i) * mv;
+    const float d = pp - ll;
+    se = fmaf(d, d, se);
+    sl = fmaf(ll, ll, sl);
+    sa += fabsf(d);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    se += __shfl_xor_sync(0xffffffffu, se, o);
+    sl += __shfl_xor_sync(0xffffffffu, sl, o);
+    sa += __shfl_xor_sync(0xffffffffu, sa, o);
+  }
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (lane == 0) {
+    red[warp][0] = se;
+    red[warp][1] = sl;
+    red[warp][2] = sa;
+  }
+  __syncthreads();
+  if (threadIdx.x < 3) {
+    float t = 0.f;
+#pragma unroll
+    for (int w = 0; w < kMtThreads / 32; ++w) t += red[w][threadIdx.x];  // fixed order: deterministic
+    out[plane * 3 + threadIdx.x] = t;
+  }
+}
+
+cudaError_t launch_grid_multistep_metrics(const float* preds_seq, const float* label_u, const float* mask, float* out,
+                                          int steps, int batch, int h, int w, cudaStream_t stream) {
+  dim3 grid(batch, steps);
+  grid_multistep_metrics_kernel<<<grid, kMtThreads, 0, stream>>>(preds_seq, label_u, mask, out, batch, h * w);
+  return cudaGetLastError();
+}
+
+__device__ __forceinline__ float frame_ld(const float* p) { return __ldg(p); }
+__device__ __forceinline__ float frame_ld(const __nv_bfloat16* p) { return __bfloat162float(__ldg(p)); }
+
+// Same job as gather_batch_kernel at hw = H*W.  grid (n_idx, 5 planes): plane 0,1 -> inputs u,v; 2 -> mask;
+// 3,4 -> label u,v.  The batch index is on x so that n_idx is not held to gridDim.y's 65,535.
+template <typename TFrame>
+__global__ void __launch_bounds__(kGbThreads)
+    grid_gather_batch_kernel(const TFrame* __restrict__ frames_in, const TFrame* __restrict__ frames_out,
+                             const float* __restrict__ case_table, const int* __restrict__ case_ids,
+                             const long long* __restrict__ idx, int n_case_params, int hw, float* __restrict__ inputs,
+                             float* __restrict__ label, float* __restrict__ mask, float* __restrict__ case_params) {
+  const int b = blockIdx.x, plane = blockIdx.y;
+  const long long i = idx[b];
+  const TFrame* src = (plane < 3 ? frames_in : frames_out) + (static_cast<size_t>(i) * 3 + (plane < 3 ? plane : plane - 3)) * hw;
+  float* dst = plane < 2   ? inputs + (static_cast<size_t>(b) * 2 + plane) * hw
+               : plane == 2 ? mask + static_cast<size_t>(b) * hw
+                            : label + (static_cast<size_t>(b) * 2 + (plane - 3)) * hw;
+  for (int e = threadIdx.x; e < hw; e += kGbThreads) dst[e] = frame_ld(src + e);
+  if (plane == 0 && threadIdx.x < n_case_params)
+    case_params[static_cast<size_t>(b) * n_case_params + threadIdx.x] =
+        __ldg(case_table + static_cast<size_t>(case_ids[i]) * n_case_params + threadIdx.x);
+}
+
+cudaError_t launch_grid_gather_batch(const void* frames_in, const void* frames_out, const float* case_table,
+                                     const int* case_ids, const long long* idx, int n_idx, int n_case_params,
+                                     int frame_bf16, float* inputs, float* label, float* mask, float* case_params, int h,
+                                     int w, cudaStream_t stream) {
+  dim3 grid(n_idx, 5);
+  if (frame_bf16)
+    grid_gather_batch_kernel<__nv_bfloat16><<<grid, kGbThreads, 0, stream>>>(
+        static_cast<const __nv_bfloat16*>(frames_in), static_cast<const __nv_bfloat16*>(frames_out), case_table, case_ids,
+        idx, n_case_params, h * w, inputs, label, mask, case_params);
+  else
+    grid_gather_batch_kernel<float><<<grid, kGbThreads, 0, stream>>>(
+        static_cast<const float*>(frames_in), static_cast<const float*>(frames_out), case_table, case_ids, idx,
+        n_case_params, h * w, inputs, label, mask, case_params);
+  return cudaGetLastError();
+}
+
+}  // namespace fno

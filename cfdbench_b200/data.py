@@ -6,6 +6,8 @@ dicts `dataset.case_params` (src/dataset/cavity.py:283-331, cylinder.py likewise
 (src/train_auto.py:33-58, 208-210) then builds each batch on the host and copies it to the GPU.  `DeviceFrames`
 uploads the split once (fp32, or bf16 to halve its footprint) and produces the same batch dict with one kernel launch
 (`fno_gather_batch`); the on-disk format and the dataset classes are untouched -- it takes the dataset object as is.
+Frames are 64x64 (cavity, cylinder) or any H x W with 24 <= H, W <= 128 (`fno_grid_gather_batch`; the tube and dam
+datasets hold (N, 3, 66, 65) frames, reference src/dataset/tube.py:228-281, dam.py:275-313).
 
     frames = DeviceFrames(train_data, device="cuda")
     for batch in frames.loader(batch_size=32, shuffle=True, generator=g):   # same index order as the DataLoader
@@ -37,8 +39,12 @@ class DeviceFrames:
         if dev.type != "cuda":
             raise ValueError("DeviceFrames keeps the split in GPU memory: pass a CUDA device")
         ins, labs = dataset.inputs, dataset.labels
-        if ins.dim() != 4 or ins.shape[1] != 3 or tuple(ins.shape[2:]) != (64, 64) or labs.shape != ins.shape:
-            raise ValueError(f"expected (N, 3, 64, 64) input / label frames, got {tuple(ins.shape)} / {tuple(labs.shape)}")
+        if ins.dim() != 4 or ins.shape[1] != 3 or labs.shape != ins.shape:
+            raise ValueError(f"expected (N, 3, H, W) input / label frames, got {tuple(ins.shape)} / {tuple(labs.shape)}")
+        self.height, self.width = int(ins.shape[2]), int(ins.shape[3])
+        from . import _lib
+        if not (_lib.GRID_MIN <= self.height <= _lib.GRID_MAX and _lib.GRID_MIN <= self.width <= _lib.GRID_MAX):
+            raise ValueError(f"frames are {self.height}x{self.width}: H and W must lie in {_lib.GRID_MIN}..{_lib.GRID_MAX}")
         self.device, self.frame_dtype = dev, frame_dtype
         self.n = ins.shape[0]
         self.frames_in = ins.to(device=dev, dtype=frame_dtype).contiguous()
@@ -63,16 +69,18 @@ class DeviceFrames:
         if int(idx.min()) < 0 or int(idx.max()) >= self.n:
             raise IndexError("sample index out of range")
         idx = idx.to(self.device, non_blocking=True)
-        b, p, dev = idx.numel(), self.n_case_params, self.device
-        out = dict(inputs=torch.empty(b, 2, 64, 64, device=dev), label=torch.empty(b, 2, 64, 64, device=dev),
-                   mask=torch.empty(b, 1, 64, 64, device=dev), case_params=torch.empty(b, p, device=dev))
+        b, p, dev, gh, gw = idx.numel(), self.n_case_params, self.device, self.height, self.width
+        out = dict(inputs=torch.empty(b, 2, gh, gw, device=dev), label=torch.empty(b, 2, gh, gw, device=dev),
+                   mask=torch.empty(b, 1, gh, gw, device=dev), case_params=torch.empty(b, p, device=dev))
+        args = (self.frames_in.data_ptr(), self.frames_out.data_ptr(), self.case_table.data_ptr(), self.case_ids.data_ptr(),
+                idx.data_ptr(), b, p, _lib.ACT_BF16 if self.frame_dtype == torch.bfloat16 else _lib.ACT_F32,
+                out["inputs"].data_ptr(), out["label"].data_ptr(), out["mask"].data_ptr(), out["case_params"].data_ptr())
         with torch.cuda.device(dev):
             st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-            _lib.check(lib.fno_gather_batch(self.frames_in.data_ptr(), self.frames_out.data_ptr(),
-                                            self.case_table.data_ptr(), self.case_ids.data_ptr(), idx.data_ptr(), b, p,
-                                            _lib.ACT_BF16 if self.frame_dtype == torch.bfloat16 else _lib.ACT_F32,
-                                            out["inputs"].data_ptr(), out["label"].data_ptr(), out["mask"].data_ptr(),
-                                            out["case_params"].data_ptr(), st), "fno_gather_batch")
+            if (gh, gw) == (64, 64):
+                _lib.check(lib.fno_gather_batch(*args, st), "fno_gather_batch")
+            else:
+                _lib.check(lib.fno_grid_gather_batch(*args, gh, gw, st), "fno_grid_gather_batch")
         idx.record_stream(torch.cuda.current_stream(dev))
         return out
 

@@ -106,3 +106,22 @@ def make_batch(seed: int, batch: int, problem: str = "cavity", in_chan: int = 2,
     if with_label:
         out["label"] = np.clip(rng.standard_normal((batch, in_chan, gh, gw)), -3, 3).astype(np.float32)
     return out
+
+
+def make_split(seed: int, n_cases: int, problem: str = "cavity", frames=(20, 20)) -> tuple[list, list]:
+    """A synthetic test split in the form `test_multistep.main` hands to `infer` (reference src/test_multistep.py:199-218):
+    one (T_c, 3, H, W) float32 array per case (u, v, mask), T_c drawn from frames[0]..frames[1], and one (p,) float32
+    case-parameter vector per case.  Each frame's mask is the case's mask with a few extra pixels zeroed, so that the
+    per-frame mask of the metrics is distinguishable from the start frame's mask of the rollout."""
+    rng = np.random.default_rng(seed)
+    gh, gw = grid(problem)
+    p = n_case_params(problem)
+    feats, cps = [], []
+    for _ in range(n_cases):
+        t = int(rng.integers(frames[0], frames[1] + 1))
+        f = np.empty((t, 3, gh, gw), dtype=np.float32)
+        f[:, :2] = np.clip(rng.standard_normal((t, 2, gh, gw)), -3, 3)
+        f[:, 2] = make_mask(rng, 1, problem)[0, 0] * (rng.random((t, gh, gw)) > 0.02)
+        feats.append(f)
+        cps.append(rng.standard_normal(p).astype(np.float32))
+    return feats, cps

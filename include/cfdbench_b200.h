@@ -306,6 +306,16 @@ int fno_grid_backward(const fno_weights* w, const fno_weights_bwd* wb, const flo
                       const float* case_params, const float* dpreds, const fno_train_saved* saved, const fno_grads* grads,
                       const fno_bwd_scratch* scratch, const fno_workspace* ws, float* d_inputs, float* d_case_params,
                       int batch, int h, int w_, void* stream);
+/* fno_multistep_metrics on an H x W grid: preds_seq [S][B][2][H][W], label_u and mask [S][B][H][W]; sums [S][B][3] as
+ * there (sums over the H*W pixels).  One CTA per (step, case) plane, fixed-order reduction: bit-reproducible.
+ * steps <= 65535. */
+int fno_grid_multistep_metrics(const float* preds_seq, const float* label_u, const float* mask, float* sums, int steps,
+                               int batch, int h, int w_, void* stream);
+/* fno_gather_batch on an H x W grid: frames_in / frames_out [N][3][H][W] float32 or bfloat16; outputs (float32)
+ * inputs [n][2][H][W], label [n][2][H][W], mask [n][1][H][W], case_params [n][p]. */
+int fno_grid_gather_batch(const void* frames_in, const void* frames_out, const float* case_table, const int32_t* case_ids,
+                          const int64_t* idx, int n_idx, int n_case_params, int frame_dtype, float* inputs, float* label,
+                          float* mask, float* case_params, int h, int w_, void* stream);
 
 #ifdef __cplusplus
 }
