@@ -13,6 +13,8 @@ products, no FFT library involved), what the reference computes with torch.fft /
 * `rollout`            <- reference src/models/fno/fno2d.py:257-295 (generate / generate_many)
 * `spectral_conv_backward`, `fno_backward` <- what torch.autograd derives for the above
   (PyTorch complex-gradient convention: grad = dL/dRe + i dL/dIm).
+* `fno_vjp`, `fno_vjp_saved` <- the same adjoint for any upstream d(preds), through the lift into the input frame and the
+  case parameters; `fno_vjp_saved` takes the hidden activations of a forward pass as given (e.g. a GPU's saved ones).
 
 Pinning: the reference ships no tests or golden vectors (SURVEY.md 4, 8c).  The oracle is pinned
 against outputs of the reference module itself, generated in the build container by
@@ -241,3 +243,71 @@ def fno_backward(sd: dict, inputs: np.ndarray, case_params: np.ndarray, mask: np
     grads["fc0.weight"] = np.einsum("bohw,bihw->oi", ga, feats, optimize=True)[:, :, None, None]
     grads["fc0.bias"] = ga.sum(axis=(0, 2, 3))
     return grads
+
+
+def _scipy_erf(x: np.ndarray) -> np.ndarray:
+    from scipy.special import erf as sp_erf
+    return sp_erf(x)
+
+
+def fno_vjp_saved(sd: dict, inputs: np.ndarray, case_params: np.ndarray, mask: np.ndarray, gpreds: np.ndarray,
+                  acts: list, pres: list, erf=_scipy_erf, chunk: int = 32):
+    """(parameter gradients, dL/dinputs, dL/dcase_params) for L = sum(gpreds * preds), float64, given the hidden
+    activations a_0..a_L and the block pre-activations pre_0..pre_{L-1} of a forward pass.  With the saved tensors fixed
+    the adjoint is a linear map of `gpreds`, so saved tensors of any forward -- this oracle's own, or a GPU's in either
+    storage mode -- give a float64 reference of what a backward pass through them computes.  The lift is differentiated
+    through a rounded a_0 and every GELU through its saved pre-activation (straight-through).  With
+    a0 = fc0(cat[u, v, mask, x, y, params]) (reference fno2d.py:195-217) and ga = dL/da0,
+        dL/du, dL/dv  = sum_o fc0_w[o][0|1] ga[b][o]          dL/dparams[b][j] = sum_o fc0_w[o][5+j] sum_hw ga[b][o].
+    `erf` is the error function of the GELU terms; the projection runs in sample chunks of `chunk` to bound the size
+    of its 128-channel temporaries."""
+    def gelu_dgelu(x):
+        e = erf(x / sqrt(2.0))
+        return 0.5 * x * (1.0 + e), 0.5 * (1.0 + e) + x * np.exp(-0.5 * x * x) / sqrt(2.0 * pi)
+
+    m = (mask[:, None] if mask.ndim == 3 else mask).astype(np.float64)
+    a_last = acts[-1]
+    grads: dict[str, np.ndarray] = {}
+    w1m = sd["fc1.weight"].reshape(sd["fc1.weight"].shape[:2]).astype(np.float64)
+    w2m = sd["fc2.weight"].reshape(sd["fc2.weight"].shape[:2]).astype(np.float64)
+    g_w2 = np.zeros(w2m.shape)
+    g_b2 = np.zeros(w2m.shape[0])
+    g_w1 = np.zeros(w1m.shape)
+    g_b1 = np.zeros(w1m.shape[0])
+    ga = np.empty(a_last.shape)
+    for b0 in range(0, a_last.shape[0], chunk):
+        sl = slice(b0, b0 + chunk)
+        a = np.asarray(a_last[sl], dtype=np.float64)
+        h1, dh1 = gelu_dgelu(conv1x1(a, sd["fc1.weight"], sd["fc1.bias"]))
+        graw = gpreds[sl].astype(np.float64) * m[sl]
+        g_w2 += np.einsum("bchw,bjhw->cj", graw, h1, optimize=True)
+        g_b2 += graw.sum(axis=(0, 2, 3))
+        gz1 = np.einsum("cj,bchw->bjhw", w2m, graw, optimize=True) * dh1
+        g_w1 += np.einsum("bjhw,bihw->ji", gz1, a, optimize=True)
+        g_b1 += gz1.sum(axis=(0, 2, 3))
+        ga[sl] = np.einsum("ji,bjhw->bihw", w1m, gz1, optimize=True)
+    grads["fc2.weight"], grads["fc2.bias"] = g_w2[:, :, None, None], g_b2
+    grads["fc1.weight"], grads["fc1.bias"] = g_w1[:, :, None, None], g_b1
+    for l in reversed(range(num_layers(sd))):
+        gpre = ga * gelu_dgelu(np.asarray(pres[l], dtype=np.float64))[1]
+        x = np.asarray(acts[l], dtype=np.float64)
+        w0 = sd[f"blocks.{l}.w0.weight"].reshape(x.shape[1], x.shape[1]).astype(np.float64)
+        grads[f"blocks.{l}.w0.weight"] = np.einsum("bohw,bihw->oi", gpre, x, optimize=True)[:, :, None, None]
+        grads[f"blocks.{l}.w0.bias"] = gpre.sum(axis=(0, 2, 3))
+        gxs, gw1, gw2 = spectral_conv_backward(x, sd[f"blocks.{l}.conv0.weights1"],
+                                               sd[f"blocks.{l}.conv0.weights2"], gpre)
+        grads[f"blocks.{l}.conv0.weights1"], grads[f"blocks.{l}.conv0.weights2"] = gw1, gw2
+        ga = gxs + np.einsum("oi,bohw->bihw", w0, gpre, optimize=True)
+    feats = lift_features(inputs, case_params, m)
+    grads["fc0.weight"] = np.einsum("bohw,bihw->oi", ga, feats, optimize=True)[:, :, None, None]
+    grads["fc0.bias"] = ga.sum(axis=(0, 2, 3))
+    w_lift = sd["fc0.weight"].reshape(sd["fc0.weight"].shape[:2]).astype(np.float64)   # [32][5+p]
+    d_inputs = np.einsum("oc,bohw->bchw", w_lift[:, :inputs.shape[1]], ga, optimize=True)
+    d_case_params = np.einsum("oj,bo->bj", w_lift[:, 5:], ga.sum(axis=(2, 3)), optimize=True)
+    return grads, d_inputs, d_case_params
+
+
+def fno_vjp(sd: dict, inputs: np.ndarray, case_params: np.ndarray, mask: np.ndarray, gpreds: np.ndarray, erf=_scipy_erf):
+    """fno_vjp_saved through this oracle's own float64 forward: the exact vector-Jacobian product of Fno2d."""
+    fwd = fno_forward(sd, inputs, case_params, mask, return_acts=True)
+    return fno_vjp_saved(sd, inputs, case_params, mask, gpreds, fwd["acts"], fwd["pres"], erf=erf)

@@ -1,9 +1,9 @@
-"""Float64 vector-Jacobian product of the FNO forward for an arbitrary upstream gradient, including the gradients w.r.t.
-the input frame and the case parameters -- the yardstick of Fno2d's input gradients (fno_backward_inputs).  It extends
-the oracle's adjoint (`oracle.fno_numpy.fno_backward`, whose parameter gradients it must reproduce) through the lift:
-with a0 = fc0(cat[u, v, mask, x, y, params]) (reference fno2d.py:195-217) and ga = dL/da0,
-    dL/du, dL/dv  = sum_o fc0_w[o][0|1] ga[b][o]          dL/dparams[b][j] = sum_o fc0_w[o][5+j] sum_hw ga[b][o].
-Checked here against autograd of the fp32 torch port and against central finite differences of the float64 forward."""
+"""The oracle's float64 vector-Jacobian product (`oracle.fno_numpy.fno_vjp` / `fno_vjp_saved`) for an arbitrary upstream
+gradient, including the gradients w.r.t. the input frame and the case parameters -- the yardstick of Fno2d's input
+gradients (fno_backward_inputs) and, fed a GPU's saved activations, of the training backward stage by stage
+(tests/test_gpu_train_conditioned.py).  Its parameter gradients must reproduce the oracle's adjoint
+(`oracle.fno_numpy.fno_backward`); checked here also against autograd of the fp32 torch port and against central
+finite differences of the float64 forward."""
 import numpy as np
 import pytest
 import torch
@@ -11,41 +11,7 @@ import torch
 from cfdbench_b200 import synth
 from oracle import fno_numpy as onp
 from oracle import fno_torch_port as port
-
-
-def fno_vjp(sd: dict, inputs: np.ndarray, case_params: np.ndarray, mask: np.ndarray, gpreds: np.ndarray):
-    """(parameter gradients, dL/dinputs, dL/dcase_params) for L = sum(gpreds * preds), float64."""
-    fwd = onp.fno_forward(sd, inputs, case_params, mask, return_acts=True)
-    m = (mask[:, None] if mask.ndim == 3 else mask).astype(np.float64)
-    acts, pres, z1 = fwd["acts"], fwd["pres"], fwd["z1"]
-    grads = {}
-    graw = gpreds.astype(np.float64) * m
-    h1 = onp.gelu(z1)
-    w2m = sd["fc2.weight"].reshape(sd["fc2.weight"].shape[:2]).astype(np.float64)
-    grads["fc2.weight"] = np.einsum("bchw,bjhw->cj", graw, h1, optimize=True)[:, :, None, None]
-    grads["fc2.bias"] = graw.sum(axis=(0, 2, 3))
-    gz1 = np.einsum("cj,bchw->bjhw", w2m, graw, optimize=True) * onp.dgelu(z1)
-    w1m = sd["fc1.weight"].reshape(sd["fc1.weight"].shape[:2]).astype(np.float64)
-    grads["fc1.weight"] = np.einsum("bjhw,bihw->ji", gz1, acts[-1], optimize=True)[:, :, None, None]
-    grads["fc1.bias"] = gz1.sum(axis=(0, 2, 3))
-    ga = np.einsum("ji,bjhw->bihw", w1m, gz1, optimize=True)
-    for l in reversed(range(onp.num_layers(sd))):
-        gpre = ga * onp.dgelu(pres[l])
-        x = acts[l]
-        w0 = sd[f"blocks.{l}.w0.weight"].reshape(x.shape[1], x.shape[1]).astype(np.float64)
-        grads[f"blocks.{l}.w0.weight"] = np.einsum("bohw,bihw->oi", gpre, x, optimize=True)[:, :, None, None]
-        grads[f"blocks.{l}.w0.bias"] = gpre.sum(axis=(0, 2, 3))
-        gxs, gw1, gw2 = onp.spectral_conv_backward(x, sd[f"blocks.{l}.conv0.weights1"],
-                                                   sd[f"blocks.{l}.conv0.weights2"], gpre)
-        grads[f"blocks.{l}.conv0.weights1"], grads[f"blocks.{l}.conv0.weights2"] = gw1, gw2
-        ga = gxs + np.einsum("oi,bohw->bihw", w0, gpre, optimize=True)
-    feats = onp.lift_features(inputs, case_params, m)
-    grads["fc0.weight"] = np.einsum("bohw,bihw->oi", ga, feats, optimize=True)[:, :, None, None]
-    grads["fc0.bias"] = ga.sum(axis=(0, 2, 3))
-    w_lift = sd["fc0.weight"].reshape(sd["fc0.weight"].shape[:2]).astype(np.float64)   # [32][5+p]
-    d_inputs = np.einsum("oc,bohw->bchw", w_lift[:, :inputs.shape[1]], ga, optimize=True)
-    d_case_params = np.einsum("oj,bo->bj", w_lift[:, 5:], ga.sum(axis=(2, 3)), optimize=True)
-    return grads, d_inputs, d_case_params
+from oracle.fno_numpy import fno_vjp
 
 
 def nmse_upstream(preds: np.ndarray, label: np.ndarray, mask: np.ndarray) -> np.ndarray:
@@ -76,6 +42,23 @@ def test_vjp_parameter_gradients_equal_oracle_backward(problem):
     assert set(grads) == set(ref)
     for k, v in ref.items():
         np.testing.assert_allclose(grads[k], v, rtol=1e-12, atol=1e-15 * float(np.abs(v).max()), err_msg=k)
+
+
+def test_vjp_saved_with_the_oracles_own_activations_reproduces_oracle_backward():
+    """fno_vjp_saved fed fno_forward's own a_0..a_L / pre_0..pre_{L-1} and the nmse upstream: fno_backward's gradients.
+    Three samples in projection chunks of two (a ragged last chunk), the GELU terms through math.erf instead of scipy."""
+    sd, bt, _ = _case("cylinder", 23, batch=3)
+    fwd = onp.fno_forward(sd, bt["inputs"], bt["case_params"], bt["mask"], return_acts=True)
+    gp = nmse_upstream(fwd["preds"], bt["label"], bt["mask"])
+    grads, d_in, d_cp = onp.fno_vjp_saved(sd, bt["inputs"], bt["case_params"], bt["mask"], gp, fwd["acts"], fwd["pres"],
+                                          erf=onp._erf, chunk=2)
+    ref = onp.fno_backward(sd, bt["inputs"], bt["case_params"], bt["mask"], bt["label"])
+    assert set(grads) == set(ref)
+    for k, v in ref.items():
+        np.testing.assert_allclose(grads[k], v, rtol=1e-12, atol=1e-12 * float(np.abs(v).max()), err_msg=k)
+    _, d_in2, d_cp2 = fno_vjp(sd, bt["inputs"], bt["case_params"], bt["mask"], gp)
+    np.testing.assert_allclose(d_in, d_in2, rtol=1e-12, atol=1e-12 * float(np.abs(d_in2).max()))
+    np.testing.assert_allclose(d_cp, d_cp2, rtol=1e-12, atol=1e-12 * float(np.abs(d_cp2).max()))
 
 
 @pytest.mark.parametrize("problem", ["cavity", "cylinder"])
