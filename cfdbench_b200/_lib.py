@@ -127,6 +127,11 @@ SIGNATURES = {
     "fno_backward_inputs": (C.c_int, [C.POINTER(FnoWeights), C.POINTER(FnoWeightsBwd), _P, _P, _P, _P,
                                       C.POINTER(FnoTrainSaved), C.POINTER(FnoGrads), C.POINTER(FnoBwdScratch),
                                       C.POINTER(FnoWorkspace), _P, _P, _I, _I, _P]),
+    "fno_rollout_forward_train": (C.c_int, [C.POINTER(FnoWeights), _P, _P, _P, _P, _I, C.POINTER(FnoTrainSaved),
+                                            C.POINTER(FnoWorkspace), _I, _I, _P]),
+    "fno_rollout_backward": (C.c_int, [C.POINTER(FnoWeights), C.POINTER(FnoWeightsBwd), _P, _P, _P, _P, _P, _I,
+                                       C.POINTER(FnoTrainSaved), C.POINTER(FnoGrads), C.POINTER(FnoBwdScratch),
+                                       C.POINTER(FnoWorkspace), _P, _P, _P, _I, _I, _P]),
     # grid-generic fp32 path (H, W in 24..128)
     "fno_grid_act_bytes": (C.c_size_t, [_I, _I, _I]),
     "fno_grid_z_bytes": (C.c_size_t, [_I, _I]),
@@ -144,6 +149,11 @@ SIGNATURES = {
     "fno_grid_backward": (C.c_int, [C.POINTER(FnoWeights), C.POINTER(FnoWeightsBwd), _P, _P, _P, _P,
                                     C.POINTER(FnoTrainSaved), C.POINTER(FnoGrads), C.POINTER(FnoBwdScratch),
                                     C.POINTER(FnoWorkspace), _P, _P, _I, _I, _I, _P]),
+    "fno_grid_rollout_forward_train": (C.c_int, [C.POINTER(FnoWeights), _P, _P, _P, _P, _I, C.POINTER(FnoTrainSaved),
+                                                 C.POINTER(FnoWorkspace), _I, _I, _I, _P]),
+    "fno_grid_rollout_backward": (C.c_int, [C.POINTER(FnoWeights), C.POINTER(FnoWeightsBwd), _P, _P, _P, _P, _P, _I,
+                                            C.POINTER(FnoTrainSaved), C.POINTER(FnoGrads), C.POINTER(FnoBwdScratch),
+                                            C.POINTER(FnoWorkspace), _P, _P, _P, _I, _I, _I, _P]),
     "fno_grid_multistep_metrics": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _P]),
     "fno_grid_gather_batch": (C.c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _P, _P, _P, _P, _I, _I, _P]),
 }

@@ -11,7 +11,7 @@ cudaError_t launch_mode_mix(const void*, const void*, void*, void*, int, cudaStr
 cudaError_t launch_block_fused(const void*, const void*, const float*, const float*, void*, int, cudaStream_t);
 size_t ym_image_bytes(int);
 cudaError_t launch_pack_spectral(const void*, const void*, void*, int, cudaStream_t);
-cudaError_t launch_unpack_spectral(const void*, void*, void*, cudaStream_t);
+cudaError_t launch_unpack_spectral(const void*, void*, void*, int, cudaStream_t);
 cudaError_t launch_dft_fwd_tc(const void*, void*, int, float, float, cudaStream_t);
 cudaError_t launch_pack_mix_operand(const void*, void*, cudaStream_t);
 cudaError_t launch_pack_mix_operand_direct(const void*, const void*, void*, int, cudaStream_t);
@@ -43,8 +43,8 @@ cudaError_t launch_chan_outer(const void*, const void*, float*, int*, int, cudaS
 cudaError_t launch_multistep_metrics(const float*, const float*, const float*, float*, int, int, cudaStream_t);
 cudaError_t launch_spectral_wgrad(const void*, const void*, void*, int, cudaStream_t);
 cudaError_t launch_lift_bwd(const float*, const float*, const float*, const float*, const float*, const float*,
-                            float*, float*, float*, int, int, cudaStream_t);
-cudaError_t launch_lift_bwd_data(const float*, const float*, float*, float*, int, int, cudaStream_t);
+                            float*, float*, float*, int, int, int, cudaStream_t);
+cudaError_t launch_lift_bwd_data(const float*, const float*, float*, float*, const float*, int, int, int, cudaStream_t);
 // grid-generic fp32 path (fno_grid.cu)
 bool grid_ok(int, int);
 void grid_tables_release(int);
@@ -63,7 +63,7 @@ int grid_project_bwd_row();
 template <int NJ, int NI>
 cudaError_t launch_grid_chan_outer(const float*, const float*, float*, int*, int, int, cudaStream_t);
 cudaError_t launch_grid_lift_bwd(const float*, const float*, const float*, const float*, const float*, const float*,
-                                 const float*, float*, float*, float*, int, int, int, int, cudaStream_t);
+                                 const float*, float*, float*, float*, const float*, int, int, int, int, int, cudaStream_t);
 int grid_lift_bwd_parts(int);
 int grid_lift_bwd_row();
 size_t grid_bwd_partials_floats();
@@ -155,7 +155,7 @@ int fno_pack_mix_operand_from_weights(const void* w1, const void* w2, void* wop,
 
 int fno_unpack_spectral_grads(const void* gwk, void* gw1, void* gw2, void* stream) {
   if (!gwk || !gw1 || !gw2) return fail(kErrArg, "fno_unpack_spectral_grads: null pointer");
-  FNO_CUDA(launch_unpack_spectral(gwk, gw1, gw2, S(stream)), "unpack_spectral_kernel");
+  FNO_CUDA(launch_unpack_spectral(gwk, gw1, gw2, 0, S(stream)), "unpack_spectral_kernel");
   return kOk;
 }
 
@@ -305,11 +305,10 @@ int fno_rollout_host(const fno_weights* w, const float* inputs_host, const float
   return kOk;
 }
 
-int fno_forward_train(const fno_weights* w, const float* inputs, const float* mask, const float* case_params,
-                      float* preds, const fno_train_saved* saved, const fno_workspace* ws, int batch,
-                      int act_dtype, void* stream) {
-  if (!w || !saved || !ws || !ws->ym || !ws->z) return fail(kErrArg, "fno_forward_train: bad argument");
-  if (w->n_layers < 1 || w->n_layers > FNO_MAX_LAYERS) return fail(kErrUnsupported, "fno_forward_train: n_layers");
+// fno_forward_train up to the saved set: the lift and the Fourier blocks, not the projection (the rollout backward
+// recomputes a step's saved set with this; the projection's output is not part of it)
+static int forward_train_body(const fno_weights* w, const float* inputs, const float* mask, const float* case_params,
+                              const fno_train_saved* saved, const fno_workspace* ws, int batch, int act_dtype, void* stream) {
   FNO_TRY(fno_lift_fwd(inputs, mask, case_params, w, saved->act[0], batch, act_dtype, stream));
   const float inv = 1.f / static_cast<float>(kHW);
   for (int l = 0; l < w->n_layers; ++l) {
@@ -320,6 +319,15 @@ int fno_forward_train(const fno_weights* w, const float* inputs, const float* ma
     FNO_TRY(fno_block_out(FNO_EPI_GELU_SAVE_PRE, ws->z, saved->act[l], w->w0t[l], w->w0_b[l], saved->act[l + 1],
                           saved->pre[l], nullptr, batch, act_dtype, stream));
   }
+  return kOk;
+}
+
+int fno_forward_train(const fno_weights* w, const float* inputs, const float* mask, const float* case_params,
+                      float* preds, const fno_train_saved* saved, const fno_workspace* ws, int batch,
+                      int act_dtype, void* stream) {
+  if (!w || !saved || !ws || !ws->ym || !ws->z) return fail(kErrArg, "fno_forward_train: bad argument");
+  if (w->n_layers < 1 || w->n_layers > FNO_MAX_LAYERS) return fail(kErrUnsupported, "fno_forward_train: n_layers");
+  FNO_TRY(forward_train_body(w, inputs, mask, case_params, saved, ws, batch, act_dtype, stream));
   return fno_project_fwd(saved->act[w->n_layers], mask, w, preds, batch, act_dtype, stream);
 }
 
@@ -328,10 +336,15 @@ int fno_forward_train(const fno_weights* w, const float* inputs, const float* ma
 // unpack_spectral_grads, lift_bwd) is skipped and only the data path runs.  d_inputs / d_case_params (either may be NULL)
 // receive the lift's data adjoint of dL/da0 (lift_bwd_data_kernel); with both NULL and g set, the launches are exactly
 // those of the parameter-only backward.
+// The rollout backward's sweep runs it once per step with two modes the single-step entry points leave off:
+//   accum    = 1: every parameter gradient is added to (the sweep's first step wrote it);
+//   hand_off = 1: lift_bwd_data_kernel<true>: d_inputs = fc0[:, 0:2]^T dL/da0 + add (the next sweep step's upstream
+//                 gradient when `add` is the previous prediction's), d_case_params += its share.
 static int backward_impl(const char* what, const fno_weights* w, const fno_weights_bwd* wb, const float* inputs,
                          const float* mask, const float* case_params, const float* dpreds, const fno_train_saved* saved,
                          const fno_grads* g, const fno_bwd_scratch* sc, const fno_workspace* ws, int batch, int act_dtype,
-                         void* stream, float* d_inputs, float* d_case_params) {
+                         void* stream, float* d_inputs, float* d_case_params, int accum = 0, int hand_off = 0,
+                         const float* add = nullptr) {
   char msg[128];
   if (!w || !wb || !inputs || !mask || !dpreds || !saved || !sc || !ws || batch <= 0 || bad_dtype(act_dtype)) {
     snprintf(msg, sizeof(msg), "%s: bad argument", what);
@@ -367,14 +380,14 @@ static int backward_impl(const char* what, const fno_weights* w, const fno_weigh
            : launch_project_bwd_tc<float>(a_l, dp, mk, pre, w->fc1_w, w->fc1_b, w->fc2_w, dout, sc->dz1, part_pb, &rows, nb, st);
     FNO_CUDA(e, "project_bwd_tc_kernel");
     if (!g) continue;   // data-only: the partial rows just written are never reduced
-    const int accum = b0 > 0 ? 1 : 0;
-    FNO_CUDA(launch_reduce_partials(part_pb, rows, project_bwd_row(), g->fc2_w, 2 * kProj, g->fc1_b, kProj, g->fc2_b, 2, accum, st),
+    const int acc_c = (accum || b0 > 0) ? 1 : 0;
+    FNO_CUDA(launch_reduce_partials(part_pb, rows, project_bwd_row(), g->fc2_w, 2 * kProj, g->fc1_b, kProj, g->fc2_b, 2, acc_c, st),
              "reduce(fc2.weight | fc1.bias | fc2.bias)");
     int n_co = 0;
     e = bf ? launch_chan_outer<float, __nv_bfloat16, 128, 32>(sc->dz1, a_l, part_co, &n_co, nb, st)
            : launch_chan_outer<float, float, 128, 32>(sc->dz1, a_l, part_co, &n_co, nb, st);
     FNO_CUDA(e, "chan_outer_kernel(fc1)");
-    FNO_CUDA(launch_reduce_partials(part_co, n_co, kProj * kC + kProj, g->fc1_w, kProj * kC, nullptr, 0, nullptr, 0, accum, st),
+    FNO_CUDA(launch_reduce_partials(part_co, n_co, kProj * kC + kProj, g->fc1_w, kProj * kC, nullptr, 0, nullptr, 0, acc_c, st),
              "reduce(fc1.weight)");
   }
   // ---- Fourier blocks, last to first
@@ -388,13 +401,13 @@ static int backward_impl(const char* what, const fno_weights* w, const fno_weigh
       cudaError_t e = bf ? launch_chan_outer<float, __nv_bfloat16, 32, 32>(dpre, saved->act[l], part_co, &n_co, batch, st)
                          : launch_chan_outer<float, float, 32, 32>(dpre, saved->act[l], part_co, &n_co, batch, st);
       FNO_CUDA(e, "chan_outer_kernel(w0)");
-      FNO_CUDA(launch_reduce_partials(part_co, n_co, kC * kC + kC, g->w0_w[l], kC * kC, g->w0_b[l], kC, nullptr, 0, 0, st),
+      FNO_CUDA(launch_reduce_partials(part_co, n_co, kC * kC + kC, g->w0_w[l], kC * kC, g->w0_b[l], kC, nullptr, 0, accum, st),
                "reduce(w0.weight | w0.bias)");
     }
     FNO_TRY(fno_spectral_dft_fwd(dpre, sc->gm, batch, FNO_ACT_F32, inv, 2.f * inv, stream));
     if (g) {
       FNO_CUDA(launch_spectral_wgrad(saved->xm[l], sc->gm, sc->gwk, batch, st), "spectral_wgrad_kernel");
-      FNO_TRY(fno_unpack_spectral_grads(sc->gwk, g->spec_w1[l], g->spec_w2[l], stream));
+      FNO_CUDA(launch_unpack_spectral(sc->gwk, g->spec_w1[l], g->spec_w2[l], accum, st), "unpack_spectral_kernel");
     }
     FNO_TRY(fno_mode_mix(sc->gm, wb->spec_wkT[l], ws->ym, batch, stream));
     FNO_TRY(fno_spectral_inv_kx(ws->ym, ws->z, batch, 1.f, 1.f, stream));
@@ -404,10 +417,12 @@ static int backward_impl(const char* what, const fno_weights* w, const fno_weigh
   }
   // sc->d[cur] = dL/da0, the gradient at the lift output (a bf16-stored a0 is differentiated straight through)
   if (g)
-    FNO_CUDA(launch_lift_bwd(sc->d[cur], inputs, mask, case_params, w->gx, w->gy, g->fc0_w, g->fc0_b, part_lb, batch, p, st),
+    FNO_CUDA(launch_lift_bwd(sc->d[cur], inputs, mask, case_params, w->gx, w->gy, g->fc0_w, g->fc0_b, part_lb, batch, p, accum,
+                             st),
              "lift_bwd_kernel");
   if (d_inputs || d_case_params)
-    FNO_CUDA(launch_lift_bwd_data(sc->d[cur], w->fc0_w, d_inputs, d_case_params, batch, p, st), "lift_bwd_data_kernel");
+    FNO_CUDA(launch_lift_bwd_data(sc->d[cur], w->fc0_w, d_inputs, d_case_params, hand_off ? add : nullptr, hand_off, batch, p, st),
+             "lift_bwd_data_kernel");
   return kOk;
 }
 
@@ -431,6 +446,82 @@ int fno_backward_inputs(const fno_weights* w, const fno_weights_bwd* wb, const f
   if ((reinterpret_cast<uintptr_t>(d_inputs) & 15) != 0) return fail(kErrArg, "fno_backward_inputs: d_inputs must be 16-byte aligned");
   return backward_impl("fno_backward_inputs", w, wb, inputs, mask, case_params, dpreds, saved, grads, scratch, ws, batch,
                        act_dtype, stream, d_inputs, d_case_params);
+}
+
+// ------------------------------------------------------------------------ training through a rollout (64x64 and grids)
+// Checks shared by the rollout training entry points: everything is validated before any device work.
+static int rollout_bwd_args(const char* what, const fno_weights* w, const fno_weights_bwd* wb, const float* inputs,
+                            const float* mask, const float* preds_seq, const float* dpreds_seq, int steps,
+                            const fno_train_saved* saved, const fno_grads* g, const fno_bwd_scratch* sc, const fno_workspace* ws,
+                            const float* carry, const float* d_inputs, const float* d_case_params, int batch) {
+  char msg[160];
+  if (steps < 1 || !w || !wb || !inputs || !mask || !dpreds_seq || !saved || !sc || !ws || batch <= 0 ||
+      (steps > 1 && (!preds_seq || !carry))) {
+    snprintf(msg, sizeof(msg), "%s: bad argument", what);
+    return fail(kErrArg, msg);
+  }
+  if (w->n_layers < 1 || w->n_layers > FNO_MAX_LAYERS) {
+    snprintf(msg, sizeof(msg), "%s: n_layers out of range", what);
+    return fail(kErrUnsupported, msg);
+  }
+  if (w->n_case_params < 0 || w->n_case_params > kMaxCaseParams) {
+    snprintf(msg, sizeof(msg), "%s: n_case_params out of range", what);
+    return fail(kErrArg, msg);
+  }
+  if (!g && !d_inputs && !d_case_params) {
+    snprintf(msg, sizeof(msg), "%s: no output requested", what);
+    return fail(kErrArg, msg);
+  }
+  if (!sc->d[0] || !sc->d[1] || !sc->dz1 || !sc->gm || !sc->gwk || !sc->partials || !ws->ym || !ws->z) {
+    snprintf(msg, sizeof(msg), "%s: null scratch buffer", what);
+    return fail(kErrArg, msg);
+  }
+  if ((carry && carry == d_inputs) || (carry && carry == dpreds_seq)) {
+    snprintf(msg, sizeof(msg), "%s: carry must be a buffer of its own", what);
+    return fail(kErrArg, msg);
+  }
+  return kOk;
+}
+
+int fno_rollout_forward_train(const fno_weights* w, const float* inputs, const float* mask, const float* case_params,
+                              float* preds_seq, int steps, const fno_train_saved* saved, const fno_workspace* ws, int batch,
+                              int act_dtype, void* stream) {
+  if (steps < 1 || !inputs || !preds_seq || batch <= 0) return fail(kErrArg, "fno_rollout_forward_train: bad argument");
+  const size_t frame = static_cast<size_t>(batch) * 2 * kHW;
+  const float* cur = inputs;
+  for (int s = 0; s < steps; ++s) {
+    float* nxt = preds_seq + static_cast<size_t>(s) * frame;
+    FNO_TRY(fno_forward_train(w, cur, mask, case_params, nxt, saved, ws, batch, act_dtype, stream));
+    cur = nxt;
+  }
+  return kOk;
+}
+
+int fno_rollout_backward(const fno_weights* w, const fno_weights_bwd* wb, const float* inputs, const float* mask,
+                         const float* case_params, const float* preds_seq, const float* dpreds_seq, int steps,
+                         const fno_train_saved* saved, const fno_grads* grads, const fno_bwd_scratch* scratch,
+                         const fno_workspace* ws, float* carry, float* d_inputs, float* d_case_params, int batch, int act_dtype,
+                         void* stream) {
+  const char* what = "fno_rollout_backward";
+  if (w && w->n_case_params == 0) d_case_params = nullptr;   // nothing to write
+  FNO_TRY(rollout_bwd_args(what, w, wb, inputs, mask, preds_seq, dpreds_seq, steps, saved, grads, scratch, ws, carry, d_inputs,
+                           d_case_params, batch));
+  if (bad_dtype(act_dtype)) return fail(kErrArg, "fno_rollout_backward: bad act_dtype");
+  if ((reinterpret_cast<uintptr_t>(d_inputs) | reinterpret_cast<uintptr_t>(carry) | reinterpret_cast<uintptr_t>(dpreds_seq)) & 15)
+    return fail(kErrArg, "fno_rollout_backward: d_inputs, carry and dpreds_seq must be 16-byte aligned");
+  const size_t frame = static_cast<size_t>(batch) * 2 * kHW;
+  if (d_case_params)   // every sweep step adds its share
+    FNO_CUDA(cudaMemsetAsync(d_case_params, 0, static_cast<size_t>(batch) * w->n_case_params * sizeof(float), S(stream)),
+             "memset(d_case_params)");
+  for (int s = steps - 1; s >= 0; --s) {
+    const float* x = s > 0 ? preds_seq + static_cast<size_t>(s - 1) * frame : inputs;
+    FNO_TRY(forward_train_body(w, x, mask, case_params, saved, ws, batch, act_dtype, stream));
+    const float* up = s == steps - 1 ? dpreds_seq + static_cast<size_t>(s) * frame : carry;
+    FNO_TRY(backward_impl(what, w, wb, x, mask, case_params, up, saved, grads, scratch, ws, batch, act_dtype, stream,
+                          s > 0 ? carry : d_inputs, d_case_params, s != steps - 1 ? 1 : 0, 1,
+                          s > 0 ? dpreds_seq + static_cast<size_t>(s - 1) * frame : nullptr));
+  }
+  return kOk;
 }
 
 int fno_multistep_metrics(const float* preds_seq, const float* label_u, const float* mask, float* sums, int steps,
@@ -549,9 +640,11 @@ int fno_grid_project_fwd(const float* act_in, const float* mask, const fno_weigh
 }
 
 // project backward over batch chunks of FNO_BWD_CHUNK (dz1 holds one chunk); gradients written when g_fc1_w is set
+// (added to with accum = 1)
 static int grid_project_bwd_impl(const float* act, const float* dpreds, const float* mask, const float* pre,
                                  const fno_weights* w, float* dpre_out, float* dz1, float* partials, float* g_fc1_w,
-                                 float* g_fc1_b, float* g_fc2_w, float* g_fc2_b, int batch, int h, int wd, cudaStream_t st) {
+                                 float* g_fc1_b, float* g_fc2_w, float* g_fc2_b, int batch, int h, int wd, cudaStream_t st,
+                                 int accum = 0) {
   const int hw = h * wd;
   float* part_pb = partials;
   float* part_co = partials + grid_partials_offset_co();
@@ -564,13 +657,13 @@ static int grid_project_bwd_impl(const float* act, const float* dpreds, const fl
                                      grads ? part_pb : nullptr, nb, hw, st),
              "grid_project_bwd_kernel");
     if (!grads) continue;
-    const int accum = b0 > 0 ? 1 : 0;
+    const int acc_c = (accum || b0 > 0) ? 1 : 0;
     FNO_CUDA(launch_reduce_partials(part_pb, grid_project_bwd_parts(nb, hw), grid_project_bwd_row(), g_fc2_w, 2 * kProj,
-                                    g_fc1_b, kProj, g_fc2_b, 2, accum, st),
+                                    g_fc1_b, kProj, g_fc2_b, 2, acc_c, st),
              "reduce(fc2.weight | fc1.bias | fc2.bias)");
     int n_co = 0;
     FNO_CUDA((launch_grid_chan_outer<kProj, kC>(dz1, act + act_off, part_co, &n_co, nb, hw, st)), "grid_chan_outer_kernel(fc1)");
-    FNO_CUDA(launch_reduce_partials(part_co, n_co, kProj * kC + kProj, g_fc1_w, kProj * kC, nullptr, 0, nullptr, 0, accum, st),
+    FNO_CUDA(launch_reduce_partials(part_co, n_co, kProj * kC + kProj, g_fc1_w, kProj * kC, nullptr, 0, nullptr, 0, acc_c, st),
              "reduce(fc1.weight)");
   }
   return kOk;
@@ -627,12 +720,10 @@ int fno_grid_rollout(const fno_weights* w, const float* inputs, const float* mas
   return kOk;
 }
 
-int fno_grid_forward_train(const fno_weights* w, const float* inputs, const float* mask, const float* case_params,
-                           float* preds, const fno_train_saved* saved, const fno_workspace* ws, int batch, int h, int wd,
-                           void* stream) {
-  FNO_TRY(grid_arg("fno_grid_forward_train", h, wd));
-  if (!w || !saved || !ws || !ws->ym || !ws->z || !saved->act[0]) return fail(kErrArg, "fno_grid_forward_train: bad argument");
-  if (w->n_layers < 1 || w->n_layers > FNO_MAX_LAYERS) return fail(kErrUnsupported, "fno_grid_forward_train: n_layers");
+// fno_grid_forward_train up to the saved set (lift and Fourier blocks, no projection)
+static int grid_forward_train_body(const fno_weights* w, const float* inputs, const float* mask, const float* case_params,
+                                   const fno_train_saved* saved, const fno_workspace* ws, int batch, int h, int wd,
+                                   void* stream) {
   FNO_TRY(fno_grid_lift_fwd(inputs, mask, case_params, w, static_cast<float*>(saved->act[0]), batch, h, wd, stream));
   for (int l = 0; l < w->n_layers; ++l) {
     if (!saved->act[l + 1] || !saved->pre[l] || !saved->xm[l])
@@ -640,7 +731,68 @@ int fno_grid_forward_train(const fno_weights* w, const float* inputs, const floa
     FNO_TRY(grid_block(w, l, static_cast<const float*>(saved->act[l]), static_cast<float*>(saved->act[l + 1]), saved->pre[l],
                        saved->xm[l], ws, batch, h, wd, stream));
   }
+  return kOk;
+}
+
+int fno_grid_forward_train(const fno_weights* w, const float* inputs, const float* mask, const float* case_params,
+                           float* preds, const fno_train_saved* saved, const fno_workspace* ws, int batch, int h, int wd,
+                           void* stream) {
+  FNO_TRY(grid_arg("fno_grid_forward_train", h, wd));
+  if (!w || !saved || !ws || !ws->ym || !ws->z || !saved->act[0]) return fail(kErrArg, "fno_grid_forward_train: bad argument");
+  if (w->n_layers < 1 || w->n_layers > FNO_MAX_LAYERS) return fail(kErrUnsupported, "fno_grid_forward_train: n_layers");
+  FNO_TRY(grid_forward_train_body(w, inputs, mask, case_params, saved, ws, batch, h, wd, stream));
   return fno_grid_project_fwd(static_cast<const float*>(saved->act[w->n_layers]), mask, w, preds, batch, h, wd, stream);
+}
+
+// The grid backward after argument checks; accum / hand_off / add as in backward_impl (the rollout sweep's modes)
+static int grid_backward_impl(const fno_weights* w, const fno_weights_bwd* wb, const float* inputs, const float* mask,
+                              const float* case_params, const float* dpreds, const fno_train_saved* saved, const fno_grads* g,
+                              const fno_bwd_scratch* sc, const fno_workspace* ws, float* d_inputs, float* d_case_params,
+                              int batch, int h, int wd, void* stream, int accum = 0, int hand_off = 0,
+                              const float* add = nullptr) {
+  cudaStream_t st = S(stream);
+  const int L = w->n_layers, p = w->n_case_params;
+  // ---- projection -> d[0] = dpre_{L-1}
+  FNO_TRY(grid_project_bwd_impl(static_cast<const float*>(saved->act[L]), dpreds, mask, saved->pre[L - 1], w, sc->d[0], sc->dz1,
+                                sc->partials, g ? g->fc1_w : nullptr, g ? g->fc1_b : nullptr, g ? g->fc2_w : nullptr,
+                                g ? g->fc2_b : nullptr, batch, h, wd, st, accum));
+  // ---- Fourier blocks, last to first
+  float* part_co = sc->partials + grid_partials_offset_co();
+  const float inv = 1.f / static_cast<float>(h * wd);
+  int cur = 0;
+  for (int l = L - 1; l >= 0; --l) {
+    float* dpre = sc->d[cur];
+    float* dnext = sc->d[cur ^ 1];
+    const float* act_l = static_cast<const float*>(saved->act[l]);
+    if (g) {
+      int n_co = 0;
+      FNO_CUDA((launch_grid_chan_outer<kC, kC>(dpre, act_l, part_co, &n_co, batch, h * wd, st)), "grid_chan_outer_kernel(w0)");
+      FNO_CUDA(launch_reduce_partials(part_co, n_co, kC * kC + kC, g->w0_w[l], kC * kC, g->w0_b[l], kC, nullptr, 0, accum, st),
+               "reduce(w0.weight | w0.bias)");
+    }
+    FNO_TRY(fno_grid_spectral_dft_fwd(dpre, sc->gm, batch, h, wd, inv, 2.f * inv, stream));
+    if (g) {
+      FNO_CUDA(launch_spectral_wgrad(saved->xm[l], sc->gm, sc->gwk, batch, st), "spectral_wgrad_kernel");
+      FNO_CUDA(launch_unpack_spectral(sc->gwk, g->spec_w1[l], g->spec_w2[l], accum, st), "unpack_spectral_kernel");
+    }
+    FNO_TRY(fno_mode_mix(sc->gm, wb->spec_wkT[l], ws->ym, batch, stream));
+    FNO_TRY(fno_grid_spectral_inv_kx(ws->ym, static_cast<float*>(ws->z), batch, h, wd, 1.f, 1.f, stream));
+    FNO_TRY(fno_grid_block_out(l > 0 ? FNO_EPI_MUL_DGELU : FNO_EPI_PLAIN, static_cast<const float*>(ws->z), dpre, wb->w0[l],
+                               nullptr, dnext, nullptr, l > 0 ? saved->pre[l - 1] : nullptr, batch, h, wd, stream));
+    cur ^= 1;
+  }
+  // ---- lift: fc0 gradients and the data adjoint of dL/da0 = d[cur]
+  float* part_lb = g ? sc->partials + grid_partials_offset_lb() : nullptr;
+  if (g || d_inputs || d_case_params) {
+    FNO_CUDA(launch_grid_lift_bwd(sc->d[cur], inputs, mask, case_params, w->gx, w->gy, w->fc0_w, part_lb, d_inputs,
+                                  d_case_params, hand_off ? add : nullptr, hand_off, batch, p, h, wd, st),
+             "grid_lift_bwd_kernel");
+  }
+  if (g)
+    FNO_CUDA(launch_reduce_partials(part_lb, grid_lift_bwd_parts(batch), grid_lift_bwd_row(), g->fc0_w, kC * (5 + p), g->fc0_b,
+                                    kC, nullptr, 0, accum, st),
+             "reduce(fc0.weight | fc0.bias)");
+  return kOk;
 }
 
 int fno_grid_backward(const fno_weights* w, const fno_weights_bwd* wb, const float* inputs, const float* mask,
@@ -657,48 +809,48 @@ int fno_grid_backward(const fno_weights* w, const fno_weights_bwd* wb, const flo
   if (!g && !d_inputs && !d_case_params) return fail(kErrArg, "fno_grid_backward: no output requested");
   if (!sc->d[0] || !sc->d[1] || !sc->dz1 || !sc->gm || !sc->gwk || !sc->partials || !ws->ym || !ws->z)
     return fail(kErrArg, "fno_grid_backward: null scratch buffer");
-  cudaStream_t st = S(stream);
-  const int L = w->n_layers, p = w->n_case_params;
-  // ---- projection -> d[0] = dpre_{L-1}
-  FNO_TRY(grid_project_bwd_impl(static_cast<const float*>(saved->act[L]), dpreds, mask, saved->pre[L - 1], w, sc->d[0], sc->dz1,
-                                sc->partials, g ? g->fc1_w : nullptr, g ? g->fc1_b : nullptr, g ? g->fc2_w : nullptr,
-                                g ? g->fc2_b : nullptr, batch, h, wd, st));
-  // ---- Fourier blocks, last to first
-  float* part_co = sc->partials + grid_partials_offset_co();
-  const float inv = 1.f / static_cast<float>(h * wd);
-  int cur = 0;
-  for (int l = L - 1; l >= 0; --l) {
-    float* dpre = sc->d[cur];
-    float* dnext = sc->d[cur ^ 1];
-    const float* act_l = static_cast<const float*>(saved->act[l]);
-    if (g) {
-      int n_co = 0;
-      FNO_CUDA((launch_grid_chan_outer<kC, kC>(dpre, act_l, part_co, &n_co, batch, h * wd, st)), "grid_chan_outer_kernel(w0)");
-      FNO_CUDA(launch_reduce_partials(part_co, n_co, kC * kC + kC, g->w0_w[l], kC * kC, g->w0_b[l], kC, nullptr, 0, 0, st),
-               "reduce(w0.weight | w0.bias)");
-    }
-    FNO_TRY(fno_grid_spectral_dft_fwd(dpre, sc->gm, batch, h, wd, inv, 2.f * inv, stream));
-    if (g) {
-      FNO_CUDA(launch_spectral_wgrad(saved->xm[l], sc->gm, sc->gwk, batch, st), "spectral_wgrad_kernel");
-      FNO_TRY(fno_unpack_spectral_grads(sc->gwk, g->spec_w1[l], g->spec_w2[l], stream));
-    }
-    FNO_TRY(fno_mode_mix(sc->gm, wb->spec_wkT[l], ws->ym, batch, stream));
-    FNO_TRY(fno_grid_spectral_inv_kx(ws->ym, static_cast<float*>(ws->z), batch, h, wd, 1.f, 1.f, stream));
-    FNO_TRY(fno_grid_block_out(l > 0 ? FNO_EPI_MUL_DGELU : FNO_EPI_PLAIN, static_cast<const float*>(ws->z), dpre, wb->w0[l],
-                               nullptr, dnext, nullptr, l > 0 ? saved->pre[l - 1] : nullptr, batch, h, wd, stream));
-    cur ^= 1;
+  return grid_backward_impl(w, wb, inputs, mask, case_params, dpreds, saved, g, sc, ws, d_inputs, d_case_params, batch, h, wd,
+                            stream);
+}
+
+int fno_grid_rollout_forward_train(const fno_weights* w, const float* inputs, const float* mask, const float* case_params,
+                                   float* preds_seq, int steps, const fno_train_saved* saved, const fno_workspace* ws,
+                                   int batch, int h, int wd, void* stream) {
+  FNO_TRY(grid_arg("fno_grid_rollout_forward_train", h, wd));
+  if (steps < 1 || !inputs || !preds_seq || batch <= 0) return fail(kErrArg, "fno_grid_rollout_forward_train: bad argument");
+  const size_t frame = static_cast<size_t>(batch) * 2 * h * wd;
+  const float* cur = inputs;
+  for (int s = 0; s < steps; ++s) {
+    float* nxt = preds_seq + static_cast<size_t>(s) * frame;
+    FNO_TRY(fno_grid_forward_train(w, cur, mask, case_params, nxt, saved, ws, batch, h, wd, stream));
+    cur = nxt;
   }
-  // ---- lift: fc0 gradients and the data adjoint of dL/da0 = d[cur]
-  float* part_lb = g ? sc->partials + grid_partials_offset_lb() : nullptr;
-  if (g || d_inputs || d_case_params) {
-    FNO_CUDA(launch_grid_lift_bwd(sc->d[cur], inputs, mask, case_params, w->gx, w->gy, w->fc0_w, part_lb, d_inputs,
-                                  d_case_params, batch, p, h, wd, st),
-             "grid_lift_bwd_kernel");
+  return kOk;
+}
+
+int fno_grid_rollout_backward(const fno_weights* w, const fno_weights_bwd* wb, const float* inputs, const float* mask,
+                              const float* case_params, const float* preds_seq, const float* dpreds_seq, int steps,
+                              const fno_train_saved* saved, const fno_grads* grads, const fno_bwd_scratch* scratch,
+                              const fno_workspace* ws, float* carry, float* d_inputs, float* d_case_params, int batch, int h,
+                              int wd, void* stream) {
+  const char* what = "fno_grid_rollout_backward";
+  FNO_TRY(grid_arg(what, h, wd));
+  if (w && w->n_case_params == 0) d_case_params = nullptr;   // nothing to write
+  FNO_TRY(rollout_bwd_args(what, w, wb, inputs, mask, preds_seq, dpreds_seq, steps, saved, grads, scratch, ws, carry, d_inputs,
+                           d_case_params, batch));
+  if (!saved->act[0]) return fail(kErrArg, "fno_grid_rollout_backward: null saved buffer");
+  const size_t frame = static_cast<size_t>(batch) * 2 * h * wd;
+  if (d_case_params)   // every sweep step adds its share
+    FNO_CUDA(cudaMemsetAsync(d_case_params, 0, static_cast<size_t>(batch) * w->n_case_params * sizeof(float), S(stream)),
+             "memset(d_case_params)");
+  for (int s = steps - 1; s >= 0; --s) {
+    const float* x = s > 0 ? preds_seq + static_cast<size_t>(s - 1) * frame : inputs;
+    FNO_TRY(grid_forward_train_body(w, x, mask, case_params, saved, ws, batch, h, wd, stream));
+    const float* up = s == steps - 1 ? dpreds_seq + static_cast<size_t>(s) * frame : carry;
+    FNO_TRY(grid_backward_impl(w, wb, x, mask, case_params, up, saved, grads, scratch, ws, s > 0 ? carry : d_inputs,
+                               d_case_params, batch, h, wd, stream, s != steps - 1 ? 1 : 0, 1,
+                               s > 0 ? dpreds_seq + static_cast<size_t>(s - 1) * frame : nullptr));
   }
-  if (g)
-    FNO_CUDA(launch_reduce_partials(part_lb, grid_lift_bwd_parts(batch), grid_lift_bwd_row(), g->fc0_w, kC * (5 + p), g->fc0_b,
-                                    kC, nullptr, 0, 0, st),
-             "reduce(fc0.weight | fc0.bias)");
   return kOk;
 }
 

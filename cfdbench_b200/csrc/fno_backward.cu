@@ -356,7 +356,8 @@ __global__ void __launch_bounds__(kLbThreads)
   }
 }
 
-// g_w[c][q] += sum_y partial[y][c][q], g_b[c] += sum_y partial[y][c][nin]   (fixed order)
+// g_w[c][q] = sum_y partial[y][c][q], g_b[c] = sum_y partial[y][c][nin]   (fixed order); kAccum: += instead of =
+template <bool kAccum>
 __global__ void lift_bwd_reduce_kernel(const float* __restrict__ partial, int n_parts, int nin, float* __restrict__ g_w,
                                        float* __restrict__ g_b) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -364,20 +365,22 @@ __global__ void lift_bwd_reduce_kernel(const float* __restrict__ partial, int n_
   const int c = i / (nin + 1), q = i % (nin + 1);
   float s = 0.f;
   for (int y = 0; y < n_parts; ++y) s += partial[(static_cast<size_t>(y) * kC + c) * (nin + 1) + q];
-  if (q < nin) g_w[c * nin + q] = s;   // the only contribution: no memset of the gradient needed
-  else g_b[c] = s;
+  float* dst = q < nin ? g_w + c * nin + q : g_b + c;
+  if constexpr (kAccum) *dst += s;   // a later step of the rollout backward's sweep
+  else *dst = s;                     // the only contribution: no memset of the gradient needed
 }
 
 cudaError_t launch_lift_bwd(const float* da0, const float* inputs, const float* mask, const float* params,
                             const float* gx, const float* gy, float* g_w, float* g_b, float* partial, int batch, int p,
-                            cudaStream_t stream) {
+                            int accumulate, cudaStream_t stream) {
   if (p < 0 || p > kMaxCaseParams) return cudaErrorInvalidValue;
   dim3 grid(kC, batch < 16 ? batch : 16);
   lift_bwd_kernel<<<grid, kLbThreads, 0, stream>>>(da0, inputs, mask, params, gx, gy, partial, batch, p);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return e;
   const int n = kC * (5 + p + 1);
-  lift_bwd_reduce_kernel<<<(n + 127) / 128, 128, 0, stream>>>(partial, static_cast<int>(grid.y), 5 + p, g_w, g_b);
+  auto reduce = accumulate ? lift_bwd_reduce_kernel<true> : lift_bwd_reduce_kernel<false>;
+  reduce<<<(n + 127) / 128, 128, 0, stream>>>(partial, static_cast<int>(grid.y), 5 + p, g_w, g_b);
   return cudaGetLastError();
 }
 
@@ -389,14 +392,19 @@ cudaError_t launch_lift_bwd(const float* da0, const float* inputs, const float* 
 // index order): no atomics, bit-reproducible.  Thread = kLdVec groups of 4 consecutive pixels, 16-byte loads and stores;
 // the case-parameter weights are applied to each thread's per-channel pixel sum on the fly, so only p values per thread
 // are reduced at the end.  One pass over d_a0 (float32 in both storage modes, 134 MB at B = 256).
+// kHandOff (the rollout backward's sweep): d_inputs = (sum_o fc0_w[o][c] d_a0) + add, where `add` (or null) is the
+// upstream gradient of the previous step's prediction, so d_inputs becomes that step's whole upstream gradient in this
+// one pass; d_params += instead of = (the case parameters feed every step).
 constexpr int kLdThreads = 512;
 constexpr int kLdVec = kHW / (4 * kLdThreads);   // float4 groups per thread and channel
 
+template <bool kHandOff>
 __global__ void __launch_bounds__(kLdThreads)
     lift_bwd_data_kernel(const float* __restrict__ da0,     // [B][32][4096]
                          const float* __restrict__ fc0_w,   // [32][5+p]
                          float* __restrict__ d_inputs,      // [B][2][4096] or null
                          float* __restrict__ d_params,      // [B][p] or null
+                         const float* __restrict__ add,     // [B][2][4096] or null (kHandOff only)
                          int p) {
   __shared__ float wu[kC], wv[kC];
   __shared__ __align__(16) float wp[kC][kMaxCaseParams];   // columns 5..5+p, zero-padded to 16
@@ -450,6 +458,18 @@ __global__ void __launch_bounds__(kLdThreads)
   if (d_inputs != nullptr) {
     float4* u_out = reinterpret_cast<float4*>(d_inputs + static_cast<size_t>(b) * 2 * kHW);
     float4* v_out = u_out + kHW / 4;
+    if constexpr (kHandOff) {
+      if (add != nullptr) {
+        const float4* u_add = reinterpret_cast<const float4*>(add + static_cast<size_t>(b) * 2 * kHW);
+        const float4* v_add = u_add + kHW / 4;
+#pragma unroll
+        for (int k = 0; k < kLdVec; ++k) {
+          const float4 a = __ldcs(u_add + k * kLdThreads + tid), c = __ldcs(v_add + k * kLdThreads + tid);
+          du[k].x += a.x; du[k].y += a.y; du[k].z += a.z; du[k].w += a.w;
+          dv[k].x += c.x; dv[k].y += c.y; dv[k].z += c.z; dv[k].w += c.w;
+        }
+      }
+    }
 #pragma unroll
     for (int k = 0; k < kLdVec; ++k) {
       u_out[k * kLdThreads + tid] = du[k];
@@ -468,17 +488,23 @@ __global__ void __launch_bounds__(kLdThreads)
     if (tid < p) {
       float t = 0.f;
       for (int w = 0; w < kLdThreads / 32; ++w) t += red[w][tid];   // warp order: fixed
-      d_params[static_cast<size_t>(b) * p + tid] = t;
+      if constexpr (kHandOff) d_params[static_cast<size_t>(b) * p + tid] += t;
+      else d_params[static_cast<size_t>(b) * p + tid] = t;
     }
   }
 }
 
-cudaError_t launch_lift_bwd_data(const float* da0, const float* fc0_w, float* d_inputs, float* d_params, int batch, int p,
-                                 cudaStream_t stream) {
+// hand_off = 0: the single-step data adjoint (d_inputs, d_params written; `add` must be null).  hand_off = 1: the
+// rollout sweep's mode described above the kernel.
+cudaError_t launch_lift_bwd_data(const float* da0, const float* fc0_w, float* d_inputs, float* d_params, const float* add,
+                                 int hand_off, int batch, int p, cudaStream_t stream) {
   if (p < 0 || p > kMaxCaseParams) return cudaErrorInvalidValue;
   if (p == 0) d_params = nullptr;
   if (d_inputs == nullptr && d_params == nullptr) return cudaSuccess;
-  lift_bwd_data_kernel<<<batch, kLdThreads, 0, stream>>>(da0, fc0_w, d_inputs, d_params, p);
+  if (hand_off)
+    lift_bwd_data_kernel<true><<<batch, kLdThreads, 0, stream>>>(da0, fc0_w, d_inputs, d_params, add, p);
+  else
+    lift_bwd_data_kernel<false><<<batch, kLdThreads, 0, stream>>>(da0, fc0_w, d_inputs, d_params, nullptr, p);
   return cudaGetLastError();
 }
 

@@ -644,15 +644,18 @@ template cudaError_t launch_grid_chan_outer<kC, kC>(const float*, const float*, 
 // -- the case-parameter columns as param * sum(dL/da0) -- to the CTA's running row in shared memory; d_case_params[b][q] =
 // sum_j fc0_w[j][5+q] sum(dL/da0[j]); d_inputs[b][c][p] = sum_j fc0_w[j][c] dL/da0[b][j][p].
 // Partial row: fc0.weight (32 x (5+p)) | fc0.bias (32), stride kGlbRow.
+// kHandOff (the rollout backward's sweep): d_inputs = (sum_j fc0_w[j][c] dL/da0) + add, `add` (or null) being the upstream
+// gradient of the previous step's prediction, and d_case_params += instead of =.
 constexpr int kGlbThreads = 256;
 constexpr int kGlbParts = 264;
 constexpr int kGlbRow = kC * (5 + kMaxCaseParams) + kC;
 
+template <bool kHandOff>
 __global__ void __launch_bounds__(kGlbThreads)
     grid_lift_bwd_kernel(const float* __restrict__ da0, const float* __restrict__ inputs, const float* __restrict__ mask,
                          const float* __restrict__ params, const float* __restrict__ gx, const float* __restrict__ gy,
                          const float* __restrict__ fc0_w, float* __restrict__ partial, float* __restrict__ d_inputs,
-                         float* __restrict__ d_params, int batch, int p, int h, int wd) {
+                         float* __restrict__ d_params, const float* __restrict__ add, int batch, int p, int h, int wd) {
   __shared__ float sums[kC][6];
   __shared__ float accw[kC * (5 + kMaxCaseParams)];
   __shared__ float accb[kC];
@@ -712,12 +715,14 @@ __global__ void __launch_bounds__(kGlbThreads)
       if (d_params && tid < p) {
         float d = 0.f;
         for (int jj = 0; jj < kC; ++jj) d = fmaf(fc0_w[jj * nin + 5 + tid], sums[jj][5], d);
-        d_params[b * p + tid] = d;
+        if constexpr (kHandOff) d_params[b * p + tid] += d;
+        else d_params[b * p + tid] = d;
       }
     } else {
       __syncthreads();   // wuv visible
     }
     if (d_inputs) {
+      const float* add_b = add != nullptr ? add + static_cast<size_t>(b) * 2 * hw : nullptr;
       for (int pix = tid; pix < hw; pix += kGlbThreads) {
         float du = 0.f, dv = 0.f;
 #pragma unroll 8
@@ -725,6 +730,12 @@ __global__ void __launch_bounds__(kGlbThreads)
           const float d = db[static_cast<size_t>(jj) * hw + pix];
           du = fmaf(wuv[0][jj], d, du);
           dv = fmaf(wuv[1][jj], d, dv);
+        }
+        if constexpr (kHandOff) {
+          if (add_b != nullptr) {
+            du += add_b[pix];
+            dv += add_b[hw + pix];
+          }
         }
         d_inputs[(static_cast<size_t>(b) * 2 + 0) * hw + pix] = du;
         d_inputs[(static_cast<size_t>(b) * 2 + 1) * hw + pix] = dv;
@@ -742,12 +753,18 @@ __global__ void __launch_bounds__(kGlbThreads)
 int grid_lift_bwd_parts(int batch) { return batch < kGlbParts ? batch : kGlbParts; }
 int grid_lift_bwd_row() { return kGlbRow; }
 
+// hand_off = 0: the single-step backward (`add` must be null); 1: the rollout sweep's mode described above the kernel
 cudaError_t launch_grid_lift_bwd(const float* da0, const float* inputs, const float* mask, const float* params,
                                  const float* gx, const float* gy, const float* fc0_w, float* partial, float* d_inputs,
-                                 float* d_params, int batch, int p, int h, int wd, cudaStream_t stream) {
+                                 float* d_params, const float* add, int hand_off, int batch, int p, int h, int wd,
+                                 cudaStream_t stream) {
   if (p < 0 || p > kMaxCaseParams) return cudaErrorInvalidValue;
-  grid_lift_bwd_kernel<<<grid_lift_bwd_parts(batch), kGlbThreads, 0, stream>>>(da0, inputs, mask, params, gx, gy, fc0_w,
-                                                                               partial, d_inputs, d_params, batch, p, h, wd);
+  if (hand_off)
+    grid_lift_bwd_kernel<true><<<grid_lift_bwd_parts(batch), kGlbThreads, 0, stream>>>(
+        da0, inputs, mask, params, gx, gy, fc0_w, partial, d_inputs, d_params, add, batch, p, h, wd);
+  else
+    grid_lift_bwd_kernel<false><<<grid_lift_bwd_parts(batch), kGlbThreads, 0, stream>>>(
+        da0, inputs, mask, params, gx, gy, fc0_w, partial, d_inputs, d_params, nullptr, batch, p, h, wd);
   return cudaGetLastError();
 }
 

@@ -318,7 +318,9 @@ cudaError_t launch_pack_spectral(const void* w1, const void* w2, void* wk, int c
   return cudaGetLastError();
 }
 
-// inverse of the pack for gradients: gWk[k][i][o] -> gw1/gw2 (Cin, Cout, 12, 12)
+// inverse of the pack for gradients: gWk[k][i][o] -> gw1/gw2 (Cin, Cout, 12, 12).  kAccum: add to gw1/gw2 instead of
+// overwriting them (the rollout backward sums the steps of its sweep into one gradient)
+template <bool kAccum>
 __global__ void unpack_spectral_kernel(const float2* __restrict__ gwk, float2* __restrict__ gw1,
                                        float2* __restrict__ gw2) {
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;  // over (i*32+o)*144 + kk for both halves
@@ -328,13 +330,20 @@ __global__ void unpack_spectral_kernel(const float2* __restrict__ gwk, float2* _
   const int io = r / (kM1 * kM2), kk = r % (kM1 * kM2);
   const int k = (half * kM1 + kk / kM2) * kM2 + kk % kM2;
   const float2 v = gwk[static_cast<size_t>(k) * kC * kC + io];
-  (half ? gw2 : gw1)[r] = v;
+  float2* dst = (half ? gw2 : gw1) + r;
+  if constexpr (kAccum) {
+    const float2 o = *dst;
+    *dst = make_float2(o.x + v.x, o.y + v.y);
+  } else {
+    *dst = v;
+  }
 }
 
-cudaError_t launch_unpack_spectral(const void* gwk, void* gw1, void* gw2, cudaStream_t stream) {
+cudaError_t launch_unpack_spectral(const void* gwk, void* gw1, void* gw2, int accumulate, cudaStream_t stream) {
   const int n = 2 * kC * kC * kM1 * kM2;
-  unpack_spectral_kernel<<<(n + 255) / 256, 256, 0, stream>>>(static_cast<const float2*>(gwk), static_cast<float2*>(gw1),
-                                                             static_cast<float2*>(gw2));
+  auto kern = accumulate ? unpack_spectral_kernel<true> : unpack_spectral_kernel<false>;
+  kern<<<(n + 255) / 256, 256, 0, stream>>>(static_cast<const float2*>(gwk), static_cast<float2*>(gw1),
+                                            static_cast<float2*>(gw2));
   return cudaGetLastError();
 }
 

@@ -12,6 +12,8 @@ Extras that the reference does not have (all optional, defaults keep reference b
   * `generate_many(..)` runs the whole rollout in one native call; host tensors in -> host tensors out
     through `fno_rollout_host` (H2D + rollout + D2H on one stream).
   * `enable_data_parallel()`: all-reduce of one flat gradient buffer (NCCL) inside backward.
+  * `rollout(..)`: a K-step rollout as one differentiable call whose backward recomputes each step, so its memory
+    grows by frames, not by saved activations, with K.
 Frames: 64x64 runs the 64x64 kernels (either storage mode); any other H x W with 24 <= H, W <= 128 (CFDBench's tube
 and dam problems: 66x65) runs the grid-generic fp32 kernels (fno_grid_* in the C ABI), routed by `inputs.shape[-2:]`.
 Like the reference, `forward` / `generate` are differentiable w.r.t. `inputs` and `case_params` (not `mask`), also with
@@ -111,6 +113,37 @@ class _TrainFn(torch.autograd.Function):
         return (None, d_inputs, None, d_cp, *grads)
 
 
+class _RolloutFn(torch.autograd.Function):
+    """One autograd node for a whole K-step rollout (backpropagation through time).  Forward = the native rollout
+    training forward: K training forwards into ONE reused saved set, keeping only the K predicted frames.  Backward = one
+    native sweep, s = K-1 .. 0, that recomputes step s's saved set from its stored input frame and runs step s's backward
+    with the upstream gradient dpreds_s + carry (carry = dL/d(frame fed to step s+1)), accumulating the parameter and
+    case-parameter gradients.  Memory: the K+1 frames and one saved set instead of K saved sets."""
+
+    @staticmethod
+    def forward(ctx, model: "Fno2d", inputs: Tensor, mask: Tensor, case_params: Tensor, steps: int, *params: Tensor):
+        if mask.requires_grad:
+            raise NotImplementedError("cfdbench_b200.Fno2d: gradients w.r.t. the mask are not implemented (inputs, "
+                                      "case_params and parameters are differentiable)")
+        seq = model._native_rollout_train(inputs, mask, case_params, steps)
+        ctx.model, ctx.steps = model, steps
+        ctx.save_for_backward(inputs, mask, case_params, seq)
+        return seq
+
+    @staticmethod
+    def backward(ctx, dseq: Tensor):
+        inputs, mask, case_params, seq = ctx.saved_tensors
+        model: "Fno2d" = ctx.model
+        need = ctx.needs_input_grad   # (model, inputs, mask, case_params, steps, *params)
+        d_inputs = torch.empty_like(inputs) if need[1] else None
+        d_cp = torch.empty_like(case_params) if need[3] else None
+        grads = model._native_rollout_backward(inputs, mask, case_params, seq, dseq.contiguous().float(), ctx.steps,
+                                               any(need[5:]), d_inputs, d_cp)
+        if grads is None:
+            grads = [None] * (len(need) - 5)
+        return (None, d_inputs, None, d_cp, None, *grads)
+
+
 class Fno2d(AutoCfdModel):
     def __init__(
         self,
@@ -178,6 +211,10 @@ class Fno2d(AutoCfdModel):
         # True: 64x64 frames in float32 storage also run the grid-generic kernels (fno_grid_*), which cross-checks the two
         # paths; False (default): 64x64 frames run the 64x64 kernels
         self.generic_grid_at_64 = False
+        # graphs of `rollout`'s training forward and backward sweep, one capture per (batch, steps, grid, storage[, which
+        # gradients]).  They read graph-owned copies of the packed weights, refreshed before a replay when the weights
+        # changed, so they survive optimizer steps (the graphs above are dropped when the weights change).
+        self._train_graphs: dict = {}
 
     # ------------------------------------------------------------------------------------ plumbing
     def invalidate_packed(self) -> None:
@@ -189,6 +226,7 @@ class Fno2d(AutoCfdModel):
         self._packed = {}
         self._graphs = {}
         self._ws_cache = {}
+        self._train_graphs = {}
 
     def _apply(self, fn, *args, **kwargs):
         out = super()._apply(fn, *args, **kwargs)
@@ -462,6 +500,25 @@ class Fno2d(AutoCfdModel):
             off += n
         return out, off
 
+    def _grad_buffers(self):
+        """One flat float32 gradient buffer, its per-parameter views (parameter order) and the FnoGrads struct."""
+        layout, total = self._grad_layout()
+        flat = torch.empty(total, dtype=torch.float32, device=self.device)
+        views: Dict[str, Tensor] = {}
+        for name, p, off, n in layout:
+            seg = flat[off:off + n]
+            views[name] = torch.view_as_complex(seg.view(*p.shape, 2)) if p.is_complex() else seg.view(p.shape)
+        g = _lib.FnoGrads()
+        g.fc0_w, g.fc0_b = views["fc0.weight"].data_ptr(), views["fc0.bias"].data_ptr()
+        for l in range(self.num_layers):
+            g.spec_w1[l] = views[f"blocks.{l}.conv0.weights1"].data_ptr()
+            g.spec_w2[l] = views[f"blocks.{l}.conv0.weights2"].data_ptr()
+            g.w0_w[l] = views[f"blocks.{l}.w0.weight"].data_ptr()
+            g.w0_b[l] = views[f"blocks.{l}.w0.bias"].data_ptr()
+        g.fc1_w, g.fc1_b = views["fc1.weight"].data_ptr(), views["fc1.bias"].data_ptr()
+        g.fc2_w, g.fc2_b = views["fc2.weight"].data_ptr(), views["fc2.bias"].data_ptr()
+        return flat, views, g
+
     def _native_backward(self, inputs, mask4, case_params, dpreds, saved_native, want_params: bool = True,
                          d_inputs: Optional[Tensor] = None, d_cp: Optional[Tensor] = None):
         """Parameter gradients in parameter order (None when `want_params` is false), from one native call:
@@ -481,21 +538,7 @@ class Fno2d(AutoCfdModel):
         ws, _ = self._grid_workspace(b, gh, gw) if grid else self._workspace(b)
         g = None
         if want_params:
-            layout, total = self._grad_layout()
-            flat = torch.empty(total, dtype=torch.float32, device=dev)
-            views: Dict[str, Tensor] = {}
-            for name, p, off, n in layout:
-                seg = flat[off:off + n]
-                views[name] = torch.view_as_complex(seg.view(*p.shape, 2)) if p.is_complex() else seg.view(p.shape)
-            g = _lib.FnoGrads()
-            g.fc0_w, g.fc0_b = views["fc0.weight"].data_ptr(), views["fc0.bias"].data_ptr()
-            for l in range(L):
-                g.spec_w1[l] = views[f"blocks.{l}.conv0.weights1"].data_ptr()
-                g.spec_w2[l] = views[f"blocks.{l}.conv0.weights2"].data_ptr()
-                g.w0_w[l] = views[f"blocks.{l}.w0.weight"].data_ptr()
-                g.w0_b[l] = views[f"blocks.{l}.w0.bias"].data_ptr()
-            g.fc1_w, g.fc1_b = views["fc1.weight"].data_ptr(), views["fc1.bias"].data_ptr()
-            g.fc2_w, g.fc2_b = views["fc2.weight"].data_ptr(), views["fc2.bias"].data_ptr()
+            flat, views, g = self._grad_buffers()
         d0 = torch.empty(b, HIDDEN, gh, gw, dtype=torch.float32, device=dev)
         d1 = torch.empty(b, HIDDEN, gh, gw, dtype=torch.float32, device=dev)
         dz1 = torch.empty(min(b, _lib.BWD_CHUNK), PROJ, gh, gw, dtype=torch.float32, device=dev)
@@ -521,6 +564,209 @@ class Fno2d(AutoCfdModel):
         if g is None:   # data-only backward: no parameter gradients, nothing to all-reduce
             return None
         if self._dp_enabled:   # one all-reduce (NCCL: ReduceOp.AVG, no division kernel) of the whole flat buffer
+            from .dp import allreduce_mean_
+            allreduce_mean_(flat, self._dp_group)
+        return [views[name] for name, _ in self.named_parameters()]
+
+    # ---------------------------------------------------------------- training through a rollout (`rollout`)
+    def _rollout_state(self, b: int, gh: int, gw: int, grid: bool) -> dict:
+        """The buffers `rollout` reuses across steps and calls: one saved set, the backward scratch (two d buffers,
+        dz1, gm, gwk, partials) and the carry frame."""
+        key = ("rollout_train", b, gh, gw, grid, self.act_dtype, self.device)
+        st = self._ws_cache.get(key)
+        if st is None:
+            lib = _lib.load()
+            dev, L = self.device, self.num_layers
+            adt = torch.float32 if grid else self._act_torch_dtype()
+            acts = [torch.empty(b, HIDDEN, gh, gw, dtype=adt, device=dev) for _ in range(L + 1)]
+            pres = [torch.empty(b, HIDDEN, gh, gw, dtype=torch.float32, device=dev) for _ in range(L)]
+            xms = [torch.empty(NMODES, b, HIDDEN, dtype=torch.complex64, device=dev) for _ in range(L)]
+            sv = _lib.FnoTrainSaved()
+            for l in range(L + 1):
+                sv.act[l] = acts[l].data_ptr()
+            for l in range(L):
+                sv.pre[l], sv.xm[l] = pres[l].data_ptr(), xms[l].data_ptr()
+            nbytes = lib.fno_grid_bwd_partials_bytes(gh, gw) if grid else lib.fno_bwd_partials_bytes()
+            bufs = dict(
+                d0=torch.empty(b, HIDDEN, gh, gw, dtype=torch.float32, device=dev),
+                d1=torch.empty(b, HIDDEN, gh, gw, dtype=torch.float32, device=dev),
+                dz1=torch.empty(min(b, _lib.BWD_CHUNK), PROJ, gh, gw, dtype=torch.float32, device=dev),
+                gm=torch.empty(NMODES, b, HIDDEN, dtype=torch.complex64, device=dev),
+                gwk=torch.empty(NMODES, HIDDEN, HIDDEN, dtype=torch.complex64, device=dev),
+                partials=torch.empty(nbytes, dtype=torch.uint8, device=dev),
+                carry=torch.empty(b, self.out_chan, gh, gw, dtype=torch.float32, device=dev),
+            )
+            sc = _lib.FnoBwdScratch()
+            sc.d[0], sc.d[1] = bufs["d0"].data_ptr(), bufs["d1"].data_ptr()
+            sc.dz1, sc.gm, sc.gwk = bufs["dz1"].data_ptr(), bufs["gm"].data_ptr(), bufs["gwk"].data_ptr()
+            sc.partials = bufs["partials"].data_ptr()
+            st = dict(sv=sv, sc=sc, bufs=bufs, saved=(acts, pres, xms))
+            if len(self._ws_cache) > 16:
+                self._ws_cache.clear()
+            self._ws_cache[key] = st
+        return st
+
+    def _static_weights(self, pk: dict, gh: int, gw: int, grid: bool) -> dict:
+        """Graph-owned copies of the packed weight images (and coordinate tables) with the weight structs pointing at
+        them; the parameters themselves are read in place.  `_refresh_static_weights` copies a new packing in."""
+        src = self._grid_struct(pk, gh, gw) if grid else pk["struct"]
+        wk = [torch.empty_like(t) for t in pk["wk"]]
+        w0t = [torch.empty_like(t) for t in pk["w0t"]]
+        wkT = [torch.empty_like(t) for t in pk["wkT"]]
+        gx = torch.empty(gh, dtype=torch.float32, device=self.device)
+        gy = torch.empty(gw, dtype=torch.float32, device=self.device)
+        st = _lib.FnoWeights.from_buffer_copy(src)
+        sb = _lib.FnoWeightsBwd.from_buffer_copy(pk["struct_bwd"])
+        for l in range(self.num_layers):
+            st.spec_wk[l], st.w0t[l], sb.spec_wkT[l] = wk[l].data_ptr(), w0t[l].data_ptr(), wkT[l].data_ptr()
+        st.gx, st.gy = gx.data_ptr(), gy.data_ptr()
+        return dict(struct=st, struct_bwd=sb, dst=wk + w0t + wkT + [gx, gy], src=None)
+
+    def _refresh_static_weights(self, sw: dict, pk: dict, gh: int, gw: int, grid: bool) -> None:
+        if sw["src"] is pk:
+            return
+        if grid:
+            self._grid_struct(pk, gh, gw)
+            _, gx, gy = pk["grid"][(gh, gw)]
+        else:
+            gx, gy = pk["gx"], pk["gy"]
+        for d, s in zip(sw["dst"], pk["wk"] + pk["w0t"] + pk["wkT"] + [gx, gy]):
+            d.copy_(s)
+        sw["src"] = pk
+
+    def _train_graph(self, key, pk: dict, gh: int, gw: int, grid: bool, make_io, run, keep) -> dict:
+        """The captured graph of `key` (captured on first use): `make_io()` builds its static buffers, `run(sw, io)`
+        issues the native call on them.  Recaptured when a parameter's storage moved."""
+        ptrs = tuple(p.data_ptr() for p in self.parameters())
+        ent = self._train_graphs.get(key)
+        if ent is not None and ent["ptrs"] != ptrs:
+            del self._train_graphs[key]
+            ent = None
+        if ent is None:
+            sw = self._static_weights(pk, gh, gw, grid)
+            self._refresh_static_weights(sw, pk, gh, gw, grid)
+            io = make_io()
+            side = torch.cuda.Stream(device=self.device)
+            side.wait_stream(torch.cuda.current_stream(self.device))
+            graph = torch.cuda.CUDAGraph()
+            with torch.cuda.stream(side):
+                run(sw, io)   # warm-up outside capture (kernel attributes, constant tables)
+                graph.capture_begin(capture_error_mode="thread_local")   # nothing is allocated during the capture
+                try:
+                    run(sw, io)
+                finally:
+                    graph.capture_end()
+            torch.cuda.current_stream(self.device).wait_stream(side)
+            ent = dict(graph=graph, io=io, sw=sw, ptrs=ptrs, keep=keep)
+            while len(self._train_graphs) >= self.max_graphs:   # oldest capture goes first
+                self._train_graphs.pop(next(iter(self._train_graphs)))
+            self._train_graphs[key] = ent
+        self._refresh_static_weights(ent["sw"], pk, gh, gw, grid)
+        return ent
+
+    def _native_rollout_train(self, inputs: Tensor, mask4: Tensor, case_params: Tensor, steps: int) -> Tensor:
+        """preds (steps, B, 2, H, W) from fno_[grid_]rollout_forward_train: the training forward's kernels, so the
+        predictions equal those of chained `generate` calls under autograd bit for bit."""
+        lib = _lib.load()
+        b, dev = inputs.shape[0], self.device
+        gh, gw = (int(s) for s in inputs.shape[-2:])
+        grid = self._on_grid_path(gh, gw)
+        pk = self._pack(need_bwd=True)
+        ws, ws_bufs = self._grid_workspace(b, gh, gw) if grid else self._workspace(b)
+        rs = self._rollout_state(b, gh, gw, grid)
+        seq = torch.empty(steps, b, self.out_chan, gh, gw, dtype=torch.float32, device=dev)
+
+        def call(st, x, mk, cp, out):
+            if grid:
+                _lib.check(lib.fno_grid_rollout_forward_train(C.byref(st), x.data_ptr(), mk.data_ptr(), cp.data_ptr(),
+                                                              out.data_ptr(), steps, C.byref(rs["sv"]), C.byref(ws), b, gh,
+                                                              gw, self._stream()), "fno_grid_rollout_forward_train")
+            else:
+                _lib.check(lib.fno_rollout_forward_train(C.byref(st), x.data_ptr(), mk.data_ptr(), cp.data_ptr(),
+                                                         out.data_ptr(), steps, C.byref(rs["sv"]), C.byref(ws), b,
+                                                         self._act_code(), self._stream()), "fno_rollout_forward_train")
+        if not self.graph_rollout:
+            call(self._grid_struct(pk, gh, gw) if grid else pk["struct"], inputs, mask4, case_params, seq)
+            return seq
+        key = ("fwd", b, steps, gh, gw, grid, self.act_dtype)
+        ent = self._train_graph(
+            key, pk, gh, gw, grid,
+            lambda: dict(x=inputs.clone(), mk=mask4.clone(), cp=case_params.clone(), seq=torch.empty_like(seq)),
+            lambda sw, io: call(sw["struct"], io["x"], io["mk"], io["cp"], io["seq"]), (ws_bufs, rs))
+        io = ent["io"]
+        io["x"].copy_(inputs)
+        io["mk"].copy_(mask4)
+        io["cp"].copy_(case_params)
+        ent["graph"].replay()
+        seq.copy_(io["seq"])
+        return seq
+
+    def _native_rollout_backward(self, inputs, mask4, case_params, seq, dseq, steps: int, want_params: bool,
+                                 d_inputs: Optional[Tensor], d_cp: Optional[Tensor]):
+        """One native sweep (fno_[grid_]rollout_backward): parameter gradients in parameter order (None when
+        `want_params` is false), dL/dinputs into `d_inputs` and dL/dcase_params into `d_cp` when given.  With data
+        parallel enabled the flat parameter-gradient buffer is all-reduced once."""
+        if self.n_case_params == 0:
+            d_cp = None
+        if not want_params and d_inputs is None and d_cp is None:
+            return None
+        lib = _lib.load()
+        b = inputs.shape[0]
+        gh, gw = (int(s) for s in inputs.shape[-2:])
+        grid = self._on_grid_path(gh, gw)
+        pk = self._pack(need_bwd=True)
+        ws, ws_bufs = self._grid_workspace(b, gh, gw) if grid else self._workspace(b)
+        rs = self._rollout_state(b, gh, gw, grid)
+        carry = rs["bufs"]["carry"]
+
+        def call(st, sb, x, mk, cp, sq, dsq, g, din, dcp):
+            g_arg = C.byref(g) if g is not None else None
+            if grid:
+                _lib.check(lib.fno_grid_rollout_backward(C.byref(st), C.byref(sb), x.data_ptr(), mk.data_ptr(),
+                                                         cp.data_ptr(), sq.data_ptr(), dsq.data_ptr(), steps,
+                                                         C.byref(rs["sv"]), g_arg, C.byref(rs["sc"]), C.byref(ws),
+                                                         carry.data_ptr(), _ptr(din), _ptr(dcp), b, gh, gw, self._stream()),
+                           "fno_grid_rollout_backward")
+            else:
+                _lib.check(lib.fno_rollout_backward(C.byref(st), C.byref(sb), x.data_ptr(), mk.data_ptr(), cp.data_ptr(),
+                                                    sq.data_ptr(), dsq.data_ptr(), steps, C.byref(rs["sv"]), g_arg,
+                                                    C.byref(rs["sc"]), C.byref(ws), carry.data_ptr(), _ptr(din), _ptr(dcp),
+                                                    b, self._act_code(), self._stream()), "fno_rollout_backward")
+        flat = views = None
+        if not self.graph_rollout:
+            g = None
+            if want_params:
+                flat, views, g = self._grad_buffers()
+            st = self._grid_struct(pk, gh, gw) if grid else pk["struct"]
+            call(st, pk["struct_bwd"], inputs, mask4, case_params, seq, dseq, g, d_inputs, d_cp)
+        else:
+            def make_io():
+                io = dict(x=inputs.clone(), mk=mask4.clone(), cp=case_params.clone(), seq=torch.empty_like(seq),
+                          dseq=torch.empty_like(dseq), g=None,
+                          din=torch.empty_like(d_inputs) if d_inputs is not None else None,
+                          dcp=torch.empty_like(d_cp) if d_cp is not None else None)
+                if want_params:
+                    io["flat"], _, io["g"] = self._grad_buffers()
+                return io
+            key = ("bwd", b, steps, gh, gw, grid, self.act_dtype, want_params, d_inputs is not None, d_cp is not None)
+            ent = self._train_graph(
+                key, pk, gh, gw, grid, make_io,
+                lambda sw, io: call(sw["struct"], sw["struct_bwd"], io["x"], io["mk"], io["cp"], io["seq"], io["dseq"],
+                                    io["g"], io["din"], io["dcp"]), (ws_bufs, rs))
+            io = ent["io"]
+            for k, t in (("x", inputs), ("mk", mask4), ("cp", case_params), ("seq", seq), ("dseq", dseq)):
+                io[k].copy_(t)
+            ent["graph"].replay()
+            if d_inputs is not None:
+                d_inputs.copy_(io["din"])
+            if d_cp is not None:
+                d_cp.copy_(io["dcp"])
+            if want_params:   # the caller owns its gradients: a fresh buffer, never a view of the graph's
+                flat, views, _ = self._grad_buffers()
+                flat.copy_(io["flat"])
+        if not want_params:
+            return None
+        if self._dp_enabled:   # one all-reduce of the whole flat buffer per backward, not one per step
             from .dp import allreduce_mean_
             allreduce_mean_(flat, self._dp_group)
         return [views[name] for name, _ in self.named_parameters()]
@@ -577,6 +823,33 @@ class Fno2d(AutoCfdModel):
                 inputs, case_params, mask4 = self._prep_inputs(inputs, case_params, mask)
                 seq = self._rollout_device(inputs, case_params, mask4, steps)
         return [seq[s] for s in range(steps)]
+
+    def rollout(self, inputs: Tensor, case_params: Tensor, mask: Optional[Tensor], steps: int) -> Tensor:
+        """`steps` autoregressive steps as one (steps, B, 2, H, W) float32 tensor, trainable through the whole rollout.
+        Arguments as `generate_many` ((c,h,w) / (p,) / (h,w) inputs get a batch axis); every grid and storage mode of
+        `forward`.  Step s is fed the (masked) prediction of step s-1, computed with the training forward's kernels, so
+        the predictions equal those of `steps` chained `generate` calls under autograd bit for bit.
+
+        With autograd on, the result is differentiable w.r.t. the parameters, `inputs` and `case_params` (a `mask` that
+        requires grad raises NotImplementedError, as in `forward`).  Unlike chained `generate` calls, each of which keeps
+        its own saved activations until backward (about 1 GB per step at B = 256), it keeps only the predicted frames and
+        one reused set of saved activations: the backward recomputes each step's activations from its input frame (one
+        extra training forward per step) while it sweeps the steps from last to first.  With autograd off it returns the
+        same predictions and builds no graph."""
+        self._require_cuda()
+        if isinstance(steps, bool) or not isinstance(steps, int) or steps < 1:
+            raise ValueError(f"steps must be a positive int; got {steps!r}")
+        if inputs.dim() == 3:
+            inputs, case_params = inputs.unsqueeze(0), case_params.unsqueeze(0)
+            mask = mask.unsqueeze(0) if mask is not None else None
+        inputs, case_params, mask4 = self._prep_inputs(inputs, case_params, mask)
+        needs_grad = torch.is_grad_enabled() and (inputs.requires_grad or case_params.requires_grad or mask4.requires_grad
+                                                  or any(p.requires_grad for p in self.parameters()))
+        with torch.cuda.device(self.device):
+            if needs_grad:
+                return _RolloutFn.apply(self, inputs, mask4, case_params, steps, *self.parameters())
+            with torch.no_grad():
+                return self._native_rollout_train(inputs, mask4, case_params, steps)
 
     def _rollout_device(self, inputs, case_params, mask4, steps) -> Tensor:
         lib = _lib.load()

@@ -217,6 +217,28 @@ int fno_backward_inputs(const fno_weights* w, const fno_weights_bwd* wb, const f
                         float* d_case_params,          /* [B][p] or NULL (must be NULL or unused when p == 0) */
                         int batch, int act_dtype, void* stream);
 
+/* Training through a K-step rollout (backpropagation through time) with memory that does not grow with K beyond the
+ * frames.  Frames are float32 [B][2][64][64]; preds_seq and dpreds_seq are [K][B][2][64][64].
+ * fno_rollout_forward_train: K chained fno_forward_train calls, step s fed the (masked) prediction of step s-1, writing
+ * preds_seq; `saved` is reused by every step (on return it holds step K-1's activations).  Its predictions are those of
+ * K chained fno_forward_train calls, bit for bit.
+ * fno_rollout_backward: the whole backward of that rollout in one call, for L = sum_s <dpreds_seq[s], preds_seq[s]>.  It
+ * sweeps s = K-1 .. 0; each step recomputes step s's saved set from its input frame (`inputs` or preds_seq[s-1]) with
+ * the training forward's kernels, then runs step s's backward with upstream gradient dpreds_seq[s] + carry, where carry
+ * = dL/d(frame fed to step s+1).  The lift's data adjoint writes fc0[:, 0:2]^T dL/da0 + dpreds_seq[s-1] straight into
+ * `carry` (float32 [B][2][64][64], its own buffer, used when K > 1).  grads (parameter gradients, summed over the steps),
+ * d_inputs (dL/dinputs) and d_case_params (summed over the steps) are overwritten; each may be NULL, not all three.
+ * Bit-reproducible (fixed-order reductions, no atomics); with K = 1 the results equal fno_forward_train +
+ * fno_backward_inputs bit for bit.  d_inputs, carry and dpreds_seq must be 16-byte aligned.  steps < 1 -> status 1. */
+int fno_rollout_forward_train(const fno_weights* w, const float* inputs, const float* mask, const float* case_params,
+                              float* preds_seq, int steps, const fno_train_saved* saved, const fno_workspace* ws, int batch,
+                              int act_dtype, void* stream);
+int fno_rollout_backward(const fno_weights* w, const fno_weights_bwd* wb, const float* inputs, const float* mask,
+                         const float* case_params, const float* preds_seq, const float* dpreds_seq, int steps,
+                         const fno_train_saved* saved, const fno_grads* grads, const fno_bwd_scratch* scratch,
+                         const fno_workspace* ws, float* carry, float* d_inputs, float* d_case_params, int batch, int act_dtype,
+                         void* stream);
+
 /* Rollout evaluation on the device (SURVEY.md 8f.1; reference src/test_multistep.py:73-83,153-177 get_metrics on the
  * masked u channel, three .item() syncs per step and case there).  preds_seq [S][B][2][64][64], label_u and mask
  * [S][B][64][64]; sums [S][B][3] = (sum (p-l)^2, sum l^2, sum |p-l|) with p, l multiplied by mask. */
@@ -306,6 +328,16 @@ int fno_grid_backward(const fno_weights* w, const fno_weights_bwd* wb, const flo
                       const float* case_params, const float* dpreds, const fno_train_saved* saved, const fno_grads* grads,
                       const fno_bwd_scratch* scratch, const fno_workspace* ws, float* d_inputs, float* d_case_params,
                       int batch, int h, int w_, void* stream);
+/* fno_rollout_forward_train / fno_rollout_backward on an H x W grid (frames, preds_seq, dpreds_seq and carry with H x W
+ * planes; no alignment requirement) */
+int fno_grid_rollout_forward_train(const fno_weights* w, const float* inputs, const float* mask, const float* case_params,
+                                   float* preds_seq, int steps, const fno_train_saved* saved, const fno_workspace* ws,
+                                   int batch, int h, int w_, void* stream);
+int fno_grid_rollout_backward(const fno_weights* w, const fno_weights_bwd* wb, const float* inputs, const float* mask,
+                              const float* case_params, const float* preds_seq, const float* dpreds_seq, int steps,
+                              const fno_train_saved* saved, const fno_grads* grads, const fno_bwd_scratch* scratch,
+                              const fno_workspace* ws, float* carry, float* d_inputs, float* d_case_params, int batch, int h,
+                              int w_, void* stream);
 /* fno_multistep_metrics on an H x W grid: preds_seq [S][B][2][H][W], label_u and mask [S][B][H][W]; sums [S][B][3] as
  * there (sums over the H*W pixels).  One CTA per (step, case) plane, fixed-order reduction: bit-reproducible.
  * steps <= 65535. */
