@@ -5,12 +5,13 @@ Public surface mirrors the reference's for this path:
     AutoCfdModel                           (reference src/models/base_model.py)
     MseLoss, loss_name_to_fn               (reference src/models/loss.py)
     infer_multistep                        (reference src/test_multistep.py infer, batched on the device)
+    evaluate_auto                          (reference src/train_auto.py evaluate, batched on the device)
 """
 from .base_model import AutoCfdModel
 from .loss import MseLoss, loss_name_to_fn
 
 __all__ = ["AutoCfdModel", "MseLoss", "loss_name_to_fn", "Fno2d", "FnoBlock", "SpectralConv2d_fast", "FusedAdam", "DeviceFrames",
-           "infer_multistep"]
+           "infer_multistep", "evaluate_auto"]
 
 
 def __getattr__(name):  # lazy: importing the package must not require the native library
@@ -26,4 +27,7 @@ def __getattr__(name):  # lazy: importing the package must not require the nativ
     if name == "infer_multistep":
         from .metrics import infer_multistep
         return infer_multistep
+    if name == "evaluate_auto":
+        from .metrics import evaluate_auto
+        return evaluate_auto
     raise AttributeError(name)

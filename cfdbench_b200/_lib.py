@@ -156,6 +156,7 @@ SIGNATURES = {
                                             C.POINTER(FnoWorkspace), _P, _P, _P, _I, _I, _I, _P]),
     "fno_grid_multistep_metrics": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _P]),
     "fno_grid_gather_batch": (C.c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _P, _P, _P, _P, _I, _I, _P]),
+    "fno_eval_sums": (C.c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _P]),
 }
 
 GRID_MIN, GRID_MAX = 24, 128

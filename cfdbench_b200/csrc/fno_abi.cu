@@ -72,6 +72,7 @@ size_t grid_partials_offset_lb();
 cudaError_t launch_grid_multistep_metrics(const float*, const float*, const float*, float*, int, int, int, int, cudaStream_t);
 cudaError_t launch_grid_gather_batch(const void*, const void*, const float*, const int*, const long long*, int, int, int,
                                      float*, float*, float*, float*, int, int, cudaStream_t);
+cudaError_t launch_eval_sums(const float*, const float*, const float*, const float*, float*, int, int, int, cudaStream_t);
 }  // namespace fno
 
 using namespace fno;
@@ -875,6 +876,14 @@ int fno_grid_gather_batch(const void* frames_in, const void* frames_out, const f
                                     reinterpret_cast<const long long*>(idx), n_idx, n_case_params,
                                     frame_dtype == FNO_ACT_BF16, inputs, label, mask, case_params, h, wd, S(stream)),
            "grid_gather_batch_kernel");
+  return kOk;
+}
+
+int fno_eval_sums(const float* preds, const float* label, const float* mask, const float* inputs, float* sums, int batch,
+                  int h, int wd, void* stream) {
+  FNO_TRY(grid_arg("fno_eval_sums", h, wd));
+  if (!preds || !label || !mask || !inputs || !sums || batch <= 0) return fail(kErrArg, "fno_eval_sums: bad argument");
+  FNO_CUDA(launch_eval_sums(preds, label, mask, inputs, sums, batch, h, wd, S(stream)), "eval_sums_kernel");
   return kOk;
 }
 

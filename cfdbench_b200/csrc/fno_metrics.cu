@@ -180,6 +180,62 @@ cudaError_t launch_grid_multistep_metrics(const float* preds_seq, const float* l
   return cudaGetLastError();
 }
 
+// Single-step evaluation (reference src/train_auto.py:61-148, `evaluate`): per sample b of a (B, 2, H, W) batch
+//   out[b][0..2] = sum (p - l*m)^2, sum |p - l*m|, sum (l*m)^2        both channels, p = preds as the model returns them
+//                                                                      (already masked), m broadcast over the channels
+//   out[b][3..5] = sum (x_u - l_u)^2, sum |x_u - l_u|, sum l_u^2       channel 0 of inputs / label, no mask
+// i.e. the terms of the model's loss on (preds, label * mask) and of the input loss on (inputs[:, :1], label[:, :1]).
+// grid (B): one CTA per sample, scalar loads (caller tensors, planes only 4-byte aligned at odd H*W), each thread's
+// pixels, the shuffle tree and the warp order fixed: a repeated launch is bit-identical (no atomics).
+constexpr int kEvThreads = 256;
+
+__global__ void __launch_bounds__(kEvThreads)
+    eval_sums_kernel(const float* __restrict__ preds, const float* __restrict__ label, const float* __restrict__ mask,
+                     const float* __restrict__ inputs, float* __restrict__ out, int hw) {
+  __shared__ float red[kEvThreads / 32][6];
+  const size_t b = blockIdx.x;
+  const float* p = preds + b * 2 * hw;
+  const float* l = label + b * 2 * hw;
+  const float* x = inputs + b * 2 * hw;   // channel 0 = u
+  const float* m = mask + b * hw;
+  float s[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+  for (int i = threadIdx.x; i < hw; i += kEvThreads) {
+    const float mv = __ldg(m + i);
+    const float p0 = __ldg(p + i), p1 = __ldg(p + hw + i);
+    const float l0 = __ldg(l + i), l1 = __ldg(l + hw + i);
+    const float x0 = __ldg(x + i);
+    const float lm0 = l0 * mv, lm1 = l1 * mv;
+    const float d0 = p0 - lm0, d1 = p1 - lm1, du = x0 - l0;
+    s[0] = fmaf(d1, d1, fmaf(d0, d0, s[0]));
+    s[1] += fabsf(d0) + fabsf(d1);
+    s[2] = fmaf(lm1, lm1, fmaf(lm0, lm0, s[2]));
+    s[3] = fmaf(du, du, s[3]);
+    s[4] += fabsf(du);
+    s[5] = fmaf(l0, l0, s[5]);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1)
+#pragma unroll
+    for (int k = 0; k < 6; ++k) s[k] += __shfl_xor_sync(0xffffffffu, s[k], o);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (lane == 0)
+#pragma unroll
+    for (int k = 0; k < 6; ++k) red[warp][k] = s[k];
+  __syncthreads();
+  if (threadIdx.x < 6) {
+    float t = 0.f;
+#pragma unroll
+    for (int w = 0; w < kEvThreads / 32; ++w) t += red[w][threadIdx.x];  // fixed order: deterministic
+    out[b * 6 + threadIdx.x] = t;
+  }
+}
+
+cudaError_t launch_eval_sums(const float* preds, const float* label, const float* mask, const float* inputs, float* out,
+                             int batch, int h, int w, cudaStream_t stream) {
+  eval_sums_kernel<<<batch, kEvThreads, 0, stream>>>(preds, label, mask, inputs, out, h * w);
+  return cudaGetLastError();
+}
+
 __device__ __forceinline__ float frame_ld(const float* p) { return __ldg(p); }
 __device__ __forceinline__ float frame_ld(const __nv_bfloat16* p) { return __bfloat162float(__ldg(p)); }
 

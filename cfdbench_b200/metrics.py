@@ -9,6 +9,12 @@ instead of three `.item()` synchronisations per step and case.
 case at a time with B = 1 (`infer_case`, :102-132) and then synchronises three times per step and case; here the cases
 run as one batched, graph-replayed rollout per chunk of at most `max_batch` cases, each followed by one metrics launch,
 and the whole split makes one device->host copy.
+
+`evaluate_auto` replaces `train_auto.evaluate` (reference src/train_auto.py:61-148), the single-step evaluation of the
+dev split every `eval_interval` epochs and of the test split (with B = 1) after training: the reference builds every
+batch on the host, runs one forward and synchronises 2 x (number of scores) times per batch; here chunks of up to
+`max_batch` samples are gathered from device-resident frames, run as one forward each and reduced by one `fno_eval_sums`
+launch per chunk, and the split makes one synchronisation.
 """
 from __future__ import annotations
 
@@ -130,3 +136,111 @@ def infer_multistep(model, all_features: Sequence[Union[Tensor, np.ndarray]], al
         blocks.append(host[s * lo * 3:s * hi * 3].reshape(s, hi - lo, 3))
     per_case = _per_case(np.concatenate(blocks, axis=1), gh * gw)   # (S, n) each
     return [{k: float(np.mean(v[i])) for k, v in per_case.items()} for i in range(s)]
+
+
+EVAL_SCORES = ("mse", "rmse", "mae", "nmse")   # what the reference's MseLoss.get_score_names can return
+
+
+def _launch_eval_sums(preds: Tensor, label: Tensor, mask: Tensor, inputs: Tensor, sums: Tensor) -> None:
+    """sums [B][6] (a contiguous float32 CUDA tensor or view) <- fno_eval_sums of the contiguous float32 CUDA tensors
+    preds, label, inputs (B,2,H,W) and mask (B,1,H,W)."""
+    b, _, gh, gw = preds.shape
+    lib = _lib.load()
+    with torch.cuda.device(preds.device):
+        st = C.c_void_p(torch.cuda.current_stream(preds.device).cuda_stream)
+        _lib.check(lib.fno_eval_sums(preds.data_ptr(), label.data_ptr(), mask.data_ptr(), inputs.data_ptr(),
+                                     sums.data_ptr(), b, gh, gw, st), "fno_eval_sums")
+
+
+def eval_scores(sums: np.ndarray, hw: int, batch_size: int, names: Sequence[str]) -> dict:
+    """The `scores` of `train_auto.evaluate` (reference src/train_auto.py:75-147) from per-sample sums.
+
+    sums: (N, 6) per-sample `fno_eval_sums` rows, hw = H*W.  The reference scores consecutive batches of `batch_size`
+    samples (the last one may be short): per batch the model's loss on (preds, label * mask) over both channels and the
+    input loss on (inputs[:, :1], label[:, :1]).  Each batch's sums are added in float64 in sample order; a batch whose
+    labels are all zero gives the inf / nan of the reference's division.  Returns dict(mean={k, input_k: mean over
+    batches}, all={k: [one score per batch]}), every value a Python float."""
+    host = np.asarray(sums, dtype=np.float64)
+    n = host.shape[0]
+    n_full = n // batch_size
+    tot = np.zeros((n_full, 6))
+    if n_full:
+        full = host[:n_full * batch_size].reshape(n_full, batch_size, 6)
+        for j in range(batch_size):   # every full batch at once, its samples added in order
+            tot += full[:, j]
+    cnt = np.full(n_full, float(batch_size))
+    if n % batch_size:                # the short last batch
+        tot = np.concatenate([tot, np.cumsum(host[n_full * batch_size:], axis=0)[-1:]])
+        cnt = np.append(cnt, float(n % batch_size))
+    with np.errstate(divide="ignore", invalid="ignore"):
+        per = {}
+        for prefix, (e2, e1, l2), size in (("", (0, 1, 2), 2 * hw), ("input_", (3, 4, 5), hw)):
+            mse = tot[:, e2] / (cnt * size)
+            per[prefix] = dict(mse=mse, rmse=np.sqrt(mse), mae=tot[:, e1] / (cnt * size),
+                               nmse=mse / (tot[:, l2] / (cnt * size)))
+    scores = {k: per[""][k].tolist() for k in names}   # lists of Python floats
+    mean = {}
+    for k in names:
+        mean[k] = float(np.mean(per[""][k]))
+        mean[f"input_{k}"] = float(np.mean(per["input_"][k]))
+    return dict(mean=mean, all=scores)
+
+
+def evaluate_auto(model, data, batch_size: int = 2, max_batch: int = 256) -> dict:
+    """What `train_auto.evaluate(model, data, output_dir, batch_size)` returns (reference src/train_auto.py:61-148),
+    without its plots:  dict(preds=(2N, 1, H, W) float32 CPU tensor, scores=dict(mean=..., all=...)).
+
+    data: the reference's dataset object (`.inputs`, `.labels` (N, 3, H, W), `.case_ids`, `.case_params`; uploaded once
+    per call) or a `DeviceFrames` of it (built once, reused by every call).  The score names are
+    `model.loss_fn.get_score_names()`, scored per reference batch of `batch_size` consecutive samples (see
+    `eval_scores`).  `preds` are the masked predictions in sample order viewed as (-1, 1, H, W), as the reference's
+    `preds.view(-1, 1, height, width)` gives them.  The model is put in eval mode and run under inference mode.
+
+    Samples run in chunks of at most `max_batch`: per chunk one `DeviceFrames.batch` gather, one forward without label
+    (the module's loss does not run), one `fno_eval_sums` launch into a device buffer for the whole split and one
+    asynchronous copy of the predictions into a pinned host tensor; the split synchronises once, at the end.  Device
+    memory beyond the frames and the (N, 6) sums is one chunk's worth.  Samples are computed independently, so the
+    result does not depend on `max_batch`."""
+    from .data import DeviceFrames
+    if batch_size < 1 or max_batch < 1:
+        raise ValueError(f"batch_size and max_batch must be positive, got {batch_size} and {max_batch}")
+    names = list(model.loss_fn.get_score_names())
+    unknown = [k for k in names if k not in EVAL_SCORES]
+    if unknown:
+        raise ValueError(f"score names {unknown} are not among {EVAL_SCORES}")
+    if isinstance(data, DeviceFrames):
+        n, gh, gw = data.n, data.height, data.width
+    else:
+        ins, labs = getattr(data, "inputs", None), getattr(data, "labels", None)
+        if not isinstance(ins, Tensor) or not isinstance(labs, Tensor) or ins.dim() != 4 or ins.shape[1] != 3 \
+                or labs.shape != ins.shape:
+            raise ValueError("data must be a DeviceFrames or a dataset with (N, 3, H, W) .inputs / .labels tensors, got "
+                             f"{getattr(ins, 'shape', None)} / {getattr(labs, 'shape', None)}")
+        n, gh, gw = int(ins.shape[0]), int(ins.shape[2]), int(ins.shape[3])
+        if n > 0 and len(np.asarray(data.case_ids)) != n:
+            raise ValueError("dataset.case_ids must have one entry per sample")
+    if n == 0:
+        raise ValueError("the split is empty")
+    _check_grid(gh, gw)
+    dev = next(model.parameters()).device
+    if dev.type != "cuda":
+        raise _lib.FnoNativeError("evaluate_auto has no CPU path: the model must be on a CUDA device")
+    if isinstance(data, DeviceFrames) and data.frames_in.device != dev:   # a tensor's device carries its index
+        raise ValueError(f"the frames are on {data.frames_in.device}, the model on {dev}")
+    check = getattr(model, "_check_grid", None)
+    if check is not None:   # the drop-in Fno2d's own grid / storage-mode check, before any device work
+        check((gh, gw))
+    model.eval()
+    preds_host = torch.empty(n, 2, gh, gw, dtype=torch.float32, pin_memory=True)   # a normal tensor, as torch.cat gives
+    with torch.inference_mode(), torch.cuda.device(dev):
+        frames = data if isinstance(data, DeviceFrames) else DeviceFrames(data, device=dev)
+        sums = torch.empty(n, 6, dtype=torch.float32, device=dev)
+        for lo in range(0, n, max_batch):
+            hi = min(n, lo + max_batch)
+            batch = frames.batch(torch.arange(lo, hi).pin_memory())   # pinned: the index upload is asynchronous
+            preds = model(inputs=batch["inputs"], case_params=batch["case_params"], mask=batch["mask"])["preds"]
+            _launch_eval_sums(preds, batch["label"], batch["mask"], batch["inputs"], sums[lo:hi])
+            preds_host[lo:hi].copy_(preds, non_blocking=True)
+            del batch, preds
+        host = sums.cpu().double().numpy()   # the only synchronisation
+    return dict(preds=preds_host.view(-1, 1, gh, gw), scores=eval_scores(host, gh * gw, batch_size, names))

@@ -349,6 +349,17 @@ int fno_grid_gather_batch(const void* frames_in, const void* frames_out, const f
                           const int64_t* idx, int n_idx, int n_case_params, int frame_dtype, float* inputs, float* label,
                           float* mask, float* case_params, int h, int w_, void* stream);
 
+/* Single-step evaluation (reference src/train_auto.py:61-148, `evaluate`, which synchronises 2 x (number of scores)
+ * times per batch): the per-sample sums its scores are made of, for any grid 24 <= H, W <= 128 (64 x 64 included).
+ * preds, label, inputs [B][2][H][W], mask [B][1][H][W], float32 caller tensors (no alignment beyond 4 bytes needed);
+ * preds as the model returns them (already masked).  sums [B][6]:
+ *   0: sum (preds - label*mask)^2   1: sum |preds - label*mask|   2: sum (label*mask)^2      both channels, H*W pixels
+ *   3: sum (inputs_u - label_u)^2   4: sum |inputs_u - label_u|   5: sum label_u^2           channel 0, no mask
+ * One CTA per sample, fixed-order reduction: bit-reproducible.  A grid outside the range returns 3, a null pointer or
+ * batch <= 0 returns 1, both before any device work. */
+int fno_eval_sums(const float* preds, const float* label, const float* mask, const float* inputs, float* sums, int batch,
+                  int h, int w_, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
