@@ -6,12 +6,13 @@ Public surface mirrors the reference's for this path:
     MseLoss, loss_name_to_fn               (reference src/models/loss.py)
     infer_multistep                        (reference src/test_multistep.py infer, batched on the device)
     evaluate_auto                          (reference src/train_auto.py evaluate, batched on the device)
+    train_auto                             (reference src/train_auto.py train, steps replayed from CUDA graphs)
 """
 from .base_model import AutoCfdModel
 from .loss import MseLoss, loss_name_to_fn
 
 __all__ = ["AutoCfdModel", "MseLoss", "loss_name_to_fn", "Fno2d", "FnoBlock", "SpectralConv2d_fast", "FusedAdam", "DeviceFrames",
-           "infer_multistep", "evaluate_auto"]
+           "infer_multistep", "evaluate_auto", "train_auto"]
 
 
 def __getattr__(name):  # lazy: importing the package must not require the native library
@@ -30,4 +31,7 @@ def __getattr__(name):  # lazy: importing the package must not require the nativ
     if name == "evaluate_auto":
         from .metrics import evaluate_auto
         return evaluate_auto
+    if name == "train_auto":
+        from .train import train_auto
+        return train_auto
     raise AttributeError(name)

@@ -119,6 +119,10 @@ SIGNATURES = {
     "fno_loss_bwd": (C.c_int, [_P, _P, _P, _P, _P, C.c_size_t, _P]),
     "fno_adam_step": (C.c_int, [C.POINTER(FnoAdamTensors), C.c_float, C.c_float, C.c_float, C.c_float, C.c_float,
                                 C.c_int64, _P]),
+    "fno_train_stage_indices": (C.c_int, [_P, C.c_int64, _I, _I, _P, _P, _P]),
+    "fno_adam_step_dev": (C.c_int, [C.POINTER(FnoAdamTensors), _P, _I, _P, _F, _F, _F, _F, _P]),
+    "fno_adam_coefficients": (C.c_int, [_F, _F, _F, C.c_int64, _I, _P]),
+    "fno_train_log_step": (C.c_int, [_P, _P, _I, _P, _P]),
     "fno_forward_train": (C.c_int, [C.POINTER(FnoWeights), _P, _P, _P, _P, C.POINTER(FnoTrainSaved),
                                     C.POINTER(FnoWorkspace), _I, _I, _P]),
     "fno_backward": (C.c_int, [C.POINTER(FnoWeights), C.POINTER(FnoWeightsBwd), _P, _P, _P, _P,

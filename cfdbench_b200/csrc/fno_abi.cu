@@ -22,6 +22,11 @@ cudaError_t launch_loss_fwd(const float*, const float*, size_t, float*, float*, 
 cudaError_t launch_loss_bwd(const float*, const float*, const float*, const float*, float*, size_t, cudaStream_t);
 size_t loss_scratch_bytes();
 cudaError_t launch_adam_step(const fno_adam_tensors*, float, float, float, float, float, long long, cudaStream_t);
+cudaError_t launch_adam_step_dev(const fno_adam_tensors*, const float*, int, const int*, float, float, float, float,
+                                 cudaStream_t);
+void adam_coefficients(float, float, float, long long, float*, float*);
+cudaError_t launch_stage_indices(const long long*, long long, int, int, const int*, long long*, cudaStream_t);
+cudaError_t launch_log_step(const float*, float*, int, int*, cudaStream_t);
 cudaError_t launch_inv_kx(const void*, void*, int, float, float, cudaStream_t);
 template <typename TAct>
 cudaError_t launch_block_tc(int, const void*, const void*, const float*, const float*, void*, float*, const float*, int,
@@ -571,6 +576,46 @@ int fno_adam_step(const fno_adam_tensors* t, float lr, float beta1, float beta2,
     if (!t->param[i] || !t->grad[i] || !t->exp_avg[i] || !t->exp_avg_sq[i] || t->n[i] <= 0)
       return fail(kErrArg, "fno_adam_step: null tensor or empty size");
   FNO_CUDA(launch_adam_step(t, lr, beta1, beta2, eps, weight_decay, step, S(stream)), "adam_step_kernel");
+  return kOk;
+}
+
+static int adam_tensors_ok(const fno_adam_tensors* t) {
+  if (!t || t->count < 0 || t->count > FNO_ADAM_MAX_TENSORS) return 0;
+  for (int i = 0; i < t->count; ++i)
+    if (!t->param[i] || !t->grad[i] || !t->exp_avg[i] || !t->exp_avg_sq[i] || t->n[i] <= 0) return 0;
+  return 1;
+}
+
+int fno_adam_step_dev(const fno_adam_tensors* t, const float* coef, int n_coef, const int32_t* cursor, float beta1,
+                      float beta2, float eps, float weight_decay, void* stream) {
+  if (!coef || !cursor || n_coef <= 0 || (reinterpret_cast<uintptr_t>(coef) & 7))
+    return fail(kErrArg, "fno_adam_step_dev: bad argument");
+  if (!adam_tensors_ok(t)) return fail(kErrArg, "fno_adam_step_dev: bad tensor table");
+  FNO_CUDA(launch_adam_step_dev(t, coef, n_coef, reinterpret_cast<const int*>(cursor), beta1, beta2, eps, weight_decay,
+                                S(stream)),
+           "adam_step_kernel<true>");
+  return kOk;
+}
+
+int fno_adam_coefficients(float lr, float beta1, float beta2, int64_t first_step, int n, float* host_out) {
+  if (!host_out || n <= 0 || first_step < 1) return fail(kErrArg, "fno_adam_coefficients: bad argument");
+  for (int i = 0; i < n; ++i) adam_coefficients(lr, beta1, beta2, first_step + i, host_out + 2 * i, host_out + 2 * i + 1);
+  return kOk;
+}
+
+int fno_train_stage_indices(const int64_t* perm, int64_t n_perm, int stride, int batch, const int32_t* cursor,
+                            int64_t* idx_out, void* stream) {
+  if (!perm || !cursor || !idx_out || n_perm <= 0 || stride <= 0 || batch <= 0 || batch > stride || batch > n_perm)
+    return fail(kErrArg, "fno_train_stage_indices: bad argument");
+  FNO_CUDA(launch_stage_indices(reinterpret_cast<const long long*>(perm), n_perm, stride, batch,
+                                reinterpret_cast<const int*>(cursor), reinterpret_cast<long long*>(idx_out), S(stream)),
+           "stage_indices_kernel");
+  return kOk;
+}
+
+int fno_train_log_step(const float* loss_out, float* log, int n_log, int32_t* cursor, void* stream) {
+  if (!loss_out || !log || !cursor || n_log <= 0) return fail(kErrArg, "fno_train_log_step: bad argument");
+  FNO_CUDA(launch_log_step(loss_out, log, n_log, reinterpret_cast<int*>(cursor), S(stream)), "log_step_kernel");
   return kOk;
 }
 

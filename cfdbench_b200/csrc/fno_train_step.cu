@@ -7,6 +7,8 @@
 //    gradients of the four dict entries (the script calls loss["nmse"].backward()).
 //  * torch.optim.Adam.step (train_auto.py:213,256; complex parameters as pairs of reals, no amsgrad): all parameter
 //    tensors of the model in ONE launch through a pointer table, against ~10 multi-tensor launches of the reference.
+//  * the per-step pieces of a graph-replayed training epoch (cfdbench_b200/train.py): index staging, Adam with its
+//    coefficients read from a device table, and the loss log.
 #include "fno_common.cuh"
 #include "../../include/cfdbench_b200.h"
 
@@ -138,11 +140,36 @@ struct AdamArgs {
   fno_adam_tensors t;
   int first_block[FNO_ADAM_MAX_TENSORS + 1];  // prefix sum of ceil(n_i / kAdamChunk)
   float lr, beta1, beta2, eps, weight_decay, step_size, inv_bc2_sqrt;
+  // kDevCoef: (step_size, inv_bc2_sqrt) = coef[*cursor], read on the device (a graph replays one launch for every step)
+  const float2* coef;
+  const int* cursor;
+  int n_coef;
 };
+
+// The bias-corrected step size and 1/sqrt(bc2) of 1-based step `step`, as torch.optim.Adam forms them: in double, from
+// lr, beta1 and beta2 as the float32 values the kernel sees.  The one copy of this arithmetic: launch_adam_step and the
+// device coefficient table (fno_adam_coefficients) both call it, so the two paths cannot drift apart.
+void adam_coefficients(float lr, float beta1, float beta2, long long step, float* step_size, float* inv_bc2_sqrt) {
+  const double bc1 = 1.0 - pow(static_cast<double>(beta1), static_cast<double>(step));
+  const double bc2 = 1.0 - pow(static_cast<double>(beta2), static_cast<double>(step));
+  *step_size = static_cast<float>(static_cast<double>(lr) / bc1);
+  *inv_bc2_sqrt = static_cast<float>(1.0 / sqrt(bc2));
+}
 
 // torch.optim.Adam, single-tensor formulation (torch/optim/adam.py _single_tensor_adam):
 //   g += wd p;  m = lerp(m, g, 1-b1);  v = b2 v + (1-b2) g g;  p -= step_size * m / (sqrt(v)/sqrt(bc2) + eps)
+//   kDevCoef = false: step_size / inv_bc2_sqrt by value (fno_adam_step);  true: from coef[*cursor] (fno_adam_step_dev),
+//   and a cursor outside 0..n_coef-1 makes the launch write nothing
+template <bool kDevCoef>
 __global__ void __launch_bounds__(kAdamThreads) adam_step_kernel(const __grid_constant__ AdamArgs a) {
+  float step_size = a.step_size, inv_bc2_sqrt = a.inv_bc2_sqrt;
+  if constexpr (kDevCoef) {
+    const int c = *a.cursor;
+    if (c < 0 || c >= a.n_coef) return;
+    const float2 k = a.coef[c];
+    step_size = k.x;
+    inv_bc2_sqrt = k.y;
+  }
   int ti = 0;
 #pragma unroll 1
   while (ti + 1 < a.t.count && static_cast<int>(blockIdx.x) >= a.first_block[ti + 1]) ++ti;
@@ -162,17 +189,15 @@ __global__ void __launch_bounds__(kAdamThreads) adam_step_kernel(const __grid_co
       float mi = m[i], vi = v[i];
       mi = fmaf(gi - mi, 1.f - a.beta1, mi);
       vi = fmaf(1.f - a.beta2, gi * gi, vi * a.beta2);
-      const float denom = sqrtf(vi) * a.inv_bc2_sqrt + a.eps;
+      const float denom = sqrtf(vi) * inv_bc2_sqrt + a.eps;
       m[i] = mi;
       v[i] = vi;
-      p[i] = pi - a.step_size * (mi / denom);
+      p[i] = pi - step_size * (mi / denom);
     }
   }
 }
 
-cudaError_t launch_adam_step(const fno_adam_tensors* t, float lr, float beta1, float beta2, float eps, float weight_decay,
-                             long long step, cudaStream_t stream) {
-  AdamArgs a;
+static int adam_blocks(const fno_adam_tensors* t, AdamArgs& a) {
   a.t = *t;
   int blocks = 0;
   for (int i = 0; i < t->count; ++i) {
@@ -180,17 +205,72 @@ cudaError_t launch_adam_step(const fno_adam_tensors* t, float lr, float beta1, f
     blocks += static_cast<int>((t->n[i] + kAdamChunk - 1) / kAdamChunk);
   }
   a.first_block[t->count] = blocks;
-  const double bc1 = 1.0 - pow(static_cast<double>(beta1), static_cast<double>(step));
-  const double bc2 = 1.0 - pow(static_cast<double>(beta2), static_cast<double>(step));
+  return blocks;
+}
+
+cudaError_t launch_adam_step(const fno_adam_tensors* t, float lr, float beta1, float beta2, float eps, float weight_decay,
+                             long long step, cudaStream_t stream) {
+  AdamArgs a = {};
+  const int blocks = adam_blocks(t, a);
   a.lr = lr;
   a.beta1 = beta1;
   a.beta2 = beta2;
   a.eps = eps;
   a.weight_decay = weight_decay;
-  a.step_size = static_cast<float>(static_cast<double>(lr) / bc1);
-  a.inv_bc2_sqrt = static_cast<float>(1.0 / sqrt(bc2));
+  adam_coefficients(lr, beta1, beta2, step, &a.step_size, &a.inv_bc2_sqrt);
   if (blocks == 0) return cudaSuccess;
-  adam_step_kernel<<<blocks, kAdamThreads, 0, stream>>>(a);
+  adam_step_kernel<false><<<blocks, kAdamThreads, 0, stream>>>(a);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_adam_step_dev(const fno_adam_tensors* t, const float* coef, int n_coef, const int* cursor, float beta1,
+                                 float beta2, float eps, float weight_decay, cudaStream_t stream) {
+  AdamArgs a = {};
+  const int blocks = adam_blocks(t, a);
+  a.beta1 = beta1;
+  a.beta2 = beta2;
+  a.eps = eps;
+  a.weight_decay = weight_decay;
+  a.coef = reinterpret_cast<const float2*>(coef);
+  a.cursor = cursor;
+  a.n_coef = n_coef;
+  if (blocks == 0) return cudaSuccess;
+  adam_step_kernel<true><<<blocks, kAdamThreads, 0, stream>>>(a);
+  return cudaGetLastError();
+}
+
+// ------------------------------------------------------------------------------------------------ graph-replayed steps
+// A CUDA graph of one training step is replayed once per step of an epoch; what changes from step to step lives on the
+// device and is indexed by a step cursor: the step's sample indices (a slice of the epoch's permutation), Adam's
+// coefficients (a table row) and the slot of the step's loss in the epoch's log.  Both kernels below refuse a cursor that
+// would read or write past their table and then write nothing.
+
+// idx_out[i] = perm[cursor * stride + i], i < batch
+__global__ void __launch_bounds__(256) stage_indices_kernel(const long long* __restrict__ perm, long long n_perm, int stride,
+                                                            int batch, const int* __restrict__ cursor,
+                                                            long long* __restrict__ idx_out) {
+  const int c = *cursor;
+  const long long base = static_cast<long long>(c) * stride;
+  if (c < 0 || base + batch > n_perm) return;
+  for (int i = threadIdx.x; i < batch; i += blockDim.x) idx_out[i] = perm[base + i];
+}
+
+// log[cursor][0..4] = loss_out[0..4], then ++cursor
+__global__ void log_step_kernel(const float* __restrict__ loss_out, float* __restrict__ log, int n_log, int* cursor) {
+  const int c = *cursor;
+  if (c < 0 || c >= n_log) return;
+#pragma unroll
+  for (int k = 0; k < 5; ++k) log[static_cast<size_t>(c) * 5 + k] = loss_out[k];
+  *cursor = c + 1;
+}
+
+cudaError_t launch_stage_indices(const long long* perm, long long n_perm, int stride, int batch, const int* cursor,
+                                 long long* idx_out, cudaStream_t stream) {
+  stage_indices_kernel<<<1, 256, 0, stream>>>(perm, n_perm, stride, batch, cursor, idx_out);
+  return cudaGetLastError();
+}
+cudaError_t launch_log_step(const float* loss_out, float* log, int n_log, int* cursor, cudaStream_t stream) {
+  log_step_kernel<<<1, 1, 0, stream>>>(loss_out, log, n_log, cursor);
   return cudaGetLastError();
 }
 

@@ -90,15 +90,23 @@ class DeviceFrames:
 
     def loader(self, batch_size: int, shuffle: bool = False, generator=None, drop_last: bool = False):
         """Batches in exactly the order `DataLoader(dataset, batch_size, shuffle, generator=generator)` visits them:
-        the index stream comes from the same torch samplers the DataLoader builds."""
-        from torch.utils.data import BatchSampler, RandomSampler, SequentialSampler
-        base: List[int] = list(range(self.n))
-        sampler = RandomSampler(base, generator=generator) if shuffle else SequentialSampler(base)
+        the index stream comes from the same torch samplers the DataLoader builds (`index_batches`)."""
+        return self.batches(index_batches(self.n, batch_size, shuffle, generator, drop_last))
 
-        def gen():
-            # a DataLoader iterator draws its worker base seed from the generator before the sampler draws the
-            # permutation (torch/utils/data/dataloader.py, _BaseDataLoaderIter.__init__); do the same so that the RNG
-            # stream, and with it the visiting order, is identical
-            torch.empty((), dtype=torch.int64).random_(generator=generator)
-            yield from self.batches(BatchSampler(sampler, batch_size, drop_last))
-        return gen()
+
+def index_batches(n: int, batch_size: int, shuffle: bool = False, generator=None,
+                  drop_last: bool = False) -> Iterator[List[int]]:
+    """The index batches one iteration of `DataLoader(dataset_of_len_n, batch_size, shuffle, generator=generator,
+    drop_last=drop_last)` yields, drawing from the RNG (`generator`, or the global one for None) exactly what that
+    iteration draws.  Lazy, like the DataLoader iterator: nothing is drawn before the first batch is requested."""
+    from torch.utils.data import BatchSampler, RandomSampler, SequentialSampler
+    base: List[int] = list(range(n))
+    sampler = RandomSampler(base, generator=generator) if shuffle else SequentialSampler(base)
+
+    def gen():
+        # a DataLoader iterator draws its worker base seed from the generator before the sampler draws the
+        # permutation (torch/utils/data/dataloader.py, _BaseDataLoaderIter.__init__); do the same so that the RNG
+        # stream, and with it the visiting order, is identical
+        torch.empty((), dtype=torch.int64).random_(generator=generator)
+        yield from BatchSampler(sampler, batch_size, drop_last)
+    return gen()

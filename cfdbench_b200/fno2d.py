@@ -575,36 +575,41 @@ class Fno2d(AutoCfdModel):
         key = ("rollout_train", b, gh, gw, grid, self.act_dtype, self.device)
         st = self._ws_cache.get(key)
         if st is None:
-            lib = _lib.load()
-            dev, L = self.device, self.num_layers
-            adt = torch.float32 if grid else self._act_torch_dtype()
-            acts = [torch.empty(b, HIDDEN, gh, gw, dtype=adt, device=dev) for _ in range(L + 1)]
-            pres = [torch.empty(b, HIDDEN, gh, gw, dtype=torch.float32, device=dev) for _ in range(L)]
-            xms = [torch.empty(NMODES, b, HIDDEN, dtype=torch.complex64, device=dev) for _ in range(L)]
-            sv = _lib.FnoTrainSaved()
-            for l in range(L + 1):
-                sv.act[l] = acts[l].data_ptr()
-            for l in range(L):
-                sv.pre[l], sv.xm[l] = pres[l].data_ptr(), xms[l].data_ptr()
-            nbytes = lib.fno_grid_bwd_partials_bytes(gh, gw) if grid else lib.fno_bwd_partials_bytes()
-            bufs = dict(
-                d0=torch.empty(b, HIDDEN, gh, gw, dtype=torch.float32, device=dev),
-                d1=torch.empty(b, HIDDEN, gh, gw, dtype=torch.float32, device=dev),
-                dz1=torch.empty(min(b, _lib.BWD_CHUNK), PROJ, gh, gw, dtype=torch.float32, device=dev),
-                gm=torch.empty(NMODES, b, HIDDEN, dtype=torch.complex64, device=dev),
-                gwk=torch.empty(NMODES, HIDDEN, HIDDEN, dtype=torch.complex64, device=dev),
-                partials=torch.empty(nbytes, dtype=torch.uint8, device=dev),
-                carry=torch.empty(b, self.out_chan, gh, gw, dtype=torch.float32, device=dev),
-            )
-            sc = _lib.FnoBwdScratch()
-            sc.d[0], sc.d[1] = bufs["d0"].data_ptr(), bufs["d1"].data_ptr()
-            sc.dz1, sc.gm, sc.gwk = bufs["dz1"].data_ptr(), bufs["gm"].data_ptr(), bufs["gwk"].data_ptr()
-            sc.partials = bufs["partials"].data_ptr()
-            st = dict(sv=sv, sc=sc, bufs=bufs, saved=(acts, pres, xms))
+            st = self._train_state(b, gh, gw, grid)
+            st["bufs"]["carry"] = torch.empty(b, self.out_chan, gh, gw, dtype=torch.float32, device=self.device)
             if len(self._ws_cache) > 16:
                 self._ws_cache.clear()
             self._ws_cache[key] = st
         return st
+
+    def _train_state(self, b: int, gh: int, gw: int, grid: bool) -> dict:
+        """One saved set and the backward scratch of a training step of batch `b` (not cached): dict(sv=FnoTrainSaved,
+        sc=FnoBwdScratch, bufs=the scratch tensors, saved=(acts, pres, xms)).  Any batch up to `b` can run on them."""
+        lib = _lib.load()
+        dev, L = self.device, self.num_layers
+        adt = torch.float32 if grid else self._act_torch_dtype()
+        acts = [torch.empty(b, HIDDEN, gh, gw, dtype=adt, device=dev) for _ in range(L + 1)]
+        pres = [torch.empty(b, HIDDEN, gh, gw, dtype=torch.float32, device=dev) for _ in range(L)]
+        xms = [torch.empty(NMODES, b, HIDDEN, dtype=torch.complex64, device=dev) for _ in range(L)]
+        sv = _lib.FnoTrainSaved()
+        for l in range(L + 1):
+            sv.act[l] = acts[l].data_ptr()
+        for l in range(L):
+            sv.pre[l], sv.xm[l] = pres[l].data_ptr(), xms[l].data_ptr()
+        nbytes = lib.fno_grid_bwd_partials_bytes(gh, gw) if grid else lib.fno_bwd_partials_bytes()
+        bufs = dict(
+            d0=torch.empty(b, HIDDEN, gh, gw, dtype=torch.float32, device=dev),
+            d1=torch.empty(b, HIDDEN, gh, gw, dtype=torch.float32, device=dev),
+            dz1=torch.empty(min(b, _lib.BWD_CHUNK), PROJ, gh, gw, dtype=torch.float32, device=dev),
+            gm=torch.empty(NMODES, b, HIDDEN, dtype=torch.complex64, device=dev),
+            gwk=torch.empty(NMODES, HIDDEN, HIDDEN, dtype=torch.complex64, device=dev),
+            partials=torch.empty(nbytes, dtype=torch.uint8, device=dev),
+        )
+        sc = _lib.FnoBwdScratch()
+        sc.d[0], sc.d[1] = bufs["d0"].data_ptr(), bufs["d1"].data_ptr()
+        sc.dz1, sc.gm, sc.gwk = bufs["dz1"].data_ptr(), bufs["gm"].data_ptr(), bufs["gwk"].data_ptr()
+        sc.partials = bufs["partials"].data_ptr()
+        return dict(sv=sv, sc=sc, bufs=bufs, saved=(acts, pres, xms))
 
     def _static_weights(self, pk: dict, gh: int, gw: int, grid: bool) -> dict:
         """Graph-owned copies of the packed weight images (and coordinate tables) with the weight structs pointing at

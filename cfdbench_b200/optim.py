@@ -23,6 +23,15 @@ class FusedAdam(torch.optim.Optimizer):
             raise ValueError("invalid Adam hyper-parameter")
         super().__init__(params, dict(lr=lr, betas=tuple(betas), eps=eps, weight_decay=weight_decay))
 
+    def init_state(self, p: torch.Tensor) -> dict:
+        """The state of parameter `p`, created as torch.optim.Adam creates it on its first step when it is empty."""
+        st = self.state[p]
+        if not st:
+            st["step"] = torch.tensor(0.0)
+            st["exp_avg"] = torch.zeros_like(p)
+            st["exp_avg_sq"] = torch.zeros_like(p)
+        return st
+
     @torch.no_grad()
     def step(self, closure=None):
         loss = None
@@ -46,11 +55,7 @@ class FusedAdam(torch.optim.Optimizer):
                 for i, p in enumerate(chunk):
                     if p.dtype not in (torch.float32, torch.complex64) or not p.is_contiguous() or p.device != dev:
                         raise _lib.FnoNativeError("FusedAdam: parameters must be contiguous float32/complex64 on one device")
-                    st = self.state[p]
-                    if not st:
-                        st["step"] = torch.tensor(0.0)
-                        st["exp_avg"] = torch.zeros_like(p)
-                        st["exp_avg_sq"] = torch.zeros_like(p)
+                    st = self.init_state(p)
                     st["step"] += 1
                     s = int(st["step"].item())
                     if step is None:

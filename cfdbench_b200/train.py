@@ -1,0 +1,382 @@
+"""`train_auto`: the reference's training loop (src/train_auto.py:181-313, `train`) with every step replayed from a CUDA
+graph and one synchronisation per epoch.
+
+The reference builds an autograd graph per batch, makes about fifteen native launches through ctypes around it and ends
+every step with `loss["nmse"].item()`, so the host never runs ahead of the GPU.  Here one training step -- stage the
+batch's indices, gather, pack the weights, training forward, loss forward and backward, backward, Adam, log the loss --
+is captured once as a CUDA graph (plus one for a ragged last batch) and replayed once per step.  What changes from step
+to step lives on the device and is read through a step cursor: the epoch's permutation, a table of Adam's bias-corrected
+coefficients and the epoch's loss log.  Per epoch the host uploads the permutation and the table (asynchronously, from
+pinned memory), resets the cursor, replays the graphs and copies the log back: that copy is the epoch's one
+synchronisation.  The result is bit-identical to the eager loop `DeviceFrames.loader` + `model(**batch)` +
+`loss["nmse"].backward()` + `FusedAdam.step()` + `zero_grad()` with the same generator and StepLR.
+
+    from cfdbench_b200 import train_auto
+    train_auto(model, train_data, dev_data, output_dir, num_epochs=..., lr=..., batch_size=...)   # for train(...)
+"""
+from __future__ import annotations
+
+import ctypes as C
+import json
+import time
+import warnings
+from pathlib import Path
+from shutil import copyfile
+from typing import List, Optional
+
+import numpy as np
+import torch
+
+from . import _lib
+from .data import DeviceFrames, case_table, index_batches
+
+LOG_COLUMNS = ("mse", "rmse", "mae", "nmse", "mean_l2")   # one row of the epoch log: fno_loss_fwd's five scalars
+
+
+# ------------------------------------------------------------------------------------------------ visiting order
+def epoch_permutation(n: int, batch_size: int, generator=None) -> np.ndarray:
+    """The sample order of one pass of `DataLoader(train_data, batch_size, shuffle=True, generator=generator)` (int64),
+    drawing from the RNG exactly what that pass draws (`index_batches`)."""
+    # the pass runs to its end: exhausting the sampler draws from an explicit generator too
+    return np.asarray([i for b in index_batches(n, batch_size, True, generator) for i in b], dtype=np.int64)
+
+
+def dev_eval_draw(generator=None) -> None:
+    """What iterating the reference's `evaluate` loader (`DataLoader(dev_data, shuffle=False)`, src/train_auto.py:72-74)
+    draws from the RNG: one base seed.  Without it every epoch after the first evaluation would be visited in another
+    order than the reference's."""
+    next(index_batches(1, 1, False, generator))
+
+
+def index_stream(n: int, batch_size: int, num_epochs: int, eval_interval: int, generator=None) -> List[np.ndarray]:
+    """The per-epoch sample orders `train_auto` visits, consuming the RNG as `train_auto` does: epoch ep's permutation,
+    then one evaluation draw when (ep + 1) % eval_interval == 0."""
+    out = []
+    for ep in range(num_epochs):
+        out.append(epoch_permutation(n, batch_size, generator))
+        if (ep + 1) % eval_interval == 0:
+            dev_eval_draw(generator)
+    return out
+
+
+def dump_json(data, path) -> None:   # reference src/utils/common.py:23-25
+    with open(path, "w", encoding="utf8") as f:
+        json.dump(data, f, indent=2, ensure_ascii=False)
+
+
+# ------------------------------------------------------------------------------------------------ the step graphs
+def _real(t: torch.Tensor) -> torch.Tensor:   # complex parameters are updated as pairs of reals, as FusedAdam does
+    return torch.view_as_real(t) if t.is_complex() else t
+
+
+class _StepGraphs:
+    """The captured training step of a full batch of `batch_size` samples and, when n % batch_size != 0, of the ragged
+    last batch.  Both graphs run on one set of static buffers sized for min(batch_size, n) samples: the ragged graph
+    uses the first r samples' worth of every buffer.  The parameters and the optimizer state are read and written in
+    place; the packed weight images are rebuilt inside the graph from the parameters as the previous replay's Adam
+    left them."""
+
+    def __init__(self, model, frames: DeviceFrames, batch_size: int, optimizer):
+        lib = self.lib = _lib.load()
+        self.model, self.frames, self.optimizer = model, frames, optimizer
+        dev = self.dev = model.device
+        n, gh, gw = frames.n, frames.height, frames.width
+        self.n, self.gh, self.gw, self.stride = n, gh, gw, batch_size
+        self.grid = grid = model._on_grid_path(gh, gw)
+        bmax = min(batch_size, n)
+        n_full, rem = divmod(n, batch_size)
+        self.sizes = [batch_size] * (n_full > 0) + [rem] * (rem > 0)   # the batch size of each graph
+        self.counts = [n_full] * (n_full > 0) + [1] * (rem > 0)      # replays of each graph per epoch
+        self.steps = n_full + (rem > 0)
+        p = frames.n_case_params
+
+        pk = model._pack(need_bwd=True)
+        self.sw = model._static_weights(pk, gh, gw, grid)   # graph-owned weight images, refilled by every replay
+        model._refresh_static_weights(self.sw, pk, gh, gw, grid)   # (also fills the coordinate tables)
+        self.ws, self.ws_bufs = model._grid_workspace(bmax, gh, gw) if grid else model._workspace(bmax)
+        self.ts = model._train_state(bmax, gh, gw, grid)
+        self.flat, _, self.grads = model._grad_buffers()
+
+        f32 = dict(dtype=torch.float32, device=dev)
+        self.io = io = dict(
+            perm=torch.zeros(n, dtype=torch.int64, device=dev),
+            idx=torch.zeros(bmax, dtype=torch.int64, device=dev),
+            inputs=torch.empty(bmax, 2, gh, gw, **f32), label=torch.empty(bmax, 2, gh, gw, **f32),
+            mask=torch.empty(bmax, 1, gh, gw, **f32), cp=torch.empty(bmax, p, **f32),
+            labm=torch.empty(bmax, 2, gh, gw, **f32), preds=torch.empty(bmax, 2, gh, gw, **f32),
+            dpreds=torch.empty(bmax, 2, gh, gw, **f32), loss=torch.empty(5, **f32),
+            scratch=torch.zeros(lib.fno_loss_scratch_bytes(), dtype=torch.uint8, device=dev),
+            gout=torch.zeros(4, **f32),   # d/d(mse, rmse, mae, nmse) of loss["nmse"]: (0, 0, 0, 1)
+            cursor=torch.zeros(1, dtype=torch.int32, device=dev),
+            coef=torch.empty(self.steps, 2, **f32), log=torch.empty(self.steps, len(LOG_COLUMNS), **f32))
+        io["gout"][3:].fill_(1.0)   # a fill kernel: assigning a Python number to a CUDA element is a blocking copy
+        self.perm_host = torch.empty(n, dtype=torch.int64, pin_memory=True)
+        self.coef_host = torch.empty(self.steps, 2, dtype=torch.float32, pin_memory=True)
+
+        # Adam over the parameters that require grad (the ones autograd gives a .grad, so the ones FusedAdam.step
+        # updates), chunked as FusedAdam.step chunks them; the state is created as FusedAdam creates it.  The backward
+        # writes every parameter's gradient into the flat buffer; a frozen parameter's is not read.
+        group = optimizer.param_groups[0]
+        layout = [ent for ent in model._grad_layout()[0] if ent[1].requires_grad]
+        self.params = [prm for _, prm, _, _ in layout]
+        states = [optimizer.init_state(prm) for prm in self.params]
+        self.adam = []
+        for i0 in range(0, len(self.params), _lib.ADAM_MAX_TENSORS):
+            t = _lib.FnoAdamTensors()
+            t.count = min(_lib.ADAM_MAX_TENSORS, len(self.params) - i0)
+            for i in range(t.count):
+                prm, st, (_, _, off, numel) = self.params[i0 + i], states[i0 + i], layout[i0 + i]
+                t.param[i] = _real(prm).data_ptr()
+                t.grad[i] = self.flat[off:off + numel].data_ptr()
+                t.exp_avg[i] = _real(st["exp_avg"]).data_ptr()
+                t.exp_avg_sq[i] = _real(st["exp_avg_sq"]).data_ptr()
+                t.n[i] = numel
+            self.adam.append(t)
+        self.states = states
+        self.betas, self.eps, self.weight_decay = group["betas"], group["eps"], group["weight_decay"]
+
+        # capture: a warm-up of every launch except Adam and the log (it updates nothing: parameters, optimizer state
+        # and cursor stay as they are), then one capture per batch size
+        cur = torch.cuda.current_stream(dev)
+        side = torch.cuda.Stream(device=dev)
+        side.wait_stream(cur)
+        self.graphs = []
+        with torch.no_grad(), torch.cuda.stream(side):
+            for b in self.sizes:
+                self._issue(b, update=False)
+            for b in self.sizes:
+                g = torch.cuda.CUDAGraph()
+                g.capture_begin(capture_error_mode="thread_local")   # nothing is allocated during the capture
+                try:
+                    self._issue(b, update=True)
+                finally:
+                    g.capture_end()
+                self.graphs.append(g)
+        cur.wait_stream(side)
+
+    def _issue(self, b: int, update: bool) -> None:
+        """One training step of batch b on the static buffers, on the current stream."""
+        lib, model, io, sw = self.lib, self.model, self.io, self.sw
+        gh, gw, grid, p = self.gh, self.gw, self.grid, self.frames.n_case_params
+        st = C.c_void_p(torch.cuda.current_stream(self.dev).cuda_stream)
+        fr = self.frames
+        _lib.check(lib.fno_train_stage_indices(io["perm"].data_ptr(), self.n, self.stride, b, io["cursor"].data_ptr(),
+                                               io["idx"].data_ptr(), st), "fno_train_stage_indices")
+        args = (fr.frames_in.data_ptr(), fr.frames_out.data_ptr(), fr.case_table.data_ptr(), fr.case_ids.data_ptr(),
+                io["idx"].data_ptr(), b, p, _lib.ACT_BF16 if fr.frame_dtype == torch.bfloat16 else _lib.ACT_F32,
+                io["inputs"].data_ptr(), io["label"].data_ptr(), io["mask"].data_ptr(), io["cp"].data_ptr())
+        if (gh, gw) == (64, 64):
+            _lib.check(lib.fno_gather_batch(*args, st), "fno_gather_batch")
+        else:
+            _lib.check(lib.fno_grid_gather_batch(*args, gh, gw, st), "fno_grid_gather_batch")
+        # the packed weights, from the parameters as the previous step's Adam left them (Fno2d._pack's images)
+        L = model.num_layers
+        wk, w0t, wkT = sw["dst"][:L], sw["dst"][L:2 * L], sw["dst"][2 * L:3 * L]
+        for l, blk in enumerate(model.blocks):
+            for dst, conj in ((wk[l], 0), (wkT[l], 1)):
+                _lib.check(lib.fno_pack_mix_operand_from_weights(blk.conv0.weights1.data_ptr(),
+                                                                 blk.conv0.weights2.data_ptr(), dst.data_ptr(), conj, st),
+                           "fno_pack_mix_operand_from_weights")
+            w0t[l].copy_(blk.w0.weight.view(w0t[l].shape).t())
+        inputs, mask, cp = io["inputs"][:b], io["mask"][:b], io["cp"][:b]
+        preds, labm, dpreds = io["preds"][:b], io["labm"][:b], io["dpreds"][:b]
+        torch.mul(io["label"][:b], mask, out=labm)   # Fno2d.forward's label * mask
+        ts, ws = self.ts, self.ws
+        if grid:
+            _lib.check(lib.fno_grid_forward_train(C.byref(sw["struct"]), inputs.data_ptr(), mask.data_ptr(), cp.data_ptr(),
+                                                  preds.data_ptr(), C.byref(ts["sv"]), C.byref(ws), b, gh, gw, st),
+                       "fno_grid_forward_train")
+        else:
+            _lib.check(lib.fno_forward_train(C.byref(sw["struct"]), inputs.data_ptr(), mask.data_ptr(), cp.data_ptr(),
+                                             preds.data_ptr(), C.byref(ts["sv"]), C.byref(ws), b, model._act_code(), st),
+                       "fno_forward_train")
+        n_el = preds.numel()
+        _lib.check(lib.fno_loss_fwd(preds.data_ptr(), labm.data_ptr(), n_el, io["scratch"].data_ptr(), io["loss"].data_ptr(),
+                                    st), "fno_loss_fwd")
+        _lib.check(lib.fno_loss_bwd(preds.data_ptr(), labm.data_ptr(), io["loss"].data_ptr(), io["gout"].data_ptr(),
+                                    dpreds.data_ptr(), n_el, st), "fno_loss_bwd")
+        if grid:
+            _lib.check(lib.fno_grid_backward(C.byref(sw["struct"]), C.byref(sw["struct_bwd"]), inputs.data_ptr(),
+                                             mask.data_ptr(), cp.data_ptr(), dpreds.data_ptr(), C.byref(ts["sv"]),
+                                             C.byref(self.grads), C.byref(ts["sc"]), C.byref(ws), None, None, b, gh, gw,
+                                             st), "fno_grid_backward")
+        else:
+            _lib.check(lib.fno_backward(C.byref(sw["struct"]), C.byref(sw["struct_bwd"]), inputs.data_ptr(), mask.data_ptr(),
+                                        cp.data_ptr(), dpreds.data_ptr(), C.byref(ts["sv"]), C.byref(self.grads),
+                                        C.byref(ts["sc"]), C.byref(ws), b, model._act_code(), st), "fno_backward")
+        if not update:
+            return
+        b1, b2 = self.betas
+        for t in self.adam:
+            _lib.check(lib.fno_adam_step_dev(C.byref(t), io["coef"].data_ptr(), self.steps, io["cursor"].data_ptr(), b1, b2,
+                                             self.eps, self.weight_decay, st), "fno_adam_step_dev")
+        _lib.check(lib.fno_train_log_step(io["loss"].data_ptr(), io["log"].data_ptr(), self.steps, io["cursor"].data_ptr(),
+                                          st), "fno_train_log_step")
+
+    def epoch(self, perm: np.ndarray, lr: float, first_step: int) -> np.ndarray:
+        """Train one epoch visiting the samples in `perm` at learning rate `lr`, Adam's 1-based step count starting at
+        `first_step`.  Returns the (steps, 5) float32 log of fno_loss_fwd's scalars per step (LOG_COLUMNS)."""
+        io = self.io
+        self.perm_host.numpy()[:] = perm   # the previous epoch's uploads completed before its log came back
+        b1, b2 = self.betas
+        _lib.check(self.lib.fno_adam_coefficients(lr, b1, b2, first_step, self.steps, self.coef_host.data_ptr()),
+                   "fno_adam_coefficients")
+        io["perm"].copy_(self.perm_host, non_blocking=True)
+        io["coef"].copy_(self.coef_host, non_blocking=True)
+        io["cursor"].zero_()
+        for g, count in zip(self.graphs, self.counts):
+            for _ in range(count):
+                g.replay()
+        log = io["log"].cpu().numpy()   # the epoch's one synchronisation
+        # the state torch.optim.Adam would hold, and the version bump FusedAdam.step makes (Fno2d's packed-weight cache
+        # and inference graphs are keyed on the parameters' versions)
+        for st in self.states:
+            st["step"] += self.steps
+        for prm in self.params:
+            torch.autograd.graph.increment_version(prm)
+        return log
+
+
+# ------------------------------------------------------------------------------------------------ train_auto
+def _positive_int(name: str, v) -> None:
+    if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or v < 1:
+        raise ValueError(f"{name} must be a positive int, got {v!r}")
+
+
+def _check_split(model, data, what: str) -> None:
+    """Refuse, before any device work, a split (a DeviceFrames or the reference's dataset object) the model cannot
+    train or evaluate on: malformed or empty frames, a case_ids list of the wrong length, a case-parameter count other
+    than the model's, or a grid / storage mode the model rejects."""
+    if isinstance(data, DeviceFrames):
+        if data.frames_in.device != model.device:
+            raise ValueError(f"{what}: the frames are on {data.frames_in.device}, the model on {model.device}")
+        n, gh, gw, p = data.n, data.height, data.width, data.n_case_params
+    else:
+        ins, labs = getattr(data, "inputs", None), getattr(data, "labels", None)
+        if not isinstance(ins, torch.Tensor) or not isinstance(labs, torch.Tensor) or ins.dim() != 4 \
+                or ins.shape[1] != 3 or labs.shape != ins.shape:
+            raise ValueError(f"{what} must be a DeviceFrames or a dataset with (N, 3, H, W) .inputs / .labels tensors, "
+                             f"got {getattr(ins, 'shape', None)} / {getattr(labs, 'shape', None)}")
+        n, gh, gw = int(ins.shape[0]), int(ins.shape[2]), int(ins.shape[3])
+        if n == 0:
+            raise ValueError(f"{what} is empty")
+        if len(np.asarray(data.case_ids)) != n:
+            raise ValueError(f"{what}: dataset.case_ids must have one entry per sample")
+        p = case_table(data.case_params).shape[1]
+    if n == 0:
+        raise ValueError(f"{what} is empty")
+    if p != model.n_case_params:
+        raise ValueError(f"{what} has {p} case parameters per sample, the model takes n_case_params="
+                         f"{model.n_case_params}")
+    model._check_grid((gh, gw))      # the model's own grid / storage-mode checks
+    model._on_grid_path(gh, gw)
+
+
+def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, lr: float = 1e-3, lr_step_size: int = 1,
+               lr_gamma: float = 0.9, batch_size: int = 2, eval_batch_size: int = 2, log_interval: int = 10,
+               eval_interval: int = 2, generator: Optional[torch.Generator] = None) -> dict:
+    """What the reference's `train(model, train_data, dev_data, output_dir, ...)` does (src/train_auto.py:181-313), with
+    its argument names and defaults, every training step replayed from a CUDA graph and one synchronisation per epoch.
+
+    model: the drop-in `Fno2d` on a CUDA device, with a loss whose score names include "nmse" (the loss the reference
+    backpropagates); the step computes that loss with the native MseLoss kernels.  train_data / dev_data: the
+    reference's dataset objects or `DeviceFrames` of them (a dataset is uploaded once, in float32).
+
+    - Optimizer: `FusedAdam(model.parameters(), lr)` with `torch.optim.lr_scheduler.StepLR(step_size=lr_step_size,
+      gamma=lr_gamma)`; each epoch runs at the learning rate StepLR leaves in the parameter group.
+    - Visiting order: the reference's for the same RNG -- `generator`, or the global RNG for None, as in the reference.
+      Each epoch draws what one pass of `DataLoader(train_data, batch_size, shuffle=True)` draws, and each evaluation
+      the one base seed that iterating the reference's `DataLoader(dev_data, shuffle=False)` draws.  The ragged last
+      batch is kept (drop_last=False).
+    - Every `eval_interval` epochs: `evaluate_auto(model, <DeviceFrames of dev_data>, batch_size=eval_batch_size)` and
+      the reference's files in `output_dir / f"ckpt-{ep}"`: dev_scores.json, train_loss.json, model.pt (the previous
+      one copied to backup_model.pt first when it exists) and scores.json (ep, train_loss, dev_loss, time).  At the end
+      `output_dir / "train_losses.json"`.  JSON is written as the reference's dump_json writes it.
+    - Logging: the reference's line every `log_interval` steps, printed at the end of the epoch from the device log, so
+      its `time` field is the time of printing, not of the step.
+    - Not reproduced: example.png, train_losses.png and the evaluation images; `measure_time`.
+
+    Returns dict(train_losses=[per-step nmse, every epoch], optimizer=the FusedAdam).  Its state holds the true step
+    count (its state_dict loads into torch.optim.Adam), and the parameters' version counters are bumped, so the
+    model's packed weights and inference graphs are rebuilt on the next call.  Raises before any device work on: a
+    model that is not the drop-in Fno2d, a CPU model (FnoNativeError), a loss without "nmse", non-positive sizes,
+    intervals or epoch count, a model whose parameters are all frozen, an empty or malformed split, a split whose
+    case-parameter count differs from the model's, data parallel enabled, or a grid / storage mode the model rejects.
+    Frozen parameters (requires_grad=False) are not updated, as FusedAdam.step skips them.  Data parallel training in
+    this loop is not supported."""
+    from .metrics import evaluate_auto
+    from .fno2d import Fno2d
+    from .optim import FusedAdam
+    if not isinstance(model, Fno2d):
+        raise TypeError(f"train_auto runs the drop-in cfdbench_b200.Fno2d, got {type(model).__name__}")
+    names = list(model.loss_fn.get_score_names())
+    if "nmse" not in names:
+        raise ValueError(f"the model's loss has scores {names}: train_auto backpropagates loss['nmse'], as the reference")
+    for name, v in (("num_epochs", num_epochs), ("lr_step_size", lr_step_size), ("batch_size", batch_size),
+                    ("eval_batch_size", eval_batch_size), ("log_interval", log_interval), ("eval_interval", eval_interval)):
+        _positive_int(name, v)
+    if model._dp_enabled:
+        raise ValueError("train_auto does not run data parallel: its step graph has no all-reduce")
+    if not any(p.requires_grad for p in model.parameters()):
+        raise ValueError("every parameter of the model is frozen: there is nothing to train")
+    dev = model.device
+    for what, data in (("train_data", train_data), ("dev_data", dev_data)):
+        _check_split(model, data, what)
+    model._require_cuda()
+    output_dir = Path(output_dir)
+    output_dir.mkdir(exist_ok=True, parents=True)
+
+    optimizer = FusedAdam(model.parameters(), lr=lr)
+    scheduler = torch.optim.lr_scheduler.StepLR(optimizer, step_size=lr_step_size, gamma=lr_gamma)
+    with torch.cuda.device(dev):
+        frames = train_data if isinstance(train_data, DeviceFrames) else DeviceFrames(train_data, device=dev)
+        dev_frames = None
+        n = frames.n
+        graphs = _StepGraphs(model, frames, batch_size, optimizer)
+        print("====== Training ======")
+        print(f"# batch: {batch_size}")
+        print(f"# examples: {n}")
+        print(f"# step: {graphs.steps}")
+        print(f"# epoch: {num_epochs}")
+        start_time = time.time()
+        global_step = 0
+        train_losses: List[float] = []
+        try:
+            for ep in range(num_epochs):
+                ep_start_time = time.time()
+                lr_ep = optimizer.param_groups[0]["lr"]
+                log = graphs.epoch(epoch_permutation(n, batch_size, generator), lr_ep, global_step + 1)
+                ep_train_losses = [float(v) for v in log[:, 3]]
+                for step in range(graphs.steps):
+                    global_step += 1
+                    if global_step % log_interval == 0:
+                        print(dict(ep=ep, step=step, mse=f"{float(log[step, 0]):.3e}", nmse=f"{float(log[step, 3]):.3e}",
+                                   lr=f"{scheduler.get_last_lr()[0]:.3e}", time=round(time.time() - start_time)))
+                with warnings.catch_warnings():   # the optimizer steps ran inside the graph, not through .step()
+                    warnings.filterwarnings("ignore", message=r"Detected call of `lr_scheduler\.step\(\)` before")
+                    scheduler.step()
+                train_losses += ep_train_losses
+                if (ep + 1) % eval_interval == 0:
+                    dev_eval_draw(generator)
+                    ckpt_dir = output_dir / f"ckpt-{ep}"
+                    ckpt_dir.mkdir(exist_ok=True, parents=True)
+                    if dev_frames is None:
+                        dev_frames = dev_data if isinstance(dev_data, DeviceFrames) else DeviceFrames(dev_data, device=dev)
+                    dev_scores = evaluate_auto(model, dev_frames, batch_size=eval_batch_size)["scores"]
+                    dump_json(dev_scores, ckpt_dir / "dev_scores.json")
+                    dump_json(ep_train_losses, ckpt_dir / "train_loss.json")
+                    ckpt_path = ckpt_dir / "model.pt"
+                    print(f"Saving checkpoint to {ckpt_path}")
+                    if ckpt_path.exists():
+                        ckpt_backup_path = ckpt_dir / "backup_model.pt"
+                        print(f"Backing up old checkpoint to {ckpt_backup_path}")
+                        copyfile(ckpt_path, ckpt_backup_path)
+                    torch.save(model.state_dict(), ckpt_path)
+                    ep_scores = dict(ep=ep, train_loss=np.mean(ep_train_losses), dev_loss=np.mean(dev_scores["all"]["nmse"]),
+                                     time=time.time() - ep_start_time)
+                    dump_json(ep_scores, ckpt_dir / "scores.json")
+        finally:
+            del graphs   # the graphs and their static buffers go with the call
+    print("====== Training done ======")
+    dump_json(train_losses, output_dir / "train_losses.json")
+    return dict(train_losses=train_losses, optimizer=optimizer)

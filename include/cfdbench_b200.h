@@ -281,6 +281,27 @@ typedef struct fno_adam_tensors {
 int fno_adam_step(const fno_adam_tensors* t, float lr, float beta1, float beta2, float eps, float weight_decay,
                   int64_t step, void* stream);
 
+/* ---- one training step replayed from a CUDA graph, step after step (cfdbench_b200.train_auto) --------------------
+ * What changes from step to step is read on the device through a step cursor `cursor` (one int32 in device memory,
+ * reset by the caller at the start of an epoch and advanced by fno_train_log_step): the step's sample indices, Adam's
+ * coefficients and the row of the step's losses.  Every entry point checks its arguments before any device work
+ * (status 1 with a fno_last_error() message); a cursor that would read or write outside a table makes the launch write
+ * nothing. */
+/* idx_out[i] = perm[cursor * stride + i] for i < batch (int64 indices); nothing is written when
+ * cursor * stride + batch > n_perm.  batch <= stride and batch <= n_perm. */
+int fno_train_stage_indices(const int64_t* perm, int64_t n_perm, int stride, int batch, const int32_t* cursor,
+                            int64_t* idx_out, void* stream);
+/* fno_adam_step with (step_size, inv_bc2_sqrt) = (coef[2c], coef[2c + 1]), c = *cursor, read on the device; nothing is
+ * written when c is outside 0..n_coef-1.  coef: 8-byte aligned float32 [n_coef][2], as fno_adam_coefficients fills it. */
+int fno_adam_step_dev(const fno_adam_tensors* t, const float* coef, int n_coef, const int32_t* cursor, float beta1,
+                      float beta2, float eps, float weight_decay, void* stream);
+/* Host function: host_out[2i], host_out[2i + 1] = the step size lr / (1 - beta1^s) and 1 / sqrt(1 - beta2^s) of step
+ * s = first_step + i, i < n, with exactly the arithmetic fno_adam_step uses (double, then float). */
+int fno_adam_coefficients(float lr, float beta1, float beta2, int64_t first_step, int n, float* host_out);
+/* log[c][0..4] = loss_out[0..4] (fno_loss_fwd's five scalars), c = *cursor, then ++*cursor; nothing is written when c is
+ * outside 0..n_log-1. */
+int fno_train_log_step(const float* loss_out, float* log, int n_log, int32_t* cursor, void* stream);
+
 /* ---------------------------------------------------------------------------------------------------
  * Grid-generic path: the same network on H x W frames with 24 <= H <= 128 and 24 <= W <= 128, e.g. CFDBench's
  * tube and dam problems (66 x 65, reference src/utils/autoregressive.py:24-26).  fp32 activation storage only (there is
