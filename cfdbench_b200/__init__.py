@@ -6,13 +6,16 @@ Public surface mirrors the reference's for this path:
     MseLoss, loss_name_to_fn               (reference src/models/loss.py)
     infer_multistep                        (reference src/test_multistep.py infer, batched on the device)
     evaluate_auto                          (reference src/train_auto.py evaluate, batched on the device)
-    train_auto                             (reference src/train_auto.py train, steps replayed from CUDA graphs)
+    train_auto                             (reference src/train_auto.py train, steps replayed from CUDA graphs;
+                                            rollout_steps=K trains through K-step rollouts)
+    rollout_windows                        (the valid K-step window starts of a split)
 """
 from .base_model import AutoCfdModel
 from .loss import MseLoss, loss_name_to_fn
 
 __all__ = ["AutoCfdModel", "MseLoss", "loss_name_to_fn", "Fno2d", "FnoBlock", "SpectralConv2d_fast", "FusedAdam", "DeviceFrames",
-           "infer_multistep", "evaluate_auto", "train_auto"]
+           "infer_multistep", "evaluate_auto", "train_auto",
+           "rollout_windows"]
 
 
 def __getattr__(name):  # lazy: importing the package must not require the native library
@@ -31,6 +34,9 @@ def __getattr__(name):  # lazy: importing the package must not require the nativ
     if name == "evaluate_auto":
         from .metrics import evaluate_auto
         return evaluate_auto
+    if name == "rollout_windows":
+        from .data import rollout_windows
+        return rollout_windows
     if name == "train_auto":
         from .train import train_auto
         return train_auto

@@ -161,6 +161,13 @@ SIGNATURES = {
     "fno_grid_multistep_metrics": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _P]),
     "fno_grid_gather_batch": (C.c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _P, _P, _P, _P, _I, _I, _P]),
     "fno_eval_sums": (C.c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _P]),
+    # training through K-step rollouts
+    "fno_gather_window": (C.c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _P, _P, _P, _P, _I, _I, C.c_int64, _P, _P]),
+    "fno_grid_gather_window": (C.c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _P, _P, _P, _P, _I, _I, C.c_int64, _P, _I, _I,
+                                         _P]),
+    "fno_loss_seq_scratch_bytes": (C.c_size_t, [_I]),
+    "fno_loss_seq_fwd": (C.c_int, [_P, _P, C.c_size_t, _I, _P, _P, _P]),
+    "fno_loss_seq_bwd": (C.c_int, [_P, _P, _P, _P, _P, C.c_size_t, _I, _P]),
 }
 
 GRID_MIN, GRID_MAX = 24, 128

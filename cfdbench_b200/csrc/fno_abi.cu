@@ -78,6 +78,14 @@ cudaError_t launch_grid_multistep_metrics(const float*, const float*, const floa
 cudaError_t launch_grid_gather_batch(const void*, const void*, const float*, const int*, const long long*, int, int, int,
                                      float*, float*, float*, float*, int, int, cudaStream_t);
 cudaError_t launch_eval_sums(const float*, const float*, const float*, const float*, float*, int, int, int, cudaStream_t);
+// training through K-step rollouts (fno_metrics.cu, fno_train_step.cu)
+cudaError_t launch_gather_window(const void*, const void*, const float*, const int*, const long long*, int, int, int, float*,
+                                 float*, float*, float*, int, int, long long, float*, cudaStream_t);
+cudaError_t launch_grid_gather_window(const void*, const void*, const float*, const int*, const long long*, int, int, int,
+                                      float*, float*, float*, float*, int, int, long long, float*, int, int, cudaStream_t);
+cudaError_t launch_loss_seq_fwd(const float*, const float*, size_t, int, float*, float*, cudaStream_t);
+cudaError_t launch_loss_seq_bwd(const float*, const float*, const float*, const float*, float*, size_t, int, cudaStream_t);
+size_t loss_seq_scratch_bytes(int);
 }  // namespace fno
 
 using namespace fno;
@@ -619,6 +627,56 @@ int fno_train_log_step(const float* loss_out, float* log, int n_log, int32_t* cu
   return kOk;
 }
 
+// ------------------------------------------------------------------------------------------------ K-step rollout training
+static constexpr int kMaxSeqSteps = (65535 - 5) / 2;   // the gathers put 5 + 2 steps planes, the losses steps, on grid.y
+
+static int gather_window_args(const char* what, const void* frames_in, const void* frames_out, const float* case_table,
+                              const int32_t* case_ids, const int64_t* idx, int n_idx, int n_case_params, int frame_dtype,
+                              const float* inputs, const float* mask, const float* case_params, int steps,
+                              int time_step_size, int64_t n_frames, const float* labels_seq) {
+  char msg[160];
+  if (!frames_in || !frames_out || !case_ids || !idx || !inputs || !mask || !labels_seq || n_idx <= 0 ||
+      n_case_params < 0 || n_case_params > kMaxCaseParams || bad_dtype(frame_dtype) ||
+      (n_case_params > 0 && (!case_table || !case_params)) || steps < 1 || steps > kMaxSeqSteps || time_step_size < 1 ||
+      n_frames < 1) {
+    snprintf(msg, sizeof(msg), "%s: bad argument", what);
+    return fail(kErrArg, msg);
+  }
+  return kOk;
+}
+
+int fno_gather_window(const void* frames_in, const void* frames_out, const float* case_table, const int32_t* case_ids,
+                      const int64_t* idx, int n_idx, int n_case_params, int frame_dtype, float* inputs, float* label,
+                      float* mask, float* case_params, int steps, int time_step_size, int64_t n_frames, float* labels_seq,
+                      void* stream) {
+  FNO_TRY(gather_window_args("fno_gather_window", frames_in, frames_out, case_table, case_ids, idx, n_idx, n_case_params,
+                             frame_dtype, inputs, mask, case_params, steps, time_step_size, n_frames, labels_seq));
+  FNO_CUDA(launch_gather_window(frames_in, frames_out, case_table, reinterpret_cast<const int*>(case_ids),
+                                reinterpret_cast<const long long*>(idx), n_idx, n_case_params, frame_dtype == FNO_ACT_BF16,
+                                inputs, label, mask, case_params, steps, time_step_size, n_frames, labels_seq, S(stream)),
+           "gather_window_kernel");
+  return kOk;
+}
+
+size_t fno_loss_seq_scratch_bytes(int steps) { return steps < 1 ? 0 : loss_seq_scratch_bytes(steps); }
+
+int fno_loss_seq_fwd(const float* preds_seq, const float* labels_seq, size_t n, int steps, void* scratch, float* out,
+                     void* stream) {
+  if (!preds_seq || !labels_seq || !scratch || !out || n == 0 || steps < 1 || steps > kMaxSeqSteps)
+    return fail(kErrArg, "fno_loss_seq_fwd: bad argument");
+  FNO_CUDA(launch_loss_seq_fwd(preds_seq, labels_seq, n, steps, static_cast<float*>(scratch), out, S(stream)),
+           "loss_seq_fwd_kernel");
+  return kOk;
+}
+
+int fno_loss_seq_bwd(const float* preds_seq, const float* labels_seq, const float* fwd, const float* gout, float* dpreds_seq,
+                     size_t n, int steps, void* stream) {
+  if (!preds_seq || !labels_seq || !fwd || !gout || !dpreds_seq || n == 0 || steps < 1 || steps > kMaxSeqSteps)
+    return fail(kErrArg, "fno_loss_seq_bwd: bad argument");
+  FNO_CUDA(launch_loss_seq_bwd(preds_seq, labels_seq, fwd, gout, dpreds_seq, n, steps, S(stream)), "loss_seq_bwd_kernel");
+  return kOk;
+}
+
 // ------------------------------------------------------------------------------------------------ grid-generic fp32 path
 static int grid_arg(const char* what, int h, int w) {
   char msg[160];
@@ -921,6 +979,22 @@ int fno_grid_gather_batch(const void* frames_in, const void* frames_out, const f
                                     reinterpret_cast<const long long*>(idx), n_idx, n_case_params,
                                     frame_dtype == FNO_ACT_BF16, inputs, label, mask, case_params, h, wd, S(stream)),
            "grid_gather_batch_kernel");
+  return kOk;
+}
+
+int fno_grid_gather_window(const void* frames_in, const void* frames_out, const float* case_table, const int32_t* case_ids,
+                           const int64_t* idx, int n_idx, int n_case_params, int frame_dtype, float* inputs, float* label,
+                           float* mask, float* case_params, int steps, int time_step_size, int64_t n_frames,
+                           float* labels_seq, int h, int wd, void* stream) {
+  FNO_TRY(grid_arg("fno_grid_gather_window", h, wd));
+  FNO_TRY(gather_window_args("fno_grid_gather_window", frames_in, frames_out, case_table, case_ids, idx, n_idx,
+                             n_case_params, frame_dtype, inputs, mask, case_params, steps, time_step_size, n_frames,
+                             labels_seq));
+  FNO_CUDA(launch_grid_gather_window(frames_in, frames_out, case_table, reinterpret_cast<const int*>(case_ids),
+                                     reinterpret_cast<const long long*>(idx), n_idx, n_case_params,
+                                     frame_dtype == FNO_ACT_BF16, inputs, label, mask, case_params, steps, time_step_size,
+                                     n_frames, labels_seq, h, wd, S(stream)),
+           "gather_window_kernel");
   return kOk;
 }
 

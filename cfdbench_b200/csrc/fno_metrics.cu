@@ -276,3 +276,101 @@ cudaError_t launch_grid_gather_batch(const void* frames_in, const void* frames_o
 }
 
 }  // namespace fno
+
+// ------------------------------------------------------------------------------------------------
+// Window gather for training through K-step rollouts (cfdbench_b200.train_auto with rollout_steps = K).  A dataset holds
+// a case's samples contiguously with inputs = frames[:-s], labels = frames[s:] (s = time_step_size), so the k-th target of
+// the window that starts at sample j is labels[j + k s].  One launch gathers the start samples as the gathers above do and
+// the K masked targets of each window:
+//   inputs, label, mask, case_params as gather_batch_kernel / grid_gather_batch_kernel for the same idx (label is skipped
+//   when null), labels_seq[k][b][c] = frames_out[idx[b] + k s][c] * frames_in[idx[b]][2]   (c = u, v; one fp32 multiply,
+//   so it equals label * mask bit for bit).
+// A window that runs past n_frames is not read and none of its sample's outputs are written, the guard style of the
+// step-cursor kernels.  grid (n_idx, 5 + 2 steps): plane 0,1 -> inputs; 2 -> mask; 3,4 -> label; 5 + 2k + c -> labels_seq.
+// kVec: 64x64 frames, 16-byte accesses as gather_batch_kernel; otherwise scalar accesses (see the grid section's header).
+// ------------------------------------------------------------------------------------------------
+namespace fno {
+
+template <typename TFrame, bool kVec>
+__global__ void __launch_bounds__(kGbThreads)
+    gather_window_kernel(const TFrame* __restrict__ frames_in, const TFrame* __restrict__ frames_out,
+                         const float* __restrict__ case_table, const int* __restrict__ case_ids,
+                         const long long* __restrict__ idx, int n_idx, int n_case_params, int hw, int steps,
+                         int time_step_size, long long n_frames, float* __restrict__ inputs, float* __restrict__ label,
+                         float* __restrict__ mask, float* __restrict__ case_params, float* __restrict__ labels_seq) {
+  const int b = blockIdx.x, plane = blockIdx.y;
+  const long long i = idx[b];
+  if (i < 0 || i + static_cast<long long>(steps - 1) * time_step_size >= n_frames) return;
+  const TFrame* src;
+  const TFrame* msk = nullptr;
+  float* dst;
+  if (plane < 3) {
+    src = frames_in + (static_cast<size_t>(i) * 3 + plane) * hw;
+    dst = plane < 2 ? inputs + (static_cast<size_t>(b) * 2 + plane) * hw : mask + static_cast<size_t>(b) * hw;
+  } else if (plane < 5) {
+    if (label == nullptr) return;
+    src = frames_out + (static_cast<size_t>(i) * 3 + (plane - 3)) * hw;
+    dst = label + (static_cast<size_t>(b) * 2 + (plane - 3)) * hw;
+  } else {
+    const int k = (plane - 5) >> 1, c = (plane - 5) & 1;
+    src = frames_out + ((static_cast<size_t>(i) + static_cast<size_t>(k) * time_step_size) * 3 + c) * hw;
+    msk = frames_in + (static_cast<size_t>(i) * 3 + 2) * hw;
+    dst = labels_seq + ((static_cast<size_t>(k) * n_idx + b) * 2 + c) * hw;
+  }
+  if constexpr (kVec) {
+    for (int e = threadIdx.x * 4; e < kHW; e += kGbThreads * 4) {
+      float4 v = gather_ld4<TFrame>(src + e);
+      if (msk) {
+        const float4 m = gather_ld4<TFrame>(msk + e);
+        v.x *= m.x;
+        v.y *= m.y;
+        v.z *= m.z;
+        v.w *= m.w;
+      }
+      *reinterpret_cast<float4*>(dst + e) = v;
+    }
+  } else {
+    for (int e = threadIdx.x; e < hw; e += kGbThreads) dst[e] = msk ? frame_ld(src + e) * frame_ld(msk + e) : frame_ld(src + e);
+  }
+  if (plane == 0 && threadIdx.x < n_case_params)
+    case_params[static_cast<size_t>(b) * n_case_params + threadIdx.x] =
+        __ldg(case_table + static_cast<size_t>(case_ids[i]) * n_case_params + threadIdx.x);
+}
+
+template <bool kVec>
+static cudaError_t launch_gather_window_impl(const void* frames_in, const void* frames_out, const float* case_table,
+                                             const int* case_ids, const long long* idx, int n_idx, int n_case_params,
+                                             int frame_bf16, float* inputs, float* label, float* mask, float* case_params,
+                                             int steps, int time_step_size, long long n_frames, float* labels_seq, int hw,
+                                             cudaStream_t stream) {
+  dim3 grid(n_idx, 5 + 2 * steps);
+  if (frame_bf16)
+    gather_window_kernel<__nv_bfloat16, kVec><<<grid, kGbThreads, 0, stream>>>(
+        static_cast<const __nv_bfloat16*>(frames_in), static_cast<const __nv_bfloat16*>(frames_out), case_table, case_ids,
+        idx, n_idx, n_case_params, hw, steps, time_step_size, n_frames, inputs, label, mask, case_params, labels_seq);
+  else
+    gather_window_kernel<float, kVec><<<grid, kGbThreads, 0, stream>>>(
+        static_cast<const float*>(frames_in), static_cast<const float*>(frames_out), case_table, case_ids, idx, n_idx,
+        n_case_params, hw, steps, time_step_size, n_frames, inputs, label, mask, case_params, labels_seq);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_gather_window(const void* frames_in, const void* frames_out, const float* case_table, const int* case_ids,
+                                 const long long* idx, int n_idx, int n_case_params, int frame_bf16, float* inputs,
+                                 float* label, float* mask, float* case_params, int steps, int time_step_size,
+                                 long long n_frames, float* labels_seq, cudaStream_t stream) {
+  return launch_gather_window_impl<true>(frames_in, frames_out, case_table, case_ids, idx, n_idx, n_case_params, frame_bf16,
+                                         inputs, label, mask, case_params, steps, time_step_size, n_frames, labels_seq, kHW,
+                                         stream);
+}
+cudaError_t launch_grid_gather_window(const void* frames_in, const void* frames_out, const float* case_table,
+                                      const int* case_ids, const long long* idx, int n_idx, int n_case_params,
+                                      int frame_bf16, float* inputs, float* label, float* mask, float* case_params,
+                                      int steps, int time_step_size, long long n_frames, float* labels_seq, int h, int w,
+                                      cudaStream_t stream) {
+  return launch_gather_window_impl<false>(frames_in, frames_out, case_table, case_ids, idx, n_idx, n_case_params,
+                                          frame_bf16, inputs, label, mask, case_params, steps, time_step_size, n_frames,
+                                          labels_seq, h * w, stream);
+}
+
+}  // namespace fno

@@ -18,19 +18,26 @@ namespace fno {
 constexpr int kLossThreads = 256;
 constexpr int kLossBlocks = 296;  // 2 per SM; also the size of the partial-sum table
 
-// out[0..4] = mse, rmse, mae, nmse, mean(l^2);  scratch: [kLossBlocks][3] floats + one uint32 ticket
-__global__ void __launch_bounds__(kLossThreads)
-    loss_fwd_kernel(const float* __restrict__ preds, const float* __restrict__ labels, size_t n, float* __restrict__ scratch,
-                    float* __restrict__ out) {
-  __shared__ float red[kLossThreads / 32][3];
-  __shared__ bool last;
-  float se = 0.f, sa = 0.f, sl = 0.f;
+// One thread's share of the three sums sum (p-l)^2, sum |p-l|, sum l^2 over n elements, in loss_fwd_kernel's partition:
+// float4 index i = block * kLossThreads + thread, grid-stride nblocks * kLossThreads, the n % 4 tail in block 0.  With
+// `aligned` false the same four elements are read one by one (a slice of a [K][B][2][H][W] tensor at odd H*W is only
+// 4-byte aligned), so the sums do not depend on the alignment.
+__device__ __forceinline__ void loss_thread_sums(const float* __restrict__ preds, const float* __restrict__ labels, size_t n,
+                                                 bool aligned, unsigned block, unsigned nblocks, float& se, float& sa,
+                                                 float& sl) {
   const size_t n4 = n / 4;
   const float4* p4 = reinterpret_cast<const float4*>(preds);
   const float4* l4 = reinterpret_cast<const float4*>(labels);
-  for (size_t i = static_cast<size_t>(blockIdx.x) * kLossThreads + threadIdx.x; i < n4;
-       i += static_cast<size_t>(gridDim.x) * kLossThreads) {
-    const float4 p = __ldg(p4 + i), l = __ldg(l4 + i);
+  for (size_t i = static_cast<size_t>(block) * kLossThreads + threadIdx.x; i < n4;
+       i += static_cast<size_t>(nblocks) * kLossThreads) {
+    float4 p, l;
+    if (aligned) {
+      p = __ldg(p4 + i);
+      l = __ldg(l4 + i);
+    } else {
+      p = make_float4(__ldg(preds + 4 * i), __ldg(preds + 4 * i + 1), __ldg(preds + 4 * i + 2), __ldg(preds + 4 * i + 3));
+      l = make_float4(__ldg(labels + 4 * i), __ldg(labels + 4 * i + 1), __ldg(labels + 4 * i + 2), __ldg(labels + 4 * i + 3));
+    }
     const float d[4] = {p.x - l.x, p.y - l.y, p.z - l.z, p.w - l.w};
     const float lv[4] = {l.x, l.y, l.z, l.w};
 #pragma unroll
@@ -40,13 +47,23 @@ __global__ void __launch_bounds__(kLossThreads)
       sl = fmaf(lv[c], lv[c], sl);
     }
   }
-  if (blockIdx.x == 0)  // tail (n not a multiple of 4)
+  if (block == 0)  // tail (n not a multiple of 4)
     for (size_t i = n4 * 4 + threadIdx.x; i < n; i += kLossThreads) {
       const float d = preds[i] - labels[i];
       se = fmaf(d, d, se);
       sa += fabsf(d);
       sl = fmaf(labels[i], labels[i], sl);
     }
+}
+
+// The block's sums into partials[block][3]; the last of nblocks blocks to arrive (ticket) sums the table in a fixed
+// order (double accumulation), writes out[0..4] = mse, rmse, mae, nmse, mean(l^2) and re-arms the ticket.  Returns true
+// in thread 0 of that block, after its out[] stores.
+__device__ __forceinline__ bool loss_block_reduce(float se, float sa, float sl, size_t n, unsigned block, unsigned nblocks,
+                                                  float* __restrict__ partials, unsigned int* ticket,
+                                                  float* __restrict__ out) {
+  __shared__ float red[kLossThreads / 32][3];
+  __shared__ bool last;
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
     se += __shfl_xor_sync(0xffffffffu, se, o);
@@ -60,7 +77,6 @@ __global__ void __launch_bounds__(kLossThreads)
     red[warp][2] = sl;
   }
   __syncthreads();
-  unsigned int* ticket = reinterpret_cast<unsigned int*>(scratch + kLossBlocks * 3);
   if (threadIdx.x == 0) {
     float t[3] = {0.f, 0.f, 0.f};
 #pragma unroll
@@ -69,20 +85,20 @@ __global__ void __launch_bounds__(kLossThreads)
       t[1] += red[w][1];
       t[2] += red[w][2];
     }
-    scratch[blockIdx.x * 3 + 0] = t[0];
-    scratch[blockIdx.x * 3 + 1] = t[1];
-    scratch[blockIdx.x * 3 + 2] = t[2];
+    partials[block * 3 + 0] = t[0];
+    partials[block * 3 + 1] = t[1];
+    partials[block * 3 + 2] = t[2];
     __threadfence();
-    last = atomicAdd(ticket, 1u) == gridDim.x - 1;
+    last = atomicAdd(ticket, 1u) == nblocks - 1;
   }
   __syncthreads();
   if (last && threadIdx.x < 32) {  // one warp sums the table in a fixed order (double accumulation)
     __threadfence();
     double t[3] = {0.0, 0.0, 0.0};
-    for (int b = threadIdx.x; b < static_cast<int>(gridDim.x); b += 32) {
-      t[0] += static_cast<double>(scratch[b * 3 + 0]);
-      t[1] += static_cast<double>(scratch[b * 3 + 1]);
-      t[2] += static_cast<double>(scratch[b * 3 + 2]);
+    for (int b = threadIdx.x; b < static_cast<int>(nblocks); b += 32) {
+      t[0] += static_cast<double>(partials[b * 3 + 0]);
+      t[1] += static_cast<double>(partials[b * 3 + 1]);
+      t[2] += static_cast<double>(partials[b * 3 + 2]);
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
@@ -99,8 +115,20 @@ __global__ void __launch_bounds__(kLossThreads)
       out[3] = static_cast<float>(mse / ml2);
       out[4] = static_cast<float>(ml2);
       *ticket = 0u;  // ready for the next call on this scratch buffer
+      return true;
     }
   }
+  return false;
+}
+
+// out[0..4] = mse, rmse, mae, nmse, mean(l^2);  scratch: [kLossBlocks][3] floats + one uint32 ticket
+__global__ void __launch_bounds__(kLossThreads)
+    loss_fwd_kernel(const float* __restrict__ preds, const float* __restrict__ labels, size_t n, float* __restrict__ scratch,
+                    float* __restrict__ out) {
+  float se = 0.f, sa = 0.f, sl = 0.f;
+  loss_thread_sums(preds, labels, n, true, blockIdx.x, gridDim.x, se, sa, sl);
+  loss_block_reduce(se, sa, sl, n, blockIdx.x, gridDim.x, scratch,
+                    reinterpret_cast<unsigned int*>(scratch + kLossBlocks * 3), out);
 }
 
 // dpreds = g_mse 2d/N + g_rmse d/(N rmse) + g_mae sign(d)/N + g_nmse 2d/(N mean(l^2))
@@ -131,6 +159,80 @@ cudaError_t launch_loss_bwd(const float* preds, const float* labels, const float
   return cudaGetLastError();
 }
 size_t loss_scratch_bytes() { return (kLossBlocks * 3 + 4) * sizeof(float); }
+
+// ------------------------------------------------------------------------------------------------ K-step loss
+// The loss of a K-step rollout, (MseLoss(preds_0, labels_0) + ... + MseLoss(preds_{K-1}, labels_{K-1})) / K, in one launch
+// each way.  Step k's slice is preds_seq + k n / labels_seq + k n (n = B*2*H*W), on grid row blockIdx.y = k with
+// loss_fwd_kernel's block partition and reduction order, so row k of the output is bit-identical to fno_loss_fwd on that
+// slice (on an aligned copy when the slice is not 16-byte aligned).  The quotient by K is a multiplication by the float32
+// reciprocal 1/K: that is what `sum(...) / K` computes on 0-dim CUDA tensors (a CUDA tensor divided by a Python number),
+// and what autograd's DivBackward computes for the upstream gradient.
+
+// out[k][0..4] = fno_loss_fwd's five scalars of step k; out[steps][c] = (out[0][c] + ... + out[steps-1][c]) * (1/steps),
+// summed left to right in float32.  scratch: [steps][kLossBlocks][3] floats, then steps + 1 uint32 tickets.
+__global__ void __launch_bounds__(kLossThreads)
+    loss_seq_fwd_kernel(const float* __restrict__ preds_seq, const float* __restrict__ labels_seq, size_t n, int steps,
+                        float* __restrict__ scratch, float* __restrict__ out) {
+  const int k = blockIdx.y;
+  const float* preds = preds_seq + static_cast<size_t>(k) * n;
+  const float* labels = labels_seq + static_cast<size_t>(k) * n;
+  const bool aligned = ((reinterpret_cast<uintptr_t>(preds) | reinterpret_cast<uintptr_t>(labels)) & 15) == 0;
+  unsigned int* tickets = reinterpret_cast<unsigned int*>(scratch + static_cast<size_t>(steps) * kLossBlocks * 3);
+  float se = 0.f, sa = 0.f, sl = 0.f;
+  loss_thread_sums(preds, labels, n, aligned, blockIdx.x, gridDim.x, se, sa, sl);
+  if (!loss_block_reduce(se, sa, sl, n, blockIdx.x, gridDim.x, scratch + static_cast<size_t>(k) * kLossBlocks * 3,
+                         tickets + k, out + static_cast<size_t>(k) * 5))
+    return;
+  // thread 0 of the block that finished step k: the last step to finish forms the aggregate row
+  __threadfence();
+  if (atomicAdd(tickets + steps, 1u) != static_cast<unsigned int>(steps) - 1) return;
+  __threadfence();
+  const float inv_k = 1.f / static_cast<float>(steps);
+#pragma unroll
+  for (int c = 0; c < 5; ++c) {
+    float s = __ldcg(out + c);
+    for (int j = 1; j < steps; ++j) s = s + __ldcg(out + static_cast<size_t>(j) * 5 + c);
+    out[static_cast<size_t>(steps) * 5 + c] = s * inv_k;
+  }
+  tickets[steps] = 0u;
+}
+
+// dpreds_seq[k] = fno_loss_bwd(preds_k, labels_k, fwd[k], gout * (1/steps)): gout holds the upstream gradients of the
+// aggregate row's (mse, rmse, mae, nmse).  loss_bwd_kernel's arithmetic, element by element (scalar accesses).
+__global__ void __launch_bounds__(kLossThreads)
+    loss_seq_bwd_kernel(const float* __restrict__ preds_seq, const float* __restrict__ labels_seq,
+                        const float* __restrict__ fwd, const float* __restrict__ gout, float* __restrict__ dpreds_seq,
+                        size_t n, int steps) {
+  const int k = blockIdx.y;
+  const size_t off = static_cast<size_t>(k) * n;
+  const float inv_k = 1.f / static_cast<float>(steps);
+  const float inv_n = 1.f / static_cast<float>(n);
+  const float g_mse = gout[0] * inv_k, g_rmse = gout[1] * inv_k, g_mae = gout[2] * inv_k, g_nmse = gout[3] * inv_k;
+  const float rmse = fwd[static_cast<size_t>(k) * 5 + 1], ml2 = fwd[static_cast<size_t>(k) * 5 + 4];
+  const float kd = inv_n * (2.f * g_mse + (rmse > 0.f ? g_rmse / rmse : 0.f) + 2.f * g_nmse / ml2);
+  const float ka = inv_n * g_mae;
+  for (size_t i = static_cast<size_t>(blockIdx.x) * kLossThreads + threadIdx.x; i < n;
+       i += static_cast<size_t>(gridDim.x) * kLossThreads) {
+    const float d = preds_seq[off + i] - labels_seq[off + i];
+    const float sgn = d > 0.f ? 1.f : (d < 0.f ? -1.f : 0.f);
+    dpreds_seq[off + i] = fmaf(kd, d, ka * sgn);
+  }
+}
+
+cudaError_t launch_loss_seq_fwd(const float* preds_seq, const float* labels_seq, size_t n, int steps, float* scratch,
+                                float* out, cudaStream_t stream) {
+  loss_seq_fwd_kernel<<<dim3(kLossBlocks, steps), kLossThreads, 0, stream>>>(preds_seq, labels_seq, n, steps, scratch, out);
+  return cudaGetLastError();
+}
+cudaError_t launch_loss_seq_bwd(const float* preds_seq, const float* labels_seq, const float* fwd, const float* gout,
+                                float* dpreds_seq, size_t n, int steps, cudaStream_t stream) {
+  loss_seq_bwd_kernel<<<dim3(kLossBlocks * 2, steps), kLossThreads, 0, stream>>>(preds_seq, labels_seq, fwd, gout,
+                                                                                 dpreds_seq, n, steps);
+  return cudaGetLastError();
+}
+size_t loss_seq_scratch_bytes(int steps) {
+  return static_cast<size_t>(steps) * kLossBlocks * 3 * sizeof(float) + (static_cast<size_t>(steps) + 1) * 4;
+}
 
 // ------------------------------------------------------------------------------------------------ Adam
 constexpr int kAdamThreads = 256;

@@ -55,6 +55,9 @@ class DeviceFrames:
         self.case_ids = torch.as_tensor(np.asarray(dataset.case_ids), dtype=torch.int32, device=dev)
         if self.case_ids.numel() != self.n:
             raise ValueError("dataset.case_ids must have one entry per sample")
+        self._case_ids_host = np.asarray(dataset.case_ids).reshape(-1)   # for the window checks, without a device read
+        # the dataset's label offset (labels = frames[s:], inputs = frames[:-s] per case), None when it has none
+        self.time_step_size = getattr(dataset, "time_step_size", None)
 
     def __len__(self) -> int:
         return self.n
@@ -84,6 +87,54 @@ class DeviceFrames:
         idx.record_stream(torch.cuda.current_stream(dev))
         return out
 
+    def rollout_batch(self, idx, steps: int, time_step_size=None) -> Dict[str, Tensor]:
+        """`batch(idx)` for the windows that start at samples `idx`, plus "labels" (steps, B, 2, H, W): step k's target
+        labels[idx + k s] * mask, masked with the start sample's mask as `Fno2d.rollout` masks its predictions
+        (s = time_step_size, by default the dataset's).  One launch (fno_[grid_]gather_window).
+
+            b = frames.rollout_batch(idx, K)
+            preds = model.rollout(b["inputs"], b["case_params"], b["mask"], K)
+            loss = sum(model.loss_fn(preds=preds[k], labels=b["labels"][k])["nmse"] for k in range(K)) / K
+
+        Raises ValueError for a non-positive steps / time_step_size, no time_step_size at all, or a window that crosses
+        a case boundary; IndexError for a window that runs past the split."""
+        from . import _lib
+        lib = _lib.load()
+        s = self.time_step_size if time_step_size is None else time_step_size
+        if isinstance(steps, bool) or not isinstance(steps, (int, np.integer)) or steps < 1:
+            raise ValueError(f"steps must be a positive int, got {steps!r}")
+        if s is None:
+            raise ValueError("time_step_size is needed: the dataset has none, pass it")
+        if isinstance(s, bool) or not isinstance(s, (int, np.integer)) or s < 1:
+            raise ValueError(f"time_step_size must be a positive int, got {s!r}")
+        idx = torch.as_tensor(idx, dtype=torch.int64)
+        if idx.dim() != 1 or idx.numel() == 0:
+            raise ValueError("idx must be a non-empty 1-D index list")
+        starts = idx.cpu().numpy()
+        ends = starts + (int(steps) - 1) * int(s)
+        if int(starts.min()) < 0 or int(ends.max()) >= self.n:
+            raise IndexError("sample index out of range, or a window runs past the split")
+        cross = np.flatnonzero(self._case_ids_host[starts] != self._case_ids_host[ends])
+        if cross.size:
+            raise ValueError(f"the {steps}-step window that starts at sample {int(starts[cross[0]])} crosses a case boundary")
+        idx = idx.to(self.device, non_blocking=True)
+        b, p, dev, gh, gw = idx.numel(), self.n_case_params, self.device, self.height, self.width
+        out = dict(inputs=torch.empty(b, 2, gh, gw, device=dev), label=torch.empty(b, 2, gh, gw, device=dev),
+                   mask=torch.empty(b, 1, gh, gw, device=dev), case_params=torch.empty(b, p, device=dev),
+                   labels=torch.empty(int(steps), b, 2, gh, gw, device=dev))
+        args = (self.frames_in.data_ptr(), self.frames_out.data_ptr(), self.case_table.data_ptr(), self.case_ids.data_ptr(),
+                idx.data_ptr(), b, p, _lib.ACT_BF16 if self.frame_dtype == torch.bfloat16 else _lib.ACT_F32,
+                out["inputs"].data_ptr(), out["label"].data_ptr(), out["mask"].data_ptr(), out["case_params"].data_ptr(),
+                int(steps), int(s), self.n, out["labels"].data_ptr())
+        with torch.cuda.device(dev):
+            st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+            if (gh, gw) == (64, 64):
+                _lib.check(lib.fno_gather_window(*args, st), "fno_gather_window")
+            else:
+                _lib.check(lib.fno_grid_gather_window(*args, gh, gw, st), "fno_grid_gather_window")
+        idx.record_stream(torch.cuda.current_stream(dev))
+        return out
+
     def batches(self, index_batches: Iterable[Sequence[int]]) -> Iterator[Dict[str, Tensor]]:
         for ib in index_batches:
             yield self.batch(ib)
@@ -110,3 +161,20 @@ def index_batches(n: int, batch_size: int, shuffle: bool = False, generator=None
         torch.empty((), dtype=torch.int64).random_(generator=generator)
         yield from BatchSampler(sampler, batch_size, drop_last)
     return gen()
+
+
+def rollout_windows(case_ids, steps: int, time_step_size: int) -> np.ndarray:
+    """The valid starts (int64, ascending) of `steps`-step windows over a split whose samples are laid out as the
+    reference's datasets lay them out: a case's samples are contiguous, with inputs = frames[:-s] and labels = frames[s:]
+    (s = time_step_size, src/dataset/cavity.py:271,295-331), so the k-th target of the window that starts at sample j is
+    labels[j + k s].  A start j is valid when j + (steps - 1) s < N and case_ids[j + (steps - 1) s] == case_ids[j]: no
+    window crosses a case.  steps = 1 gives arange(N)."""
+    for name, v in (("steps", steps), ("time_step_size", time_step_size)):
+        if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or v < 1:
+            raise ValueError(f"{name} must be a positive int, got {v!r}")
+    cid = np.asarray(case_ids).reshape(-1)
+    span = (int(steps) - 1) * int(time_step_size)
+    if cid.size <= span:
+        return np.zeros(0, dtype=np.int64)
+    j = np.arange(cid.size - span, dtype=np.int64)
+    return j[cid[j + span] == cid[j]]

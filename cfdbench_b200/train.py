@@ -13,6 +13,7 @@ synchronisation.  The result is bit-identical to the eager loop `DeviceFrames.lo
 
     from cfdbench_b200 import train_auto
     train_auto(model, train_data, dev_data, output_dir, num_epochs=..., lr=..., batch_size=...)   # for train(...)
+    train_auto(..., rollout_steps=4)   # trained through 4-step rollouts of the model's own predictions
 """
 from __future__ import annotations
 
@@ -28,7 +29,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .data import DeviceFrames, case_table, index_batches
+from .data import DeviceFrames, case_table, index_batches, rollout_windows
 
 LOG_COLUMNS = ("mse", "rmse", "mae", "nmse", "mean_l2")   # one row of the epoch log: fno_loss_fwd's five scalars
 
@@ -76,11 +77,12 @@ class _StepGraphs:
     place; the packed weight images are rebuilt inside the graph from the parameters as the previous replay's Adam
     left them."""
 
-    def __init__(self, model, frames: DeviceFrames, batch_size: int, optimizer):
+    def __init__(self, model, frames: DeviceFrames, batch_size: int, optimizer, n: Optional[int] = None):
+        """n: the length of an epoch's permutation (default: every sample)."""
         lib = self.lib = _lib.load()
         self.model, self.frames, self.optimizer = model, frames, optimizer
         dev = self.dev = model.device
-        n, gh, gw = frames.n, frames.height, frames.width
+        n, gh, gw = frames.n if n is None else n, frames.height, frames.width
         self.n, self.gh, self.gw, self.stride = n, gh, gw, batch_size
         self.grid = grid = model._on_grid_path(gh, gw)
         bmax = min(batch_size, n)
@@ -97,19 +99,7 @@ class _StepGraphs:
         self.ts = model._train_state(bmax, gh, gw, grid)
         self.flat, _, self.grads = model._grad_buffers()
 
-        f32 = dict(dtype=torch.float32, device=dev)
-        self.io = io = dict(
-            perm=torch.zeros(n, dtype=torch.int64, device=dev),
-            idx=torch.zeros(bmax, dtype=torch.int64, device=dev),
-            inputs=torch.empty(bmax, 2, gh, gw, **f32), label=torch.empty(bmax, 2, gh, gw, **f32),
-            mask=torch.empty(bmax, 1, gh, gw, **f32), cp=torch.empty(bmax, p, **f32),
-            labm=torch.empty(bmax, 2, gh, gw, **f32), preds=torch.empty(bmax, 2, gh, gw, **f32),
-            dpreds=torch.empty(bmax, 2, gh, gw, **f32), loss=torch.empty(5, **f32),
-            scratch=torch.zeros(lib.fno_loss_scratch_bytes(), dtype=torch.uint8, device=dev),
-            gout=torch.zeros(4, **f32),   # d/d(mse, rmse, mae, nmse) of loss["nmse"]: (0, 0, 0, 1)
-            cursor=torch.zeros(1, dtype=torch.int32, device=dev),
-            coef=torch.empty(self.steps, 2, **f32), log=torch.empty(self.steps, len(LOG_COLUMNS), **f32))
-        io["gout"][3:].fill_(1.0)   # a fill kernel: assigning a Python number to a CUDA element is a blocking copy
+        self.io = self._make_io(bmax, gh, gw, p)
         self.perm_host = torch.empty(n, dtype=torch.int64, pin_memory=True)
         self.coef_host = torch.empty(self.steps, 2, dtype=torch.float32, pin_memory=True)
 
@@ -154,14 +144,31 @@ class _StepGraphs:
                 self.graphs.append(g)
         cur.wait_stream(side)
 
+    def _make_io(self, bmax: int, gh: int, gw: int, p: int) -> dict:
+        """The static buffers of the step graphs."""
+        lib, dev, n = self.lib, self.dev, self.n
+        f32 = dict(dtype=torch.float32, device=dev)
+        io = dict(
+            perm=torch.zeros(n, dtype=torch.int64, device=dev),
+            idx=torch.zeros(bmax, dtype=torch.int64, device=dev),
+            inputs=torch.empty(bmax, 2, gh, gw, **f32), label=torch.empty(bmax, 2, gh, gw, **f32),
+            mask=torch.empty(bmax, 1, gh, gw, **f32), cp=torch.empty(bmax, p, **f32),
+            labm=torch.empty(bmax, 2, gh, gw, **f32), preds=torch.empty(bmax, 2, gh, gw, **f32),
+            dpreds=torch.empty(bmax, 2, gh, gw, **f32), loss=torch.empty(5, **f32),
+            scratch=torch.zeros(lib.fno_loss_scratch_bytes(), dtype=torch.uint8, device=dev),
+            gout=torch.zeros(4, **f32),   # d/d(mse, rmse, mae, nmse) of loss["nmse"]: (0, 0, 0, 1)
+            cursor=torch.zeros(1, dtype=torch.int32, device=dev),
+            coef=torch.empty(self.steps, 2, **f32), log=torch.empty(self.steps, len(LOG_COLUMNS), **f32))
+        io["gout"][3:].fill_(1.0)   # a fill kernel: assigning a Python number to a CUDA element is a blocking copy
+        return io
+
     def _issue(self, b: int, update: bool) -> None:
         """One training step of batch b on the static buffers, on the current stream."""
         lib, model, io, sw = self.lib, self.model, self.io, self.sw
         gh, gw, grid, p = self.gh, self.gw, self.grid, self.frames.n_case_params
         st = C.c_void_p(torch.cuda.current_stream(self.dev).cuda_stream)
         fr = self.frames
-        _lib.check(lib.fno_train_stage_indices(io["perm"].data_ptr(), self.n, self.stride, b, io["cursor"].data_ptr(),
-                                               io["idx"].data_ptr(), st), "fno_train_stage_indices")
+        self._stage_indices(b, st)
         args = (fr.frames_in.data_ptr(), fr.frames_out.data_ptr(), fr.case_table.data_ptr(), fr.case_ids.data_ptr(),
                 io["idx"].data_ptr(), b, p, _lib.ACT_BF16 if fr.frame_dtype == torch.bfloat16 else _lib.ACT_F32,
                 io["inputs"].data_ptr(), io["label"].data_ptr(), io["mask"].data_ptr(), io["cp"].data_ptr())
@@ -169,15 +176,7 @@ class _StepGraphs:
             _lib.check(lib.fno_gather_batch(*args, st), "fno_gather_batch")
         else:
             _lib.check(lib.fno_grid_gather_batch(*args, gh, gw, st), "fno_grid_gather_batch")
-        # the packed weights, from the parameters as the previous step's Adam left them (Fno2d._pack's images)
-        L = model.num_layers
-        wk, w0t, wkT = sw["dst"][:L], sw["dst"][L:2 * L], sw["dst"][2 * L:3 * L]
-        for l, blk in enumerate(model.blocks):
-            for dst, conj in ((wk[l], 0), (wkT[l], 1)):
-                _lib.check(lib.fno_pack_mix_operand_from_weights(blk.conv0.weights1.data_ptr(),
-                                                                 blk.conv0.weights2.data_ptr(), dst.data_ptr(), conj, st),
-                           "fno_pack_mix_operand_from_weights")
-            w0t[l].copy_(blk.w0.weight.view(w0t[l].shape).t())
+        self._repack(st)
         inputs, mask, cp = io["inputs"][:b], io["mask"][:b], io["cp"][:b]
         preds, labm, dpreds = io["preds"][:b], io["labm"][:b], io["dpreds"][:b]
         torch.mul(io["label"][:b], mask, out=labm)   # Fno2d.forward's label * mask
@@ -204,14 +203,35 @@ class _StepGraphs:
             _lib.check(lib.fno_backward(C.byref(sw["struct"]), C.byref(sw["struct_bwd"]), inputs.data_ptr(), mask.data_ptr(),
                                         cp.data_ptr(), dpreds.data_ptr(), C.byref(ts["sv"]), C.byref(self.grads),
                                         C.byref(ts["sc"]), C.byref(ws), b, model._act_code(), st), "fno_backward")
-        if not update:
-            return
+        if update:
+            self._adam_and_log(io["loss"].data_ptr(), st)
+
+    def _stage_indices(self, b: int, st) -> None:
+        io = self.io
+        _lib.check(self.lib.fno_train_stage_indices(io["perm"].data_ptr(), self.n, self.stride, b, io["cursor"].data_ptr(),
+                                                    io["idx"].data_ptr(), st), "fno_train_stage_indices")
+
+    def _repack(self, st) -> None:
+        """The packed weights, from the parameters as the previous step's Adam left them (Fno2d._pack's images)."""
+        lib, model, sw = self.lib, self.model, self.sw
+        L = model.num_layers
+        wk, w0t, wkT = sw["dst"][:L], sw["dst"][L:2 * L], sw["dst"][2 * L:3 * L]
+        for l, blk in enumerate(model.blocks):
+            for dst, conj in ((wk[l], 0), (wkT[l], 1)):
+                _lib.check(lib.fno_pack_mix_operand_from_weights(blk.conv0.weights1.data_ptr(),
+                                                                 blk.conv0.weights2.data_ptr(), dst.data_ptr(), conj, st),
+                           "fno_pack_mix_operand_from_weights")
+            w0t[l].copy_(blk.w0.weight.view(w0t[l].shape).t())
+
+    def _adam_and_log(self, loss_row: int, st) -> None:
+        """Adam on the flat gradients, then the step's five loss scalars (at device address loss_row) into the log."""
+        lib, io = self.lib, self.io
         b1, b2 = self.betas
         for t in self.adam:
             _lib.check(lib.fno_adam_step_dev(C.byref(t), io["coef"].data_ptr(), self.steps, io["cursor"].data_ptr(), b1, b2,
                                              self.eps, self.weight_decay, st), "fno_adam_step_dev")
-        _lib.check(lib.fno_train_log_step(io["loss"].data_ptr(), io["log"].data_ptr(), self.steps, io["cursor"].data_ptr(),
-                                          st), "fno_train_log_step")
+        _lib.check(lib.fno_train_log_step(loss_row, io["log"].data_ptr(), self.steps, io["cursor"].data_ptr(), st),
+                   "fno_train_log_step")
 
     def epoch(self, perm: np.ndarray, lr: float, first_step: int) -> np.ndarray:
         """Train one epoch visiting the samples in `perm` at learning rate `lr`, Adam's 1-based step count starting at
@@ -235,6 +255,102 @@ class _StepGraphs:
         for prm in self.params:
             torch.autograd.graph.increment_version(prm)
         return log
+
+
+class _RolloutStepGraphs(_StepGraphs):
+    """The captured step of training through `k`-step rollouts (train_auto with rollout_steps = k > 1): the epoch's
+    permutation holds window starts, and a step is stage indices -> gather window (inputs, mask and case parameters of
+    the start sample, the k masked targets) -> weight repack -> rollout training forward into one reused saved set ->
+    K-step loss forward and backward -> rollout backward (one recomputing sweep, no input gradients) into the flat
+    gradient buffer -> Adam -> log of the aggregate loss row.  Same graphs, buffers-per-batch layout and epoch as
+    _StepGraphs; the per-step buffers are [k][b] blocks of the first k*b samples' worth of (k, bmax, ...) buffers."""
+
+    def __init__(self, model, frames: DeviceFrames, batch_size: int, optimizer, n_windows: int, steps: int,
+                 time_step_size: int):
+        self.k, self.tss = steps, time_step_size
+        super().__init__(model, frames, batch_size, optimizer, n=n_windows)
+
+    def _make_io(self, bmax: int, gh: int, gw: int, p: int) -> dict:
+        lib, dev, n, k = self.lib, self.dev, self.n, self.k
+        f32 = dict(dtype=torch.float32, device=dev)
+        io = dict(
+            perm=torch.zeros(n, dtype=torch.int64, device=dev),
+            idx=torch.zeros(bmax, dtype=torch.int64, device=dev),
+            inputs=torch.empty(bmax, 2, gh, gw, **f32), mask=torch.empty(bmax, 1, gh, gw, **f32),
+            cp=torch.empty(bmax, p, **f32), labels=torch.empty(k, bmax, 2, gh, gw, **f32),
+            preds=torch.empty(k, bmax, 2, gh, gw, **f32), dpreds=torch.empty(k, bmax, 2, gh, gw, **f32),
+            carry=torch.empty(bmax, 2, gh, gw, **f32), loss=torch.empty(k + 1, 5, **f32),
+            scratch=torch.zeros(lib.fno_loss_seq_scratch_bytes(k), dtype=torch.uint8, device=dev),
+            gout=torch.zeros(4, **f32),   # d/d(mse, rmse, mae, nmse) of the aggregate's nmse: (0, 0, 0, 1)
+            cursor=torch.zeros(1, dtype=torch.int32, device=dev),
+            coef=torch.empty(self.steps, 2, **f32), log=torch.empty(self.steps, len(LOG_COLUMNS), **f32))
+        io["gout"][3:].fill_(1.0)
+        return io
+
+    def _issue(self, b: int, update: bool) -> None:
+        lib, model, io, sw, fr = self.lib, self.model, self.io, self.sw, self.frames
+        gh, gw, grid, p, k = self.gh, self.gw, self.grid, fr.n_case_params, self.k
+        st = C.c_void_p(torch.cuda.current_stream(self.dev).cuda_stream)
+        self._stage_indices(b, st)
+        args = (fr.frames_in.data_ptr(), fr.frames_out.data_ptr(), fr.case_table.data_ptr(), fr.case_ids.data_ptr(),
+                io["idx"].data_ptr(), b, p, _lib.ACT_BF16 if fr.frame_dtype == torch.bfloat16 else _lib.ACT_F32,
+                io["inputs"].data_ptr(), None, io["mask"].data_ptr(), io["cp"].data_ptr(), k, self.tss, fr.n,
+                io["labels"].data_ptr())
+        if (gh, gw) == (64, 64):
+            _lib.check(lib.fno_gather_window(*args, st), "fno_gather_window")
+        else:
+            _lib.check(lib.fno_grid_gather_window(*args, gh, gw, st), "fno_grid_gather_window")
+        self._repack(st)
+        x, mk, cp = io["inputs"].data_ptr(), io["mask"].data_ptr(), io["cp"].data_ptr()
+        preds, labels, dpreds = io["preds"].data_ptr(), io["labels"].data_ptr(), io["dpreds"].data_ptr()
+        ts, ws = self.ts, self.ws
+        if grid:
+            _lib.check(lib.fno_grid_rollout_forward_train(C.byref(sw["struct"]), x, mk, cp, preds, k, C.byref(ts["sv"]),
+                                                          C.byref(ws), b, gh, gw, st), "fno_grid_rollout_forward_train")
+        else:
+            _lib.check(lib.fno_rollout_forward_train(C.byref(sw["struct"]), x, mk, cp, preds, k, C.byref(ts["sv"]),
+                                                     C.byref(ws), b, model._act_code(), st), "fno_rollout_forward_train")
+        n_el = b * 2 * gh * gw   # per step
+        _lib.check(lib.fno_loss_seq_fwd(preds, labels, n_el, k, io["scratch"].data_ptr(), io["loss"].data_ptr(), st),
+                   "fno_loss_seq_fwd")
+        _lib.check(lib.fno_loss_seq_bwd(preds, labels, io["loss"].data_ptr(), io["gout"].data_ptr(), dpreds, n_el, k, st),
+                   "fno_loss_seq_bwd")
+        carry = io["carry"].data_ptr()
+        if grid:
+            _lib.check(lib.fno_grid_rollout_backward(C.byref(sw["struct"]), C.byref(sw["struct_bwd"]), x, mk, cp, preds,
+                                                     dpreds, k, C.byref(ts["sv"]), C.byref(self.grads), C.byref(ts["sc"]),
+                                                     C.byref(ws), carry, None, None, b, gh, gw, st),
+                       "fno_grid_rollout_backward")
+        else:
+            _lib.check(lib.fno_rollout_backward(C.byref(sw["struct"]), C.byref(sw["struct_bwd"]), x, mk, cp, preds, dpreds,
+                                                k, C.byref(ts["sv"]), C.byref(self.grads), C.byref(ts["sc"]), C.byref(ws),
+                                                carry, None, None, b, model._act_code(), st), "fno_rollout_backward")
+        if update:
+            self._adam_and_log(io["loss"][k].data_ptr(), st)
+
+
+def _check_chain(frames: DeviceFrames, starts: np.ndarray, steps: int, time_step_size: int) -> None:
+    """Refuse a split whose frames do not chain where the windows starting at `starts` need them to: step k of the
+    window at j is fed the prediction of step k-1 where the data has frames_in[j + k s], and trained against
+    frames_out[j + (k-1) s], so the two must be the same frame (bit for bit, mask channel included).  Compared on the
+    device in chunks; one synchronisation for the whole check.  The error names the first bad sample."""
+    s, dev, n = time_step_size, frames.device, frames.n
+    rows = np.unique((starts[:, None] + s * np.arange(steps - 1, dtype=np.int64)[None, :]).ravel())
+    host = torch.from_numpy(rows).pin_memory()
+    rows_dev = host.to(dev, non_blocking=True)
+    bits = torch.int32 if frames.frame_dtype == torch.float32 else torch.int16
+    first = torch.full((), n, dtype=torch.int64, device=dev)
+    chunk = 512
+    for c0 in range(0, rows.size, chunk):
+        i = rows_dev[c0:c0 + chunk]
+        a = frames.frames_in.index_select(0, i + s).view(bits)
+        b = frames.frames_out.index_select(0, i).view(bits)
+        bad = (a != b).flatten(1).any(1)
+        first = torch.minimum(first, torch.where(bad, i, first).min())
+    bad_row = int(first)   # the check's one synchronisation
+    if bad_row < n:
+        raise ValueError(f"train_data does not chain with time_step_size={s}: sample {bad_row + s}'s input frame is not "
+                         f"sample {bad_row}'s label frame, which a {steps}-step rollout window feeds it")
 
 
 # ------------------------------------------------------------------------------------------------ train_auto
@@ -274,7 +390,8 @@ def _check_split(model, data, what: str) -> None:
 
 def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, lr: float = 1e-3, lr_step_size: int = 1,
                lr_gamma: float = 0.9, batch_size: int = 2, eval_batch_size: int = 2, log_interval: int = 10,
-               eval_interval: int = 2, generator: Optional[torch.Generator] = None) -> dict:
+               eval_interval: int = 2, generator: Optional[torch.Generator] = None, rollout_steps: int = 1,
+               time_step_size: Optional[int] = None) -> dict:
     """What the reference's `train(model, train_data, dev_data, output_dir, ...)` does (src/train_auto.py:181-313), with
     its argument names and defaults, every training step replayed from a CUDA graph and one synchronisation per epoch.
 
@@ -295,13 +412,24 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
     - Logging: the reference's line every `log_interval` steps, printed at the end of the epoch from the device log, so
       its `time` field is the time of printing, not of the step.
     - Not reproduced: example.png, train_losses.png and the evaluation images; `measure_time`.
+    - rollout_steps = K > 1 trains through K-step rollouts (`Fno2d.rollout`): each step of an epoch takes a batch of
+      window starts j and trains on (nmse_0 + ... + nmse_{K-1}) / K, nmse_k = MseLoss(step k's prediction,
+      labels[j + k s] * mask_j)["nmse"], s = time_step_size (default: train_data.time_step_size), every step masked with
+      the start sample's mask.  The windows are `rollout_windows(case_ids, K, s)`, which never cross a case; each epoch
+      visits a permutation of them that draws from the RNG what a DataLoader over that many samples draws.  The log and
+      train_losses hold the aggregate (each column the mean over the K steps).  The split must chain
+      (frames_in[j + k s] == frames_out[j + (k-1) s] for every pair a window uses): that is checked once on the device
+      before training.  The dev evaluation, and with it checkpoint selection, stays single-step.  rollout_steps = 1 is
+      the single-step loop above, launch for launch.
 
     Returns dict(train_losses=[per-step nmse, every epoch], optimizer=the FusedAdam).  Its state holds the true step
     count (its state_dict loads into torch.optim.Adam), and the parameters' version counters are bumped, so the
     model's packed weights and inference graphs are rebuilt on the next call.  Raises before any device work on: a
     model that is not the drop-in Fno2d, a CPU model (FnoNativeError), a loss without "nmse", non-positive sizes,
     intervals or epoch count, a model whose parameters are all frozen, an empty or malformed split, a split whose
-    case-parameter count differs from the model's, data parallel enabled, or a grid / storage mode the model rejects.
+    case-parameter count differs from the model's, data parallel enabled, or a grid / storage mode the model rejects;
+    and, as ValueError before any training step, a non-positive rollout_steps or time_step_size, rollout_steps > 1 with
+    no time_step_size, a split without a single K-step window, or a split whose frames do not chain.
     Frozen parameters (requires_grad=False) are not updated, as FusedAdam.step skips them.  Data parallel training in
     this loop is not supported."""
     from .metrics import evaluate_auto
@@ -313,7 +441,8 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
     if "nmse" not in names:
         raise ValueError(f"the model's loss has scores {names}: train_auto backpropagates loss['nmse'], as the reference")
     for name, v in (("num_epochs", num_epochs), ("lr_step_size", lr_step_size), ("batch_size", batch_size),
-                    ("eval_batch_size", eval_batch_size), ("log_interval", log_interval), ("eval_interval", eval_interval)):
+                    ("eval_batch_size", eval_batch_size), ("log_interval", log_interval), ("eval_interval", eval_interval),
+                    ("rollout_steps", rollout_steps)):
         _positive_int(name, v)
     if model._dp_enabled:
         raise ValueError("train_auto does not run data parallel: its step graph has no all-reduce")
@@ -322,6 +451,18 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
     dev = model.device
     for what, data in (("train_data", train_data), ("dev_data", dev_data)):
         _check_split(model, data, what)
+    windows = None   # rollout_steps > 1: the window starts of the train split
+    if rollout_steps > 1:
+        tss = getattr(train_data, "time_step_size", None) if time_step_size is None else time_step_size
+        if tss is None:
+            raise ValueError(f"rollout_steps={rollout_steps} needs a time_step_size: train_data has none, pass it")
+        _positive_int("time_step_size", tss)
+        case_ids = train_data._case_ids_host if isinstance(train_data, DeviceFrames) else train_data.case_ids
+        windows = rollout_windows(case_ids, rollout_steps, int(tss))
+        if windows.size == 0:
+            raise ValueError(f"train_data has no {rollout_steps}-step window with time_step_size={tss} inside one case")
+    elif time_step_size is not None:
+        _positive_int("time_step_size", time_step_size)
     model._require_cuda()
     output_dir = Path(output_dir)
     output_dir.mkdir(exist_ok=True, parents=True)
@@ -332,10 +473,16 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
         frames = train_data if isinstance(train_data, DeviceFrames) else DeviceFrames(train_data, device=dev)
         dev_frames = None
         n = frames.n
-        graphs = _StepGraphs(model, frames, batch_size, optimizer)
+        if windows is None:
+            graphs = _StepGraphs(model, frames, batch_size, optimizer)
+        else:
+            _check_chain(frames, windows, rollout_steps, int(tss))
+            graphs = _RolloutStepGraphs(model, frames, batch_size, optimizer, windows.size, rollout_steps, int(tss))
         print("====== Training ======")
         print(f"# batch: {batch_size}")
         print(f"# examples: {n}")
+        if windows is not None:
+            print(f"# rollout steps: {rollout_steps}, windows: {windows.size}")
         print(f"# step: {graphs.steps}")
         print(f"# epoch: {num_epochs}")
         start_time = time.time()
@@ -345,7 +492,11 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
             for ep in range(num_epochs):
                 ep_start_time = time.time()
                 lr_ep = optimizer.param_groups[0]["lr"]
-                log = graphs.epoch(epoch_permutation(n, batch_size, generator), lr_ep, global_step + 1)
+                if windows is None:
+                    perm = epoch_permutation(n, batch_size, generator)
+                else:
+                    perm = windows[epoch_permutation(windows.size, batch_size, generator)]
+                log = graphs.epoch(perm, lr_ep, global_step + 1)
                 ep_train_losses = [float(v) for v in log[:, 3]]
                 for step in range(graphs.steps):
                     global_step += 1

@@ -302,6 +302,31 @@ int fno_adam_coefficients(float lr, float beta1, float beta2, int64_t first_step
  * outside 0..n_log-1. */
 int fno_train_log_step(const float* loss_out, float* log, int n_log, int32_t* cursor, void* stream);
 
+/* ---- training through K-step rollouts (cfdbench_b200.train_auto with rollout_steps = K) --------------------------
+ * A dataset holds a case's samples contiguously with inputs = frames[:-s], labels = frames[s:] (s = time_step_size), so
+ * the k-th target of the window that starts at sample j is labels[j + k s].  Every entry point checks its arguments before
+ * any device work (status 1; a grid outside 24..128 returns 3); steps <= 32765. */
+/* fno_gather_batch for the window starts idx, plus labels_seq [steps][n][2][64][64] float32:
+ * labels_seq[k][b] = frames_out[idx[b] + k s][0:2] * frames_in[idx[b]][2] (one float32 multiply: label * mask).  inputs,
+ * label, mask and case_params are fno_gather_batch's, bit for bit; label may be NULL (not written).  A window with
+ * idx[b] + (steps - 1) s >= n_frames (the split's sample count) is not read and none of sample b's outputs are written. */
+int fno_gather_window(const void* frames_in, const void* frames_out, const float* case_table, const int32_t* case_ids,
+                      const int64_t* idx, int n_idx, int n_case_params, int frame_dtype, float* inputs, float* label,
+                      float* mask, float* case_params, int steps, int time_step_size, int64_t n_frames, float* labels_seq,
+                      void* stream);
+/* MseLoss of each step of a rollout and their mean, one launch: preds_seq / labels_seq [steps][n] float32 (n elements per
+ * step, no alignment requirement).  out[k][0..4] = fno_loss_fwd's five scalars of step k, bit for bit (the same
+ * reduction order); out[steps][c] = (out[0][c] + ... + out[steps-1][c]) * (1/steps), a left-to-right float32 sum times
+ * the float32 reciprocal of steps, as `sum(...) / steps` computes it on 0-dim CUDA tensors.  scratch:
+ * fno_loss_seq_scratch_bytes(steps) bytes, zero-initialised once by the caller (the kernel leaves it zeroed). */
+size_t fno_loss_seq_scratch_bytes(int steps);
+int fno_loss_seq_fwd(const float* preds_seq, const float* labels_seq, size_t n, int steps, void* scratch, float* out,
+                     void* stream);
+/* dpreds_seq[k] = fno_loss_bwd(preds_k, labels_k, fwd[k], gout * (1/steps)), bit for bit: gout = the upstream gradients
+ * of the aggregate row's (mse, rmse, mae, nmse); fwd = the out[] of the matching fno_loss_seq_fwd call. */
+int fno_loss_seq_bwd(const float* preds_seq, const float* labels_seq, const float* fwd, const float* gout, float* dpreds_seq,
+                     size_t n, int steps, void* stream);
+
 /* ---------------------------------------------------------------------------------------------------
  * Grid-generic path: the same network on H x W frames with 24 <= H <= 128 and 24 <= W <= 128, e.g. CFDBench's
  * tube and dam problems (66 x 65, reference src/utils/autoregressive.py:24-26).  fp32 activation storage only (there is
@@ -369,6 +394,11 @@ int fno_grid_multistep_metrics(const float* preds_seq, const float* label_u, con
 int fno_grid_gather_batch(const void* frames_in, const void* frames_out, const float* case_table, const int32_t* case_ids,
                           const int64_t* idx, int n_idx, int n_case_params, int frame_dtype, float* inputs, float* label,
                           float* mask, float* case_params, int h, int w_, void* stream);
+/* fno_gather_window on an H x W grid (frames_in / frames_out [N][3][H][W], labels_seq [steps][n][2][H][W]) */
+int fno_grid_gather_window(const void* frames_in, const void* frames_out, const float* case_table, const int32_t* case_ids,
+                           const int64_t* idx, int n_idx, int n_case_params, int frame_dtype, float* inputs, float* label,
+                           float* mask, float* case_params, int steps, int time_step_size, int64_t n_frames,
+                           float* labels_seq, int h, int w_, void* stream);
 
 /* Single-step evaluation (reference src/train_auto.py:61-148, `evaluate`, which synchronises 2 x (number of scores)
  * times per batch): the per-sample sums its scores are made of, for any grid 24 <= H, W <= 128 (64 x 64 included).
