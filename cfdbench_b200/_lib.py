@@ -168,6 +168,8 @@ SIGNATURES = {
     "fno_loss_seq_scratch_bytes": (C.c_size_t, [_I]),
     "fno_loss_seq_fwd": (C.c_int, [_P, _P, C.c_size_t, _I, _P, _P, _P]),
     "fno_loss_seq_bwd": (C.c_int, [_P, _P, _P, _P, _P, C.c_size_t, _I, _P]),
+    # training noise
+    "fno_add_input_noise": (C.c_int, [_P, _P, _P, _I, _I, _I, _F, C.c_uint64, _P, _P, _P]),
 }
 
 GRID_MIN, GRID_MAX = 24, 128

@@ -86,6 +86,8 @@ cudaError_t launch_grid_gather_window(const void*, const void*, const float*, co
 cudaError_t launch_loss_seq_fwd(const float*, const float*, size_t, int, float*, float*, cudaStream_t);
 cudaError_t launch_loss_seq_bwd(const float*, const float*, const float*, const float*, float*, size_t, int, cudaStream_t);
 size_t loss_seq_scratch_bytes(int);
+cudaError_t launch_add_input_noise(float*, const float*, const long long*, int, int, int, float, unsigned long long,
+                                   const long long*, const int*, cudaStream_t);
 }  // namespace fno
 
 using namespace fno;
@@ -995,6 +997,18 @@ int fno_grid_gather_window(const void* frames_in, const void* frames_out, const 
                                      frame_dtype == FNO_ACT_BF16, inputs, label, mask, case_params, steps, time_step_size,
                                      n_frames, labels_seq, h, wd, S(stream)),
            "gather_window_kernel");
+  return kOk;
+}
+
+int fno_add_input_noise(float* inputs, const float* mask, const int64_t* idx, int n, int h, int wd, float std,
+                        uint64_t seed, const int64_t* step_base, const int32_t* step_offset, void* stream) {
+  FNO_TRY(grid_arg("fno_add_input_noise", h, wd));
+  if (!inputs || !mask || !idx || !step_base || n <= 0 || !(std >= 0.f) || !isfinite(std))
+    return fail(kErrArg, "fno_add_input_noise: bad argument");
+  FNO_CUDA(launch_add_input_noise(inputs, mask, reinterpret_cast<const long long*>(idx), n, h, wd, std, seed,
+                                  reinterpret_cast<const long long*>(step_base), reinterpret_cast<const int*>(step_offset),
+                                  S(stream)),
+           "add_input_noise_kernel");
   return kOk;
 }
 

@@ -376,4 +376,96 @@ cudaError_t launch_log_step(const float* loss_out, float* log, int n_log, int* c
   return cudaGetLastError();
 }
 
+// ------------------------------------------------------------------------------------------------ input noise
+// inputs[b][e] += (std * z) * mask[b][e mod HW] where mask != 0, e over the flattened (2, H, W) frame of sample b.  The
+// normal z of element e = 4q + r is component r of Box-Muller on Philox4x32-10(counter = (q, j, step_lo, step_hi),
+// key = (seed_lo, seed_hi)), j = idx[b]: a pure function of (seed, step, j, e), whatever the batch slot, the launch or the
+// replay.  step = *step_base (+ *step_offset), read on the device so that a captured launch sees each replay's step.
+// One thread per quad; the 64x64 path moves a quad as one float4 (it never straddles the two channels).
+constexpr int kNoiseThreads = 256;
+
+__device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint2 k) {
+#pragma unroll
+  for (int r = 0; r < 10; ++r) {
+    if (r > 0) {
+      k.x += 0x9E3779B9u;
+      k.y += 0xBB67AE85u;
+    }
+    const unsigned lo0 = 0xD2511F53u * c.x, hi0 = __umulhi(0xD2511F53u, c.x);
+    const unsigned lo1 = 0xCD9E8D57u * c.z, hi1 = __umulhi(0xCD9E8D57u, c.z);
+    c = make_uint4(hi1 ^ c.y ^ k.x, lo1, hi0 ^ c.w ^ k.y, lo0);
+  }
+  return c;
+}
+
+// curand's uniform in (0, 1]: x 2^-32 + 2^-33 in float32
+__device__ __forceinline__ float noise_uniform(unsigned x) {
+  return __fadd_rn(__fmul_rn(__uint2float_rn(x), 2.3283064365386963e-10f), 1.1641532182693481e-10f);
+}
+
+__device__ __forceinline__ float4 noise_normals(unsigned long long seed, unsigned long long step, unsigned j, unsigned q) {
+  const uint4 x = philox4x32_10(make_uint4(q, j, static_cast<unsigned>(step), static_cast<unsigned>(step >> 32)),
+                                make_uint2(static_cast<unsigned>(seed), static_cast<unsigned>(seed >> 32)));
+  const float r0 = sqrtf(-2.f * logf(noise_uniform(x.x))), t0 = 2.f * noise_uniform(x.y);
+  const float r1 = sqrtf(-2.f * logf(noise_uniform(x.z))), t1 = 2.f * noise_uniform(x.w);
+  return make_float4(r0 * cospif(t0), r0 * sinpif(t0), r1 * cospif(t1), r1 * sinpif(t1));
+}
+
+template <bool kVec>
+__global__ void __launch_bounds__(kNoiseThreads)
+    add_input_noise_kernel(float* __restrict__ inputs, const float* __restrict__ mask, const long long* __restrict__ idx,
+                           int hw, float std, unsigned long long seed, const long long* __restrict__ step_base,
+                           const int* __restrict__ step_offset) {
+  const int b = blockIdx.y;
+  const int n_el = 2 * hw;
+  const unsigned q = blockIdx.x * kNoiseThreads + threadIdx.x;
+  if (4 * q >= static_cast<unsigned>(n_el)) return;
+  const unsigned long long step =
+      static_cast<unsigned long long>(*step_base) + (step_offset ? static_cast<long long>(*step_offset) : 0ll);
+  const float4 z = noise_normals(seed, step, static_cast<unsigned>(idx[b]), q);
+  const float zs[4] = {z.x, z.y, z.z, z.w};
+  float* x = inputs + static_cast<size_t>(b) * n_el;
+  const float* m = mask + static_cast<size_t>(b) * hw;
+  if constexpr (kVec) {   // hw % 4 == 0 and 16-byte aligned slices: the quad lies in one channel
+    const int e = 4 * q, cell = e < hw ? e : e - hw;
+    const float4 mv = __ldg(reinterpret_cast<const float4*>(m + cell));
+    float4 xv = *reinterpret_cast<const float4*>(x + e);
+    const float ms[4] = {mv.x, mv.y, mv.z, mv.w};
+    float xs[4] = {xv.x, xv.y, xv.z, xv.w};
+#pragma unroll
+    for (int r = 0; r < 4; ++r) xs[r] = fmaf(std * zs[r], ms[r], xs[r]);
+    if (ms[0] != 0.f && ms[1] != 0.f && ms[2] != 0.f && ms[3] != 0.f) {
+      *reinterpret_cast<float4*>(x + e) = make_float4(xs[0], xs[1], xs[2], xs[3]);
+    } else {
+#pragma unroll
+      for (int r = 0; r < 4; ++r)
+        if (ms[r] != 0.f) x[e + r] = xs[r];
+    }
+  } else {
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+      const int e = 4 * q + r;
+      if (e < n_el) {
+        const float mv = __ldg(m + (e < hw ? e : e - hw));
+        if (mv != 0.f) x[e] = fmaf(std * zs[r], mv, x[e]);
+      }
+    }
+  }
+}
+
+cudaError_t launch_add_input_noise(float* inputs, const float* mask, const long long* idx, int n, int h, int w, float std,
+                                   unsigned long long seed, const long long* step_base, const int* step_offset,
+                                   cudaStream_t stream) {
+  const int hw = h * w, quads = (2 * hw + 3) / 4;
+  const dim3 grid((quads + kNoiseThreads - 1) / kNoiseThreads, n);
+  const bool vec = hw % 4 == 0 && ((reinterpret_cast<uintptr_t>(inputs) | reinterpret_cast<uintptr_t>(mask)) & 15) == 0;
+  if (vec)
+    add_input_noise_kernel<true><<<grid, kNoiseThreads, 0, stream>>>(inputs, mask, idx, hw, std, seed, step_base,
+                                                                      step_offset);
+  else
+    add_input_noise_kernel<false><<<grid, kNoiseThreads, 0, stream>>>(inputs, mask, idx, hw, std, seed, step_base,
+                                                                       step_offset);
+  return cudaGetLastError();
+}
+
 }  // namespace fno

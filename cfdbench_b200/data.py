@@ -62,9 +62,17 @@ class DeviceFrames:
     def __len__(self) -> int:
         return self.n
 
-    def batch(self, idx) -> Dict[str, Tensor]:
-        """The dict collate_fn returns for samples `idx` (reference src/train_auto.py:53-58), all on the device."""
+    def batch(self, idx, noise_std: float = 0.0, noise_seed: int = 0, noise_step: int = 0) -> Dict[str, Tensor]:
+        """The dict collate_fn returns for samples `idx` (reference src/train_auto.py:53-58), all on the device.
+
+        noise_std > 0 then adds seeded Gaussian noise to the input frames where the mask is non-zero, one more launch
+        (`fno_add_input_noise`): inputs += noise_std * z * mask, z a pure function of (noise_seed, noise_step, the sample
+        index, the element), so the same sample gets the same noise in any batch.  Labels, mask and case parameters are
+        not perturbed; noise_std = 0 launches nothing extra.  `train_auto(input_noise_std=...)` passes Adam's 1-based
+        step as noise_step.  Raises ValueError for a negative or non-finite noise_std, a noise_seed outside [0, 2^64)
+        or a noise_step outside [0, 2^63)."""
         from . import _lib
+        noise_std = check_noise_args(noise_std, noise_seed, noise_step)
         lib = _lib.load()
         idx = torch.as_tensor(idx, dtype=torch.int64)
         if idx.dim() != 1 or idx.numel() == 0:
@@ -84,10 +92,20 @@ class DeviceFrames:
                 _lib.check(lib.fno_gather_batch(*args, st), "fno_gather_batch")
             else:
                 _lib.check(lib.fno_grid_gather_batch(*args, gh, gw, st), "fno_grid_gather_batch")
+            if noise_std > 0:
+                self._add_noise(out, idx, noise_std, noise_seed, noise_step, st)
         idx.record_stream(torch.cuda.current_stream(dev))
         return out
 
-    def rollout_batch(self, idx, steps: int, time_step_size=None) -> Dict[str, Tensor]:
+    def _add_noise(self, out: Dict[str, Tensor], idx: Tensor, std: float, seed: int, step: int, st) -> None:
+        from . import _lib
+        step_dev = torch.full((1,), int(step), dtype=torch.int64, device=self.device)   # a fill kernel, no copy
+        _lib.check(_lib.load().fno_add_input_noise(out["inputs"].data_ptr(), out["mask"].data_ptr(), idx.data_ptr(),
+                                                   idx.numel(), self.height, self.width, std, int(seed),
+                                                   step_dev.data_ptr(), None, st), "fno_add_input_noise")
+
+    def rollout_batch(self, idx, steps: int, time_step_size=None, noise_std: float = 0.0, noise_seed: int = 0,
+                      noise_step: int = 0) -> Dict[str, Tensor]:
         """`batch(idx)` for the windows that start at samples `idx`, plus "labels" (steps, B, 2, H, W): step k's target
         labels[idx + k s] * mask, masked with the start sample's mask as `Fno2d.rollout` masks its predictions
         (s = time_step_size, by default the dataset's).  One launch (fno_[grid_]gather_window).
@@ -96,9 +114,13 @@ class DeviceFrames:
             preds = model.rollout(b["inputs"], b["case_params"], b["mask"], K)
             loss = sum(model.loss_fn(preds=preds[k], labels=b["labels"][k])["nmse"] for k in range(K)) / K
 
-        Raises ValueError for a non-positive steps / time_step_size, no time_step_size at all, or a window that crosses
-        a case boundary; IndexError for a window that runs past the split."""
+        noise_std, noise_seed and noise_step perturb the start samples' input frames as in `batch`; the targets are
+        not perturbed.
+
+        Raises ValueError for a non-positive steps / time_step_size, no time_step_size at all, a window that crosses
+        a case boundary or bad noise arguments (as `batch`); IndexError for a window that runs past the split."""
         from . import _lib
+        noise_std = check_noise_args(noise_std, noise_seed, noise_step)
         lib = _lib.load()
         s = self.time_step_size if time_step_size is None else time_step_size
         if isinstance(steps, bool) or not isinstance(steps, (int, np.integer)) or steps < 1:
@@ -132,6 +154,8 @@ class DeviceFrames:
                 _lib.check(lib.fno_gather_window(*args, st), "fno_gather_window")
             else:
                 _lib.check(lib.fno_grid_gather_window(*args, gh, gw, st), "fno_grid_gather_window")
+            if noise_std > 0:
+                self._add_noise(out, idx, noise_std, noise_seed, noise_step, st)
         idx.record_stream(torch.cuda.current_stream(dev))
         return out
 
@@ -143,6 +167,20 @@ class DeviceFrames:
         """Batches in exactly the order `DataLoader(dataset, batch_size, shuffle, generator=generator)` visits them:
         the index stream comes from the same torch samplers the DataLoader builds (`index_batches`)."""
         return self.batches(index_batches(self.n, batch_size, shuffle, generator, drop_last))
+
+
+def check_noise_args(noise_std, noise_seed, noise_step=0, std_name: str = "noise_std") -> float:
+    """Refuse training-noise arguments the noise kernel cannot take: a noise_std that is not a real >= 0 and finite in
+    float32, a
+    noise_seed that is not an int in [0, 2^64), a noise_step that is not an int in [0, 2^63).  Returns noise_std as a
+    float."""
+    if isinstance(noise_std, bool) or not isinstance(noise_std, (int, float, np.integer, np.floating)) \
+            or not np.isfinite(noise_std) or noise_std < 0 or noise_std > float(np.finfo(np.float32).max):
+        raise ValueError(f"{std_name} must be a real number >= 0, finite in float32, got {noise_std!r}")
+    for name, v, hi in (("noise_seed", noise_seed, 2 ** 64), ("noise_step", noise_step, 2 ** 63)):
+        if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or not 0 <= int(v) < hi:
+            raise ValueError(f"{name} must be an int in [0, 2^{hi.bit_length() - 1}), got {v!r}")
+    return float(noise_std)
 
 
 def index_batches(n: int, batch_size: int, shuffle: bool = False, generator=None,

@@ -14,6 +14,8 @@ synchronisation.  The result is bit-identical to the eager loop `DeviceFrames.lo
     from cfdbench_b200 import train_auto
     train_auto(model, train_data, dev_data, output_dir, num_epochs=..., lr=..., batch_size=...)   # for train(...)
     train_auto(..., rollout_steps=4)   # trained through 4-step rollouts of the model's own predictions
+    train_auto(..., rollout_steps=4, rollout_grad_steps=1)   # pushforward: 3 steps without gradient, the 4th trained
+    train_auto(..., input_noise_std=0.01, noise_seed=1)      # Gaussian noise on every step's input frame
 """
 from __future__ import annotations
 
@@ -29,7 +31,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .data import DeviceFrames, case_table, index_batches, rollout_windows
+from .data import DeviceFrames, case_table, check_noise_args, index_batches, rollout_windows
 
 LOG_COLUMNS = ("mse", "rmse", "mae", "nmse", "mean_l2")   # one row of the epoch log: fno_loss_fwd's five scalars
 
@@ -77,9 +79,12 @@ class _StepGraphs:
     place; the packed weight images are rebuilt inside the graph from the parameters as the previous replay's Adam
     left them."""
 
-    def __init__(self, model, frames: DeviceFrames, batch_size: int, optimizer, n: Optional[int] = None):
-        """n: the length of an epoch's permutation (default: every sample)."""
+    def __init__(self, model, frames: DeviceFrames, batch_size: int, optimizer, n: Optional[int] = None,
+                 noise_std: float = 0.0, noise_seed: int = 0):
+        """n: the length of an epoch's permutation (default: every sample).  noise_std > 0: every step adds
+        fno_add_input_noise(noise_std, noise_seed, step = Adam's 1-based step) to its input frames after the gather."""
         lib = self.lib = _lib.load()
+        self.noise_std, self.noise_seed = noise_std, noise_seed
         self.model, self.frames, self.optimizer = model, frames, optimizer
         dev = self.dev = model.device
         n, gh, gw = frames.n if n is None else n, frames.height, frames.width
@@ -100,6 +105,9 @@ class _StepGraphs:
         self.flat, _, self.grads = model._grad_buffers()
 
         self.io = self._make_io(bmax, gh, gw, p)
+        if noise_std > 0:   # the epoch's first Adam step; a step's noise step is this plus the cursor
+            self.io["step_base"] = torch.zeros(1, dtype=torch.int64, device=dev)
+            self.step_base_host = torch.empty(1, dtype=torch.int64, pin_memory=True)
         self.perm_host = torch.empty(n, dtype=torch.int64, pin_memory=True)
         self.coef_host = torch.empty(self.steps, 2, dtype=torch.float32, pin_memory=True)
 
@@ -176,6 +184,7 @@ class _StepGraphs:
             _lib.check(lib.fno_gather_batch(*args, st), "fno_gather_batch")
         else:
             _lib.check(lib.fno_grid_gather_batch(*args, gh, gw, st), "fno_grid_gather_batch")
+        self._add_noise(b, st)
         self._repack(st)
         inputs, mask, cp = io["inputs"][:b], io["mask"][:b], io["cp"][:b]
         preds, labm, dpreds = io["preds"][:b], io["labm"][:b], io["dpreds"][:b]
@@ -211,6 +220,15 @@ class _StepGraphs:
         _lib.check(self.lib.fno_train_stage_indices(io["perm"].data_ptr(), self.n, self.stride, b, io["cursor"].data_ptr(),
                                                     io["idx"].data_ptr(), st), "fno_train_stage_indices")
 
+    def _add_noise(self, b: int, st) -> None:
+        """The input noise of the gathered batch (nothing when noise_std is 0): step = step_base + cursor."""
+        if self.noise_std > 0:
+            io = self.io
+            _lib.check(self.lib.fno_add_input_noise(io["inputs"].data_ptr(), io["mask"].data_ptr(), io["idx"].data_ptr(), b,
+                                                    self.gh, self.gw, self.noise_std, self.noise_seed,
+                                                    io["step_base"].data_ptr(), io["cursor"].data_ptr(), st),
+                       "fno_add_input_noise")
+
     def _repack(self, st) -> None:
         """The packed weights, from the parameters as the previous step's Adam left them (Fno2d._pack's images)."""
         lib, model, sw = self.lib, self.model, self.sw
@@ -243,6 +261,9 @@ class _StepGraphs:
                    "fno_adam_coefficients")
         io["perm"].copy_(self.perm_host, non_blocking=True)
         io["coef"].copy_(self.coef_host, non_blocking=True)
+        if self.noise_std > 0:
+            self.step_base_host[0] = first_step
+            io["step_base"].copy_(self.step_base_host, non_blocking=True)
         io["cursor"].zero_()
         for g, count in zip(self.graphs, self.counts):
             for _ in range(count):
@@ -260,36 +281,45 @@ class _StepGraphs:
 class _RolloutStepGraphs(_StepGraphs):
     """The captured step of training through `k`-step rollouts (train_auto with rollout_steps = k > 1): the epoch's
     permutation holds window starts, and a step is stage indices -> gather window (inputs, mask and case parameters of
-    the start sample, the k masked targets) -> weight repack -> rollout training forward into one reused saved set ->
-    K-step loss forward and backward -> rollout backward (one recomputing sweep, no input gradients) into the flat
-    gradient buffer -> Adam -> log of the aggregate loss row.  Same graphs, buffers-per-batch layout and epoch as
-    _StepGraphs; the per-step buffers are [k][b] blocks of the first k*b samples' worth of (k, bmax, ...) buffers."""
+    the start sample, the k masked targets) -> [input noise] -> weight repack -> [pushforward prefix] -> rollout
+    training forward into one reused saved set -> K-step loss forward and backward -> rollout backward (one recomputing
+    sweep, no input gradients) into the flat gradient buffer -> Adam -> log of the aggregate loss row.  Same graphs,
+    buffers-per-batch layout and epoch as _StepGraphs; the per-step buffers are [k][b] blocks of the first k*b samples'
+    worth of (k, bmax, ...) buffers.
+
+    grad_steps = g < k (pushforward): the first k - g steps run without gradient through the inference rollout
+    (fno_[grid_]rollout, the kernels generate_many runs) into a (k - g, bmax, ...) prefix buffer, on the step's
+    workspace (the model's inference workspace for bmax samples, with the bf16 ym_img image); the training rollout, the
+    loss against targets k - g ... k - 1 and the backward then cover the last g steps from the prefix's last frame."""
 
     def __init__(self, model, frames: DeviceFrames, batch_size: int, optimizer, n_windows: int, steps: int,
-                 time_step_size: int):
+                 time_step_size: int, grad_steps: Optional[int] = None, noise_std: float = 0.0, noise_seed: int = 0):
         self.k, self.tss = steps, time_step_size
-        super().__init__(model, frames, batch_size, optimizer, n=n_windows)
+        self.g = steps if grad_steps is None else grad_steps
+        super().__init__(model, frames, batch_size, optimizer, n=n_windows, noise_std=noise_std, noise_seed=noise_seed)
 
     def _make_io(self, bmax: int, gh: int, gw: int, p: int) -> dict:
-        lib, dev, n, k = self.lib, self.dev, self.n, self.k
+        lib, dev, n, k, g = self.lib, self.dev, self.n, self.k, self.g
         f32 = dict(dtype=torch.float32, device=dev)
         io = dict(
             perm=torch.zeros(n, dtype=torch.int64, device=dev),
             idx=torch.zeros(bmax, dtype=torch.int64, device=dev),
             inputs=torch.empty(bmax, 2, gh, gw, **f32), mask=torch.empty(bmax, 1, gh, gw, **f32),
             cp=torch.empty(bmax, p, **f32), labels=torch.empty(k, bmax, 2, gh, gw, **f32),
-            preds=torch.empty(k, bmax, 2, gh, gw, **f32), dpreds=torch.empty(k, bmax, 2, gh, gw, **f32),
-            carry=torch.empty(bmax, 2, gh, gw, **f32), loss=torch.empty(k + 1, 5, **f32),
-            scratch=torch.zeros(lib.fno_loss_seq_scratch_bytes(k), dtype=torch.uint8, device=dev),
+            preds=torch.empty(g, bmax, 2, gh, gw, **f32), dpreds=torch.empty(g, bmax, 2, gh, gw, **f32),
+            carry=torch.empty(bmax, 2, gh, gw, **f32), loss=torch.empty(g + 1, 5, **f32),
+            scratch=torch.zeros(lib.fno_loss_seq_scratch_bytes(g), dtype=torch.uint8, device=dev),
             gout=torch.zeros(4, **f32),   # d/d(mse, rmse, mae, nmse) of the aggregate's nmse: (0, 0, 0, 1)
             cursor=torch.zeros(1, dtype=torch.int32, device=dev),
             coef=torch.empty(self.steps, 2, **f32), log=torch.empty(self.steps, len(LOG_COLUMNS), **f32))
+        if g < k:
+            io["prefix"] = torch.empty(k - g, bmax, 2, gh, gw, **f32)
         io["gout"][3:].fill_(1.0)
         return io
 
     def _issue(self, b: int, update: bool) -> None:
         lib, model, io, sw, fr = self.lib, self.model, self.io, self.sw, self.frames
-        gh, gw, grid, p, k = self.gh, self.gw, self.grid, fr.n_case_params, self.k
+        gh, gw, grid, p, k, g = self.gh, self.gw, self.grid, fr.n_case_params, self.k, self.g
         st = C.c_void_p(torch.cuda.current_stream(self.dev).cuda_stream)
         self._stage_indices(b, st)
         args = (fr.frames_in.data_ptr(), fr.frames_out.data_ptr(), fr.case_table.data_ptr(), fr.case_ids.data_ptr(),
@@ -300,33 +330,44 @@ class _RolloutStepGraphs(_StepGraphs):
             _lib.check(lib.fno_gather_window(*args, st), "fno_gather_window")
         else:
             _lib.check(lib.fno_grid_gather_window(*args, gh, gw, st), "fno_grid_gather_window")
+        self._add_noise(b, st)
         self._repack(st)
         x, mk, cp = io["inputs"].data_ptr(), io["mask"].data_ptr(), io["cp"].data_ptr()
         preds, labels, dpreds = io["preds"].data_ptr(), io["labels"].data_ptr(), io["dpreds"].data_ptr()
         ts, ws = self.ts, self.ws
+        n_el = b * 2 * gh * gw   # per step
+        if g < k:   # the pushforward prefix, without gradient; the trained steps start from its last frame
+            pre = io["prefix"].data_ptr()
+            if grid:
+                _lib.check(lib.fno_grid_rollout(C.byref(sw["struct"]), x, mk, cp, pre, k - g, C.byref(ws), b, gh, gw, st),
+                           "fno_grid_rollout")
+            else:
+                _lib.check(lib.fno_rollout(C.byref(sw["struct"]), x, mk, cp, pre, k - g, C.byref(ws), b, model._act_code(),
+                                           st), "fno_rollout")
+            x = pre + (k - g - 1) * n_el * 4
+            labels += (k - g) * n_el * 4
         if grid:
-            _lib.check(lib.fno_grid_rollout_forward_train(C.byref(sw["struct"]), x, mk, cp, preds, k, C.byref(ts["sv"]),
+            _lib.check(lib.fno_grid_rollout_forward_train(C.byref(sw["struct"]), x, mk, cp, preds, g, C.byref(ts["sv"]),
                                                           C.byref(ws), b, gh, gw, st), "fno_grid_rollout_forward_train")
         else:
-            _lib.check(lib.fno_rollout_forward_train(C.byref(sw["struct"]), x, mk, cp, preds, k, C.byref(ts["sv"]),
+            _lib.check(lib.fno_rollout_forward_train(C.byref(sw["struct"]), x, mk, cp, preds, g, C.byref(ts["sv"]),
                                                      C.byref(ws), b, model._act_code(), st), "fno_rollout_forward_train")
-        n_el = b * 2 * gh * gw   # per step
-        _lib.check(lib.fno_loss_seq_fwd(preds, labels, n_el, k, io["scratch"].data_ptr(), io["loss"].data_ptr(), st),
+        _lib.check(lib.fno_loss_seq_fwd(preds, labels, n_el, g, io["scratch"].data_ptr(), io["loss"].data_ptr(), st),
                    "fno_loss_seq_fwd")
-        _lib.check(lib.fno_loss_seq_bwd(preds, labels, io["loss"].data_ptr(), io["gout"].data_ptr(), dpreds, n_el, k, st),
+        _lib.check(lib.fno_loss_seq_bwd(preds, labels, io["loss"].data_ptr(), io["gout"].data_ptr(), dpreds, n_el, g, st),
                    "fno_loss_seq_bwd")
         carry = io["carry"].data_ptr()
         if grid:
             _lib.check(lib.fno_grid_rollout_backward(C.byref(sw["struct"]), C.byref(sw["struct_bwd"]), x, mk, cp, preds,
-                                                     dpreds, k, C.byref(ts["sv"]), C.byref(self.grads), C.byref(ts["sc"]),
+                                                     dpreds, g, C.byref(ts["sv"]), C.byref(self.grads), C.byref(ts["sc"]),
                                                      C.byref(ws), carry, None, None, b, gh, gw, st),
                        "fno_grid_rollout_backward")
         else:
             _lib.check(lib.fno_rollout_backward(C.byref(sw["struct"]), C.byref(sw["struct_bwd"]), x, mk, cp, preds, dpreds,
-                                                k, C.byref(ts["sv"]), C.byref(self.grads), C.byref(ts["sc"]), C.byref(ws),
+                                                g, C.byref(ts["sv"]), C.byref(self.grads), C.byref(ts["sc"]), C.byref(ws),
                                                 carry, None, None, b, model._act_code(), st), "fno_rollout_backward")
         if update:
-            self._adam_and_log(io["loss"][k].data_ptr(), st)
+            self._adam_and_log(io["loss"][g].data_ptr(), st)
 
 
 def _check_chain(frames: DeviceFrames, starts: np.ndarray, steps: int, time_step_size: int) -> None:
@@ -391,7 +432,8 @@ def _check_split(model, data, what: str) -> None:
 def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, lr: float = 1e-3, lr_step_size: int = 1,
                lr_gamma: float = 0.9, batch_size: int = 2, eval_batch_size: int = 2, log_interval: int = 10,
                eval_interval: int = 2, generator: Optional[torch.Generator] = None, rollout_steps: int = 1,
-               time_step_size: Optional[int] = None) -> dict:
+               time_step_size: Optional[int] = None, input_noise_std: float = 0.0, noise_seed: int = 0,
+               rollout_grad_steps: Optional[int] = None) -> dict:
     """What the reference's `train(model, train_data, dev_data, output_dir, ...)` does (src/train_auto.py:181-313), with
     its argument names and defaults, every training step replayed from a CUDA graph and one synchronisation per epoch.
 
@@ -421,6 +463,25 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
       (frames_in[j + k s] == frames_out[j + (k-1) s] for every pair a window uses): that is checked once on the device
       before training.  The dev evaluation, and with it checkpoint selection, stays single-step.  rollout_steps = 1 is
       the single-step loop above, launch for launch.
+    - rollout_grad_steps = G (1 <= G <= K, default K) is pushforward training: of each window's K steps the first
+      K - G run without gradient through the inference rollout (the kernels `generate_many` runs), and only the last
+      G are trained, from the prefix's last frame, on (nmse_{K-G} + ... + nmse_{K-1}) / G; the log and train_losses
+      hold that mean.  G = K is the full rollout above, launch for launch; with K = 1 only G = 1 is valid.
+    - input_noise_std = sigma > 0 adds Gaussian noise to every step's (start) input frame where the mask is non-zero,
+      `DeviceFrames.batch(..., noise_std=sigma, noise_seed=noise_seed, noise_step=t)` with t Adam's 1-based global step
+      of that update.  The noise comes from a counter-based RNG seeded by `noise_seed` (an int in [0, 2^64)), never
+      from `generator`, so the visiting order is the one without noise; 0 launches nothing extra.  One step is
+      bit-identical to the eager loop
+
+          b = frames.rollout_batch(idx, K, noise_std=sigma, noise_seed=noise_seed, noise_step=t)
+          x = b["inputs"]
+          if K > G:
+              with torch.no_grad():
+                  x = model.generate_many(x, b["case_params"], b["mask"], K - G)[-1]
+          seq = model.rollout(x, b["case_params"], b["mask"], G)
+          loss = sum(model.loss_fn(preds=seq[g], labels=b["labels"][K - G + g])["nmse"] for g in range(G)) / G
+
+      (at K = 1: `frames.batch(idx, noise_std=...)` and the single-step loss).
 
     Returns dict(train_losses=[per-step nmse, every epoch], optimizer=the FusedAdam).  Its state holds the true step
     count (its state_dict loads into torch.optim.Adam), and the parameters' version counters are bumped, so the
@@ -429,7 +490,9 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
     intervals or epoch count, a model whose parameters are all frozen, an empty or malformed split, a split whose
     case-parameter count differs from the model's, data parallel enabled, or a grid / storage mode the model rejects;
     and, as ValueError before any training step, a non-positive rollout_steps or time_step_size, rollout_steps > 1 with
-    no time_step_size, a split without a single K-step window, or a split whose frames do not chain.
+    no time_step_size, a split without a single K-step window, or a split whose frames do not chain.  Also raises
+    ValueError before any device work for an input_noise_std that is negative, NaN, infinite or not a real number, a
+    noise_seed that is not an int in [0, 2^64), or a rollout_grad_steps that is not an int in 1..rollout_steps.
     Frozen parameters (requires_grad=False) are not updated, as FusedAdam.step skips them.  Data parallel training in
     this loop is not supported."""
     from .metrics import evaluate_auto
@@ -444,6 +507,11 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
                     ("eval_batch_size", eval_batch_size), ("log_interval", log_interval), ("eval_interval", eval_interval),
                     ("rollout_steps", rollout_steps)):
         _positive_int(name, v)
+    input_noise_std = check_noise_args(input_noise_std, noise_seed, std_name="input_noise_std")
+    grad_steps = rollout_steps if rollout_grad_steps is None else rollout_grad_steps
+    if isinstance(grad_steps, bool) or not isinstance(grad_steps, (int, np.integer)) or not 1 <= grad_steps <= rollout_steps:
+        raise ValueError(f"rollout_grad_steps must be an int in 1..rollout_steps={rollout_steps}, got {rollout_grad_steps!r}")
+    grad_steps = int(grad_steps)
     if model._dp_enabled:
         raise ValueError("train_auto does not run data parallel: its step graph has no all-reduce")
     if not any(p.requires_grad for p in model.parameters()):
@@ -473,16 +541,22 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
         frames = train_data if isinstance(train_data, DeviceFrames) else DeviceFrames(train_data, device=dev)
         dev_frames = None
         n = frames.n
+        noise = dict(noise_std=input_noise_std, noise_seed=int(noise_seed))
         if windows is None:
-            graphs = _StepGraphs(model, frames, batch_size, optimizer)
+            graphs = _StepGraphs(model, frames, batch_size, optimizer, **noise)
         else:
             _check_chain(frames, windows, rollout_steps, int(tss))
-            graphs = _RolloutStepGraphs(model, frames, batch_size, optimizer, windows.size, rollout_steps, int(tss))
+            graphs = _RolloutStepGraphs(model, frames, batch_size, optimizer, windows.size, rollout_steps, int(tss),
+                                        grad_steps, **noise)
         print("====== Training ======")
         print(f"# batch: {batch_size}")
         print(f"# examples: {n}")
         if windows is not None:
             print(f"# rollout steps: {rollout_steps}, windows: {windows.size}")
+            if grad_steps < rollout_steps:
+                print(f"# trained steps: the last {grad_steps} (pushforward)")
+        if input_noise_std > 0:
+            print(f"# input noise std: {input_noise_std}, seed {int(noise_seed)}")
         print(f"# step: {graphs.steps}")
         print(f"# epoch: {num_epochs}")
         start_time = time.time()

@@ -327,6 +327,20 @@ int fno_loss_seq_fwd(const float* preds_seq, const float* labels_seq, size_t n, 
 int fno_loss_seq_bwd(const float* preds_seq, const float* labels_seq, const float* fwd, const float* gout, float* dpreds_seq,
                      size_t n, int steps, void* stream);
 
+/* ---- training noise (cfdbench_b200.train_auto with input_noise_std > 0, DeviceFrames.batch(noise_std=...)) ----------
+ * In place on n gathered input frames inputs [n][2][h][w] float32 with their masks mask [n][1][h][w]:
+ *   inputs[b][c][y][x] = fmaf(std * z, mask[b][0][y][x], inputs[b][c][y][x])   where mask != 0 (other cells not written)
+ * z is a standard normal and a pure function of (seed, step, j = idx[b], e), e = c h w + y w + x the element's index in
+ * the sample's flattened (2, h, w) frame: (x0, x1, x2, x3) = Philox4x32-10(counter = (q, j, step & 0xffffffff,
+ * step >> 32), key = (seed & 0xffffffff, seed >> 32)) for the quad q = e / 4 (the last quad is partial when h w is odd),
+ * u_i = x_i 2^-32 + 2^-33 in float32, r = sqrtf(-2 logf(u0)), (z0, z1) = r (cospif(2 u1), sinpif(2 u1)), and (z2, z3)
+ * likewise from (x2, x3); element e takes z_{e mod 4}.  step = *step_base + *step_offset (int64 + int32, both in device
+ * memory, read when the kernel runs; step_offset may be NULL for 0), so a captured launch sees each replay's step.
+ * 64x64 or any grid with 24 <= h, w <= 128; inputs and mask need only 4-byte alignment.  Status 3 for a grid outside
+ * the range; status 1 for a null pointer (other than step_offset), n <= 0 or a negative or non-finite std. */
+int fno_add_input_noise(float* inputs, const float* mask, const int64_t* idx, int n, int h, int w_, float std, uint64_t seed,
+                        const int64_t* step_base, const int32_t* step_offset, void* stream);
+
 /* ---------------------------------------------------------------------------------------------------
  * Grid-generic path: the same network on H x W frames with 24 <= H <= 128 and 24 <= W <= 128, e.g. CFDBench's
  * tube and dam problems (66 x 65, reference src/utils/autoregressive.py:24-26).  fp32 activation storage only (there is
