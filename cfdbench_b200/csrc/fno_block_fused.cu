@@ -12,10 +12,13 @@
 //          K-major B operand of GEMM2 per image row (96 KB for 16 rows).  Bias rides in the row that irfft2's C2R stage
 //          ignores (Im of ky = 0).
 //   GEMM2 per image row h:  D[64 w][32 o] = E[w][(ky, ri) 24] Zt_h + X_h[w][32 i] W0^T
-//          E Zt_h: m64n32k8 tf32, 3xTF32 (E = C2R stage with c_ky/HW folded in, fno_block_tc.cu builds it).
-//          X_h W0^T: m64n32k16 bf16 straight from the TMA slot that holds the row as [i][w] (the M-major A operand), W0 as
-//          three bf16 terms (24 mantissa bits), accumulated into the same fp32 registers.  x is exact in bf16.
-//          Epilogue exact-erf GELU -> bf16 -> swizzled [o][w] staging tile -> one TMA store per row.
+//          E Zt_h: m64n32k8 tf32, 3xTF32 (E = C2R stage with c_ky/HW folded in, fno_block_tc.cu builds it); E's hi / lo
+//          A fragments are loaded into registers once per CTA, so only Zt_h is read from shared memory.
+//          X_h W0^T: m64n32k16 bf16, A = the row of the TMA slot that holds it as [i][w], read once per row by
+//          ldmatrix.trans into A fragments and used by all three bf16 terms of W0 (24 mantissa bits), accumulated into
+//          the same fp32 registers.  x is exact in bf16.
+//          Epilogue exact-erf GELU -> bf16x2 -> stmatrix.trans into the swizzled [o][w] staging tile -> one TMA store
+//          per row.
 // Roles: warp 8 lanes 0/1 -- producers of the two image slots (24 KB = one ky pair, hi + lo, two bulk copies each);
 // warpgroups 0 / 1 -- the even / odd ky pairs of GEMM1 and the even / odd rows of GEMM2.  Each warpgroup owns a ring of
 // kFzXSlots activation rows; its thread 0 refills a slot as soon as the MMAs that read it have completed, so the ring
@@ -42,7 +45,6 @@ constexpr int kFzFFloats = 2 * (2 * kFzRows) * kImgK;  // [n = 2 h' + ri (32)][4
 constexpr int kFzEFloats = 2 * kW * kZK;               // [64 w][24] hi | lo
 constexpr uint32_t kFzZtFloats = kC * kZK;             // one image row, hi or lo: [32 o][24 k] K-major
 constexpr uint32_t kLboF = (2 * kFzRows / 8) * 128;    // 512
-constexpr uint32_t kLboE = (kW / 8) * 128;             // 1024
 constexpr uint32_t kLboO = (kC / 8) * 128;             // 512: B operands with 32 rows (o)
 // One image row of all 32 channels of a bf16 activation: TMA box {w 64, h 1, (b, c) 32}, [c][w] with the 128-byte swizzle.
 // The same box is the load of x and the store of out.
@@ -63,8 +65,6 @@ struct FzSmem {
   alignas(128) float zt[kFzRows][2][kFzZtFloats];      // GEMM2 B operand per row: hi, lo
   alignas(128) float f_hi[kFzFFloats / 2];
   alignas(128) float f_lo[kFzFFloats / 2];
-  alignas(128) float e_hi[kFzEFloats / 2];
-  alignas(128) float e_lo[kFzEFloats / 2];
   alignas(128) unsigned char w0[3][kFzW0Bytes];        // B[n = o][k = i] = W0[o][i] = t1 + t2 + t3 (bf16 terms)
   alignas(16) float bias[kC];
   alignas(8) uint64_t y_full[2], y_free[2];
@@ -101,10 +101,6 @@ __global__ void __launch_bounds__(kFzThreads, 1)
   for (int e = tid; e < kFzFFloats / 2; e += kFzThreads) {
     sm.f_hi[e] = __ldg(ftab + chunk * kFzFFloats + e);
     sm.f_lo[e] = __ldg(ftab + chunk * kFzFFloats + kFzFFloats / 2 + e);
-  }
-  for (int e = tid; e < kFzEFloats / 2; e += kFzThreads) {
-    sm.e_hi[e] = __ldg(etab + e);
-    sm.e_lo[e] = __ldg(etab + kFzEFloats / 2 + e);
   }
   for (int e = tid; e < kC * kC; e += kFzThreads) {  // B[n = o][k = i] = W0[o][i] = w0t[i][o]: three bf16 terms
     const int i = e / kC, o = e % kC;
@@ -155,6 +151,17 @@ __global__ void __launch_bounds__(kFzThreads, 1)
   if (t == 0)
     for (int n = 0; n < kFzXSlots && n < n_fills; ++n) x_fill(n);
   const uint32_t w0_s = tc::smem_addr(sm.w0[0]);
+  // A fragments of E (tf32 m64k8, rows w = m0, m0 + 8) for the C2R passes of every row: e_frag[0 / 1] = hi / lo
+  uint32_t e_frag[2][kZK / 8][4];
+#pragma unroll
+  for (int hl = 0; hl < 2; ++hl)
+#pragma unroll
+    for (int ks = 0; ks < kZK / 8; ++ks)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const uint32_t off = tc::kmajor_offset(m0 + 8 * (j & 1), 8 * ks + q + 4 * (j >> 1), kW) / 4;
+        e_frag[hl][ks][j] = __float_as_uint(__ldg(etab + hl * (kFzEFloats / 2) + off));
+      }
 
   for (int u = 0; u < n_units; ++u) {
     const int b = b0 + u * bstride;
@@ -215,29 +222,36 @@ __global__ void __launch_bounds__(kFzThreads, 1)
     // ---------------------------------------------------------------- GEMM2: rows g, g + 2, ..., 14 + g
     // Iteration r issues row r's MMAs into acc[r & 1], then finishes row r - 1: wait for its MMAs (all but the newest
     // group), GELU into staging tile (r - 1) & 1, one TMA store, and the refill of the activation slot it read.
+    // The MMAs read x_frag[r & 1] from registers until that wait, so the next row loads into the other set.
     float acc[2][16];
+    uint32_t x_frag[2][kC / 16][4];
 #pragma unroll
     for (int r = 0; r <= kFzWgRows; ++r) {
       if (r < kFzWgRows) {
         const int n = kFzWgRows * u + r, hl = g + 2 * r;
         mbar_wait(&sm.x_full[g][fz_x_slot(n)], fz_x_parity(n));
+        // A[m = w][k = i] of K step ks from lines i of the slot: matrix j = lines 16 ks + 8 (j >> 1) .. + 7, pixels
+        // 16 wq + 8 (j & 1) .. + 7 (one 16-byte chunk per line, distinct swizzle phases: no bank conflicts)
+        const uint32_t a_x = tc::smem_addr(sm.x[g][fz_x_slot(n)]);
+#pragma unroll
+        for (int ks = 0; ks < kC / 16; ++ks)
+          tc::ldmatrix_x4_trans(x_frag[r & 1][ks], a_x + sw128_bf16_offset(16 * ks + 8 * (lane >> 4) + (lane & 7),
+                                                                             16 * wq + 8 * ((lane >> 3) & 1)));
         tc::wg_fence();
-        const uint32_t a_e[3] = {tc::smem_addr(sm.e_hi), tc::smem_addr(sm.e_lo), tc::smem_addr(sm.e_hi)};
         const uint32_t b_z[3] = {tc::smem_addr(sm.zt[hl][0]), tc::smem_addr(sm.zt[hl][0]), tc::smem_addr(sm.zt[hl][1])};
 #pragma unroll
-        for (int pass = 0; pass < 3; ++pass)
+        for (int pass = 0; pass < 3; ++pass)   // E_hi Zt_hi + E_lo Zt_hi + E_hi Zt_lo
 #pragma unroll
           for (int ks = 0; ks < kZK / 8; ++ks)
-            tc::wg_tf32_ss_n32(acc[r & 1], tc::make_smem_desc(a_e[pass] + ks * 2 * kLboE, kLboE, 128),
+            tc::wg_tf32_rs_n32(acc[r & 1], e_frag[pass == 1][ks],
                                tc::make_smem_desc(b_z[pass] + ks * 2 * kLboO, kLboO, 128), (pass | ks) ? 1u : 0u);
         tc::wg_fence();   // the bf16 MMAs below have another shape: order their accumulator accesses explicitly
-        const uint32_t a_x = tc::smem_addr(sm.x[g][fz_x_slot(n)]);
 #pragma unroll
         for (int term = 0; term < 3; ++term)
 #pragma unroll
-          for (int ks = 0; ks < kC / 16; ++ks)   // K = 16 channels = 16 lines of 128 B
-            tc::wg_bf16_ss_n32_mn_a(acc[r & 1], tc::make_smem_desc_sw128_mn(a_x + ks * 2048),
-                                    tc::make_smem_desc(w0_s + term * kFzW0Bytes + ks * 2 * kLboO, kLboO, 128), 1u);
+          for (int ks = 0; ks < kC / 16; ++ks)   // K = 16 channels
+            tc::wg_bf16_rs_n32(acc[r & 1], x_frag[r & 1][ks],
+                               tc::make_smem_desc(w0_s + term * kFzW0Bytes + ks * 2 * kLboO, kLboO, 128), 1u);
         tc::wg_commit();
       }
       if (r == 0) continue;
@@ -249,18 +263,24 @@ __global__ void __launch_bounds__(kFzThreads, 1)
         tc::wg_wait<0>();
       }
       tc::wg_fence_acc(acc[rr & 1]);
-      // d[4 i + 2 hh + e] = D[w = m0 + 8 hh][o = 8 i + 2 q + e] -> staging line o, element w.  Per store instruction a
-      // warp writes 8 consecutive pixels of 4 channels whose lines have distinct swizzle phases: no bank conflicts.
+      // d[4 i + 2 hh + e] = D[w = m0 + 8 hh][o = 8 i + 2 q + e] -> staging line o, element w.  The pair e = 0, 1 is one
+      // bf16x2 register of the transposed 8x8 matrix (i, hh): its rows are lines 8 i .. 8 i + 7, each one 16-byte chunk
+      // at pixel 16 wq + 8 hh.  Eight lines have distinct swizzle phases: no bank conflicts.
       unsigned char* stile = sm.st[g][rr & 1];
 #pragma unroll
-      for (int i = 0; i < 4; ++i)
+      for (int i2 = 0; i2 < 2; ++i2) {   // matrix j of the x4 store: i = 2 i2 + (j >> 1), hh = j & 1
+        uint32_t v[4];
 #pragma unroll
-        for (int hh = 0; hh < 2; ++hh) {
-          const float2 v = gelu_erf2(make_float2(d[4 * i + 2 * hh], d[4 * i + 2 * hh + 1]));
-          const int w = m0 + 8 * hh, o = 8 * i + 2 * q;
-          *reinterpret_cast<__nv_bfloat16*>(stile + sw128_bf16_offset(o, w)) = __float2bfloat16_rn(v.x);
-          *reinterpret_cast<__nv_bfloat16*>(stile + sw128_bf16_offset(o + 1, w)) = __float2bfloat16_rn(v.y);
+        for (int j = 0; j < 4; ++j) {
+          const int i = 2 * i2 + (j >> 1), hh = j & 1;
+          const float2 y = gelu_erf2(make_float2(d[4 * i + 2 * hh], d[4 * i + 2 * hh + 1]));
+          const __nv_bfloat162 p = __floats2bfloat162_rn(y.x, y.y);
+          v[j] = *reinterpret_cast<const uint32_t*>(&p);
         }
+        tc::stmatrix_x4_trans(tc::smem_addr(stile) + sw128_bf16_offset(16 * i2 + 8 * (lane >> 4) + (lane & 7),
+                                                                       16 * wq + 8 * ((lane >> 3) & 1)),
+                              v);
+      }
       tc::fence_proxy_async_smem();
       // the store of the previous row has read its tile, which the next row's epilogue overwrites
       if (t == 0) bulk_wait_group_read<0>();

@@ -50,12 +50,6 @@ __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_
 __device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t saddr) {
   return make_smem_desc(saddr, 16, 1024) | (static_cast<uint64_t>(1) << 62);
 }
-// M-major (MN-major) bf16 operand of 64 rows written by TMA with the 128-byte swizzle: line k holds the 64 M values of
-// K index k (128 B), 8-line atoms of 1024 B, 1024-byte aligned.  SBO = the K distance between 8-line groups (1024); LBO
-// would step to the next 64 M values, which a 64-row operand does not have.  A K step of 16 advances the start by 2048.
-__device__ __forceinline__ uint64_t make_smem_desc_sw128_mn(uint32_t saddr) {
-  return make_smem_desc(saddr, 16, 1024) | (static_cast<uint64_t>(1) << 62);
-}
 
 // ---- warpgroup MMA ----------------------------------------------------------------------------------
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
@@ -94,19 +88,21 @@ __device__ __forceinline__ void wg_bf16_ss_n72(float* d, uint64_t a, uint64_t b,
       : "l"(a), "l"(b), "r"(acc)
       : "memory");
 }
-// A M-major (transpose bit set, descriptor above), B K-major.
-__device__ __forceinline__ void wg_bf16_ss_n32_mn_a(float* d, uint64_t a, uint64_t b, uint32_t acc) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
-      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 1, 0;\n}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-      : "l"(a), "l"(b), "r"(acc)
-      : "memory");
-}
 __device__ __forceinline__ void wg_tf32_rs_n32(float* d, const uint32_t* a, uint64_t b, uint32_t acc) {
   asm volatile(
       "{\n.reg .pred p;\nsetp.ne.b32 p, %21, 0;\n"
       "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p, 1, 1;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(acc)
+      : "memory");
+}
+// A from registers (bf16 m64k16 fragment: warp w, lane l, r = 16 w + l / 4, q = l % 4, each register two bf16 along K,
+// the lower half first: a[0] = A[r][2q..], a[1] = A[r + 8][2q..], a[2] = A[r][2q + 8..], a[3] = A[r + 8][2q + 8..]),
+// B K-major.
+__device__ __forceinline__ void wg_bf16_rs_n32(float* d, const uint32_t* a, uint64_t b, uint32_t acc) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %21, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p, 1, 1, 0;\n}\n"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(acc)
       : "memory");
@@ -129,6 +125,22 @@ __device__ __forceinline__ void wg_tf32_rs_n64(float* d, const uint32_t* a, uint
 }
 
 // ---- operand staging helpers -------------------------------------------------------------------------
+// Four 8x8 b16 matrices, transposed on the way: lanes 8j .. 8j + 7 give the shared addresses of the eight 16-byte rows of
+// matrix j; register j of lane l receives elements [2 (l % 4)] and [2 (l % 4) + 1] of column l / 4 (lower half first).
+__device__ __forceinline__ void ldmatrix_x4_trans(uint32_t (&r)[4], uint32_t saddr) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(saddr)
+               : "memory");
+}
+// The inverse: register j of lane l holds elements [2 (l % 4)] and [2 (l % 4) + 1] of column l / 4 of matrix j, whose
+// eight rows go to the addresses lanes 8j .. 8j + 7 give.
+__device__ __forceinline__ void stmatrix_x4_trans(uint32_t saddr, const uint32_t (&r)[4]) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.trans.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(saddr), "r"(r[0]),
+               "r"(r[1]), "r"(r[2]), "r"(r[3])
+               : "memory");
+}
+
 // byte offset of element (row, k) inside a K-major un-swizzled tf32 operand tile with `rows` rows:
 // core matrix (row/8, k/4) at ((k/4) * (rows/8) + row/8) * 128
 __host__ __device__ constexpr uint32_t kmajor_offset(int row, int k, int rows) {
