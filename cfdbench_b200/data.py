@@ -16,7 +16,7 @@ datasets hold (N, 3, 66, 65) frames, reference src/dataset/tube.py:228-281, dam.
 from __future__ import annotations
 
 import ctypes as C
-from typing import Dict, Iterable, Iterator, List, Sequence
+from typing import Dict, Iterable, Iterator, List, Optional, Sequence
 
 import numpy as np
 import torch
@@ -73,7 +73,7 @@ class DeviceFrames:
         or a noise_step outside [0, 2^63)."""
         from . import _lib
         noise_std = check_noise_args(noise_std, noise_seed, noise_step)
-        lib = _lib.load()
+        _lib.load()   # a missing library raises before any device work
         idx = torch.as_tensor(idx, dtype=torch.int64)
         if idx.dim() != 1 or idx.numel() == 0:
             raise ValueError("idx must be a non-empty 1-D index list")
@@ -83,15 +83,9 @@ class DeviceFrames:
         b, p, dev, gh, gw = idx.numel(), self.n_case_params, self.device, self.height, self.width
         out = dict(inputs=torch.empty(b, 2, gh, gw, device=dev), label=torch.empty(b, 2, gh, gw, device=dev),
                    mask=torch.empty(b, 1, gh, gw, device=dev), case_params=torch.empty(b, p, device=dev))
-        args = (self.frames_in.data_ptr(), self.frames_out.data_ptr(), self.case_table.data_ptr(), self.case_ids.data_ptr(),
-                idx.data_ptr(), b, p, _lib.ACT_BF16 if self.frame_dtype == torch.bfloat16 else _lib.ACT_F32,
-                out["inputs"].data_ptr(), out["label"].data_ptr(), out["mask"].data_ptr(), out["case_params"].data_ptr())
         with torch.cuda.device(dev):
             st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-            if (gh, gw) == (64, 64):
-                _lib.check(lib.fno_gather_batch(*args, st), "fno_gather_batch")
-            else:
-                _lib.check(lib.fno_grid_gather_batch(*args, gh, gw, st), "fno_grid_gather_batch")
+            _gather(self, idx, b, out["inputs"], out["label"], out["mask"], out["case_params"], st)
             if noise_std > 0:
                 self._add_noise(out, idx, noise_std, noise_seed, noise_step, st)
         idx.record_stream(torch.cuda.current_stream(dev))
@@ -121,7 +115,7 @@ class DeviceFrames:
         a case boundary or bad noise arguments (as `batch`); IndexError for a window that runs past the split."""
         from . import _lib
         noise_std = check_noise_args(noise_std, noise_seed, noise_step)
-        lib = _lib.load()
+        _lib.load()   # a missing library raises before any device work
         s = self.time_step_size if time_step_size is None else time_step_size
         if isinstance(steps, bool) or not isinstance(steps, (int, np.integer)) or steps < 1:
             raise ValueError(f"steps must be a positive int, got {steps!r}")
@@ -144,16 +138,10 @@ class DeviceFrames:
         out = dict(inputs=torch.empty(b, 2, gh, gw, device=dev), label=torch.empty(b, 2, gh, gw, device=dev),
                    mask=torch.empty(b, 1, gh, gw, device=dev), case_params=torch.empty(b, p, device=dev),
                    labels=torch.empty(int(steps), b, 2, gh, gw, device=dev))
-        args = (self.frames_in.data_ptr(), self.frames_out.data_ptr(), self.case_table.data_ptr(), self.case_ids.data_ptr(),
-                idx.data_ptr(), b, p, _lib.ACT_BF16 if self.frame_dtype == torch.bfloat16 else _lib.ACT_F32,
-                out["inputs"].data_ptr(), out["label"].data_ptr(), out["mask"].data_ptr(), out["case_params"].data_ptr(),
-                int(steps), int(s), self.n, out["labels"].data_ptr())
         with torch.cuda.device(dev):
             st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-            if (gh, gw) == (64, 64):
-                _lib.check(lib.fno_gather_window(*args, st), "fno_gather_window")
-            else:
-                _lib.check(lib.fno_grid_gather_window(*args, gh, gw, st), "fno_grid_gather_window")
+            _gather(self, idx, b, out["inputs"], out["label"], out["mask"], out["case_params"], st,
+                    window=(int(steps), int(s), out["labels"]))
             if noise_std > 0:
                 self._add_noise(out, idx, noise_std, noise_seed, noise_step, st)
         idx.record_stream(torch.cuda.current_stream(dev))
@@ -167,6 +155,31 @@ class DeviceFrames:
         """Batches in exactly the order `DataLoader(dataset, batch_size, shuffle, generator=generator)` visits them:
         the index stream comes from the same torch samplers the DataLoader builds (`index_batches`)."""
         return self.batches(index_batches(self.n, batch_size, shuffle, generator, drop_last))
+
+
+def _gather(frames: DeviceFrames, idx: Tensor, b: int, inputs: Tensor, label: Optional[Tensor], mask: Tensor,
+            case_params: Tensor, st, window: tuple = ()) -> None:
+    """One launch that gathers samples idx[:b] of `frames` into the batch buffers, chosen by the frames' shape:
+    fno_gather_batch on 64x64 frames, fno_grid_gather_batch on any other grid.  window = (steps, time_step_size, labels)
+    gathers the windows that start there (fno_[grid_]gather_window), each step's masked target into `labels`; `label`
+    may then be None."""
+    from . import _lib
+    args = (frames.frames_in.data_ptr(), frames.frames_out.data_ptr(), frames.case_table.data_ptr(),
+            frames.case_ids.data_ptr(), idx.data_ptr(), b, frames.n_case_params,
+            _lib.ACT_BF16 if frames.frame_dtype == torch.bfloat16 else _lib.ACT_F32, inputs.data_ptr(),
+            None if label is None else label.data_ptr(), mask.data_ptr(), case_params.data_ptr())
+    name = "gather_batch"
+    if window:
+        steps, s, labels = window
+        args += (steps, s, frames.n, labels.data_ptr())
+        name = "gather_window"
+    lib, gh, gw = _lib.load(), frames.height, frames.width
+    if (gh, gw) == (64, 64):
+        name = "fno_" + name
+        _lib.check(getattr(lib, name)(*args, st), name)
+    else:
+        name = "fno_grid_" + name
+        _lib.check(getattr(lib, name)(*args, gh, gw, st), name)
 
 
 def check_noise_args(noise_std, noise_seed, noise_step=0, std_name: str = "noise_std") -> float:

@@ -21,8 +21,9 @@ every parameter frozen.
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
-from typing import Dict, List, Optional
+from typing import Dict, List, NamedTuple, Optional
 
 import numpy as np
 import torch
@@ -77,6 +78,71 @@ def _ptr(t: Optional[Tensor]) -> int:
     return 0 if t is None else t.data_ptr()
 
 
+def capture_graph(run) -> torch.cuda.CUDAGraph:
+    """A CUDA graph of the launches `run()` issues on the current stream.  capture_begin / capture_end directly: the
+    torch.cuda.graph() context manager also runs gc.collect() and empty_cache(), which turns the caller's next
+    allocation into a multi-millisecond cudaMalloc.  Nothing is allocated during a capture (all buffers are static), so
+    no private pool is needed."""
+    graph = torch.cuda.CUDAGraph()
+    graph.capture_begin(capture_error_mode="thread_local")
+    try:
+        run()
+    finally:
+        graph.capture_end()
+    return graph
+
+
+@contextlib.contextmanager
+def side_stream(device):
+    """Run the block (warm-ups and captures) on a new stream that starts after the current stream's work; the current
+    stream then waits for it."""
+    cur = torch.cuda.current_stream(device)
+    side = torch.cuda.Stream(device=device)
+    side.wait_stream(cur)
+    with torch.cuda.stream(side):
+        yield
+    cur.wait_stream(side)
+
+
+class _Route(NamedTuple):
+    """The kernels that run (gh, gw) frames (`Fno2d._route`): the 64x64 kernels (fno_X, either storage mode) or the
+    grid-generic fp32 kernels (fno_grid_X).  The two take the same arguments in the same order except the tail: (batch,
+    act_dtype, stream) for 64x64, (batch, h, w, stream) for grids."""
+    gh: int
+    gw: int
+    grid: bool
+    act: int   # ACT_F32 on the grid route
+
+    @property
+    def act_dtype(self) -> torch.dtype:
+        return torch.bfloat16 if self.act == _lib.ACT_BF16 else torch.float32
+
+    def call(self, name: str, *args) -> None:
+        """fno_<name> or fno_grid_<name> on `args`: the shared arguments, then batch and stream.  "backward" is
+        fno_backward_inputs on 64x64 (with null d_inputs and d_case_params it issues exactly fno_backward's launches)."""
+        lib = _lib.load()
+        *head, stream = args
+        if self.grid:
+            fn = "fno_grid_" + name
+            status = getattr(lib, fn)(*head, self.gh, self.gw, stream)
+        else:
+            fn = "fno_backward_inputs" if name == "backward" else "fno_" + name
+            status = getattr(lib, fn)(*head, self.act, stream)
+        _lib.check(status, fn)
+
+    def bwd_partials_bytes(self) -> int:
+        lib = _lib.load()
+        return lib.fno_grid_bwd_partials_bytes(self.gh, self.gw) if self.grid else lib.fno_bwd_partials_bytes()
+
+
+def _refuse_mask_grad(mask: Tensor) -> None:
+    if mask.requires_grad:
+        # the masked projection keeps no unmasked output, so dL/dmask cannot be formed -- say so instead of silently
+        # returning None
+        raise NotImplementedError("cfdbench_b200.Fno2d: gradients w.r.t. the mask are not implemented (inputs, "
+                                  "case_params and parameters are differentiable)")
+
+
 class _TrainFn(torch.autograd.Function):
     """One autograd node for the whole network: forward = fno_forward_train, backward = fno_backward_inputs (parameter
     gradients and / or the gradients w.r.t. inputs / case_params).  Every call keeps its own saved activations, so
@@ -84,11 +150,7 @@ class _TrainFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, model: "Fno2d", inputs: Tensor, mask: Tensor, case_params: Tensor, *params: Tensor):
-        if mask.requires_grad:
-            # the masked projection keeps no unmasked output, so dL/dmask cannot be formed -- say so instead of
-            # silently returning None
-            raise NotImplementedError("cfdbench_b200.Fno2d: gradients w.r.t. the mask are not implemented (inputs, "
-                                      "case_params and parameters are differentiable)")
+        _refuse_mask_grad(mask)
         preds, saved = model._native_forward_train(inputs, mask, case_params)
         ctx.model = model
         ctx.saved_native = saved
@@ -122,9 +184,7 @@ class _RolloutFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, model: "Fno2d", inputs: Tensor, mask: Tensor, case_params: Tensor, steps: int, *params: Tensor):
-        if mask.requires_grad:
-            raise NotImplementedError("cfdbench_b200.Fno2d: gradients w.r.t. the mask are not implemented (inputs, "
-                                      "case_params and parameters are differentiable)")
+        _refuse_mask_grad(mask)
         seq = model._native_rollout_train(inputs, mask, case_params, steps)
         ctx.model, ctx.steps = model, steps
         ctx.save_for_backward(inputs, mask, case_params, seq)
@@ -246,9 +306,6 @@ class Fno2d(AutoCfdModel):
     def _act_code(self) -> int:
         return _lib.ACT_BF16 if self.act_dtype == "bfloat16" else _lib.ACT_F32
 
-    def _act_torch_dtype(self):
-        return torch.bfloat16 if self.act_dtype == "bfloat16" else torch.float32
-
     def _require_cuda(self):
         if self.device.type != "cuda":
             raise _lib.FnoNativeError(
@@ -256,6 +313,11 @@ class Fno2d(AutoCfdModel):
 
     def _stream(self) -> C.c_void_p:
         return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+
+    def _needs_grad(self, *tensors: Tensor) -> bool:
+        """Whether a call on `tensors` has to build an autograd graph."""
+        return torch.is_grad_enabled() and (any(t.requires_grad for t in tensors)
+                                            or any(p.requires_grad for p in self.parameters()))
 
     def _pack(self, need_bwd: bool = False) -> dict:
         """(Re)build kernel-layout weights when any parameter changed (version counters / pointers)."""
@@ -290,6 +352,7 @@ class Fno2d(AutoCfdModel):
             w.fc2_w, w.fc2_b = self.fc2.weight.data_ptr(), self.fc2.bias.data_ptr()
             w.gx, w.gy = pk["gx"].data_ptr(), pk["gy"].data_ptr()
             pk["struct"] = w
+            pk["coords"] = {(H, W): (w, pk["gx"], pk["gy"])}   # (gh, gw) -> (struct, gx, gy), see _coords
             self._packed, self._pack_key = pk, key
             self._graphs.clear()
         if need_bwd and pk.get("wkT") is None:
@@ -314,23 +377,28 @@ class Fno2d(AutoCfdModel):
                    "fno_pack_mix_operand_from_weights")
         return wop
 
-    def _workspace(self, batch: int, slot: int = 0):
-        key = (batch, self.act_dtype, self.device, slot, self.fused_block)
+    def _workspace(self, batch: int, route: Optional[_Route] = None, slot: int = 0):
+        """(FnoWorkspace, bufs) for `batch` samples on the kernels of `route` (default: the 64x64 kernels, whatever
+        generic_grid_at_64 says); `slot` keeps apart 64x64 workspaces of one batch size that are in use together."""
+        route = route or _Route(H, W, False, self._act_code())
+        gh, gw = route.gh, route.gw
+        key = ("grid", batch, gh, gw, self.device) if route.grid else (batch, self.act_dtype, self.device, slot,
+                                                                        self.fused_block)
         ws = self._ws_cache.get(key)
         if ws is None:
             dev = self.device
-            adt = self._act_torch_dtype()
+            adt = route.act_dtype
             bufs = dict(
-                act0=torch.empty(batch, HIDDEN, H, W, dtype=adt, device=dev),
-                act1=torch.empty(batch, HIDDEN, H, W, dtype=adt, device=dev),
+                act0=torch.empty(batch, HIDDEN, gh, gw, dtype=adt, device=dev),
+                act1=torch.empty(batch, HIDDEN, gh, gw, dtype=adt, device=dev),
                 xm=torch.empty(NMODES, batch, HIDDEN, dtype=torch.complex64, device=dev),
                 ym=torch.empty(NMODES, batch, HIDDEN, dtype=torch.complex64, device=dev),
-                z=torch.empty(batch, H, 2 * MODES, HIDDEN, dtype=torch.float32, device=dev),
+                z=torch.empty(batch, gh, 2 * MODES, HIDDEN, dtype=torch.float32, device=dev),
             )
             st = _lib.FnoWorkspace()
             st.act[0], st.act[1] = bufs["act0"].data_ptr(), bufs["act1"].data_ptr()
             st.xm, st.ym, st.z = bufs["xm"].data_ptr(), bufs["ym"].data_ptr(), bufs["z"].data_ptr()
-            if self.act_dtype == "bfloat16" and self.fused_block:
+            if route.act == _lib.ACT_BF16 and self.fused_block:
                 # operand image of the fused output stage (fno_block_fused): inference never touches ym / z then
                 bufs["ym_img"] = torch.empty(_lib.load().fno_ym_image_bytes(batch), dtype=torch.uint8, device=dev)
                 st.ym_img = bufs["ym_img"].data_ptr()
@@ -340,25 +408,31 @@ class Fno2d(AutoCfdModel):
             self._ws_cache[key] = ws
         return ws
 
-    def _check_grid(self, shape) -> tuple:
-        """(H, W) of an input frame: 64x64 runs the 64x64 kernels in either storage mode, any other grid with
-        24 <= H, W <= 128 the grid-generic fp32 kernels."""
-        gh, gw = int(shape[-2]), int(shape[-1])
+    def _route(self, gh: int, gw: int) -> _Route:
+        """The kernels that run (gh, gw) frames: 64x64 runs the 64x64 kernels in either storage mode (the grid-generic
+        kernels with generic_grid_at_64, which cross-checks the two), any other grid with 24 <= H, W <= 128 the
+        grid-generic fp32 kernels.  Raises ValueError for any other grid or a storage mode its kernels do not run."""
+        gh, gw = int(gh), int(gw)
         if (gh, gw) == (H, W):
-            return gh, gw
-        if not (_lib.GRID_MIN <= gh <= _lib.GRID_MAX and _lib.GRID_MIN <= gw <= _lib.GRID_MAX):
-            raise ValueError(f"cfdbench_b200.Fno2d supports {H}x{W} frames and grids with {_lib.GRID_MIN} <= H, W <= "
-                             f"{_lib.GRID_MAX}; got {gh}x{gw}")
-        if self.act_dtype != "float32":
-            raise ValueError(f"cfdbench_b200.Fno2d: act_dtype={self.act_dtype!r} is supported on {H}x{W} frames only; "
-                             f"the {gh}x{gw} grid runs with act_dtype='float32'")
-        return gh, gw
+            if not self.generic_grid_at_64:
+                return _Route(gh, gw, False, self._act_code())
+            if self.act_dtype != "float32":
+                raise ValueError("generic_grid_at_64 needs act_dtype='float32'")
+        else:
+            if not (_lib.GRID_MIN <= gh <= _lib.GRID_MAX and _lib.GRID_MIN <= gw <= _lib.GRID_MAX):
+                raise ValueError(f"cfdbench_b200.Fno2d supports {H}x{W} frames and grids with {_lib.GRID_MIN} <= H, "
+                                 f"W <= {_lib.GRID_MAX}; got {gh}x{gw}")
+            if self.act_dtype != "float32":
+                raise ValueError(f"cfdbench_b200.Fno2d: act_dtype={self.act_dtype!r} is supported on {H}x{W} frames "
+                                 f"only; the {gh}x{gw} grid runs with act_dtype='float32'")
+        return _Route(gh, gw, True, _lib.ACT_F32)
 
     def _prep_inputs(self, inputs: Tensor, case_params: Tensor, mask: Optional[Tensor]):
+        """Inputs, case parameters and the (B, 1, H, W) mask as contiguous float32 device tensors; the mask follows the
+        input's grid, which `_route` checks."""
         if inputs.dim() != 4 or inputs.shape[1] != self.in_chan:
             raise ValueError(f"inputs must be (B,{self.in_chan},H,W); got {tuple(inputs.shape)}")
-        if tuple(inputs.shape[-2:]) != (H, W):
-            return self._prep_inputs_grid(inputs, case_params, mask)
+        gh, gw = self._route(*inputs.shape[-2:])[:2]
         b = inputs.shape[0]
         dev = self.device
         inputs = inputs.to(device=dev, dtype=torch.float32, non_blocking=True).contiguous()
@@ -366,25 +440,7 @@ class Fno2d(AutoCfdModel):
             raise ValueError(f"case_params must be ({b},{self.n_case_params}); got {tuple(case_params.shape)}")
         case_params = case_params.to(device=dev, dtype=torch.float32, non_blocking=True).contiguous()
         if mask is None:
-            mask4 = torch.ones((b, 1, H, W), device=dev)  # reference fno2d.py:197-199
-        else:
-            mask4 = mask.unsqueeze(1) if mask.dim() == 3 else mask
-            if tuple(mask4.shape) != (b, 1, H, W):
-                raise ValueError(f"mask must be (B,{H},{W}) or (B,1,{H},{W}); got {tuple(mask.shape)}")
-            mask4 = mask4.to(device=dev, dtype=torch.float32, non_blocking=True).contiguous()
-        return inputs, case_params, mask4
-
-    def _prep_inputs_grid(self, inputs: Tensor, case_params: Tensor, mask: Optional[Tensor]):
-        """_prep_inputs for a non-64x64 frame: the mask follows the input's grid."""
-        gh, gw = self._check_grid(inputs.shape)
-        b = inputs.shape[0]
-        dev = self.device
-        inputs = inputs.to(device=dev, dtype=torch.float32, non_blocking=True).contiguous()
-        if case_params.shape != (b, self.n_case_params):
-            raise ValueError(f"case_params must be ({b},{self.n_case_params}); got {tuple(case_params.shape)}")
-        case_params = case_params.to(device=dev, dtype=torch.float32, non_blocking=True).contiguous()
-        if mask is None:
-            mask4 = torch.ones((b, 1, gh, gw), device=dev)
+            mask4 = torch.ones((b, 1, gh, gw), device=dev)  # reference fno2d.py:197-199
         else:
             mask4 = mask.unsqueeze(1) if mask.dim() == 3 else mask
             if tuple(mask4.shape) != (b, 1, gh, gw):
@@ -392,104 +448,70 @@ class Fno2d(AutoCfdModel):
             mask4 = mask4.to(device=dev, dtype=torch.float32, non_blocking=True).contiguous()
         return inputs, case_params, mask4
 
-    # ------------------------------------------------------------------------ grid-generic path
-    # Frames other than 64x64 (CFDBench's tube and dam problems: 66x65) run the grid-generic fp32 kernels
-    # (fno_grid_* in the C ABI).  Coordinate tables, workspaces and graphs are keyed by (H, W).
-    def _on_grid_path(self, gh: int, gw: int) -> bool:
-        if (gh, gw) != (H, W):
-            return True
-        if self.generic_grid_at_64 and self.act_dtype != "float32":
-            raise ValueError("generic_grid_at_64 needs act_dtype='float32'")
-        return self.generic_grid_at_64
-
-    def _grid_struct(self, pk: dict, gh: int, gw: int) -> "_lib.FnoWeights":
-        """The packed weight struct with the (gh, gw) coordinate tables (float32(np.linspace(0, 1, n)))."""
-        grids = pk.setdefault("grid", {})
-        ent = grids.get((gh, gw))
+    def _coords(self, pk: dict, gh: int, gw: int) -> tuple:
+        """(weight struct, gx, gy) of (gh, gw) frames: the packed weight struct with coordinate tables
+        float32(np.linspace(0, 1, n)) of the frame's size; on 64x64 pk["struct"] and its own tables."""
+        ent = pk["coords"].get((gh, gw))
         if ent is None:
             gx = torch.tensor(np.linspace(0, 1, gh), dtype=torch.float).to(self.device)
             gy = torch.tensor(np.linspace(0, 1, gw), dtype=torch.float).to(self.device)
             st = _lib.FnoWeights.from_buffer_copy(pk["struct"])
             st.gx, st.gy = gx.data_ptr(), gy.data_ptr()
-            ent = (st, gx, gy)
-            grids[(gh, gw)] = ent
-        return ent[0]
+            ent = pk["coords"][(gh, gw)] = (st, gx, gy)
+        return ent
 
-    def _grid_workspace(self, batch: int, gh: int, gw: int):
-        key = ("grid", batch, gh, gw, self.device)
-        ws = self._ws_cache.get(key)
-        if ws is None:
-            dev = self.device
-            bufs = dict(
-                act0=torch.empty(batch, HIDDEN, gh, gw, dtype=torch.float32, device=dev),
-                act1=torch.empty(batch, HIDDEN, gh, gw, dtype=torch.float32, device=dev),
-                xm=torch.empty(NMODES, batch, HIDDEN, dtype=torch.complex64, device=dev),
-                ym=torch.empty(NMODES, batch, HIDDEN, dtype=torch.complex64, device=dev),
-                z=torch.empty(batch, gh, 2 * MODES, HIDDEN, dtype=torch.float32, device=dev),
-            )
-            st = _lib.FnoWorkspace()
-            st.act[0], st.act[1] = bufs["act0"].data_ptr(), bufs["act1"].data_ptr()
-            st.xm, st.ym, st.z = bufs["xm"].data_ptr(), bufs["ym"].data_ptr(), bufs["z"].data_ptr()
-            ws = (st, bufs)
-            if len(self._ws_cache) > 16:
-                self._ws_cache.clear()
-            self._ws_cache[key] = ws
-        return ws
-
-    # ------------------------------------------------------------------------------ native calls
-    def _native_forward(self, inputs: Tensor, mask4: Tensor, case_params: Tensor) -> Tensor:
-        lib = _lib.load()
-        b = inputs.shape[0]
-        pk = self._pack()
-        gh, gw = inputs.shape[-2:]
-        if self._on_grid_path(gh, gw):
-            ws, _ = self._grid_workspace(b, gh, gw)
-            preds = torch.empty(b, self.out_chan, gh, gw, dtype=torch.float32, device=self.device)
-            _lib.check(lib.fno_grid_forward(C.byref(self._grid_struct(pk, gh, gw)), inputs.data_ptr(), mask4.data_ptr(),
-                                            case_params.data_ptr(), preds.data_ptr(), C.byref(ws), b, gh, gw,
-                                            self._stream()), "fno_grid_forward")
-            return preds
-        ws, _ = self._workspace(b)
-        preds = torch.empty(b, self.out_chan, H, W, dtype=torch.float32, device=self.device)
-        _lib.check(lib.fno_forward(C.byref(pk["struct"]), inputs.data_ptr(), mask4.data_ptr(), case_params.data_ptr(),
-                                   preds.data_ptr(), C.byref(ws), b, self._act_code(), self._stream()), "fno_forward")
-        return preds
-
-    def _native_forward_train(self, inputs: Tensor, mask4: Tensor, case_params: Tensor):
-        lib = _lib.load()
-        b, L, dev = inputs.shape[0], self.num_layers, self.device
-        pk = self._pack(need_bwd=True)
-        gh, gw = inputs.shape[-2:]
-        if self._on_grid_path(gh, gw):
-            ws, _ = self._grid_workspace(b, gh, gw)
-            acts = [torch.empty(b, HIDDEN, gh, gw, dtype=torch.float32, device=dev) for _ in range(L + 1)]
-            pres = [torch.empty(b, HIDDEN, gh, gw, dtype=torch.float32, device=dev) for _ in range(L)]
-            xms = [torch.empty(NMODES, b, HIDDEN, dtype=torch.complex64, device=dev) for _ in range(L)]
-            sv = _lib.FnoTrainSaved()
-            for l in range(L + 1):
-                sv.act[l] = acts[l].data_ptr()
-            for l in range(L):
-                sv.pre[l], sv.xm[l] = pres[l].data_ptr(), xms[l].data_ptr()
-            preds = torch.empty(b, self.out_chan, gh, gw, dtype=torch.float32, device=dev)
-            _lib.check(lib.fno_grid_forward_train(C.byref(self._grid_struct(pk, gh, gw)), inputs.data_ptr(),
-                                                  mask4.data_ptr(), case_params.data_ptr(), preds.data_ptr(), C.byref(sv),
-                                                  C.byref(ws), b, gh, gw, self._stream()), "fno_grid_forward_train")
-            return preds, (sv, acts, pres, xms)
-        ws, _ = self._workspace(b)
-        adt = self._act_torch_dtype()
-        acts = [torch.empty(b, HIDDEN, H, W, dtype=adt, device=dev) for _ in range(L + 1)]
-        pres = [torch.empty(b, HIDDEN, H, W, dtype=torch.float32, device=dev) for _ in range(L)]
+    def _saved_set(self, b: int, route: _Route) -> tuple:
+        """The saved activations of one training forward of `b` samples: (FnoTrainSaved, acts, pres, xms)."""
+        dev, L, gh, gw = self.device, self.num_layers, route.gh, route.gw
+        acts = [torch.empty(b, HIDDEN, gh, gw, dtype=route.act_dtype, device=dev) for _ in range(L + 1)]
+        pres = [torch.empty(b, HIDDEN, gh, gw, dtype=torch.float32, device=dev) for _ in range(L)]
         xms = [torch.empty(NMODES, b, HIDDEN, dtype=torch.complex64, device=dev) for _ in range(L)]
         sv = _lib.FnoTrainSaved()
         for l in range(L + 1):
             sv.act[l] = acts[l].data_ptr()
         for l in range(L):
             sv.pre[l], sv.xm[l] = pres[l].data_ptr(), xms[l].data_ptr()
-        preds = torch.empty(b, self.out_chan, H, W, dtype=torch.float32, device=dev)
-        _lib.check(lib.fno_forward_train(C.byref(pk["struct"]), inputs.data_ptr(), mask4.data_ptr(),
-                                         case_params.data_ptr(), preds.data_ptr(), C.byref(sv), C.byref(ws), b,
-                                         self._act_code(), self._stream()), "fno_forward_train")
-        return preds, (sv, acts, pres, xms)
+        return sv, acts, pres, xms
+
+    def _bwd_scratch(self, b: int, route: _Route) -> tuple:
+        """The backward's scratch for `b` samples: (FnoBwdScratch, bufs = two d buffers, dz1, gm, gwk, partials)."""
+        dev, gh, gw = self.device, route.gh, route.gw
+        bufs = dict(
+            d0=torch.empty(b, HIDDEN, gh, gw, dtype=torch.float32, device=dev),
+            d1=torch.empty(b, HIDDEN, gh, gw, dtype=torch.float32, device=dev),
+            dz1=torch.empty(min(b, _lib.BWD_CHUNK), PROJ, gh, gw, dtype=torch.float32, device=dev),
+            gm=torch.empty(NMODES, b, HIDDEN, dtype=torch.complex64, device=dev),
+            gwk=torch.empty(NMODES, HIDDEN, HIDDEN, dtype=torch.complex64, device=dev),
+            partials=torch.empty(route.bwd_partials_bytes(), dtype=torch.uint8, device=dev),
+        )
+        sc = _lib.FnoBwdScratch()
+        sc.d[0], sc.d[1] = bufs["d0"].data_ptr(), bufs["d1"].data_ptr()
+        sc.dz1, sc.gm, sc.gwk = bufs["dz1"].data_ptr(), bufs["gm"].data_ptr(), bufs["gwk"].data_ptr()
+        sc.partials = bufs["partials"].data_ptr()
+        return sc, bufs
+
+    # ------------------------------------------------------------------------------ native calls
+    def _native_forward(self, inputs: Tensor, mask4: Tensor, case_params: Tensor) -> Tensor:
+        b = inputs.shape[0]
+        pk = self._pack()
+        route = self._route(*inputs.shape[-2:])
+        ws, _ = self._workspace(b, route)
+        preds = torch.empty(b, self.out_chan, route.gh, route.gw, dtype=torch.float32, device=self.device)
+        route.call("forward", C.byref(self._coords(pk, route.gh, route.gw)[0]), inputs.data_ptr(), mask4.data_ptr(),
+                   case_params.data_ptr(), preds.data_ptr(), C.byref(ws), b, self._stream())
+        return preds
+
+    def _native_forward_train(self, inputs: Tensor, mask4: Tensor, case_params: Tensor):
+        b = inputs.shape[0]
+        pk = self._pack(need_bwd=True)
+        route = self._route(*inputs.shape[-2:])
+        ws, _ = self._workspace(b, route)
+        saved = self._saved_set(b, route)
+        preds = torch.empty(b, self.out_chan, route.gh, route.gw, dtype=torch.float32, device=self.device)
+        route.call("forward_train", C.byref(self._coords(pk, route.gh, route.gw)[0]), inputs.data_ptr(),
+                   mask4.data_ptr(), case_params.data_ptr(), preds.data_ptr(), C.byref(saved[0]), C.byref(ws), b,
+                   self._stream())
+        return preds, saved
 
     def _grad_layout(self):
         """(name, param, offset, n_real) for one flat float32 gradient buffer, parameter order."""
@@ -529,92 +551,56 @@ class Fno2d(AutoCfdModel):
             d_cp = None   # a (B, 0) gradient: nothing to write
         if not want_params and d_inputs is None and d_cp is None:
             return None
-        lib = _lib.load()
-        sv, acts, pres, xms = saved_native
-        b, L, dev = inputs.shape[0], self.num_layers, self.device
+        b = inputs.shape[0]
         pk = self._pack(need_bwd=True)
-        gh, gw = inputs.shape[-2:]
-        grid = self._on_grid_path(gh, gw)
-        ws, _ = self._grid_workspace(b, gh, gw) if grid else self._workspace(b)
-        g = None
+        route = self._route(*inputs.shape[-2:])
+        ws, _ = self._workspace(b, route)
+        flat = views = g = None
         if want_params:
             flat, views, g = self._grad_buffers()
-        d0 = torch.empty(b, HIDDEN, gh, gw, dtype=torch.float32, device=dev)
-        d1 = torch.empty(b, HIDDEN, gh, gw, dtype=torch.float32, device=dev)
-        dz1 = torch.empty(min(b, _lib.BWD_CHUNK), PROJ, gh, gw, dtype=torch.float32, device=dev)
-        gm = torch.empty(NMODES, b, HIDDEN, dtype=torch.complex64, device=dev)
-        gwk = torch.empty(NMODES, HIDDEN, HIDDEN, dtype=torch.complex64, device=dev)
-        sc = _lib.FnoBwdScratch()
-        sc.d[0], sc.d[1] = d0.data_ptr(), d1.data_ptr()
-        sc.dz1, sc.gm, sc.gwk = dz1.data_ptr(), gm.data_ptr(), gwk.data_ptr()
-        nbytes = lib.fno_grid_bwd_partials_bytes(gh, gw) if grid else lib.fno_bwd_partials_bytes()
-        partials = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-        sc.partials = partials.data_ptr()
-        g_arg = C.byref(g) if g is not None else None
-        if grid:
-            _lib.check(lib.fno_grid_backward(C.byref(self._grid_struct(pk, gh, gw)), C.byref(pk["struct_bwd"]),
-                                             inputs.data_ptr(), mask4.data_ptr(), case_params.data_ptr(), dpreds.data_ptr(),
-                                             C.byref(sv), g_arg, C.byref(sc), C.byref(ws), _ptr(d_inputs), _ptr(d_cp), b,
-                                             gh, gw, self._stream()), "fno_grid_backward")
-        else:
-            _lib.check(lib.fno_backward_inputs(C.byref(pk["struct"]), C.byref(pk["struct_bwd"]), inputs.data_ptr(),
-                                               mask4.data_ptr(), case_params.data_ptr(), dpreds.data_ptr(), C.byref(sv),
-                                               g_arg, C.byref(sc), C.byref(ws), _ptr(d_inputs), _ptr(d_cp), b,
-                                               self._act_code(), self._stream()), "fno_backward_inputs")
+        sc, scratch = self._bwd_scratch(b, route)   # `scratch` holds the tensors `sc` points into
+        route.call("backward", C.byref(self._coords(pk, route.gh, route.gw)[0]), C.byref(pk["struct_bwd"]),
+                   inputs.data_ptr(), mask4.data_ptr(), case_params.data_ptr(), dpreds.data_ptr(),
+                   C.byref(saved_native[0]), C.byref(g) if g is not None else None, C.byref(sc), C.byref(ws),
+                   _ptr(d_inputs), _ptr(d_cp), b, self._stream())
         if g is None:   # data-only backward: no parameter gradients, nothing to all-reduce
             return None
-        if self._dp_enabled:   # one all-reduce (NCCL: ReduceOp.AVG, no division kernel) of the whole flat buffer
+        return self._grad_result(flat, views)
+
+    def _grad_result(self, flat: Tensor, views: Dict[str, Tensor]) -> List[Tensor]:
+        """The parameter gradients in parameter order, after one all-reduce (NCCL: ReduceOp.AVG, no division kernel) of
+        the whole flat buffer when data parallel is enabled."""
+        if self._dp_enabled:
             from .dp import allreduce_mean_
             allreduce_mean_(flat, self._dp_group)
         return [views[name] for name, _ in self.named_parameters()]
 
     # ---------------------------------------------------------------- training through a rollout (`rollout`)
-    def _rollout_state(self, b: int, gh: int, gw: int, grid: bool) -> dict:
+    def _rollout_state(self, b: int, route: _Route) -> dict:
         """The buffers `rollout` reuses across steps and calls: one saved set, the backward scratch (two d buffers,
         dz1, gm, gwk, partials) and the carry frame."""
-        key = ("rollout_train", b, gh, gw, grid, self.act_dtype, self.device)
+        key = ("rollout_train", b, route.gh, route.gw, route.grid, self.act_dtype, self.device)
         st = self._ws_cache.get(key)
         if st is None:
-            st = self._train_state(b, gh, gw, grid)
-            st["bufs"]["carry"] = torch.empty(b, self.out_chan, gh, gw, dtype=torch.float32, device=self.device)
+            st = self._train_state(b, route)
+            st["bufs"]["carry"] = torch.empty(b, self.out_chan, route.gh, route.gw, dtype=torch.float32,
+                                              device=self.device)
             if len(self._ws_cache) > 16:
                 self._ws_cache.clear()
             self._ws_cache[key] = st
         return st
 
-    def _train_state(self, b: int, gh: int, gw: int, grid: bool) -> dict:
+    def _train_state(self, b: int, route: _Route) -> dict:
         """One saved set and the backward scratch of a training step of batch `b` (not cached): dict(sv=FnoTrainSaved,
         sc=FnoBwdScratch, bufs=the scratch tensors, saved=(acts, pres, xms)).  Any batch up to `b` can run on them."""
-        lib = _lib.load()
-        dev, L = self.device, self.num_layers
-        adt = torch.float32 if grid else self._act_torch_dtype()
-        acts = [torch.empty(b, HIDDEN, gh, gw, dtype=adt, device=dev) for _ in range(L + 1)]
-        pres = [torch.empty(b, HIDDEN, gh, gw, dtype=torch.float32, device=dev) for _ in range(L)]
-        xms = [torch.empty(NMODES, b, HIDDEN, dtype=torch.complex64, device=dev) for _ in range(L)]
-        sv = _lib.FnoTrainSaved()
-        for l in range(L + 1):
-            sv.act[l] = acts[l].data_ptr()
-        for l in range(L):
-            sv.pre[l], sv.xm[l] = pres[l].data_ptr(), xms[l].data_ptr()
-        nbytes = lib.fno_grid_bwd_partials_bytes(gh, gw) if grid else lib.fno_bwd_partials_bytes()
-        bufs = dict(
-            d0=torch.empty(b, HIDDEN, gh, gw, dtype=torch.float32, device=dev),
-            d1=torch.empty(b, HIDDEN, gh, gw, dtype=torch.float32, device=dev),
-            dz1=torch.empty(min(b, _lib.BWD_CHUNK), PROJ, gh, gw, dtype=torch.float32, device=dev),
-            gm=torch.empty(NMODES, b, HIDDEN, dtype=torch.complex64, device=dev),
-            gwk=torch.empty(NMODES, HIDDEN, HIDDEN, dtype=torch.complex64, device=dev),
-            partials=torch.empty(nbytes, dtype=torch.uint8, device=dev),
-        )
-        sc = _lib.FnoBwdScratch()
-        sc.d[0], sc.d[1] = bufs["d0"].data_ptr(), bufs["d1"].data_ptr()
-        sc.dz1, sc.gm, sc.gwk = bufs["dz1"].data_ptr(), bufs["gm"].data_ptr(), bufs["gwk"].data_ptr()
-        sc.partials = bufs["partials"].data_ptr()
+        sv, acts, pres, xms = self._saved_set(b, route)
+        sc, bufs = self._bwd_scratch(b, route)
         return dict(sv=sv, sc=sc, bufs=bufs, saved=(acts, pres, xms))
 
-    def _static_weights(self, pk: dict, gh: int, gw: int, grid: bool) -> dict:
+    def _static_weights(self, pk: dict, gh: int, gw: int) -> dict:
         """Graph-owned copies of the packed weight images (and coordinate tables) with the weight structs pointing at
         them; the parameters themselves are read in place.  `_refresh_static_weights` copies a new packing in."""
-        src = self._grid_struct(pk, gh, gw) if grid else pk["struct"]
+        src = self._coords(pk, gh, gw)[0]
         wk = [torch.empty_like(t) for t in pk["wk"]]
         w0t = [torch.empty_like(t) for t in pk["w0t"]]
         wkT = [torch.empty_like(t) for t in pk["wkT"]]
@@ -627,19 +613,15 @@ class Fno2d(AutoCfdModel):
         st.gx, st.gy = gx.data_ptr(), gy.data_ptr()
         return dict(struct=st, struct_bwd=sb, dst=wk + w0t + wkT + [gx, gy], src=None)
 
-    def _refresh_static_weights(self, sw: dict, pk: dict, gh: int, gw: int, grid: bool) -> None:
+    def _refresh_static_weights(self, sw: dict, pk: dict, gh: int, gw: int) -> None:
         if sw["src"] is pk:
             return
-        if grid:
-            self._grid_struct(pk, gh, gw)
-            _, gx, gy = pk["grid"][(gh, gw)]
-        else:
-            gx, gy = pk["gx"], pk["gy"]
+        _, gx, gy = self._coords(pk, gh, gw)
         for d, s in zip(sw["dst"], pk["wk"] + pk["w0t"] + pk["wkT"] + [gx, gy]):
             d.copy_(s)
         sw["src"] = pk
 
-    def _train_graph(self, key, pk: dict, gh: int, gw: int, grid: bool, make_io, run, keep) -> dict:
+    def _train_graph(self, key, pk: dict, route: _Route, make_io, run, keep) -> dict:
         """The captured graph of `key` (captured on first use): `make_io()` builds its static buffers, `run(sw, io)`
         issues the native call on them.  Recaptured when a parameter's storage moved."""
         ptrs = tuple(p.data_ptr() for p in self.parameters())
@@ -648,54 +630,39 @@ class Fno2d(AutoCfdModel):
             del self._train_graphs[key]
             ent = None
         if ent is None:
-            sw = self._static_weights(pk, gh, gw, grid)
-            self._refresh_static_weights(sw, pk, gh, gw, grid)
+            sw = self._static_weights(pk, route.gh, route.gw)
+            self._refresh_static_weights(sw, pk, route.gh, route.gw)
             io = make_io()
-            side = torch.cuda.Stream(device=self.device)
-            side.wait_stream(torch.cuda.current_stream(self.device))
-            graph = torch.cuda.CUDAGraph()
-            with torch.cuda.stream(side):
+            with side_stream(self.device):
                 run(sw, io)   # warm-up outside capture (kernel attributes, constant tables)
-                graph.capture_begin(capture_error_mode="thread_local")   # nothing is allocated during the capture
-                try:
-                    run(sw, io)
-                finally:
-                    graph.capture_end()
-            torch.cuda.current_stream(self.device).wait_stream(side)
+                graph = capture_graph(lambda: run(sw, io))
             ent = dict(graph=graph, io=io, sw=sw, ptrs=ptrs, keep=keep)
             while len(self._train_graphs) >= self.max_graphs:   # oldest capture goes first
                 self._train_graphs.pop(next(iter(self._train_graphs)))
             self._train_graphs[key] = ent
-        self._refresh_static_weights(ent["sw"], pk, gh, gw, grid)
+        self._refresh_static_weights(ent["sw"], pk, route.gh, route.gw)
         return ent
 
     def _native_rollout_train(self, inputs: Tensor, mask4: Tensor, case_params: Tensor, steps: int) -> Tensor:
         """preds (steps, B, 2, H, W) from fno_[grid_]rollout_forward_train: the training forward's kernels, so the
         predictions equal those of chained `generate` calls under autograd bit for bit."""
-        lib = _lib.load()
-        b, dev = inputs.shape[0], self.device
-        gh, gw = (int(s) for s in inputs.shape[-2:])
-        grid = self._on_grid_path(gh, gw)
+        b = inputs.shape[0]
+        route = self._route(*inputs.shape[-2:])
+        gh, gw = route.gh, route.gw
         pk = self._pack(need_bwd=True)
-        ws, ws_bufs = self._grid_workspace(b, gh, gw) if grid else self._workspace(b)
-        rs = self._rollout_state(b, gh, gw, grid)
-        seq = torch.empty(steps, b, self.out_chan, gh, gw, dtype=torch.float32, device=dev)
+        ws, ws_bufs = self._workspace(b, route)
+        rs = self._rollout_state(b, route)
+        seq = torch.empty(steps, b, self.out_chan, gh, gw, dtype=torch.float32, device=self.device)
 
         def call(st, x, mk, cp, out):
-            if grid:
-                _lib.check(lib.fno_grid_rollout_forward_train(C.byref(st), x.data_ptr(), mk.data_ptr(), cp.data_ptr(),
-                                                              out.data_ptr(), steps, C.byref(rs["sv"]), C.byref(ws), b, gh,
-                                                              gw, self._stream()), "fno_grid_rollout_forward_train")
-            else:
-                _lib.check(lib.fno_rollout_forward_train(C.byref(st), x.data_ptr(), mk.data_ptr(), cp.data_ptr(),
-                                                         out.data_ptr(), steps, C.byref(rs["sv"]), C.byref(ws), b,
-                                                         self._act_code(), self._stream()), "fno_rollout_forward_train")
+            route.call("rollout_forward_train", C.byref(st), x.data_ptr(), mk.data_ptr(), cp.data_ptr(), out.data_ptr(),
+                       steps, C.byref(rs["sv"]), C.byref(ws), b, self._stream())
         if not self.graph_rollout:
-            call(self._grid_struct(pk, gh, gw) if grid else pk["struct"], inputs, mask4, case_params, seq)
+            call(self._coords(pk, gh, gw)[0], inputs, mask4, case_params, seq)
             return seq
-        key = ("fwd", b, steps, gh, gw, grid, self.act_dtype)
+        key = ("fwd", b, steps, gh, gw, route.grid, self.act_dtype)
         ent = self._train_graph(
-            key, pk, gh, gw, grid,
+            key, pk, route,
             lambda: dict(x=inputs.clone(), mk=mask4.clone(), cp=case_params.clone(), seq=torch.empty_like(seq)),
             lambda sw, io: call(sw["struct"], io["x"], io["mk"], io["cp"], io["seq"]), (ws_bufs, rs))
         io = ent["io"]
@@ -715,35 +682,25 @@ class Fno2d(AutoCfdModel):
             d_cp = None
         if not want_params and d_inputs is None and d_cp is None:
             return None
-        lib = _lib.load()
         b = inputs.shape[0]
-        gh, gw = (int(s) for s in inputs.shape[-2:])
-        grid = self._on_grid_path(gh, gw)
+        route = self._route(*inputs.shape[-2:])
+        gh, gw = route.gh, route.gw
         pk = self._pack(need_bwd=True)
-        ws, ws_bufs = self._grid_workspace(b, gh, gw) if grid else self._workspace(b)
-        rs = self._rollout_state(b, gh, gw, grid)
+        ws, ws_bufs = self._workspace(b, route)
+        rs = self._rollout_state(b, route)
         carry = rs["bufs"]["carry"]
 
         def call(st, sb, x, mk, cp, sq, dsq, g, din, dcp):
-            g_arg = C.byref(g) if g is not None else None
-            if grid:
-                _lib.check(lib.fno_grid_rollout_backward(C.byref(st), C.byref(sb), x.data_ptr(), mk.data_ptr(),
-                                                         cp.data_ptr(), sq.data_ptr(), dsq.data_ptr(), steps,
-                                                         C.byref(rs["sv"]), g_arg, C.byref(rs["sc"]), C.byref(ws),
-                                                         carry.data_ptr(), _ptr(din), _ptr(dcp), b, gh, gw, self._stream()),
-                           "fno_grid_rollout_backward")
-            else:
-                _lib.check(lib.fno_rollout_backward(C.byref(st), C.byref(sb), x.data_ptr(), mk.data_ptr(), cp.data_ptr(),
-                                                    sq.data_ptr(), dsq.data_ptr(), steps, C.byref(rs["sv"]), g_arg,
-                                                    C.byref(rs["sc"]), C.byref(ws), carry.data_ptr(), _ptr(din), _ptr(dcp),
-                                                    b, self._act_code(), self._stream()), "fno_rollout_backward")
+            route.call("rollout_backward", C.byref(st), C.byref(sb), x.data_ptr(), mk.data_ptr(), cp.data_ptr(),
+                       sq.data_ptr(), dsq.data_ptr(), steps, C.byref(rs["sv"]), C.byref(g) if g is not None else None,
+                       C.byref(rs["sc"]), C.byref(ws), carry.data_ptr(), _ptr(din), _ptr(dcp), b, self._stream())
         flat = views = None
         if not self.graph_rollout:
             g = None
             if want_params:
                 flat, views, g = self._grad_buffers()
-            st = self._grid_struct(pk, gh, gw) if grid else pk["struct"]
-            call(st, pk["struct_bwd"], inputs, mask4, case_params, seq, dseq, g, d_inputs, d_cp)
+            call(self._coords(pk, gh, gw)[0], pk["struct_bwd"], inputs, mask4, case_params, seq, dseq, g, d_inputs,
+                 d_cp)
         else:
             def make_io():
                 io = dict(x=inputs.clone(), mk=mask4.clone(), cp=case_params.clone(), seq=torch.empty_like(seq),
@@ -753,9 +710,10 @@ class Fno2d(AutoCfdModel):
                 if want_params:
                     io["flat"], _, io["g"] = self._grad_buffers()
                 return io
-            key = ("bwd", b, steps, gh, gw, grid, self.act_dtype, want_params, d_inputs is not None, d_cp is not None)
+            key = ("bwd", b, steps, gh, gw, route.grid, self.act_dtype, want_params, d_inputs is not None,
+                   d_cp is not None)
             ent = self._train_graph(
-                key, pk, gh, gw, grid, make_io,
+                key, pk, route, make_io,
                 lambda sw, io: call(sw["struct"], sw["struct_bwd"], io["x"], io["mk"], io["cp"], io["seq"], io["dseq"],
                                     io["g"], io["din"], io["dcp"]), (ws_bufs, rs))
             io = ent["io"]
@@ -771,10 +729,7 @@ class Fno2d(AutoCfdModel):
                 flat.copy_(io["flat"])
         if not want_params:
             return None
-        if self._dp_enabled:   # one all-reduce of the whole flat buffer per backward, not one per step
-            from .dp import allreduce_mean_
-            allreduce_mean_(flat, self._dp_group)
-        return [views[name] for name, _ in self.named_parameters()]
+        return self._grad_result(flat, views)   # one all-reduce per backward, not one per step
 
     # -------------------------------------------------------------------------------- public API
     def enable_data_parallel(self, group=None) -> None:
@@ -794,10 +749,8 @@ class Fno2d(AutoCfdModel):
         gives d(preds)/d(inputs) and `generate` can be chained for unrolled training."""
         self._require_cuda()
         inputs, case_params, mask4 = self._prep_inputs(inputs, case_params, mask)
-        needs_grad = torch.is_grad_enabled() and (inputs.requires_grad or case_params.requires_grad or mask4.requires_grad
-                                                  or any(p.requires_grad for p in self.parameters()))
         with torch.cuda.device(self.device):
-            if needs_grad:
+            if self._needs_grad(inputs, case_params, mask4):
                 preds = _TrainFn.apply(self, inputs, mask4, case_params, *self.parameters())
             else:
                 preds = self._native_forward(inputs, mask4, case_params)
@@ -848,37 +801,29 @@ class Fno2d(AutoCfdModel):
             inputs, case_params = inputs.unsqueeze(0), case_params.unsqueeze(0)
             mask = mask.unsqueeze(0) if mask is not None else None
         inputs, case_params, mask4 = self._prep_inputs(inputs, case_params, mask)
-        needs_grad = torch.is_grad_enabled() and (inputs.requires_grad or case_params.requires_grad or mask4.requires_grad
-                                                  or any(p.requires_grad for p in self.parameters()))
         with torch.cuda.device(self.device):
-            if needs_grad:
+            if self._needs_grad(inputs, case_params, mask4):
                 return _RolloutFn.apply(self, inputs, mask4, case_params, steps, *self.parameters())
             with torch.no_grad():
                 return self._native_rollout_train(inputs, mask4, case_params, steps)
 
     def _rollout_device(self, inputs, case_params, mask4, steps) -> Tensor:
-        lib = _lib.load()
         b = inputs.shape[0]
         pk = self._pack()
-        gh, gw = inputs.shape[-2:]
-        grid = self._on_grid_path(gh, gw)
-        ws, ws_bufs = self._grid_workspace(b, gh, gw) if grid else self._workspace(b)
+        route = self._route(*inputs.shape[-2:])
+        gh, gw = route.gh, route.gw
+        ws, ws_bufs = self._workspace(b, route)
         seq = torch.empty(steps, b, self.out_chan, gh, gw, dtype=torch.float32, device=self.device)
+        weights = self._coords(pk, gh, gw)[0]
 
         def rollout(x, mk, cp, out):
-            if grid:
-                _lib.check(lib.fno_grid_rollout(C.byref(self._grid_struct(pk, gh, gw)), x.data_ptr(), mk.data_ptr(),
-                                                cp.data_ptr(), out.data_ptr(), steps, C.byref(ws), b, gh, gw,
-                                                self._stream()), "fno_grid_rollout")
-            else:
-                _lib.check(lib.fno_rollout(C.byref(pk["struct"]), x.data_ptr(), mk.data_ptr(), cp.data_ptr(),
-                                           out.data_ptr(), steps, C.byref(ws), b, self._act_code(), self._stream()),
-                           "fno_rollout")
+            route.call("rollout", C.byref(weights), x.data_ptr(), mk.data_ptr(), cp.data_ptr(), out.data_ptr(), steps,
+                       C.byref(ws), b, self._stream())
         if not self.graph_rollout:
             rollout(inputs, mask4, case_params, seq)
             return seq
         # CUDA-graph replay: static buffers, one capture per (batch, steps[, grid])
-        key = (b, steps, "grid", gh, gw) if grid else (b, steps, self.act_dtype)
+        key = (b, steps, "grid", gh, gw) if route.grid else (b, steps, self.act_dtype)
         ent = self._graphs.get(key)
         if ent is None:
             s_in, s_cp, s_mk = inputs.clone(), case_params.clone(), mask4.clone()
@@ -886,20 +831,9 @@ class Fno2d(AutoCfdModel):
 
             def run():
                 rollout(s_in, s_mk, s_cp, s_seq)
-            side = torch.cuda.Stream(device=self.device)
-            side.wait_stream(torch.cuda.current_stream(self.device))
-            graph = torch.cuda.CUDAGraph()
-            with torch.cuda.stream(side):
+            with side_stream(self.device):
                 run()  # warm-up: sets kernel attributes / builds constant tables outside capture
-                # capture_begin/end directly: the torch.cuda.graph() context manager also runs gc.collect() and
-                # empty_cache(), which turns the caller's next allocation into a multi-millisecond cudaMalloc.
-                # Nothing is allocated during the capture (all buffers are static), so no private pool is needed.
-                graph.capture_begin(capture_error_mode="thread_local")
-                try:
-                    run()
-                finally:
-                    graph.capture_end()
-            torch.cuda.current_stream(self.device).wait_stream(side)
+                graph = capture_graph(run)
             ent = (graph, s_in, s_cp, s_mk, s_seq, ws_bufs, pk)  # the capture holds raw pointers into these
             while len(self._graphs) >= self.max_graphs:  # oldest capture (and its static buffers) goes first
                 self._graphs.pop(next(iter(self._graphs)))
@@ -996,13 +930,7 @@ class Fno2d(AutoCfdModel):
                                                    C.byref(ws), cb, self._act_code(),
                                                    C.c_void_p(s_cmp.cuda_stream)), "fno_forward")
                     run()   # warm-up outside capture (kernel attributes, constant tables)
-                    g = torch.cuda.CUDAGraph()
-                    g.capture_begin(capture_error_mode="thread_local")
-                    try:
-                        run()
-                    finally:
-                        g.capture_end()
-                    graphs.append(g)
+                    graphs.append(capture_graph(run))
             ent["graphs"] = graphs
             s_cmp.synchronize()
         out2 = out.view(b, self.out_chan, H, W)
@@ -1026,8 +954,8 @@ class Fno2d(AutoCfdModel):
         """Host tensors on a non-64x64 grid: upload, device rollout (graph-replayed like device tensors), and a copy into
         a fresh pinned tensor the caller owns."""
         b = inputs.shape[0]
-        gh, gw = self._check_grid(inputs.shape)
-        d_in, d_cp, mask4 = self._prep_inputs_grid(inputs, case_params, mask.reshape(b, gh, gw))
+        gh, gw = self._route(*inputs.shape[-2:])[:2]
+        d_in, d_cp, mask4 = self._prep_inputs(inputs, case_params, mask.reshape(b, gh, gw))
         seq = self._rollout_device(d_in, d_cp, mask4, steps)
         out = torch.empty(steps, b, self.out_chan, gh, gw, dtype=torch.float32, pin_memory=True)
         out.copy_(seq, non_blocking=True)

@@ -227,9 +227,9 @@ def evaluate_auto(model, data, batch_size: int = 2, max_batch: int = 256) -> dic
         raise _lib.FnoNativeError("evaluate_auto has no CPU path: the model must be on a CUDA device")
     if isinstance(data, DeviceFrames) and data.frames_in.device != dev:   # a tensor's device carries its index
         raise ValueError(f"the frames are on {data.frames_in.device}, the model on {dev}")
-    check = getattr(model, "_check_grid", None)
-    if check is not None:   # the drop-in Fno2d's own grid / storage-mode check, before any device work
-        check((gh, gw))
+    route = getattr(model, "_route", None)
+    if route is not None:   # the drop-in Fno2d's own grid / storage-mode check, before any device work
+        route(gh, gw)
     model.eval()
     preds_host = torch.empty(n, 2, gh, gw, dtype=torch.float32, pin_memory=True)   # a normal tensor, as torch.cat gives
     with torch.inference_mode(), torch.cuda.device(dev):

@@ -31,7 +31,8 @@ import numpy as np
 import torch
 
 from . import _lib
-from .data import DeviceFrames, case_table, check_noise_args, index_batches, rollout_windows
+from .data import DeviceFrames, _gather, case_table, check_noise_args, index_batches, rollout_windows
+from .fno2d import capture_graph, side_stream
 
 LOG_COLUMNS = ("mse", "rmse", "mae", "nmse", "mean_l2")   # one row of the epoch log: fno_loss_fwd's five scalars
 
@@ -89,7 +90,7 @@ class _StepGraphs:
         dev = self.dev = model.device
         n, gh, gw = frames.n if n is None else n, frames.height, frames.width
         self.n, self.gh, self.gw, self.stride = n, gh, gw, batch_size
-        self.grid = grid = model._on_grid_path(gh, gw)
+        self.route = route = model._route(gh, gw)
         bmax = min(batch_size, n)
         n_full, rem = divmod(n, batch_size)
         self.sizes = [batch_size] * (n_full > 0) + [rem] * (rem > 0)   # the batch size of each graph
@@ -98,10 +99,10 @@ class _StepGraphs:
         p = frames.n_case_params
 
         pk = model._pack(need_bwd=True)
-        self.sw = model._static_weights(pk, gh, gw, grid)   # graph-owned weight images, refilled by every replay
-        model._refresh_static_weights(self.sw, pk, gh, gw, grid)   # (also fills the coordinate tables)
-        self.ws, self.ws_bufs = model._grid_workspace(bmax, gh, gw) if grid else model._workspace(bmax)
-        self.ts = model._train_state(bmax, gh, gw, grid)
+        self.sw = model._static_weights(pk, gh, gw)   # graph-owned weight images, refilled by every replay
+        model._refresh_static_weights(self.sw, pk, gh, gw)   # (also fills the coordinate tables)
+        self.ws, self.ws_bufs = model._workspace(bmax, route)
+        self.ts = model._train_state(bmax, route)
         self.flat, _, self.grads = model._grad_buffers()
 
         self.io = self._make_io(bmax, gh, gw, p)
@@ -135,22 +136,10 @@ class _StepGraphs:
 
         # capture: a warm-up of every launch except Adam and the log (it updates nothing: parameters, optimizer state
         # and cursor stay as they are), then one capture per batch size
-        cur = torch.cuda.current_stream(dev)
-        side = torch.cuda.Stream(device=dev)
-        side.wait_stream(cur)
-        self.graphs = []
-        with torch.no_grad(), torch.cuda.stream(side):
+        with torch.no_grad(), side_stream(dev):
             for b in self.sizes:
                 self._issue(b, update=False)
-            for b in self.sizes:
-                g = torch.cuda.CUDAGraph()
-                g.capture_begin(capture_error_mode="thread_local")   # nothing is allocated during the capture
-                try:
-                    self._issue(b, update=True)
-                finally:
-                    g.capture_end()
-                self.graphs.append(g)
-        cur.wait_stream(side)
+            self.graphs = [capture_graph(lambda b=b: self._issue(b, update=True)) for b in self.sizes]
 
     def _make_io(self, bmax: int, gh: int, gw: int, p: int) -> dict:
         """The static buffers of the step graphs."""
@@ -172,46 +161,26 @@ class _StepGraphs:
 
     def _issue(self, b: int, update: bool) -> None:
         """One training step of batch b on the static buffers, on the current stream."""
-        lib, model, io, sw = self.lib, self.model, self.io, self.sw
-        gh, gw, grid, p = self.gh, self.gw, self.grid, self.frames.n_case_params
+        lib, io, sw, route = self.lib, self.io, self.sw, self.route
         st = C.c_void_p(torch.cuda.current_stream(self.dev).cuda_stream)
-        fr = self.frames
         self._stage_indices(b, st)
-        args = (fr.frames_in.data_ptr(), fr.frames_out.data_ptr(), fr.case_table.data_ptr(), fr.case_ids.data_ptr(),
-                io["idx"].data_ptr(), b, p, _lib.ACT_BF16 if fr.frame_dtype == torch.bfloat16 else _lib.ACT_F32,
-                io["inputs"].data_ptr(), io["label"].data_ptr(), io["mask"].data_ptr(), io["cp"].data_ptr())
-        if (gh, gw) == (64, 64):
-            _lib.check(lib.fno_gather_batch(*args, st), "fno_gather_batch")
-        else:
-            _lib.check(lib.fno_grid_gather_batch(*args, gh, gw, st), "fno_grid_gather_batch")
+        _gather(self.frames, io["idx"], b, io["inputs"], io["label"], io["mask"], io["cp"], st)
         self._add_noise(b, st)
         self._repack(st)
         inputs, mask, cp = io["inputs"][:b], io["mask"][:b], io["cp"][:b]
         preds, labm, dpreds = io["preds"][:b], io["labm"][:b], io["dpreds"][:b]
         torch.mul(io["label"][:b], mask, out=labm)   # Fno2d.forward's label * mask
         ts, ws = self.ts, self.ws
-        if grid:
-            _lib.check(lib.fno_grid_forward_train(C.byref(sw["struct"]), inputs.data_ptr(), mask.data_ptr(), cp.data_ptr(),
-                                                  preds.data_ptr(), C.byref(ts["sv"]), C.byref(ws), b, gh, gw, st),
-                       "fno_grid_forward_train")
-        else:
-            _lib.check(lib.fno_forward_train(C.byref(sw["struct"]), inputs.data_ptr(), mask.data_ptr(), cp.data_ptr(),
-                                             preds.data_ptr(), C.byref(ts["sv"]), C.byref(ws), b, model._act_code(), st),
-                       "fno_forward_train")
+        route.call("forward_train", C.byref(sw["struct"]), inputs.data_ptr(), mask.data_ptr(), cp.data_ptr(),
+                   preds.data_ptr(), C.byref(ts["sv"]), C.byref(ws), b, st)
         n_el = preds.numel()
         _lib.check(lib.fno_loss_fwd(preds.data_ptr(), labm.data_ptr(), n_el, io["scratch"].data_ptr(), io["loss"].data_ptr(),
                                     st), "fno_loss_fwd")
         _lib.check(lib.fno_loss_bwd(preds.data_ptr(), labm.data_ptr(), io["loss"].data_ptr(), io["gout"].data_ptr(),
                                     dpreds.data_ptr(), n_el, st), "fno_loss_bwd")
-        if grid:
-            _lib.check(lib.fno_grid_backward(C.byref(sw["struct"]), C.byref(sw["struct_bwd"]), inputs.data_ptr(),
-                                             mask.data_ptr(), cp.data_ptr(), dpreds.data_ptr(), C.byref(ts["sv"]),
-                                             C.byref(self.grads), C.byref(ts["sc"]), C.byref(ws), None, None, b, gh, gw,
-                                             st), "fno_grid_backward")
-        else:
-            _lib.check(lib.fno_backward(C.byref(sw["struct"]), C.byref(sw["struct_bwd"]), inputs.data_ptr(), mask.data_ptr(),
-                                        cp.data_ptr(), dpreds.data_ptr(), C.byref(ts["sv"]), C.byref(self.grads),
-                                        C.byref(ts["sc"]), C.byref(ws), b, model._act_code(), st), "fno_backward")
+        route.call("backward", C.byref(sw["struct"]), C.byref(sw["struct_bwd"]), inputs.data_ptr(), mask.data_ptr(),
+                   cp.data_ptr(), dpreds.data_ptr(), C.byref(ts["sv"]), C.byref(self.grads), C.byref(ts["sc"]),
+                   C.byref(ws), None, None, b, st)
         if update:
             self._adam_and_log(io["loss"].data_ptr(), st)
 
@@ -318,54 +287,31 @@ class _RolloutStepGraphs(_StepGraphs):
         return io
 
     def _issue(self, b: int, update: bool) -> None:
-        lib, model, io, sw, fr = self.lib, self.model, self.io, self.sw, self.frames
-        gh, gw, grid, p, k, g = self.gh, self.gw, self.grid, fr.n_case_params, self.k, self.g
+        lib, io, sw, route, k, g = self.lib, self.io, self.sw, self.route, self.k, self.g
         st = C.c_void_p(torch.cuda.current_stream(self.dev).cuda_stream)
         self._stage_indices(b, st)
-        args = (fr.frames_in.data_ptr(), fr.frames_out.data_ptr(), fr.case_table.data_ptr(), fr.case_ids.data_ptr(),
-                io["idx"].data_ptr(), b, p, _lib.ACT_BF16 if fr.frame_dtype == torch.bfloat16 else _lib.ACT_F32,
-                io["inputs"].data_ptr(), None, io["mask"].data_ptr(), io["cp"].data_ptr(), k, self.tss, fr.n,
-                io["labels"].data_ptr())
-        if (gh, gw) == (64, 64):
-            _lib.check(lib.fno_gather_window(*args, st), "fno_gather_window")
-        else:
-            _lib.check(lib.fno_grid_gather_window(*args, gh, gw, st), "fno_grid_gather_window")
+        _gather(self.frames, io["idx"], b, io["inputs"], None, io["mask"], io["cp"], st,
+                window=(k, self.tss, io["labels"]))
         self._add_noise(b, st)
         self._repack(st)
         x, mk, cp = io["inputs"].data_ptr(), io["mask"].data_ptr(), io["cp"].data_ptr()
         preds, labels, dpreds = io["preds"].data_ptr(), io["labels"].data_ptr(), io["dpreds"].data_ptr()
         ts, ws = self.ts, self.ws
-        n_el = b * 2 * gh * gw   # per step
+        n_el = b * 2 * self.gh * self.gw   # per step
         if g < k:   # the pushforward prefix, without gradient; the trained steps start from its last frame
             pre = io["prefix"].data_ptr()
-            if grid:
-                _lib.check(lib.fno_grid_rollout(C.byref(sw["struct"]), x, mk, cp, pre, k - g, C.byref(ws), b, gh, gw, st),
-                           "fno_grid_rollout")
-            else:
-                _lib.check(lib.fno_rollout(C.byref(sw["struct"]), x, mk, cp, pre, k - g, C.byref(ws), b, model._act_code(),
-                                           st), "fno_rollout")
+            route.call("rollout", C.byref(sw["struct"]), x, mk, cp, pre, k - g, C.byref(ws), b, st)
             x = pre + (k - g - 1) * n_el * 4
             labels += (k - g) * n_el * 4
-        if grid:
-            _lib.check(lib.fno_grid_rollout_forward_train(C.byref(sw["struct"]), x, mk, cp, preds, g, C.byref(ts["sv"]),
-                                                          C.byref(ws), b, gh, gw, st), "fno_grid_rollout_forward_train")
-        else:
-            _lib.check(lib.fno_rollout_forward_train(C.byref(sw["struct"]), x, mk, cp, preds, g, C.byref(ts["sv"]),
-                                                     C.byref(ws), b, model._act_code(), st), "fno_rollout_forward_train")
+        route.call("rollout_forward_train", C.byref(sw["struct"]), x, mk, cp, preds, g, C.byref(ts["sv"]), C.byref(ws),
+                   b, st)
         _lib.check(lib.fno_loss_seq_fwd(preds, labels, n_el, g, io["scratch"].data_ptr(), io["loss"].data_ptr(), st),
                    "fno_loss_seq_fwd")
         _lib.check(lib.fno_loss_seq_bwd(preds, labels, io["loss"].data_ptr(), io["gout"].data_ptr(), dpreds, n_el, g, st),
                    "fno_loss_seq_bwd")
-        carry = io["carry"].data_ptr()
-        if grid:
-            _lib.check(lib.fno_grid_rollout_backward(C.byref(sw["struct"]), C.byref(sw["struct_bwd"]), x, mk, cp, preds,
-                                                     dpreds, g, C.byref(ts["sv"]), C.byref(self.grads), C.byref(ts["sc"]),
-                                                     C.byref(ws), carry, None, None, b, gh, gw, st),
-                       "fno_grid_rollout_backward")
-        else:
-            _lib.check(lib.fno_rollout_backward(C.byref(sw["struct"]), C.byref(sw["struct_bwd"]), x, mk, cp, preds, dpreds,
-                                                g, C.byref(ts["sv"]), C.byref(self.grads), C.byref(ts["sc"]), C.byref(ws),
-                                                carry, None, None, b, model._act_code(), st), "fno_rollout_backward")
+        route.call("rollout_backward", C.byref(sw["struct"]), C.byref(sw["struct_bwd"]), x, mk, cp, preds, dpreds, g,
+                   C.byref(ts["sv"]), C.byref(self.grads), C.byref(ts["sc"]), C.byref(ws), io["carry"].data_ptr(), None,
+                   None, b, st)
         if update:
             self._adam_and_log(io["loss"][g].data_ptr(), st)
 
@@ -425,8 +371,7 @@ def _check_split(model, data, what: str) -> None:
     if p != model.n_case_params:
         raise ValueError(f"{what} has {p} case parameters per sample, the model takes n_case_params="
                          f"{model.n_case_params}")
-    model._check_grid((gh, gw))      # the model's own grid / storage-mode checks
-    model._on_grid_path(gh, gw)
+    model._route(gh, gw)      # the model's own grid / storage-mode checks
 
 
 def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, lr: float = 1e-3, lr_step_size: int = 1,

@@ -143,7 +143,7 @@ def main() -> None:
               modes1=12, modes2=12)
     m.load_state_dict({k: torch.from_numpy(v) for k, v in sd.items()})
     pk = m._pack(need_bwd=True)
-    w = m._grid_struct(pk, gh, gw)
+    w = m._coords(pk, gh, gw)[0]
     st = C.c_void_p(torch.cuda.current_stream().cuda_stream)
     a0, a1, pre = (torch.randn(B, 32, gh, gw, device=dev) for _ in range(3))
     xm = torch.empty(288, B, 32, dtype=torch.complex64, device=dev)
