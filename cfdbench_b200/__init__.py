@@ -9,13 +9,14 @@ Public surface mirrors the reference's for this path:
     train_auto                             (reference src/train_auto.py train, steps replayed from CUDA graphs;
                                             rollout_steps=K trains through K-step rollouts)
     rollout_windows                        (the valid K-step window starts of a split)
+    RolloutNoise, add_input_noise          (per-step input noise of Fno2d.rollout, and its eager form)
 """
 from .base_model import AutoCfdModel
 from .loss import MseLoss, loss_name_to_fn
 
 __all__ = ["AutoCfdModel", "MseLoss", "loss_name_to_fn", "Fno2d", "FnoBlock", "SpectralConv2d_fast", "FusedAdam", "DeviceFrames",
            "infer_multistep", "evaluate_auto", "train_auto",
-           "rollout_windows"]
+           "rollout_windows", "RolloutNoise", "add_input_noise"]
 
 
 def __getattr__(name):  # lazy: importing the package must not require the native library
@@ -34,9 +35,9 @@ def __getattr__(name):  # lazy: importing the package must not require the nativ
     if name == "evaluate_auto":
         from .metrics import evaluate_auto
         return evaluate_auto
-    if name == "rollout_windows":
-        from .data import rollout_windows
-        return rollout_windows
+    if name in ("rollout_windows", "RolloutNoise", "add_input_noise"):
+        from . import data
+        return getattr(data, name)
     if name == "train_auto":
         from .train import train_auto
         return train_auto

@@ -80,6 +80,14 @@ class FnoAdamTensors(C.Structure):
                 ("n", C.c_int64 * ADAM_MAX_TENSORS)]
 
 
+class FnoNoise(C.Structure):
+    """fno_noise: the per-step noise of a rollout driver (include/cfdbench_b200.h)."""
+    _fields_ = [("std", C.c_float), ("seed", C.c_uint64), ("idx", C.c_void_p), ("step_base", C.c_void_p),
+                ("step_offset", C.c_void_p), ("k0", C.c_int32)]
+
+
+NOISE_STREAMS = 2 ** 16
+
 _P = C.c_void_p
 _I = C.c_int
 _F = C.c_float
@@ -170,6 +178,24 @@ SIGNATURES = {
     "fno_loss_seq_bwd": (C.c_int, [_P, _P, _P, _P, _P, C.c_size_t, _I, _P]),
     # training noise
     "fno_add_input_noise": (C.c_int, [_P, _P, _P, _I, _I, _I, _F, C.c_uint64, _P, _P, _P]),
+    "fno_add_input_noise_stream": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _F, C.c_uint64, _P, _P, _I, _P]),
+    # noise on every step of a rollout
+    "fno_rollout_noise": (C.c_int, [C.POINTER(FnoWeights), _P, _P, _P, _P, _I, C.POINTER(FnoWorkspace),
+                                    C.POINTER(FnoNoise), _P, _I, _I, _P]),
+    "fno_rollout_forward_train_noise": (C.c_int, [C.POINTER(FnoWeights), _P, _P, _P, _P, _I, C.POINTER(FnoTrainSaved),
+                                                  C.POINTER(FnoWorkspace), C.POINTER(FnoNoise), _P, _I, _I, _P]),
+    "fno_rollout_backward_noise": (C.c_int, [C.POINTER(FnoWeights), C.POINTER(FnoWeightsBwd), _P, _P, _P, _P, _P, _I,
+                                             C.POINTER(FnoTrainSaved), C.POINTER(FnoGrads), C.POINTER(FnoBwdScratch),
+                                             C.POINTER(FnoWorkspace), C.POINTER(FnoNoise), _P, _P, _P, _P, _I, _I, _P]),
+    "fno_grid_rollout_noise": (C.c_int, [C.POINTER(FnoWeights), _P, _P, _P, _P, _I, C.POINTER(FnoWorkspace),
+                                         C.POINTER(FnoNoise), _P, _I, _I, _I, _P]),
+    "fno_grid_rollout_forward_train_noise": (C.c_int, [C.POINTER(FnoWeights), _P, _P, _P, _P, _I,
+                                                       C.POINTER(FnoTrainSaved), C.POINTER(FnoWorkspace),
+                                                       C.POINTER(FnoNoise), _P, _I, _I, _I, _P]),
+    "fno_grid_rollout_backward_noise": (C.c_int, [C.POINTER(FnoWeights), C.POINTER(FnoWeightsBwd), _P, _P, _P, _P, _P, _I,
+                                                  C.POINTER(FnoTrainSaved), C.POINTER(FnoGrads), C.POINTER(FnoBwdScratch),
+                                                  C.POINTER(FnoWorkspace), C.POINTER(FnoNoise), _P, _P, _P, _P, _I, _I,
+                                                  _I, _P]),
 }
 
 GRID_MIN, GRID_MAX = 24, 128

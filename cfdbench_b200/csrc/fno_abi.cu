@@ -88,6 +88,8 @@ cudaError_t launch_loss_seq_bwd(const float*, const float*, const float*, const 
 size_t loss_seq_scratch_bytes(int);
 cudaError_t launch_add_input_noise(float*, const float*, const long long*, int, int, int, float, unsigned long long,
                                    const long long*, const int*, cudaStream_t);
+cudaError_t launch_input_noise_stream(const float*, float*, const float*, const long long*, int, int, int, float,
+                                      unsigned long long, const long long*, const int*, int, cudaStream_t);
 }  // namespace fno
 
 using namespace fno;
@@ -120,6 +122,76 @@ static int fail(int code, const char* what, cudaError_t e = cudaSuccess) {
 
 static inline cudaStream_t S(void* s) { return static_cast<cudaStream_t>(s); }
 static inline bool bad_dtype(int d) { return d != FNO_ACT_F32 && d != FNO_ACT_BF16; }
+
+// ------------------------------------------------------------------------ per-step noise of a rollout (fno_noise)
+// Call step s of a rollout driver is fed x_s (the call's inputs, or the prediction of step s-1).  With a noise descriptor
+// and stream k0 + s >= 1 it is fed fed[s] = x_s + the noise of that stream instead (stream 0, the start frame's noise, is
+// the gather's); fed is [steps][batch][2][h][w] like preds_seq.  nz == NULL: the frame is x_s, as without noise.
+static int noise_args(const char* what, const fno_noise* nz, const float* fed, int steps) {
+  char msg[160];
+  if (!nz || !fed || !nz->idx || !nz->step_base || !(nz->std >= 0.f) || !isfinite(nz->std) || nz->k0 < 0 ||
+      static_cast<long long>(nz->k0) + steps > FNO_NOISE_STREAMS) {
+    snprintf(msg, sizeof(msg), "%s: bad noise argument", what);
+    return fail(kErrArg, msg);
+  }
+  return kOk;
+}
+
+// What the per-step forward of a *_noise forward driver would refuse (fno_[grid_]forward with saved == NULL,
+// fno_[grid_]forward_train otherwise), checked before the driver's first launch: with k0 >= 1 the noise of step 0 runs
+// before step 0's forward, and reads inputs and mask.  Same status codes as the forward: 3 for n_layers, else 1.
+static int noise_forward_args(const char* what, const fno_weights* w, const float* inputs, const float* mask,
+                              const float* case_params, const fno_train_saved* saved, const fno_workspace* ws, int batch,
+                              bool grid, int act_dtype) {
+  char msg[160];
+  bool bad = !w || !inputs || !mask || !ws || batch <= 0 || (!grid && bad_dtype(act_dtype));
+  if (!bad && saved) {
+    bad = !ws->ym || !ws->z;
+  } else if (!bad) {
+    const bool fused = !grid && act_dtype == FNO_ACT_BF16 && ws->ym_img;   // the bf16 inference blocks need no ym / z
+    bad = !ws->act[0] || !ws->act[1] || !ws->xm || (!fused && (!ws->ym || !ws->z));
+  }
+  if (!bad) bad = (w->n_case_params > 0 && !case_params) || (grid && (!w->gx || !w->gy));
+  if (bad) {
+    snprintf(msg, sizeof(msg), "%s: bad argument", what);
+    return fail(kErrArg, msg);
+  }
+  if (w->n_layers < 1 || w->n_layers > FNO_MAX_LAYERS) {
+    snprintf(msg, sizeof(msg), "%s: n_layers out of range", what);
+    return fail(kErrUnsupported, msg);
+  }
+  if (saved) {
+    bool ok = saved->act[0] != nullptr;
+    for (int l = 0; l < w->n_layers; ++l) ok = ok && saved->act[l + 1] && saved->pre[l] && saved->xm[l];
+    if (!ok) {
+      snprintf(msg, sizeof(msg), "%s: null saved buffer", what);
+      return fail(kErrArg, msg);
+    }
+  }
+  return kOk;
+}
+
+static inline bool noisy_step(const fno_noise* nz, int s) { return nz && nz->k0 + s > 0; }
+
+// x = the frame call step s is fed: x itself, or fed[s] written from it (one launch)
+static int feed_step(const fno_noise* nz, float* fed, const float* mask, int s, size_t frame, int batch, int h, int wd,
+                     const float*& x, void* stream) {
+  if (!noisy_step(nz, s)) return kOk;
+  float* out = fed + static_cast<size_t>(s) * frame;
+  FNO_CUDA(launch_input_noise_stream(x, out, mask, reinterpret_cast<const long long*>(nz->idx), batch, h, wd, nz->std,
+                                     nz->seed, reinterpret_cast<const long long*>(nz->step_base),
+                                     reinterpret_cast<const int*>(nz->step_offset), nz->k0 + s, S(stream)),
+           "input_noise_stream_kernel");
+  x = out;
+  return kOk;
+}
+
+// the frame the backward sweep's step s was fed: fed[s] for a noisy step, else the input or the previous prediction
+static inline const float* fed_frame(const fno_noise* nz, const float* fed, const float* inputs, const float* preds_seq, int s,
+                                     size_t frame) {
+  if (noisy_step(nz, s)) return fed + static_cast<size_t>(s) * frame;
+  return s > 0 ? preds_seq + static_cast<size_t>(s - 1) * frame : inputs;
+}
 
 extern "C" {
 
@@ -279,17 +351,38 @@ int fno_forward(const fno_weights* w, const float* inputs, const float* mask, co
   return fno_project_fwd(ws->act[cur], mask, w, preds, batch, act_dtype, stream);
 }
 
-int fno_rollout(const fno_weights* w, const float* inputs, const float* mask, const float* case_params,
-                float* preds_seq, int steps, const fno_workspace* ws, int batch, int act_dtype, void* stream) {
-  if (steps < 0 || !preds_seq) return fail(kErrArg, "fno_rollout: bad argument");
+static int rollout_impl(const char* what, const fno_weights* w, const float* inputs, const float* mask,
+                        const float* case_params, float* preds_seq, int steps, const fno_workspace* ws, const fno_noise* nz,
+                        float* fed, int batch, int act_dtype, void* stream) {
+  char msg[160];
+  if (steps < 0 || !preds_seq) {
+    snprintf(msg, sizeof(msg), "%s: bad argument", what);
+    return fail(kErrArg, msg);
+  }
   const size_t frame = static_cast<size_t>(batch) * 2 * kHW;
   const float* cur = inputs;
   for (int s = 0; s < steps; ++s) {
     float* nxt = preds_seq + static_cast<size_t>(s) * frame;
+    FNO_TRY(feed_step(nz, fed, mask, s, frame, batch, kH, kW, cur, stream));
     FNO_TRY(fno_forward(w, cur, mask, case_params, nxt, ws, batch, act_dtype, stream));
     cur = nxt;
   }
   return kOk;
+}
+
+int fno_rollout(const fno_weights* w, const float* inputs, const float* mask, const float* case_params,
+                float* preds_seq, int steps, const fno_workspace* ws, int batch, int act_dtype, void* stream) {
+  return rollout_impl("fno_rollout", w, inputs, mask, case_params, preds_seq, steps, ws, nullptr, nullptr, batch, act_dtype,
+                      stream);
+}
+
+int fno_rollout_noise(const fno_weights* w, const float* inputs, const float* mask, const float* case_params,
+                      float* preds_seq, int steps, const fno_workspace* ws, const fno_noise* noise, float* fed, int batch,
+                      int act_dtype, void* stream) {
+  FNO_TRY(noise_args("fno_rollout_noise", noise, fed, steps));
+  FNO_TRY(noise_forward_args("fno_rollout_noise", w, inputs, mask, case_params, nullptr, ws, batch, false, act_dtype));
+  return rollout_impl("fno_rollout_noise", w, inputs, mask, case_params, preds_seq, steps, ws, noise, fed, batch, act_dtype,
+                      stream);
 }
 
 size_t fno_rollout_host_scratch_bytes(int batch, int n_case_params, int steps) {
@@ -499,16 +592,71 @@ static int rollout_bwd_args(const char* what, const fno_weights* w, const fno_we
   return kOk;
 }
 
-int fno_rollout_forward_train(const fno_weights* w, const float* inputs, const float* mask, const float* case_params,
-                              float* preds_seq, int steps, const fno_train_saved* saved, const fno_workspace* ws, int batch,
-                              int act_dtype, void* stream) {
-  if (steps < 1 || !inputs || !preds_seq || batch <= 0) return fail(kErrArg, "fno_rollout_forward_train: bad argument");
+static int rollout_forward_train_impl(const char* what, const fno_weights* w, const float* inputs, const float* mask,
+                                      const float* case_params, float* preds_seq, int steps, const fno_train_saved* saved,
+                                      const fno_workspace* ws, const fno_noise* nz, float* fed, int batch, int act_dtype,
+                                      void* stream) {
+  char msg[160];
+  if (steps < 1 || !inputs || !preds_seq || batch <= 0) {
+    snprintf(msg, sizeof(msg), "%s: bad argument", what);
+    return fail(kErrArg, msg);
+  }
   const size_t frame = static_cast<size_t>(batch) * 2 * kHW;
   const float* cur = inputs;
   for (int s = 0; s < steps; ++s) {
     float* nxt = preds_seq + static_cast<size_t>(s) * frame;
+    FNO_TRY(feed_step(nz, fed, mask, s, frame, batch, kH, kW, cur, stream));
     FNO_TRY(fno_forward_train(w, cur, mask, case_params, nxt, saved, ws, batch, act_dtype, stream));
     cur = nxt;
+  }
+  return kOk;
+}
+
+int fno_rollout_forward_train(const fno_weights* w, const float* inputs, const float* mask, const float* case_params,
+                              float* preds_seq, int steps, const fno_train_saved* saved, const fno_workspace* ws, int batch,
+                              int act_dtype, void* stream) {
+  return rollout_forward_train_impl("fno_rollout_forward_train", w, inputs, mask, case_params, preds_seq, steps, saved, ws,
+                                    nullptr, nullptr, batch, act_dtype, stream);
+}
+
+int fno_rollout_forward_train_noise(const fno_weights* w, const float* inputs, const float* mask, const float* case_params,
+                                    float* preds_seq, int steps, const fno_train_saved* saved, const fno_workspace* ws,
+                                    const fno_noise* noise, float* fed, int batch, int act_dtype, void* stream) {
+  FNO_TRY(noise_args("fno_rollout_forward_train_noise", noise, fed, steps));
+  FNO_TRY(noise_forward_args("fno_rollout_forward_train_noise", w, inputs, mask, case_params, saved, ws, batch, false,
+                             act_dtype));
+  return rollout_forward_train_impl("fno_rollout_forward_train_noise", w, inputs, mask, case_params, preds_seq, steps, saved,
+                                    ws, noise, fed, batch, act_dtype, stream);
+}
+
+static int rollout_backward_impl(const char* what, const fno_weights* w, const fno_weights_bwd* wb, const float* inputs,
+                                 const float* mask, const float* case_params, const float* preds_seq, const float* dpreds_seq,
+                                 int steps, const fno_train_saved* saved, const fno_grads* grads, const fno_bwd_scratch* scratch,
+                                 const fno_workspace* ws, const fno_noise* nz, const float* fed, float* carry, float* d_inputs,
+                                 float* d_case_params, int batch, int act_dtype, void* stream) {
+  char msg[160];
+  if (w && w->n_case_params == 0) d_case_params = nullptr;   // nothing to write
+  FNO_TRY(rollout_bwd_args(what, w, wb, inputs, mask, preds_seq, dpreds_seq, steps, saved, grads, scratch, ws, carry, d_inputs,
+                           d_case_params, batch));
+  if (bad_dtype(act_dtype)) {
+    snprintf(msg, sizeof(msg), "%s: bad act_dtype", what);
+    return fail(kErrArg, msg);
+  }
+  if ((reinterpret_cast<uintptr_t>(d_inputs) | reinterpret_cast<uintptr_t>(carry) | reinterpret_cast<uintptr_t>(dpreds_seq)) & 15) {
+    snprintf(msg, sizeof(msg), "%s: d_inputs, carry and dpreds_seq must be 16-byte aligned", what);
+    return fail(kErrArg, msg);
+  }
+  const size_t frame = static_cast<size_t>(batch) * 2 * kHW;
+  if (d_case_params)   // every sweep step adds its share
+    FNO_CUDA(cudaMemsetAsync(d_case_params, 0, static_cast<size_t>(batch) * w->n_case_params * sizeof(float), S(stream)),
+             "memset(d_case_params)");
+  for (int s = steps - 1; s >= 0; --s) {
+    const float* x = fed_frame(nz, fed, inputs, preds_seq, s, frame);
+    FNO_TRY(forward_train_body(w, x, mask, case_params, saved, ws, batch, act_dtype, stream));
+    const float* up = s == steps - 1 ? dpreds_seq + static_cast<size_t>(s) * frame : carry;
+    FNO_TRY(backward_impl(what, w, wb, x, mask, case_params, up, saved, grads, scratch, ws, batch, act_dtype, stream,
+                          s > 0 ? carry : d_inputs, d_case_params, s != steps - 1 ? 1 : 0, 1,
+                          s > 0 ? dpreds_seq + static_cast<size_t>(s - 1) * frame : nullptr));
   }
   return kOk;
 }
@@ -518,26 +666,19 @@ int fno_rollout_backward(const fno_weights* w, const fno_weights_bwd* wb, const 
                          const fno_train_saved* saved, const fno_grads* grads, const fno_bwd_scratch* scratch,
                          const fno_workspace* ws, float* carry, float* d_inputs, float* d_case_params, int batch, int act_dtype,
                          void* stream) {
-  const char* what = "fno_rollout_backward";
-  if (w && w->n_case_params == 0) d_case_params = nullptr;   // nothing to write
-  FNO_TRY(rollout_bwd_args(what, w, wb, inputs, mask, preds_seq, dpreds_seq, steps, saved, grads, scratch, ws, carry, d_inputs,
-                           d_case_params, batch));
-  if (bad_dtype(act_dtype)) return fail(kErrArg, "fno_rollout_backward: bad act_dtype");
-  if ((reinterpret_cast<uintptr_t>(d_inputs) | reinterpret_cast<uintptr_t>(carry) | reinterpret_cast<uintptr_t>(dpreds_seq)) & 15)
-    return fail(kErrArg, "fno_rollout_backward: d_inputs, carry and dpreds_seq must be 16-byte aligned");
-  const size_t frame = static_cast<size_t>(batch) * 2 * kHW;
-  if (d_case_params)   // every sweep step adds its share
-    FNO_CUDA(cudaMemsetAsync(d_case_params, 0, static_cast<size_t>(batch) * w->n_case_params * sizeof(float), S(stream)),
-             "memset(d_case_params)");
-  for (int s = steps - 1; s >= 0; --s) {
-    const float* x = s > 0 ? preds_seq + static_cast<size_t>(s - 1) * frame : inputs;
-    FNO_TRY(forward_train_body(w, x, mask, case_params, saved, ws, batch, act_dtype, stream));
-    const float* up = s == steps - 1 ? dpreds_seq + static_cast<size_t>(s) * frame : carry;
-    FNO_TRY(backward_impl(what, w, wb, x, mask, case_params, up, saved, grads, scratch, ws, batch, act_dtype, stream,
-                          s > 0 ? carry : d_inputs, d_case_params, s != steps - 1 ? 1 : 0, 1,
-                          s > 0 ? dpreds_seq + static_cast<size_t>(s - 1) * frame : nullptr));
-  }
-  return kOk;
+  return rollout_backward_impl("fno_rollout_backward", w, wb, inputs, mask, case_params, preds_seq, dpreds_seq, steps, saved,
+                               grads, scratch, ws, nullptr, nullptr, carry, d_inputs, d_case_params, batch, act_dtype, stream);
+}
+
+int fno_rollout_backward_noise(const fno_weights* w, const fno_weights_bwd* wb, const float* inputs, const float* mask,
+                               const float* case_params, const float* preds_seq, const float* dpreds_seq, int steps,
+                               const fno_train_saved* saved, const fno_grads* grads, const fno_bwd_scratch* scratch,
+                               const fno_workspace* ws, const fno_noise* noise, const float* fed, float* carry,
+                               float* d_inputs, float* d_case_params, int batch, int act_dtype, void* stream) {
+  FNO_TRY(noise_args("fno_rollout_backward_noise", noise, fed, steps));
+  return rollout_backward_impl("fno_rollout_backward_noise", w, wb, inputs, mask, case_params, preds_seq, dpreds_seq, steps,
+                               saved, grads, scratch, ws, noise, fed, carry, d_inputs, d_case_params, batch, act_dtype,
+                               stream);
 }
 
 int fno_multistep_metrics(const float* preds_seq, const float* label_u, const float* mask, float* sums, int steps,
@@ -812,18 +953,40 @@ int fno_grid_forward(const fno_weights* w, const float* inputs, const float* mas
   return fno_grid_project_fwd(act[cur], mask, w, preds, batch, h, wd, stream);
 }
 
-int fno_grid_rollout(const fno_weights* w, const float* inputs, const float* mask, const float* case_params, float* preds_seq,
-                     int steps, const fno_workspace* ws, int batch, int h, int wd, void* stream) {
-  FNO_TRY(grid_arg("fno_grid_rollout", h, wd));
-  if (steps < 0 || !preds_seq || batch <= 0) return fail(kErrArg, "fno_grid_rollout: bad argument");
+static int grid_rollout_impl(const char* what, const fno_weights* w, const float* inputs, const float* mask,
+                             const float* case_params, float* preds_seq, int steps, const fno_workspace* ws,
+                             const fno_noise* nz, float* fed, int batch, int h, int wd, void* stream) {
+  char msg[160];
+  FNO_TRY(grid_arg(what, h, wd));
+  if (steps < 0 || !preds_seq || batch <= 0) {
+    snprintf(msg, sizeof(msg), "%s: bad argument", what);
+    return fail(kErrArg, msg);
+  }
   const size_t frame = static_cast<size_t>(batch) * 2 * h * wd;
   const float* cur = inputs;
   for (int s = 0; s < steps; ++s) {
     float* nxt = preds_seq + static_cast<size_t>(s) * frame;
+    FNO_TRY(feed_step(nz, fed, mask, s, frame, batch, h, wd, cur, stream));
     FNO_TRY(fno_grid_forward(w, cur, mask, case_params, nxt, ws, batch, h, wd, stream));
     cur = nxt;
   }
   return kOk;
+}
+
+int fno_grid_rollout(const fno_weights* w, const float* inputs, const float* mask, const float* case_params, float* preds_seq,
+                     int steps, const fno_workspace* ws, int batch, int h, int wd, void* stream) {
+  return grid_rollout_impl("fno_grid_rollout", w, inputs, mask, case_params, preds_seq, steps, ws, nullptr, nullptr, batch, h,
+                           wd, stream);
+}
+
+int fno_grid_rollout_noise(const fno_weights* w, const float* inputs, const float* mask, const float* case_params,
+                           float* preds_seq, int steps, const fno_workspace* ws, const fno_noise* noise, float* fed,
+                           int batch, int h, int wd, void* stream) {
+  FNO_TRY(grid_arg("fno_grid_rollout_noise", h, wd));
+  FNO_TRY(noise_args("fno_grid_rollout_noise", noise, fed, steps));
+  FNO_TRY(noise_forward_args("fno_grid_rollout_noise", w, inputs, mask, case_params, nullptr, ws, batch, true, 0));
+  return grid_rollout_impl("fno_grid_rollout_noise", w, inputs, mask, case_params, preds_seq, steps, ws, noise, fed, batch, h,
+                           wd, stream);
 }
 
 // fno_grid_forward_train up to the saved set (lift and Fourier blocks, no projection)
@@ -919,17 +1082,72 @@ int fno_grid_backward(const fno_weights* w, const fno_weights_bwd* wb, const flo
                             stream);
 }
 
-int fno_grid_rollout_forward_train(const fno_weights* w, const float* inputs, const float* mask, const float* case_params,
-                                   float* preds_seq, int steps, const fno_train_saved* saved, const fno_workspace* ws,
-                                   int batch, int h, int wd, void* stream) {
-  FNO_TRY(grid_arg("fno_grid_rollout_forward_train", h, wd));
-  if (steps < 1 || !inputs || !preds_seq || batch <= 0) return fail(kErrArg, "fno_grid_rollout_forward_train: bad argument");
+static int grid_rollout_forward_train_impl(const char* what, const fno_weights* w, const float* inputs, const float* mask,
+                                           const float* case_params, float* preds_seq, int steps,
+                                           const fno_train_saved* saved, const fno_workspace* ws, const fno_noise* nz,
+                                           float* fed, int batch, int h, int wd, void* stream) {
+  char msg[160];
+  FNO_TRY(grid_arg(what, h, wd));
+  if (steps < 1 || !inputs || !preds_seq || batch <= 0) {
+    snprintf(msg, sizeof(msg), "%s: bad argument", what);
+    return fail(kErrArg, msg);
+  }
   const size_t frame = static_cast<size_t>(batch) * 2 * h * wd;
   const float* cur = inputs;
   for (int s = 0; s < steps; ++s) {
     float* nxt = preds_seq + static_cast<size_t>(s) * frame;
+    FNO_TRY(feed_step(nz, fed, mask, s, frame, batch, h, wd, cur, stream));
     FNO_TRY(fno_grid_forward_train(w, cur, mask, case_params, nxt, saved, ws, batch, h, wd, stream));
     cur = nxt;
+  }
+  return kOk;
+}
+
+int fno_grid_rollout_forward_train(const fno_weights* w, const float* inputs, const float* mask, const float* case_params,
+                                   float* preds_seq, int steps, const fno_train_saved* saved, const fno_workspace* ws,
+                                   int batch, int h, int wd, void* stream) {
+  return grid_rollout_forward_train_impl("fno_grid_rollout_forward_train", w, inputs, mask, case_params, preds_seq, steps,
+                                         saved, ws, nullptr, nullptr, batch, h, wd, stream);
+}
+
+int fno_grid_rollout_forward_train_noise(const fno_weights* w, const float* inputs, const float* mask,
+                                         const float* case_params, float* preds_seq, int steps, const fno_train_saved* saved,
+                                         const fno_workspace* ws, const fno_noise* noise, float* fed, int batch, int h, int wd,
+                                         void* stream) {
+  FNO_TRY(grid_arg("fno_grid_rollout_forward_train_noise", h, wd));
+  FNO_TRY(noise_args("fno_grid_rollout_forward_train_noise", noise, fed, steps));
+  FNO_TRY(noise_forward_args("fno_grid_rollout_forward_train_noise", w, inputs, mask, case_params, saved, ws, batch, true,
+                             0));
+  return grid_rollout_forward_train_impl("fno_grid_rollout_forward_train_noise", w, inputs, mask, case_params, preds_seq,
+                                         steps, saved, ws, noise, fed, batch, h, wd, stream);
+}
+
+static int grid_rollout_backward_impl(const char* what, const fno_weights* w, const fno_weights_bwd* wb, const float* inputs,
+                                      const float* mask, const float* case_params, const float* preds_seq,
+                                      const float* dpreds_seq, int steps, const fno_train_saved* saved, const fno_grads* grads,
+                                      const fno_bwd_scratch* scratch, const fno_workspace* ws, const fno_noise* nz,
+                                      const float* fed, float* carry, float* d_inputs, float* d_case_params, int batch, int h,
+                                      int wd, void* stream) {
+  char msg[160];
+  FNO_TRY(grid_arg(what, h, wd));
+  if (w && w->n_case_params == 0) d_case_params = nullptr;   // nothing to write
+  FNO_TRY(rollout_bwd_args(what, w, wb, inputs, mask, preds_seq, dpreds_seq, steps, saved, grads, scratch, ws, carry, d_inputs,
+                           d_case_params, batch));
+  if (!saved->act[0]) {
+    snprintf(msg, sizeof(msg), "%s: null saved buffer", what);
+    return fail(kErrArg, msg);
+  }
+  const size_t frame = static_cast<size_t>(batch) * 2 * h * wd;
+  if (d_case_params)   // every sweep step adds its share
+    FNO_CUDA(cudaMemsetAsync(d_case_params, 0, static_cast<size_t>(batch) * w->n_case_params * sizeof(float), S(stream)),
+             "memset(d_case_params)");
+  for (int s = steps - 1; s >= 0; --s) {
+    const float* x = fed_frame(nz, fed, inputs, preds_seq, s, frame);
+    FNO_TRY(grid_forward_train_body(w, x, mask, case_params, saved, ws, batch, h, wd, stream));
+    const float* up = s == steps - 1 ? dpreds_seq + static_cast<size_t>(s) * frame : carry;
+    FNO_TRY(grid_backward_impl(w, wb, x, mask, case_params, up, saved, grads, scratch, ws, s > 0 ? carry : d_inputs,
+                               d_case_params, batch, h, wd, stream, s != steps - 1 ? 1 : 0, 1,
+                               s > 0 ? dpreds_seq + static_cast<size_t>(s - 1) * frame : nullptr));
   }
   return kOk;
 }
@@ -939,25 +1157,21 @@ int fno_grid_rollout_backward(const fno_weights* w, const fno_weights_bwd* wb, c
                               const fno_train_saved* saved, const fno_grads* grads, const fno_bwd_scratch* scratch,
                               const fno_workspace* ws, float* carry, float* d_inputs, float* d_case_params, int batch, int h,
                               int wd, void* stream) {
-  const char* what = "fno_grid_rollout_backward";
-  FNO_TRY(grid_arg(what, h, wd));
-  if (w && w->n_case_params == 0) d_case_params = nullptr;   // nothing to write
-  FNO_TRY(rollout_bwd_args(what, w, wb, inputs, mask, preds_seq, dpreds_seq, steps, saved, grads, scratch, ws, carry, d_inputs,
-                           d_case_params, batch));
-  if (!saved->act[0]) return fail(kErrArg, "fno_grid_rollout_backward: null saved buffer");
-  const size_t frame = static_cast<size_t>(batch) * 2 * h * wd;
-  if (d_case_params)   // every sweep step adds its share
-    FNO_CUDA(cudaMemsetAsync(d_case_params, 0, static_cast<size_t>(batch) * w->n_case_params * sizeof(float), S(stream)),
-             "memset(d_case_params)");
-  for (int s = steps - 1; s >= 0; --s) {
-    const float* x = s > 0 ? preds_seq + static_cast<size_t>(s - 1) * frame : inputs;
-    FNO_TRY(grid_forward_train_body(w, x, mask, case_params, saved, ws, batch, h, wd, stream));
-    const float* up = s == steps - 1 ? dpreds_seq + static_cast<size_t>(s) * frame : carry;
-    FNO_TRY(grid_backward_impl(w, wb, x, mask, case_params, up, saved, grads, scratch, ws, s > 0 ? carry : d_inputs,
-                               d_case_params, batch, h, wd, stream, s != steps - 1 ? 1 : 0, 1,
-                               s > 0 ? dpreds_seq + static_cast<size_t>(s - 1) * frame : nullptr));
-  }
-  return kOk;
+  return grid_rollout_backward_impl("fno_grid_rollout_backward", w, wb, inputs, mask, case_params, preds_seq, dpreds_seq, steps,
+                                    saved, grads, scratch, ws, nullptr, nullptr, carry, d_inputs, d_case_params, batch, h, wd,
+                                    stream);
+}
+
+int fno_grid_rollout_backward_noise(const fno_weights* w, const fno_weights_bwd* wb, const float* inputs, const float* mask,
+                                    const float* case_params, const float* preds_seq, const float* dpreds_seq, int steps,
+                                    const fno_train_saved* saved, const fno_grads* grads, const fno_bwd_scratch* scratch,
+                                    const fno_workspace* ws, const fno_noise* noise, const float* fed, float* carry,
+                                    float* d_inputs, float* d_case_params, int batch, int h, int wd, void* stream) {
+  FNO_TRY(grid_arg("fno_grid_rollout_backward_noise", h, wd));
+  FNO_TRY(noise_args("fno_grid_rollout_backward_noise", noise, fed, steps));
+  return grid_rollout_backward_impl("fno_grid_rollout_backward_noise", w, wb, inputs, mask, case_params, preds_seq, dpreds_seq,
+                                    steps, saved, grads, scratch, ws, noise, fed, carry, d_inputs, d_case_params, batch, h,
+                                    wd, stream);
 }
 
 int fno_grid_multistep_metrics(const float* preds_seq, const float* label_u, const float* mask, float* sums, int steps,
@@ -1009,6 +1223,20 @@ int fno_add_input_noise(float* inputs, const float* mask, const int64_t* idx, in
                                   reinterpret_cast<const long long*>(step_base), reinterpret_cast<const int*>(step_offset),
                                   S(stream)),
            "add_input_noise_kernel");
+  return kOk;
+}
+
+int fno_add_input_noise_stream(const float* in, float* out, const float* mask, const int64_t* idx, int n, int h, int wd,
+                               float std, uint64_t seed, const int64_t* step_base, const int32_t* step_offset,
+                               int noise_stream, void* stream) {
+  FNO_TRY(grid_arg("fno_add_input_noise_stream", h, wd));
+  if (!in || !out || !mask || !idx || !step_base || n <= 0 || !(std >= 0.f) || !isfinite(std) || noise_stream < 0 ||
+      noise_stream >= FNO_NOISE_STREAMS)
+    return fail(kErrArg, "fno_add_input_noise_stream: bad argument");
+  FNO_CUDA(launch_input_noise_stream(in, out, mask, reinterpret_cast<const long long*>(idx), n, h, wd, std, seed,
+                                     reinterpret_cast<const long long*>(step_base), reinterpret_cast<const int*>(step_offset),
+                                     noise_stream, S(stream)),
+           "input_noise_stream_kernel");
   return kOk;
 }
 

@@ -382,6 +382,9 @@ cudaError_t launch_log_step(const float* loss_out, float* log, int n_log, int* c
 // key = (seed_lo, seed_hi)), j = idx[b]: a pure function of (seed, step, j, e), whatever the batch slot, the launch or the
 // replay.  step = *step_base (+ *step_offset), read on the device so that a captured launch sees each replay's step.
 // One thread per quad; the 64x64 path moves a quad as one float4 (it never straddles the two channels).
+// Noise streams (input_noise_stream_kernel, the per-step noise of a rollout): stream k draws from counter.x = q + (k << 16)
+// instead of q.  q < 2 * 128 * 128 / 4 = 2^13, so streams k < 2^16 never share a counter, and stream 0 is the counter above:
+// the same noise as add_input_noise_kernel, bit for bit.
 constexpr int kNoiseThreads = 256;
 
 __device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint2 k) {
@@ -411,35 +414,46 @@ __device__ __forceinline__ float4 noise_normals(unsigned long long seed, unsigne
   return make_float4(r0 * cospif(t0), r0 * sinpif(t0), r1 * cospif(t1), r1 * sinpif(t1));
 }
 
-template <bool kVec>
-__global__ void __launch_bounds__(kNoiseThreads)
-    add_input_noise_kernel(float* __restrict__ inputs, const float* __restrict__ mask, const long long* __restrict__ idx,
-                           int hw, float std, unsigned long long seed, const long long* __restrict__ step_base,
-                           const int* __restrict__ step_offset) {
+// The body of both noise kernels for sample b = blockIdx.y and quad q.  kInPlace (add_input_noise_kernel, out == in):
+// only the cells where mask != 0 are written.  Otherwise (input_noise_stream_kernel) out = in + noise where mask != 0 and
+// out = in elsewhere, so `out` is a whole frame; `out` may still equal `in`.
+template <bool kVec, bool kInPlace>
+__device__ __forceinline__ void input_noise(const float* in, float* out, const float* __restrict__ mask,
+                                            const long long* __restrict__ idx, int hw, float std, unsigned long long seed,
+                                            const long long* __restrict__ step_base, const int* __restrict__ step_offset,
+                                            unsigned stream) {
   const int b = blockIdx.y;
   const int n_el = 2 * hw;
   const unsigned q = blockIdx.x * kNoiseThreads + threadIdx.x;
   if (4 * q >= static_cast<unsigned>(n_el)) return;
   const unsigned long long step =
       static_cast<unsigned long long>(*step_base) + (step_offset ? static_cast<long long>(*step_offset) : 0ll);
-  const float4 z = noise_normals(seed, step, static_cast<unsigned>(idx[b]), q);
+  const float4 z = noise_normals(seed, step, static_cast<unsigned>(idx[b]), q + (stream << 16));
   const float zs[4] = {z.x, z.y, z.z, z.w};
-  float* x = inputs + static_cast<size_t>(b) * n_el;
+  const float* x = in + static_cast<size_t>(b) * n_el;
+  float* y = out + static_cast<size_t>(b) * n_el;
   const float* m = mask + static_cast<size_t>(b) * hw;
   if constexpr (kVec) {   // hw % 4 == 0 and 16-byte aligned slices: the quad lies in one channel
     const int e = 4 * q, cell = e < hw ? e : e - hw;
     const float4 mv = __ldg(reinterpret_cast<const float4*>(m + cell));
-    float4 xv = *reinterpret_cast<const float4*>(x + e);
+    const float4 xv = *reinterpret_cast<const float4*>(x + e);
     const float ms[4] = {mv.x, mv.y, mv.z, mv.w};
-    float xs[4] = {xv.x, xv.y, xv.z, xv.w};
+    const float x0[4] = {xv.x, xv.y, xv.z, xv.w};
+    float xs[4];
 #pragma unroll
-    for (int r = 0; r < 4; ++r) xs[r] = fmaf(std * zs[r], ms[r], xs[r]);
-    if (ms[0] != 0.f && ms[1] != 0.f && ms[2] != 0.f && ms[3] != 0.f) {
-      *reinterpret_cast<float4*>(x + e) = make_float4(xs[0], xs[1], xs[2], xs[3]);
+    for (int r = 0; r < 4; ++r) xs[r] = fmaf(std * zs[r], ms[r], x0[r]);
+    if constexpr (kInPlace) {
+      if (ms[0] != 0.f && ms[1] != 0.f && ms[2] != 0.f && ms[3] != 0.f) {
+        *reinterpret_cast<float4*>(y + e) = make_float4(xs[0], xs[1], xs[2], xs[3]);
+      } else {
+#pragma unroll
+        for (int r = 0; r < 4; ++r)
+          if (ms[r] != 0.f) y[e + r] = xs[r];
+      }
     } else {
 #pragma unroll
-      for (int r = 0; r < 4; ++r)
-        if (ms[r] != 0.f) x[e + r] = xs[r];
+      for (int r = 0; r < 4; ++r) xs[r] = ms[r] != 0.f ? xs[r] : x0[r];
+      *reinterpret_cast<float4*>(y + e) = make_float4(xs[0], xs[1], xs[2], xs[3]);
     }
   } else {
 #pragma unroll
@@ -447,10 +461,32 @@ __global__ void __launch_bounds__(kNoiseThreads)
       const int e = 4 * q + r;
       if (e < n_el) {
         const float mv = __ldg(m + (e < hw ? e : e - hw));
-        if (mv != 0.f) x[e] = fmaf(std * zs[r], mv, x[e]);
+        if constexpr (kInPlace) {
+          if (mv != 0.f) y[e] = fmaf(std * zs[r], mv, x[e]);
+        } else {
+          const float xv = x[e];
+          y[e] = mv != 0.f ? fmaf(std * zs[r], mv, xv) : xv;
+        }
       }
     }
   }
+}
+
+template <bool kVec>
+__global__ void __launch_bounds__(kNoiseThreads)
+    add_input_noise_kernel(float* __restrict__ inputs, const float* __restrict__ mask, const long long* __restrict__ idx,
+                           int hw, float std, unsigned long long seed, const long long* __restrict__ step_base,
+                           const int* __restrict__ step_offset) {
+  input_noise<kVec, true>(inputs, inputs, mask, idx, hw, std, seed, step_base, step_offset, 0u);
+}
+
+// out = in + noise of stream `stream` (input_noise's out-of-place form; in == out is allowed)
+template <bool kVec>
+__global__ void __launch_bounds__(kNoiseThreads)
+    input_noise_stream_kernel(const float* in, float* out, const float* __restrict__ mask, const long long* __restrict__ idx,
+                              int hw, float std, unsigned long long seed, const long long* __restrict__ step_base,
+                              const int* __restrict__ step_offset, unsigned stream) {
+  input_noise<kVec, false>(in, out, mask, idx, hw, std, seed, step_base, step_offset, stream);
 }
 
 cudaError_t launch_add_input_noise(float* inputs, const float* mask, const long long* idx, int n, int h, int w, float std,
@@ -465,6 +501,23 @@ cudaError_t launch_add_input_noise(float* inputs, const float* mask, const long 
   else
     add_input_noise_kernel<false><<<grid, kNoiseThreads, 0, stream>>>(inputs, mask, idx, hw, std, seed, step_base,
                                                                        step_offset);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_input_noise_stream(const float* in, float* out, const float* mask, const long long* idx, int n, int h,
+                                      int w, float std, unsigned long long seed, const long long* step_base,
+                                      const int* step_offset, int noise_stream, cudaStream_t stream) {
+  const int hw = h * w, quads = (2 * hw + 3) / 4;
+  const dim3 grid((quads + kNoiseThreads - 1) / kNoiseThreads, n);
+  const bool vec = hw % 4 == 0 && ((reinterpret_cast<uintptr_t>(in) | reinterpret_cast<uintptr_t>(out) |
+                                    reinterpret_cast<uintptr_t>(mask)) & 15) == 0;
+  const unsigned k = static_cast<unsigned>(noise_stream);
+  if (vec)
+    input_noise_stream_kernel<true><<<grid, kNoiseThreads, 0, stream>>>(in, out, mask, idx, hw, std, seed, step_base,
+                                                                         step_offset, k);
+  else
+    input_noise_stream_kernel<false><<<grid, kNoiseThreads, 0, stream>>>(in, out, mask, idx, hw, std, seed, step_base,
+                                                                          step_offset, k);
   return cudaGetLastError();
 }
 

@@ -16,7 +16,7 @@ datasets hold (N, 3, 66, 65) frames, reference src/dataset/tube.py:228-281, dam.
 from __future__ import annotations
 
 import ctypes as C
-from typing import Dict, Iterable, Iterator, List, Optional, Sequence
+from typing import Dict, Iterable, Iterator, List, NamedTuple, Optional, Sequence
 
 import numpy as np
 import torch
@@ -194,6 +194,93 @@ def check_noise_args(noise_std, noise_seed, noise_step=0, std_name: str = "noise
         if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or not 0 <= int(v) < hi:
             raise ValueError(f"{name} must be an int in [0, 2^{hi.bit_length() - 1}), got {v!r}")
     return float(noise_std)
+
+
+class RolloutNoise(NamedTuple):
+    """The per-step input noise of `Fno2d.rollout(noise=...)`: Gaussian noise of standard deviation `std` from the
+    counter-based RNG of `add_input_noise`, keyed by `seed` and counted by `step` (train_auto passes Adam's 1-based
+    step), `ids` ((B,) int64 on the model's device: each sample's dataset index, so the noise does not depend on the
+    batch slot) and the noise stream; rollout step s draws from stream k0 + s."""
+    std: float
+    seed: int
+    step: int
+    ids: Tensor
+    k0: int = 0
+
+
+def check_rollout_noise(noise, batch: int, steps) -> Optional[RolloutNoise]:
+    """Refuse a `Fno2d.rollout` noise record the native drivers cannot take: not a RolloutNoise, noise arguments
+    `check_noise_args` refuses, ids that are not a (batch,) int64 tensor, or a k0 that is not an int >= 0 with
+    k0 + steps <= 2^16 (the streams).  Returns None for no noise (None, or std 0: the path without noise), else the
+    record with std as a float and the ints as Python ints."""
+    if noise is None:
+        return None
+    if not isinstance(noise, RolloutNoise):
+        raise ValueError(f"noise must be a RolloutNoise or None, got {type(noise).__name__}")
+    std = check_noise_args(noise.std, noise.seed, noise.step)
+    ids, k0 = noise.ids, noise.k0
+    if not isinstance(ids, Tensor) or ids.dtype != torch.int64 or tuple(ids.shape) != (batch,):
+        raise ValueError(f"noise.ids must be a ({batch},) int64 tensor, got "
+                         f"{getattr(ids, 'dtype', type(ids).__name__)} {tuple(getattr(ids, 'shape', ()))}")
+    n_steps = steps if isinstance(steps, int) and not isinstance(steps, bool) else 1
+    if isinstance(k0, bool) or not isinstance(k0, (int, np.integer)) or k0 < 0 or int(k0) + n_steps > 2 ** 16:
+        raise ValueError(f"noise.k0 must be an int >= 0 with k0 + steps <= 2^16, got {k0!r} with steps={steps!r}")
+    if std == 0:
+        return None
+    return RolloutNoise(std, int(noise.seed), int(noise.step), ids.contiguous(), int(k0))
+
+
+class _NoiseFn(torch.autograd.Function):
+    """frames + noise with the identity as its gradient w.r.t. the frames (the noise does not depend on them)."""
+
+    @staticmethod
+    def forward(ctx, frames: Tensor, noise_args: tuple) -> Tensor:
+        return _noise_out_of_place(frames, *noise_args)
+
+    @staticmethod
+    def backward(ctx, grad: Tensor):
+        return grad, None
+
+
+def _noise_out_of_place(frames: Tensor, mask: Tensor, ids: Tensor, std: float, seed: int, step: int,
+                        stream: int) -> Tensor:
+    from . import _lib
+    out = torch.empty_like(frames)
+    b, _, gh, gw = frames.shape
+    with torch.cuda.device(frames.device):
+        step_dev = torch.full((1,), step, dtype=torch.int64, device=frames.device)   # a fill kernel, no copy
+        st = C.c_void_p(torch.cuda.current_stream(frames.device).cuda_stream)
+        _lib.check(_lib.load().fno_add_input_noise_stream(frames.data_ptr(), out.data_ptr(), mask.data_ptr(), ids.data_ptr(),
+                                                          b, gh, gw, std, seed, step_dev.data_ptr(), None, stream, st),
+                   "fno_add_input_noise_stream")
+    return out
+
+
+def add_input_noise(frames: Tensor, mask: Tensor, ids: Tensor, std: float, seed: int, step: int,
+                    stream: int = 0) -> Tensor:
+    """A new tensor: `frames` ((B, 2, H, W) float32 on a CUDA device) plus seeded Gaussian noise where `mask` ((B, 1, H,
+    W) or (B, H, W)) is non-zero, `frames` elsewhere.  The noise is that of `DeviceFrames.batch(noise_std=std,
+    noise_seed=seed, noise_step=step)` for the samples with dataset indices `ids` ((B,) int64), drawn from noise stream
+    `stream` (0 <= stream < 2^16): stream 0 is exactly the noise `batch` adds, and `Fno2d.rollout(noise=RolloutNoise(std,
+    seed, step, ids, k0))` feeds its step s a frame perturbed with stream k0 + s.  One launch
+    (`fno_add_input_noise_stream`).  Differentiable w.r.t. `frames`, with the identity as gradient.  Raises ValueError
+    for bad noise arguments (as `DeviceFrames.batch`), a stream outside 0 .. 2^16 - 1 or mismatched shapes."""
+    std = check_noise_args(std, seed, step, std_name="std")
+    if isinstance(stream, bool) or not isinstance(stream, (int, np.integer)) or not 0 <= stream < 2 ** 16:
+        raise ValueError(f"stream must be an int in [0, 2^16), got {stream!r}")
+    if not isinstance(frames, Tensor) or frames.dim() != 4 or frames.shape[1] != 2 or frames.dtype != torch.float32:
+        raise ValueError(f"frames must be a (B, 2, H, W) float32 tensor, got {getattr(frames, 'shape', None)}")
+    b, _, gh, gw = frames.shape
+    if mask.shape not in ((b, 1, gh, gw), (b, gh, gw)):
+        raise ValueError(f"mask must be ({b}, 1, {gh}, {gw}) or ({b}, {gh}, {gw}), got {tuple(mask.shape)}")
+    if not isinstance(ids, Tensor) or ids.dtype != torch.int64 or tuple(ids.shape) != (b,):
+        raise ValueError(f"ids must be a ({b},) int64 tensor")
+    if frames.device.type != "cuda" or mask.device != frames.device or ids.device != frames.device:
+        raise ValueError("frames, mask and ids must be on the same CUDA device")
+    args = (mask.to(torch.float32).contiguous(), ids.contiguous(), std, int(seed), int(step), int(stream))
+    if frames.requires_grad and torch.is_grad_enabled():
+        return _NoiseFn.apply(frames.contiguous(), args)
+    return _noise_out_of_place(frames.detach().contiguous(), *args)
 
 
 def index_batches(n: int, batch_size: int, shuffle: bool = False, generator=None,

@@ -32,6 +32,7 @@ from torch import Tensor
 
 from . import _lib
 from .base_model import AutoCfdModel
+from .data import check_rollout_noise
 
 H = W = 64
 HIDDEN = 32
@@ -180,28 +181,30 @@ class _RolloutFn(torch.autograd.Function):
     training forward: K training forwards into ONE reused saved set, keeping only the K predicted frames.  Backward = one
     native sweep, s = K-1 .. 0, that recomputes step s's saved set from its stored input frame and runs step s's backward
     with the upstream gradient dpreds_s + carry (carry = dL/d(frame fed to step s+1)), accumulating the parameter and
-    case-parameter gradients.  Memory: the K+1 frames and one saved set instead of K saved sets."""
+    case-parameter gradients.  Memory: the K+1 frames and one saved set instead of K saved sets.  With `noise` (a
+    RolloutNoise) the perturbed frames the steps were fed are kept as well, one more frame per step, and the sweep
+    recomputes from them."""
 
     @staticmethod
-    def forward(ctx, model: "Fno2d", inputs: Tensor, mask: Tensor, case_params: Tensor, steps: int, *params: Tensor):
+    def forward(ctx, model: "Fno2d", inputs: Tensor, mask: Tensor, case_params: Tensor, steps: int, noise, *params: Tensor):
         _refuse_mask_grad(mask)
-        seq = model._native_rollout_train(inputs, mask, case_params, steps)
-        ctx.model, ctx.steps = model, steps
-        ctx.save_for_backward(inputs, mask, case_params, seq)
+        seq, fed = model._native_rollout_train(inputs, mask, case_params, steps, noise)
+        ctx.model, ctx.steps, ctx.noise = model, steps, noise
+        ctx.save_for_backward(inputs, mask, case_params, seq, fed)
         return seq
 
     @staticmethod
     def backward(ctx, dseq: Tensor):
-        inputs, mask, case_params, seq = ctx.saved_tensors
+        inputs, mask, case_params, seq, fed = ctx.saved_tensors
         model: "Fno2d" = ctx.model
-        need = ctx.needs_input_grad   # (model, inputs, mask, case_params, steps, *params)
+        need = ctx.needs_input_grad   # (model, inputs, mask, case_params, steps, noise, *params)
         d_inputs = torch.empty_like(inputs) if need[1] else None
         d_cp = torch.empty_like(case_params) if need[3] else None
         grads = model._native_rollout_backward(inputs, mask, case_params, seq, dseq.contiguous().float(), ctx.steps,
-                                               any(need[5:]), d_inputs, d_cp)
+                                               any(need[6:]), d_inputs, d_cp, ctx.noise, fed)
         if grads is None:
-            grads = [None] * (len(need) - 5)
-        return (None, d_inputs, None, d_cp, None, *grads)
+            grads = [None] * (len(need) - 6)
+        return (None, d_inputs, None, d_cp, None, None, *grads)
 
 
 class Fno2d(AutoCfdModel):
@@ -643,9 +646,23 @@ class Fno2d(AutoCfdModel):
         self._refresh_static_weights(ent["sw"], pk, route.gh, route.gw)
         return ent
 
-    def _native_rollout_train(self, inputs: Tensor, mask4: Tensor, case_params: Tensor, steps: int) -> Tensor:
-        """preds (steps, B, 2, H, W) from fno_[grid_]rollout_forward_train: the training forward's kernels, so the
-        predictions equal those of chained `generate` calls under autograd bit for bit."""
+    def _noise_io(self, noise) -> dict:
+        """Device copies of a RolloutNoise's sample indices and step, and the fno_noise descriptor pointing at them
+        (kept together: the descriptor holds raw pointers).  A captured graph owns one and refills it per call."""
+        io = dict(ids=noise.ids.clone(), step=torch.full((1,), noise.step, dtype=torch.int64, device=self.device))
+        io["desc"] = _lib.FnoNoise(noise.std, noise.seed, io["ids"].data_ptr(), io["step"].data_ptr(), None, noise.k0)
+        return io
+
+    @staticmethod
+    def _refill_noise_io(nio: dict, noise) -> None:
+        nio["ids"].copy_(noise.ids)
+        nio["step"].fill_(noise.step)   # a fill kernel: no host-to-device copy
+
+    def _native_rollout_train(self, inputs: Tensor, mask4: Tensor, case_params: Tensor, steps: int, noise=None):
+        """(preds, fed): preds (steps, B, 2, H, W) from fno_[grid_]rollout_forward_train: the training forward's kernels,
+        so the predictions equal those of chained `generate` calls under autograd bit for bit.  fed is None, or with
+        `noise` (a RolloutNoise) the (steps, B, 2, H, W) frames the steps were fed (fno_[grid_]rollout_forward_train_noise:
+        slot s holds step s's perturbed input when its stream k0 + s is at least 1)."""
         b = inputs.shape[0]
         route = self._route(*inputs.shape[-2:])
         gh, gw = route.gh, route.gw
@@ -653,31 +670,52 @@ class Fno2d(AutoCfdModel):
         ws, ws_bufs = self._workspace(b, route)
         rs = self._rollout_state(b, route)
         seq = torch.empty(steps, b, self.out_chan, gh, gw, dtype=torch.float32, device=self.device)
+        fed = None if noise is None else torch.empty_like(seq)
 
-        def call(st, x, mk, cp, out):
-            route.call("rollout_forward_train", C.byref(st), x.data_ptr(), mk.data_ptr(), cp.data_ptr(), out.data_ptr(),
-                       steps, C.byref(rs["sv"]), C.byref(ws), b, self._stream())
+        def call(st, x, mk, cp, out, nio, fd):
+            if nio is None:
+                route.call("rollout_forward_train", C.byref(st), x.data_ptr(), mk.data_ptr(), cp.data_ptr(),
+                           out.data_ptr(), steps, C.byref(rs["sv"]), C.byref(ws), b, self._stream())
+            else:
+                route.call("rollout_forward_train_noise", C.byref(st), x.data_ptr(), mk.data_ptr(), cp.data_ptr(),
+                           out.data_ptr(), steps, C.byref(rs["sv"]), C.byref(ws), C.byref(nio["desc"]), fd.data_ptr(), b,
+                           self._stream())
         if not self.graph_rollout:
-            call(self._coords(pk, gh, gw)[0], inputs, mask4, case_params, seq)
-            return seq
-        key = ("fwd", b, steps, gh, gw, route.grid, self.act_dtype)
+            call(self._coords(pk, gh, gw)[0], inputs, mask4, case_params, seq,
+                 None if noise is None else self._noise_io(noise), fed)
+            return seq, fed
+        key = ("fwd", b, steps, gh, gw, route.grid, self.act_dtype,
+               None if noise is None else (noise.std, noise.seed, noise.k0))
+
+        def make_io():
+            io = dict(x=inputs.clone(), mk=mask4.clone(), cp=case_params.clone(), seq=torch.empty_like(seq),
+                      noise=None, fed=None)
+            if noise is not None:
+                io["noise"], io["fed"] = self._noise_io(noise), torch.empty_like(seq)
+            return io
         ent = self._train_graph(
-            key, pk, route,
-            lambda: dict(x=inputs.clone(), mk=mask4.clone(), cp=case_params.clone(), seq=torch.empty_like(seq)),
-            lambda sw, io: call(sw["struct"], io["x"], io["mk"], io["cp"], io["seq"]), (ws_bufs, rs))
+            key, pk, route, make_io,
+            lambda sw, io: call(sw["struct"], io["x"], io["mk"], io["cp"], io["seq"], io["noise"], io["fed"]),
+            (ws_bufs, rs))
         io = ent["io"]
         io["x"].copy_(inputs)
         io["mk"].copy_(mask4)
         io["cp"].copy_(case_params)
+        if noise is not None:
+            self._refill_noise_io(io["noise"], noise)
         ent["graph"].replay()
         seq.copy_(io["seq"])
-        return seq
+        if noise is not None:
+            fed.copy_(io["fed"])
+        return seq, fed
 
     def _native_rollout_backward(self, inputs, mask4, case_params, seq, dseq, steps: int, want_params: bool,
-                                 d_inputs: Optional[Tensor], d_cp: Optional[Tensor]):
+                                 d_inputs: Optional[Tensor], d_cp: Optional[Tensor], noise=None,
+                                 fed: Optional[Tensor] = None):
         """One native sweep (fno_[grid_]rollout_backward): parameter gradients in parameter order (None when
         `want_params` is false), dL/dinputs into `d_inputs` and dL/dcase_params into `d_cp` when given.  With data
-        parallel enabled the flat parameter-gradient buffer is all-reduced once."""
+        parallel enabled the flat parameter-gradient buffer is all-reduced once.  With `noise` the sweep
+        (fno_[grid_]rollout_backward_noise) recomputes each noisy step from its frame in `fed`."""
         if self.n_case_params == 0:
             d_cp = None
         if not want_params and d_inputs is None and d_cp is None:
@@ -690,35 +728,48 @@ class Fno2d(AutoCfdModel):
         rs = self._rollout_state(b, route)
         carry = rs["bufs"]["carry"]
 
-        def call(st, sb, x, mk, cp, sq, dsq, g, din, dcp):
-            route.call("rollout_backward", C.byref(st), C.byref(sb), x.data_ptr(), mk.data_ptr(), cp.data_ptr(),
-                       sq.data_ptr(), dsq.data_ptr(), steps, C.byref(rs["sv"]), C.byref(g) if g is not None else None,
-                       C.byref(rs["sc"]), C.byref(ws), carry.data_ptr(), _ptr(din), _ptr(dcp), b, self._stream())
+        def call(st, sb, x, mk, cp, sq, dsq, g, din, dcp, nio, fd):
+            g = C.byref(g) if g is not None else None
+            if nio is None:
+                route.call("rollout_backward", C.byref(st), C.byref(sb), x.data_ptr(), mk.data_ptr(), cp.data_ptr(),
+                           sq.data_ptr(), dsq.data_ptr(), steps, C.byref(rs["sv"]), g, C.byref(rs["sc"]), C.byref(ws),
+                           carry.data_ptr(), _ptr(din), _ptr(dcp), b, self._stream())
+            else:
+                route.call("rollout_backward_noise", C.byref(st), C.byref(sb), x.data_ptr(), mk.data_ptr(),
+                           cp.data_ptr(), sq.data_ptr(), dsq.data_ptr(), steps, C.byref(rs["sv"]), g, C.byref(rs["sc"]),
+                           C.byref(ws), C.byref(nio["desc"]), fd.data_ptr(), carry.data_ptr(), _ptr(din), _ptr(dcp), b,
+                           self._stream())
         flat = views = None
         if not self.graph_rollout:
             g = None
             if want_params:
                 flat, views, g = self._grad_buffers()
             call(self._coords(pk, gh, gw)[0], pk["struct_bwd"], inputs, mask4, case_params, seq, dseq, g, d_inputs,
-                 d_cp)
+                 d_cp, None if noise is None else self._noise_io(noise), fed)
         else:
             def make_io():
                 io = dict(x=inputs.clone(), mk=mask4.clone(), cp=case_params.clone(), seq=torch.empty_like(seq),
                           dseq=torch.empty_like(dseq), g=None,
                           din=torch.empty_like(d_inputs) if d_inputs is not None else None,
-                          dcp=torch.empty_like(d_cp) if d_cp is not None else None)
+                          dcp=torch.empty_like(d_cp) if d_cp is not None else None, noise=None, fed=None)
                 if want_params:
                     io["flat"], _, io["g"] = self._grad_buffers()
+                if noise is not None:
+                    io["noise"], io["fed"] = self._noise_io(noise), torch.empty_like(fed)
                 return io
+            # the sweep draws no noise: of the descriptor it reads only k0 (the other fields, from the capturing call,
+            # are checked and never read), so std, seed, step and ids do not key the capture
             key = ("bwd", b, steps, gh, gw, route.grid, self.act_dtype, want_params, d_inputs is not None,
-                   d_cp is not None)
+                   d_cp is not None, None if noise is None else noise.k0)
             ent = self._train_graph(
                 key, pk, route, make_io,
                 lambda sw, io: call(sw["struct"], sw["struct_bwd"], io["x"], io["mk"], io["cp"], io["seq"], io["dseq"],
-                                    io["g"], io["din"], io["dcp"]), (ws_bufs, rs))
+                                    io["g"], io["din"], io["dcp"], io["noise"], io["fed"]), (ws_bufs, rs))
             io = ent["io"]
             for k, t in (("x", inputs), ("mk", mask4), ("cp", case_params), ("seq", seq), ("dseq", dseq)):
                 io[k].copy_(t)
+            if noise is not None:
+                io["fed"].copy_(fed)
             ent["graph"].replay()
             if d_inputs is not None:
                 d_inputs.copy_(io["din"])
@@ -782,7 +833,7 @@ class Fno2d(AutoCfdModel):
                 seq = self._rollout_device(inputs, case_params, mask4, steps)
         return [seq[s] for s in range(steps)]
 
-    def rollout(self, inputs: Tensor, case_params: Tensor, mask: Optional[Tensor], steps: int) -> Tensor:
+    def rollout(self, inputs: Tensor, case_params: Tensor, mask: Optional[Tensor], steps: int, noise=None) -> Tensor:
         """`steps` autoregressive steps as one (steps, B, 2, H, W) float32 tensor, trainable through the whole rollout.
         Arguments as `generate_many` ((c,h,w) / (p,) / (h,w) inputs get a batch axis); every grid and storage mode of
         `forward`.  Step s is fed the (masked) prediction of step s-1, computed with the training forward's kernels, so
@@ -793,7 +844,17 @@ class Fno2d(AutoCfdModel):
         its own saved activations until backward (about 1 GB per step at B = 256), it keeps only the predicted frames and
         one reused set of saved activations: the backward recomputes each step's activations from its input frame (one
         extra training forward per step) while it sweeps the steps from last to first.  With autograd off it returns the
-        same predictions and builds no graph."""
+        same predictions and builds no graph.
+
+        noise = RolloutNoise(std, seed, step, ids, k0) perturbs the frame every step is fed: step s is fed
+        `add_input_noise(x_s, mask, ids, std, seed, step, stream=k0 + s)` where x_s is `inputs` (s = 0) or the
+        prediction of step s-1, except that stream 0 is never applied here (the start frame's stream-0 noise is
+        `DeviceFrames.batch(noise_std=...)`'s).  The predictions themselves stay clean, and the gradient through each
+        perturbed frame is the identity, so they and the gradients equal those of the chain of one-step `rollout`
+        calls on frames perturbed with `add_input_noise`.  It costs one launch and keeps one more frame per noisy step.
+        noise=None, or std 0, runs exactly what runs without it.  Raises ValueError for a malformed record (see
+        `check_rollout_noise`)."""
+        noise = check_rollout_noise(noise, inputs.shape[0] if inputs.dim() == 4 else 1, steps)
         self._require_cuda()
         if isinstance(steps, bool) or not isinstance(steps, int) or steps < 1:
             raise ValueError(f"steps must be a positive int; got {steps!r}")
@@ -801,11 +862,13 @@ class Fno2d(AutoCfdModel):
             inputs, case_params = inputs.unsqueeze(0), case_params.unsqueeze(0)
             mask = mask.unsqueeze(0) if mask is not None else None
         inputs, case_params, mask4 = self._prep_inputs(inputs, case_params, mask)
+        if noise is not None and noise.ids.device != self.device:
+            raise ValueError(f"noise.ids is on {noise.ids.device}, the model on {self.device}")
         with torch.cuda.device(self.device):
             if self._needs_grad(inputs, case_params, mask4):
-                return _RolloutFn.apply(self, inputs, mask4, case_params, steps, *self.parameters())
+                return _RolloutFn.apply(self, inputs, mask4, case_params, steps, noise, *self.parameters())
             with torch.no_grad():
-                return self._native_rollout_train(inputs, mask4, case_params, steps)
+                return self._native_rollout_train(inputs, mask4, case_params, steps, noise)[0]
 
     def _rollout_device(self, inputs, case_params, mask4, steps) -> Tensor:
         b = inputs.shape[0]

@@ -16,6 +16,7 @@ synchronisation.  The result is bit-identical to the eager loop `DeviceFrames.lo
     train_auto(..., rollout_steps=4)   # trained through 4-step rollouts of the model's own predictions
     train_auto(..., rollout_steps=4, rollout_grad_steps=1)   # pushforward: 3 steps without gradient, the 4th trained
     train_auto(..., input_noise_std=0.01, noise_seed=1)      # Gaussian noise on every step's input frame
+    train_auto(..., rollout_steps=4, input_noise_std=0.01, noise_every_step=True)   # ... and on every rollout step's
 """
 from __future__ import annotations
 
@@ -259,12 +260,19 @@ class _RolloutStepGraphs(_StepGraphs):
     grad_steps = g < k (pushforward): the first k - g steps run without gradient through the inference rollout
     (fno_[grid_]rollout, the kernels generate_many runs) into a (k - g, bmax, ...) prefix buffer, on the step's
     workspace (the model's inference workspace for bmax samples, with the bf16 ym_img image); the training rollout, the
-    loss against targets k - g ... k - 1 and the backward then cover the last g steps from the prefix's last frame."""
+    loss against targets k - g ... k - 1 and the backward then cover the last g steps from the prefix's last frame.
+
+    noise_every_step (with noise_std > 0): rollout step s of the window (prefix and trained steps alike) is fed its
+    input plus the noise of stream s (the start frame keeps the gather's stream-0 noise).  The prefix and the trained
+    steps run the *_noise drivers with k0 = 0 and k0 = k - g, writing the perturbed frames into (k - g, bmax, ...) and
+    (g, bmax, ...) fed-frame buffers: k more frames per sample than without, and one more launch per rollout step."""
 
     def __init__(self, model, frames: DeviceFrames, batch_size: int, optimizer, n_windows: int, steps: int,
-                 time_step_size: int, grad_steps: Optional[int] = None, noise_std: float = 0.0, noise_seed: int = 0):
+                 time_step_size: int, grad_steps: Optional[int] = None, noise_std: float = 0.0, noise_seed: int = 0,
+                 noise_every_step: bool = False):
         self.k, self.tss = steps, time_step_size
         self.g = steps if grad_steps is None else grad_steps
+        self.every = noise_every_step and noise_std > 0
         super().__init__(model, frames, batch_size, optimizer, n=n_windows, noise_std=noise_std, noise_seed=noise_seed)
 
     def _make_io(self, bmax: int, gh: int, gw: int, p: int) -> dict:
@@ -283,8 +291,19 @@ class _RolloutStepGraphs(_StepGraphs):
             coef=torch.empty(self.steps, 2, **f32), log=torch.empty(self.steps, len(LOG_COLUMNS), **f32))
         if g < k:
             io["prefix"] = torch.empty(k - g, bmax, 2, gh, gw, **f32)
+        if self.every:
+            io["fed"] = torch.empty(g, bmax, 2, gh, gw, **f32)
+            if g < k:
+                io["fed_prefix"] = torch.empty(k - g, bmax, 2, gh, gw, **f32)
         io["gout"][3:].fill_(1.0)
         return io
+
+    def _noise(self, k0: int):
+        """The fno_noise of the step's rollout calls whose first step is window step k0: step = step_base + cursor,
+        as the start frame's noise."""
+        io = self.io
+        return C.byref(_lib.FnoNoise(self.noise_std, self.noise_seed, io["idx"].data_ptr(), io["step_base"].data_ptr(),
+                                     io["cursor"].data_ptr(), k0))
 
     def _issue(self, b: int, update: bool) -> None:
         lib, io, sw, route, k, g = self.lib, self.io, self.sw, self.route, self.k, self.g
@@ -300,18 +319,31 @@ class _RolloutStepGraphs(_StepGraphs):
         n_el = b * 2 * self.gh * self.gw   # per step
         if g < k:   # the pushforward prefix, without gradient; the trained steps start from its last frame
             pre = io["prefix"].data_ptr()
-            route.call("rollout", C.byref(sw["struct"]), x, mk, cp, pre, k - g, C.byref(ws), b, st)
+            if self.every:
+                route.call("rollout_noise", C.byref(sw["struct"]), x, mk, cp, pre, k - g, C.byref(ws), self._noise(0),
+                           io["fed_prefix"].data_ptr(), b, st)
+            else:
+                route.call("rollout", C.byref(sw["struct"]), x, mk, cp, pre, k - g, C.byref(ws), b, st)
             x = pre + (k - g - 1) * n_el * 4
             labels += (k - g) * n_el * 4
-        route.call("rollout_forward_train", C.byref(sw["struct"]), x, mk, cp, preds, g, C.byref(ts["sv"]), C.byref(ws),
-                   b, st)
+        if self.every:
+            route.call("rollout_forward_train_noise", C.byref(sw["struct"]), x, mk, cp, preds, g, C.byref(ts["sv"]),
+                       C.byref(ws), self._noise(k - g), io["fed"].data_ptr(), b, st)
+        else:
+            route.call("rollout_forward_train", C.byref(sw["struct"]), x, mk, cp, preds, g, C.byref(ts["sv"]),
+                       C.byref(ws), b, st)
         _lib.check(lib.fno_loss_seq_fwd(preds, labels, n_el, g, io["scratch"].data_ptr(), io["loss"].data_ptr(), st),
                    "fno_loss_seq_fwd")
         _lib.check(lib.fno_loss_seq_bwd(preds, labels, io["loss"].data_ptr(), io["gout"].data_ptr(), dpreds, n_el, g, st),
                    "fno_loss_seq_bwd")
-        route.call("rollout_backward", C.byref(sw["struct"]), C.byref(sw["struct_bwd"]), x, mk, cp, preds, dpreds, g,
-                   C.byref(ts["sv"]), C.byref(self.grads), C.byref(ts["sc"]), C.byref(ws), io["carry"].data_ptr(), None,
-                   None, b, st)
+        if self.every:
+            route.call("rollout_backward_noise", C.byref(sw["struct"]), C.byref(sw["struct_bwd"]), x, mk, cp, preds,
+                       dpreds, g, C.byref(ts["sv"]), C.byref(self.grads), C.byref(ts["sc"]), C.byref(ws),
+                       self._noise(k - g), io["fed"].data_ptr(), io["carry"].data_ptr(), None, None, b, st)
+        else:
+            route.call("rollout_backward", C.byref(sw["struct"]), C.byref(sw["struct_bwd"]), x, mk, cp, preds, dpreds,
+                       g, C.byref(ts["sv"]), C.byref(self.grads), C.byref(ts["sc"]), C.byref(ws), io["carry"].data_ptr(),
+                       None, None, b, st)
         if update:
             self._adam_and_log(io["loss"][g].data_ptr(), st)
 
@@ -378,7 +410,7 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
                lr_gamma: float = 0.9, batch_size: int = 2, eval_batch_size: int = 2, log_interval: int = 10,
                eval_interval: int = 2, generator: Optional[torch.Generator] = None, rollout_steps: int = 1,
                time_step_size: Optional[int] = None, input_noise_std: float = 0.0, noise_seed: int = 0,
-               rollout_grad_steps: Optional[int] = None) -> dict:
+               rollout_grad_steps: Optional[int] = None, noise_every_step: bool = False) -> dict:
     """What the reference's `train(model, train_data, dev_data, output_dir, ...)` does (src/train_auto.py:181-313), with
     its argument names and defaults, every training step replayed from a CUDA graph and one synchronisation per epoch.
 
@@ -427,6 +459,23 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
           loss = sum(model.loss_fn(preds=seq[g], labels=b["labels"][K - G + g])["nmse"] for g in range(G)) / G
 
       (at K = 1: `frames.batch(idx, noise_std=...)` and the single-step loss).
+    - noise_every_step=True (with input_noise_std > 0 and K > 1) perturbs the frame every rollout step is fed, not
+      only the start frame: window step k >= 1 is fed its (clean) predecessor plus the noise of stream k,
+      `add_input_noise(x, mask, idx, sigma, noise_seed, t, stream=k)`, in the pushforward prefix and in the trained
+      steps alike.  Predictions and targets stay clean.  It costs one launch and one frame per sample per rollout
+      step.  Without noise, or at K = 1, the flag changes nothing, launch for launch.  One step is bit-identical to
+      the eager loop
+
+          b = frames.rollout_batch(idx, K, noise_std=sigma, noise_seed=noise_seed, noise_step=t)
+          ids = torch.as_tensor(idx, device=b["inputs"].device)
+          x = b["inputs"]
+          for k in range(K - G):
+              if k > 0:
+                  x = add_input_noise(x, b["mask"], ids, sigma, noise_seed, t, stream=k)
+              with torch.no_grad():
+                  x = model.generate_many(x, b["case_params"], b["mask"], 1)[0]
+          seq = model.rollout(x, b["case_params"], b["mask"], G, noise=RolloutNoise(sigma, noise_seed, t, ids, K - G))
+          loss = sum(model.loss_fn(preds=seq[g], labels=b["labels"][K - G + g])["nmse"] for g in range(G)) / G
 
     Returns dict(train_losses=[per-step nmse, every epoch], optimizer=the FusedAdam).  Its state holds the true step
     count (its state_dict loads into torch.optim.Adam), and the parameters' version counters are bumped, so the
@@ -437,7 +486,8 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
     and, as ValueError before any training step, a non-positive rollout_steps or time_step_size, rollout_steps > 1 with
     no time_step_size, a split without a single K-step window, or a split whose frames do not chain.  Also raises
     ValueError before any device work for an input_noise_std that is negative, NaN, infinite or not a real number, a
-    noise_seed that is not an int in [0, 2^64), or a rollout_grad_steps that is not an int in 1..rollout_steps.
+    noise_seed that is not an int in [0, 2^64), a rollout_grad_steps that is not an int in 1..rollout_steps, or a
+    noise_every_step that is not a bool.
     Frozen parameters (requires_grad=False) are not updated, as FusedAdam.step skips them.  Data parallel training in
     this loop is not supported."""
     from .metrics import evaluate_auto
@@ -453,6 +503,8 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
                     ("rollout_steps", rollout_steps)):
         _positive_int(name, v)
     input_noise_std = check_noise_args(input_noise_std, noise_seed, std_name="input_noise_std")
+    if not isinstance(noise_every_step, bool):
+        raise ValueError(f"noise_every_step must be a bool, got {noise_every_step!r}")
     grad_steps = rollout_steps if rollout_grad_steps is None else rollout_grad_steps
     if isinstance(grad_steps, bool) or not isinstance(grad_steps, (int, np.integer)) or not 1 <= grad_steps <= rollout_steps:
         raise ValueError(f"rollout_grad_steps must be an int in 1..rollout_steps={rollout_steps}, got {rollout_grad_steps!r}")
@@ -492,7 +544,7 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
         else:
             _check_chain(frames, windows, rollout_steps, int(tss))
             graphs = _RolloutStepGraphs(model, frames, batch_size, optimizer, windows.size, rollout_steps, int(tss),
-                                        grad_steps, **noise)
+                                        grad_steps, noise_every_step=noise_every_step, **noise)
         print("====== Training ======")
         print(f"# batch: {batch_size}")
         print(f"# examples: {n}")
@@ -501,7 +553,8 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
             if grad_steps < rollout_steps:
                 print(f"# trained steps: the last {grad_steps} (pushforward)")
         if input_noise_std > 0:
-            print(f"# input noise std: {input_noise_std}, seed {int(noise_seed)}")
+            every = ", on every rollout step" if noise_every_step and windows is not None else ""
+            print(f"# input noise std: {input_noise_std}, seed {int(noise_seed)}{every}")
         print(f"# step: {graphs.steps}")
         print(f"# epoch: {num_epochs}")
         start_time = time.time()

@@ -340,6 +340,48 @@ int fno_loss_seq_bwd(const float* preds_seq, const float* labels_seq, const floa
  * the range; status 1 for a null pointer (other than step_offset), n <= 0 or a negative or non-finite std. */
 int fno_add_input_noise(float* inputs, const float* mask, const int64_t* idx, int n, int h, int w_, float std, uint64_t seed,
                         const int64_t* step_base, const int32_t* step_offset, void* stream);
+/* Noise streams: the same noise with counter.x = q + (noise_stream << 16) instead of q, 0 <= noise_stream < 2^16.  Since
+ * q < 2 * 128 * 128 / 4 = 2^13, no two streams share a counter, and stream 0 is fno_add_input_noise's noise bit for bit.
+ * Out of place: out[b][c][y][x] = fmaf(std * z, mask[b][0][y][x], in[b][c][y][x]) where mask != 0, = in[b][c][y][x]
+ * elsewhere; out may equal in.  Arguments and status codes as fno_add_input_noise (in, out: float32 [n][2][h][w]); also
+ * status 1 for noise_stream outside 0 .. 2^16 - 1. */
+#define FNO_NOISE_STREAMS 65536
+int fno_add_input_noise_stream(const float* in, float* out, const float* mask, const int64_t* idx, int n, int h, int w_,
+                               float std, uint64_t seed, const int64_t* step_base, const int32_t* step_offset,
+                               int noise_stream, void* stream);
+
+/* ---- noise on every step of a rollout (train_auto(noise_every_step=True), Fno2d.rollout(noise=...)) ---------------
+ * The *_noise rollout drivers below take a noise descriptor and a fed-frames buffer `fed` [steps][B][2][H][W] float32 next
+ * to preds_seq.  Call step s normally reads the frame x_s (inputs for s = 0, else preds_seq[s-1]); with stream
+ * k = k0 + s >= 1 it reads fed[s] = fno_add_input_noise_stream(x_s, stream k) instead, which the forward drivers write
+ * (one launch per such step) and the backward driver reads for its recomputation and the fc0 weight gradient (it
+ * draws no noise: of the descriptor it reads only k0, the other fields are only checked).  Before its first launch a
+ * forward driver also refuses what its per-step forward would refuse (status 1, or 3 for n_layers).  Stream 0
+ * (a step 0 with k0 = 0) is never applied: the start frame's noise is the gather's (fno_add_input_noise, stream 0), so
+ * fed[0] is then unused.  Full BPTT and a pushforward prefix pass k0 = 0, a trained tail after K - G prefix steps
+ * k0 = K - G.  Predictions stay clean; dfed[s] / dx_s = I, so the gradients w.r.t. the frames flow as without noise.
+ * The step is read on the device (*step_base + *step_offset) when each launch runs.  Every other argument is as in the
+ * driver without noise; status 1 (before any device work) for a null descriptor, fed, idx or step_base, a negative or
+ * non-finite std, k0 < 0 or k0 + steps > 2^16. */
+typedef struct fno_noise {
+  float std;
+  uint64_t seed;
+  const int64_t* idx;          /* [B] dataset index of each window start */
+  const int64_t* step_base;    /* device int64 */
+  const int32_t* step_offset;  /* device int32, or NULL for 0 */
+  int32_t k0;                  /* the noise stream of the call's step 0 */
+} fno_noise;
+int fno_rollout_noise(const fno_weights* w, const float* inputs, const float* mask, const float* case_params,
+                      float* preds_seq, int steps, const fno_workspace* ws, const fno_noise* noise, float* fed, int batch,
+                      int act_dtype, void* stream);
+int fno_rollout_forward_train_noise(const fno_weights* w, const float* inputs, const float* mask, const float* case_params,
+                                    float* preds_seq, int steps, const fno_train_saved* saved, const fno_workspace* ws,
+                                    const fno_noise* noise, float* fed, int batch, int act_dtype, void* stream);
+int fno_rollout_backward_noise(const fno_weights* w, const fno_weights_bwd* wb, const float* inputs, const float* mask,
+                               const float* case_params, const float* preds_seq, const float* dpreds_seq, int steps,
+                               const fno_train_saved* saved, const fno_grads* grads, const fno_bwd_scratch* scratch,
+                               const fno_workspace* ws, const fno_noise* noise, const float* fed, float* carry,
+                               float* d_inputs, float* d_case_params, int batch, int act_dtype, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------
  * Grid-generic path: the same network on H x W frames with 24 <= H <= 128 and 24 <= W <= 128, e.g. CFDBench's
@@ -398,6 +440,19 @@ int fno_grid_rollout_backward(const fno_weights* w, const fno_weights_bwd* wb, c
                               const fno_train_saved* saved, const fno_grads* grads, const fno_bwd_scratch* scratch,
                               const fno_workspace* ws, float* carry, float* d_inputs, float* d_case_params, int batch, int h,
                               int w_, void* stream);
+/* the *_noise rollout drivers (above) on an H x W grid */
+int fno_grid_rollout_noise(const fno_weights* w, const float* inputs, const float* mask, const float* case_params,
+                           float* preds_seq, int steps, const fno_workspace* ws, const fno_noise* noise, float* fed,
+                           int batch, int h, int w_, void* stream);
+int fno_grid_rollout_forward_train_noise(const fno_weights* w, const float* inputs, const float* mask,
+                                         const float* case_params, float* preds_seq, int steps, const fno_train_saved* saved,
+                                         const fno_workspace* ws, const fno_noise* noise, float* fed, int batch, int h, int w_,
+                                         void* stream);
+int fno_grid_rollout_backward_noise(const fno_weights* w, const fno_weights_bwd* wb, const float* inputs, const float* mask,
+                                    const float* case_params, const float* preds_seq, const float* dpreds_seq, int steps,
+                                    const fno_train_saved* saved, const fno_grads* grads, const fno_bwd_scratch* scratch,
+                                    const fno_workspace* ws, const fno_noise* noise, const float* fed, float* carry,
+                                    float* d_inputs, float* d_case_params, int batch, int h, int w_, void* stream);
 /* fno_multistep_metrics on an H x W grid: preds_seq [S][B][2][H][W], label_u and mask [S][B][H][W]; sums [S][B][3] as
  * there (sums over the H*W pixels).  One CTA per (step, case) plane, fixed-order reduction: bit-reproducible.
  * steps <= 65535. */
