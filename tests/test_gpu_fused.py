@@ -21,6 +21,7 @@ import pytest
 import torch
 
 from cfdbench_b200 import synth
+from oracle import error_bounds as eb
 from oracle import fno_numpy as onp
 from oracle import fno_torch_port as opt
 
@@ -159,7 +160,11 @@ def test_mode_mix_ring_recycling_large_batch(lib):
 @pytest.mark.parametrize("batch", [1, 3, 80])
 def test_block_fused_kernel(lib, batch):
     """irfft2 (both stages on tensor cores, Z kept on chip) + 1x1 conv + bias + GELU, bf16 in / bf16 out.
-    80 samples = 320 work units on 132 CTAs: every CTA runs two or three units (image ring phase wrap-around)."""
+    80 samples = 320 work units on 132 CTAs: every CTA runs two or three units (image ring phase wrap-around).
+    Every store is checked by the bf16 interval rule; the share of stores that differ from the rounded float64 value
+    (rounding flips) is printed.  Against the earlier "one ulp + 2e-6 max(1, |lin|)" rule it is stricter for large
+    outputs (a store off by one ulp must have its float64 value within the bound of the rounding boundary) and looser for
+    outputs near 0, where the absolute part of the bound (~1e-4 at this test's C2R scale) spans several bf16 ulps."""
     from cfdbench_b200 import _lib
     rng = np.random.default_rng(20 + batch)
     ym = (rng.standard_normal((batch, 32, 24, 12)) + 1j * rng.standard_normal((batch, 32, 24, 12))) * 40.0
@@ -173,18 +178,14 @@ def test_block_fused_kernel(lib, batch):
     _lib.check(lib.fno_block_fused(img.data_ptr(), xd.data_ptr(), w0td.data_ptr(), biasd.data_ptr(), out.data_ptr(), batch,
                                    stream()), "block_fused")
     torch.cuda.synchronize()
-    spec = onp.spectral_inverse(ym.astype(np.complex128), 64, 64, 12, 12)
-    lin = spec + np.einsum("oi,bihw->bohw", w0.astype(np.float64), x.float().numpy().astype(np.float64))
-    lin = lin + bias.astype(np.float64)[None, :, None, None]
-    ref = onp.gelu(lin)
     got = out.float().cpu().numpy().astype(np.float64)
-    ref16 = torch.from_numpy(ref.astype(np.float32)).to(torch.bfloat16).float().numpy().astype(np.float64)
+    # float64 block on the mode image the kernel read (hi + lo); each store must be the bf16 rounding of a value within the
+    # kernel's fp32 evaluation error (oracle/error_bounds.py: KAPPA_BLOCK_FUSED, GELU)
+    dec, _ = decode_ym_image(img.cpu().numpy(), batch)
+    ref, bound, _, _ = eb.block_out(dec, x.float().numpy().astype(np.float64), w0, bias, "gelu", eb.KAPPA_BLOCK_FUSED)
     assert rel(got, ref) < 3e-3, rel(got, ref)          # bf16 output rounding alone is ~1.6e-3
-    diff = np.abs(got - ref16)
-    # one ulp of the rounded result + the fp32 evaluation error of the pre-activation (3xTF32 sums ~1e-6 |lin|, GELU 3e-7)
-    allowed = 1.0001 * bf16_ulp(ref16) + 2e-6 * np.maximum(1.0, np.abs(lin))
-    assert np.all(diff <= allowed), float((diff / allowed).max())
-    assert (diff > 0).mean() < 5e-3, float((diff > 0).mean())   # rounding flips only (measured 1e-3 .. 3e-3)
+    flips = eb.check(f"block_fused B={batch}", got, ref, bound, tiles=eb.pixel_tiles(), bf16=True)
+    print(f"\n[block_fused B={batch}] flipped share {flips:.3g}")
 
 
 def test_block_fused_equals_unfused_path(lib):

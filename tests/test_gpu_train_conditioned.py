@@ -7,7 +7,8 @@ different bf16 neighbours and the layers behind amplify those flips (DESIGN.md 5
 stage of the forward, and the whole backward, is a fixed computation with no rounding boundary in between: the backward
 is a linear map of d(preds) evaluated in fp32.  So each is compared here with a float64 restatement fed the same saved
 tensors (`oracle.fno_numpy.fno_vjp_saved` for the backward), at fp32-level bounds in BOTH storage modes.  The only
-exception is a bf16 store, which must be the correctly rounded float64 value up to one-ulp flips.
+exception is a bf16 store, which must be the bf16 rounding of some value within the fp32 evaluation error of the float64
+value (oracle.error_bounds.bf16_interval).
 
 Every check is reported (`-s` prints the measured maxima) before it is asserted."""
 import json
@@ -18,15 +19,15 @@ import torch
 from scipy.special import erf
 
 from cfdbench_b200 import synth
+from oracle import error_bounds as eb
 from oracle import fno_numpy as onp
 
-from test_gpu_fused import assert_within_flip_ambiguity, bf16_ulp
+from test_gpu_fused import assert_within_flip_ambiguity
 
 pytestmark = pytest.mark.gpu
 
 CHUNK_EDGES = (0, 31, 32, 63, 64)   # first / last samples of the project backward's 32-sample chunks
 BARS = {"a0": 2e-6, "xm": 2e-6, "pre": 3e-6, "act": 1e-6, "preds": 3e-6}   # forward stages, per-sample max rel L2
-BF16_FLIP_FRACTION = 5e-3   # bf16 stores: at most this share of elements one bf16 ulp off the rounded float64 value
 
 
 def backward_bar(depth: int, what: str) -> float:
@@ -124,14 +125,13 @@ def _bf16_key(x):
     return np.where(u & 0x8000, -(u & 0x7FFF), u)
 
 
-def _bf16_store_errors(got, ref64, eval_err=0.0):
-    """A bf16 store against the float64 value rounded to bf16: (largest distance in bf16 ulps, share of elements that
-    differ, number of elements more than one ulp off and farther than one ulp + `eval_err` from the float64 value, where
-    `eval_err` bounds the fp32 evaluation error of the stored value).  `got` holds the stored bf16 values (exact in
-    float64)."""
+def _bf16_store_errors(got, ref64, bound):
+    """A bf16 store against the float64 value: (largest distance in bf16 ulps from the float64 value rounded to bf16,
+    share of elements that differ from it, number of elements that are not the bf16 rounding of any value within `bound`
+    of the float64 value, where `bound` bounds the fp32 evaluation error of the stored value).  `got` holds the stored
+    bf16 values (exact in float64)."""
     steps = np.abs(_bf16_key(got) - _bf16_key(onp.bf16_round(ref64)))
-    beyond = (steps > 1) & (np.abs(got - ref64) > eval_err + bf16_ulp(got))
-    return int(steps.max()), float((steps != 0).mean()), int(beyond.sum())
+    return int(steps.max()), float((steps != 0).mean()), int(eb.bf16_interval(got, ref64, bound).sum())
 
 
 def _project(sd, a, mask, chunk=32):
@@ -178,12 +178,12 @@ def test_training_pass_stages_against_float64_conditioned_on_saved_tensors(where
         if not value <= bar:
             fails.append((name, value, bar))
 
-    def check_store(name, got, ref64, eval_err=0.0):
+    def check_store(name, got, ref64, eval_err):
         if bf:
-            ulps, share, beyond = _bf16_store_errors(got, ref64, eval_err)
-            errs[name + ".ulps"], errs[name + ".flip_share"], errs[name + ".beyond"] = ulps, share, beyond
-            if beyond or share >= BF16_FLIP_FRACTION:
-                fails.append((name, ulps, share, beyond))
+            ulps, share, outside = _bf16_store_errors(got, ref64, eval_err)
+            errs[name + ".ulps"], errs[name + ".flip_share"], errs[name + ".outside"] = ulps, share, outside
+            if outside:
+                fails.append((name, ulps, share, outside))
         else:
             check(name, _max_rel(got, ref64), BARS["a0" if name == "a0" else "act"])
 
@@ -202,7 +202,9 @@ def test_training_pass_stages_against_float64_conditioned_on_saved_tensors(where
         pre = onp.spectral_inverse(np.einsum("bikl,iokl->bokl", xm, wt, optimize=True), gh, gw, 12, 12) \
             + onp.conv1x1(acts[l], sd[f"blocks.{l}.w0.weight"], sd[f"blocks.{l}.w0.bias"])
         check(f"pre[{l}]", _max_rel(pres[l], pre), BARS["pre"])
-        check_store(f"act[{l + 1}]", acts[l + 1], _gelu(pres[l]))
+        # the GELU of the saved fp32 pre-activation: the degree-8 fit's error and the fp32 rounding of its result
+        ref_act = _gelu(pres[l])
+        check_store(f"act[{l + 1}]", acts[l + 1], ref_act, eb.GELU_FIT[8] + 2.0 ** -24 * np.abs(ref_act))
     preds_np = _f64(preds)
     preds_ref = _project(sd, acts[depth], mask)
     if bf:
