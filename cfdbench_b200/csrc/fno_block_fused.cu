@@ -7,10 +7,11 @@
 // constant is loaded once.  Per unit:
 //   GEMM1 (inverse DFT along kx, 3xTF32):  Z1[(ky, o) 384][(h', re|im) 32] = Y^T[(ky, o)][(kx, re|im) 48] * F[(h', ri)][.]^T
 //          six m64n32k8 chains, one per ky pair; A = the mode image of the sample (fno_mode_mix.cu writes it with the
-//          tf32 hi/lo split done), loaded from shared memory into A-fragment registers -- the image's 32-byte chunk
-//          swizzle makes those loads conflict-free -- and B = the constant F (K-major); Z1 -> tf32 hi/lo -> Zt, the
-//          K-major B operand of GEMM2 per image row (96 KB for 16 rows).  Bias rides in the row that irfft2's C2R stage
-//          ignores (Im of ky = 0).
+//          tf32 hi/lo split done), loaded from the warpgroup's image slot into A-fragment registers -- the image's
+//          32-byte chunk swizzle makes those loads conflict-free -- and B = the constant F (K-major); Z1 -> tf32 hi/lo ->
+//          Zt, the K-major B operand of GEMM2 per image row (96 KB for 16 rows).  GEMM1's M rows are ordered so that a thread's two fragment rows are
+//          the two ky of its pair at one channel: its four values of an (h', o) form one 16-byte chunk of Zt, one
+//          st.shared.v4 per hi / lo.  Bias rides in the row that irfft2's C2R stage ignores (Im of ky = 0).
 //   GEMM2 per image row h:  D[64 w][32 o] = E[w][(ky, ri) 24] Zt_h + X_h[w][32 i] W0^T
 //          E Zt_h: m64n32k8 tf32, 3xTF32 (E = C2R stage with c_ky/HW folded in, fno_block_tc.cu builds it); E's hi / lo
 //          A fragments are loaded into registers once per CTA, so only Zt_h is read from shared memory.
@@ -19,11 +20,15 @@
 //          the same fp32 registers.  x is exact in bf16.
 //          Epilogue exact-erf GELU -> bf16x2 -> stmatrix.trans into the swizzled [o][w] staging tile -> one TMA store
 //          per row.
-// Roles: warp 8 lanes 0/1 -- producers of the two image slots (24 KB = one ky pair, hi + lo, two bulk copies each);
-// warpgroups 0 / 1 -- the even / odd ky pairs of GEMM1 and the even / odd rows of GEMM2.  Each warpgroup owns a ring of
-// kFzXSlots activation rows; its thread 0 refills a slot as soon as the MMAs that read it have completed, so the ring
-// runs up to kFzXSlots rows ahead, across GEMM1 and across unit boundaries.  GEMM2 keeps two accumulator sets: the MMAs of
-// row r + 1 run while row r's epilogue does.
+// Roles: warpgroups 0 / 1 -- the even / odd ky pairs of GEMM1 and the even / odd rows of GEMM2.  Each warpgroup owns
+// one image slot (24 KB = one ky pair, hi + lo, two bulk copies by its thread 0) and reads the three pairs of the next
+// unit from it into three fragment sets during GEMM2, one pair every other row; the slot is refilled right after the
+// row barrier that follows its reads.  So GEMM1 waits for no image, and with two accumulator sets pair 1's MMAs run
+// while pair 0 is split and stored, pair 2's while pair 1 is.  (A ninth, producer warp would cap the registers at
+// those of three warpgroups, 168, too few for the fragment sets.)  Each warpgroup owns a ring of kFzXSlots activation
+// rows; its thread 0 refills a slot as soon as the MMAs that read it have completed, so the ring runs up to kFzXSlots rows
+// ahead, across GEMM1 and across unit boundaries.  GEMM2 keeps two accumulator sets: the MMAs of row r + 1 run while row
+// r's epilogue does.
 #include "fno_common.cuh"
 #include "tc_common.cuh"
 #include "tc_tma.cuh"
@@ -35,12 +40,12 @@ namespace fno {
 constexpr int kFzRows = 16;                            // image rows per unit
 constexpr int kFzChunks = kH / kFzRows;                // 4
 constexpr int kFzWgRows = kFzRows / 2;                 // GEMM2 rows per warpgroup and unit
-constexpr int kFzThreads = 9 * 32;                     // 2 warpgroups + producer warp
-constexpr int kFzProdWarp = 8;
+constexpr int kFzThreads = 8 * 32;                     // 2 warpgroups
 constexpr int kZK = 2 * kM2;                           // 24: (ky, re|im)
 constexpr int kImgK = 2 * kKX;                         // 48: (kx, re|im) image rows
 constexpr size_t kYmImgBytes = 147456;                 // per sample: [hi|lo][ky 12][48 rows][32 o] fp32
-constexpr uint32_t kFzStage = 4 * 6144;                // one ky pair: hi (2 x 6144 B) then lo
+constexpr uint32_t kImgKyBytes = kImgK * kC * 4;       // 6144: one ky of the hi or the lo image
+constexpr uint32_t kFzStage = 4 * kImgKyBytes;         // one ky pair: hi (2 x 6144 B) then lo
 constexpr int kFzFFloats = 2 * (2 * kFzRows) * kImgK;  // [n = 2 h' + ri (32)][48], hi | lo: per chunk
 constexpr int kFzEFloats = 2 * kW * kZK;               // [64 w][24] hi | lo
 constexpr uint32_t kFzZtFloats = kC * kZK;             // one image row, hi or lo: [32 o][24 k] K-major
@@ -61,13 +66,13 @@ __host__ __device__ constexpr uint32_t fz_x_parity(int n) { return static_cast<u
 struct FzSmem {
   alignas(1024) unsigned char x[2][kFzXSlots][kFzRowBytes];   // per warpgroup: activation ring (TMA, 128B swizzle)
   alignas(1024) unsigned char st[2][2][kFzRowBytes];          // per warpgroup: double-buffered output staging tile
-  alignas(128) unsigned char y[2][kFzStage];           // image ring (slot = parity of the ky pair)
+  alignas(128) unsigned char y[2][kFzStage];           // per warpgroup: image slot
   alignas(128) float zt[kFzRows][2][kFzZtFloats];      // GEMM2 B operand per row: hi, lo
   alignas(128) float f_hi[kFzFFloats / 2];
   alignas(128) float f_lo[kFzFFloats / 2];
   alignas(128) unsigned char w0[3][kFzW0Bytes];        // B[n = o][k = i] = W0[o][i] = t1 + t2 + t3 (bf16 terms)
   alignas(16) float bias[kC];
-  alignas(8) uint64_t y_full[2], y_free[2];
+  alignas(8) uint64_t y_full[2];
   alignas(8) uint64_t x_full[2][kFzXSlots];
 };
 static_assert(sizeof(FzSmem) <= 232448, "block_fused_kernel: shared memory over the per-block opt-in limit");
@@ -92,8 +97,7 @@ __global__ void __launch_bounds__(kFzThreads, 1)
   // ---------------------------------------------------------------- prologue (constants and weights only)
   if (tid == 0) {
     for (int i = 0; i < 2; ++i) {
-      mbar_init(&sm.y_full[i], 1);
-      mbar_init(&sm.y_free[i], 4);   // the four warps of the warpgroup that reads the slot
+      mbar_init(&sm.y_full[i], 1);   // thread 0 of the warpgroup: expect_tx
       for (int s = 0; s < kFzXSlots; ++s) mbar_init(&sm.x_full[i][s], 1);   // thread 0 of the warpgroup: expect_tx
     }
     fence_mbar_init();
@@ -120,25 +124,6 @@ __global__ void __launch_bounds__(kFzThreads, 1)
   pdl_wait();   // the image and x come from the previous kernels of the chain
   pdl_launch_dependents();
 
-  // ================================================================ producers: lane s fills image slot s
-  if (warp == kFzProdWarp) {
-    if (lane < 2) {
-      const int s = lane;
-      for (int u = 0; u < n_units; ++u) {
-        const unsigned char* src = img + static_cast<size_t>(b0 + u * bstride) * kYmImgBytes;
-        for (int pi = 0; pi < 3; ++pi) {
-          const int p = s + 2 * pi, f = 3 * u + pi;   // ky pair p, fill number f of the slot
-          if (f >= 1) mbar_wait(&sm.y_free[s], (f - 1) & 1);
-          mbar_expect_tx(&sm.y_full[s], kFzStage);
-          bulk_g2s(sm.y[s], src + p * (kFzStage / 2), kFzStage / 2, &sm.y_full[s]);
-          bulk_g2s(sm.y[s] + kFzStage / 2, src + kYmImgBytes / 2 + p * (kFzStage / 2), kFzStage / 2, &sm.y_full[s]);
-        }
-      }
-    }
-    return;
-  }
-
-  // ================================================================ consumers
   const int g = warp >> 2, wq = warp & 3, q = lane & 3, t = tid & 127;
   const int m0 = 16 * wq + (lane >> 2);   // fragment rows m0, m0 + 8
   const int n_fills = kFzWgRows * n_units;
@@ -148,8 +133,20 @@ __global__ void __launch_bounds__(kFzThreads, 1)
     mbar_expect_tx(&sm.x_full[g][s], kFzRowBytes);
     tma_load_3d(sm.x[g][s], &x_map, 0, kFzRows * chunk + g + 2 * r, (b0 + u * bstride) * kC, &sm.x_full[g][s]);
   };
-  if (t == 0)
+  // fill f of this warpgroup's image slot: ky pair g + 2 (f % 3) of unit f / 3, hi and lo (thread t == 0); fill f
+  // completes phase f of y_full[g] and is issued once all 128 threads have read fill f - 1
+  const int n_yfills = 3 * n_units;
+  auto y_fill = [&](int f) {
+    const unsigned char* src = img + static_cast<size_t>(b0 + (f / 3) * bstride) * kYmImgBytes +
+                               (g + 2 * (f % 3)) * (kFzStage / 2);
+    mbar_expect_tx(&sm.y_full[g], kFzStage);
+    bulk_g2s(sm.y[g], src, kFzStage / 2, &sm.y_full[g]);
+    bulk_g2s(sm.y[g] + kFzStage / 2, src + kYmImgBytes / 2, kFzStage / 2, &sm.y_full[g]);
+  };
+  if (t == 0) {
+    if (n_yfills > 0) y_fill(0);
     for (int n = 0; n < kFzXSlots && n < n_fills; ++n) x_fill(n);
+  }
   const uint32_t w0_s = tc::smem_addr(sm.w0[0]);
   // A fragments of E (tf32 m64k8, rows w = m0, m0 + 8) for the C2R passes of every row: e_frag[0 / 1] = hi / lo
   uint32_t e_frag[2][kZK / 8][4];
@@ -163,59 +160,86 @@ __global__ void __launch_bounds__(kFzThreads, 1)
         e_frag[hl][ks][j] = __float_as_uint(__ldg(etab + hl * (kFzEFloats / 2) + off));
       }
 
-  for (int u = 0; u < n_units; ++u) {
-    const int b = b0 + u * bstride;
-    // ---------------------------------------------------------------- GEMM1: ky pairs g, g + 2, g + 4
-    for (int pi = 0; pi < 3; ++pi) {
-      const int p = g + 2 * pi, f = 3 * u + pi;
-      mbar_wait(&sm.y_full[g], f & 1);
-      // A[m = (ky - 2p) * 32 + o][kk] = image[ky][kk][o]: line kk, 32-byte chunk (o / 8) ^ (kk & 3)
-      uint32_t a_hi[6][4], a_lo[6][4];
+  // GEMM1 row m = 16 wq + 8 hh + j holds ky = 2p + hh and channel o = 8 wq + j, so the fragment rows m0, m0 + 8 of a
+  // thread are (2p, o1) and (2p + 1, o1) with o1 = 8 wq + lane / 4.
+  const int o1 = 8 * wq + (lane >> 2);
+  // A fragments of fill f of the slot, tf32 hi [0] / lo [1]: A[m][kk] = image[2p + hh][kk][o], line kk of the ky,
+  // 32-byte chunk (o / 8) ^ (kk & 3) = wq ^ (kk & 3), word o & 7; the lanes of a load cover 8 words of 4 chunks with
+  // distinct swizzle phases: no bank conflicts.
+  auto load_pair = [&](uint32_t (&a)[2][kImgK / 8][4], int f) {
+    mbar_wait(&sm.y_full[g], f & 1);
+#pragma unroll
+    for (int ks = 0; ks < kImgK / 8; ++ks)
+#pragma unroll
+      for (int r = 0; r < 4; ++r) {
+        const int kk = 8 * ks + q + 4 * (r >> 1);
+        const uint32_t off = (r & 1) * kImgKyBytes + kk * 128 + ((wq ^ (kk & 3)) << 5) + (lane >> 2) * 4;
+        a[0][ks][r] = *reinterpret_cast<const uint32_t*>(sm.y[g] + off);
+        a[1][ks][r] = *reinterpret_cast<const uint32_t*>(sm.y[g] + kFzStage / 2 + off);
+      }
+  };
+  // the 18 MMAs of one ky pair, one commit group: Y_hi F_hi + Y_lo F_hi + Y_hi F_lo
+  auto issue_pair = [&](float (&acc)[16], const uint32_t (&a)[2][kImgK / 8][4]) {
+    tc::wg_fence();
+#pragma unroll
+    for (int pass = 0; pass < 3; ++pass) {
+      const uint32_t fb = tc::smem_addr(pass == 2 ? sm.f_lo : sm.f_hi);
 #pragma unroll
       for (int ks = 0; ks < kImgK / 8; ++ks)
-#pragma unroll
-        for (int r = 0; r < 4; ++r) {
-          const int m = m0 + 8 * (r & 1), kk = 8 * ks + q + 4 * (r >> 1), o = m & 31;
-          const uint32_t off = (m >> 5) * 6144 + kk * 128 + (((o >> 3) ^ (kk & 3)) << 5) + (o & 7) * 4;
-          a_hi[ks][r] = *reinterpret_cast<const uint32_t*>(sm.y[g] + off);
-          a_lo[ks][r] = *reinterpret_cast<const uint32_t*>(sm.y[g] + kFzStage / 2 + off);
-        }
-      float acc[16];
-      tc::wg_fence();
-#pragma unroll
-      for (int pass = 0; pass < 3; ++pass) {   // Y_hi F_hi + Y_lo F_hi + Y_hi F_lo
-        const uint32_t fb = tc::smem_addr(pass == 2 ? sm.f_lo : sm.f_hi);
-#pragma unroll
-        for (int ks = 0; ks < kImgK / 8; ++ks)
-          tc::wg_tf32_rs_n32(acc, pass == 1 ? a_lo[ks] : a_hi[ks], tc::make_smem_desc(fb + ks * 2 * kLboF, kLboF, 128),
-                             (pass | ks) ? 1u : 0u);
-      }
-      tc::wg_commit();
-      // the MMAs above were issued, so the fragments they take from registers have been loaded from the stage: the
-      // producer may refill it while they run
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&sm.y_free[g]);
-      tc::wg_wait<0>();
-      tc::wg_fence_acc(acc);
-      if (pi == 0) tc::named_barrier(1, 256);   // both warpgroups are done with the previous unit's Zt
-      // acc[4 i + 2 hh + e] = Z1[m0 + 8 hh][n = 8 i + 2 q + e]: row h' = 4 i + q, re|im = e
-#pragma unroll
-      for (int hh = 0; hh < 2; ++hh) {
-        const int m = m0 + 8 * hh, ky = 2 * p + (m >> 5), o = m & 31;
-#pragma unroll
-        for (int i = 0; i < 4; ++i)
-#pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            float v = acc[4 * i + 2 * hh + e];
-            if (ky == 0 && e == 1) v = sm.bias[o];   // Im of ky = 0: C2R ignores it, the E column there is 1
-            float hi, lo;
-            tc::split_tf32(v, hi, lo);
-            const uint32_t off = tc::kmajor_offset(o, 2 * ky + e, kC) / 4;
-            sm.zt[4 * i + q][0][off] = hi;
-            sm.zt[4 * i + q][1][off] = lo;
-          }
-      }
+        tc::wg_tf32_rs_n32(acc, a[pass == 1][ks], tc::make_smem_desc(fb + ks * 2 * kLboF, kLboF, 128),
+                           (pass | ks) ? 1u : 0u);
     }
+    tc::wg_commit();
+  };
+  // acc[4 i + 2 hh + e] = Z1[(2p + hh, o1)][n = 8 i + 2 q + e]: row h' = 4 i + q, k = 4p + 2 hh + e, i.e. the four
+  // values of a given i are the 16-byte chunk (o1, k = 4p .. 4p + 3) of Zt row h'
+  auto store_pair = [&](const float (&acc)[16], int p) {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      float v[4] = {acc[4 * i], acc[4 * i + 1], acc[4 * i + 2], acc[4 * i + 3]};
+      if (p == 0) v[1] = sm.bias[o1];   // Im of ky = 0: C2R ignores it, the E column there is 1
+      float4 hi, lo;
+      tc::split_tf32(v[0], hi.x, lo.x);
+      tc::split_tf32(v[1], hi.y, lo.y);
+      tc::split_tf32(v[2], hi.z, lo.z);
+      tc::split_tf32(v[3], hi.w, lo.w);
+      const uint32_t off = tc::kmajor_offset(o1, 4 * p, kC) / 4;
+      *reinterpret_cast<float4*>(&sm.zt[4 * i + q][0][off]) = hi;
+      *reinterpret_cast<float4*>(&sm.zt[4 * i + q][1][off]) = lo;
+    }
+  };
+  // ky pairs g, g + 2, g + 4 of unit u in fragment sets a0, a1, a2 (fills 3 u, 3 u + 1, 3 u + 2), read during unit
+  // u - 1's GEMM2 (unit 0: here)
+  uint32_t a0[2][kImgK / 8][4], a1[2][kImgK / 8][4], a2[2][kImgK / 8][4];
+  auto first_pair = [&](uint32_t (&a)[2][kImgK / 8][4], int f) {
+    load_pair(a, f);
+    tc::named_barrier(2 + g, 128);   // all 128 threads have read fill f
+    if (t == 0 && f + 1 < n_yfills) y_fill(f + 1);
+  };
+  if (n_units > 0) {
+    first_pair(a0, 0);
+    first_pair(a1, 1);
+    first_pair(a2, 2);
+  }
+
+  for (int u = 0; u < n_units; ++u) {
+    const int b = b0 + u * bstride;
+    const bool more = u + 1 < n_units;
+    // ---------------------------------------------------------------- GEMM1: ky pairs g, g + 2, g + 4
+    float acc1[2][16];
+    issue_pair(acc1[0], a0);
+    issue_pair(acc1[1], a1);
+    tc::wg_wait<1>();   // pair g
+    tc::wg_fence_acc(acc1[0]);
+    tc::named_barrier(1, 256);   // both warpgroups are done with the previous unit's Zt
+    store_pair(acc1[0], g);
+    issue_pair(acc1[0], a2);
+    tc::wg_wait<1>();   // pair g + 2
+    tc::wg_fence_acc(acc1[1]);
+    store_pair(acc1[1], g + 2);
+    tc::wg_wait<0>();   // pair g + 4: a0, a1, a2 are free
+    tc::wg_fence_acc(acc1[0]);
+    store_pair(acc1[0], g + 4);
     tc::fence_proxy_async_smem();
     tc::named_barrier(1, 256);   // Zt of all 16 rows is complete
 
@@ -253,6 +277,11 @@ __global__ void __launch_bounds__(kFzThreads, 1)
             tc::wg_bf16_rs_n32(acc[r & 1], x_frag[r & 1][ks],
                                tc::make_smem_desc(w0_s + term * kFzW0Bytes + ks * 2 * kLboO, kLboO, 128), 1u);
         tc::wg_commit();
+        // the next unit's image fragments, one ky pair every other row (fill 3 u + 3 + r / 2); the row barrier below
+        // frees the slot for the next fill, which then has two rows to land
+        if (more && r == 1) load_pair(a0, 3 * u + 3);
+        if (more && r == 3) load_pair(a1, 3 * u + 4);
+        if (more && r == 5) load_pair(a2, 3 * u + 5);
       }
       if (r == 0) continue;
       const int rr = r - 1, h = kFzRows * chunk + g + 2 * rr;
@@ -291,6 +320,8 @@ __global__ void __launch_bounds__(kFzThreads, 1)
         bulk_commit_group();
         const int nf = kFzWgRows * u + rr + kFzXSlots;
         if (nf < n_fills) x_fill(nf);
+        // all 128 threads have read image fill 3 u + 3 + r / 2 (this row's loads precede the barrier above)
+        if (more && (r == 1 || r == 3 || r == 5) && 3 * u + 4 + (r >> 1) < n_yfills) y_fill(3 * u + 4 + (r >> 1));
       }
     }
   }
