@@ -6,6 +6,8 @@ Public surface mirrors the reference's for this path:
     MseLoss, loss_name_to_fn               (reference src/models/loss.py)
     infer_multistep                        (reference src/test_multistep.py infer, batched on the device)
     evaluate_auto                          (reference src/train_auto.py evaluate, batched on the device)
+    evaluate_rollout_auto                  (a split's S-step rollout error, on the device; train_auto's
+                                            dev_rollout_steps=S selects checkpoints by it)
     train_auto                             (reference src/train_auto.py train, steps replayed from CUDA graphs;
                                             rollout_steps=K trains through K-step rollouts)
     rollout_windows                        (the valid K-step window starts of a split)
@@ -15,7 +17,7 @@ from .base_model import AutoCfdModel
 from .loss import MseLoss, loss_name_to_fn
 
 __all__ = ["AutoCfdModel", "MseLoss", "loss_name_to_fn", "Fno2d", "FnoBlock", "SpectralConv2d_fast", "FusedAdam", "DeviceFrames",
-           "infer_multistep", "evaluate_auto", "train_auto",
+           "infer_multistep", "evaluate_auto", "evaluate_rollout_auto", "train_auto",
            "rollout_windows", "RolloutNoise", "add_input_noise"]
 
 
@@ -35,6 +37,9 @@ def __getattr__(name):  # lazy: importing the package must not require the nativ
     if name == "evaluate_auto":
         from .metrics import evaluate_auto
         return evaluate_auto
+    if name == "evaluate_rollout_auto":
+        from .metrics import evaluate_rollout_auto
+        return evaluate_rollout_auto
     if name in ("rollout_windows", "RolloutNoise", "add_input_noise"):
         from . import data
         return getattr(data, name)

@@ -176,6 +176,9 @@ SIGNATURES = {
     "fno_loss_seq_scratch_bytes": (C.c_size_t, [_I]),
     "fno_loss_seq_fwd": (C.c_int, [_P, _P, C.c_size_t, _I, _P, _P, _P]),
     "fno_loss_seq_bwd": (C.c_int, [_P, _P, _P, _P, _P, C.c_size_t, _I, _P]),
+    # rollout metrics of a split's windows
+    "fno_window_metrics": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, C.c_int64, _I, _P, _P]),
+    "fno_grid_window_metrics": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, C.c_int64, _I, _P, _I, _I, _P]),
     # training noise
     "fno_add_input_noise": (C.c_int, [_P, _P, _P, _I, _I, _I, _F, C.c_uint64, _P, _P, _P]),
     "fno_add_input_noise_stream": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _F, C.c_uint64, _P, _P, _I, _P]),

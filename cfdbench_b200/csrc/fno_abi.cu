@@ -86,6 +86,11 @@ cudaError_t launch_grid_gather_window(const void*, const void*, const float*, co
 cudaError_t launch_loss_seq_fwd(const float*, const float*, size_t, int, float*, float*, cudaStream_t);
 cudaError_t launch_loss_seq_bwd(const float*, const float*, const float*, const float*, float*, size_t, int, cudaStream_t);
 size_t loss_seq_scratch_bytes(int);
+// rollout metrics of a device-resident split's windows (fno_metrics.cu)
+cudaError_t launch_window_metrics(const float*, const void*, const void*, const long long*, int, int, int, long long, int,
+                                  float*, cudaStream_t);
+cudaError_t launch_grid_window_metrics(const float*, const void*, const void*, const long long*, int, int, int, long long,
+                                       int, float*, int, int, cudaStream_t);
 cudaError_t launch_add_input_noise(float*, const float*, const long long*, int, int, int, float, unsigned long long,
                                    const long long*, const int*, cudaStream_t);
 cudaError_t launch_input_noise_stream(const float*, float*, const float*, const long long*, int, int, int, float,
@@ -1249,3 +1254,43 @@ int fno_eval_sums(const float* preds, const float* label, const float* mask, con
 }
 
 }  // extern "C"
+
+// ------------------------------------------------------------------------------------------------ window rollout metrics
+static int window_metrics_args(const char* what, const float* preds_seq, const void* frames_in, const void* frames_out,
+                               const int64_t* starts, int steps, int batch, int time_step_size, int64_t n_frames,
+                               int frame_dtype, const float* sums) {
+  char msg[160];
+  if (!preds_seq || !frames_in || !frames_out || !starts || !sums || steps < 1 || steps > 65535 || batch < 1 ||
+      time_step_size < 1 || n_frames < 1 || bad_dtype(frame_dtype)) {
+    snprintf(msg, sizeof(msg), "%s: bad argument", what);
+    return fail(kErrArg, msg);
+  }
+  return kOk;
+}
+
+int fno_window_metrics(const float* preds_seq, const void* frames_in, const void* frames_out, const int64_t* starts,
+                       int steps, int batch, int time_step_size, int64_t n_frames, int frame_dtype, float* sums,
+                       void* stream) {
+  FNO_TRY(window_metrics_args("fno_window_metrics", preds_seq, frames_in, frames_out, starts, steps, batch, time_step_size,
+                              n_frames, frame_dtype, sums));
+  const uintptr_t frame_align = frame_dtype == FNO_ACT_BF16 ? 7 : 15;   // the 64x64 kernel's vector loads
+  if ((reinterpret_cast<uintptr_t>(preds_seq) & 15) ||
+      ((reinterpret_cast<uintptr_t>(frames_in) | reinterpret_cast<uintptr_t>(frames_out)) & frame_align))
+    return fail(kErrArg, "fno_window_metrics: preds_seq must be 16-byte aligned, the frames 16-byte (fp32) or 8-byte (bf16)");
+  FNO_CUDA(launch_window_metrics(preds_seq, frames_in, frames_out, reinterpret_cast<const long long*>(starts), steps, batch,
+                                 time_step_size, n_frames, frame_dtype == FNO_ACT_BF16, sums, S(stream)),
+           "window_metrics_kernel");
+  return kOk;
+}
+
+int fno_grid_window_metrics(const float* preds_seq, const void* frames_in, const void* frames_out, const int64_t* starts,
+                            int steps, int batch, int time_step_size, int64_t n_frames, int frame_dtype, float* sums, int h,
+                            int wd, void* stream) {
+  FNO_TRY(grid_arg("fno_grid_window_metrics", h, wd));
+  FNO_TRY(window_metrics_args("fno_grid_window_metrics", preds_seq, frames_in, frames_out, starts, steps, batch,
+                              time_step_size, n_frames, frame_dtype, sums));
+  FNO_CUDA(launch_grid_window_metrics(preds_seq, frames_in, frames_out, reinterpret_cast<const long long*>(starts), steps,
+                                      batch, time_step_size, n_frames, frame_dtype == FNO_ACT_BF16, sums, h, wd, S(stream)),
+           "window_metrics_kernel");
+  return kOk;
+}

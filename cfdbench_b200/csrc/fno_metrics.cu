@@ -8,24 +8,21 @@ namespace fno {
 
 constexpr int kMtThreads = 256;
 
-// preds_seq [S][B][2][64][64] (channel 0 = u), label_u [S][B][64][64], mask [S][B][64][64]
-// out [S][B][3] = (sum (p-l)^2, sum l^2, sum |p-l|) over the 4096 pixels, with p, l multiplied by the mask
-__global__ void __launch_bounds__(kMtThreads)
-    multistep_metrics_kernel(const float* __restrict__ preds_seq, const float* __restrict__ label_u,
-                             const float* __restrict__ mask, float* __restrict__ out, int batch) {
+// The per-plane reduction of every rollout-metrics kernel (multistep_metrics_kernel, grid_multistep_metrics_kernel,
+// window_metrics_kernel), one function so that their sums agree bit for bit on the same pixels.  A plane is n_items
+// items of kVec consecutive pixels; thread t takes items t, t + 256, ..., and `load(i, pp, ll)` gives item i's masked
+// predictions and labels.  Per pixel, in order: d = pp - ll, se = fmaf(d, d, se), sl = fmaf(ll, ll, sl), sa += |d|;
+// then the xor shuffle tree and the eight warps added in a fixed order (no atomics: a repeated launch is bit-identical).
+// out[plane][0..2] = (sum d^2, sum ll^2, sum |d|).
+template <int kVec, typename Load>
+__device__ __forceinline__ void reduce_plane_sums(int n_items, Load load, float* __restrict__ out, size_t plane) {
   __shared__ float red[kMtThreads / 32][3];
-  const int b = blockIdx.x, s = blockIdx.y;
-  const size_t plane = static_cast<size_t>(s) * batch + b;
-  const float4* p = reinterpret_cast<const float4*>(preds_seq + plane * 2 * kHW);
-  const float4* l = reinterpret_cast<const float4*>(label_u + plane * kHW);
-  const float4* m = reinterpret_cast<const float4*>(mask + plane * kHW);
   float se = 0.f, sl = 0.f, sa = 0.f;
-  for (int i = threadIdx.x; i < kHW / 4; i += kMtThreads) {
-    const float4 pv = __ldg(p + i), lv = __ldg(l + i), mv = __ldg(m + i);
-    const float pp[4] = {pv.x * mv.x, pv.y * mv.y, pv.z * mv.z, pv.w * mv.w};
-    const float ll[4] = {lv.x * mv.x, lv.y * mv.y, lv.z * mv.z, lv.w * mv.w};
+  for (int i = threadIdx.x; i < n_items; i += kMtThreads) {
+    float pp[kVec], ll[kVec];
+    load(i, pp, ll);
 #pragma unroll
-    for (int c = 0; c < 4; ++c) {
+    for (int c = 0; c < kVec; ++c) {
       const float d = pp[c] - ll[c];
       se = fmaf(d, d, se);
       sl = fmaf(ll[c], ll[c], sl);
@@ -51,6 +48,23 @@ __global__ void __launch_bounds__(kMtThreads)
     for (int w = 0; w < kMtThreads / 32; ++w) t += red[w][threadIdx.x];  // fixed order: deterministic
     out[plane * 3 + threadIdx.x] = t;
   }
+}
+
+// preds_seq [S][B][2][64][64] (channel 0 = u), label_u [S][B][64][64], mask [S][B][64][64]
+// out [S][B][3] = (sum (p-l)^2, sum l^2, sum |p-l|) over the 4096 pixels, with p, l multiplied by the mask
+__global__ void __launch_bounds__(kMtThreads)
+    multistep_metrics_kernel(const float* __restrict__ preds_seq, const float* __restrict__ label_u,
+                             const float* __restrict__ mask, float* __restrict__ out, int batch) {
+  const int b = blockIdx.x, s = blockIdx.y;
+  const size_t plane = static_cast<size_t>(s) * batch + b;
+  const float4* p = reinterpret_cast<const float4*>(preds_seq + plane * 2 * kHW);
+  const float4* l = reinterpret_cast<const float4*>(label_u + plane * kHW);
+  const float4* m = reinterpret_cast<const float4*>(mask + plane * kHW);
+  reduce_plane_sums<4>(kHW / 4, [&](int i, float (&pp)[4], float (&ll)[4]) {
+    const float4 pv = __ldg(p + i), lv = __ldg(l + i), mv = __ldg(m + i);
+    pp[0] = pv.x * mv.x, pp[1] = pv.y * mv.y, pp[2] = pv.z * mv.z, pp[3] = pv.w * mv.w;
+    ll[0] = lv.x * mv.x, ll[1] = lv.y * mv.y, ll[2] = lv.z * mv.z, ll[3] = lv.w * mv.w;
+  }, out, plane);
 }
 
 cudaError_t launch_multistep_metrics(const float* preds_seq, const float* label_u, const float* mask, float* out,
@@ -131,46 +145,20 @@ cudaError_t launch_gather_batch(const void* frames_in, const void* frames_out, c
 // ------------------------------------------------------------------------------------------------
 namespace fno {
 
-// Same layouts and sums as multistep_metrics_kernel with hw = H*W in place of 4096.  grid (B, S): one CTA per
-// (step, case) plane.  Each thread's pixels, the shuffle tree and the warp order are fixed, so a repeated launch is
-// bit-identical (no atomics).
+// Same layouts and sums as multistep_metrics_kernel with hw = H*W in place of 4096, one pixel per item.  grid (B, S): one
+// CTA per (step, case) plane.
 __global__ void __launch_bounds__(kMtThreads)
     grid_multistep_metrics_kernel(const float* __restrict__ preds_seq, const float* __restrict__ label_u,
                                   const float* __restrict__ mask, float* __restrict__ out, int batch, int hw) {
-  __shared__ float red[kMtThreads / 32][3];
   const int b = blockIdx.x, s = blockIdx.y;
   const size_t plane = static_cast<size_t>(s) * batch + b;
   const float* p = preds_seq + plane * 2 * hw;   // channel 0 = u
   const float* l = label_u + plane * hw;
   const float* m = mask + plane * hw;
-  float se = 0.f, sl = 0.f, sa = 0.f;
-  for (int i = threadIdx.x; i < hw; i += kMtThreads) {
+  reduce_plane_sums<1>(hw, [&](int i, float (&pp)[1], float (&ll)[1]) {
     const float mv = __ldg(m + i);
-    const float pp = __ldg(p + i) * mv, ll = __ldg(l + i) * mv;
-    const float d = pp - ll;
-    se = fmaf(d, d, se);
-    sl = fmaf(ll, ll, sl);
-    sa += fabsf(d);
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    se += __shfl_xor_sync(0xffffffffu, se, o);
-    sl += __shfl_xor_sync(0xffffffffu, sl, o);
-    sa += __shfl_xor_sync(0xffffffffu, sa, o);
-  }
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (lane == 0) {
-    red[warp][0] = se;
-    red[warp][1] = sl;
-    red[warp][2] = sa;
-  }
-  __syncthreads();
-  if (threadIdx.x < 3) {
-    float t = 0.f;
-#pragma unroll
-    for (int w = 0; w < kMtThreads / 32; ++w) t += red[w][threadIdx.x];  // fixed order: deterministic
-    out[plane * 3 + threadIdx.x] = t;
-  }
+    pp[0] = __ldg(p + i) * mv, ll[0] = __ldg(l + i) * mv;
+  }, out, plane);
 }
 
 cudaError_t launch_grid_multistep_metrics(const float* preds_seq, const float* label_u, const float* mask, float* out,
@@ -371,6 +359,77 @@ cudaError_t launch_grid_gather_window(const void* frames_in, const void* frames_
   return launch_gather_window_impl<false>(frames_in, frames_out, case_table, case_ids, idx, n_idx, n_case_params,
                                           frame_bf16, inputs, label, mask, case_params, steps, time_step_size, n_frames,
                                           labels_seq, h * w, stream);
+}
+
+}  // namespace fno
+
+// ------------------------------------------------------------------------------------------------
+// Rollout metrics of the windows of a device-resident split (cfdbench_b200.evaluate_rollout_auto).  Step k (0-based) of
+// the window that starts at sample j = starts[b] is compared with the true frame k steps on, frames_out[j + k s]
+// (s = time_step_size), u channel only, both sides multiplied by the start sample's mask frames_in[j][2] -- the mask the
+// inference rollout applies to its predictions:
+//   out[k][b][0..2] = (sum (p-l)^2, sum l^2, sum |p-l|),  p = preds_seq[k][b][0] * m,  l = frames_out[j + k s][0] * m.
+// The sums are reduce_plane_sums', so they equal fno_[grid_]multistep_metrics' on the gathered (label_u, mask) bit for
+// bit, without the (S, B, H, W) label and mask sequences: only the u plane of each target and the start mask are read.
+// A window with j < 0 or j + (steps - 1) s >= n_frames is not read and its sums are not written.  grid (B, S).
+// kVec: 64x64 frames, 16-byte fp32 / 8-byte bf16 loads; otherwise scalar loads (see the grid section's header).
+// ------------------------------------------------------------------------------------------------
+namespace fno {
+
+template <typename TFrame, bool kVec>
+__global__ void __launch_bounds__(kMtThreads)
+    window_metrics_kernel(const float* __restrict__ preds_seq, const TFrame* __restrict__ frames_in,
+                          const TFrame* __restrict__ frames_out, const long long* __restrict__ starts, int batch,
+                          int steps, int time_step_size, long long n_frames, int hw, float* __restrict__ out) {
+  const int b = blockIdx.x, k = blockIdx.y;
+  const long long j = starts[b];
+  if (j < 0 || j + static_cast<long long>(steps - 1) * time_step_size >= n_frames) return;
+  const size_t plane = static_cast<size_t>(k) * batch + b;
+  const float* p = preds_seq + plane * 2 * hw;   // channel 0 = u
+  const TFrame* l = frames_out + static_cast<size_t>(j + static_cast<long long>(k) * time_step_size) * 3 * hw;
+  const TFrame* m = frames_in + (static_cast<size_t>(j) * 3 + 2) * hw;
+  if constexpr (kVec) {
+    reduce_plane_sums<4>(kHW / 4, [&](int i, float (&pp)[4], float (&ll)[4]) {
+      const float4 pv = __ldg(reinterpret_cast<const float4*>(p) + i);
+      const float4 lv = gather_ld4<TFrame>(l + 4 * i), mv = gather_ld4<TFrame>(m + 4 * i);
+      pp[0] = pv.x * mv.x, pp[1] = pv.y * mv.y, pp[2] = pv.z * mv.z, pp[3] = pv.w * mv.w;
+      ll[0] = lv.x * mv.x, ll[1] = lv.y * mv.y, ll[2] = lv.z * mv.z, ll[3] = lv.w * mv.w;
+    }, out, plane);
+  } else {
+    reduce_plane_sums<1>(hw, [&](int i, float (&pp)[1], float (&ll)[1]) {
+      const float mv = frame_ld(m + i);
+      pp[0] = __ldg(p + i) * mv, ll[0] = frame_ld(l + i) * mv;
+    }, out, plane);
+  }
+}
+
+template <bool kVec>
+static cudaError_t launch_window_metrics_impl(const float* preds_seq, const void* frames_in, const void* frames_out,
+                                              const long long* starts, int steps, int batch, int time_step_size,
+                                              long long n_frames, int frame_bf16, float* out, int hw, cudaStream_t stream) {
+  dim3 grid(batch, steps);
+  if (frame_bf16)
+    window_metrics_kernel<__nv_bfloat16, kVec><<<grid, kMtThreads, 0, stream>>>(
+        preds_seq, static_cast<const __nv_bfloat16*>(frames_in), static_cast<const __nv_bfloat16*>(frames_out), starts,
+        batch, steps, time_step_size, n_frames, hw, out);
+  else
+    window_metrics_kernel<float, kVec><<<grid, kMtThreads, 0, stream>>>(
+        preds_seq, static_cast<const float*>(frames_in), static_cast<const float*>(frames_out), starts, batch, steps,
+        time_step_size, n_frames, hw, out);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_window_metrics(const float* preds_seq, const void* frames_in, const void* frames_out,
+                                  const long long* starts, int steps, int batch, int time_step_size, long long n_frames,
+                                  int frame_bf16, float* out, cudaStream_t stream) {
+  return launch_window_metrics_impl<true>(preds_seq, frames_in, frames_out, starts, steps, batch, time_step_size, n_frames,
+                                          frame_bf16, out, kHW, stream);
+}
+cudaError_t launch_grid_window_metrics(const float* preds_seq, const void* frames_in, const void* frames_out,
+                                       const long long* starts, int steps, int batch, int time_step_size,
+                                       long long n_frames, int frame_bf16, float* out, int h, int w, cudaStream_t stream) {
+  return launch_window_metrics_impl<false>(preds_seq, frames_in, frames_out, starts, steps, batch, time_step_size,
+                                           n_frames, frame_bf16, out, h * w, stream);
 }
 
 }  // namespace fno

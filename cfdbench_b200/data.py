@@ -316,3 +316,29 @@ def rollout_windows(case_ids, steps: int, time_step_size: int) -> np.ndarray:
         return np.zeros(0, dtype=np.int64)
     j = np.arange(cid.size - span, dtype=np.int64)
     return j[cid[j + span] == cid[j]]
+
+
+def _check_chain(frames: DeviceFrames, starts: np.ndarray, steps: int, time_step_size: int,
+                 what: str = "train_data") -> None:
+    """Refuse a split whose frames do not chain where the windows starting at `starts` need them to: step k of the
+    window at j is fed the prediction of step k-1 where the data has frames_in[j + k s], and trained against
+    frames_out[j + (k-1) s], so the two must be the same frame (bit for bit, mask channel included).  Compared on the
+    device in chunks; one synchronisation for the whole check.  The error names the split (`what`) and the
+    first bad sample."""
+    s, dev, n = time_step_size, frames.device, frames.n
+    rows = np.unique((starts[:, None] + s * np.arange(steps - 1, dtype=np.int64)[None, :]).ravel())
+    host = torch.from_numpy(rows).pin_memory()
+    rows_dev = host.to(dev, non_blocking=True)
+    bits = torch.int32 if frames.frame_dtype == torch.float32 else torch.int16
+    first = torch.full((), n, dtype=torch.int64, device=dev)
+    chunk = 512
+    for c0 in range(0, rows.size, chunk):
+        i = rows_dev[c0:c0 + chunk]
+        a = frames.frames_in.index_select(0, i + s).view(bits)
+        b = frames.frames_out.index_select(0, i).view(bits)
+        bad = (a != b).flatten(1).any(1)
+        first = torch.minimum(first, torch.where(bad, i, first).min())
+    bad_row = int(first)   # the check's one synchronisation
+    if bad_row < n:
+        raise ValueError(f"{what} does not chain with time_step_size={s}: sample {bad_row + s}'s input frame is not "
+                         f"sample {bad_row}'s label frame, which a {steps}-step rollout window feeds it")

@@ -15,6 +15,12 @@ dev split every `eval_interval` epochs and of the test split (with B = 1) after 
 batch on the host, runs one forward and synchronises 2 x (number of scores) times per batch; here chunks of up to
 `max_batch` samples are gathered from device-resident frames, run as one forward each and reduced by one `fno_eval_sums`
 launch per chunk, and the split makes one synchronisation.
+
+`evaluate_rollout_auto` scores a split by rollout error, for choosing `train_auto` checkpoints of models trained
+against rollout drift: every S-step window of the split rolls out from its start sample and each step is compared with
+the true frame that many steps on.  Per chunk of windows one gather, one graph-replayed rollout and one
+`fno_[grid_]window_metrics` launch that reads the targets straight from the device-resident frames; one
+synchronisation for the split's chain check and one for the sums.
 """
 from __future__ import annotations
 
@@ -244,3 +250,127 @@ def evaluate_auto(model, data, batch_size: int = 2, max_batch: int = 256) -> dic
             del batch, preds
         host = sums.cpu().double().numpy()   # the only synchronisation
     return dict(preds=preds_host.view(-1, 1, gh, gw), scores=eval_scores(host, gh * gw, batch_size, names))
+
+
+def rollout_scores(sums: np.ndarray, hw: int) -> dict:
+    """The result of `evaluate_rollout_auto` from its window sums: sums (S, n, 3) float64, step k of window i in
+    sums[k][i] (fno_[grid_]window_metrics' (sum (p-l)^2, sum l^2, sum |p-l|)), hw = H*W.  Per window and step the
+    reference's get_metrics (`_per_case`: mse, nmse = mse / mean(l^2), mae); per step each the mean over the windows,
+    added in float64 in window order; loss = the mean over the steps of nmse, added in step order.  A window whose
+    label plane is all zero gives the inf / nan of the reference's division."""
+    host = np.asarray(sums, dtype=np.float64)
+    s, n = host.shape[:2]
+    with np.errstate(divide="ignore", invalid="ignore"):
+        per = _per_case(host, hw)   # (S, n) each
+    steps = []
+    for k in range(s):
+        row = {}
+        for name, v in per.items():
+            tot = 0.0
+            for x in v[k].tolist():   # window order
+                tot += x
+            row[name] = tot / n
+        steps.append(row)
+    loss = 0.0
+    for row in steps:
+        loss += row["nmse"]
+    return dict(steps=steps, loss=loss / s, windows=int(n))
+
+
+def _launch_window_metrics(frames, preds: Tensor, starts: Tensor, time_step_size: int, sums: Tensor) -> None:
+    """sums [S][B][3] (a contiguous float32 CUDA tensor or view) <- fno_[grid_]window_metrics of the contiguous
+    (S, B, 2, H, W) float32 rollout `preds` from the window starts `starts` ((B,) int64 on the device) of `frames`."""
+    s, b, _, gh, gw = preds.shape
+    lib = _lib.load()
+    code = _lib.ACT_BF16 if frames.frame_dtype == torch.bfloat16 else _lib.ACT_F32
+    args = (preds.data_ptr(), frames.frames_in.data_ptr(), frames.frames_out.data_ptr(), starts.data_ptr(), s, b,
+            time_step_size, frames.n, code, sums.data_ptr())
+    st = C.c_void_p(torch.cuda.current_stream(preds.device).cuda_stream)
+    if (gh, gw) == (64, 64):
+        _lib.check(lib.fno_window_metrics(*args, st), "fno_window_metrics")
+    else:
+        _lib.check(lib.fno_grid_window_metrics(*args, gh, gw, st), "fno_grid_window_metrics")
+
+
+def evaluate_rollout_auto(model, data, steps: int, time_step_size=None, max_batch: int = 256) -> dict:
+    """The rollout error of `model` on a split: every window of `steps` = S samples inside one case rolls out S steps
+    from its start sample, and step k (0-based) of the window that starts at sample j is compared with
+    frames_out[j + k s] (s = `time_step_size`, by default the split's), the true frame k + 1 time steps on -- the
+    targets `train_auto(rollout_steps=...)` trains against.  This is deliberately not test_multistep.infer's indexing,
+    which compares prediction s with frame s of the case (`infer_multistep`).  Both sides are the u channel multiplied
+    by the start sample's mask, the mask the rollout applies to its predictions.
+
+    data: the reference's dataset object (uploaded once per call) or a `DeviceFrames` of it.  The windows are
+    `rollout_windows(case_ids, S, s)`; the split must chain (frames_in[j + k s] == frames_out[j + (k-1) s] for every
+    pair a window uses), which is checked on the device with one synchronisation.  model: the drop-in `Fno2d` on a
+    CUDA device, in either storage mode; it is put in eval mode, and the gathers and metrics run under inference mode
+    (the rollout's captured graph outlives the call, so it runs under no_grad, as `generate_many`).
+
+    Windows run in chunks of at most `max_batch`: per chunk one `DeviceFrames.batch` gather of the start samples, one
+    graph-replayed inference rollout (the kernels `generate_many` runs) whose contiguous (S, B, 2, H, W) output is read
+    as it is, and one `fno_[grid_]window_metrics` launch into a device buffer for the whole split, which reads each
+    target's u plane and the start mask from the frames: no label sequence is gathered.  The sums are copied to the
+    host once, where `rollout_scores` reduces them in float64; with the chain check the call synchronises twice.
+    Windows are computed independently, so the result does not depend on `max_batch`.
+
+    Returns dict(steps=[{mse, nmse, mae} per step, each the mean over the windows], loss=the mean over the steps of
+    nmse, windows=the window count).  Raises before any device work: TypeError for a model that is not the drop-in
+    Fno2d; ValueError for a `steps`, `time_step_size` or `max_batch` that is not a positive int, no time step size at
+    all, an empty or malformed split, a case-parameter count other than the model's, a grid or storage mode the model
+    rejects, or a split without a single S-step window; FnoNativeError for a CPU model.  A split that does not chain
+    raises ValueError naming the first bad sample."""
+    from .data import DeviceFrames, _check_chain, rollout_windows
+    from .fno2d import Fno2d
+    from .train import _check_split, _positive_int
+    for name, v in (("steps", steps), ("time_step_size", time_step_size), ("max_batch", max_batch)):
+        if v is not None or name != "time_step_size":
+            _positive_int(name, v)
+    steps, max_batch = int(steps), int(max_batch)
+    if not isinstance(model, Fno2d):
+        raise TypeError(f"evaluate_rollout_auto runs the drop-in cfdbench_b200.Fno2d, got {type(model).__name__}")
+    _check_split(model, data, "the split")
+    tss = getattr(data, "time_step_size", None) if time_step_size is None else time_step_size
+    if tss is None:
+        raise ValueError("evaluate_rollout_auto needs a time_step_size: the split has none, pass it")
+    _positive_int("time_step_size", tss)
+    tss = int(tss)
+    case_ids = data._case_ids_host if isinstance(data, DeviceFrames) else data.case_ids
+    windows = rollout_windows(case_ids, steps, tss)
+    if windows.size == 0:
+        raise ValueError(f"the split has no {steps}-step window with time_step_size={tss} inside one case")
+    model._require_cuda()
+    with torch.inference_mode(), torch.cuda.device(model.device):
+        frames = data if isinstance(data, DeviceFrames) else DeviceFrames(data, device=model.device)
+        _check_chain(frames, windows, steps, tss, what="the split")
+    return _evaluate_rollout(model, frames, windows, steps, tss, max_batch)
+
+
+def _evaluate_rollout(model, frames, windows: np.ndarray, steps: int, time_step_size: int, max_batch: int = 256) -> dict:
+    """evaluate_rollout_auto on checked arguments: `frames` a DeviceFrames on the model's device, `windows` its
+    S-step window starts, the chain already checked."""
+    model.eval()
+    with torch.inference_mode(), torch.cuda.device(model.device):
+        sums = _window_sums(model, frames, windows, steps, time_step_size, max_batch)
+    return rollout_scores(sums, frames.height * frames.width)
+
+
+def _window_sums(model, frames, windows: np.ndarray, steps: int, time_step_size: int, max_batch: int) -> np.ndarray:
+    """The (S, n, 3) float64 fno_[grid_]window_metrics sums of the windows starting at `windows` (checked: inside one
+    case each, the split chaining), in window order: per chunk of at most max_batch windows one gather, one rollout and
+    one metrics launch; one synchronisation.  Runs in the caller's inference mode and device context."""
+    dev, n = model.device, int(windows.size)
+    sums = torch.empty(steps * n * 3, dtype=torch.float32, device=dev)   # chunk [lo, hi)'s (S, B, 3) at S*lo*3
+    for lo in range(0, n, max_batch):
+        hi = min(n, lo + max_batch)
+        starts = torch.from_numpy(windows[lo:hi]).pin_memory()   # pinned: the index uploads are asynchronous
+        b0 = frames.batch(starts)
+        with torch.inference_mode(False), torch.no_grad():   # the captured rollout's static buffers outlive the call
+            x, cp, mk = model._prep_inputs(b0["inputs"], b0["case_params"], b0["mask"])
+            preds = model._rollout_device(x, cp, mk, steps)     # (S, B, 2, H, W), contiguous
+        _launch_window_metrics(frames, preds, starts.to(dev, non_blocking=True), time_step_size,
+                               sums[steps * lo * 3:steps * hi * 3])
+        del b0, preds
+    host = sums.cpu().double().numpy()   # the one synchronisation
+    blocks = [host[steps * lo * 3:steps * min(n, lo + max_batch) * 3].reshape(steps, -1, 3)
+              for lo in range(0, n, max_batch)]
+    return np.concatenate(blocks, axis=1)

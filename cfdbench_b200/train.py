@@ -32,7 +32,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .data import DeviceFrames, _gather, case_table, check_noise_args, index_batches, rollout_windows
+from .data import DeviceFrames, _check_chain, _gather, case_table, check_noise_args, index_batches, rollout_windows
 from .fno2d import capture_graph, side_stream
 
 LOG_COLUMNS = ("mse", "rmse", "mae", "nmse", "mean_l2")   # one row of the epoch log: fno_loss_fwd's five scalars
@@ -348,30 +348,6 @@ class _RolloutStepGraphs(_StepGraphs):
             self._adam_and_log(io["loss"][g].data_ptr(), st)
 
 
-def _check_chain(frames: DeviceFrames, starts: np.ndarray, steps: int, time_step_size: int) -> None:
-    """Refuse a split whose frames do not chain where the windows starting at `starts` need them to: step k of the
-    window at j is fed the prediction of step k-1 where the data has frames_in[j + k s], and trained against
-    frames_out[j + (k-1) s], so the two must be the same frame (bit for bit, mask channel included).  Compared on the
-    device in chunks; one synchronisation for the whole check.  The error names the first bad sample."""
-    s, dev, n = time_step_size, frames.device, frames.n
-    rows = np.unique((starts[:, None] + s * np.arange(steps - 1, dtype=np.int64)[None, :]).ravel())
-    host = torch.from_numpy(rows).pin_memory()
-    rows_dev = host.to(dev, non_blocking=True)
-    bits = torch.int32 if frames.frame_dtype == torch.float32 else torch.int16
-    first = torch.full((), n, dtype=torch.int64, device=dev)
-    chunk = 512
-    for c0 in range(0, rows.size, chunk):
-        i = rows_dev[c0:c0 + chunk]
-        a = frames.frames_in.index_select(0, i + s).view(bits)
-        b = frames.frames_out.index_select(0, i).view(bits)
-        bad = (a != b).flatten(1).any(1)
-        first = torch.minimum(first, torch.where(bad, i, first).min())
-    bad_row = int(first)   # the check's one synchronisation
-    if bad_row < n:
-        raise ValueError(f"train_data does not chain with time_step_size={s}: sample {bad_row + s}'s input frame is not "
-                         f"sample {bad_row}'s label frame, which a {steps}-step rollout window feeds it")
-
-
 # ------------------------------------------------------------------------------------------------ train_auto
 def _positive_int(name: str, v) -> None:
     if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or v < 1:
@@ -410,7 +386,8 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
                lr_gamma: float = 0.9, batch_size: int = 2, eval_batch_size: int = 2, log_interval: int = 10,
                eval_interval: int = 2, generator: Optional[torch.Generator] = None, rollout_steps: int = 1,
                time_step_size: Optional[int] = None, input_noise_std: float = 0.0, noise_seed: int = 0,
-               rollout_grad_steps: Optional[int] = None, noise_every_step: bool = False) -> dict:
+               rollout_grad_steps: Optional[int] = None, noise_every_step: bool = False,
+               dev_rollout_steps: Optional[int] = None) -> dict:
     """What the reference's `train(model, train_data, dev_data, output_dir, ...)` does (src/train_auto.py:181-313), with
     its argument names and defaults, every training step replayed from a CUDA graph and one synchronisation per epoch.
 
@@ -438,8 +415,8 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
       visits a permutation of them that draws from the RNG what a DataLoader over that many samples draws.  The log and
       train_losses hold the aggregate (each column the mean over the K steps).  The split must chain
       (frames_in[j + k s] == frames_out[j + (k-1) s] for every pair a window uses): that is checked once on the device
-      before training.  The dev evaluation, and with it checkpoint selection, stays single-step.  rollout_steps = 1 is
-      the single-step loop above, launch for launch.
+      before training.  The dev evaluation stays single-step unless dev_rollout_steps is given (below).
+      rollout_steps = 1 is the single-step loop above, launch for launch.
     - rollout_grad_steps = G (1 <= G <= K, default K) is pushforward training: of each window's K steps the first
       K - G run without gradient through the inference rollout (the kernels `generate_many` runs), and only the last
       G are trained, from the prefix's last frame, on (nmse_{K-G} + ... + nmse_{K-1}) / G; the log and train_losses
@@ -477,6 +454,16 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
           seq = model.rollout(x, b["case_params"], b["mask"], G, noise=RolloutNoise(sigma, noise_seed, t, ids, K - G))
           loss = sum(model.loss_fn(preds=seq[g], labels=b["labels"][K - G + g])["nmse"] for g in range(G)) / G
 
+    - dev_rollout_steps = S selects checkpoints by rollout error: every evaluation also runs
+      `evaluate_rollout_auto(model, <DeviceFrames of dev_data>, S, time_step_size)` -- every S-step window of the dev
+      split rolled out from its start sample, step k against the frame k + 1 time steps on -- writes its result to
+      `ckpt-{ep}/dev_rollout_scores.json`, and writes scores.json with dev_loss = its `loss` (the mean over the S steps
+      of the nmse) and dev_loss_single_step = the single-step dev_loss, so that the reference's get_best_ckpt /
+      load_best_ckpt, which pick the lowest dev_loss, pick the checkpoint with the lowest rollout error.
+      dev_scores.json stays the single-step evaluation.  The dev split's time step size is the time_step_size
+      argument, else dev_data.time_step_size; it must have an S-step window and chain (checked once on the device
+      before training).  The evaluation draws nothing from the RNG, so training is bit-identical with and without it;
+      None (the default) runs exactly what runs without the option.
     Returns dict(train_losses=[per-step nmse, every epoch], optimizer=the FusedAdam).  Its state holds the true step
     count (its state_dict loads into torch.optim.Adam), and the parameters' version counters are bumped, so the
     model's packed weights and inference graphs are rebuilt on the next call.  Raises before any device work on: a
@@ -486,11 +473,13 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
     and, as ValueError before any training step, a non-positive rollout_steps or time_step_size, rollout_steps > 1 with
     no time_step_size, a split without a single K-step window, or a split whose frames do not chain.  Also raises
     ValueError before any device work for an input_noise_std that is negative, NaN, infinite or not a real number, a
-    noise_seed that is not an int in [0, 2^64), a rollout_grad_steps that is not an int in 1..rollout_steps, or a
-    noise_every_step that is not a bool.
+    noise_seed that is not an int in [0, 2^64), a rollout_grad_steps that is not an int in 1..rollout_steps, a
+    noise_every_step that is not a bool, or a dev_rollout_steps that is not None or a positive int; with
+    dev_rollout_steps, as ValueError before any training step, a dev split without a time step size, without a single
+    S-step window, or whose frames do not chain.
     Frozen parameters (requires_grad=False) are not updated, as FusedAdam.step skips them.  Data parallel training in
     this loop is not supported."""
-    from .metrics import evaluate_auto
+    from .metrics import _evaluate_rollout, evaluate_auto
     from .fno2d import Fno2d
     from .optim import FusedAdam
     if not isinstance(model, Fno2d):
@@ -505,6 +494,9 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
     input_noise_std = check_noise_args(input_noise_std, noise_seed, std_name="input_noise_std")
     if not isinstance(noise_every_step, bool):
         raise ValueError(f"noise_every_step must be a bool, got {noise_every_step!r}")
+    if dev_rollout_steps is not None:
+        _positive_int("dev_rollout_steps", dev_rollout_steps)
+        dev_rollout_steps = int(dev_rollout_steps)
     grad_steps = rollout_steps if rollout_grad_steps is None else rollout_grad_steps
     if isinstance(grad_steps, bool) or not isinstance(grad_steps, (int, np.integer)) or not 1 <= grad_steps <= rollout_steps:
         raise ValueError(f"rollout_grad_steps must be an int in 1..rollout_steps={rollout_steps}, got {rollout_grad_steps!r}")
@@ -528,6 +520,18 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
             raise ValueError(f"train_data has no {rollout_steps}-step window with time_step_size={tss} inside one case")
     elif time_step_size is not None:
         _positive_int("time_step_size", time_step_size)
+    dev_windows = None   # dev_rollout_steps = S: the window starts of the dev split
+    if dev_rollout_steps is not None:
+        dev_tss = getattr(dev_data, "time_step_size", None) if time_step_size is None else time_step_size
+        if dev_tss is None:
+            raise ValueError(f"dev_rollout_steps={dev_rollout_steps} needs a time_step_size: dev_data has none, pass it")
+        _positive_int("time_step_size", dev_tss)
+        dev_tss = int(dev_tss)
+        dev_ids = dev_data._case_ids_host if isinstance(dev_data, DeviceFrames) else dev_data.case_ids
+        dev_windows = rollout_windows(dev_ids, dev_rollout_steps, dev_tss)
+        if dev_windows.size == 0:
+            raise ValueError(f"dev_data has no {dev_rollout_steps}-step window with time_step_size={dev_tss} inside one "
+                             "case")
     model._require_cuda()
     output_dir = Path(output_dir)
     output_dir.mkdir(exist_ok=True, parents=True)
@@ -537,6 +541,9 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
     with torch.cuda.device(dev):
         frames = train_data if isinstance(train_data, DeviceFrames) else DeviceFrames(train_data, device=dev)
         dev_frames = None
+        if dev_windows is not None:
+            dev_frames = dev_data if isinstance(dev_data, DeviceFrames) else DeviceFrames(dev_data, device=dev)
+            _check_chain(dev_frames, dev_windows, dev_rollout_steps, dev_tss, what="dev_data")
         n = frames.n
         noise = dict(noise_std=input_noise_std, noise_seed=int(noise_seed))
         if windows is None:
@@ -555,6 +562,9 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
         if input_noise_std > 0:
             every = ", on every rollout step" if noise_every_step and windows is not None else ""
             print(f"# input noise std: {input_noise_std}, seed {int(noise_seed)}{every}")
+        if dev_windows is not None:
+            print(f"# dev rollout steps: {dev_rollout_steps}, windows: {dev_windows.size} (checkpoints scored by rollout "
+                  "nmse)")
         print(f"# step: {graphs.steps}")
         print(f"# epoch: {num_epochs}")
         start_time = time.time()
@@ -595,8 +605,15 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
                         print(f"Backing up old checkpoint to {ckpt_backup_path}")
                         copyfile(ckpt_path, ckpt_backup_path)
                     torch.save(model.state_dict(), ckpt_path)
-                    ep_scores = dict(ep=ep, train_loss=np.mean(ep_train_losses), dev_loss=np.mean(dev_scores["all"]["nmse"]),
-                                     time=time.time() - ep_start_time)
+                    dev_loss = np.mean(dev_scores["all"]["nmse"])
+                    if dev_windows is None:
+                        ep_scores = dict(ep=ep, train_loss=np.mean(ep_train_losses), dev_loss=dev_loss,
+                                         time=time.time() - ep_start_time)
+                    else:
+                        rollout = _evaluate_rollout(model, dev_frames, dev_windows, dev_rollout_steps, dev_tss)
+                        dump_json(rollout, ckpt_dir / "dev_rollout_scores.json")
+                        ep_scores = dict(ep=ep, train_loss=np.mean(ep_train_losses), dev_loss=rollout["loss"],
+                                         dev_loss_single_step=dev_loss, time=time.time() - ep_start_time)
                     dump_json(ep_scores, ckpt_dir / "scores.json")
         finally:
             del graphs   # the graphs and their static buffers go with the call

@@ -469,6 +469,25 @@ int fno_grid_gather_window(const void* frames_in, const void* frames_out, const 
                            float* mask, float* case_params, int steps, int time_step_size, int64_t n_frames,
                            float* labels_seq, int h, int w_, void* stream);
 
+/* Rollout metrics of the S-step windows of a device-resident split (cfdbench_b200.evaluate_rollout_auto), without
+ * gathering the targets: frames_in / frames_out [N][3][64][64] (u, v, mask; n_frames = N) float32 (frame_dtype =
+ * FNO_ACT_F32) or bfloat16 (FNO_ACT_BF16), starts [B] int64 window starts, preds_seq [S][B][2][64][64] float32 (the
+ * inference rollout from the start samples).  With j = starts[b], m = frames_in[j][2] and s = time_step_size:
+ *   sums[k][b] = (sum (p-l)^2, sum l^2, sum |p-l|),  p = preds_seq[k][b][0] * m,  l = frames_out[j + k s][0] * m,
+ * equal bit for bit to fno_multistep_metrics on label_u[k][b] = frames_out[j + k s][0], mask[k][b] = m.  A window with
+ * j < 0 or j + (S - 1) s >= n_frames is not read and its sums are not written.  One CTA per (step, window), fixed-order
+ * reduction: bit-reproducible.  preds_seq must be 16-byte aligned, the frames 16-byte (fp32) or 8-byte (bf16) aligned.
+ * A null pointer, steps outside 1..65535, batch, time_step_size or n_frames < 1 or a bad frame_dtype returns 1 before any
+ * device work. */
+int fno_window_metrics(const float* preds_seq, const void* frames_in, const void* frames_out, const int64_t* starts,
+                       int steps, int batch, int time_step_size, int64_t n_frames, int frame_dtype, float* sums,
+                       void* stream);
+/* fno_window_metrics on an H x W grid (frames [N][3][H][W], preds_seq [S][B][2][H][W]; no alignment beyond the element
+ * needed).  A grid outside 24..128 returns 3. */
+int fno_grid_window_metrics(const float* preds_seq, const void* frames_in, const void* frames_out, const int64_t* starts,
+                            int steps, int batch, int time_step_size, int64_t n_frames, int frame_dtype, float* sums, int h,
+                            int w_, void* stream);
+
 /* Single-step evaluation (reference src/train_auto.py:61-148, `evaluate`, which synchronises 2 x (number of scores)
  * times per batch): the per-sample sums its scores are made of, for any grid 24 <= H, W <= 128 (64 x 64 included).
  * preds, label, inputs [B][2][H][W], mask [B][1][H][W], float32 caller tensors (no alignment beyond 4 bytes needed);
