@@ -182,7 +182,7 @@ typedef struct fno_grads {
 typedef struct fno_bwd_scratch {
   float* d[2];   /* two float32 [B][32][64][64] gradient buffers (ping-pong) */
   float* dz1;    /* float32 [min(B,FNO_BWD_CHUNK)][128][64][64] */
-  void* gm;      /* complex64 [B][288][32]: scaled modes of the block's upstream gradient */
+  void* gm;      /* complex64 [288][B][32] (mode-major): scaled modes of the block's upstream gradient */
   void* gwk;     /* complex64 [288][32][32] */
   float* partials; /* fno_bwd_partials_bytes() bytes: per-CTA shares of the small gradients (fc0/fc1/fc2/w0), summed in a
                     * fixed order by a second launch instead of float atomics -> bit-reproducible gradients */

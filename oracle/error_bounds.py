@@ -1,4 +1,4 @@
-"""TEST INFRASTRUCTURE -- per-element error bounds of every forward kernel stage against float64.
+"""TEST INFRASTRUCTURE -- per-element error bounds of every kernel stage against float64.
 
 A relative L2 over a whole output cannot see a defect confined to one tile, one image row or one element (a ragged last
 tile, the first refill after a ring wraps, an edge row): one element computed single-pass TF32 moves the relative L2 of a
@@ -111,6 +111,11 @@ KAPPA_GRID_BLOCK_OUT = kappa(57, TWIDDLE) + KAPPA_INV_KX   # measured 0.068 (MUL
 KAPPA_FC1 = {"f32": kappa(97, SPLIT_3XTF32), "bf16": kappa(65, SPLIT_2XTF32), "grid": kappa(33)}
 # fc2: 128 FFMA per output (four lane partial sums added in a fixed order) + bias
 KAPPA_FC2 = kappa(129)   # projection measured 0.014 (64 x 64), 0.028 (grids); grid_project_bwd's dpre 0.068
+# da = W1^T dz1 of the project backward (K = 128 hidden units).  project_bwd_tc_kernel's GEMM2 is 3xTF32 in both storage
+# modes (dz1 is fp32 either way): 3 x 128 additions; its split error covers dz1's re-split into tf32 hi / lo in the
+# epilogue (one of the three 2^-22 terms) and W1's.  Its GEMM1 is fc1 (KAPPA_FC1["f32"] / ["bf16"]).  grid: 128 FFMA.
+KAPPA_DA = {"tc": kappa(384, SPLIT_3XTF32), "grid": kappa(128)}   # dpre measured 0.060 (64 x 64), 0.056 (grids);
+# dz1 (kappa(3) and the GELU' terms of project_bwd) 0.084 (64 x 64), 0.095 (grids)
 
 
 # ------------------------------------------------------------------------------------------ references and scales
@@ -225,10 +230,25 @@ def project(a, w1, b1, w2, b2, mask, kappa_fc1: float, gelu_degree: int):
     return ref * m, bound * m
 
 
-def project_bwd(a, dpreds, mask, pre, w1, b1, w2, kappa_fc1: float = KAPPA_FC1["grid"]):
+def project_hidden(a, w1, b1, kappa_fc1: float):
+    """GELU(z1), z1 = fc1(a), as the project backward recomputes it (degree-8 fit): (ref, bound), the bound carrying fc1's
+    error through GELU (1.13 e_z1) plus the fit's 2.7e-7 and the fp32 rounding of the result.  The Q operand of the
+    fc2.weight gradient."""
+    w1m = w1.reshape(w1.shape[:2])
+    g = onp.gelu(onp.conv1x1(a, w1m, b1))
+    e_z1 = kappa_fc1 * onp.conv1x1(np.abs(a), np.abs(w1m), np.abs(b1))
+    return g, SUP_DGELU * e_z1 + GELU_FIT[8] + 2.0 ** -24 * np.abs(g)
+
+
+def project_bwd(a, dpreds, mask, pre, w1, b1, w2, kappa_fc1: float = KAPPA_FC1["grid"],
+                kappa_da: float = KAPPA_DA["grid"], with_dz1: bool = False):
     """dpre = (W1^T ((W2^T (dpreds mask)) GELU'(z1))) GELU'(pre), the last block's adjoint through the projection:
     (ref, bound), the same rules on the adjoint: each product carries the bound of its factors (|x| e_y + |y| e_x), each
-    contraction |W|^T (e) + kappa(n) |W|^T |.|, GELU' of a computed z1 moves by at most 0.8 e_z1 + its fit's error."""
+    contraction |W|^T (e) + kappa(n) |W|^T |.|, GELU' of a computed z1 moves by at most 0.8 e_z1 + its fit's error.
+    kappa_fc1 / kappa_da are the kappas of the two contractions, z1 = W1 a + b1 and da = W1^T dz1 (KAPPA_FC1,
+    KAPPA_DA: the grid kernel's FFMA chains by default, the tensor-core kernel's 3xTF32 / 2-pass GEMMs for 64 x 64).
+    pre = None: no GELU'(pre) factor.  with_dz1: also (dz1_ref, dz1_bound), dz1 = (W2^T dpreds mask) GELU'(z1), the
+    kernel's second output (the operand of the fc1 gradients)."""
     w1m, w2m = w1.reshape(w1.shape[:2]), w2.reshape(w2.shape[:2])
     m = mask[:, None] if mask.ndim == 3 else mask
     graw = dpreds * m
@@ -240,10 +260,160 @@ def project_bwd(a, dpreds, mask, pre, w1, b1, w2, kappa_fc1: float = KAPPA_FC1["
     gz1 = g2 * d1
     e_gz1 = kappa(3) * s_g2 * np.abs(d1) + s_g2 * (SUP_D2GELU * e_z1 + DGELU_FIT)
     ga = np.einsum("ji,bjhw->bihw", w1m, gz1, optimize=True)
-    e_ga = np.einsum("ji,bjhw->bihw", np.abs(w1m), e_gz1 + kappa(128) * np.abs(gz1), optimize=True)
-    d = onp.dgelu(pre)
-    ref = ga * d
-    return ref, e_ga * np.abs(d) + DGELU_FIT * np.abs(ga) + 2.0 ** -24 * np.abs(ref)
+    e_ga = np.einsum("ji,bjhw->bihw", np.abs(w1m), e_gz1 + kappa_da * np.abs(gz1), optimize=True)
+    if pre is None:
+        ref, bound = ga, e_ga
+    else:
+        d = onp.dgelu(pre)
+        ref = ga * d
+        bound = e_ga * np.abs(d) + DGELU_FIT * np.abs(ga) + 2.0 ** -24 * np.abs(ref)
+    return (ref, bound, gz1, e_gz1) if with_dz1 else (ref, bound)
+
+
+# ------------------------------------------------------------------------------------------ backward reductions
+# A weight gradient is a sum over samples and pixels, G[j][i] = sum_{b,pix} P[b][j][pix] Q[b][i][pix] (bias gradients:
+# Q = 1), spread over CTAs, thread groups and a second reduce_partials launch.  Its rounding term is kappa(n) sum|P||Q|
+# with n the LONGEST chain of additions any one term passes through, not the B H W term count: with the term count the
+# bound is sqrt(#CTAs #groups) looser and a defect confined to one thread tile or one CTA's share stays under it.  Each
+# chain below is read off the kernel's launch code, as a function of the batch (nb: the samples of one launch), the
+# grid and, where the grid is capped by it, the SM count.  Where an operand carries its own bound (dz1, GELU(z1)), the
+# propagation |Q|^T e_P + |P|^T e_Q is added (Outer).  The reductions' real errors cancel far more than sum|P||Q| allows
+# for, so they use little of these bounds; a missing pixel group, sample or wrong column still exceeds them 80x to 1e5x
+# in tests/test_backward_bounds_host.py.  Largest |err| / bound measured by tests/test_gpu_backward_bounds.py on an
+# H100 80GB HBM3 (SXM, 700 W power limit), 22 configurations (64 x 64 both storage modes, B = 1 .. 256; 66 x 65,
+# 25 x 127, 24 x 24 at B = 265):
+#   fc2.weight 4.9e-4, fc2.bias 1.0e-3, fc1.bias 9.2e-4, fc1.weight 1.9e-3, w0.weight 3.6e-3, w0.bias 1.8e-3,
+#   weights1 | weights2 0.14, fc0.weight 3.4e-3, fc0.bias 1.9e-3, d_inputs 0.13, d_case_params 2.1e-3;
+#   the data path on the existing stage bounds: gm (fp32 DFT at (1/HW, 2/HW)) 0.070 (64 x 64), 0.21 (grids), ym (adjoint
+#   mix, KAPPA_MIX) 0.12, z (inv_kx at (1, 1)) 0.060, dL/da0 (block_out PLAIN) 0.078.
+def _cdiv(a: int, b: int) -> int:
+    return -(-a // b)
+
+
+def chain_reduce_partials(n_parts: int, n_launches: int = 1) -> int:
+    """reduce_partials_kernel: thread (tx, ty) adds rows ty, ty + 32, .. (at most ceil(n / 32) into one of its four
+    sums), the four sums pairwise (2), then the 32 row groups in order (31); a further batch chunk adds its sum to the
+    gradient (+1 per launch after the first)."""
+    return _cdiv(n_parts, 32) + 2 + 31 + (n_launches - 1)
+
+
+def chain_chan_outer(nb: int, nj: int, n_launches: int = 1) -> int:
+    """chan_outer_kernel<NJ, 32> (64 x 64) + reduce_partials: items = nb 4096 / PIX chunks on min(items, 296) CTAs; a
+    thread adds PXG pixels of each of its ceil(items / grid) items in one FFMA chain, then the NG pixel groups' tiles are
+    added in order.  NJ = 128 (fc1): NG = 2, PIX = 64, PXG = 32; NJ = 32 (w0): NG = 8, PIX = 128, PXG = 16."""
+    ng, pix = 256 // nj, (64 if nj >= 128 else 128)
+    items = nb * (4096 // pix)
+    grid = min(items, 296)
+    return _cdiv(items, grid) * (pix // ng) + (ng - 1) + chain_reduce_partials(grid, n_launches)
+
+
+def chain_project_bwd_tc(nb: int, n_sm: int, n_launches: int = 1) -> int:
+    """project_bwd_tc_kernel's fc2.weight / fc1.bias / fc2.bias partials + reduce_partials: 64 one-row tiles per sample
+    on 2 min(ceil(32 nb), n_sm, 256) pipelines; per tile a sum over two rows (2, fc2.bias: in the thread's running sum),
+    the halving transpose-reduction over 8 lanes (3), the four warps (3), then the pipeline's running total, one add per
+    tile."""
+    tiles = 64 * nb
+    grid = min(_cdiv(tiles, 2), n_sm, 256)
+    per_pipe = _cdiv(tiles, 2 * grid)
+    return 2 * per_pipe + 8 + chain_reduce_partials(2 * grid, n_launches)
+
+
+def chain_spectral_wgrad(b: int) -> int:
+    """spectral_wgrad_kernel: warp w takes samples w, w + 4, .. (ceil(B / 4)); conj(x) g adds two FFMA chains of that
+    length (2 ceil(B / 4) + 1), then the four warps (3)."""
+    return 2 * _cdiv(b, 4) + 4
+
+
+def chain_lift_bwd(b: int) -> int:
+    """lift_bwd_kernel + lift_bwd_reduce (64 x 64): grid.y = min(B, 16) slices; a thread adds 16 terms per sample (four
+    float4 groups, each a 4-FFMA chain) over ceil(B / grid.y) samples, the warp butterfly (5), the 8 warps (7), then the
+    grid.y partial rows (grid.y).  The case-parameter columns (per-sample plane sums times params) are shorter."""
+    gy = min(b, 16)
+    return 16 * _cdiv(b, gy) + 12 + gy
+
+
+# lift_bwd_data_kernel: d_inputs = 32 FFMA over the channels; d_case_params: a thread's 8-pixel sum (8), 32 FFMA over
+# the channels, the warp butterfly (5) and 16 warps (15)
+CHAIN_LIFT_DATA = {"d_inputs": 32, "d_case_params": 60}
+
+
+def chain_grid_project_bwd(nb: int, hw: int, n_launches: int = 1) -> int:
+    """grid_project_bwd_kernel + reduce_partials: nb ceil(hw / 32) 32-pixel tiles on min(tiles, 1024) CTAs, 32 FFMA per
+    tile (fc2.bias: a 32-term sum per tile)"""
+    tiles = nb * _cdiv(hw, 32)
+    parts = min(tiles, 1024)
+    return 32 * _cdiv(tiles, parts) + chain_reduce_partials(parts, n_launches)
+
+
+def chain_grid_chan_outer(nb: int, hw: int, n_launches: int = 1) -> int:
+    """grid_chan_outer_kernel + reduce_partials: 32-pixel tiles on min(tiles, 528) CTAs, 32 FFMA per tile"""
+    tiles = nb * _cdiv(hw, 32)
+    parts = min(tiles, 528)
+    return 32 * _cdiv(tiles, parts) + chain_reduce_partials(parts, n_launches)
+
+
+def chain_grid_lift_bwd(b: int, hw: int) -> int:
+    """grid_lift_bwd_kernel + reduce_partials: min(B, 264) CTAs take ceil(B / parts) samples each; per sample a lane's
+    ceil(hw / 32) FFMA, the warp butterfly (5) and one add into the CTA's running row"""
+    parts = min(b, 264)
+    return _cdiv(b, parts) * (_cdiv(hw, 32) + 6) + chain_reduce_partials(parts)
+
+
+def chain_grid_lift_data(hw: int) -> dict:
+    """grid_lift_bwd_kernel's data adjoint: d_inputs 32 FFMA; d_case_params a lane's ceil(hw / 32) pixels, the warp
+    butterfly (5) and 32 FFMA over the channels"""
+    return {"d_inputs": 32, "d_case_params": _cdiv(hw, 32) + 37}
+
+
+class Outer:
+    """G[j][i] = sum_{b,pix} P[b][j][pix] Q[b][i][pix] and the row sums r[j] = sum P[b][j][pix], accumulated over
+    sample chunks (`add`), with their scales sum |P||Q| and sum |P| and the propagation of the operands' own bounds,
+    |Q|^T e_P + |P|^T e_Q (row sums: sum e_P).  `weight(chain)` / `rowsum(chain)` give (ref, bound)."""
+
+    def __init__(self):
+        self.g = self.s = self.e = self.r = self.rs = self.re = 0.0
+
+    def add(self, p, q, e_p=None, e_q=None):
+        b, nj, ni = p.shape[0], p.shape[1], q.shape[1]
+        p, q = p.reshape(b, nj, -1), q.reshape(b, ni, -1)
+        ap, aq = np.abs(p), np.abs(q)
+        self.g = self.g + np.einsum("bjn,bin->ji", p, q, optimize=True)
+        self.s = self.s + np.einsum("bjn,bin->ji", ap, aq, optimize=True)
+        self.r = self.r + p.sum(axis=(0, 2))
+        self.rs = self.rs + ap.sum(axis=(0, 2))
+        if e_p is not None:
+            e_p = e_p.reshape(b, nj, -1)
+            self.e = self.e + np.einsum("bjn,bin->ji", e_p, aq, optimize=True)
+            self.re = self.re + e_p.sum(axis=(0, 2))
+        if e_q is not None:
+            self.e = self.e + np.einsum("bjn,bin->ji", ap, e_q.reshape(b, ni, -1), optimize=True)
+        return self
+
+    def weight(self, chain: int):
+        return self.g, kappa(chain) * self.s + self.e
+
+    def rowsum(self, chain: int):
+        return self.r, kappa(chain) * self.rs + self.re
+
+
+def spectral_wgrad(xm, gm, chain: int):
+    """gW[i][o][kx][ky] = sum_b conj(X[b][i][kx][ky]) G[b][o][kx][ky]: (ref complex, bound for Re and Im), scale
+    sum_b (|Re x| + |Im x|)(|Re g| + |Im g|)."""
+    ref = np.einsum("bikl,bokl->iokl", np.conj(xm), gm, optimize=True)
+    return ref, kappa(chain) * np.einsum("bikl,bokl->iokl", _cabs(xm), _cabs(gm), optimize=True)
+
+
+def lift_data(da0, w_lift, chains: dict):
+    """The lift's data adjoint from dL/da0 [B][32][H][W] and fc0.weight [32][5 + p] (columns u, v, mask, x, y, params):
+    d_inputs = W[:, :2]^T da0 (scale |W|^T |da0|) and d_case_params[b][j] = sum_o W[o][5 + j] sum_pix da0[b][o] (scale
+    sum_o |W| sum_pix |da0|): ((ref, bound), (ref, bound))."""
+    w = w_lift.reshape(w_lift.shape[:2])
+    wi, wp = w[:, :2], w[:, 5:]
+    d_in = np.einsum("oc,bohw->bchw", wi, da0, optimize=True)
+    s_in = np.einsum("oc,bohw->bchw", np.abs(wi), np.abs(da0), optimize=True)
+    d_cp = np.einsum("oj,bo->bj", wp, da0.sum(axis=(2, 3)), optimize=True)
+    s_cp = np.einsum("oj,bo->bj", np.abs(wp), np.abs(da0).sum(axis=(2, 3)), optimize=True)
+    return (d_in, kappa(chains["d_inputs"]) * s_in), (d_cp, kappa(chains["d_case_params"]) * s_cp)
 
 
 # ------------------------------------------------------------------------------------------ the checks
@@ -291,6 +461,26 @@ def mode_tiles():
     return {"mode (kx, ky)": lambda kx, ky, b, c: np.stack([kx, ky], 1),
             "128-sample tile": lambda kx, ky, b, c: b // 128,
             "sample": lambda kx, ky, b, c: b}
+
+
+WEIGHT_AXES = ("row", "column")
+
+
+def weight_tiles(thread_of):
+    """groupings of [J][I] weight-gradient failures: (row, column) and the thread tile that owns the element
+    (`thread_of(j, i)` -> thread id arrays, e.g. chan_outer's interleaved 8 x 4 tiles)"""
+    return {"(row, column)": lambda j, i: np.stack([j, i], 1),
+            "thread tile": lambda j, i: np.stack(thread_of(j, i), 1)}
+
+
+def chan_outer_thread(nj: int, ni: int = 32):
+    """chan_outer_kernel's thread (tj, ti) of G[j][i]: rows j = a NJ/8 + tj, columns i = c NI/4 + ti"""
+    return lambda j, i: (j % (nj // 8), i % (ni // 4))
+
+
+def grid_chan_outer_thread(nj: int, ni: int = 32):
+    """grid_chan_outer_kernel's thread (tj, ti): a contiguous RJ x 4 block, RJ = NJ / 32"""
+    return lambda j, i: (j // (nj // 32), i // 4)
 
 
 def check(name: str, got, ref, bound, axes=PIXEL_AXES, tiles=None, bf16: bool = False) -> float:
