@@ -71,6 +71,7 @@ class FnoBwdScratch(C.Structure):
 
 BWD_CHUNK = 32
 ADAM_MAX_TENSORS = 32
+GRAD_NORM_MAX_TABLES = 8
 
 
 class FnoAdamTensors(C.Structure):
@@ -131,6 +132,13 @@ SIGNATURES = {
     "fno_adam_step_dev": (C.c_int, [C.POINTER(FnoAdamTensors), _P, _I, _P, _F, _F, _F, _F, _P]),
     "fno_adam_coefficients": (C.c_int, [_F, _F, _F, C.c_int64, _I, _P]),
     "fno_train_log_step": (C.c_int, [_P, _P, _I, _P, _P]),
+    # gradient-norm clipping and the EMA of the weights
+    "fno_grad_norm_scratch_bytes": (C.c_size_t, []),
+    "fno_grad_norm": (C.c_int, [C.POINTER(FnoAdamTensors), _I, _F, _P, _P, _P, _I, _P, _P]),
+    "fno_adam_step_ex": (C.c_int, [C.POINTER(FnoAdamTensors), _F, _F, _F, _F, _F, C.c_int64, _P, C.POINTER(_P),
+                                   C.c_double, _P]),
+    "fno_adam_step_dev_ex": (C.c_int, [C.POINTER(FnoAdamTensors), _P, _I, _P, _F, _F, _F, _F, _P, C.POINTER(_P), _P, _P]),
+    "fno_ema_decays": (C.c_int, [C.c_double, C.c_int64, _I, _P]),
     "fno_forward_train": (C.c_int, [C.POINTER(FnoWeights), _P, _P, _P, _P, C.POINTER(FnoTrainSaved),
                                     C.POINTER(FnoWorkspace), _I, _I, _P]),
     "fno_backward": (C.c_int, [C.POINTER(FnoWeights), C.POINTER(FnoWeightsBwd), _P, _P, _P, _P,

@@ -25,6 +25,13 @@ cudaError_t launch_adam_step(const fno_adam_tensors*, float, float, float, float
 cudaError_t launch_adam_step_dev(const fno_adam_tensors*, const float*, int, const int*, float, float, float, float,
                                  cudaStream_t);
 void adam_coefficients(float, float, float, long long, float*, float*);
+cudaError_t launch_adam_step_ex(const fno_adam_tensors*, float, float, float, float, float, long long, const float*,
+                                void* const*, double, cudaStream_t);
+cudaError_t launch_adam_step_dev_ex(const fno_adam_tensors*, const float*, int, const int*, float, float, float, float,
+                                    const float*, void* const*, const float*, cudaStream_t);
+float ema_decay_at(double, long long);
+cudaError_t launch_grad_norm(const fno_adam_tensors*, int, float, float*, void*, float*, int, const int*, cudaStream_t);
+size_t grad_norm_scratch_bytes();
 cudaError_t launch_stage_indices(const long long*, long long, int, int, const int*, long long*, cudaStream_t);
 cudaError_t launch_log_step(const float*, float*, int, int*, cudaStream_t);
 cudaError_t launch_inv_kx(const void*, void*, int, float, float, cudaStream_t);
@@ -756,6 +763,61 @@ int fno_adam_step_dev(const fno_adam_tensors* t, const float* coef, int n_coef, 
 int fno_adam_coefficients(float lr, float beta1, float beta2, int64_t first_step, int n, float* host_out) {
   if (!host_out || n <= 0 || first_step < 1) return fail(kErrArg, "fno_adam_coefficients: bad argument");
   for (int i = 0; i < n; ++i) adam_coefficients(lr, beta1, beta2, first_step + i, host_out + 2 * i, host_out + 2 * i + 1);
+  return kOk;
+}
+
+// ---------------------------------------------------------------- gradient-norm clipping and the EMA of the weights
+static bool ema_ok(const fno_adam_tensors* t, void* const* ema) {
+  if (!ema) return true;
+  for (int i = 0; i < t->count; ++i)
+    if (!ema[i]) return false;
+  return true;
+}
+static inline bool decay_ok(double d) { return d >= 0.0 && d < 1.0; }   // false for NaN
+
+size_t fno_grad_norm_scratch_bytes(void) { return grad_norm_scratch_bytes(); }
+
+int fno_grad_norm(const fno_adam_tensors* tables, int n_tables, float max_norm, float* out, void* scratch, float* log,
+                  int n_log, const int32_t* cursor, void* stream) {
+  if (!tables || n_tables < 1 || n_tables > FNO_GRAD_NORM_MAX_TABLES || !(max_norm > 0.f) || !isfinite(max_norm) || !out ||
+      !scratch || (reinterpret_cast<uintptr_t>(scratch) & 7) || (log && (!cursor || n_log <= 0)))
+    return fail(kErrArg, "fno_grad_norm: bad argument");
+  for (int k = 0; k < n_tables; ++k) {   // only the grad and n fields are read
+    const fno_adam_tensors& t = tables[k];
+    if (t.count < 0 || t.count > FNO_ADAM_MAX_TENSORS) return fail(kErrArg, "fno_grad_norm: bad tensor table");
+    for (int i = 0; i < t.count; ++i)
+      if (!t.grad[i] || t.n[i] <= 0) return fail(kErrArg, "fno_grad_norm: bad tensor table");
+  }
+  FNO_CUDA(launch_grad_norm(tables, n_tables, max_norm, out, scratch, log, n_log, reinterpret_cast<const int*>(cursor),
+                            S(stream)),
+           "grad_norm_kernel");
+  return kOk;
+}
+
+int fno_adam_step_ex(const fno_adam_tensors* t, float lr, float beta1, float beta2, float eps, float weight_decay,
+                     int64_t step, const float* clip_coef, void* const* ema, double ema_decay, void* stream) {
+  if (step < 1 || (ema && !decay_ok(ema_decay))) return fail(kErrArg, "fno_adam_step_ex: bad argument");
+  if (!adam_tensors_ok(t) || !ema_ok(t, ema)) return fail(kErrArg, "fno_adam_step_ex: bad tensor table");
+  FNO_CUDA(launch_adam_step_ex(t, lr, beta1, beta2, eps, weight_decay, step, clip_coef, ema, ema_decay, S(stream)),
+           "adam_step_ex_kernel");
+  return kOk;
+}
+
+int fno_adam_step_dev_ex(const fno_adam_tensors* t, const float* coef, int n_coef, const int32_t* cursor, float beta1,
+                         float beta2, float eps, float weight_decay, const float* clip_coef, void* const* ema,
+                         const float* ema_decay_tab, void* stream) {
+  if (!coef || !cursor || n_coef <= 0 || (reinterpret_cast<uintptr_t>(coef) & 7) || (ema && !ema_decay_tab))
+    return fail(kErrArg, "fno_adam_step_dev_ex: bad argument");
+  if (!adam_tensors_ok(t) || !ema_ok(t, ema)) return fail(kErrArg, "fno_adam_step_dev_ex: bad tensor table");
+  FNO_CUDA(launch_adam_step_dev_ex(t, coef, n_coef, reinterpret_cast<const int*>(cursor), beta1, beta2, eps, weight_decay,
+                                   clip_coef, ema, ema ? ema_decay_tab : nullptr, S(stream)),
+           "adam_step_ex_kernel<true>");
+  return kOk;
+}
+
+int fno_ema_decays(double ema_decay, int64_t first_step, int n, float* host_out) {
+  if (!host_out || n <= 0 || first_step < 1 || !decay_ok(ema_decay)) return fail(kErrArg, "fno_ema_decays: bad argument");
+  for (int i = 0; i < n; ++i) host_out[i] = ema_decay_at(ema_decay, first_step + i);
   return kOk;
 }
 

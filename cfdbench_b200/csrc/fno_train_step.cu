@@ -258,20 +258,45 @@ void adam_coefficients(float lr, float beta1, float beta2, long long step, float
   *inv_bc2_sqrt = static_cast<float>(1.0 / sqrt(bc2));
 }
 
+// The EMA decay of 1-based step `step`: min(decay, 1 - step^(-3/4)), in double, rounded to float32.  This is diffusers'
+// EMAModel.get_decay(step) with use_ema_warmup=True, inv_gamma=1, power=3/4, update_after_step=0, min_decay=0 (its
+// `step - 1` plus its `1 +`), so step 1 gives 0 and the EMA starts as a copy of the weights.  The one copy of this
+// arithmetic: launch_adam_step_ex and the device table (fno_ema_decays) both call it.
+float ema_decay_at(double decay, long long step) {
+  const double warm = 1.0 - pow(static_cast<double>(step), -0.75);
+  return static_cast<float>(warm < decay ? warm : decay);
+}
+
+// What the _ex Adam adds (all unused by adam_step_kernel): the clip coefficient (device, written by fno_grad_norm), the
+// EMA tensors of the table's entries and the step's EMA decay (by value, or decay_tab[*cursor] with kDevCoef).
+struct AdamExt {
+  const float* clip;
+  float* ema[FNO_ADAM_MAX_TENSORS];
+  const float* decay_tab;
+  float decay;
+};
+
 // torch.optim.Adam, single-tensor formulation (torch/optim/adam.py _single_tensor_adam):
 //   g += wd p;  m = lerp(m, g, 1-b1);  v = b2 v + (1-b2) g g;  p -= step_size * m / (sqrt(v)/sqrt(bc2) + eps)
 //   kDevCoef = false: step_size / inv_bc2_sqrt by value (fno_adam_step);  true: from coef[*cursor] (fno_adam_step_dev),
 //   and a cursor outside 0..n_coef-1 makes the launch write nothing
-template <bool kDevCoef>
-__global__ void __launch_bounds__(kAdamThreads) adam_step_kernel(const __grid_constant__ AdamArgs a) {
+//   kClip: g = g * clip coefficient before the weight decay (clip_grad_norm_ before optimizer.step());
+//   kEma: ema = fmaf(-d, p_new - ema, p_new) with the step's decay d, p_new still in registers
+template <bool kDevCoef, bool kClip, bool kEma>
+__device__ __forceinline__ void adam_update(const AdamArgs& a, const AdamExt& x) {
   float step_size = a.step_size, inv_bc2_sqrt = a.inv_bc2_sqrt;
+  float decay = 0.f;
+  if constexpr (kEma) decay = x.decay;
   if constexpr (kDevCoef) {
     const int c = *a.cursor;
     if (c < 0 || c >= a.n_coef) return;
     const float2 k = a.coef[c];
     step_size = k.x;
     inv_bc2_sqrt = k.y;
+    if constexpr (kEma) decay = x.decay_tab[c];
   }
+  float coef = 1.f;
+  if constexpr (kClip) coef = *x.clip;
   int ti = 0;
 #pragma unroll 1
   while (ti + 1 < a.t.count && static_cast<int>(blockIdx.x) >= a.first_block[ti + 1]) ++ti;
@@ -280,12 +305,15 @@ __global__ void __launch_bounds__(kAdamThreads) adam_step_kernel(const __grid_co
   const float* __restrict__ g = static_cast<const float*>(a.t.grad[ti]);
   float* __restrict__ m = static_cast<float*>(a.t.exp_avg[ti]);
   float* __restrict__ v = static_cast<float*>(a.t.exp_avg_sq[ti]);
+  float* __restrict__ e = nullptr;
+  if constexpr (kEma) e = x.ema[ti];
   const long long base = static_cast<long long>(blockIdx.x - a.first_block[ti]) * kAdamChunk;
 #pragma unroll
   for (int r = 0; r < 4; ++r) {
     const long long i = base + r * kAdamThreads + threadIdx.x;
     if (i < n) {
       float gi = g[i];
+      if constexpr (kClip) gi = gi * coef;
       const float pi = p[i];
       if (a.weight_decay != 0.f) gi = fmaf(a.weight_decay, pi, gi);
       float mi = m[i], vi = v[i];
@@ -294,9 +322,22 @@ __global__ void __launch_bounds__(kAdamThreads) adam_step_kernel(const __grid_co
       const float denom = sqrtf(vi) * inv_bc2_sqrt + a.eps;
       m[i] = mi;
       v[i] = vi;
-      p[i] = pi - step_size * (mi / denom);
+      const float pn = pi - step_size * (mi / denom);
+      p[i] = pn;
+      if constexpr (kEma) e[i] = fmaf(-decay, pn - e[i], pn);
     }
   }
+}
+
+template <bool kDevCoef>
+__global__ void __launch_bounds__(kAdamThreads) adam_step_kernel(const __grid_constant__ AdamArgs a) {
+  adam_update<kDevCoef, false, false>(a, AdamExt{});
+}
+
+template <bool kDevCoef, bool kClip, bool kEma>
+__global__ void __launch_bounds__(kAdamThreads)
+    adam_step_ex_kernel(const __grid_constant__ AdamArgs a, const __grid_constant__ AdamExt x) {
+  adam_update<kDevCoef, kClip, kEma>(a, x);
 }
 
 static int adam_blocks(const fno_adam_tensors* t, AdamArgs& a) {
@@ -340,6 +381,156 @@ cudaError_t launch_adam_step_dev(const fno_adam_tensors* t, const float* coef, i
   adam_step_kernel<true><<<blocks, kAdamThreads, 0, stream>>>(a);
   return cudaGetLastError();
 }
+
+template <bool kDevCoef>
+static cudaError_t launch_adam_ex(const AdamArgs& a, const AdamExt& x, int blocks, cudaStream_t stream) {
+  if (blocks == 0) return cudaSuccess;
+  const bool clip = x.clip != nullptr, ema = x.ema[0] != nullptr;
+  if (clip && ema)
+    adam_step_ex_kernel<kDevCoef, true, true><<<blocks, kAdamThreads, 0, stream>>>(a, x);
+  else if (clip)
+    adam_step_ex_kernel<kDevCoef, true, false><<<blocks, kAdamThreads, 0, stream>>>(a, x);
+  else if (ema)
+    adam_step_ex_kernel<kDevCoef, false, true><<<blocks, kAdamThreads, 0, stream>>>(a, x);
+  else
+    adam_step_kernel<kDevCoef><<<blocks, kAdamThreads, 0, stream>>>(a);
+  return cudaGetLastError();
+}
+
+static AdamExt adam_ext(const fno_adam_tensors* t, const float* clip_coef, void* const* ema) {
+  AdamExt x = {};
+  x.clip = clip_coef;
+  if (ema)
+    for (int i = 0; i < t->count; ++i) x.ema[i] = static_cast<float*>(ema[i]);
+  return x;
+}
+
+cudaError_t launch_adam_step_ex(const fno_adam_tensors* t, float lr, float beta1, float beta2, float eps, float weight_decay,
+                                long long step, const float* clip_coef, void* const* ema, double ema_decay,
+                                cudaStream_t stream) {
+  AdamArgs a = {};
+  const int blocks = adam_blocks(t, a);
+  a.lr = lr;
+  a.beta1 = beta1;
+  a.beta2 = beta2;
+  a.eps = eps;
+  a.weight_decay = weight_decay;
+  adam_coefficients(lr, beta1, beta2, step, &a.step_size, &a.inv_bc2_sqrt);
+  AdamExt x = adam_ext(t, clip_coef, ema);
+  if (ema) x.decay = ema_decay_at(ema_decay, step);
+  return launch_adam_ex<false>(a, x, blocks, stream);
+}
+
+cudaError_t launch_adam_step_dev_ex(const fno_adam_tensors* t, const float* coef, int n_coef, const int* cursor, float beta1,
+                                    float beta2, float eps, float weight_decay, const float* clip_coef, void* const* ema,
+                                    const float* ema_decay_tab, cudaStream_t stream) {
+  AdamArgs a = {};
+  const int blocks = adam_blocks(t, a);
+  a.beta1 = beta1;
+  a.beta2 = beta2;
+  a.eps = eps;
+  a.weight_decay = weight_decay;
+  a.coef = reinterpret_cast<const float2*>(coef);
+  a.cursor = cursor;
+  a.n_coef = n_coef;
+  AdamExt x = adam_ext(t, clip_coef, ema);
+  x.decay_tab = ema_decay_tab;
+  return launch_adam_ex<true>(a, x, blocks, stream);
+}
+
+// ------------------------------------------------------------------------------------------------ global gradient norm
+// ||g||_2 over the gradients of up to FNO_GRAD_NORM_MAX_TABLES Adam tables, torch.nn.utils.clip_grad_norm_'s total norm,
+// in one launch of a fixed kNormBlocks x kNormThreads grid.  Thread t of block b sums g*g in float64 over the elements
+// i = (b * kNormThreads + t) + k * kNormBlocks * kNormThreads of every tensor in table order; the block reduces its
+// threads in a fixed shuffle / warp order into partials[b], and the last block to arrive (an integer ticket) sums the
+// kNormBlocks partials in a fixed order.  No float atomics: the result does not depend on the block schedule.
+constexpr int kNormThreads = 256;
+constexpr int kNormBlocks = 264;   // 2 per SM of an H100 SXM; fixed, so the reduction order is too
+constexpr int kNormMaxTensors = FNO_GRAD_NORM_MAX_TABLES * FNO_ADAM_MAX_TENSORS;
+
+struct NormArgs {
+  const float* grad[kNormMaxTensors];
+  long long n[kNormMaxTensors];
+  int count;
+  float max_norm;
+  float* out;           // [2]: norm, coef
+  double* partials;     // [kNormBlocks], then a uint32 ticket
+  float* log;           // log[*cursor] = norm (optional)
+  int n_log;
+  const int* cursor;
+};
+
+__global__ void __launch_bounds__(kNormThreads) grad_norm_kernel(const __grid_constant__ NormArgs a) {
+  __shared__ double red[kNormThreads / 32];
+  __shared__ bool last;
+  const long long stride = static_cast<long long>(kNormBlocks) * kNormThreads;
+  const long long first = static_cast<long long>(blockIdx.x) * kNormThreads + threadIdx.x;
+  double s = 0.0;
+#pragma unroll 1
+  for (int j = 0; j < a.count; ++j) {
+    const float* __restrict__ g = a.grad[j];
+    const long long n = a.n[j];
+#pragma unroll 4
+    for (long long i = first; i < n; i += stride) {
+      const double v = static_cast<double>(__ldg(g + i));
+      s = fma(v, v, s);
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (lane == 0) red[warp] = s;
+  __syncthreads();
+  unsigned int* ticket = reinterpret_cast<unsigned int*>(a.partials + kNormBlocks);
+  if (threadIdx.x == 0) {
+    double t = 0.0;
+#pragma unroll
+    for (int w = 0; w < kNormThreads / 32; ++w) t += red[w];
+    a.partials[blockIdx.x] = t;
+    __threadfence();
+    last = atomicAdd(ticket, 1u) == kNormBlocks - 1;
+  }
+  __syncthreads();
+  if (!last || threadIdx.x >= 32) return;
+  __threadfence();
+  double t = 0.0;
+  for (int b = threadIdx.x; b < kNormBlocks; b += 32) t += __ldcg(a.partials + b);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
+  if (threadIdx.x != 0) return;
+  // clip_grad_norm_'s coefficient in float32, max_norm / (norm + 1e-6) clamped to at most 1, as torch evaluates it: a
+  // Python number over a tensor is reciprocal(tensor) * number.  A NaN norm gives NaN and an infinite one 0, as
+  // torch.clamp(max=1) gives them.
+  const float norm = static_cast<float>(sqrt(t));
+  const float q = __fmul_rn(__frcp_rn(__fadd_rn(norm, 1e-6f)), a.max_norm);
+  a.out[0] = norm;
+  a.out[1] = q > 1.f ? 1.f : q;
+  if (a.log) {
+    const int c = *a.cursor;
+    if (c >= 0 && c < a.n_log) a.log[c] = norm;
+  }
+  *ticket = 0u;   // ready for the next call on this scratch buffer
+}
+
+cudaError_t launch_grad_norm(const fno_adam_tensors* tables, int n_tables, float max_norm, float* out, void* scratch,
+                             float* log, int n_log, const int* cursor, cudaStream_t stream) {
+  NormArgs a = {};
+  for (int k = 0; k < n_tables; ++k)
+    for (int i = 0; i < tables[k].count; ++i) {
+      a.grad[a.count] = static_cast<const float*>(tables[k].grad[i]);
+      a.n[a.count] = tables[k].n[i];
+      ++a.count;
+    }
+  a.max_norm = max_norm;
+  a.out = out;
+  a.partials = static_cast<double*>(scratch);
+  a.log = log;
+  a.n_log = n_log;
+  a.cursor = cursor;
+  grad_norm_kernel<<<kNormBlocks, kNormThreads, 0, stream>>>(a);
+  return cudaGetLastError();
+}
+size_t grad_norm_scratch_bytes() { return kNormBlocks * sizeof(double) + 16; }
 
 // ------------------------------------------------------------------------------------------------ graph-replayed steps
 // A CUDA graph of one training step is replayed once per step of an epoch; what changes from step to step lives on the

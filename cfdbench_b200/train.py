@@ -107,6 +107,18 @@ class _StepGraphs:
         self.flat, _, self.grads = model._grad_buffers()
 
         self.io = self._make_io(bmax, gh, gw, p)
+        # FusedAdam(max_grad_norm=...): the step's global norm and clip coefficient, the epoch's norm log;
+        # FusedAdam(ema_decay=...): the epoch's table of EMA decays, read by the cursor as the Adam coefficients are
+        self.max_grad_norm, self.ema_decay = optimizer.max_grad_norm, optimizer.ema_decay
+        if self.max_grad_norm is not None:
+            self.io.update(norm=torch.empty(2, dtype=torch.float32, device=dev),
+                           norm_log=torch.empty(self.steps, dtype=torch.float32, device=dev),
+                           norm_scratch=torch.zeros((lib.fno_grad_norm_scratch_bytes() + 7) // 8, dtype=torch.float64,
+                                                    device=dev))
+            self.norm_host = torch.empty(self.steps, dtype=torch.float32, pin_memory=True)
+        if self.ema_decay is not None:
+            self.io["ema_d"] = torch.empty(self.steps, dtype=torch.float32, device=dev)
+            self.ema_host = torch.empty(self.steps, dtype=torch.float32, pin_memory=True)
         if noise_std > 0:   # the epoch's first Adam step; a step's noise step is this plus the cursor
             self.io["step_base"] = torch.zeros(1, dtype=torch.int64, device=dev)
             self.step_base_host = torch.empty(1, dtype=torch.int64, pin_memory=True)
@@ -133,6 +145,12 @@ class _StepGraphs:
                 t.n[i] = numel
             self.adam.append(t)
         self.states = states
+        self.adam_arr = (_lib.FnoAdamTensors * len(self.adam))(*self.adam)   # the norm launch's tables
+        self.ema_ptrs = [None] * len(self.adam)
+        if self.ema_decay is not None:
+            self.ema_ptrs = [(C.c_void_p * t.count)(*[_real(st["ema"]).data_ptr()
+                                                      for st in states[i0:i0 + t.count]])
+                             for i0, t in zip(range(0, len(states), _lib.ADAM_MAX_TENSORS), self.adam)]
         self.betas, self.eps, self.weight_decay = group["betas"], group["eps"], group["weight_decay"]
 
         # capture: a warm-up of every launch except Adam and the log (it updates nothing: parameters, optimizer state
@@ -215,15 +233,29 @@ class _StepGraphs:
         """Adam on the flat gradients, then the step's five loss scalars (at device address loss_row) into the log."""
         lib, io = self.lib, self.io
         b1, b2 = self.betas
-        for t in self.adam:
-            _lib.check(lib.fno_adam_step_dev(C.byref(t), io["coef"].data_ptr(), self.steps, io["cursor"].data_ptr(), b1, b2,
-                                             self.eps, self.weight_decay, st), "fno_adam_step_dev")
+        if self.max_grad_norm is None and self.ema_decay is None:
+            for t in self.adam:
+                _lib.check(lib.fno_adam_step_dev(C.byref(t), io["coef"].data_ptr(), self.steps, io["cursor"].data_ptr(),
+                                                 b1, b2, self.eps, self.weight_decay, st), "fno_adam_step_dev")
+        else:   # the global norm into its log row, then Adam with the clip and / or the EMA
+            clip = None
+            if self.max_grad_norm is not None:
+                _lib.check(lib.fno_grad_norm(self.adam_arr, len(self.adam), self.max_grad_norm, io["norm"].data_ptr(),
+                                             io["norm_scratch"].data_ptr(), io["norm_log"].data_ptr(), self.steps,
+                                             io["cursor"].data_ptr(), st), "fno_grad_norm")
+                clip = io["norm"][1:].data_ptr()
+            ema_d = io["ema_d"].data_ptr() if self.ema_decay is not None else None
+            for t, ema in zip(self.adam, self.ema_ptrs):
+                _lib.check(lib.fno_adam_step_dev_ex(C.byref(t), io["coef"].data_ptr(), self.steps, io["cursor"].data_ptr(),
+                                                    b1, b2, self.eps, self.weight_decay, clip, ema, ema_d, st),
+                           "fno_adam_step_dev_ex")
         _lib.check(lib.fno_train_log_step(loss_row, io["log"].data_ptr(), self.steps, io["cursor"].data_ptr(), st),
                    "fno_train_log_step")
 
     def epoch(self, perm: np.ndarray, lr: float, first_step: int) -> np.ndarray:
         """Train one epoch visiting the samples in `perm` at learning rate `lr`, Adam's 1-based step count starting at
-        `first_step`.  Returns the (steps, 5) float32 log of fno_loss_fwd's scalars per step (LOG_COLUMNS)."""
+        `first_step`.  Returns the (steps, 5) float32 log of fno_loss_fwd's scalars per step (LOG_COLUMNS); with
+        clipping, `self.norms` then holds the (steps,) float32 pre-clip gradient norms."""
         io = self.io
         self.perm_host.numpy()[:] = perm   # the previous epoch's uploads completed before its log came back
         b1, b2 = self.betas
@@ -231,6 +263,10 @@ class _StepGraphs:
                    "fno_adam_coefficients")
         io["perm"].copy_(self.perm_host, non_blocking=True)
         io["coef"].copy_(self.coef_host, non_blocking=True)
+        if self.ema_decay is not None:
+            _lib.check(self.lib.fno_ema_decays(self.ema_decay, first_step, self.steps, self.ema_host.data_ptr()),
+                       "fno_ema_decays")
+            io["ema_d"].copy_(self.ema_host, non_blocking=True)
         if self.noise_std > 0:
             self.step_base_host[0] = first_step
             io["step_base"].copy_(self.step_base_host, non_blocking=True)
@@ -238,7 +274,12 @@ class _StepGraphs:
         for g, count in zip(self.graphs, self.counts):
             for _ in range(count):
                 g.replay()
+        if self.max_grad_norm is not None:   # complete once the log below has come back
+            self.norm_host.copy_(io["norm_log"], non_blocking=True)
         log = io["log"].cpu().numpy()   # the epoch's one synchronisation
+        if self.max_grad_norm is not None:
+            self.norms = self.norm_host.numpy().copy()
+            self.optimizer.last_grad_norm = io["norm"][0].clone()
         # the state torch.optim.Adam would hold, and the version bump FusedAdam.step makes (Fno2d's packed-weight cache
         # and inference graphs are keyed on the parameters' versions)
         for st in self.states:
@@ -382,12 +423,28 @@ def _check_split(model, data, what: str) -> None:
     model._route(gh, gw)      # the model's own grid / storage-mode checks
 
 
+def _ema_shadow(model):
+    """A Fno2d with `model`'s configuration, storage mode, device and kernel choices, holding a copy of its weights: the
+    model the EMA weights are evaluated and saved through.  Built without drawing from the CPU RNG (the parameters'
+    initialisation would shift the visiting order of a train_auto that uses the global RNG)."""
+    from .fno2d import Fno2d
+    with torch.random.fork_rng(devices=[]):
+        shadow = Fno2d(model.in_chan, model.out_chan, model.n_case_params, model.loss_fn, model.num_layers,
+                       modes1=model.modes1, modes2=model.modes2, hidden_dim=model.hidden_dim, act_dtype=model.act_dtype,
+                       device=model.device)
+    for name in ("graph_rollout", "fused_block", "max_graphs", "generic_grid_at_64"):
+        setattr(shadow, name, getattr(model, name))
+    shadow.load_state_dict(model.state_dict())
+    return shadow
+
+
 def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, lr: float = 1e-3, lr_step_size: int = 1,
                lr_gamma: float = 0.9, batch_size: int = 2, eval_batch_size: int = 2, log_interval: int = 10,
                eval_interval: int = 2, generator: Optional[torch.Generator] = None, rollout_steps: int = 1,
                time_step_size: Optional[int] = None, input_noise_std: float = 0.0, noise_seed: int = 0,
                rollout_grad_steps: Optional[int] = None, noise_every_step: bool = False,
-               dev_rollout_steps: Optional[int] = None) -> dict:
+               dev_rollout_steps: Optional[int] = None, max_grad_norm: Optional[float] = None,
+               ema_decay: Optional[float] = None) -> dict:
     """What the reference's `train(model, train_data, dev_data, output_dir, ...)` does (src/train_auto.py:181-313), with
     its argument names and defaults, every training step replayed from a CUDA graph and one synchronisation per epoch.
 
@@ -464,6 +521,20 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
       argument, else dev_data.time_step_size; it must have an S-step window and chain (checked once on the device
       before training).  The evaluation draws nothing from the RNG, so training is bit-identical with and without it;
       None (the default) runs exactly what runs without the option.
+    - max_grad_norm = c clips the global gradient norm to c before every update, `clip_grad_norm_(every trainable
+      parameter, c)`, inside the step graph: one float64 norm launch (bit-reproducible) and the coefficient read by the
+      Adam launch.  Each step's pre-clip norm is logged on the device: the log line gains grad_norm, the result
+      `grad_norms` (every step, every epoch) and `output_dir / "grad_norms.json"` holds them.
+    - ema_decay = d keeps an exponential moving average of the weights, updated by the Adam launch: diffusers'
+      EMAModel with warmup, decay min(d, 1 - t^(-3/4)) at Adam's step t (0 at t = 1: the EMA starts as the trained
+      weights), inv_gamma 1, power 3/4, as train_diffusers.py configures it.  Every evaluation runs on an EMA copy of the
+      model (same configuration, storage mode and device; `FusedAdam.copy_ema_to`), so dev_scores.json, scores.json's
+      dev_loss (and the rollout score with dev_rollout_steps) and model.pt are the EMA weights', which the reference's
+      load_best_ckpt and test_multistep then read.  `model` itself ends with the trained weights; the result gains
+      `ema_model`.
+      With either option one step is bit-identical to the eager loops above with
+      `FusedAdam(model.parameters(), lr, max_grad_norm=max_grad_norm, ema_decay=ema_decay)`, its state["ema"] and
+      `last_grad_norm` included.  None (the defaults) launches exactly what runs without the options.
     Returns dict(train_losses=[per-step nmse, every epoch], optimizer=the FusedAdam).  Its state holds the true step
     count (its state_dict loads into torch.optim.Adam), and the parameters' version counters are bumped, so the
     model's packed weights and inference graphs are rebuilt on the next call.  Raises before any device work on: a
@@ -474,14 +545,15 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
     no time_step_size, a split without a single K-step window, or a split whose frames do not chain.  Also raises
     ValueError before any device work for an input_noise_std that is negative, NaN, infinite or not a real number, a
     noise_seed that is not an int in [0, 2^64), a rollout_grad_steps that is not an int in 1..rollout_steps, a
-    noise_every_step that is not a bool, or a dev_rollout_steps that is not None or a positive int; with
+    noise_every_step that is not a bool, a dev_rollout_steps that is not None or a positive int, a max_grad_norm
+    that is not None or a finite real > 0, or an ema_decay that is not None or a real in [0, 1); with
     dev_rollout_steps, as ValueError before any training step, a dev split without a time step size, without a single
     S-step window, or whose frames do not chain.
     Frozen parameters (requires_grad=False) are not updated, as FusedAdam.step skips them.  Data parallel training in
     this loop is not supported."""
     from .metrics import _evaluate_rollout, evaluate_auto
     from .fno2d import Fno2d
-    from .optim import FusedAdam
+    from .optim import FusedAdam, check_stabiliser_args
     if not isinstance(model, Fno2d):
         raise TypeError(f"train_auto runs the drop-in cfdbench_b200.Fno2d, got {type(model).__name__}")
     names = list(model.loss_fn.get_score_names())
@@ -497,6 +569,7 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
     if dev_rollout_steps is not None:
         _positive_int("dev_rollout_steps", dev_rollout_steps)
         dev_rollout_steps = int(dev_rollout_steps)
+    max_grad_norm, ema_decay = check_stabiliser_args(max_grad_norm, ema_decay)
     grad_steps = rollout_steps if rollout_grad_steps is None else rollout_grad_steps
     if isinstance(grad_steps, bool) or not isinstance(grad_steps, (int, np.integer)) or not 1 <= grad_steps <= rollout_steps:
         raise ValueError(f"rollout_grad_steps must be an int in 1..rollout_steps={rollout_steps}, got {rollout_grad_steps!r}")
@@ -536,7 +609,7 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
     output_dir = Path(output_dir)
     output_dir.mkdir(exist_ok=True, parents=True)
 
-    optimizer = FusedAdam(model.parameters(), lr=lr)
+    optimizer = FusedAdam(model.parameters(), lr=lr, max_grad_norm=max_grad_norm, ema_decay=ema_decay)
     scheduler = torch.optim.lr_scheduler.StepLR(optimizer, step_size=lr_step_size, gamma=lr_gamma)
     with torch.cuda.device(dev):
         frames = train_data if isinstance(train_data, DeviceFrames) else DeviceFrames(train_data, device=dev)
@@ -545,6 +618,7 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
             dev_frames = dev_data if isinstance(dev_data, DeviceFrames) else DeviceFrames(dev_data, device=dev)
             _check_chain(dev_frames, dev_windows, dev_rollout_steps, dev_tss, what="dev_data")
         n = frames.n
+        ema_model = None if ema_decay is None else _ema_shadow(model)
         noise = dict(noise_std=input_noise_std, noise_seed=int(noise_seed))
         if windows is None:
             graphs = _StepGraphs(model, frames, batch_size, optimizer, **noise)
@@ -562,6 +636,10 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
         if input_noise_std > 0:
             every = ", on every rollout step" if noise_every_step and windows is not None else ""
             print(f"# input noise std: {input_noise_std}, seed {int(noise_seed)}{every}")
+        if max_grad_norm is not None:
+            print(f"# max grad norm: {max_grad_norm}")
+        if ema_decay is not None:
+            print(f"# ema decay: {ema_decay} (evaluated and saved: the EMA weights)")
         if dev_windows is not None:
             print(f"# dev rollout steps: {dev_rollout_steps}, windows: {dev_windows.size} (checkpoints scored by rollout "
                   "nmse)")
@@ -570,6 +648,7 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
         start_time = time.time()
         global_step = 0
         train_losses: List[float] = []
+        grad_norms: List[float] = []
         try:
             for ep in range(num_epochs):
                 ep_start_time = time.time()
@@ -580,11 +659,16 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
                     perm = windows[epoch_permutation(windows.size, batch_size, generator)]
                 log = graphs.epoch(perm, lr_ep, global_step + 1)
                 ep_train_losses = [float(v) for v in log[:, 3]]
+                if max_grad_norm is not None:
+                    grad_norms += [float(v) for v in graphs.norms]
                 for step in range(graphs.steps):
                     global_step += 1
                     if global_step % log_interval == 0:
-                        print(dict(ep=ep, step=step, mse=f"{float(log[step, 0]):.3e}", nmse=f"{float(log[step, 3]):.3e}",
-                                   lr=f"{scheduler.get_last_lr()[0]:.3e}", time=round(time.time() - start_time)))
+                        line = dict(ep=ep, step=step, mse=f"{float(log[step, 0]):.3e}", nmse=f"{float(log[step, 3]):.3e}",
+                                    lr=f"{scheduler.get_last_lr()[0]:.3e}", time=round(time.time() - start_time))
+                        if max_grad_norm is not None:
+                            line["grad_norm"] = f"{float(graphs.norms[step]):.3e}"
+                        print(line)
                 with warnings.catch_warnings():   # the optimizer steps ran inside the graph, not through .step()
                     warnings.filterwarnings("ignore", message=r"Detected call of `lr_scheduler\.step\(\)` before")
                     scheduler.step()
@@ -595,7 +679,11 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
                     ckpt_dir.mkdir(exist_ok=True, parents=True)
                     if dev_frames is None:
                         dev_frames = dev_data if isinstance(dev_data, DeviceFrames) else DeviceFrames(dev_data, device=dev)
-                    dev_scores = evaluate_auto(model, dev_frames, batch_size=eval_batch_size)["scores"]
+                    eval_model = model
+                    if ema_model is not None:   # evaluate and save the EMA weights
+                        optimizer.copy_ema_to(ema_model)
+                        eval_model = ema_model
+                    dev_scores = evaluate_auto(eval_model, dev_frames, batch_size=eval_batch_size)["scores"]
                     dump_json(dev_scores, ckpt_dir / "dev_scores.json")
                     dump_json(ep_train_losses, ckpt_dir / "train_loss.json")
                     ckpt_path = ckpt_dir / "model.pt"
@@ -604,13 +692,13 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
                         ckpt_backup_path = ckpt_dir / "backup_model.pt"
                         print(f"Backing up old checkpoint to {ckpt_backup_path}")
                         copyfile(ckpt_path, ckpt_backup_path)
-                    torch.save(model.state_dict(), ckpt_path)
+                    torch.save(eval_model.state_dict(), ckpt_path)
                     dev_loss = np.mean(dev_scores["all"]["nmse"])
                     if dev_windows is None:
                         ep_scores = dict(ep=ep, train_loss=np.mean(ep_train_losses), dev_loss=dev_loss,
                                          time=time.time() - ep_start_time)
                     else:
-                        rollout = _evaluate_rollout(model, dev_frames, dev_windows, dev_rollout_steps, dev_tss)
+                        rollout = _evaluate_rollout(eval_model, dev_frames, dev_windows, dev_rollout_steps, dev_tss)
                         dump_json(rollout, ckpt_dir / "dev_rollout_scores.json")
                         ep_scores = dict(ep=ep, train_loss=np.mean(ep_train_losses), dev_loss=rollout["loss"],
                                          dev_loss_single_step=dev_loss, time=time.time() - ep_start_time)
@@ -619,4 +707,11 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
             del graphs   # the graphs and their static buffers go with the call
     print("====== Training done ======")
     dump_json(train_losses, output_dir / "train_losses.json")
-    return dict(train_losses=train_losses, optimizer=optimizer)
+    out = dict(train_losses=train_losses, optimizer=optimizer)
+    if max_grad_norm is not None:
+        dump_json(grad_norms, output_dir / "grad_norms.json")
+        out["grad_norms"] = grad_norms
+    if ema_model is not None:
+        optimizer.copy_ema_to(ema_model)
+        out["ema_model"] = ema_model
+    return out

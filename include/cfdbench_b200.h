@@ -302,6 +302,41 @@ int fno_adam_coefficients(float lr, float beta1, float beta2, int64_t first_step
  * outside 0..n_log-1. */
 int fno_train_log_step(const float* loss_out, float* log, int n_log, int32_t* cursor, void* stream);
 
+/* ---- gradient-norm clipping and an EMA of the weights (FusedAdam(max_grad_norm=..., ema_decay=...), train_auto) -----
+ * torch.nn.utils.clip_grad_norm_(params, max_norm) followed by torch.optim.Adam.step, and diffusers' EMAModel.step after
+ * it, fused into the Adam launch.  Argument checks come before any device work (status 1). */
+/* The global norm: out[0] = ||g||_2 over the gradients of every entry of tables[0..n_tables-1] (the grad and n fields;
+ * complex gradients as their real pairs, as torch counts them), out[1] = clip_grad_norm_'s coefficient
+ * min(1, max_norm / (out[0] + 1e-6)) in float32 (evaluated as torch does, reciprocal(out[0] + 1e-6) * max_norm; a NaN
+ * norm gives a NaN coefficient, an infinite norm 0).  The squares are summed in float64 by a fixed grid with per-block
+ * partials and an in-order final sum (no float atomics), so the result is bit-reproducible; the norm is the float32
+ * rounding of the square root.  With log != NULL also log[c] = out[0] for c = *cursor when 0 <= c < n_log (the step's row,
+ * as fno_train_log_step picks it; the cursor is not advanced).  out: float32 [2] in device memory.  scratch:
+ * fno_grad_norm_scratch_bytes() bytes, 8-byte aligned, zero-initialised once by the caller (the kernel leaves it zeroed);
+ * one scratch buffer serves one stream at a time.  No host synchronisation; can be captured into a graph.  Status 1 for
+ * n_tables outside 1..FNO_GRAD_NORM_MAX_TABLES, a bad table, max_norm not finite and > 0, or a null out / scratch
+ * (or cursor, with log). */
+#define FNO_GRAD_NORM_MAX_TABLES 8
+size_t fno_grad_norm_scratch_bytes(void);
+int fno_grad_norm(const fno_adam_tensors* tables, int n_tables, float max_norm, float* out, void* scratch, float* log,
+                  int n_log, const int32_t* cursor, void* stream);
+/* fno_adam_step with two optional additions, each selected by a non-NULL argument (with both NULL it is fno_adam_step):
+ *   clip_coef (device float32, e.g. fno_grad_norm's out + 1): every gradient is read as g * (*clip_coef) before the
+ *     weight decay -- clip_grad_norm_ before optimizer.step();
+ *   ema (host array of t->count device pointers, ema[i] holding n[i] float32 like param[i]): after the update,
+ *     ema[i] = fmaf(-d, p_new - ema[i], p_new) with d = min(ema_decay, 1 - step^(-3/4)) computed in double and rounded
+ *     to float32 (fno_ema_decays), diffusers' EMAModel with use_ema_warmup, inv_gamma 1, power 3/4.  d = 0 at step 1, so
+ *     the EMA then equals the weights.  ema_decay in [0, 1). */
+int fno_adam_step_ex(const fno_adam_tensors* t, float lr, float beta1, float beta2, float eps, float weight_decay,
+                     int64_t step, const float* clip_coef, void* const* ema, double ema_decay, void* stream);
+/* fno_adam_step_dev with the same additions; the EMA decay is ema_decay_tab[c] (device float32 [n_coef], as
+ * fno_ema_decays fills it) for c = *cursor, read on the device.  ema_decay_tab is required with ema and ignored without. */
+int fno_adam_step_dev_ex(const fno_adam_tensors* t, const float* coef, int n_coef, const int32_t* cursor, float beta1,
+                         float beta2, float eps, float weight_decay, const float* clip_coef, void* const* ema,
+                         const float* ema_decay_tab, void* stream);
+/* Host function: host_out[i] = the EMA decay fno_adam_step_ex uses at step first_step + i, i < n. */
+int fno_ema_decays(double ema_decay, int64_t first_step, int n, float* host_out);
+
 /* ---- training through K-step rollouts (cfdbench_b200.train_auto with rollout_steps = K) --------------------------
  * A dataset holds a case's samples contiguously with inputs = frames[:-s], labels = frames[s:] (s = time_step_size), so
  * the k-th target of the window that starts at sample j is labels[j + k s].  Every entry point checks its arguments before
