@@ -17,6 +17,7 @@ synchronisation.  The result is bit-identical to the eager loop `DeviceFrames.lo
     train_auto(..., rollout_steps=4, rollout_grad_steps=1)   # pushforward: 3 steps without gradient, the 4th trained
     train_auto(..., input_noise_std=0.01, noise_seed=1)      # Gaussian noise on every step's input frame
     train_auto(..., rollout_steps=4, input_noise_std=0.01, noise_every_step=True)   # ... and on every rollout step's
+    train_auto(..., resumable=True)   # relaunching the same call continues an interrupted run bit for bit
 """
 from __future__ import annotations
 
@@ -31,7 +32,7 @@ from typing import List, Optional
 import numpy as np
 import torch
 
-from . import _lib
+from . import _lib, resume
 from .data import DeviceFrames, _check_chain, _gather, case_table, check_noise_args, index_batches, rollout_windows
 from .fno2d import capture_graph, side_stream
 
@@ -53,11 +54,13 @@ def dev_eval_draw(generator=None) -> None:
     next(index_batches(1, 1, False, generator))
 
 
-def index_stream(n: int, batch_size: int, num_epochs: int, eval_interval: int, generator=None) -> List[np.ndarray]:
-    """The per-epoch sample orders `train_auto` visits, consuming the RNG as `train_auto` does: epoch ep's permutation,
-    then one evaluation draw when (ep + 1) % eval_interval == 0."""
+def index_stream(n: int, batch_size: int, num_epochs: int, eval_interval: int, generator=None,
+                 start_epoch: int = 0) -> List[np.ndarray]:
+    """The per-epoch sample orders `train_auto` visits in epochs start_epoch .. num_epochs - 1, consuming the RNG as
+    `train_auto` does: epoch ep's permutation, then one evaluation draw when (ep + 1) % eval_interval == 0.  A resumed
+    run starts at the epoch after its state's, with the RNG restored to where that epoch left it."""
     out = []
-    for ep in range(num_epochs):
+    for ep in range(start_epoch, num_epochs):
         out.append(epoch_permutation(n, batch_size, generator))
         if (ep + 1) % eval_interval == 0:
             dev_eval_draw(generator)
@@ -444,7 +447,7 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
                time_step_size: Optional[int] = None, input_noise_std: float = 0.0, noise_seed: int = 0,
                rollout_grad_steps: Optional[int] = None, noise_every_step: bool = False,
                dev_rollout_steps: Optional[int] = None, max_grad_norm: Optional[float] = None,
-               ema_decay: Optional[float] = None) -> dict:
+               ema_decay: Optional[float] = None, resumable: bool = False) -> dict:
     """What the reference's `train(model, train_data, dev_data, output_dir, ...)` does (src/train_auto.py:181-313), with
     its argument names and defaults, every training step replayed from a CUDA graph and one synchronisation per epoch.
 
@@ -535,7 +538,22 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
       With either option one step is bit-identical to the eager loops above with
       `FusedAdam(model.parameters(), lr, max_grad_norm=max_grad_norm, ema_decay=ema_decay)`, its state["ema"] and
       `last_grad_norm` included.  None (the defaults) launches exactly what runs without the options.
-    Returns dict(train_losses=[per-step nmse, every epoch], optimizer=the FusedAdam).  Its state holds the true step
+    - resumable=True keeps the full training state in `output_dir / "training_state.pt"` (cfdbench_b200.resume): the
+      trained weights, FusedAdam's state (step, both moments, the EMA), StepLR's, the visiting order's RNG state,
+      Adam's global step, train_losses / grad_norms and a config record.  It is written atomically (a temporary file,
+      then os.replace) after each evaluation epoch's checkpoint files and after the last epoch, one file overwritten
+      each time.  At start-up an existing state is checked against this call (the model's configuration, every
+      argument that changes the trajectory or the checkpoint scores, and each split's size, grid, case-parameter count,
+      frame dtype and case_ids hash -- not the frame contents; num_epochs and log_interval may change), loaded into
+      `model` and the new optimizer, scheduler and RNG, and training continues from the epoch after the one it records,
+      bit-identical to a run that was never interrupted; its train_losses / grad_norms cover the whole run.  With
+      num_epochs no larger than the epochs already trained no step runs and the finished run's result is returned
+      (the JSON files rewritten); a larger num_epochs extends the run, equal to a longer straight run.  Without a state
+      an output_dir that holds ckpt-* directories is refused, and otherwise the run starts fresh.  So relaunching the
+      same call is the whole recovery procedure; a killed run retrains at most the epochs since the last evaluation.
+      False (the default) writes and reads nothing more than without the option.
+    Returns dict(train_losses=[per-step nmse, every epoch], optimizer=the FusedAdam, start_epoch=the first epoch this
+    call trained: 0, or E + 1 after resuming from epoch E).  Its state holds the true step
     count (its state_dict loads into torch.optim.Adam), and the parameters' version counters are bumped, so the
     model's packed weights and inference graphs are rebuilt on the next call.  Raises before any device work on: a
     model that is not the drop-in Fno2d, a CPU model (FnoNativeError), a loss without "nmse", non-positive sizes,
@@ -548,7 +566,10 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
     noise_every_step that is not a bool, a dev_rollout_steps that is not None or a positive int, a max_grad_norm
     that is not None or a finite real > 0, or an ema_decay that is not None or a real in [0, 1); with
     dev_rollout_steps, as ValueError before any training step, a dev split without a time step size, without a single
-    S-step window, or whose frames do not chain.
+    S-step window, or whose frames do not chain.  With resumable=True, also ValueError before any device work for a
+    training_state.pt that does not load, has another format version or was written with another config (naming every
+    differing field), or for an output_dir with ckpt-* directories and no training_state.pt; ValueError for a
+    resumable that is not a bool.
     Frozen parameters (requires_grad=False) are not updated, as FusedAdam.step skips them.  Data parallel training in
     this loop is not supported."""
     from .metrics import _evaluate_rollout, evaluate_auto
@@ -566,6 +587,8 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
     input_noise_std = check_noise_args(input_noise_std, noise_seed, std_name="input_noise_std")
     if not isinstance(noise_every_step, bool):
         raise ValueError(f"noise_every_step must be a bool, got {noise_every_step!r}")
+    if not isinstance(resumable, bool):
+        raise ValueError(f"resumable must be a bool, got {resumable!r}")
     if dev_rollout_steps is not None:
         _positive_int("dev_rollout_steps", dev_rollout_steps)
         dev_rollout_steps = int(dev_rollout_steps)
@@ -605,12 +628,36 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
         if dev_windows.size == 0:
             raise ValueError(f"dev_data has no {dev_rollout_steps}-step window with time_step_size={dev_tss} inside one "
                              "case")
+    state = config = None
+    if resumable:
+        # Python floats, so that StepLR's decay of a restored learning rate runs in the same arithmetic as a straight
+        # run's, and the state holds no numpy scalar (it must load with weights_only=True)
+        lr, lr_gamma = float(lr), float(lr_gamma)
+        config = resume.run_config(
+            model, train_data, dev_data, lr=lr, lr_step_size=int(lr_step_size), lr_gamma=lr_gamma,
+            batch_size=int(batch_size), eval_batch_size=int(eval_batch_size), eval_interval=int(eval_interval),
+            rollout_steps=int(rollout_steps), time_step_size=int(tss) if windows is not None else None,
+            rollout_grad_steps=grad_steps, input_noise_std=float(input_noise_std), noise_seed=int(noise_seed),
+            noise_every_step=noise_every_step, dev_rollout_steps=dev_rollout_steps,
+            dev_time_step_size=dev_tss if dev_windows is not None else None, max_grad_norm=max_grad_norm,
+            ema_decay=ema_decay, generator=generator is not None)
+        state = resume.find_state(output_dir, config)
     model._require_cuda()
     output_dir = Path(output_dir)
     output_dir.mkdir(exist_ok=True, parents=True)
 
     optimizer = FusedAdam(model.parameters(), lr=lr, max_grad_norm=max_grad_norm, ema_decay=ema_decay)
     scheduler = torch.optim.lr_scheduler.StepLR(optimizer, step_size=lr_step_size, gamma=lr_gamma)
+    start_epoch, global_step = 0, 0
+    train_losses: List[float] = []
+    grad_norms: List[float] = []
+    if state is not None:   # before the graphs are captured: they hold raw pointers to the optimizer state
+        model.load_state_dict(state["model"])
+        optimizer.load_state_dict(state["optimizer"])
+        scheduler.load_state_dict(state["scheduler"])
+        resume.restore_rng(state, generator)
+        start_epoch, global_step = state["epoch"] + 1, state["global_step"]
+        train_losses, grad_norms = list(state["train_losses"]), list(state.get("grad_norms", []))
     with torch.cuda.device(dev):
         frames = train_data if isinstance(train_data, DeviceFrames) else DeviceFrames(train_data, device=dev)
         dev_frames = None
@@ -620,12 +667,15 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
         n = frames.n
         ema_model = None if ema_decay is None else _ema_shadow(model)
         noise = dict(noise_std=input_noise_std, noise_seed=int(noise_seed))
-        if windows is None:
-            graphs = _StepGraphs(model, frames, batch_size, optimizer, **noise)
-        else:
+        if windows is not None:
             _check_chain(frames, windows, rollout_steps, int(tss))
-            graphs = _RolloutStepGraphs(model, frames, batch_size, optimizer, windows.size, rollout_steps, int(tss),
-                                        grad_steps, noise_every_step=noise_every_step, **noise)
+        graphs = None   # a resumed run with no epoch left to train captures nothing
+        if start_epoch < num_epochs:
+            if windows is None:
+                graphs = _StepGraphs(model, frames, batch_size, optimizer, **noise)
+            else:
+                graphs = _RolloutStepGraphs(model, frames, batch_size, optimizer, windows.size, rollout_steps,
+                                            int(tss), grad_steps, noise_every_step=noise_every_step, **noise)
         print("====== Training ======")
         print(f"# batch: {batch_size}")
         print(f"# examples: {n}")
@@ -643,14 +693,13 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
         if dev_windows is not None:
             print(f"# dev rollout steps: {dev_rollout_steps}, windows: {dev_windows.size} (checkpoints scored by rollout "
                   "nmse)")
-        print(f"# step: {graphs.steps}")
+        print(f"# step: {-(-(n if windows is None else windows.size) // batch_size)}")
         print(f"# epoch: {num_epochs}")
+        if state is not None:
+            print(f"# resumed from epoch {state['epoch']} (step {global_step}): {output_dir / resume.STATE_NAME}")
         start_time = time.time()
-        global_step = 0
-        train_losses: List[float] = []
-        grad_norms: List[float] = []
         try:
-            for ep in range(num_epochs):
+            for ep in range(start_epoch, num_epochs):
                 ep_start_time = time.time()
                 lr_ep = optimizer.param_groups[0]["lr"]
                 if windows is None:
@@ -703,11 +752,15 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
                         ep_scores = dict(ep=ep, train_loss=np.mean(ep_train_losses), dev_loss=rollout["loss"],
                                          dev_loss_single_step=dev_loss, time=time.time() - ep_start_time)
                     dump_json(ep_scores, ckpt_dir / "scores.json")
+                if resumable and ((ep + 1) % eval_interval == 0 or ep == num_epochs - 1):   # after the checkpoint
+                    resume.write_state(resume.build_state(ep, global_step, model, optimizer, scheduler, generator,
+                                                          train_losses, grad_norms if max_grad_norm is not None else None,
+                                                          config), output_dir)
         finally:
             del graphs   # the graphs and their static buffers go with the call
     print("====== Training done ======")
     dump_json(train_losses, output_dir / "train_losses.json")
-    out = dict(train_losses=train_losses, optimizer=optimizer)
+    out = dict(train_losses=train_losses, optimizer=optimizer, start_epoch=start_epoch)
     if max_grad_norm is not None:
         dump_json(grad_norms, output_dir / "grad_norms.json")
         out["grad_norms"] = grad_norms
