@@ -21,9 +21,6 @@ cudaError_t launch_gather_batch(const void*, const void*, const float*, const in
 cudaError_t launch_loss_fwd(const float*, const float*, size_t, float*, float*, cudaStream_t);
 cudaError_t launch_loss_bwd(const float*, const float*, const float*, const float*, float*, size_t, cudaStream_t);
 size_t loss_scratch_bytes();
-cudaError_t launch_adam_step(const fno_adam_tensors*, float, float, float, float, float, long long, cudaStream_t);
-cudaError_t launch_adam_step_dev(const fno_adam_tensors*, const float*, int, const int*, float, float, float, float,
-                                 cudaStream_t);
 void adam_coefficients(float, float, float, long long, float*, float*);
 cudaError_t launch_adam_step_ex(const fno_adam_tensors*, float, float, float, float, float, long long, const float*,
                                 void* const*, double, cudaStream_t);
@@ -731,33 +728,60 @@ int fno_loss_bwd(const float* preds, const float* labels, const float* fwd, cons
   return kOk;
 }
 
-int fno_adam_step(const fno_adam_tensors* t, float lr, float beta1, float beta2, float eps, float weight_decay,
-                  int64_t step, void* stream) {
-  if (!t || t->count < 0 || t->count > FNO_ADAM_MAX_TENSORS || step < 1)
-    return fail(kErrArg, "fno_adam_step: bad argument");
-  for (int i = 0; i < t->count; ++i)
-    if (!t->param[i] || !t->grad[i] || !t->exp_avg[i] || !t->exp_avg_sq[i] || t->n[i] <= 0)
-      return fail(kErrArg, "fno_adam_step: null tensor or empty size");
-  FNO_CUDA(launch_adam_step(t, lr, beta1, beta2, eps, weight_decay, step, S(stream)), "adam_step_kernel");
-  return kOk;
-}
-
 static int adam_tensors_ok(const fno_adam_tensors* t) {
   if (!t || t->count < 0 || t->count > FNO_ADAM_MAX_TENSORS) return 0;
   for (int i = 0; i < t->count; ++i)
     if (!t->param[i] || !t->grad[i] || !t->exp_avg[i] || !t->exp_avg_sq[i] || t->n[i] <= 0) return 0;
   return 1;
 }
+static bool ema_ok(const fno_adam_tensors* t, void* const* ema) {
+  if (!ema) return true;
+  for (int i = 0; i < t->count; ++i)
+    if (!ema[i]) return false;
+  return true;
+}
+static inline bool decay_ok(double d) { return d >= 0.0 && d < 1.0; }   // false for NaN
+
+// The checks and launch behind fno_adam_step and fno_adam_step_ex (clip_coef and ema NULL: the plain update); `what` is
+// the entry point, named in fno_last_error().
+static int adam_step_impl(const char* what, const fno_adam_tensors* t, float lr, float beta1, float beta2, float eps,
+                          float weight_decay, int64_t step, const float* clip_coef, void* const* ema, double ema_decay,
+                          void* stream) {
+  const bool args_ok = step >= 1 && (!ema || decay_ok(ema_decay));
+  if (!args_ok || !adam_tensors_ok(t) || !ema_ok(t, ema)) {
+    char msg[96];
+    snprintf(msg, sizeof(msg), "%s: %s", what, args_ok ? "bad tensor table" : "bad argument");
+    return fail(kErrArg, msg);
+  }
+  FNO_CUDA(launch_adam_step_ex(t, lr, beta1, beta2, eps, weight_decay, step, clip_coef, ema, ema_decay, S(stream)), what);
+  return kOk;
+}
+
+// The same for fno_adam_step_dev and fno_adam_step_dev_ex.
+static int adam_step_dev_impl(const char* what, const fno_adam_tensors* t, const float* coef, int n_coef,
+                              const int32_t* cursor, float beta1, float beta2, float eps, float weight_decay,
+                              const float* clip_coef, void* const* ema, const float* ema_decay_tab, void* stream) {
+  const bool args_ok = coef && cursor && n_coef > 0 && !(reinterpret_cast<uintptr_t>(coef) & 7) && (!ema || ema_decay_tab);
+  if (!args_ok || !adam_tensors_ok(t) || !ema_ok(t, ema)) {
+    char msg[96];
+    snprintf(msg, sizeof(msg), "%s: %s", what, args_ok ? "bad tensor table" : "bad argument");
+    return fail(kErrArg, msg);
+  }
+  FNO_CUDA(launch_adam_step_dev_ex(t, coef, n_coef, reinterpret_cast<const int*>(cursor), beta1, beta2, eps, weight_decay,
+                                   clip_coef, ema, ema ? ema_decay_tab : nullptr, S(stream)),
+           what);
+  return kOk;
+}
+
+int fno_adam_step(const fno_adam_tensors* t, float lr, float beta1, float beta2, float eps, float weight_decay,
+                  int64_t step, void* stream) {
+  return adam_step_impl("fno_adam_step", t, lr, beta1, beta2, eps, weight_decay, step, nullptr, nullptr, 0.0, stream);
+}
 
 int fno_adam_step_dev(const fno_adam_tensors* t, const float* coef, int n_coef, const int32_t* cursor, float beta1,
                       float beta2, float eps, float weight_decay, void* stream) {
-  if (!coef || !cursor || n_coef <= 0 || (reinterpret_cast<uintptr_t>(coef) & 7))
-    return fail(kErrArg, "fno_adam_step_dev: bad argument");
-  if (!adam_tensors_ok(t)) return fail(kErrArg, "fno_adam_step_dev: bad tensor table");
-  FNO_CUDA(launch_adam_step_dev(t, coef, n_coef, reinterpret_cast<const int*>(cursor), beta1, beta2, eps, weight_decay,
-                                S(stream)),
-           "adam_step_kernel<true>");
-  return kOk;
+  return adam_step_dev_impl("fno_adam_step_dev", t, coef, n_coef, cursor, beta1, beta2, eps, weight_decay, nullptr, nullptr,
+                            nullptr, stream);
 }
 
 int fno_adam_coefficients(float lr, float beta1, float beta2, int64_t first_step, int n, float* host_out) {
@@ -767,14 +791,6 @@ int fno_adam_coefficients(float lr, float beta1, float beta2, int64_t first_step
 }
 
 // ---------------------------------------------------------------- gradient-norm clipping and the EMA of the weights
-static bool ema_ok(const fno_adam_tensors* t, void* const* ema) {
-  if (!ema) return true;
-  for (int i = 0; i < t->count; ++i)
-    if (!ema[i]) return false;
-  return true;
-}
-static inline bool decay_ok(double d) { return d >= 0.0 && d < 1.0; }   // false for NaN
-
 size_t fno_grad_norm_scratch_bytes(void) { return grad_norm_scratch_bytes(); }
 
 int fno_grad_norm(const fno_adam_tensors* tables, int n_tables, float max_norm, float* out, void* scratch, float* log,
@@ -796,23 +812,15 @@ int fno_grad_norm(const fno_adam_tensors* tables, int n_tables, float max_norm, 
 
 int fno_adam_step_ex(const fno_adam_tensors* t, float lr, float beta1, float beta2, float eps, float weight_decay,
                      int64_t step, const float* clip_coef, void* const* ema, double ema_decay, void* stream) {
-  if (step < 1 || (ema && !decay_ok(ema_decay))) return fail(kErrArg, "fno_adam_step_ex: bad argument");
-  if (!adam_tensors_ok(t) || !ema_ok(t, ema)) return fail(kErrArg, "fno_adam_step_ex: bad tensor table");
-  FNO_CUDA(launch_adam_step_ex(t, lr, beta1, beta2, eps, weight_decay, step, clip_coef, ema, ema_decay, S(stream)),
-           "adam_step_ex_kernel");
-  return kOk;
+  return adam_step_impl("fno_adam_step_ex", t, lr, beta1, beta2, eps, weight_decay, step, clip_coef, ema, ema_decay,
+                        stream);
 }
 
 int fno_adam_step_dev_ex(const fno_adam_tensors* t, const float* coef, int n_coef, const int32_t* cursor, float beta1,
                          float beta2, float eps, float weight_decay, const float* clip_coef, void* const* ema,
                          const float* ema_decay_tab, void* stream) {
-  if (!coef || !cursor || n_coef <= 0 || (reinterpret_cast<uintptr_t>(coef) & 7) || (ema && !ema_decay_tab))
-    return fail(kErrArg, "fno_adam_step_dev_ex: bad argument");
-  if (!adam_tensors_ok(t) || !ema_ok(t, ema)) return fail(kErrArg, "fno_adam_step_dev_ex: bad tensor table");
-  FNO_CUDA(launch_adam_step_dev_ex(t, coef, n_coef, reinterpret_cast<const int*>(cursor), beta1, beta2, eps, weight_decay,
-                                   clip_coef, ema, ema ? ema_decay_tab : nullptr, S(stream)),
-           "adam_step_ex_kernel<true>");
-  return kOk;
+  return adam_step_dev_impl("fno_adam_step_dev_ex", t, coef, n_coef, cursor, beta1, beta2, eps, weight_decay, clip_coef, ema,
+                            ema_decay_tab, stream);
 }
 
 int fno_ema_decays(double ema_decay, int64_t first_step, int n, float* host_out) {

@@ -249,8 +249,8 @@ struct AdamArgs {
 };
 
 // The bias-corrected step size and 1/sqrt(bc2) of 1-based step `step`, as torch.optim.Adam forms them: in double, from
-// lr, beta1 and beta2 as the float32 values the kernel sees.  The one copy of this arithmetic: launch_adam_step and the
-// device coefficient table (fno_adam_coefficients) both call it, so the two paths cannot drift apart.
+// lr, beta1 and beta2 as the float32 values the kernel sees.  The one copy of this arithmetic: launch_adam_step_ex and
+// the device coefficient table (fno_adam_coefficients) both call it, so the two paths cannot drift apart.
 void adam_coefficients(float lr, float beta1, float beta2, long long step, float* step_size, float* inv_bc2_sqrt) {
   const double bc1 = 1.0 - pow(static_cast<double>(beta1), static_cast<double>(step));
   const double bc2 = 1.0 - pow(static_cast<double>(beta2), static_cast<double>(step));
@@ -351,37 +351,7 @@ static int adam_blocks(const fno_adam_tensors* t, AdamArgs& a) {
   return blocks;
 }
 
-cudaError_t launch_adam_step(const fno_adam_tensors* t, float lr, float beta1, float beta2, float eps, float weight_decay,
-                             long long step, cudaStream_t stream) {
-  AdamArgs a = {};
-  const int blocks = adam_blocks(t, a);
-  a.lr = lr;
-  a.beta1 = beta1;
-  a.beta2 = beta2;
-  a.eps = eps;
-  a.weight_decay = weight_decay;
-  adam_coefficients(lr, beta1, beta2, step, &a.step_size, &a.inv_bc2_sqrt);
-  if (blocks == 0) return cudaSuccess;
-  adam_step_kernel<false><<<blocks, kAdamThreads, 0, stream>>>(a);
-  return cudaGetLastError();
-}
-
-cudaError_t launch_adam_step_dev(const fno_adam_tensors* t, const float* coef, int n_coef, const int* cursor, float beta1,
-                                 float beta2, float eps, float weight_decay, cudaStream_t stream) {
-  AdamArgs a = {};
-  const int blocks = adam_blocks(t, a);
-  a.beta1 = beta1;
-  a.beta2 = beta2;
-  a.eps = eps;
-  a.weight_decay = weight_decay;
-  a.coef = reinterpret_cast<const float2*>(coef);
-  a.cursor = cursor;
-  a.n_coef = n_coef;
-  if (blocks == 0) return cudaSuccess;
-  adam_step_kernel<true><<<blocks, kAdamThreads, 0, stream>>>(a);
-  return cudaGetLastError();
-}
-
+// Without a clip coefficient or EMA tensors this launches adam_step_kernel, the plain update of fno_adam_step[_dev].
 template <bool kDevCoef>
 static cudaError_t launch_adam_ex(const AdamArgs& a, const AdamExt& x, int blocks, cudaStream_t stream) {
   if (blocks == 0) return cudaSuccess;

@@ -1,10 +1,10 @@
 """FusedAdam: torch.optim.Adam's update (reference src/train_auto.py:213: Adam(model.parameters(), lr), betas
 (0.9, 0.999), eps 1e-8, weight_decay 0, no amsgrad) for every parameter tensor of the model in ONE kernel launch
-(`fno_adam_step`).  Complex parameters are updated as pairs of reals, exactly as torch.optim.Adam treats them
+(`fno_adam_step_ex`).  Complex parameters are updated as pairs of reals, exactly as torch.optim.Adam treats them
 (torch.view_as_real).  State keys match torch's ("step", "exp_avg", "exp_avg_sq"), so `state_dict()` round-trips
 with the stock optimizer.  An opt-in: the reference script builds its own torch.optim.Adam, which keeps working.
 
-Two opt-in safeguards run inside that launch (`fno_adam_step_ex`):
+Two opt-in safeguards run inside that launch:
 - max_grad_norm: `torch.nn.utils.clip_grad_norm_(all parameters with a gradient, max_grad_norm)` before the update,
   one float64 norm launch (`fno_grad_norm`) over every param group; the pre-clip norm stays on the device as
   `last_grad_norm`.
@@ -89,9 +89,11 @@ class FusedAdam(torch.optim.Optimizer):
             b.copy_(st["ema"] if st and "ema" in st else a)
 
     @staticmethod
-    def _tables(ps, grads, extra=None):
-        """FnoAdamTensors tables of up to ADAM_MAX_TENSORS entries over (param, grad) pairs; extra(t, slot, p) fills
-        the rest of entry `slot`."""
+    def _tables(ps, grads, states=None, ema: bool = False) -> list:
+        """The FnoAdamTensors tables of one update over the parameters `ps` with gradients `grads`, in order, up to
+        ADAM_MAX_TENSORS entries each; complex tensors enter as pairs of reals.  With `states` (init_state's dicts) the
+        entries also point at the moments (the norm reads only grad and n).  Each table's `ema` is the array of its
+        entries' state["ema"] pointers when `ema`, else None."""
         out = []
         for i0 in range(0, len(ps), _lib.ADAM_MAX_TENSORS):
             t = _lib.FnoAdamTensors()
@@ -101,79 +103,37 @@ class FusedAdam(torch.optim.Optimizer):
                 t.param[j] = _real_view(p).data_ptr()
                 t.grad[j] = _real_view(g).data_ptr()
                 t.n[j] = p.numel() * (2 if p.is_complex() else 1)
-                if extra is not None:
-                    extra(t, j, p)
+                if states is not None:
+                    t.exp_avg[j] = _real_view(states[i0 + j]["exp_avg"]).data_ptr()
+                    t.exp_avg_sq[j] = _real_view(states[i0 + j]["exp_avg_sq"]).data_ptr()
+            t.ema = (C.c_void_p * t.count)(*[_real_view(st["ema"]).data_ptr() for st in states[i0:i0 + t.count]]) \
+                if ema else None
             out.append(t)
         return out
 
     @torch.no_grad()
     def step(self, closure=None):
+        """One Adam update of every parameter with a gradient.  Every group is validated and its step count advanced
+        before the first launch, so a refused input launches nothing.  Then, with max_grad_norm, one fno_grad_norm over
+        every group's gradients, and one fno_adam_step_ex per group and table (no clip coefficient and no EMA tensors
+        without the options: the plain update)."""
         loss = None
         if closure is not None:
             with torch.enable_grad():
                 loss = closure()
-        if self.max_grad_norm is not None or self.ema_decay is not None:
-            self._step_ex()
-            return loss
         lib = _lib.load()
+        one_device = self.max_grad_norm is not None or self.ema_decay is not None   # the norm spans every group
+        groups, dev = [], None
         for group in self.param_groups:
             ps = [p for p in group["params"] if p.grad is not None]
             if not ps:
                 continue
-            dev = ps[0].device
-            if dev.type != "cuda":
-                raise _lib.FnoNativeError("FusedAdam needs CUDA parameters (there is no CPU path)")
-            step = None
-            keep = []  # contiguous gradient copies must outlive the asynchronous launch
-            for i0 in range(0, len(ps), _lib.ADAM_MAX_TENSORS):
-                chunk = ps[i0:i0 + _lib.ADAM_MAX_TENSORS]
-                t = _lib.FnoAdamTensors()
-                t.count = len(chunk)
-                for i, p in enumerate(chunk):
-                    if p.dtype not in (torch.float32, torch.complex64) or not p.is_contiguous() or p.device != dev:
-                        raise _lib.FnoNativeError("FusedAdam: parameters must be contiguous float32/complex64 on one device")
-                    st = self.init_state(p)
-                    st["step"] += 1
-                    s = int(st["step"].item())
-                    if step is None:
-                        step = s
-                    elif s != step:
-                        raise _lib.FnoNativeError("FusedAdam: parameters of one group must share the step count")
-                    g = p.grad if p.grad.is_contiguous() else p.grad.contiguous()
-                    keep.append(g)
-                    t.param[i] = _real_view(p).data_ptr()
-                    t.grad[i] = _real_view(g).data_ptr()
-                    t.exp_avg[i] = _real_view(st["exp_avg"]).data_ptr()
-                    t.exp_avg_sq[i] = _real_view(st["exp_avg_sq"]).data_ptr()
-                    t.n[i] = p.numel() * (2 if p.is_complex() else 1)
-                with torch.cuda.device(dev):
-                    stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-                    b1, b2 = group["betas"]
-                    _lib.check(lib.fno_adam_step(C.byref(t), group["lr"], b1, b2, group["eps"], group["weight_decay"],
-                                                 step, stream), "fno_adam_step")
-            for g in keep:
-                g.record_stream(torch.cuda.current_stream(dev))
-            # the kernel wrote through raw pointers: tell autograd (and Fno2d's packed-weight cache, which is keyed on
-            # the parameters' version counters) that the tensors changed
+            if dev is None or not one_device:
+                dev = ps[0].device
+                if dev.type != "cuda":
+                    raise _lib.FnoNativeError("FusedAdam needs CUDA parameters (there is no CPU path)")
+            step, states = None, []
             for p in ps:
-                torch.autograd.graph.increment_version(p)
-        return loss
-
-    def _step_ex(self) -> None:
-        """step() with max_grad_norm and / or ema_decay: one norm launch over every group's gradients (clipping), then one
-        fno_adam_step_ex launch per group and table."""
-        lib = _lib.load()
-        groups, dev = [], None
-        for group in self.param_groups:   # validate, advance the step counts and collect the gradients
-            ps = [p for p in group["params"] if p.grad is not None]
-            if not ps:
-                continue
-            step = None
-            for p in ps:
-                if dev is None:
-                    dev = p.device
-                    if dev.type != "cuda":
-                        raise _lib.FnoNativeError("FusedAdam needs CUDA parameters (there is no CPU path)")
                 if p.dtype not in (torch.float32, torch.complex64) or not p.is_contiguous() or p.device != dev:
                     raise _lib.FnoNativeError("FusedAdam: parameters must be contiguous float32/complex64 on one device")
                 st = self.init_state(p)
@@ -183,42 +143,38 @@ class FusedAdam(torch.optim.Optimizer):
                     step = s
                 elif s != step:
                     raise _lib.FnoNativeError("FusedAdam: parameters of one group must share the step count")
+                states.append(st)
+            # contiguous gradient copies must outlive the asynchronous launches
             grads = [p.grad if p.grad.is_contiguous() else p.grad.contiguous() for p in ps]
-            groups.append((group, ps, grads, step))
+            groups.append((group, dev, ps, grads, step, self._tables(ps, grads, states, self.ema_decay is not None)))
         if not groups:
-            return
-        with torch.cuda.device(dev):
-            cur = torch.cuda.current_stream(dev)
-            stream = C.c_void_p(cur.cuda_stream)
-            clip = None
-            if self.max_grad_norm is not None:
-                tables = [t for _, ps, grads, _ in groups for t in self._tables(ps, grads)]
-                if len(tables) > _lib.GRAD_NORM_MAX_TABLES:
-                    raise _lib.FnoNativeError(f"FusedAdam(max_grad_norm=...): at most "
-                                              f"{_lib.GRAD_NORM_MAX_TABLES * _lib.ADAM_MAX_TENSORS} parameter tensors")
-                arr = (_lib.FnoAdamTensors * len(tables))(*tables)
+            return loss
+        clip = None
+        if self.max_grad_norm is not None:
+            tables = [t for *_, tabs in groups for t in tabs]
+            if len(tables) > _lib.GRAD_NORM_MAX_TABLES:
+                raise _lib.FnoNativeError(f"FusedAdam(max_grad_norm=...): at most "
+                                          f"{_lib.GRAD_NORM_MAX_TABLES * _lib.ADAM_MAX_TENSORS} parameter tensors")
+            with torch.cuda.device(dev):
                 out = torch.empty(2, dtype=torch.float32, device=dev)   # norm, coefficient
-                _lib.check(lib.fno_grad_norm(arr, len(tables), self.max_grad_norm, out.data_ptr(),
-                                             self.norm_scratch(dev).data_ptr(), None, 0, None, stream), "fno_grad_norm")
-                self.last_grad_norm = out[0]
-                clip = out[1:].data_ptr()
-            ema = self.ema_decay is not None
-            for group, ps, grads, step in groups:
-                def fill(t, j, p):
-                    st = self.state[p]
-                    t.exp_avg[j] = _real_view(st["exp_avg"]).data_ptr()
-                    t.exp_avg_sq[j] = _real_view(st["exp_avg_sq"]).data_ptr()
-                b1, b2 = group["betas"]
-                for i0, t in zip(range(0, len(ps), _lib.ADAM_MAX_TENSORS), self._tables(ps, grads, fill)):
-                    ema_ptrs = None
-                    if ema:
-                        ema_ptrs = (C.c_void_p * t.count)(*[_real_view(self.state[p]["ema"]).data_ptr()
-                                                            for p in ps[i0:i0 + t.count]])
+                _lib.check(lib.fno_grad_norm((_lib.FnoAdamTensors * len(tables))(*tables), len(tables), self.max_grad_norm,
+                                             out.data_ptr(), self.norm_scratch(dev).data_ptr(), None, 0, None,
+                                             C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), "fno_grad_norm")
+            self.last_grad_norm = out[0]
+            clip = out[1:].data_ptr()
+        ema_decay = 0.0 if self.ema_decay is None else self.ema_decay
+        for group, dev, ps, grads, step, tabs in groups:
+            b1, b2 = group["betas"]
+            with torch.cuda.device(dev):
+                cur = torch.cuda.current_stream(dev)
+                for t in tabs:
                     _lib.check(lib.fno_adam_step_ex(C.byref(t), group["lr"], b1, b2, group["eps"], group["weight_decay"],
-                                                    step, clip, ema_ptrs, self.ema_decay if ema else 0.0, stream),
+                                                    step, clip, t.ema, ema_decay, C.c_void_p(cur.cuda_stream)),
                                "fno_adam_step_ex")
-            for _, ps, grads, _ in groups:
                 for g in grads:
                     g.record_stream(cur)
-                for p in ps:
-                    torch.autograd.graph.increment_version(p)
+            # the kernel wrote through raw pointers: tell autograd (and Fno2d's packed-weight cache, which is keyed on
+            # the parameters' version counters) that the tensors changed
+            for p in ps:
+                torch.autograd.graph.increment_version(p)
+        return loss

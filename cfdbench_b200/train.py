@@ -35,6 +35,7 @@ import torch
 from . import _lib, resume
 from .data import DeviceFrames, _check_chain, _gather, case_table, check_noise_args, index_batches, rollout_windows
 from .fno2d import capture_graph, side_stream
+from .optim import FusedAdam
 
 LOG_COLUMNS = ("mse", "rmse", "mae", "nmse", "mean_l2")   # one row of the epoch log: fno_loss_fwd's five scalars
 
@@ -73,10 +74,6 @@ def dump_json(data, path) -> None:   # reference src/utils/common.py:23-25
 
 
 # ------------------------------------------------------------------------------------------------ the step graphs
-def _real(t: torch.Tensor) -> torch.Tensor:   # complex parameters are updated as pairs of reals, as FusedAdam does
-    return torch.view_as_real(t) if t.is_complex() else t
-
-
 class _StepGraphs:
     """The captured training step of a full batch of `batch_size` samples and, when n % batch_size != 0, of the ragged
     last batch.  Both graphs run on one set of static buffers sized for min(batch_size, n) samples: the ragged graph
@@ -129,31 +126,15 @@ class _StepGraphs:
         self.coef_host = torch.empty(self.steps, 2, dtype=torch.float32, pin_memory=True)
 
         # Adam over the parameters that require grad (the ones autograd gives a .grad, so the ones FusedAdam.step
-        # updates), chunked as FusedAdam.step chunks them; the state is created as FusedAdam creates it.  The backward
-        # writes every parameter's gradient into the flat buffer; a frozen parameter's is not read.
+        # updates), in FusedAdam.step's tables; the state is created as FusedAdam creates it.  The backward writes every
+        # parameter's gradient into the flat buffer; a frozen parameter's is not read.
         group = optimizer.param_groups[0]
         layout = [ent for ent in model._grad_layout()[0] if ent[1].requires_grad]
         self.params = [prm for _, prm, _, _ in layout]
-        states = [optimizer.init_state(prm) for prm in self.params]
-        self.adam = []
-        for i0 in range(0, len(self.params), _lib.ADAM_MAX_TENSORS):
-            t = _lib.FnoAdamTensors()
-            t.count = min(_lib.ADAM_MAX_TENSORS, len(self.params) - i0)
-            for i in range(t.count):
-                prm, st, (_, _, off, numel) = self.params[i0 + i], states[i0 + i], layout[i0 + i]
-                t.param[i] = _real(prm).data_ptr()
-                t.grad[i] = self.flat[off:off + numel].data_ptr()
-                t.exp_avg[i] = _real(st["exp_avg"]).data_ptr()
-                t.exp_avg_sq[i] = _real(st["exp_avg_sq"]).data_ptr()
-                t.n[i] = numel
-            self.adam.append(t)
-        self.states = states
+        self.states = [optimizer.init_state(prm) for prm in self.params]
+        self.adam = FusedAdam._tables(self.params, [self.flat[off:off + numel] for _, _, off, numel in layout],
+                                      self.states, self.ema_decay is not None)
         self.adam_arr = (_lib.FnoAdamTensors * len(self.adam))(*self.adam)   # the norm launch's tables
-        self.ema_ptrs = [None] * len(self.adam)
-        if self.ema_decay is not None:
-            self.ema_ptrs = [(C.c_void_p * t.count)(*[_real(st["ema"]).data_ptr()
-                                                      for st in states[i0:i0 + t.count]])
-                             for i0, t in zip(range(0, len(states), _lib.ADAM_MAX_TENSORS), self.adam)]
         self.betas, self.eps, self.weight_decay = group["betas"], group["eps"], group["weight_decay"]
 
         # capture: a warm-up of every launch except Adam and the log (it updates nothing: parameters, optimizer state
@@ -236,22 +217,17 @@ class _StepGraphs:
         """Adam on the flat gradients, then the step's five loss scalars (at device address loss_row) into the log."""
         lib, io = self.lib, self.io
         b1, b2 = self.betas
-        if self.max_grad_norm is None and self.ema_decay is None:
-            for t in self.adam:
-                _lib.check(lib.fno_adam_step_dev(C.byref(t), io["coef"].data_ptr(), self.steps, io["cursor"].data_ptr(),
-                                                 b1, b2, self.eps, self.weight_decay, st), "fno_adam_step_dev")
-        else:   # the global norm into its log row, then Adam with the clip and / or the EMA
-            clip = None
-            if self.max_grad_norm is not None:
-                _lib.check(lib.fno_grad_norm(self.adam_arr, len(self.adam), self.max_grad_norm, io["norm"].data_ptr(),
-                                             io["norm_scratch"].data_ptr(), io["norm_log"].data_ptr(), self.steps,
-                                             io["cursor"].data_ptr(), st), "fno_grad_norm")
-                clip = io["norm"][1:].data_ptr()
-            ema_d = io["ema_d"].data_ptr() if self.ema_decay is not None else None
-            for t, ema in zip(self.adam, self.ema_ptrs):
-                _lib.check(lib.fno_adam_step_dev_ex(C.byref(t), io["coef"].data_ptr(), self.steps, io["cursor"].data_ptr(),
-                                                    b1, b2, self.eps, self.weight_decay, clip, ema, ema_d, st),
-                           "fno_adam_step_dev_ex")
+        clip = None
+        if self.max_grad_norm is not None:   # the global norm into its log row
+            _lib.check(lib.fno_grad_norm(self.adam_arr, len(self.adam), self.max_grad_norm, io["norm"].data_ptr(),
+                                         io["norm_scratch"].data_ptr(), io["norm_log"].data_ptr(), self.steps,
+                                         io["cursor"].data_ptr(), st), "fno_grad_norm")
+            clip = io["norm"][1:].data_ptr()
+        ema_d = io["ema_d"].data_ptr() if self.ema_decay is not None else None
+        for t in self.adam:
+            _lib.check(lib.fno_adam_step_dev_ex(C.byref(t), io["coef"].data_ptr(), self.steps, io["cursor"].data_ptr(),
+                                                b1, b2, self.eps, self.weight_decay, clip, t.ema, ema_d, st),
+                       "fno_adam_step_dev_ex")
         _lib.check(lib.fno_train_log_step(loss_row, io["log"].data_ptr(), self.steps, io["cursor"].data_ptr(), st),
                    "fno_train_log_step")
 

@@ -221,6 +221,77 @@ def test_non_binding_clip_is_bit_identical_to_no_clip():
             assert torch.equal(oa.state[a][k], ob.state[b][k])
 
 
+def _seeded_adam_inputs(seed):
+    """_params(seed) with seeded gradients, exp_avg and exp_avg_sq (>= 0), and an independent copy of all of them."""
+    g = torch.Generator().manual_seed(seed)
+    ps, states = _params(seed), []
+    for p in ps:
+        def draw(scale, square=False):
+            x = torch.randn(_real(p).shape, generator=g) * scale
+            x = x * x if square else x
+            return (torch.view_as_complex(x) if p.is_complex() else x).cuda()
+        p.grad = draw(1.0)
+        states.append(dict(exp_avg=draw(0.1), exp_avg_sq=draw(0.1, square=True)))
+    qs = [torch.nn.Parameter(p.detach().clone()) for p in ps]
+    for q, p in zip(qs, ps):
+        q.grad = p.grad.clone()
+    return (ps, states), (qs, [{k: v.clone() for k, v in st.items()} for st in states])
+
+
+def _assert_same_bits(a, b):
+    (pa, sa), (pb, sb) = a, b
+    bits = lambda t: _real(t.detach()).contiguous().view(torch.int32)
+    for x, y, u, v in zip(pa, pb, sa, sb):
+        assert torch.equal(bits(x), bits(y))
+        for k in ("exp_avg", "exp_avg_sq"):
+            assert torch.equal(bits(u[k]), bits(v[k])), k
+
+
+def test_plain_adam_entry_points_match_their_ex_forms():
+    """fno_adam_step is fno_adam_step_ex(..., NULL, NULL, 0.0) and fno_adam_step_dev is fno_adam_step_dev_ex(..., NULL,
+    NULL, NULL), bit for bit; FusedAdam.step (which issues the _ex form) is direct fno_adam_step calls."""
+    lib = _lib.load()
+    st = C.c_void_p(torch.cuda.current_stream().cuda_stream)
+    lr, b1, b2, eps, wd = 1e-3, 0.9, 0.999, 1e-8, 0.01
+
+    def tables(ps, states):
+        return FusedAdam._tables(ps, [p.grad for p in ps], states)
+
+    a, b = _seeded_adam_inputs(21)
+    before = a[0][0].detach().clone()
+    for step in (1, 2, 9):
+        for t, u in zip(tables(*a), tables(*b)):
+            assert lib.fno_adam_step(C.byref(t), lr, b1, b2, eps, wd, step, st) == 0
+            assert lib.fno_adam_step_ex(C.byref(u), lr, b1, b2, eps, wd, step, None, None, 0.0, st) == 0
+    _assert_same_bits(a, b)
+    assert not torch.equal(a[0][0], before)
+
+    a, b = _seeded_adam_inputs(22)
+    n = 3
+    coef = np.empty((n, 2), np.float32)
+    assert lib.fno_adam_coefficients(lr, b1, b2, 4, n, coef.ctypes.data) == 0
+    coef = torch.from_numpy(coef).cuda()
+    cursor = torch.zeros(1, dtype=torch.int32, device="cuda")
+    for c in range(n + 1):   # the last cursor is outside the table: both write nothing
+        cursor.fill_(c)
+        for t, u in zip(tables(*a), tables(*b)):
+            assert lib.fno_adam_step_dev(C.byref(t), coef.data_ptr(), n, cursor.data_ptr(), b1, b2, eps, wd, st) == 0
+            assert lib.fno_adam_step_dev_ex(C.byref(u), coef.data_ptr(), n, cursor.data_ptr(), b1, b2, eps, wd, None, None,
+                                            None, st) == 0
+    _assert_same_bits(a, b)
+
+    a, b = _seeded_adam_inputs(23)
+    opt = FusedAdam(a[0], lr=lr, betas=(b1, b2), eps=eps, weight_decay=wd)
+    for p, s in zip(*a):
+        opt.state[p].update(step=torch.tensor(6.0), **s)
+    for step in (7, 8):
+        opt.step()
+        for t in tables(*b):
+            assert lib.fno_adam_step(C.byref(t), lr, b1, b2, eps, wd, step, st) == 0
+    _assert_same_bits(a, b)
+    assert all(float(opt.state[p]["step"]) == 8 for p in a[0])
+
+
 # ------------------------------------------------------------------------------------------------ 3. EMA
 @pytest.mark.parametrize("decay,steps", [(0.9, 40), (0.999, 25)])
 def test_ema_against_a_float64_recurrence(decay, steps):

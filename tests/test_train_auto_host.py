@@ -69,6 +69,12 @@ def test_new_entry_points_reject_bad_arguments(lib):
     bad.grad[0] = None
     assert adam(tab=bad) == 1
 
+    def adam_host(tab=t, step=1):   # the host-coefficient form
+        return lib.fno_adam_step(C.byref(tab) if tab is not None else None, 1e-3, 0.9, 0.999, 1e-8, 0.0, step, st)
+    for kw in (dict(tab=None), dict(step=0), dict(tab=bad)):
+        assert adam_host(**kw) == 1, kw
+        assert lib.fno_last_error().startswith(b"fno_adam_step:")
+
     out = (C.c_float * 8)()
     assert lib.fno_adam_coefficients(1e-3, 0.9, 0.999, 0, 4, out) == 1
     assert lib.fno_adam_coefficients(1e-3, 0.9, 0.999, 1, 0, out) == 1
