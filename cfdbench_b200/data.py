@@ -16,7 +16,7 @@ datasets hold (N, 3, 66, 65) frames, reference src/dataset/tube.py:228-281, dam.
 from __future__ import annotations
 
 import ctypes as C
-from typing import Dict, Iterable, Iterator, List, NamedTuple, Optional, Sequence
+from typing import Dict, Iterable, Iterator, List, NamedTuple, Optional, Sequence, Tuple
 
 import numpy as np
 import torch
@@ -31,6 +31,20 @@ def case_table(case_params: Sequence[dict]) -> np.ndarray:
     return np.asarray([[cp[k] for k in keys] for cp in case_params], dtype=np.float32).reshape(len(case_params), len(keys))
 
 
+def _positive_int(name: str, v) -> int:
+    """`v` as an int; ValueError unless it is a positive int (a bool is not)."""
+    if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or v < 1:
+        raise ValueError(f"{name} must be a positive int, got {v!r}")
+    return int(v)
+
+
+def _check_grid(gh: int, gw: int) -> None:
+    """ValueError for a grid outside the grid-generic kernels' range (64x64 lies inside it)."""
+    from . import _lib
+    if not (_lib.GRID_MIN <= gh <= _lib.GRID_MAX and _lib.GRID_MIN <= gw <= _lib.GRID_MAX):
+        raise ValueError(f"grid {gh}x{gw} is outside the supported range {_lib.GRID_MIN}..{_lib.GRID_MAX} in H and W")
+
+
 class DeviceFrames:
     def __init__(self, dataset, device="cuda", frame_dtype: torch.dtype = torch.float32):
         if frame_dtype not in (torch.float32, torch.bfloat16):
@@ -38,26 +52,17 @@ class DeviceFrames:
         dev = torch.device(device)
         if dev.type != "cuda":
             raise ValueError("DeviceFrames keeps the split in GPU memory: pass a CUDA device")
-        ins, labs = dataset.inputs, dataset.labels
-        if ins.dim() != 4 or ins.shape[1] != 3 or labs.shape != ins.shape:
-            raise ValueError(f"expected (N, 3, H, W) input / label frames, got {tuple(ins.shape)} / {tuple(labs.shape)}")
-        self.height, self.width = int(ins.shape[2]), int(ins.shape[3])
-        from . import _lib
-        if not (_lib.GRID_MIN <= self.height <= _lib.GRID_MAX and _lib.GRID_MIN <= self.width <= _lib.GRID_MAX):
-            raise ValueError(f"frames are {self.height}x{self.width}: H and W must lie in {_lib.GRID_MIN}..{_lib.GRID_MAX}")
+        split = describe_split(dataset, "dataset")
+        _check_grid(split.height, split.width)
+        self.n, self.height, self.width, self.n_case_params = split.n, split.height, split.width, split.n_case_params
         self.device, self.frame_dtype = dev, frame_dtype
-        self.n = ins.shape[0]
-        self.frames_in = ins.to(device=dev, dtype=frame_dtype).contiguous()
-        self.frames_out = labs.to(device=dev, dtype=frame_dtype).contiguous()
-        table = case_table(dataset.case_params)
-        self.n_case_params = table.shape[1]
-        self.case_table = torch.from_numpy(table).to(dev)
-        self.case_ids = torch.as_tensor(np.asarray(dataset.case_ids), dtype=torch.int32, device=dev)
-        if self.case_ids.numel() != self.n:
-            raise ValueError("dataset.case_ids must have one entry per sample")
-        self._case_ids_host = np.asarray(dataset.case_ids).reshape(-1)   # for the window checks, without a device read
+        self.frames_in = dataset.inputs.to(device=dev, dtype=frame_dtype).contiguous()
+        self.frames_out = dataset.labels.to(device=dev, dtype=frame_dtype).contiguous()
+        self.case_table = torch.from_numpy(case_table(dataset.case_params)).to(dev)
+        self.case_ids = torch.as_tensor(split.case_ids, dtype=torch.int32, device=dev)
+        self._case_ids_host = split.case_ids   # for the window checks, without a device read
         # the dataset's label offset (labels = frames[s:], inputs = frames[:-s] per case), None when it has none
-        self.time_step_size = getattr(dataset, "time_step_size", None)
+        self.time_step_size = split.time_step_size
 
     def __len__(self) -> int:
         return self.n
@@ -117,17 +122,15 @@ class DeviceFrames:
         noise_std = check_noise_args(noise_std, noise_seed, noise_step)
         _lib.load()   # a missing library raises before any device work
         s = self.time_step_size if time_step_size is None else time_step_size
-        if isinstance(steps, bool) or not isinstance(steps, (int, np.integer)) or steps < 1:
-            raise ValueError(f"steps must be a positive int, got {steps!r}")
+        steps = _positive_int("steps", steps)
         if s is None:
             raise ValueError("time_step_size is needed: the dataset has none, pass it")
-        if isinstance(s, bool) or not isinstance(s, (int, np.integer)) or s < 1:
-            raise ValueError(f"time_step_size must be a positive int, got {s!r}")
+        s = _positive_int("time_step_size", s)
         idx = torch.as_tensor(idx, dtype=torch.int64)
         if idx.dim() != 1 or idx.numel() == 0:
             raise ValueError("idx must be a non-empty 1-D index list")
         starts = idx.cpu().numpy()
-        ends = starts + (int(steps) - 1) * int(s)
+        ends = starts + (steps - 1) * s
         if int(starts.min()) < 0 or int(ends.max()) >= self.n:
             raise IndexError("sample index out of range, or a window runs past the split")
         cross = np.flatnonzero(self._case_ids_host[starts] != self._case_ids_host[ends])
@@ -137,11 +140,11 @@ class DeviceFrames:
         b, p, dev, gh, gw = idx.numel(), self.n_case_params, self.device, self.height, self.width
         out = dict(inputs=torch.empty(b, 2, gh, gw, device=dev), label=torch.empty(b, 2, gh, gw, device=dev),
                    mask=torch.empty(b, 1, gh, gw, device=dev), case_params=torch.empty(b, p, device=dev),
-                   labels=torch.empty(int(steps), b, 2, gh, gw, device=dev))
+                   labels=torch.empty(steps, b, 2, gh, gw, device=dev))
         with torch.cuda.device(dev):
             st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
             _gather(self, idx, b, out["inputs"], out["label"], out["mask"], out["case_params"], st,
-                    window=(int(steps), int(s), out["labels"]))
+                    window=(steps, s, out["labels"]))
             if noise_std > 0:
                 self._add_noise(out, idx, noise_std, noise_seed, noise_step, st)
         idx.record_stream(torch.cuda.current_stream(dev))
@@ -180,6 +183,65 @@ def _gather(frames: DeviceFrames, idx: Tensor, b: int, inputs: Tensor, label: Op
     else:
         name = "fno_grid_" + name
         _lib.check(getattr(lib, name)(*args, gh, gw, st), name)
+
+
+class SplitInfo(NamedTuple):
+    """What `describe_split` reads of a split."""
+    n: int
+    height: int
+    width: int
+    n_case_params: int
+    frame_dtype: torch.dtype         # the frames' storage: float32 for a dataset object, which is uploaded so
+    case_ids: np.ndarray             # (n,), on the host
+    time_step_size: Optional[int]    # the split's label offset, None when it has none
+    device: Optional[torch.device]   # the frames' device (with its index), None for a dataset object
+
+
+def describe_split(data, what: str, nonempty: bool = False) -> SplitInfo:
+    """The facts of a split: a DeviceFrames, or the reference's dataset object (`.inputs` / `.labels` (N, 3, H, W)
+    tensors, `.case_ids`, `.case_params`, optionally `.time_step_size`).  No device work.  Raises ValueError, naming the
+    split `what`, for a dataset whose frames are malformed or whose case_ids do not have one entry per sample, and with
+    nonempty=True for a split without samples."""
+    if isinstance(data, DeviceFrames):
+        n = data.n
+    else:
+        ins, labs = getattr(data, "inputs", None), getattr(data, "labels", None)
+        if not isinstance(ins, Tensor) or not isinstance(labs, Tensor) or ins.dim() != 4 or ins.shape[1] != 3 \
+                or labs.shape != ins.shape:
+            raise ValueError(f"{what} must be a dataset with (N, 3, H, W) .inputs / .labels tensors, got "
+                             f"{getattr(ins, 'shape', None)} / {getattr(labs, 'shape', None)}")
+        n = int(ins.shape[0])
+    if nonempty and n == 0:   # before the case table: an empty dataset may have no case parameters
+        raise ValueError(f"{what} is empty")
+    tss = getattr(data, "time_step_size", None)
+    if isinstance(data, DeviceFrames):
+        frames_in = getattr(data, "frames_in", None)   # None on a DeviceFrames made without __init__
+        return SplitInfo(n, data.height, data.width, data.n_case_params, data.frame_dtype, data._case_ids_host, tss,
+                         None if frames_in is None else frames_in.device)
+    ids = np.asarray(data.case_ids).reshape(-1)
+    if ids.size != n:
+        raise ValueError(f"{what} must have one case_ids entry per sample")
+    return SplitInfo(n, int(ins.shape[2]), int(ins.shape[3]), case_table(data.case_params).shape[1], torch.float32, ids,
+                     tss, None)
+
+
+def _check_split(model, data, what: str) -> SplitInfo:
+    """`describe_split(data, what, nonempty=True)`, refusing also a split the drop-in Fno2d `model` cannot train or
+    evaluate on: frames on another device than the model, a case-parameter count other than the model's, or a grid /
+    storage mode the model rejects.  No device work."""
+    split = describe_split(data, what, nonempty=True)
+    if split.device is not None and split.device != model.device:
+        raise ValueError(f"{what}: the frames are on {split.device}, the model on {model.device}")
+    if split.n_case_params != model.n_case_params:
+        raise ValueError(f"{what} has {split.n_case_params} case parameters per sample, the model takes n_case_params="
+                         f"{model.n_case_params}")
+    model._route(split.height, split.width)   # the model's own grid / storage-mode checks
+    return split
+
+
+def as_device_frames(data, device) -> DeviceFrames:
+    """`data` if it is a DeviceFrames, else a DeviceFrames of it on `device` (float32 frames)."""
+    return data if isinstance(data, DeviceFrames) else DeviceFrames(data, device=device)
 
 
 def check_noise_args(noise_std, noise_seed, noise_step=0, std_name: str = "noise_std") -> float:
@@ -307,15 +369,26 @@ def rollout_windows(case_ids, steps: int, time_step_size: int) -> np.ndarray:
     (s = time_step_size, src/dataset/cavity.py:271,295-331), so the k-th target of the window that starts at sample j is
     labels[j + k s].  A start j is valid when j + (steps - 1) s < N and case_ids[j + (steps - 1) s] == case_ids[j]: no
     window crosses a case.  steps = 1 gives arange(N)."""
-    for name, v in (("steps", steps), ("time_step_size", time_step_size)):
-        if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or v < 1:
-            raise ValueError(f"{name} must be a positive int, got {v!r}")
+    steps, time_step_size = _positive_int("steps", steps), _positive_int("time_step_size", time_step_size)
+    span = (steps - 1) * time_step_size
     cid = np.asarray(case_ids).reshape(-1)
-    span = (int(steps) - 1) * int(time_step_size)
     if cid.size <= span:
         return np.zeros(0, dtype=np.int64)
     j = np.arange(cid.size - span, dtype=np.int64)
     return j[cid[j + span] == cid[j]]
+
+
+def split_windows(split: SplitInfo, steps: int, time_step_size, what: str, steps_name: str) -> Tuple[np.ndarray, int]:
+    """(windows, s): the `rollout_windows` of `split` for `steps`-step rollouts and their time step size s, the
+    `time_step_size` argument unless it is None, else the split's.  ValueError, naming the split `what` and the steps
+    argument `steps_name`, for no time step size at all, one that is not a positive int, or no single window."""
+    s = split.time_step_size if time_step_size is None else time_step_size
+    if s is None:
+        raise ValueError(f"{steps_name}={steps} needs a time_step_size: {what} has none, pass it")
+    windows = rollout_windows(split.case_ids, steps, s)
+    if windows.size == 0:
+        raise ValueError(f"{what} has no {steps}-step window with time_step_size={s} inside one case")
+    return windows, int(s)
 
 
 def _check_chain(frames: DeviceFrames, starts: np.ndarray, steps: int, time_step_size: int,

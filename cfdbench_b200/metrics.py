@@ -32,13 +32,10 @@ import torch
 from torch import Tensor
 
 from . import _lib
+from .data import (_check_chain, _check_grid, _check_split, _positive_int, as_device_frames, describe_split,
+                   split_windows)
 
 HW = 64 * 64
-
-
-def _check_grid(gh: int, gw: int) -> None:
-    if not (_lib.GRID_MIN <= gh <= _lib.GRID_MAX and _lib.GRID_MIN <= gw <= _lib.GRID_MAX):
-        raise ValueError(f"grid {gh}x{gw} is outside the supported range {_lib.GRID_MIN}..{_lib.GRID_MAX} in H and W")
 
 
 def _launch_metrics(preds: Tensor, label_u: Tensor, mask: Tensor, sums: Tensor) -> None:
@@ -54,6 +51,14 @@ def _launch_metrics(preds: Tensor, label_u: Tensor, mask: Tensor, sums: Tensor) 
         else:
             _lib.check(lib.fno_grid_multistep_metrics(preds.data_ptr(), label_u.data_ptr(), mask.data_ptr(),
                                                       sums.data_ptr(), s, b, gh, gw, st), "fno_grid_multistep_metrics")
+
+
+def _chunked_sums(host: np.ndarray, steps: int, n: int, max_batch: int) -> np.ndarray:
+    """The (S, n, 3) sums of n items from the flat host copy of a device buffer that chunk [lo, hi) of at most
+    max_batch items filled with its (S, hi - lo, 3) block at offset S*lo*3."""
+    blocks = [host[steps * lo * 3:steps * min(n, lo + max_batch) * 3].reshape(steps, -1, 3)
+              for lo in range(0, n, max_batch)]
+    return np.concatenate(blocks, axis=1)
 
 
 def _per_case(host: np.ndarray, hw: int) -> Dict[str, np.ndarray]:
@@ -136,11 +141,7 @@ def infer_multistep(model, all_features: Sequence[Union[Tensor, np.ndarray]], al
             mask = fr[:, :, 2].transpose(0, 1).contiguous()
             _launch_metrics(preds, label_u, mask, sums[s * lo * 3:s * hi * 3])
     host = sums.double().cpu().numpy()   # the only synchronisation
-    blocks = []
-    for lo in range(0, n, max_batch):
-        hi = min(n, lo + max_batch)
-        blocks.append(host[s * lo * 3:s * hi * 3].reshape(s, hi - lo, 3))
-    per_case = _per_case(np.concatenate(blocks, axis=1), gh * gw)   # (S, n) each
+    per_case = _per_case(_chunked_sums(host, s, n, max_batch), gh * gw)   # (S, n) each
     return [{k: float(np.mean(v[i])) for k, v in per_case.items()} for i in range(s)]
 
 
@@ -207,39 +208,27 @@ def evaluate_auto(model, data, batch_size: int = 2, max_batch: int = 256) -> dic
     asynchronous copy of the predictions into a pinned host tensor; the split synchronises once, at the end.  Device
     memory beyond the frames and the (N, 6) sums is one chunk's worth.  Samples are computed independently, so the
     result does not depend on `max_batch`."""
-    from .data import DeviceFrames
     if batch_size < 1 or max_batch < 1:
         raise ValueError(f"batch_size and max_batch must be positive, got {batch_size} and {max_batch}")
     names = list(model.loss_fn.get_score_names())
     unknown = [k for k in names if k not in EVAL_SCORES]
     if unknown:
         raise ValueError(f"score names {unknown} are not among {EVAL_SCORES}")
-    if isinstance(data, DeviceFrames):
-        n, gh, gw = data.n, data.height, data.width
-    else:
-        ins, labs = getattr(data, "inputs", None), getattr(data, "labels", None)
-        if not isinstance(ins, Tensor) or not isinstance(labs, Tensor) or ins.dim() != 4 or ins.shape[1] != 3 \
-                or labs.shape != ins.shape:
-            raise ValueError("data must be a DeviceFrames or a dataset with (N, 3, H, W) .inputs / .labels tensors, got "
-                             f"{getattr(ins, 'shape', None)} / {getattr(labs, 'shape', None)}")
-        n, gh, gw = int(ins.shape[0]), int(ins.shape[2]), int(ins.shape[3])
-        if n > 0 and len(np.asarray(data.case_ids)) != n:
-            raise ValueError("dataset.case_ids must have one entry per sample")
-    if n == 0:
-        raise ValueError("the split is empty")
+    split = describe_split(data, "the split", nonempty=True)
+    n, gh, gw = split.n, split.height, split.width
     _check_grid(gh, gw)
     dev = next(model.parameters()).device
     if dev.type != "cuda":
         raise _lib.FnoNativeError("evaluate_auto has no CPU path: the model must be on a CUDA device")
-    if isinstance(data, DeviceFrames) and data.frames_in.device != dev:   # a tensor's device carries its index
-        raise ValueError(f"the frames are on {data.frames_in.device}, the model on {dev}")
+    if split.device is not None and split.device != dev:
+        raise ValueError(f"the split: the frames are on {split.device}, the model on {dev}")
     route = getattr(model, "_route", None)
     if route is not None:   # the drop-in Fno2d's own grid / storage-mode check, before any device work
         route(gh, gw)
     model.eval()
     preds_host = torch.empty(n, 2, gh, gw, dtype=torch.float32, pin_memory=True)   # a normal tensor, as torch.cat gives
     with torch.inference_mode(), torch.cuda.device(dev):
-        frames = data if isinstance(data, DeviceFrames) else DeviceFrames(data, device=dev)
+        frames = as_device_frames(data, dev)
         sums = torch.empty(n, 6, dtype=torch.float32, device=dev)
         for lo in range(0, n, max_batch):
             hi = min(n, lo + max_batch)
@@ -319,28 +308,18 @@ def evaluate_rollout_auto(model, data, steps: int, time_step_size=None, max_batc
     all, an empty or malformed split, a case-parameter count other than the model's, a grid or storage mode the model
     rejects, or a split without a single S-step window; FnoNativeError for a CPU model.  A split that does not chain
     raises ValueError naming the first bad sample."""
-    from .data import DeviceFrames, _check_chain, rollout_windows
     from .fno2d import Fno2d
-    from .train import _check_split, _positive_int
-    for name, v in (("steps", steps), ("time_step_size", time_step_size), ("max_batch", max_batch)):
-        if v is not None or name != "time_step_size":
-            _positive_int(name, v)
-    steps, max_batch = int(steps), int(max_batch)
+    steps = _positive_int("steps", steps)
+    if time_step_size is not None:
+        _positive_int("time_step_size", time_step_size)
+    max_batch = _positive_int("max_batch", max_batch)
     if not isinstance(model, Fno2d):
         raise TypeError(f"evaluate_rollout_auto runs the drop-in cfdbench_b200.Fno2d, got {type(model).__name__}")
-    _check_split(model, data, "the split")
-    tss = getattr(data, "time_step_size", None) if time_step_size is None else time_step_size
-    if tss is None:
-        raise ValueError("evaluate_rollout_auto needs a time_step_size: the split has none, pass it")
-    _positive_int("time_step_size", tss)
-    tss = int(tss)
-    case_ids = data._case_ids_host if isinstance(data, DeviceFrames) else data.case_ids
-    windows = rollout_windows(case_ids, steps, tss)
-    if windows.size == 0:
-        raise ValueError(f"the split has no {steps}-step window with time_step_size={tss} inside one case")
+    split = _check_split(model, data, "the split")
+    windows, tss = split_windows(split, steps, time_step_size, "the split", "steps")
     model._require_cuda()
     with torch.inference_mode(), torch.cuda.device(model.device):
-        frames = data if isinstance(data, DeviceFrames) else DeviceFrames(data, device=model.device)
+        frames = as_device_frames(data, model.device)
         _check_chain(frames, windows, steps, tss, what="the split")
     return _evaluate_rollout(model, frames, windows, steps, tss, max_batch)
 
@@ -370,7 +349,4 @@ def _window_sums(model, frames, windows: np.ndarray, steps: int, time_step_size:
         _launch_window_metrics(frames, preds, starts.to(dev, non_blocking=True), time_step_size,
                                sums[steps * lo * 3:steps * hi * 3])
         del b0, preds
-    host = sums.cpu().double().numpy()   # the one synchronisation
-    blocks = [host[steps * lo * 3:steps * min(n, lo + max_batch) * 3].reshape(steps, -1, 3)
-              for lo in range(0, n, max_batch)]
-    return np.concatenate(blocks, axis=1)
+    return _chunked_sums(sums.cpu().double().numpy(), steps, n, max_batch)   # the one synchronisation

@@ -27,7 +27,7 @@ from typing import Optional
 import numpy as np
 import torch
 
-from .data import DeviceFrames, case_table
+from .data import DeviceFrames, describe_split  # noqa: F401  (DeviceFrames is re-exported)
 
 STATE_NAME = "training_state.pt"
 STATE_VERSION = 1
@@ -45,16 +45,12 @@ def model_config(model) -> dict:
 
 def split_fingerprint(data) -> dict:
     """Sample count, grid, case-parameter count, frame storage dtype and a SHA-256 of the case_ids sequence of a split
-    (a DeviceFrames or the reference's dataset object, which train_auto uploads in float32).  The frames themselves are
-    not hashed."""
-    if isinstance(data, DeviceFrames):
-        n, gh, gw, p = data.n, data.height, data.width, data.n_case_params
-        dtype, ids = data.frame_dtype, data._case_ids_host
-    else:
-        n, gh, gw = int(data.inputs.shape[0]), int(data.inputs.shape[2]), int(data.inputs.shape[3])
-        p, dtype, ids = case_table(data.case_params).shape[1], torch.float32, data.case_ids
-    ids = np.ascontiguousarray(np.asarray(ids).reshape(-1), dtype=np.int64)
-    return dict(n=int(n), height=int(gh), width=int(gw), n_case_params=int(p), frame_dtype=str(dtype).replace("torch.", ""),
+    (`describe_split`: a DeviceFrames or the reference's dataset object, which train_auto uploads in float32).  The
+    frames themselves are not hashed."""
+    split = describe_split(data, "data")
+    ids = np.ascontiguousarray(split.case_ids, dtype=np.int64)
+    return dict(n=int(split.n), height=int(split.height), width=int(split.width), n_case_params=int(split.n_case_params),
+                frame_dtype=str(split.frame_dtype).replace("torch.", ""),
                 case_ids_sha256=hashlib.sha256(ids.tobytes()).hexdigest())
 
 

@@ -33,8 +33,10 @@ import numpy as np
 import torch
 
 from . import _lib, resume
-from .data import DeviceFrames, _check_chain, _gather, case_table, check_noise_args, index_batches, rollout_windows
+from .data import (DeviceFrames, _check_chain, _check_split, _gather, _positive_int, as_device_frames, check_noise_args,
+                   index_batches, split_windows)
 from .fno2d import capture_graph, side_stream
+from .metrics import _evaluate_rollout, evaluate_auto
 from .optim import FusedAdam
 
 LOG_COLUMNS = ("mse", "rmse", "mae", "nmse", "mean_l2")   # one row of the epoch log: fno_loss_fwd's five scalars
@@ -369,39 +371,6 @@ class _RolloutStepGraphs(_StepGraphs):
 
 
 # ------------------------------------------------------------------------------------------------ train_auto
-def _positive_int(name: str, v) -> None:
-    if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or v < 1:
-        raise ValueError(f"{name} must be a positive int, got {v!r}")
-
-
-def _check_split(model, data, what: str) -> None:
-    """Refuse, before any device work, a split (a DeviceFrames or the reference's dataset object) the model cannot
-    train or evaluate on: malformed or empty frames, a case_ids list of the wrong length, a case-parameter count other
-    than the model's, or a grid / storage mode the model rejects."""
-    if isinstance(data, DeviceFrames):
-        if data.frames_in.device != model.device:
-            raise ValueError(f"{what}: the frames are on {data.frames_in.device}, the model on {model.device}")
-        n, gh, gw, p = data.n, data.height, data.width, data.n_case_params
-    else:
-        ins, labs = getattr(data, "inputs", None), getattr(data, "labels", None)
-        if not isinstance(ins, torch.Tensor) or not isinstance(labs, torch.Tensor) or ins.dim() != 4 \
-                or ins.shape[1] != 3 or labs.shape != ins.shape:
-            raise ValueError(f"{what} must be a DeviceFrames or a dataset with (N, 3, H, W) .inputs / .labels tensors, "
-                             f"got {getattr(ins, 'shape', None)} / {getattr(labs, 'shape', None)}")
-        n, gh, gw = int(ins.shape[0]), int(ins.shape[2]), int(ins.shape[3])
-        if n == 0:
-            raise ValueError(f"{what} is empty")
-        if len(np.asarray(data.case_ids)) != n:
-            raise ValueError(f"{what}: dataset.case_ids must have one entry per sample")
-        p = case_table(data.case_params).shape[1]
-    if n == 0:
-        raise ValueError(f"{what} is empty")
-    if p != model.n_case_params:
-        raise ValueError(f"{what} has {p} case parameters per sample, the model takes n_case_params="
-                         f"{model.n_case_params}")
-    model._route(gh, gw)      # the model's own grid / storage-mode checks
-
-
 def _ema_shadow(model):
     """A Fno2d with `model`'s configuration, storage mode, device and kernel choices, holding a copy of its weights: the
     model the EMA weights are evaluated and saved through.  Built without drawing from the CPU RNG (the parameters'
@@ -548,7 +517,6 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
     resumable that is not a bool.
     Frozen parameters (requires_grad=False) are not updated, as FusedAdam.step skips them.  Data parallel training in
     this loop is not supported."""
-    from .metrics import _evaluate_rollout, evaluate_auto
     from .fno2d import Fno2d
     from .optim import FusedAdam, check_stabiliser_args
     if not isinstance(model, Fno2d):
@@ -566,8 +534,7 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
     if not isinstance(resumable, bool):
         raise ValueError(f"resumable must be a bool, got {resumable!r}")
     if dev_rollout_steps is not None:
-        _positive_int("dev_rollout_steps", dev_rollout_steps)
-        dev_rollout_steps = int(dev_rollout_steps)
+        dev_rollout_steps = _positive_int("dev_rollout_steps", dev_rollout_steps)
     max_grad_norm, ema_decay = check_stabiliser_args(max_grad_norm, ema_decay)
     grad_steps = rollout_steps if rollout_grad_steps is None else rollout_grad_steps
     if isinstance(grad_steps, bool) or not isinstance(grad_steps, (int, np.integer)) or not 1 <= grad_steps <= rollout_steps:
@@ -578,32 +545,16 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
     if not any(p.requires_grad for p in model.parameters()):
         raise ValueError("every parameter of the model is frozen: there is nothing to train")
     dev = model.device
-    for what, data in (("train_data", train_data), ("dev_data", dev_data)):
-        _check_split(model, data, what)
-    windows = None   # rollout_steps > 1: the window starts of the train split
+    train_split = _check_split(model, train_data, "train_data")
+    dev_split = _check_split(model, dev_data, "dev_data")
+    windows = tss = None   # rollout_steps > 1: the window starts of the train split and their time step size
     if rollout_steps > 1:
-        tss = getattr(train_data, "time_step_size", None) if time_step_size is None else time_step_size
-        if tss is None:
-            raise ValueError(f"rollout_steps={rollout_steps} needs a time_step_size: train_data has none, pass it")
-        _positive_int("time_step_size", tss)
-        case_ids = train_data._case_ids_host if isinstance(train_data, DeviceFrames) else train_data.case_ids
-        windows = rollout_windows(case_ids, rollout_steps, int(tss))
-        if windows.size == 0:
-            raise ValueError(f"train_data has no {rollout_steps}-step window with time_step_size={tss} inside one case")
+        windows, tss = split_windows(train_split, rollout_steps, time_step_size, "train_data", "rollout_steps")
     elif time_step_size is not None:
         _positive_int("time_step_size", time_step_size)
-    dev_windows = None   # dev_rollout_steps = S: the window starts of the dev split
+    dev_windows = dev_tss = None   # dev_rollout_steps = S: the window starts of the dev split, likewise
     if dev_rollout_steps is not None:
-        dev_tss = getattr(dev_data, "time_step_size", None) if time_step_size is None else time_step_size
-        if dev_tss is None:
-            raise ValueError(f"dev_rollout_steps={dev_rollout_steps} needs a time_step_size: dev_data has none, pass it")
-        _positive_int("time_step_size", dev_tss)
-        dev_tss = int(dev_tss)
-        dev_ids = dev_data._case_ids_host if isinstance(dev_data, DeviceFrames) else dev_data.case_ids
-        dev_windows = rollout_windows(dev_ids, dev_rollout_steps, dev_tss)
-        if dev_windows.size == 0:
-            raise ValueError(f"dev_data has no {dev_rollout_steps}-step window with time_step_size={dev_tss} inside one "
-                             "case")
+        dev_windows, dev_tss = split_windows(dev_split, dev_rollout_steps, time_step_size, "dev_data", "dev_rollout_steps")
     state = config = None
     if resumable:
         # Python floats, so that StepLR's decay of a restored learning rate runs in the same arithmetic as a straight
@@ -612,10 +563,9 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
         config = resume.run_config(
             model, train_data, dev_data, lr=lr, lr_step_size=int(lr_step_size), lr_gamma=lr_gamma,
             batch_size=int(batch_size), eval_batch_size=int(eval_batch_size), eval_interval=int(eval_interval),
-            rollout_steps=int(rollout_steps), time_step_size=int(tss) if windows is not None else None,
-            rollout_grad_steps=grad_steps, input_noise_std=float(input_noise_std), noise_seed=int(noise_seed),
-            noise_every_step=noise_every_step, dev_rollout_steps=dev_rollout_steps,
-            dev_time_step_size=dev_tss if dev_windows is not None else None, max_grad_norm=max_grad_norm,
+            rollout_steps=int(rollout_steps), time_step_size=tss, rollout_grad_steps=grad_steps,
+            input_noise_std=float(input_noise_std), noise_seed=int(noise_seed), noise_every_step=noise_every_step,
+            dev_rollout_steps=dev_rollout_steps, dev_time_step_size=dev_tss, max_grad_norm=max_grad_norm,
             ema_decay=ema_decay, generator=generator is not None)
         state = resume.find_state(output_dir, config)
     model._require_cuda()
@@ -635,23 +585,23 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
         start_epoch, global_step = state["epoch"] + 1, state["global_step"]
         train_losses, grad_norms = list(state["train_losses"]), list(state.get("grad_norms", []))
     with torch.cuda.device(dev):
-        frames = train_data if isinstance(train_data, DeviceFrames) else DeviceFrames(train_data, device=dev)
+        frames = as_device_frames(train_data, dev)
         dev_frames = None
         if dev_windows is not None:
-            dev_frames = dev_data if isinstance(dev_data, DeviceFrames) else DeviceFrames(dev_data, device=dev)
+            dev_frames = as_device_frames(dev_data, dev)
             _check_chain(dev_frames, dev_windows, dev_rollout_steps, dev_tss, what="dev_data")
         n = frames.n
         ema_model = None if ema_decay is None else _ema_shadow(model)
         noise = dict(noise_std=input_noise_std, noise_seed=int(noise_seed))
         if windows is not None:
-            _check_chain(frames, windows, rollout_steps, int(tss))
+            _check_chain(frames, windows, rollout_steps, tss)
         graphs = None   # a resumed run with no epoch left to train captures nothing
         if start_epoch < num_epochs:
             if windows is None:
                 graphs = _StepGraphs(model, frames, batch_size, optimizer, **noise)
             else:
                 graphs = _RolloutStepGraphs(model, frames, batch_size, optimizer, windows.size, rollout_steps,
-                                            int(tss), grad_steps, noise_every_step=noise_every_step, **noise)
+                                            tss, grad_steps, noise_every_step=noise_every_step, **noise)
         print("====== Training ======")
         print(f"# batch: {batch_size}")
         print(f"# examples: {n}")
@@ -703,7 +653,7 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
                     ckpt_dir = output_dir / f"ckpt-{ep}"
                     ckpt_dir.mkdir(exist_ok=True, parents=True)
                     if dev_frames is None:
-                        dev_frames = dev_data if isinstance(dev_data, DeviceFrames) else DeviceFrames(dev_data, device=dev)
+                        dev_frames = as_device_frames(dev_data, dev)
                     eval_model = model
                     if ema_model is not None:   # evaluate and save the EMA weights
                         optimizer.copy_ema_to(ema_model)
