@@ -242,3 +242,14 @@ def check(status: int, what: str) -> None:
     if status != 0:
         msg = load().fno_last_error()
         raise FnoNativeError(f"{what} failed with status {status}: {msg.decode() if msg else '?'}")
+
+
+def aligned(t):
+    """`t` as a contiguous tensor whose data pointer is 16-byte aligned: `t` itself when it already is, else a copy.
+
+    The C ABI refuses a caller pointer that is less aligned than its kernels' widest access through it (16 bytes for the
+    float4 / TMA reads of the 64x64 path).  A contiguous view can start at any element of its storage -- e.g.
+    `flat[p * B:].view(B, 2, 64, 64)` of a staging buffer -- so the modules pass every caller tensor that reaches such a
+    pointer through this: the ABI refuses, the module copies."""
+    t = t.contiguous()
+    return t if t.data_ptr() % 16 == 0 else t.clone()

@@ -132,6 +132,21 @@ static int fail(int code, const char* what, cudaError_t e = cudaSuccess) {
 static inline cudaStream_t S(void* s) { return static_cast<cudaStream_t>(s); }
 static inline bool bad_dtype(int d) { return d != FNO_ACT_F32 && d != FNO_ACT_BF16; }
 
+// Alignment of a caller device pointer, checked by every entry point before any device work: `bytes` is the widest access
+// the entry point's kernels make through it -- 16 for float4 / uint4 loads and stores, TMA and bulk copies; 8 for
+// float2 (complex64), int64 and four-bf16 (uint2) accesses; 4 or 2 for scalar fp32 / bf16 ones.  A misaligned vector
+// access faults the device (and ends the CUDA context); this refuses the call instead, naming the argument.  NULL passes
+// (the entry point's own null checks decide about it).
+static int need_align(const char* what, const char* arg, const void* p, unsigned bytes) {
+  if ((reinterpret_cast<uintptr_t>(p) & (bytes - 1)) == 0) return kOk;
+  char msg[192];
+  snprintf(msg, sizeof(msg), "%s: %s must be %u-byte aligned", what, arg, bytes);
+  return fail(kErrArg, msg);
+}
+#define FNO_ALIGN(what, p, bytes) FNO_TRY(need_align(what, #p, p, bytes))
+static inline unsigned act_bytes(int act_dtype) { return act_dtype == FNO_ACT_BF16 ? 2u : 4u; }   // scalar activation
+static inline unsigned frame_vec_bytes(int frame_dtype) { return frame_dtype == FNO_ACT_BF16 ? 8u : 16u; }   // 4 frames
+
 // ------------------------------------------------------------------------ per-step noise of a rollout (fno_noise)
 // Call step s of a rollout driver is fed x_s (the call's inputs, or the prediction of step s-1).  With a noise descriptor
 // and stream k0 + s >= 1 it is fed fed[s] = x_s + the noise of that stream instead (stream 0, the start frame's noise, is
@@ -181,6 +196,15 @@ static int noise_forward_args(const char* what, const fno_weights* w, const floa
 }
 
 static inline bool noisy_step(const fno_noise* nz, int s) { return nz && nz->k0 + s > 0; }
+
+// The caller frames of a forward / rollout / backward driver: the 64x64 lift and its backward read inputs and mask as
+// float4 (vec = 16); the grid kernels read every frame one float at a time (vec = 4).  case_params is read per float.
+static int frames_align(const char* what, const float* inputs, const float* mask, const float* case_params, unsigned vec) {
+  FNO_ALIGN(what, inputs, vec);
+  FNO_ALIGN(what, mask, vec);
+  FNO_ALIGN(what, case_params, 4);
+  return kOk;
+}
 
 // x = the frame call step s is fed: x itself, or fed[s] written from it (one launch)
 static int feed_step(const fno_noise* nz, float* fed, const float* mask, int s, size_t frame, int batch, int h, int wd,
@@ -232,6 +256,9 @@ size_t fno_bwd_partials_bytes(void) {
 
 int fno_pack_spectral_weights(const void* w1, const void* w2, void* wk, int conj_transpose, void* stream) {
   if (!w1 || !w2 || !wk) return fail(kErrArg, "fno_pack_spectral_weights: null pointer");
+  FNO_TRY(need_align("fno_pack_spectral_weights", "weights1", w1, 8));
+  FNO_TRY(need_align("fno_pack_spectral_weights", "weights2", w2, 8));
+  FNO_ALIGN("fno_pack_spectral_weights", wk, 8);
   FNO_CUDA(launch_pack_spectral(w1, w2, wk, conj_transpose, S(stream)), "pack_spectral_kernel");
   return kOk;
 }
@@ -240,18 +267,26 @@ size_t fno_mix_operand_bytes(void) { return mix_operand_bytes(); }
 
 int fno_pack_mix_operand(const void* wk, void* wop, void* stream) {
   if (!wk || !wop) return fail(kErrArg, "fno_pack_mix_operand: null pointer");
+  FNO_ALIGN("fno_pack_mix_operand", wk, 8);
+  FNO_ALIGN("fno_pack_mix_operand", wop, 4);
   FNO_CUDA(launch_pack_mix_operand(wk, wop, S(stream)), "pack_mix_operand_kernel");
   return kOk;
 }
 
 int fno_pack_mix_operand_from_weights(const void* w1, const void* w2, void* wop, int conj_transpose, void* stream) {
   if (!w1 || !w2 || !wop) return fail(kErrArg, "fno_pack_mix_operand_from_weights: null pointer");
+  FNO_TRY(need_align("fno_pack_mix_operand_from_weights", "weights1", w1, 8));
+  FNO_TRY(need_align("fno_pack_mix_operand_from_weights", "weights2", w2, 8));
+  FNO_ALIGN("fno_pack_mix_operand_from_weights", wop, 16);
   FNO_CUDA(launch_pack_mix_operand_direct(w1, w2, wop, conj_transpose, S(stream)), "pack_mix_operand_direct_kernel");
   return kOk;
 }
 
 int fno_unpack_spectral_grads(const void* gwk, void* gw1, void* gw2, void* stream) {
   if (!gwk || !gw1 || !gw2) return fail(kErrArg, "fno_unpack_spectral_grads: null pointer");
+  FNO_ALIGN("fno_unpack_spectral_grads", gwk, 8);
+  FNO_ALIGN("fno_unpack_spectral_grads", gw1, 8);
+  FNO_ALIGN("fno_unpack_spectral_grads", gw2, 8);
   FNO_CUDA(launch_unpack_spectral(gwk, gw1, gw2, 0, S(stream)), "unpack_spectral_kernel");
   return kOk;
 }
@@ -261,6 +296,10 @@ int fno_lift_fwd(const float* inputs, const float* mask, const float* case_param
   if (!inputs || !mask || !w || !act_out || batch <= 0 || bad_dtype(act_dtype))
     return fail(kErrArg, "fno_lift_fwd: bad argument");
   if (w->n_case_params > 0 && !case_params) return fail(kErrArg, "fno_lift_fwd: case_params is null");
+  FNO_ALIGN("fno_lift_fwd", inputs, 16);
+  FNO_ALIGN("fno_lift_fwd", mask, 16);
+  FNO_ALIGN("fno_lift_fwd", case_params, 4);
+  FNO_ALIGN("fno_lift_fwd", act_out, 16);
   cudaError_t e = act_dtype == FNO_ACT_F32
                       ? launch_lift<float>(inputs, mask, case_params, w->fc0_w, w->fc0_b, w->gx, w->gy, act_out, batch,
                                            w->n_case_params, S(stream))
@@ -272,6 +311,8 @@ int fno_lift_fwd(const float* inputs, const float* mask, const float* case_param
 
 int fno_spectral_dft_fwd(const void* act_in, void* xm, int batch, int act_dtype, float s0, float s1, void* stream) {
   if (!act_in || !xm || batch <= 0 || bad_dtype(act_dtype)) return fail(kErrArg, "fno_spectral_dft_fwd: bad argument");
+  FNO_ALIGN("fno_spectral_dft_fwd", act_in, 16);
+  FNO_ALIGN("fno_spectral_dft_fwd", xm, act_dtype == FNO_ACT_BF16 ? 16u : 8u);   // launch_dft_fwd_tc requires 16
   if (act_dtype == FNO_ACT_BF16) {   // bf16 planes: the two-GEMM tensor-core kernel (fno_dft_fwd_tc.cu)
     FNO_CUDA(launch_dft_fwd_tc(act_in, xm, batch, s0, s1, S(stream)), "dft_fwd_tc_kernel");
     return kOk;
@@ -282,12 +323,18 @@ int fno_spectral_dft_fwd(const void* act_in, void* xm, int batch, int act_dtype,
 
 int fno_mode_mix(const void* xm, const void* wk, void* ym, int batch, void* stream) {
   if (!xm || !wk || !ym || batch <= 0) return fail(kErrArg, "fno_mode_mix: bad argument");
+  FNO_ALIGN("fno_mode_mix", xm, 16);
+  FNO_TRY(need_align("fno_mode_mix", "wop", wk, 16));
+  FNO_ALIGN("fno_mode_mix", ym, 8);
   FNO_CUDA(launch_mode_mix(xm, wk, ym, nullptr, batch, S(stream)), "mode_mix_tc_kernel");
   return kOk;
 }
 
 int fno_mode_mix_image(const void* xm, const void* wk, void* ym_img, int batch, void* stream) {
   if (!xm || !wk || !ym_img || batch <= 0) return fail(kErrArg, "fno_mode_mix_image: bad argument");
+  FNO_ALIGN("fno_mode_mix_image", xm, 16);
+  FNO_TRY(need_align("fno_mode_mix_image", "wop", wk, 16));
+  FNO_ALIGN("fno_mode_mix_image", ym_img, 4);
   FNO_CUDA(launch_mode_mix(xm, wk, nullptr, ym_img, batch, S(stream)), "mode_mix_tc_kernel(image)");
   return kOk;
 }
@@ -295,12 +342,19 @@ int fno_mode_mix_image(const void* xm, const void* wk, void* ym_img, int batch, 
 int fno_block_fused(const void* ym_img, const void* act_in, const float* w0t, const float* bias, void* act_out, int batch,
                     void* stream) {
   if (!ym_img || !act_in || !w0t || !act_out || batch <= 0) return fail(kErrArg, "fno_block_fused: bad argument");
+  FNO_ALIGN("fno_block_fused", ym_img, 16);
+  FNO_TRY(need_align("fno_block_fused", "act_in_bf16", act_in, 16));
+  FNO_ALIGN("fno_block_fused", w0t, 4);
+  FNO_ALIGN("fno_block_fused", bias, 4);
+  FNO_TRY(need_align("fno_block_fused", "act_out_bf16", act_out, 16));
   FNO_CUDA(launch_block_fused(ym_img, act_in, w0t, bias, act_out, batch, S(stream)), "block_fused_kernel");
   return kOk;
 }
 
 int fno_spectral_inv_kx(const void* ym, void* z, int batch, float s0, float s1, void* stream) {
   if (!ym || !z || batch <= 0) return fail(kErrArg, "fno_spectral_inv_kx: bad argument");
+  FNO_ALIGN("fno_spectral_inv_kx", ym, 8);
+  FNO_ALIGN("fno_spectral_inv_kx", z, 4);
   FNO_CUDA(launch_inv_kx(ym, z, batch, s0, s1, S(stream)), "inv_kx_kernel");
   return kOk;
 }
@@ -311,6 +365,13 @@ int fno_block_out(int epilogue, const void* z, const void* act_in, const float* 
     return fail(kErrArg, "fno_block_out: bad argument");
   if (epilogue == FNO_EPI_GELU_SAVE_PRE && !pre_out) return fail(kErrArg, "fno_block_out: pre_out is null");
   if (epilogue == FNO_EPI_MUL_DGELU && !pre_in) return fail(kErrArg, "fno_block_out: pre_in is null");
+  FNO_ALIGN("fno_block_out", z, 4);
+  FNO_ALIGN("fno_block_out", act_in, act_bytes(act_dtype));
+  FNO_ALIGN("fno_block_out", w0t, 4);
+  FNO_ALIGN("fno_block_out", bias, 4);
+  FNO_ALIGN("fno_block_out", act_out, act_bytes(act_dtype));
+  FNO_ALIGN("fno_block_out", pre_out, 4);
+  FNO_ALIGN("fno_block_out", pre_in, 4);
   cudaError_t e = act_dtype == FNO_ACT_F32
                       ? launch_block_tc<float>(epilogue, z, act_in, w0t, bias, act_out, pre_out, pre_in, batch, S(stream))
                       : launch_block_tc<__nv_bfloat16>(epilogue, z, act_in, w0t, bias, act_out, pre_out, pre_in, batch,
@@ -322,8 +383,12 @@ int fno_block_out(int epilogue, const void* z, const void* act_in, const float* 
 int fno_block_fwd(const fno_weights* w, int layer, const void* act_in, void* act_out, float* pre_out,
                   const fno_workspace* ws, int batch, int act_dtype, void* stream) {
   if (!w || !ws || layer < 0 || layer >= w->n_layers) return fail(kErrArg, "fno_block_fwd: bad argument");
+  const bool fused = act_dtype == FNO_ACT_BF16 && ws->ym_img && !pre_out;   // TMA reads and writes the activations
+  FNO_ALIGN("fno_block_fwd", act_in, 16);
+  FNO_ALIGN("fno_block_fwd", act_out, fused ? 16u : act_bytes(act_dtype));
+  FNO_ALIGN("fno_block_fwd", pre_out, 4);
   FNO_TRY(fno_spectral_dft_fwd(act_in, ws->xm, batch, act_dtype, 1.f, 1.f, stream));
-  if (act_dtype == FNO_ACT_BF16 && ws->ym_img && !pre_out) {   // inference, bf16 storage: fused output stage
+  if (fused) {   // inference, bf16 storage: fused output stage
     FNO_TRY(fno_mode_mix_image(ws->xm, w->spec_wk[layer], ws->ym_img, batch, stream));
     return fno_block_fused(ws->ym_img, act_in, w->w0t[layer], w->w0_b[layer], act_out, batch, stream);
   }
@@ -338,6 +403,9 @@ int fno_project_fwd(const void* act_in, const float* mask, const fno_weights* w,
                     int act_dtype, void* stream) {
   if (!act_in || !mask || !w || !preds || batch <= 0 || bad_dtype(act_dtype))
     return fail(kErrArg, "fno_project_fwd: bad argument");
+  FNO_ALIGN("fno_project_fwd", act_in, act_bytes(act_dtype));
+  FNO_ALIGN("fno_project_fwd", mask, 4);
+  FNO_ALIGN("fno_project_fwd", preds, 4);
   cudaError_t e =
       act_dtype == FNO_ACT_F32
           ? launch_project_tc<float>(act_in, w->fc1_w, w->fc1_b, w->fc2_w, w->fc2_b, mask, preds, batch, S(stream))
@@ -351,6 +419,8 @@ int fno_forward(const fno_weights* w, const float* inputs, const float* mask, co
   if (!w || !ws || !ws->act[0] || !ws->act[1] || !ws->xm) return fail(kErrArg, "fno_forward: bad workspace");
   if (!(act_dtype == FNO_ACT_BF16 && ws->ym_img) && (!ws->ym || !ws->z)) return fail(kErrArg, "fno_forward: bad workspace");
   if (w->n_layers < 1 || w->n_layers > FNO_MAX_LAYERS) return fail(kErrUnsupported, "fno_forward: n_layers out of range");
+  FNO_TRY(frames_align("fno_forward", inputs, mask, case_params, 16));
+  FNO_ALIGN("fno_forward", preds, 4);
   FNO_TRY(fno_lift_fwd(inputs, mask, case_params, w, ws->act[0], batch, act_dtype, stream));
   int cur = 0;
   for (int l = 0; l < w->n_layers; ++l) {
@@ -368,6 +438,9 @@ static int rollout_impl(const char* what, const fno_weights* w, const float* inp
     snprintf(msg, sizeof(msg), "%s: bad argument", what);
     return fail(kErrArg, msg);
   }
+  FNO_TRY(frames_align(what, inputs, mask, case_params, 16));
+  FNO_ALIGN(what, preds_seq, 16);   // step s + 1's lift reads preds_seq[s]
+  FNO_ALIGN(what, fed, 16);
   const size_t frame = static_cast<size_t>(batch) * 2 * kHW;
   const float* cur = inputs;
   for (int s = 0; s < steps; ++s) {
@@ -405,6 +478,7 @@ int fno_rollout_host(const fno_weights* w, const float* inputs_host, const float
                      void* dev_io, int batch, int act_dtype, void* stream) {
   if (!w || !inputs_host || !mask_host || !preds_seq_host || !dev_io || batch <= 0 || steps <= 0)
     return fail(kErrArg, "fno_rollout_host: bad argument");
+  FNO_ALIGN("fno_rollout_host", dev_io, 16);   // the device frames it holds are the rollout's inputs / mask / preds_seq
   const size_t b = static_cast<size_t>(batch);
   float* d_in = static_cast<float*>(dev_io);
   float* d_mask = d_in + b * 2 * kHW;
@@ -445,6 +519,8 @@ int fno_forward_train(const fno_weights* w, const float* inputs, const float* ma
                       int act_dtype, void* stream) {
   if (!w || !saved || !ws || !ws->ym || !ws->z) return fail(kErrArg, "fno_forward_train: bad argument");
   if (w->n_layers < 1 || w->n_layers > FNO_MAX_LAYERS) return fail(kErrUnsupported, "fno_forward_train: n_layers");
+  FNO_TRY(frames_align("fno_forward_train", inputs, mask, case_params, 16));
+  FNO_ALIGN("fno_forward_train", preds, 4);
   FNO_TRY(forward_train_body(w, inputs, mask, case_params, saved, ws, batch, act_dtype, stream));
   return fno_project_fwd(saved->act[w->n_layers], mask, w, preds, batch, act_dtype, stream);
 }
@@ -472,6 +548,10 @@ static int backward_impl(const char* what, const fno_weights* w, const fno_weigh
     snprintf(msg, sizeof(msg), "%s: null scratch buffer", what);
     return fail(kErrArg, msg);
   }
+  FNO_TRY(frames_align(what, inputs, mask, case_params, 16));
+  FNO_ALIGN(what, dpreds, 4);   // read one float at a time by project_bwd_tc_kernel
+  FNO_ALIGN(what, d_inputs, 16);
+  FNO_ALIGN(what, d_case_params, 4);
   cudaStream_t st = S(stream);
   const int L = w->n_layers, p = w->n_case_params;
   const bool bf = act_dtype == FNO_ACT_BF16;
@@ -561,9 +641,27 @@ int fno_backward_inputs(const fno_weights* w, const fno_weights_bwd* wb, const f
     return fail(kErrArg, "fno_backward_inputs: n_case_params out of range");
   if (w && w->n_case_params == 0) d_case_params = nullptr;   // nothing to write
   if (!grads && !d_inputs && !d_case_params) return fail(kErrArg, "fno_backward_inputs: no output requested");
-  if ((reinterpret_cast<uintptr_t>(d_inputs) & 15) != 0) return fail(kErrArg, "fno_backward_inputs: d_inputs must be 16-byte aligned");
   return backward_impl("fno_backward_inputs", w, wb, inputs, mask, case_params, dpreds, saved, grads, scratch, ws, batch,
                        act_dtype, stream, d_inputs, d_case_params);
+}
+
+// The arguments of the batch and window gathers: the 64x64 kernels (vec) move four frame elements at a time -- float4, or
+// uint2 for bf16 frames -- and store float4; the grid kernels move one element at a time.
+static int gather_align(const char* what, const void* frames_in, const void* frames_out, const float* case_table,
+                        const int32_t* case_ids, const int64_t* idx, int frame_dtype, const float* inputs, const float* label,
+                        const float* mask, const float* case_params, const float* labels_seq, bool vec) {
+  const unsigned f = vec ? frame_vec_bytes(frame_dtype) : (frame_dtype == FNO_ACT_BF16 ? 2u : 4u), o = vec ? 16u : 4u;
+  FNO_ALIGN(what, frames_in, f);
+  FNO_ALIGN(what, frames_out, f);
+  FNO_ALIGN(what, case_table, 4);
+  FNO_ALIGN(what, case_ids, 4);
+  FNO_ALIGN(what, idx, 8);
+  FNO_ALIGN(what, inputs, o);
+  FNO_ALIGN(what, label, o);
+  FNO_ALIGN(what, mask, o);
+  FNO_ALIGN(what, case_params, 4);
+  FNO_ALIGN(what, labels_seq, o);
+  return kOk;
 }
 
 // ------------------------------------------------------------------------ training through a rollout (64x64 and grids)
@@ -610,6 +708,9 @@ static int rollout_forward_train_impl(const char* what, const fno_weights* w, co
     snprintf(msg, sizeof(msg), "%s: bad argument", what);
     return fail(kErrArg, msg);
   }
+  FNO_TRY(frames_align(what, inputs, mask, case_params, 16));
+  FNO_ALIGN(what, preds_seq, 16);   // step s + 1's lift reads preds_seq[s]
+  FNO_ALIGN(what, fed, 16);
   const size_t frame = static_cast<size_t>(batch) * 2 * kHW;
   const float* cur = inputs;
   for (int s = 0; s < steps; ++s) {
@@ -651,10 +752,15 @@ static int rollout_backward_impl(const char* what, const fno_weights* w, const f
     snprintf(msg, sizeof(msg), "%s: bad act_dtype", what);
     return fail(kErrArg, msg);
   }
-  if ((reinterpret_cast<uintptr_t>(d_inputs) | reinterpret_cast<uintptr_t>(carry) | reinterpret_cast<uintptr_t>(dpreds_seq)) & 15) {
-    snprintf(msg, sizeof(msg), "%s: d_inputs, carry and dpreds_seq must be 16-byte aligned", what);
-    return fail(kErrArg, msg);
-  }
+  // the sweep's recomputed lift and lift backward read its frames (inputs, preds_seq, fed) as float4; its hand-off
+  // writes carry / d_inputs and reads dpreds_seq as float4
+  FNO_TRY(frames_align(what, inputs, mask, case_params, 16));
+  FNO_ALIGN(what, preds_seq, 16);
+  FNO_ALIGN(what, dpreds_seq, 16);
+  FNO_ALIGN(what, fed, 16);
+  FNO_ALIGN(what, carry, 16);
+  FNO_ALIGN(what, d_inputs, 16);
+  FNO_ALIGN(what, d_case_params, 4);
   const size_t frame = static_cast<size_t>(batch) * 2 * kHW;
   if (d_case_params)   // every sweep step adds its share
     FNO_CUDA(cudaMemsetAsync(d_case_params, 0, static_cast<size_t>(batch) * w->n_case_params * sizeof(float), S(stream)),
@@ -694,6 +800,10 @@ int fno_multistep_metrics(const float* preds_seq, const float* label_u, const fl
                           int batch, void* stream) {
   if (!preds_seq || !label_u || !mask || !sums || steps <= 0 || batch <= 0)
     return fail(kErrArg, "fno_multistep_metrics: bad argument");
+  FNO_ALIGN("fno_multistep_metrics", preds_seq, 16);
+  FNO_ALIGN("fno_multistep_metrics", label_u, 16);
+  FNO_ALIGN("fno_multistep_metrics", mask, 16);
+  FNO_ALIGN("fno_multistep_metrics", sums, 4);
   FNO_CUDA(launch_multistep_metrics(preds_seq, label_u, mask, sums, steps, batch, S(stream)), "multistep_metrics_kernel");
   return kOk;
 }
@@ -704,6 +814,8 @@ int fno_gather_batch(const void* frames_in, const void* frames_out, const float*
   if (!frames_in || !frames_out || !case_ids || !idx || !inputs || !label || !mask || n_idx <= 0 || n_case_params < 0 ||
       n_case_params > kMaxCaseParams || bad_dtype(frame_dtype) || (n_case_params > 0 && (!case_table || !case_params)))
     return fail(kErrArg, "fno_gather_batch: bad argument");
+  FNO_TRY(gather_align("fno_gather_batch", frames_in, frames_out, case_table, case_ids, idx, frame_dtype, inputs, label, mask,
+                       case_params, nullptr, true));
   FNO_CUDA(launch_gather_batch(frames_in, frames_out, case_table, reinterpret_cast<const int*>(case_ids),
                                reinterpret_cast<const long long*>(idx), n_idx, n_case_params, frame_dtype == FNO_ACT_BF16,
                                inputs, label, mask, case_params, S(stream)),
@@ -715,8 +827,10 @@ size_t fno_loss_scratch_bytes(void) { return loss_scratch_bytes(); }
 
 int fno_loss_fwd(const float* preds, const float* labels, size_t n, void* scratch, float* out, void* stream) {
   if (!preds || !labels || !scratch || !out || n == 0) return fail(kErrArg, "fno_loss_fwd: bad argument");
-  if ((reinterpret_cast<uintptr_t>(preds) | reinterpret_cast<uintptr_t>(labels)) & 15)
-    return fail(kErrArg, "fno_loss_fwd: preds / labels must be 16-byte aligned");
+  FNO_ALIGN("fno_loss_fwd", preds, 16);
+  FNO_ALIGN("fno_loss_fwd", labels, 16);
+  FNO_ALIGN("fno_loss_fwd", scratch, 4);
+  FNO_ALIGN("fno_loss_fwd", out, 4);
   FNO_CUDA(launch_loss_fwd(preds, labels, n, static_cast<float*>(scratch), out, S(stream)), "loss_fwd_kernel");
   return kOk;
 }
@@ -724,6 +838,11 @@ int fno_loss_fwd(const float* preds, const float* labels, size_t n, void* scratc
 int fno_loss_bwd(const float* preds, const float* labels, const float* fwd, const float* gout, float* dpreds, size_t n,
                  void* stream) {
   if (!preds || !labels || !fwd || !gout || !dpreds || n == 0) return fail(kErrArg, "fno_loss_bwd: bad argument");
+  FNO_ALIGN("fno_loss_bwd", preds, 4);
+  FNO_ALIGN("fno_loss_bwd", labels, 4);
+  FNO_ALIGN("fno_loss_bwd", fwd, 4);
+  FNO_ALIGN("fno_loss_bwd", gout, 4);
+  FNO_ALIGN("fno_loss_bwd", dpreds, 4);
   FNO_CUDA(launch_loss_bwd(preds, labels, fwd, gout, dpreds, n, S(stream)), "loss_bwd_kernel");
   return kOk;
 }
@@ -753,6 +872,7 @@ static int adam_step_impl(const char* what, const fno_adam_tensors* t, float lr,
     snprintf(msg, sizeof(msg), "%s: %s", what, args_ok ? "bad tensor table" : "bad argument");
     return fail(kErrArg, msg);
   }
+  FNO_ALIGN(what, clip_coef, 4);
   FNO_CUDA(launch_adam_step_ex(t, lr, beta1, beta2, eps, weight_decay, step, clip_coef, ema, ema_decay, S(stream)), what);
   return kOk;
 }
@@ -761,12 +881,16 @@ static int adam_step_impl(const char* what, const fno_adam_tensors* t, float lr,
 static int adam_step_dev_impl(const char* what, const fno_adam_tensors* t, const float* coef, int n_coef,
                               const int32_t* cursor, float beta1, float beta2, float eps, float weight_decay,
                               const float* clip_coef, void* const* ema, const float* ema_decay_tab, void* stream) {
-  const bool args_ok = coef && cursor && n_coef > 0 && !(reinterpret_cast<uintptr_t>(coef) & 7) && (!ema || ema_decay_tab);
+  const bool args_ok = coef && cursor && n_coef > 0 && (!ema || ema_decay_tab);
   if (!args_ok || !adam_tensors_ok(t) || !ema_ok(t, ema)) {
     char msg[96];
     snprintf(msg, sizeof(msg), "%s: %s", what, args_ok ? "bad tensor table" : "bad argument");
     return fail(kErrArg, msg);
   }
+  FNO_ALIGN(what, coef, 8);   // one float2 per step
+  FNO_ALIGN(what, cursor, 4);
+  FNO_ALIGN(what, clip_coef, 4);
+  FNO_ALIGN(what, ema_decay_tab, 4);
   FNO_CUDA(launch_adam_step_dev_ex(t, coef, n_coef, reinterpret_cast<const int*>(cursor), beta1, beta2, eps, weight_decay,
                                    clip_coef, ema, ema ? ema_decay_tab : nullptr, S(stream)),
            what);
@@ -796,8 +920,12 @@ size_t fno_grad_norm_scratch_bytes(void) { return grad_norm_scratch_bytes(); }
 int fno_grad_norm(const fno_adam_tensors* tables, int n_tables, float max_norm, float* out, void* scratch, float* log,
                   int n_log, const int32_t* cursor, void* stream) {
   if (!tables || n_tables < 1 || n_tables > FNO_GRAD_NORM_MAX_TABLES || !(max_norm > 0.f) || !isfinite(max_norm) || !out ||
-      !scratch || (reinterpret_cast<uintptr_t>(scratch) & 7) || (log && (!cursor || n_log <= 0)))
+      !scratch || (log && (!cursor || n_log <= 0)))
     return fail(kErrArg, "fno_grad_norm: bad argument");
+  FNO_ALIGN("fno_grad_norm", out, 4);
+  FNO_ALIGN("fno_grad_norm", scratch, 8);   // float64 partial sums
+  FNO_ALIGN("fno_grad_norm", log, 4);
+  FNO_ALIGN("fno_grad_norm", cursor, 4);
   for (int k = 0; k < n_tables; ++k) {   // only the grad and n fields are read
     const fno_adam_tensors& t = tables[k];
     if (t.count < 0 || t.count > FNO_ADAM_MAX_TENSORS) return fail(kErrArg, "fno_grad_norm: bad tensor table");
@@ -833,6 +961,9 @@ int fno_train_stage_indices(const int64_t* perm, int64_t n_perm, int stride, int
                             int64_t* idx_out, void* stream) {
   if (!perm || !cursor || !idx_out || n_perm <= 0 || stride <= 0 || batch <= 0 || batch > stride || batch > n_perm)
     return fail(kErrArg, "fno_train_stage_indices: bad argument");
+  FNO_ALIGN("fno_train_stage_indices", perm, 8);
+  FNO_ALIGN("fno_train_stage_indices", cursor, 4);
+  FNO_ALIGN("fno_train_stage_indices", idx_out, 8);
   FNO_CUDA(launch_stage_indices(reinterpret_cast<const long long*>(perm), n_perm, stride, batch,
                                 reinterpret_cast<const int*>(cursor), reinterpret_cast<long long*>(idx_out), S(stream)),
            "stage_indices_kernel");
@@ -841,6 +972,9 @@ int fno_train_stage_indices(const int64_t* perm, int64_t n_perm, int stride, int
 
 int fno_train_log_step(const float* loss_out, float* log, int n_log, int32_t* cursor, void* stream) {
   if (!loss_out || !log || !cursor || n_log <= 0) return fail(kErrArg, "fno_train_log_step: bad argument");
+  FNO_ALIGN("fno_train_log_step", loss_out, 4);
+  FNO_ALIGN("fno_train_log_step", log, 4);
+  FNO_ALIGN("fno_train_log_step", cursor, 4);
   FNO_CUDA(launch_log_step(loss_out, log, n_log, reinterpret_cast<int*>(cursor), S(stream)), "log_step_kernel");
   return kOk;
 }
@@ -869,6 +1003,8 @@ int fno_gather_window(const void* frames_in, const void* frames_out, const float
                       void* stream) {
   FNO_TRY(gather_window_args("fno_gather_window", frames_in, frames_out, case_table, case_ids, idx, n_idx, n_case_params,
                              frame_dtype, inputs, mask, case_params, steps, time_step_size, n_frames, labels_seq));
+  FNO_TRY(gather_align("fno_gather_window", frames_in, frames_out, case_table, case_ids, idx, frame_dtype, inputs, label, mask,
+                       case_params, labels_seq, true));
   FNO_CUDA(launch_gather_window(frames_in, frames_out, case_table, reinterpret_cast<const int*>(case_ids),
                                 reinterpret_cast<const long long*>(idx), n_idx, n_case_params, frame_dtype == FNO_ACT_BF16,
                                 inputs, label, mask, case_params, steps, time_step_size, n_frames, labels_seq, S(stream)),
@@ -882,6 +1018,10 @@ int fno_loss_seq_fwd(const float* preds_seq, const float* labels_seq, size_t n, 
                      void* stream) {
   if (!preds_seq || !labels_seq || !scratch || !out || n == 0 || steps < 1 || steps > kMaxSeqSteps)
     return fail(kErrArg, "fno_loss_seq_fwd: bad argument");
+  FNO_ALIGN("fno_loss_seq_fwd", preds_seq, 4);
+  FNO_ALIGN("fno_loss_seq_fwd", labels_seq, 4);
+  FNO_ALIGN("fno_loss_seq_fwd", scratch, 4);
+  FNO_ALIGN("fno_loss_seq_fwd", out, 4);
   FNO_CUDA(launch_loss_seq_fwd(preds_seq, labels_seq, n, steps, static_cast<float*>(scratch), out, S(stream)),
            "loss_seq_fwd_kernel");
   return kOk;
@@ -891,6 +1031,11 @@ int fno_loss_seq_bwd(const float* preds_seq, const float* labels_seq, const floa
                      size_t n, int steps, void* stream) {
   if (!preds_seq || !labels_seq || !fwd || !gout || !dpreds_seq || n == 0 || steps < 1 || steps > kMaxSeqSteps)
     return fail(kErrArg, "fno_loss_seq_bwd: bad argument");
+  FNO_ALIGN("fno_loss_seq_bwd", preds_seq, 4);
+  FNO_ALIGN("fno_loss_seq_bwd", labels_seq, 4);
+  FNO_ALIGN("fno_loss_seq_bwd", fwd, 4);
+  FNO_ALIGN("fno_loss_seq_bwd", gout, 4);
+  FNO_ALIGN("fno_loss_seq_bwd", dpreds_seq, 4);
   FNO_CUDA(launch_loss_seq_bwd(preds_seq, labels_seq, fwd, gout, dpreds_seq, n, steps, S(stream)), "loss_seq_bwd_kernel");
   return kOk;
 }
@@ -920,6 +1065,10 @@ int fno_grid_lift_fwd(const float* inputs, const float* mask, const float* case_
   FNO_TRY(grid_arg("fno_grid_lift_fwd", h, wd));
   if (!inputs || !mask || !w || !act_out || batch <= 0 || !w->gx || !w->gy) return fail(kErrArg, "fno_grid_lift_fwd: bad argument");
   if (w->n_case_params > 0 && !case_params) return fail(kErrArg, "fno_grid_lift_fwd: case_params is null");
+  FNO_ALIGN("fno_grid_lift_fwd", inputs, 4);
+  FNO_ALIGN("fno_grid_lift_fwd", mask, 4);
+  FNO_ALIGN("fno_grid_lift_fwd", case_params, 4);
+  FNO_ALIGN("fno_grid_lift_fwd", act_out, 4);
   FNO_CUDA(launch_grid_lift(inputs, mask, case_params, w->fc0_w, w->fc0_b, w->gx, w->gy, act_out, batch, w->n_case_params, h,
                             wd, S(stream)),
            "grid_lift_kernel");
@@ -929,6 +1078,8 @@ int fno_grid_lift_fwd(const float* inputs, const float* mask, const float* case_
 int fno_grid_spectral_dft_fwd(const float* act_in, void* xm, int batch, int h, int wd, float s0, float s1, void* stream) {
   FNO_TRY(grid_arg("fno_grid_spectral_dft_fwd", h, wd));
   if (!act_in || !xm || batch <= 0) return fail(kErrArg, "fno_grid_spectral_dft_fwd: bad argument");
+  FNO_ALIGN("fno_grid_spectral_dft_fwd", act_in, 4);
+  FNO_ALIGN("fno_grid_spectral_dft_fwd", xm, 8);
   FNO_CUDA(launch_grid_dft(act_in, xm, batch, h, wd, s0, s1, S(stream)), "grid_dft_kernel");
   return kOk;
 }
@@ -936,6 +1087,8 @@ int fno_grid_spectral_dft_fwd(const float* act_in, void* xm, int batch, int h, i
 int fno_grid_spectral_inv_kx(const void* ym, float* z, int batch, int h, int wd, float s0, float s1, void* stream) {
   FNO_TRY(grid_arg("fno_grid_spectral_inv_kx", h, wd));
   if (!ym || !z || batch <= 0) return fail(kErrArg, "fno_grid_spectral_inv_kx: bad argument");
+  FNO_ALIGN("fno_grid_spectral_inv_kx", ym, 8);
+  FNO_ALIGN("fno_grid_spectral_inv_kx", z, 4);
   FNO_CUDA(launch_grid_inv_kx(ym, z, batch, h, wd, s0, s1, S(stream)), "grid_inv_kx_kernel");
   return kOk;
 }
@@ -947,6 +1100,13 @@ int fno_grid_block_out(int epilogue, const float* z, const float* act_in, const 
     return fail(kErrArg, "fno_grid_block_out: bad argument");
   if (epilogue == FNO_EPI_GELU_SAVE_PRE && !pre_out) return fail(kErrArg, "fno_grid_block_out: pre_out is null");
   if (epilogue == FNO_EPI_MUL_DGELU && !pre_in) return fail(kErrArg, "fno_grid_block_out: pre_in is null");
+  FNO_ALIGN("fno_grid_block_out", z, 16);
+  FNO_ALIGN("fno_grid_block_out", act_in, 4);
+  FNO_ALIGN("fno_grid_block_out", w0t, 4);
+  FNO_ALIGN("fno_grid_block_out", bias, 4);
+  FNO_ALIGN("fno_grid_block_out", act_out, 4);
+  FNO_ALIGN("fno_grid_block_out", pre_out, 4);
+  FNO_ALIGN("fno_grid_block_out", pre_in, 4);
   FNO_CUDA(launch_grid_block_out(epilogue, z, act_in, w0t, bias, act_out, pre_out, pre_in, batch, h, wd, S(stream)),
            "grid_block_out_kernel");
   return kOk;
@@ -956,6 +1116,9 @@ int fno_grid_project_fwd(const float* act_in, const float* mask, const fno_weigh
                          void* stream) {
   FNO_TRY(grid_arg("fno_grid_project_fwd", h, wd));
   if (!act_in || !mask || !w || !preds || batch <= 0) return fail(kErrArg, "fno_grid_project_fwd: bad argument");
+  FNO_ALIGN("fno_grid_project_fwd", act_in, 4);
+  FNO_ALIGN("fno_grid_project_fwd", mask, 4);
+  FNO_ALIGN("fno_grid_project_fwd", preds, 4);
   FNO_CUDA(launch_grid_project(act_in, w->fc1_w, w->fc1_b, w->fc2_w, w->fc2_b, mask, preds, batch, h * wd, S(stream)),
            "grid_project_kernel");
   return kOk;
@@ -999,6 +1162,17 @@ int fno_grid_project_bwd(const float* act_in, const float* dpreds, const float* 
     return fail(kErrArg, "fno_grid_project_bwd: bad argument");
   const bool any = g_fc1_w || g_fc1_b || g_fc2_w || g_fc2_b, all = g_fc1_w && g_fc1_b && g_fc2_w && g_fc2_b;
   if (any && !all) return fail(kErrArg, "fno_grid_project_bwd: pass all four gradient pointers or none");
+  FNO_ALIGN("fno_grid_project_bwd", act_in, 4);
+  FNO_ALIGN("fno_grid_project_bwd", dpreds, 4);
+  FNO_ALIGN("fno_grid_project_bwd", mask, 4);
+  FNO_ALIGN("fno_grid_project_bwd", pre, 4);
+  FNO_ALIGN("fno_grid_project_bwd", dpre_out, 4);
+  FNO_ALIGN("fno_grid_project_bwd", dz1, 4);
+  FNO_ALIGN("fno_grid_project_bwd", partials, 4);
+  FNO_ALIGN("fno_grid_project_bwd", g_fc1_w, 4);
+  FNO_ALIGN("fno_grid_project_bwd", g_fc1_b, 4);
+  FNO_ALIGN("fno_grid_project_bwd", g_fc2_w, 4);
+  FNO_ALIGN("fno_grid_project_bwd", g_fc2_b, 4);
   return grid_project_bwd_impl(act_in, dpreds, mask, pre, w, dpre_out, dz1, partials, g_fc1_w, g_fc1_b, g_fc2_w, g_fc2_b,
                                batch, h, wd, S(stream));
 }
@@ -1018,6 +1192,8 @@ int fno_grid_forward(const fno_weights* w, const float* inputs, const float* mas
   FNO_TRY(grid_arg("fno_grid_forward", h, wd));
   if (!w || !ws || !ws->act[0] || !ws->act[1] || !ws->xm || !ws->ym || !ws->z) return fail(kErrArg, "fno_grid_forward: bad workspace");
   if (w->n_layers < 1 || w->n_layers > FNO_MAX_LAYERS) return fail(kErrUnsupported, "fno_grid_forward: n_layers out of range");
+  FNO_TRY(frames_align("fno_grid_forward", inputs, mask, case_params, 4));
+  FNO_ALIGN("fno_grid_forward", preds, 4);
   float* act[2] = {static_cast<float*>(ws->act[0]), static_cast<float*>(ws->act[1])};
   FNO_TRY(fno_grid_lift_fwd(inputs, mask, case_params, w, act[0], batch, h, wd, stream));
   int cur = 0;
@@ -1037,6 +1213,9 @@ static int grid_rollout_impl(const char* what, const fno_weights* w, const float
     snprintf(msg, sizeof(msg), "%s: bad argument", what);
     return fail(kErrArg, msg);
   }
+  FNO_TRY(frames_align(what, inputs, mask, case_params, 4));
+  FNO_ALIGN(what, preds_seq, 4);
+  FNO_ALIGN(what, fed, 4);
   const size_t frame = static_cast<size_t>(batch) * 2 * h * wd;
   const float* cur = inputs;
   for (int s = 0; s < steps; ++s) {
@@ -1084,6 +1263,8 @@ int fno_grid_forward_train(const fno_weights* w, const float* inputs, const floa
   FNO_TRY(grid_arg("fno_grid_forward_train", h, wd));
   if (!w || !saved || !ws || !ws->ym || !ws->z || !saved->act[0]) return fail(kErrArg, "fno_grid_forward_train: bad argument");
   if (w->n_layers < 1 || w->n_layers > FNO_MAX_LAYERS) return fail(kErrUnsupported, "fno_grid_forward_train: n_layers");
+  FNO_TRY(frames_align("fno_grid_forward_train", inputs, mask, case_params, 4));
+  FNO_ALIGN("fno_grid_forward_train", preds, 4);
   FNO_TRY(grid_forward_train_body(w, inputs, mask, case_params, saved, ws, batch, h, wd, stream));
   return fno_grid_project_fwd(static_cast<const float*>(saved->act[w->n_layers]), mask, w, preds, batch, h, wd, stream);
 }
@@ -1153,6 +1334,10 @@ int fno_grid_backward(const fno_weights* w, const fno_weights_bwd* wb, const flo
   if (!g && !d_inputs && !d_case_params) return fail(kErrArg, "fno_grid_backward: no output requested");
   if (!sc->d[0] || !sc->d[1] || !sc->dz1 || !sc->gm || !sc->gwk || !sc->partials || !ws->ym || !ws->z)
     return fail(kErrArg, "fno_grid_backward: null scratch buffer");
+  FNO_TRY(frames_align("fno_grid_backward", inputs, mask, case_params, 4));
+  FNO_ALIGN("fno_grid_backward", dpreds, 4);
+  FNO_ALIGN("fno_grid_backward", d_inputs, 4);
+  FNO_ALIGN("fno_grid_backward", d_case_params, 4);
   return grid_backward_impl(w, wb, inputs, mask, case_params, dpreds, saved, g, sc, ws, d_inputs, d_case_params, batch, h, wd,
                             stream);
 }
@@ -1167,6 +1352,9 @@ static int grid_rollout_forward_train_impl(const char* what, const fno_weights* 
     snprintf(msg, sizeof(msg), "%s: bad argument", what);
     return fail(kErrArg, msg);
   }
+  FNO_TRY(frames_align(what, inputs, mask, case_params, 4));
+  FNO_ALIGN(what, preds_seq, 4);
+  FNO_ALIGN(what, fed, 4);
   const size_t frame = static_cast<size_t>(batch) * 2 * h * wd;
   const float* cur = inputs;
   for (int s = 0; s < steps; ++s) {
@@ -1212,6 +1400,13 @@ static int grid_rollout_backward_impl(const char* what, const fno_weights* w, co
     snprintf(msg, sizeof(msg), "%s: null saved buffer", what);
     return fail(kErrArg, msg);
   }
+  FNO_TRY(frames_align(what, inputs, mask, case_params, 4));
+  FNO_ALIGN(what, preds_seq, 4);
+  FNO_ALIGN(what, dpreds_seq, 4);
+  FNO_ALIGN(what, fed, 4);
+  FNO_ALIGN(what, carry, 4);
+  FNO_ALIGN(what, d_inputs, 4);
+  FNO_ALIGN(what, d_case_params, 4);
   const size_t frame = static_cast<size_t>(batch) * 2 * h * wd;
   if (d_case_params)   // every sweep step adds its share
     FNO_CUDA(cudaMemsetAsync(d_case_params, 0, static_cast<size_t>(batch) * w->n_case_params * sizeof(float), S(stream)),
@@ -1254,6 +1449,10 @@ int fno_grid_multistep_metrics(const float* preds_seq, const float* label_u, con
   FNO_TRY(grid_arg("fno_grid_multistep_metrics", h, wd));
   if (!preds_seq || !label_u || !mask || !sums || steps <= 0 || steps > 65535 || batch <= 0)
     return fail(kErrArg, "fno_grid_multistep_metrics: bad argument");
+  FNO_ALIGN("fno_grid_multistep_metrics", preds_seq, 4);
+  FNO_ALIGN("fno_grid_multistep_metrics", label_u, 4);
+  FNO_ALIGN("fno_grid_multistep_metrics", mask, 4);
+  FNO_ALIGN("fno_grid_multistep_metrics", sums, 4);
   FNO_CUDA(launch_grid_multistep_metrics(preds_seq, label_u, mask, sums, steps, batch, h, wd, S(stream)),
            "grid_multistep_metrics_kernel");
   return kOk;
@@ -1266,6 +1465,8 @@ int fno_grid_gather_batch(const void* frames_in, const void* frames_out, const f
   if (!frames_in || !frames_out || !case_ids || !idx || !inputs || !label || !mask || n_idx <= 0 || n_case_params < 0 ||
       n_case_params > kMaxCaseParams || bad_dtype(frame_dtype) || (n_case_params > 0 && (!case_table || !case_params)))
     return fail(kErrArg, "fno_grid_gather_batch: bad argument");
+  FNO_TRY(gather_align("fno_grid_gather_batch", frames_in, frames_out, case_table, case_ids, idx, frame_dtype, inputs, label,
+                       mask, case_params, nullptr, false));
   FNO_CUDA(launch_grid_gather_batch(frames_in, frames_out, case_table, reinterpret_cast<const int*>(case_ids),
                                     reinterpret_cast<const long long*>(idx), n_idx, n_case_params,
                                     frame_dtype == FNO_ACT_BF16, inputs, label, mask, case_params, h, wd, S(stream)),
@@ -1281,6 +1482,8 @@ int fno_grid_gather_window(const void* frames_in, const void* frames_out, const 
   FNO_TRY(gather_window_args("fno_grid_gather_window", frames_in, frames_out, case_table, case_ids, idx, n_idx,
                              n_case_params, frame_dtype, inputs, mask, case_params, steps, time_step_size, n_frames,
                              labels_seq));
+  FNO_TRY(gather_align("fno_grid_gather_window", frames_in, frames_out, case_table, case_ids, idx, frame_dtype, inputs, label,
+                       mask, case_params, labels_seq, false));
   FNO_CUDA(launch_grid_gather_window(frames_in, frames_out, case_table, reinterpret_cast<const int*>(case_ids),
                                      reinterpret_cast<const long long*>(idx), n_idx, n_case_params,
                                      frame_dtype == FNO_ACT_BF16, inputs, label, mask, case_params, steps, time_step_size,
@@ -1294,6 +1497,11 @@ int fno_add_input_noise(float* inputs, const float* mask, const int64_t* idx, in
   FNO_TRY(grid_arg("fno_add_input_noise", h, wd));
   if (!inputs || !mask || !idx || !step_base || n <= 0 || !(std >= 0.f) || !isfinite(std))
     return fail(kErrArg, "fno_add_input_noise: bad argument");
+  FNO_ALIGN("fno_add_input_noise", inputs, 4);   // float4 only where both frames are 16-byte aligned
+  FNO_ALIGN("fno_add_input_noise", mask, 4);
+  FNO_ALIGN("fno_add_input_noise", idx, 8);
+  FNO_ALIGN("fno_add_input_noise", step_base, 8);
+  FNO_ALIGN("fno_add_input_noise", step_offset, 4);
   FNO_CUDA(launch_add_input_noise(inputs, mask, reinterpret_cast<const long long*>(idx), n, h, wd, std, seed,
                                   reinterpret_cast<const long long*>(step_base), reinterpret_cast<const int*>(step_offset),
                                   S(stream)),
@@ -1308,6 +1516,12 @@ int fno_add_input_noise_stream(const float* in, float* out, const float* mask, c
   if (!in || !out || !mask || !idx || !step_base || n <= 0 || !(std >= 0.f) || !isfinite(std) || noise_stream < 0 ||
       noise_stream >= FNO_NOISE_STREAMS)
     return fail(kErrArg, "fno_add_input_noise_stream: bad argument");
+  FNO_ALIGN("fno_add_input_noise_stream", in, 4);   // float4 only where the frames are 16-byte aligned
+  FNO_ALIGN("fno_add_input_noise_stream", out, 4);
+  FNO_ALIGN("fno_add_input_noise_stream", mask, 4);
+  FNO_ALIGN("fno_add_input_noise_stream", idx, 8);
+  FNO_ALIGN("fno_add_input_noise_stream", step_base, 8);
+  FNO_ALIGN("fno_add_input_noise_stream", step_offset, 4);
   FNO_CUDA(launch_input_noise_stream(in, out, mask, reinterpret_cast<const long long*>(idx), n, h, wd, std, seed,
                                      reinterpret_cast<const long long*>(step_base), reinterpret_cast<const int*>(step_offset),
                                      noise_stream, S(stream)),
@@ -1319,6 +1533,11 @@ int fno_eval_sums(const float* preds, const float* label, const float* mask, con
                   int h, int wd, void* stream) {
   FNO_TRY(grid_arg("fno_eval_sums", h, wd));
   if (!preds || !label || !mask || !inputs || !sums || batch <= 0) return fail(kErrArg, "fno_eval_sums: bad argument");
+  FNO_ALIGN("fno_eval_sums", preds, 4);
+  FNO_ALIGN("fno_eval_sums", label, 4);
+  FNO_ALIGN("fno_eval_sums", mask, 4);
+  FNO_ALIGN("fno_eval_sums", inputs, 4);
+  FNO_ALIGN("fno_eval_sums", sums, 4);
   FNO_CUDA(launch_eval_sums(preds, label, mask, inputs, sums, batch, h, wd, S(stream)), "eval_sums_kernel");
   return kOk;
 }
@@ -1343,10 +1562,12 @@ int fno_window_metrics(const float* preds_seq, const void* frames_in, const void
                        void* stream) {
   FNO_TRY(window_metrics_args("fno_window_metrics", preds_seq, frames_in, frames_out, starts, steps, batch, time_step_size,
                               n_frames, frame_dtype, sums));
-  const uintptr_t frame_align = frame_dtype == FNO_ACT_BF16 ? 7 : 15;   // the 64x64 kernel's vector loads
-  if ((reinterpret_cast<uintptr_t>(preds_seq) & 15) ||
-      ((reinterpret_cast<uintptr_t>(frames_in) | reinterpret_cast<uintptr_t>(frames_out)) & frame_align))
-    return fail(kErrArg, "fno_window_metrics: preds_seq must be 16-byte aligned, the frames 16-byte (fp32) or 8-byte (bf16)");
+  // the 64x64 kernel's vector loads: float4 predictions, four frame elements at a time
+  FNO_ALIGN("fno_window_metrics", preds_seq, 16);
+  FNO_ALIGN("fno_window_metrics", frames_in, frame_vec_bytes(frame_dtype));
+  FNO_ALIGN("fno_window_metrics", frames_out, frame_vec_bytes(frame_dtype));
+  FNO_ALIGN("fno_window_metrics", starts, 8);
+  FNO_ALIGN("fno_window_metrics", sums, 4);
   FNO_CUDA(launch_window_metrics(preds_seq, frames_in, frames_out, reinterpret_cast<const long long*>(starts), steps, batch,
                                  time_step_size, n_frames, frame_dtype == FNO_ACT_BF16, sums, S(stream)),
            "window_metrics_kernel");
@@ -1359,6 +1580,11 @@ int fno_grid_window_metrics(const float* preds_seq, const void* frames_in, const
   FNO_TRY(grid_arg("fno_grid_window_metrics", h, wd));
   FNO_TRY(window_metrics_args("fno_grid_window_metrics", preds_seq, frames_in, frames_out, starts, steps, batch,
                               time_step_size, n_frames, frame_dtype, sums));
+  FNO_ALIGN("fno_grid_window_metrics", preds_seq, 4);
+  FNO_ALIGN("fno_grid_window_metrics", frames_in, frame_dtype == FNO_ACT_BF16 ? 2u : 4u);
+  FNO_ALIGN("fno_grid_window_metrics", frames_out, frame_dtype == FNO_ACT_BF16 ? 2u : 4u);
+  FNO_ALIGN("fno_grid_window_metrics", starts, 8);
+  FNO_ALIGN("fno_grid_window_metrics", sums, 4);
   FNO_CUDA(launch_grid_window_metrics(preds_seq, frames_in, frames_out, reinterpret_cast<const long long*>(starts), steps,
                                       batch, time_step_size, n_frames, frame_dtype == FNO_ACT_BF16, sums, h, wd, S(stream)),
            "window_metrics_kernel");

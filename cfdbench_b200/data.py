@@ -56,8 +56,9 @@ class DeviceFrames:
         _check_grid(split.height, split.width)
         self.n, self.height, self.width, self.n_case_params = split.n, split.height, split.width, split.n_case_params
         self.device, self.frame_dtype = dev, frame_dtype
-        self.frames_in = dataset.inputs.to(device=dev, dtype=frame_dtype).contiguous()
-        self.frames_out = dataset.labels.to(device=dev, dtype=frame_dtype).contiguous()
+        from . import _lib
+        self.frames_in = _lib.aligned(dataset.inputs.to(device=dev, dtype=frame_dtype))   # the gathers' vector reads
+        self.frames_out = _lib.aligned(dataset.labels.to(device=dev, dtype=frame_dtype))
         self.case_table = torch.from_numpy(case_table(dataset.case_params)).to(dev)
         self.case_ids = torch.as_tensor(split.case_ids, dtype=torch.int32, device=dev)
         self._case_ids_host = split.case_ids   # for the window checks, without a device read

@@ -168,7 +168,7 @@ class _TrainFn(torch.autograd.Function):
         need = ctx.needs_input_grad   # (model, inputs, mask, case_params, *params)
         d_inputs = torch.empty_like(inputs) if need[1] else None
         d_cp = torch.empty_like(case_params) if need[3] else None
-        grads = model._native_backward(inputs, mask, case_params, dpreds.contiguous().float(), ctx.saved_native,
+        grads = model._native_backward(inputs, mask, case_params, _lib.aligned(dpreds.float()), ctx.saved_native,
                                        any(need[4:]), d_inputs, d_cp)
         ctx.saved_native = None   # the saved activations (up to 1.2 GB at B=256) are released with the first backward
         if grads is None:
@@ -200,7 +200,7 @@ class _RolloutFn(torch.autograd.Function):
         need = ctx.needs_input_grad   # (model, inputs, mask, case_params, steps, noise, *params)
         d_inputs = torch.empty_like(inputs) if need[1] else None
         d_cp = torch.empty_like(case_params) if need[3] else None
-        grads = model._native_rollout_backward(inputs, mask, case_params, seq, dseq.contiguous().float(), ctx.steps,
+        grads = model._native_rollout_backward(inputs, mask, case_params, seq, _lib.aligned(dseq.float()), ctx.steps,
                                                any(need[6:]), d_inputs, d_cp, ctx.noise, fed)
         if grads is None:
             grads = [None] * (len(need) - 6)
@@ -431,14 +431,15 @@ class Fno2d(AutoCfdModel):
         return _Route(gh, gw, True, _lib.ACT_F32)
 
     def _prep_inputs(self, inputs: Tensor, case_params: Tensor, mask: Optional[Tensor]):
-        """Inputs, case parameters and the (B, 1, H, W) mask as contiguous float32 device tensors; the mask follows the
-        input's grid, which `_route` checks."""
+        """Inputs, case parameters and the (B, 1, H, W) mask as contiguous, 16-byte aligned float32 device tensors
+        (`_lib.aligned`: a view that starts inside its storage is copied); the mask follows the input's grid, which
+        `_route` checks."""
         if inputs.dim() != 4 or inputs.shape[1] != self.in_chan:
             raise ValueError(f"inputs must be (B,{self.in_chan},H,W); got {tuple(inputs.shape)}")
         gh, gw = self._route(*inputs.shape[-2:])[:2]
         b = inputs.shape[0]
         dev = self.device
-        inputs = inputs.to(device=dev, dtype=torch.float32, non_blocking=True).contiguous()
+        inputs = _lib.aligned(inputs.to(device=dev, dtype=torch.float32, non_blocking=True))
         if case_params.shape != (b, self.n_case_params):
             raise ValueError(f"case_params must be ({b},{self.n_case_params}); got {tuple(case_params.shape)}")
         case_params = case_params.to(device=dev, dtype=torch.float32, non_blocking=True).contiguous()
@@ -448,7 +449,7 @@ class Fno2d(AutoCfdModel):
             mask4 = mask.unsqueeze(1) if mask.dim() == 3 else mask
             if tuple(mask4.shape) != (b, 1, gh, gw):
                 raise ValueError(f"mask must be (B,{gh},{gw}) or (B,1,{gh},{gw}); got {tuple(mask.shape)}")
-            mask4 = mask4.to(device=dev, dtype=torch.float32, non_blocking=True).contiguous()
+            mask4 = _lib.aligned(mask4.to(device=dev, dtype=torch.float32, non_blocking=True))
         return inputs, case_params, mask4
 
     def _coords(self, pk: dict, gh: int, gw: int) -> tuple:

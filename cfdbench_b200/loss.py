@@ -26,8 +26,8 @@ class _NativeLoss(torch.autograd.Function):
     def forward(ctx, preds: Tensor, labels: Tensor) -> Tensor:
         from . import _lib
         lib = _lib.load()
-        p = preds.detach().contiguous().float()
-        l = labels.detach().contiguous().float()
+        p = _lib.aligned(preds.detach().float())   # fno_loss_fwd reads both as float4
+        l = _lib.aligned(labels.detach().float())
         if p.shape != l.shape:
             raise ValueError(f"preds {tuple(p.shape)} and labels {tuple(l.shape)} differ")
         dev = p.device

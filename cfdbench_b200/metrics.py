@@ -83,9 +83,9 @@ def multistep_metrics(preds: Union[Tensor, Sequence[Tensor]], label_u: Tensor, m
                          f"{tuple(label_u.shape)}, {tuple(mask.shape)}")
     if preds.device.type != "cuda":
         raise _lib.FnoNativeError("multistep_metrics has no CPU path: pass CUDA tensors")
-    preds = preds.contiguous().float()
-    label_u = label_u.to(preds.device).contiguous().float()
-    mask = mask.to(preds.device).contiguous().float()
+    preds = _lib.aligned(preds.float())
+    label_u = _lib.aligned(label_u.to(preds.device).float())
+    mask = _lib.aligned(mask.to(preds.device).float())
     sums = torch.empty(s, b, 3, dtype=torch.float32, device=preds.device)
     _launch_metrics(preds, label_u, mask, sums)
     host = sums.double().cpu()  # the only synchronisation
@@ -137,8 +137,8 @@ def infer_multistep(model, all_features: Sequence[Union[Tensor, np.ndarray]], al
             cp = torch.stack([p.to(device=dev, dtype=torch.float32).reshape(-1) for p in all_case_params[lo:hi]])
             preds = model.generate_many(inputs=fr[:, 0, :2], case_params=cp, mask=fr[:, 0, 2], steps=s)
             preds = torch.stack(preds)                             # (S, B, 2, H, W)
-            label_u = fr[:, :, 0].transpose(0, 1).contiguous()     # (S, B, H, W): frame s of each case
-            mask = fr[:, :, 2].transpose(0, 1).contiguous()
+            label_u = _lib.aligned(fr[:, :, 0].transpose(0, 1))     # (S, B, H, W): frame s of each case
+            mask = _lib.aligned(fr[:, :, 2].transpose(0, 1))
             _launch_metrics(preds, label_u, mask, sums[s * lo * 3:s * hi * 3])
     host = sums.double().cpu().numpy()   # the only synchronisation
     per_case = _per_case(_chunked_sums(host, s, n, max_batch), gh * gw)   # (S, n) each
