@@ -337,15 +337,6 @@ __global__ void __launch_bounds__(kFzThreads, 1)
 // ------------------------------------------------------------------------------------------------
 void c2r_operand_table(float* host, double s0, double s1);
 
-static float fz_round_tf32_host(double v) {
-  float f = static_cast<float>(v);
-  uint32_t u;
-  memcpy(&u, &f, 4);
-  u = (u + 0x1000u) & 0xffffe000u;
-  memcpy(&f, &u, 4);
-  return f;
-}
-
 struct FzTables {
   float* etab = nullptr;
   float* ftab = nullptr;
@@ -368,10 +359,10 @@ static cudaError_t fz_ensure(int dev, cudaStream_t stream) {
         const int rip = k & 1, kxi = 2 * ((k % 24) >> 1) + k / 24, kx = kxi < kM1 ? kxi : kxi + (kH - kKX);
         const double ang = two_pi * ((kx * h) % 64) / 64.0;
         const double val = (ri == rip) ? cos(ang) : (ri == 0 ? -sin(ang) : sin(ang));
-        const float hi = fz_round_tf32_host(val);
+        const float hi = tc::round_tf32(static_cast<float>(val));
         const uint32_t off = tc::kmajor_offset(n, k, 2 * kFzRows) / 4;
         h_f[c * kFzFFloats + off] = hi;
-        h_f[c * kFzFFloats + kFzFFloats / 2 + off] = fz_round_tf32_host(val - static_cast<double>(hi));
+        h_f[c * kFzFFloats + kFzFFloats / 2 + off] = tc::round_tf32(static_cast<float>(val - static_cast<double>(hi)));
       }
     }
   cudaError_t e = cudaMalloc(&t.etab, sizeof(h_e));

@@ -258,15 +258,6 @@ __global__ void __launch_bounds__(kBtThreads, 1)
 // the conv bias, which folds the bias add into the MMA.  Built in float64, split into tf32 hi/lo (round-to-nearest),
 // laid out K-major: hi image then lo image.  Also the constant of block_fused_kernel (with s0 = 1/HW, s1 = 2/HW).
 // ------------------------------------------------------------------------------------------------
-static float round_tf32_host(double v) {
-  float f = static_cast<float>(v);
-  uint32_t u;
-  memcpy(&u, &f, 4);
-  u = (u + 0x1000u) & 0xffffe000u;  // round half away from zero on the magnitude (cvt.rna)
-  memcpy(&f, &u, 4);
-  return f;
-}
-
 void c2r_operand_table(float* host, double s0, double s1) {
   for (int i = 0; i < kETabFloats; ++i) host[i] = 0.f;
   for (int w = 0; w < kBtM; ++w)
@@ -275,8 +266,8 @@ void c2r_operand_table(float* host, double s0, double s1) {
       const double c = ky == 0 ? s0 : s1;
       const double val[2] = {c * cos(ang), ky == 0 ? 1.0 : -c * sin(ang)};  // ky = 0, ri = 1: the bias column
       for (int ri = 0; ri < 2; ++ri) {
-        const float hi = round_tf32_host(val[ri]);
-        const float lo = round_tf32_host(val[ri] - static_cast<double>(hi));
+        const float hi = tc::round_tf32(static_cast<float>(val[ri]));
+        const float lo = tc::round_tf32(static_cast<float>(val[ri] - static_cast<double>(hi)));
         const uint32_t off = tc::kmajor_offset(w, 2 * ky + ri, kBtM) / 4;
         host[off] = hi;
         host[kBtM * kKE + off] = lo;

@@ -215,14 +215,6 @@ static double td_bf16_value(uint16_t b) {
   memcpy(&f, &u, 4);
   return static_cast<double>(f);
 }
-static float td_round_tf32(double v) {
-  float f = static_cast<float>(v);
-  uint32_t u;
-  memcpy(&u, &f, 4);
-  u = (u + 0x1000u) & 0xffffe000u;
-  memcpy(&f, &u, 4);
-  return f;
-}
 
 struct TdTables {
   unsigned char* ta = nullptr;
@@ -260,9 +252,9 @@ static cudaError_t td_ensure(int dev, cudaStream_t stream) {
         const double ang = two_pi * ((kx * h) % 64) / 64.0;
         const double val = cs ? sin(ang) : cos(ang);
         const uint32_t off = tc::kmajor_offset(2 * kxi + cs, h, kTdN2) / 4;
-        const float hi = td_round_tf32(val);
+        const float hi = tc::round_tf32(static_cast<float>(val));
         h_t[off] = hi;
-        h_t[kTdTFloats + off] = td_round_tf32(val - static_cast<double>(hi));
+        h_t[kTdTFloats + off] = tc::round_tf32(static_cast<float>(val - static_cast<double>(hi)));
       }
   }
   cudaError_t e = cudaMalloc(&t.ta, sizeof(h_ta));

@@ -1,5 +1,5 @@
 // Hopper (sm_90a) tensor-core primitives used by the wgmma kernels: shared-memory matrix descriptors, warpgroup MMA
-// (wgmma.mma_async) wrappers for the shapes the kernels issue, and the tf32 hi/lo split of 3xTF32.
+// (wgmma.mma_async) wrappers for the shapes the kernels issue, and (from tf32_round.cuh) the tf32 hi/lo split of 3xTF32.
 //
 // Operand layout ("canonical K-major, no swizzle"): the matrix is tiled in core matrices of 8 rows (M or N) x 16 bytes
 // (4 tf32 / 8 bf16 along K), each stored as 128 contiguous bytes (row r at r*16 B).  SBO = byte distance between core
@@ -12,6 +12,8 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include "tf32_round.cuh"  // round_tf32 / split_tf32
 
 namespace fno {
 namespace tc {
@@ -145,20 +147,6 @@ __device__ __forceinline__ void stmatrix_x4_trans(uint32_t saddr, const uint32_t
 // core matrix (row/8, k/4) at ((k/4) * (rows/8) + row/8) * 128
 __host__ __device__ constexpr uint32_t kmajor_offset(int row, int k, int rows) {
   return static_cast<uint32_t>(((k >> 2) * (rows >> 3) + (row >> 3)) * 128 + (row & 7) * 16 + (k & 3) * 4);
-}
-// hi/lo split for 3xTF32.  The tensor core TRUNCATES the low 13 mantissa bits of what it reads, which
-// would bias every product; so both parts are rounded to nearest tf32 here (cvt.rna) and the hardware
-// truncation is then a no-op: hi = rna(x), lo = rna(x - hi), |x - hi - lo| <= 2^-22 |x|, unbiased.
-// Round-to-nearest (ties away from zero, like cvt.rna.tf32.f32) as two integer ops on the bit pattern: add half an
-// ulp of the 10-bit mantissa, clear the 13 low bits.  ptxas expands cvt.rna into ~5 instructions because it also
-// preserves NaN/Inf payloads; activations and weights here are finite, and Inf/NaN still map to Inf/NaN (the
-// exponent field is untouched unless the mantissa carry overflows a value within 2^-11 of FLT_MAX).
-__device__ __forceinline__ float round_tf32(float x) {
-  return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xffffe000u);
-}
-__device__ __forceinline__ void split_tf32(float x, float& hi, float& lo) {
-  hi = round_tf32(x);
-  lo = round_tf32(x - hi);
 }
 
 }  // namespace tc

@@ -432,34 +432,39 @@ def test_non_finite_neighbour(grid, act):
 def _poisoned_batch(grid, b):
     bad = _batch(grid, b)
     bad["inputs"][1, 0, 9, 17] = float("nan")
-    bad["inputs"][1, 1, 30, 40] = float("inf")
+    bad["inputs"][1, 1, min(30, grid[0] - 2), min(40, grid[1] - 2)] = float("inf")
     bad["case_params"][b - 2, 0] = float("nan")
     return bad, [1, b - 2]
 
 
-# tc::round_tf32 (tc_common.cuh) rounds by adding 0x1000 to the bit pattern: the canonical NaN 0x7fffffff that arithmetic
-# produces carries into the sign bit and comes out as -0.0 (0xffffffff as +0.0).  Every 3xTF32 / bf16 tensor-core stage
-# splits its operands through it -- mode_mix_tc, block_tc, project_tc and the second GEMM of dft_fwd_tc -- so a NaN
-# sample turns into a finite one there (measured: layer 0's modes are NaN, its pre-activation finite in fp32 storage; in
-# bf16 storage dft_fwd_tc already returns finite modes).  Fixing it changes those kernels' code, which is left to its own
-# change; until then the element check below fails with an AssertionError.
-@pytest.mark.xfail(raises=AssertionError, strict=False,
-                   reason="tc::round_tf32 turns the canonical NaN 0x7fffffff into -0.0, so the tensor-core stages swallow "
-                          "a NaN sample")
-@pytest.mark.parametrize("act", ["float32", "bfloat16"])
-def test_non_finite_sample_surfaces(act):
-    """The poisoned samples' predictions are non-finite wherever the float64 oracle's are."""
-    b = _tile_batch("ragged")
+# A NaN or Inf in a sample has to reach that sample's predictions on every route.  The DFT spreads one non-finite pixel
+# over all of a plane's modes, so from the first Fourier layer on the oracle's poisoned samples are non-finite
+# throughout; every later stage -- the 3xTF32 / bf16 tensor-core stages of the 64 x 64 path included, whose operand split
+# tc::round_tf32 keeps NaN a NaN -- must carry that through, in one forward, in generate_many's feedback and in
+# Fno2d.rollout.  test_gpu_non_finite checks the same stage by stage, element by element.
+@pytest.mark.parametrize("grid, act", [((64, 64), "float32"), ((64, 64), "bfloat16"), ((66, 65), "float32"),
+                                       ((25, 127), "float32")], ids=["64-f32", "64-bf16", "66x65", "25x127"])
+def test_non_finite_sample_surfaces(grid, act):
+    """The poisoned samples' predictions are non-finite wherever the float64 oracle's are: forward, generate_many and
+    Fno2d.rollout, two steps."""
+    b = _tile_batch("ragged") if grid == (64, 64) else 33
+    steps = 2
     m, sd = _model(act)
-    bad, hit = _poisoned_batch((64, 64), b)
+    bad, hit = _poisoned_batch(grid, b)
+    x, c, mk = bad["inputs"], bad["case_params"], bad["mask"]
     with torch.no_grad():
-        zp = m(inputs=bad["inputs"], case_params=bad["case_params"], mask=bad["mask"])["preds"][hit].cpu().numpy()
+        got = {"forward": m(inputs=x, case_params=c, mask=mk)["preds"][hit][None],
+               "generate_many": torch.stack(m.generate_many(x, c, mk, steps))[:, hit],
+               "rollout": m.rollout(x, c, mk, steps)[:, hit]}
     bn = {k: v[hit].cpu().numpy() for k, v in bad.items()}
     with np.errstate(invalid="ignore", over="ignore"):
-        r = onp.fno_forward(sd, bn["inputs"], bn["case_params"], bn["mask"][:, None])["preds"]
-    if np.isfinite(r).all():
+        r = np.stack(onp.rollout(sd, bn["inputs"], bn["case_params"], bn["mask"], steps))
+    if np.isfinite(r[0]).all():
         pytest.fail("the oracle's predictions of the poisoned samples are finite: the set-up is wrong")
-    assert (~np.isfinite(zp))[~np.isfinite(r)].all(), "an element the oracle makes non-finite came out finite"
+    for what, t in got.items():
+        z = t.float().cpu().numpy()
+        assert (~np.isfinite(z))[~np.isfinite(r[:len(z)])].all(), \
+            f"{what}: an element the oracle makes non-finite came out finite"
 
 
 
