@@ -10,6 +10,7 @@ Public surface mirrors the reference's for this path:
                                             dev_rollout_steps=S selects checkpoints by it)
     train_auto                             (reference src/train_auto.py train, steps replayed from CUDA graphs;
                                             rollout_steps=K trains through K-step rollouts)
+    unroll_lengths                         (the per-step prefix lengths of train_auto(random_unroll=True))
     rollout_windows                        (the valid K-step window starts of a split)
     RolloutNoise, add_input_noise          (per-step input noise of Fno2d.rollout, and its eager form)
 """
@@ -17,7 +18,7 @@ from .base_model import AutoCfdModel
 from .loss import MseLoss, loss_name_to_fn
 
 __all__ = ["AutoCfdModel", "MseLoss", "loss_name_to_fn", "Fno2d", "FnoBlock", "SpectralConv2d_fast", "FusedAdam", "DeviceFrames",
-           "infer_multistep", "evaluate_auto", "evaluate_rollout_auto", "train_auto",
+           "infer_multistep", "evaluate_auto", "evaluate_rollout_auto", "train_auto", "unroll_lengths",
            "rollout_windows", "RolloutNoise", "add_input_noise"]
 
 
@@ -43,7 +44,7 @@ def __getattr__(name):  # lazy: importing the package must not require the nativ
     if name in ("rollout_windows", "RolloutNoise", "add_input_noise"):
         from . import data
         return getattr(data, name)
-    if name == "train_auto":
-        from .train import train_auto
-        return train_auto
+    if name in ("train_auto", "unroll_lengths"):
+        from . import train
+        return getattr(train, name)
     raise AttributeError(name)

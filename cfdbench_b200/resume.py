@@ -15,6 +15,7 @@ last epoch.  It loads with `torch.load(..., weights_only=True)`: tensors, number
     train_losses  every step's loss so far
     grad_norms    every step's pre-clip gradient norm so far (with max_grad_norm only)
     config        run_config(...): every setting the trajectory or the checkpoint scores depend on, compared on resume
+                  (random_unroll and unroll_seed only in the record of a random_unroll=True run)
 """
 from __future__ import annotations
 

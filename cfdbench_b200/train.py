@@ -15,6 +15,7 @@ synchronisation.  The result is bit-identical to the eager loop `DeviceFrames.lo
     train_auto(model, train_data, dev_data, output_dir, num_epochs=..., lr=..., batch_size=...)   # for train(...)
     train_auto(..., rollout_steps=4)   # trained through 4-step rollouts of the model's own predictions
     train_auto(..., rollout_steps=4, rollout_grad_steps=1)   # pushforward: 3 steps without gradient, the 4th trained
+    train_auto(..., rollout_steps=4, rollout_grad_steps=1, random_unroll=True)   # ... 0 to 3 of them, drawn per step
     train_auto(..., input_noise_std=0.01, noise_seed=1)      # Gaussian noise on every step's input frame
     train_auto(..., rollout_steps=4, input_noise_std=0.01, noise_every_step=True)   # ... and on every rollout step's
     train_auto(..., resumable=True)   # relaunching the same call continues an interrupted run bit for bit
@@ -68,6 +69,15 @@ def index_stream(n: int, batch_size: int, num_epochs: int, eval_interval: int, g
         if (ep + 1) % eval_interval == 0:
             dev_eval_draw(generator)
     return out
+
+
+def unroll_lengths(unroll_seed: int, first_step: int, n: int, max_prefix: int) -> np.ndarray:
+    """The prefix lengths `train_auto(random_unroll=True)` draws for Adam's 1-based steps first_step ..
+    first_step + n - 1 (int64): step t runs `np.random.default_rng((unroll_seed, t)).integers(0, max_prefix + 1)`
+    inference steps before its trained ones.  A pure function of (unroll_seed, t, max_prefix), so a resumed run draws
+    what the uninterrupted one drew, whatever the epochs and batches."""
+    return np.asarray([np.random.default_rng((unroll_seed, t)).integers(0, max_prefix + 1)
+                       for t in range(first_step, first_step + n)], dtype=np.int64)
 
 
 def dump_json(data, path) -> None:   # reference src/utils/common.py:23-25
@@ -139,12 +149,21 @@ class _StepGraphs:
         self.adam_arr = (_lib.FnoAdamTensors * len(self.adam))(*self.adam)   # the norm launch's tables
         self.betas, self.eps, self.weight_decay = group["betas"], group["eps"], group["weight_decay"]
 
-        # capture: a warm-up of every launch except Adam and the log (it updates nothing: parameters, optimizer state
-        # and cursor stay as they are), then one capture per batch size
         with torch.no_grad(), side_stream(dev):
-            for b in self.sizes:
-                self._issue(b, update=False)
-            self.graphs = [capture_graph(lambda b=b: self._issue(b, update=True)) for b in self.sizes]
+            self.graphs = self._capture()
+
+    def _capture(self) -> list:
+        """A warm-up of every launch except Adam and the log (it updates nothing: parameters, optimizer state and cursor
+        stay as they are), then one capture per batch size."""
+        for b in self.sizes:
+            self._issue(b, update=False)
+        return [capture_graph(lambda b=b: self._issue(b, update=True)) for b in self.sizes]
+
+    def _replay(self, first_step: int) -> None:
+        """The epoch's replays: each graph `count` times, in the order of `sizes`."""
+        for g, count in zip(self.graphs, self.counts):
+            for _ in range(count):
+                g.replay()
 
     def _make_io(self, bmax: int, gh: int, gw: int, p: int) -> dict:
         """The static buffers of the step graphs."""
@@ -252,9 +271,7 @@ class _StepGraphs:
             self.step_base_host[0] = first_step
             io["step_base"].copy_(self.step_base_host, non_blocking=True)
         io["cursor"].zero_()
-        for g, count in zip(self.graphs, self.counts):
-            for _ in range(count):
-                g.replay()
+        self._replay(first_step)
         if self.max_grad_norm is not None:   # complete once the log below has come back
             self.norm_host.copy_(io["norm_log"], non_blocking=True)
         log = io["log"].cpu().numpy()   # the epoch's one synchronisation
@@ -287,14 +304,20 @@ class _RolloutStepGraphs(_StepGraphs):
     noise_every_step (with noise_std > 0): rollout step s of the window (prefix and trained steps alike) is fed its
     input plus the noise of stream s (the start frame keeps the gather's stream-0 noise).  The prefix and the trained
     steps run the *_noise drivers with k0 = 0 and k0 = k - g, writing the perturbed frames into (k - g, bmax, ...) and
-    (g, bmax, ...) fed-frame buffers: k more frames per sample than without, and one more launch per rollout step."""
+    (g, bmax, ...) fed-frame buffers: k more frames per sample than without, and one more launch per rollout step.
+
+    random_unroll (g < k): Adam's step t runs u_t = unroll_lengths(unroll_seed, t, 1, k - g)[0] prefix steps instead of
+    k - g, and trains steps u_t .. u_t + g - 1 of the window (u_t = 0: no prefix launch, the start frame is trained).
+    One step is captured per u in 0 .. k - g and batch size, every capture on the same buffers (the prefix buffer holds
+    the longest prefix); the epoch replays the graph of each step's u_t."""
 
     def __init__(self, model, frames: DeviceFrames, batch_size: int, optimizer, n_windows: int, steps: int,
                  time_step_size: int, grad_steps: Optional[int] = None, noise_std: float = 0.0, noise_seed: int = 0,
-                 noise_every_step: bool = False):
+                 noise_every_step: bool = False, random_unroll: bool = False, unroll_seed: int = 0):
         self.k, self.tss = steps, time_step_size
         self.g = steps if grad_steps is None else grad_steps
         self.every = noise_every_step and noise_std > 0
+        self.random_unroll, self.unroll_seed = random_unroll, unroll_seed
         super().__init__(model, frames, batch_size, optimizer, n=n_windows, noise_std=noise_std, noise_seed=noise_seed)
 
     def _make_io(self, bmax: int, gh: int, gw: int, p: int) -> dict:
@@ -327,8 +350,30 @@ class _RolloutStepGraphs(_StepGraphs):
         return C.byref(_lib.FnoNoise(self.noise_std, self.noise_seed, io["idx"].data_ptr(), io["step_base"].data_ptr(),
                                      io["cursor"].data_ptr(), k0))
 
-    def _issue(self, b: int, update: bool) -> None:
+    def _capture(self) -> list:
+        """Without random_unroll, _StepGraphs' graphs; with it, graphs[u][i]: prefix length u, batch size sizes[i]."""
+        if not self.random_unroll:
+            return super()._capture()
+        us = range(self.k - self.g + 1)
+        for u in us:
+            for b in self.sizes:
+                self._issue(b, update=False, u=u)
+        return [[capture_graph(lambda b=b, u=u: self._issue(b, update=True, u=u)) for b in self.sizes] for u in us]
+
+    def _replay(self, first_step: int) -> None:
+        if not self.random_unroll:
+            return super()._replay(first_step)
+        # drawn step by step (about 30 us each), so that the host draws step t + 1 while the device runs step t
+        t = first_step
+        for i, count in enumerate(self.counts):
+            for _ in range(count):
+                self.graphs[int(unroll_lengths(self.unroll_seed, t, 1, self.k - self.g)[0])][i].replay()
+                t += 1
+
+    def _issue(self, b: int, update: bool, u: Optional[int] = None) -> None:
+        """u: the prefix length (default k - g)."""
         lib, io, sw, route, k, g = self.lib, self.io, self.sw, self.route, self.k, self.g
+        u = k - g if u is None else u
         st = C.c_void_p(torch.cuda.current_stream(self.dev).cuda_stream)
         self._stage_indices(b, st)
         _gather(self.frames, io["idx"], b, io["inputs"], None, io["mask"], io["cp"], st,
@@ -339,18 +384,18 @@ class _RolloutStepGraphs(_StepGraphs):
         preds, labels, dpreds = io["preds"].data_ptr(), io["labels"].data_ptr(), io["dpreds"].data_ptr()
         ts, ws = self.ts, self.ws
         n_el = b * 2 * self.gh * self.gw   # per step
-        if g < k:   # the pushforward prefix, without gradient; the trained steps start from its last frame
+        if u > 0:   # the pushforward prefix, without gradient; the trained steps start from its last frame
             pre = io["prefix"].data_ptr()
             if self.every:
-                route.call("rollout_noise", C.byref(sw["struct"]), x, mk, cp, pre, k - g, C.byref(ws), self._noise(0),
+                route.call("rollout_noise", C.byref(sw["struct"]), x, mk, cp, pre, u, C.byref(ws), self._noise(0),
                            io["fed_prefix"].data_ptr(), b, st)
             else:
-                route.call("rollout", C.byref(sw["struct"]), x, mk, cp, pre, k - g, C.byref(ws), b, st)
-            x = pre + (k - g - 1) * n_el * 4
-            labels += (k - g) * n_el * 4
+                route.call("rollout", C.byref(sw["struct"]), x, mk, cp, pre, u, C.byref(ws), b, st)
+            x = pre + (u - 1) * n_el * 4
+            labels += u * n_el * 4
         if self.every:
             route.call("rollout_forward_train_noise", C.byref(sw["struct"]), x, mk, cp, preds, g, C.byref(ts["sv"]),
-                       C.byref(ws), self._noise(k - g), io["fed"].data_ptr(), b, st)
+                       C.byref(ws), self._noise(u), io["fed"].data_ptr(), b, st)
         else:
             route.call("rollout_forward_train", C.byref(sw["struct"]), x, mk, cp, preds, g, C.byref(ts["sv"]),
                        C.byref(ws), b, st)
@@ -361,7 +406,7 @@ class _RolloutStepGraphs(_StepGraphs):
         if self.every:
             route.call("rollout_backward_noise", C.byref(sw["struct"]), C.byref(sw["struct_bwd"]), x, mk, cp, preds,
                        dpreds, g, C.byref(ts["sv"]), C.byref(self.grads), C.byref(ts["sc"]), C.byref(ws),
-                       self._noise(k - g), io["fed"].data_ptr(), io["carry"].data_ptr(), None, None, b, st)
+                       self._noise(u), io["fed"].data_ptr(), io["carry"].data_ptr(), None, None, b, st)
         else:
             route.call("rollout_backward", C.byref(sw["struct"]), C.byref(sw["struct_bwd"]), x, mk, cp, preds, dpreds,
                        g, C.byref(ts["sv"]), C.byref(self.grads), C.byref(ts["sc"]), C.byref(ws), io["carry"].data_ptr(),
@@ -392,7 +437,8 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
                time_step_size: Optional[int] = None, input_noise_std: float = 0.0, noise_seed: int = 0,
                rollout_grad_steps: Optional[int] = None, noise_every_step: bool = False,
                dev_rollout_steps: Optional[int] = None, max_grad_norm: Optional[float] = None,
-               ema_decay: Optional[float] = None, resumable: bool = False) -> dict:
+               ema_decay: Optional[float] = None, resumable: bool = False, random_unroll: bool = False,
+               unroll_seed: int = 0) -> dict:
     """What the reference's `train(model, train_data, dev_data, output_dir, ...)` does (src/train_auto.py:181-313), with
     its argument names and defaults, every training step replayed from a CUDA graph and one synchronisation per epoch.
 
@@ -426,6 +472,16 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
       K - G run without gradient through the inference rollout (the kernels `generate_many` runs), and only the last
       G are trained, from the prefix's last frame, on (nmse_{K-G} + ... + nmse_{K-1}) / G; the log and train_losses
       hold that mean.  G = K is the full rollout above, launch for launch; with K = 1 only G = 1 is valid.
+    - random_unroll=True (needs G < K) draws the prefix length per step, as Brandstetter, Worrall & Welling's
+      pushforward trick does per batch: Adam's step t runs u_t = unroll_lengths(unroll_seed, t, 1, K - G)[0] inference
+      steps (uniform in 0 .. K - G; u_t = 0 launches no prefix) and trains the G steps after them, from prefix frame
+      u_t - 1 or the start frame, on (nmse_{u_t} + ... + nmse_{u_t+G-1}) / G.  The windows, the permutation and the
+      draws from `generator` are those of the fixed-prefix call; u_t depends on (unroll_seed, t, K - G) only, an int
+      >= 0 never drawn from `generator`.  One step graph is captured per prefix length, all on the same buffers.  With
+      input noise the start frame is perturbed as above; with noise_every_step the prefix runs k0 = 0 over u_t steps
+      and the trained steps k0 = u_t (window step k is fed noise stream k).  One step is bit-identical to the eager
+      loop of the pushforward one with u = unroll_lengths(unroll_seed, t, 1, K - G)[0] in place of K - G (INTEGRATION
+      §3).  False (the default) launches and replays exactly what runs without the option.
     - input_noise_std = sigma > 0 adds Gaussian noise to every step's (start) input frame where the mask is non-zero,
       `DeviceFrames.batch(..., noise_std=sigma, noise_seed=noise_seed, noise_step=t)` with t Adam's 1-based global step
       of that update.  The noise comes from a counter-based RNG seeded by `noise_seed` (an int in [0, 2^64)), never
@@ -514,7 +570,8 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
     S-step window, or whose frames do not chain.  With resumable=True, also ValueError before any device work for a
     training_state.pt that does not load, has another format version or was written with another config (naming every
     differing field), or for an output_dir with ckpt-* directories and no training_state.pt; ValueError for a
-    resumable that is not a bool.
+    resumable that is not a bool; for a random_unroll that is not a bool, an unroll_seed that is not an int >= 0, or
+    random_unroll=True with rollout_steps = 1 or rollout_grad_steps = rollout_steps.
     Frozen parameters (requires_grad=False) are not updated, as FusedAdam.step skips them.  Data parallel training in
     this loop is not supported."""
     from .fno2d import Fno2d
@@ -540,6 +597,14 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
     if isinstance(grad_steps, bool) or not isinstance(grad_steps, (int, np.integer)) or not 1 <= grad_steps <= rollout_steps:
         raise ValueError(f"rollout_grad_steps must be an int in 1..rollout_steps={rollout_steps}, got {rollout_grad_steps!r}")
     grad_steps = int(grad_steps)
+    if not isinstance(random_unroll, bool):
+        raise ValueError(f"random_unroll must be a bool, got {random_unroll!r}")
+    if isinstance(unroll_seed, bool) or not isinstance(unroll_seed, (int, np.integer)) or unroll_seed < 0:
+        raise ValueError(f"unroll_seed must be a non-negative int, got {unroll_seed!r}")
+    if random_unroll and not grad_steps < rollout_steps:
+        raise ValueError(f"random_unroll draws the pushforward prefix length: it needs rollout_steps > 1 and "
+                         f"rollout_grad_steps < rollout_steps, got rollout_steps={rollout_steps}, "
+                         f"rollout_grad_steps={rollout_grad_steps!r}")
     if model._dp_enabled:
         raise ValueError("train_auto does not run data parallel: its step graph has no all-reduce")
     if not any(p.requires_grad for p in model.parameters()):
@@ -567,6 +632,8 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
             input_noise_std=float(input_noise_std), noise_seed=int(noise_seed), noise_every_step=noise_every_step,
             dev_rollout_steps=dev_rollout_steps, dev_time_step_size=dev_tss, max_grad_norm=max_grad_norm,
             ema_decay=ema_decay, generator=generator is not None)
+        if random_unroll:   # recorded only when set: a fixed-prefix run's record is that of earlier versions
+            config.update(random_unroll=True, unroll_seed=int(unroll_seed))
         state = resume.find_state(output_dir, config)
     model._require_cuda()
     output_dir = Path(output_dir)
@@ -601,14 +668,19 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
                 graphs = _StepGraphs(model, frames, batch_size, optimizer, **noise)
             else:
                 graphs = _RolloutStepGraphs(model, frames, batch_size, optimizer, windows.size, rollout_steps,
-                                            tss, grad_steps, noise_every_step=noise_every_step, **noise)
+                                            tss, grad_steps, noise_every_step=noise_every_step,
+                                            random_unroll=random_unroll, unroll_seed=int(unroll_seed), **noise)
         print("====== Training ======")
         print(f"# batch: {batch_size}")
         print(f"# examples: {n}")
         if windows is not None:
             print(f"# rollout steps: {rollout_steps}, windows: {windows.size}")
             if grad_steps < rollout_steps:
-                print(f"# trained steps: the last {grad_steps} (pushforward)")
+                if random_unroll:
+                    print(f"# trained steps: {grad_steps} after a random prefix of 0..{rollout_steps - grad_steps} "
+                          f"steps (pushforward, unroll seed {int(unroll_seed)})")
+                else:
+                    print(f"# trained steps: the last {grad_steps} (pushforward)")
         if input_noise_std > 0:
             every = ", on every rollout step" if noise_every_step and windows is not None else ""
             print(f"# input noise std: {input_noise_std}, seed {int(noise_seed)}{every}")
