@@ -13,13 +13,14 @@ Public surface mirrors the reference's for this path:
     unroll_lengths                         (the per-step prefix lengths of train_auto(random_unroll=True))
     rollout_windows                        (the valid K-step window starts of a split)
     RolloutNoise, add_input_noise          (per-step input noise of Fno2d.rollout, and its eager form)
+    TeacherForcing, teacher_forcing_flags  (teacher forcing of Fno2d.rollout, and its device-drawn flags)
 """
 from .base_model import AutoCfdModel
 from .loss import MseLoss, loss_name_to_fn
 
 __all__ = ["AutoCfdModel", "MseLoss", "loss_name_to_fn", "Fno2d", "FnoBlock", "SpectralConv2d_fast", "FusedAdam", "DeviceFrames",
            "infer_multistep", "evaluate_auto", "evaluate_rollout_auto", "train_auto", "unroll_lengths",
-           "rollout_windows", "RolloutNoise", "add_input_noise"]
+           "rollout_windows", "RolloutNoise", "add_input_noise", "TeacherForcing", "teacher_forcing_flags"]
 
 
 def __getattr__(name):  # lazy: importing the package must not require the native library
@@ -41,7 +42,7 @@ def __getattr__(name):  # lazy: importing the package must not require the nativ
     if name == "evaluate_rollout_auto":
         from .metrics import evaluate_rollout_auto
         return evaluate_rollout_auto
-    if name in ("rollout_windows", "RolloutNoise", "add_input_noise"):
+    if name in ("rollout_windows", "RolloutNoise", "add_input_noise", "TeacherForcing", "teacher_forcing_flags"):
         from . import data
         return getattr(data, name)
     if name in ("train_auto", "unroll_lengths"):

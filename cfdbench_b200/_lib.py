@@ -87,6 +87,11 @@ class FnoNoise(C.Structure):
                 ("step_offset", C.c_void_p), ("k0", C.c_int32)]
 
 
+class FnoTeacher(C.Structure):
+    """fno_teacher: the true frames and per-sample flags of a teacher-forced rollout driver (include/cfdbench_b200.h)."""
+    _fields_ = [("frames", C.c_void_p), ("flags", C.c_void_p)]
+
+
 NOISE_STREAMS = 2 ** 16
 
 _P = C.c_void_p
@@ -207,6 +212,22 @@ SIGNATURES = {
                                                   C.POINTER(FnoTrainSaved), C.POINTER(FnoGrads), C.POINTER(FnoBwdScratch),
                                                   C.POINTER(FnoWorkspace), C.POINTER(FnoNoise), _P, _P, _P, _P, _I, _I,
                                                   _I, _P]),
+    # teacher forcing of a rollout
+    "fno_teacher_flags": (C.c_int, [_P, _I, _I, _P, C.c_uint64, _P, _P, _P, _P]),
+    "fno_rollout_forward_train_feed": (C.c_int, [C.POINTER(FnoWeights), _P, _P, _P, _P, _I, C.POINTER(FnoTrainSaved),
+                                                 C.POINTER(FnoWorkspace), C.POINTER(FnoNoise), C.POINTER(FnoTeacher), _P,
+                                                 _I, _I, _P]),
+    "fno_rollout_backward_feed": (C.c_int, [C.POINTER(FnoWeights), C.POINTER(FnoWeightsBwd), _P, _P, _P, _P, _P, _I,
+                                            C.POINTER(FnoTrainSaved), C.POINTER(FnoGrads), C.POINTER(FnoBwdScratch),
+                                            C.POINTER(FnoWorkspace), C.POINTER(FnoNoise), C.POINTER(FnoTeacher), _P, _P, _P,
+                                            _P, _I, _I, _P]),
+    "fno_grid_rollout_forward_train_feed": (C.c_int, [C.POINTER(FnoWeights), _P, _P, _P, _P, _I, C.POINTER(FnoTrainSaved),
+                                                      C.POINTER(FnoWorkspace), C.POINTER(FnoNoise), C.POINTER(FnoTeacher),
+                                                      _P, _I, _I, _I, _P]),
+    "fno_grid_rollout_backward_feed": (C.c_int, [C.POINTER(FnoWeights), C.POINTER(FnoWeightsBwd), _P, _P, _P, _P, _P, _I,
+                                                 C.POINTER(FnoTrainSaved), C.POINTER(FnoGrads), C.POINTER(FnoBwdScratch),
+                                                 C.POINTER(FnoWorkspace), C.POINTER(FnoNoise), C.POINTER(FnoTeacher), _P,
+                                                 _P, _P, _P, _I, _I, _I, _P]),
 }
 
 GRID_MIN, GRID_MAX = 24, 128

@@ -53,7 +53,8 @@ cudaError_t launch_multistep_metrics(const float*, const float*, const float*, f
 cudaError_t launch_spectral_wgrad(const void*, const void*, void*, int, cudaStream_t);
 cudaError_t launch_lift_bwd(const float*, const float*, const float*, const float*, const float*, const float*,
                             float*, float*, float*, int, int, int, cudaStream_t);
-cudaError_t launch_lift_bwd_data(const float*, const float*, float*, float*, const float*, int, int, int, cudaStream_t);
+cudaError_t launch_lift_bwd_data(const float*, const float*, float*, float*, const float*, int, int, int, cudaStream_t,
+                                 const unsigned char*);
 // grid-generic fp32 path (fno_grid.cu)
 bool grid_ok(int, int);
 void grid_tables_release(int);
@@ -72,7 +73,8 @@ int grid_project_bwd_row();
 template <int NJ, int NI>
 cudaError_t launch_grid_chan_outer(const float*, const float*, float*, int*, int, int, cudaStream_t);
 cudaError_t launch_grid_lift_bwd(const float*, const float*, const float*, const float*, const float*, const float*,
-                                 const float*, float*, float*, float*, const float*, int, int, int, int, int, cudaStream_t);
+                                 const float*, float*, float*, float*, const float*, int, int, int, int, int, cudaStream_t,
+                                 const unsigned char*);
 int grid_lift_bwd_parts(int);
 int grid_lift_bwd_row();
 size_t grid_bwd_partials_floats();
@@ -99,6 +101,10 @@ cudaError_t launch_add_input_noise(float*, const float*, const long long*, int, 
                                    const long long*, const int*, cudaStream_t);
 cudaError_t launch_input_noise_stream(const float*, float*, const float*, const long long*, int, int, int, float,
                                       unsigned long long, const long long*, const int*, int, cudaStream_t);
+cudaError_t launch_teacher_feed(const float*, const float*, const unsigned char*, float*, const float*, const long long*, int,
+                                int, int, float, unsigned long long, const long long*, const int*, int, bool, cudaStream_t);
+cudaError_t launch_teacher_flags(const long long*, int, int, const float*, unsigned long long, const long long*, const int*,
+                                 unsigned char*, cudaStream_t);
 }  // namespace fno
 
 using namespace fno;
@@ -197,6 +203,25 @@ static int noise_forward_args(const char* what, const fno_weights* w, const floa
 
 static inline bool noisy_step(const fno_noise* nz, int s) { return nz && nz->k0 + s > 0; }
 
+// ------------------------------------------------------------------------ teacher forcing of a rollout (fno_teacher)
+// With a teacher descriptor every call step s >= 1 is fed fed[s] = (flags[s-1][b] ? frames[s-1][b] : x_s[b]), plus the
+// noise of stream k0 + s with a noise descriptor, written by one launch; the backward sweep recomputes step s from fed[s]
+// and hands dpreds[s-1] alone (not fc0^T dL/da0 + dpreds[s-1]) to prediction s-1 of a forced sample.  The backward reads
+// only flags.
+static int teacher_args(const char* what, const fno_teacher* tc, const float* fed, bool forward) {
+  char msg[160];
+  if (!tc || !fed || !tc->flags || (forward && !tc->frames)) {
+    snprintf(msg, sizeof(msg), "%s: bad teacher argument", what);
+    return fail(kErrArg, msg);
+  }
+  FNO_ALIGN(what, tc->frames, 4);   // float4 only where every frame of the feed is 16-byte aligned
+  return kOk;
+}
+
+static inline bool fed_step(const fno_noise* nz, const fno_teacher* tc, int s) {
+  return (tc && s > 0) || noisy_step(nz, s);
+}
+
 // The caller frames of a forward / rollout / backward driver: the 64x64 lift and its backward read inputs and mask as
 // float4 (vec = 16); the grid kernels read every frame one float at a time (vec = 4).  case_params is read per float.
 static int frames_align(const char* what, const float* inputs, const float* mask, const float* case_params, unsigned vec) {
@@ -207,10 +232,21 @@ static int frames_align(const char* what, const float* inputs, const float* mask
 }
 
 // x = the frame call step s is fed: x itself, or fed[s] written from it (one launch)
-static int feed_step(const fno_noise* nz, float* fed, const float* mask, int s, size_t frame, int batch, int h, int wd,
-                     const float*& x, void* stream) {
-  if (!noisy_step(nz, s)) return kOk;
+static int feed_step(const fno_noise* nz, const fno_teacher* tc, float* fed, const float* mask, int s, size_t frame, int batch,
+                     int h, int wd, const float*& x, void* stream) {
+  if (!fed_step(nz, tc, s)) return kOk;
   float* out = fed + static_cast<size_t>(s) * frame;
+  if (tc && s > 0) {
+    FNO_CUDA(launch_teacher_feed(x, tc->frames + static_cast<size_t>(s - 1) * frame, tc->flags + static_cast<size_t>(s - 1) * batch,
+                                 out, mask, nz ? reinterpret_cast<const long long*>(nz->idx) : nullptr, batch, h, wd,
+                                 nz ? nz->std : 0.f, nz ? nz->seed : 0ull,
+                                 nz ? reinterpret_cast<const long long*>(nz->step_base) : nullptr,
+                                 nz ? reinterpret_cast<const int*>(nz->step_offset) : nullptr, nz ? nz->k0 + s : 0, nz != nullptr,
+                                 S(stream)),
+             "input_noise_stream_kernel(teacher)");
+    x = out;
+    return kOk;
+  }
   FNO_CUDA(launch_input_noise_stream(x, out, mask, reinterpret_cast<const long long*>(nz->idx), batch, h, wd, nz->std,
                                      nz->seed, reinterpret_cast<const long long*>(nz->step_base),
                                      reinterpret_cast<const int*>(nz->step_offset), nz->k0 + s, S(stream)),
@@ -220,9 +256,9 @@ static int feed_step(const fno_noise* nz, float* fed, const float* mask, int s, 
 }
 
 // the frame the backward sweep's step s was fed: fed[s] for a noisy step, else the input or the previous prediction
-static inline const float* fed_frame(const fno_noise* nz, const float* fed, const float* inputs, const float* preds_seq, int s,
-                                     size_t frame) {
-  if (noisy_step(nz, s)) return fed + static_cast<size_t>(s) * frame;
+static inline const float* fed_frame(const fno_noise* nz, const fno_teacher* tc, const float* fed, const float* inputs,
+                                     const float* preds_seq, int s, size_t frame) {
+  if (fed_step(nz, tc, s)) return fed + static_cast<size_t>(s) * frame;
   return s > 0 ? preds_seq + static_cast<size_t>(s - 1) * frame : inputs;
 }
 
@@ -433,6 +469,7 @@ int fno_forward(const fno_weights* w, const float* inputs, const float* mask, co
 static int rollout_impl(const char* what, const fno_weights* w, const float* inputs, const float* mask,
                         const float* case_params, float* preds_seq, int steps, const fno_workspace* ws, const fno_noise* nz,
                         float* fed, int batch, int act_dtype, void* stream) {
+  const fno_teacher* tc = nullptr;   // the inference rollout has no teacher
   char msg[160];
   if (steps < 0 || !preds_seq) {
     snprintf(msg, sizeof(msg), "%s: bad argument", what);
@@ -445,7 +482,7 @@ static int rollout_impl(const char* what, const fno_weights* w, const float* inp
   const float* cur = inputs;
   for (int s = 0; s < steps; ++s) {
     float* nxt = preds_seq + static_cast<size_t>(s) * frame;
-    FNO_TRY(feed_step(nz, fed, mask, s, frame, batch, kH, kW, cur, stream));
+    FNO_TRY(feed_step(nz, tc, fed, mask, s, frame, batch, kH, kW, cur, stream));
     FNO_TRY(fno_forward(w, cur, mask, case_params, nxt, ws, batch, act_dtype, stream));
     cur = nxt;
   }
@@ -533,12 +570,13 @@ int fno_forward_train(const fno_weights* w, const float* inputs, const float* ma
 // The rollout backward's sweep runs it once per step with two modes the single-step entry points leave off:
 //   accum    = 1: every parameter gradient is added to (the sweep's first step wrote it);
 //   hand_off = 1: lift_bwd_data_kernel<true>: d_inputs = fc0[:, 0:2]^T dL/da0 + add (the next sweep step's upstream
+//                 gradient when `add` is the previous prediction's; `add` alone for a sample whose `gate` is set),
 //                 gradient when `add` is the previous prediction's), d_case_params += its share.
 static int backward_impl(const char* what, const fno_weights* w, const fno_weights_bwd* wb, const float* inputs,
                          const float* mask, const float* case_params, const float* dpreds, const fno_train_saved* saved,
                          const fno_grads* g, const fno_bwd_scratch* sc, const fno_workspace* ws, int batch, int act_dtype,
                          void* stream, float* d_inputs, float* d_case_params, int accum = 0, int hand_off = 0,
-                         const float* add = nullptr) {
+                         const float* add = nullptr, const unsigned char* gate = nullptr) {
   char msg[128];
   if (!w || !wb || !inputs || !mask || !dpreds || !saved || !sc || !ws || batch <= 0 || bad_dtype(act_dtype)) {
     snprintf(msg, sizeof(msg), "%s: bad argument", what);
@@ -619,7 +657,8 @@ static int backward_impl(const char* what, const fno_weights* w, const fno_weigh
                              st),
              "lift_bwd_kernel");
   if (d_inputs || d_case_params)
-    FNO_CUDA(launch_lift_bwd_data(sc->d[cur], w->fc0_w, d_inputs, d_case_params, hand_off ? add : nullptr, hand_off, batch, p, st),
+    FNO_CUDA(launch_lift_bwd_data(sc->d[cur], w->fc0_w, d_inputs, d_case_params, hand_off ? add : nullptr, hand_off, batch, p, st,
+                                  hand_off ? gate : nullptr),
              "lift_bwd_data_kernel");
   return kOk;
 }
@@ -701,8 +740,8 @@ static int rollout_bwd_args(const char* what, const fno_weights* w, const fno_we
 
 static int rollout_forward_train_impl(const char* what, const fno_weights* w, const float* inputs, const float* mask,
                                       const float* case_params, float* preds_seq, int steps, const fno_train_saved* saved,
-                                      const fno_workspace* ws, const fno_noise* nz, float* fed, int batch, int act_dtype,
-                                      void* stream) {
+                                      const fno_workspace* ws, const fno_noise* nz, const fno_teacher* tc, float* fed,
+                                      int batch, int act_dtype, void* stream) {
   char msg[160];
   if (steps < 1 || !inputs || !preds_seq || batch <= 0) {
     snprintf(msg, sizeof(msg), "%s: bad argument", what);
@@ -715,7 +754,7 @@ static int rollout_forward_train_impl(const char* what, const fno_weights* w, co
   const float* cur = inputs;
   for (int s = 0; s < steps; ++s) {
     float* nxt = preds_seq + static_cast<size_t>(s) * frame;
-    FNO_TRY(feed_step(nz, fed, mask, s, frame, batch, kH, kW, cur, stream));
+    FNO_TRY(feed_step(nz, tc, fed, mask, s, frame, batch, kH, kW, cur, stream));
     FNO_TRY(fno_forward_train(w, cur, mask, case_params, nxt, saved, ws, batch, act_dtype, stream));
     cur = nxt;
   }
@@ -726,7 +765,7 @@ int fno_rollout_forward_train(const fno_weights* w, const float* inputs, const f
                               float* preds_seq, int steps, const fno_train_saved* saved, const fno_workspace* ws, int batch,
                               int act_dtype, void* stream) {
   return rollout_forward_train_impl("fno_rollout_forward_train", w, inputs, mask, case_params, preds_seq, steps, saved, ws,
-                                    nullptr, nullptr, batch, act_dtype, stream);
+                                    nullptr, nullptr, nullptr, batch, act_dtype, stream);
 }
 
 int fno_rollout_forward_train_noise(const fno_weights* w, const float* inputs, const float* mask, const float* case_params,
@@ -736,14 +775,26 @@ int fno_rollout_forward_train_noise(const fno_weights* w, const float* inputs, c
   FNO_TRY(noise_forward_args("fno_rollout_forward_train_noise", w, inputs, mask, case_params, saved, ws, batch, false,
                              act_dtype));
   return rollout_forward_train_impl("fno_rollout_forward_train_noise", w, inputs, mask, case_params, preds_seq, steps, saved,
-                                    ws, noise, fed, batch, act_dtype, stream);
+                                    ws, noise, nullptr, fed, batch, act_dtype, stream);
+}
+
+int fno_rollout_forward_train_feed(const fno_weights* w, const float* inputs, const float* mask, const float* case_params,
+                                   float* preds_seq, int steps, const fno_train_saved* saved, const fno_workspace* ws,
+                                   const fno_noise* noise, const fno_teacher* teacher, float* fed, int batch, int act_dtype,
+                                   void* stream) {
+  const char* what = "fno_rollout_forward_train_feed";
+  if (noise) FNO_TRY(noise_args(what, noise, fed, steps));
+  FNO_TRY(teacher_args(what, teacher, fed, true));
+  FNO_TRY(noise_forward_args(what, w, inputs, mask, case_params, saved, ws, batch, false, act_dtype));
+  return rollout_forward_train_impl(what, w, inputs, mask, case_params, preds_seq, steps, saved, ws, noise, teacher, fed, batch,
+                                    act_dtype, stream);
 }
 
 static int rollout_backward_impl(const char* what, const fno_weights* w, const fno_weights_bwd* wb, const float* inputs,
                                  const float* mask, const float* case_params, const float* preds_seq, const float* dpreds_seq,
                                  int steps, const fno_train_saved* saved, const fno_grads* grads, const fno_bwd_scratch* scratch,
-                                 const fno_workspace* ws, const fno_noise* nz, const float* fed, float* carry, float* d_inputs,
-                                 float* d_case_params, int batch, int act_dtype, void* stream) {
+                                 const fno_workspace* ws, const fno_noise* nz, const fno_teacher* tc, const float* fed,
+                                 float* carry, float* d_inputs, float* d_case_params, int batch, int act_dtype, void* stream) {
   char msg[160];
   if (w && w->n_case_params == 0) d_case_params = nullptr;   // nothing to write
   FNO_TRY(rollout_bwd_args(what, w, wb, inputs, mask, preds_seq, dpreds_seq, steps, saved, grads, scratch, ws, carry, d_inputs,
@@ -766,12 +817,13 @@ static int rollout_backward_impl(const char* what, const fno_weights* w, const f
     FNO_CUDA(cudaMemsetAsync(d_case_params, 0, static_cast<size_t>(batch) * w->n_case_params * sizeof(float), S(stream)),
              "memset(d_case_params)");
   for (int s = steps - 1; s >= 0; --s) {
-    const float* x = fed_frame(nz, fed, inputs, preds_seq, s, frame);
+    const float* x = fed_frame(nz, tc, fed, inputs, preds_seq, s, frame);
     FNO_TRY(forward_train_body(w, x, mask, case_params, saved, ws, batch, act_dtype, stream));
     const float* up = s == steps - 1 ? dpreds_seq + static_cast<size_t>(s) * frame : carry;
     FNO_TRY(backward_impl(what, w, wb, x, mask, case_params, up, saved, grads, scratch, ws, batch, act_dtype, stream,
                           s > 0 ? carry : d_inputs, d_case_params, s != steps - 1 ? 1 : 0, 1,
-                          s > 0 ? dpreds_seq + static_cast<size_t>(s - 1) * frame : nullptr));
+                          s > 0 ? dpreds_seq + static_cast<size_t>(s - 1) * frame : nullptr,
+                          tc && s > 0 ? tc->flags + static_cast<size_t>(s - 1) * batch : nullptr));
   }
   return kOk;
 }
@@ -782,7 +834,8 @@ int fno_rollout_backward(const fno_weights* w, const fno_weights_bwd* wb, const 
                          const fno_workspace* ws, float* carry, float* d_inputs, float* d_case_params, int batch, int act_dtype,
                          void* stream) {
   return rollout_backward_impl("fno_rollout_backward", w, wb, inputs, mask, case_params, preds_seq, dpreds_seq, steps, saved,
-                               grads, scratch, ws, nullptr, nullptr, carry, d_inputs, d_case_params, batch, act_dtype, stream);
+                               grads, scratch, ws, nullptr, nullptr, nullptr, carry, d_inputs, d_case_params, batch, act_dtype,
+                               stream);
 }
 
 int fno_rollout_backward_noise(const fno_weights* w, const fno_weights_bwd* wb, const float* inputs, const float* mask,
@@ -792,8 +845,20 @@ int fno_rollout_backward_noise(const fno_weights* w, const fno_weights_bwd* wb, 
                                float* d_inputs, float* d_case_params, int batch, int act_dtype, void* stream) {
   FNO_TRY(noise_args("fno_rollout_backward_noise", noise, fed, steps));
   return rollout_backward_impl("fno_rollout_backward_noise", w, wb, inputs, mask, case_params, preds_seq, dpreds_seq, steps,
-                               saved, grads, scratch, ws, noise, fed, carry, d_inputs, d_case_params, batch, act_dtype,
+                               saved, grads, scratch, ws, noise, nullptr, fed, carry, d_inputs, d_case_params, batch, act_dtype,
                                stream);
+}
+
+int fno_rollout_backward_feed(const fno_weights* w, const fno_weights_bwd* wb, const float* inputs, const float* mask,
+                              const float* case_params, const float* preds_seq, const float* dpreds_seq, int steps,
+                              const fno_train_saved* saved, const fno_grads* grads, const fno_bwd_scratch* scratch,
+                              const fno_workspace* ws, const fno_noise* noise, const fno_teacher* teacher, const float* fed,
+                              float* carry, float* d_inputs, float* d_case_params, int batch, int act_dtype, void* stream) {
+  const char* what = "fno_rollout_backward_feed";
+  if (noise) FNO_TRY(noise_args(what, noise, fed, steps));
+  FNO_TRY(teacher_args(what, teacher, fed, false));
+  return rollout_backward_impl(what, w, wb, inputs, mask, case_params, preds_seq, dpreds_seq, steps, saved, grads, scratch, ws,
+                               noise, teacher, fed, carry, d_inputs, d_case_params, batch, act_dtype, stream);
 }
 
 int fno_multistep_metrics(const float* preds_seq, const float* label_u, const float* mask, float* sums, int steps,
@@ -1208,6 +1273,7 @@ static int grid_rollout_impl(const char* what, const fno_weights* w, const float
                              const float* case_params, float* preds_seq, int steps, const fno_workspace* ws,
                              const fno_noise* nz, float* fed, int batch, int h, int wd, void* stream) {
   char msg[160];
+  const fno_teacher* tc = nullptr;   // the inference rollout has no teacher
   FNO_TRY(grid_arg(what, h, wd));
   if (steps < 0 || !preds_seq || batch <= 0) {
     snprintf(msg, sizeof(msg), "%s: bad argument", what);
@@ -1220,7 +1286,7 @@ static int grid_rollout_impl(const char* what, const fno_weights* w, const float
   const float* cur = inputs;
   for (int s = 0; s < steps; ++s) {
     float* nxt = preds_seq + static_cast<size_t>(s) * frame;
-    FNO_TRY(feed_step(nz, fed, mask, s, frame, batch, h, wd, cur, stream));
+    FNO_TRY(feed_step(nz, tc, fed, mask, s, frame, batch, h, wd, cur, stream));
     FNO_TRY(fno_grid_forward(w, cur, mask, case_params, nxt, ws, batch, h, wd, stream));
     cur = nxt;
   }
@@ -1269,12 +1335,12 @@ int fno_grid_forward_train(const fno_weights* w, const float* inputs, const floa
   return fno_grid_project_fwd(static_cast<const float*>(saved->act[w->n_layers]), mask, w, preds, batch, h, wd, stream);
 }
 
-// The grid backward after argument checks; accum / hand_off / add as in backward_impl (the rollout sweep's modes)
+// The grid backward after argument checks; accum / hand_off / add / gate as in backward_impl (the rollout sweep's modes)
 static int grid_backward_impl(const fno_weights* w, const fno_weights_bwd* wb, const float* inputs, const float* mask,
                               const float* case_params, const float* dpreds, const fno_train_saved* saved, const fno_grads* g,
                               const fno_bwd_scratch* sc, const fno_workspace* ws, float* d_inputs, float* d_case_params,
                               int batch, int h, int wd, void* stream, int accum = 0, int hand_off = 0,
-                              const float* add = nullptr) {
+                              const float* add = nullptr, const unsigned char* gate = nullptr) {
   cudaStream_t st = S(stream);
   const int L = w->n_layers, p = w->n_case_params;
   // ---- projection -> d[0] = dpre_{L-1}
@@ -1310,7 +1376,8 @@ static int grid_backward_impl(const fno_weights* w, const fno_weights_bwd* wb, c
   float* part_lb = g ? sc->partials + grid_partials_offset_lb() : nullptr;
   if (g || d_inputs || d_case_params) {
     FNO_CUDA(launch_grid_lift_bwd(sc->d[cur], inputs, mask, case_params, w->gx, w->gy, w->fc0_w, part_lb, d_inputs,
-                                  d_case_params, hand_off ? add : nullptr, hand_off, batch, p, h, wd, st),
+                                  d_case_params, hand_off ? add : nullptr, hand_off, batch, p, h, wd, st,
+                                  hand_off ? gate : nullptr),
              "grid_lift_bwd_kernel");
   }
   if (g)
@@ -1345,7 +1412,7 @@ int fno_grid_backward(const fno_weights* w, const fno_weights_bwd* wb, const flo
 static int grid_rollout_forward_train_impl(const char* what, const fno_weights* w, const float* inputs, const float* mask,
                                            const float* case_params, float* preds_seq, int steps,
                                            const fno_train_saved* saved, const fno_workspace* ws, const fno_noise* nz,
-                                           float* fed, int batch, int h, int wd, void* stream) {
+                                           const fno_teacher* tc, float* fed, int batch, int h, int wd, void* stream) {
   char msg[160];
   FNO_TRY(grid_arg(what, h, wd));
   if (steps < 1 || !inputs || !preds_seq || batch <= 0) {
@@ -1359,7 +1426,7 @@ static int grid_rollout_forward_train_impl(const char* what, const fno_weights* 
   const float* cur = inputs;
   for (int s = 0; s < steps; ++s) {
     float* nxt = preds_seq + static_cast<size_t>(s) * frame;
-    FNO_TRY(feed_step(nz, fed, mask, s, frame, batch, h, wd, cur, stream));
+    FNO_TRY(feed_step(nz, tc, fed, mask, s, frame, batch, h, wd, cur, stream));
     FNO_TRY(fno_grid_forward_train(w, cur, mask, case_params, nxt, saved, ws, batch, h, wd, stream));
     cur = nxt;
   }
@@ -1370,7 +1437,7 @@ int fno_grid_rollout_forward_train(const fno_weights* w, const float* inputs, co
                                    float* preds_seq, int steps, const fno_train_saved* saved, const fno_workspace* ws,
                                    int batch, int h, int wd, void* stream) {
   return grid_rollout_forward_train_impl("fno_grid_rollout_forward_train", w, inputs, mask, case_params, preds_seq, steps,
-                                         saved, ws, nullptr, nullptr, batch, h, wd, stream);
+                                         saved, ws, nullptr, nullptr, nullptr, batch, h, wd, stream);
 }
 
 int fno_grid_rollout_forward_train_noise(const fno_weights* w, const float* inputs, const float* mask,
@@ -1382,15 +1449,28 @@ int fno_grid_rollout_forward_train_noise(const fno_weights* w, const float* inpu
   FNO_TRY(noise_forward_args("fno_grid_rollout_forward_train_noise", w, inputs, mask, case_params, saved, ws, batch, true,
                              0));
   return grid_rollout_forward_train_impl("fno_grid_rollout_forward_train_noise", w, inputs, mask, case_params, preds_seq,
-                                         steps, saved, ws, noise, fed, batch, h, wd, stream);
+                                         steps, saved, ws, noise, nullptr, fed, batch, h, wd, stream);
+}
+
+int fno_grid_rollout_forward_train_feed(const fno_weights* w, const float* inputs, const float* mask,
+                                        const float* case_params, float* preds_seq, int steps, const fno_train_saved* saved,
+                                        const fno_workspace* ws, const fno_noise* noise, const fno_teacher* teacher, float* fed,
+                                        int batch, int h, int wd, void* stream) {
+  const char* what = "fno_grid_rollout_forward_train_feed";
+  FNO_TRY(grid_arg(what, h, wd));
+  if (noise) FNO_TRY(noise_args(what, noise, fed, steps));
+  FNO_TRY(teacher_args(what, teacher, fed, true));
+  FNO_TRY(noise_forward_args(what, w, inputs, mask, case_params, saved, ws, batch, true, 0));
+  return grid_rollout_forward_train_impl(what, w, inputs, mask, case_params, preds_seq, steps, saved, ws, noise, teacher, fed,
+                                         batch, h, wd, stream);
 }
 
 static int grid_rollout_backward_impl(const char* what, const fno_weights* w, const fno_weights_bwd* wb, const float* inputs,
                                       const float* mask, const float* case_params, const float* preds_seq,
                                       const float* dpreds_seq, int steps, const fno_train_saved* saved, const fno_grads* grads,
                                       const fno_bwd_scratch* scratch, const fno_workspace* ws, const fno_noise* nz,
-                                      const float* fed, float* carry, float* d_inputs, float* d_case_params, int batch, int h,
-                                      int wd, void* stream) {
+                                      const fno_teacher* tc, const float* fed, float* carry, float* d_inputs,
+                                      float* d_case_params, int batch, int h, int wd, void* stream) {
   char msg[160];
   FNO_TRY(grid_arg(what, h, wd));
   if (w && w->n_case_params == 0) d_case_params = nullptr;   // nothing to write
@@ -1412,12 +1492,13 @@ static int grid_rollout_backward_impl(const char* what, const fno_weights* w, co
     FNO_CUDA(cudaMemsetAsync(d_case_params, 0, static_cast<size_t>(batch) * w->n_case_params * sizeof(float), S(stream)),
              "memset(d_case_params)");
   for (int s = steps - 1; s >= 0; --s) {
-    const float* x = fed_frame(nz, fed, inputs, preds_seq, s, frame);
+    const float* x = fed_frame(nz, tc, fed, inputs, preds_seq, s, frame);
     FNO_TRY(grid_forward_train_body(w, x, mask, case_params, saved, ws, batch, h, wd, stream));
     const float* up = s == steps - 1 ? dpreds_seq + static_cast<size_t>(s) * frame : carry;
     FNO_TRY(grid_backward_impl(w, wb, x, mask, case_params, up, saved, grads, scratch, ws, s > 0 ? carry : d_inputs,
                                d_case_params, batch, h, wd, stream, s != steps - 1 ? 1 : 0, 1,
-                               s > 0 ? dpreds_seq + static_cast<size_t>(s - 1) * frame : nullptr));
+                               s > 0 ? dpreds_seq + static_cast<size_t>(s - 1) * frame : nullptr,
+                               tc && s > 0 ? tc->flags + static_cast<size_t>(s - 1) * batch : nullptr));
   }
   return kOk;
 }
@@ -1428,8 +1509,8 @@ int fno_grid_rollout_backward(const fno_weights* w, const fno_weights_bwd* wb, c
                               const fno_workspace* ws, float* carry, float* d_inputs, float* d_case_params, int batch, int h,
                               int wd, void* stream) {
   return grid_rollout_backward_impl("fno_grid_rollout_backward", w, wb, inputs, mask, case_params, preds_seq, dpreds_seq, steps,
-                                    saved, grads, scratch, ws, nullptr, nullptr, carry, d_inputs, d_case_params, batch, h, wd,
-                                    stream);
+                                    saved, grads, scratch, ws, nullptr, nullptr, nullptr, carry, d_inputs, d_case_params, batch,
+                                    h, wd, stream);
 }
 
 int fno_grid_rollout_backward_noise(const fno_weights* w, const fno_weights_bwd* wb, const float* inputs, const float* mask,
@@ -1440,8 +1521,22 @@ int fno_grid_rollout_backward_noise(const fno_weights* w, const fno_weights_bwd*
   FNO_TRY(grid_arg("fno_grid_rollout_backward_noise", h, wd));
   FNO_TRY(noise_args("fno_grid_rollout_backward_noise", noise, fed, steps));
   return grid_rollout_backward_impl("fno_grid_rollout_backward_noise", w, wb, inputs, mask, case_params, preds_seq, dpreds_seq,
-                                    steps, saved, grads, scratch, ws, noise, fed, carry, d_inputs, d_case_params, batch, h,
-                                    wd, stream);
+                                    steps, saved, grads, scratch, ws, noise, nullptr, fed, carry, d_inputs, d_case_params,
+                                    batch, h, wd, stream);
+}
+
+int fno_grid_rollout_backward_feed(const fno_weights* w, const fno_weights_bwd* wb, const float* inputs, const float* mask,
+                                   const float* case_params, const float* preds_seq, const float* dpreds_seq, int steps,
+                                   const fno_train_saved* saved, const fno_grads* grads, const fno_bwd_scratch* scratch,
+                                   const fno_workspace* ws, const fno_noise* noise, const fno_teacher* teacher,
+                                   const float* fed, float* carry, float* d_inputs, float* d_case_params, int batch, int h,
+                                   int wd, void* stream) {
+  const char* what = "fno_grid_rollout_backward_feed";
+  FNO_TRY(grid_arg(what, h, wd));
+  if (noise) FNO_TRY(noise_args(what, noise, fed, steps));
+  FNO_TRY(teacher_args(what, teacher, fed, false));
+  return grid_rollout_backward_impl(what, w, wb, inputs, mask, case_params, preds_seq, dpreds_seq, steps, saved, grads, scratch,
+                                    ws, noise, teacher, fed, carry, d_inputs, d_case_params, batch, h, wd, stream);
 }
 
 int fno_grid_multistep_metrics(const float* preds_seq, const float* label_u, const float* mask, float* sums, int steps,
@@ -1526,6 +1621,22 @@ int fno_add_input_noise_stream(const float* in, float* out, const float* mask, c
                                      reinterpret_cast<const long long*>(step_base), reinterpret_cast<const int*>(step_offset),
                                      noise_stream, S(stream)),
            "input_noise_stream_kernel");
+  return kOk;
+}
+
+int fno_teacher_flags(const int64_t* idx, int batch, int steps, const float* prob, uint64_t seed, const int64_t* step_base,
+                      const int32_t* step_offset, uint8_t* flags, void* stream) {
+  if (!idx || !prob || !step_base || !flags || batch <= 0 || steps < 2 || steps > FNO_NOISE_STREAMS ||
+      static_cast<long long>(steps - 1) * batch > 0x7fffffffll)
+    return fail(kErrArg, "fno_teacher_flags: bad argument");
+  FNO_ALIGN("fno_teacher_flags", idx, 8);
+  FNO_ALIGN("fno_teacher_flags", prob, 4);
+  FNO_ALIGN("fno_teacher_flags", step_base, 8);
+  FNO_ALIGN("fno_teacher_flags", step_offset, 4);
+  FNO_CUDA(launch_teacher_flags(reinterpret_cast<const long long*>(idx), batch, steps, prob, seed,
+                                reinterpret_cast<const long long*>(step_base), reinterpret_cast<const int*>(step_offset),
+                                flags, S(stream)),
+           "teacher_flags_kernel");
   return kOk;
 }
 

@@ -394,7 +394,9 @@ cudaError_t launch_lift_bwd(const float* da0, const float* inputs, const float* 
 // are reduced at the end.  One pass over d_a0 (float32 in both storage modes, 134 MB at B = 256).
 // kHandOff (the rollout backward's sweep): d_inputs = (sum_o fc0_w[o][c] d_a0) + add, where `add` (or null) is the
 // upstream gradient of the previous step's prediction, so d_inputs becomes that step's whole upstream gradient in this
-// one pass; d_params += instead of = (the case parameters feed every step).
+// one pass; d_params += instead of = (the case parameters feed every step).  `gate` (or null; kHandOff only, teacher
+// forcing): where gate[b] != 0 the previous prediction was not fed to this step, so d_inputs = add, a copy bit for bit
+// (nothing of d_a0, a NaN included, reaches it); d_params still takes the step's share.
 constexpr int kLdThreads = 512;
 constexpr int kLdVec = kHW / (4 * kLdThreads);   // float4 groups per thread and channel
 
@@ -405,6 +407,7 @@ __global__ void __launch_bounds__(kLdThreads)
                          float* __restrict__ d_inputs,      // [B][2][4096] or null
                          float* __restrict__ d_params,      // [B][p] or null
                          const float* __restrict__ add,     // [B][2][4096] or null (kHandOff only)
+                         const unsigned char* __restrict__ gate,   // [B] or null (kHandOff only)
                          int p) {
   __shared__ float wu[kC], wv[kC];
   __shared__ __align__(16) float wp[kC][kMaxCaseParams];   // columns 5..5+p, zero-padded to 16
@@ -462,11 +465,19 @@ __global__ void __launch_bounds__(kLdThreads)
       if (add != nullptr) {
         const float4* u_add = reinterpret_cast<const float4*>(add + static_cast<size_t>(b) * 2 * kHW);
         const float4* v_add = u_add + kHW / 4;
+        if (gate != nullptr && gate[b] != 0) {   // a forced sample: the carry is add alone
 #pragma unroll
-        for (int k = 0; k < kLdVec; ++k) {
-          const float4 a = __ldcs(u_add + k * kLdThreads + tid), c = __ldcs(v_add + k * kLdThreads + tid);
-          du[k].x += a.x; du[k].y += a.y; du[k].z += a.z; du[k].w += a.w;
-          dv[k].x += c.x; dv[k].y += c.y; dv[k].z += c.z; dv[k].w += c.w;
+          for (int k = 0; k < kLdVec; ++k) {
+            du[k] = __ldcs(u_add + k * kLdThreads + tid);
+            dv[k] = __ldcs(v_add + k * kLdThreads + tid);
+          }
+        } else {
+#pragma unroll
+          for (int k = 0; k < kLdVec; ++k) {
+            const float4 a = __ldcs(u_add + k * kLdThreads + tid), c = __ldcs(v_add + k * kLdThreads + tid);
+            du[k].x += a.x; du[k].y += a.y; du[k].z += a.z; du[k].w += a.w;
+            dv[k].x += c.x; dv[k].y += c.y; dv[k].z += c.z; dv[k].w += c.w;
+          }
         }
       }
     }
@@ -494,17 +505,17 @@ __global__ void __launch_bounds__(kLdThreads)
   }
 }
 
-// hand_off = 0: the single-step data adjoint (d_inputs, d_params written; `add` must be null).  hand_off = 1: the
-// rollout sweep's mode described above the kernel.
+// hand_off = 0: the single-step data adjoint (d_inputs, d_params written; `add` and `gate` must be null).  hand_off = 1:
+// the rollout sweep's mode described above the kernel.
 cudaError_t launch_lift_bwd_data(const float* da0, const float* fc0_w, float* d_inputs, float* d_params, const float* add,
-                                 int hand_off, int batch, int p, cudaStream_t stream) {
+                                 int hand_off, int batch, int p, cudaStream_t stream, const unsigned char* gate) {
   if (p < 0 || p > kMaxCaseParams) return cudaErrorInvalidValue;
   if (p == 0) d_params = nullptr;
   if (d_inputs == nullptr && d_params == nullptr) return cudaSuccess;
   if (hand_off)
-    lift_bwd_data_kernel<true><<<batch, kLdThreads, 0, stream>>>(da0, fc0_w, d_inputs, d_params, add, p);
+    lift_bwd_data_kernel<true><<<batch, kLdThreads, 0, stream>>>(da0, fc0_w, d_inputs, d_params, add, gate, p);
   else
-    lift_bwd_data_kernel<false><<<batch, kLdThreads, 0, stream>>>(da0, fc0_w, d_inputs, d_params, nullptr, p);
+    lift_bwd_data_kernel<false><<<batch, kLdThreads, 0, stream>>>(da0, fc0_w, d_inputs, d_params, nullptr, nullptr, p);
   return cudaGetLastError();
 }
 

@@ -645,7 +645,8 @@ template cudaError_t launch_grid_chan_outer<kC, kC>(const float*, const float*, 
 // sum_j fc0_w[j][5+q] sum(dL/da0[j]); d_inputs[b][c][p] = sum_j fc0_w[j][c] dL/da0[b][j][p].
 // Partial row: fc0.weight (32 x (5+p)) | fc0.bias (32), stride kGlbRow.
 // kHandOff (the rollout backward's sweep): d_inputs = (sum_j fc0_w[j][c] dL/da0) + add, `add` (or null) being the upstream
-// gradient of the previous step's prediction, and d_case_params += instead of =.
+// gradient of the previous step's prediction, and d_case_params += instead of =.  `gate` (or null; kHandOff only, teacher
+// forcing): where gate[b] != 0, d_inputs = add, a copy bit for bit; d_case_params and the partials still take b's share.
 constexpr int kGlbThreads = 256;
 constexpr int kGlbParts = 264;
 constexpr int kGlbRow = kC * (5 + kMaxCaseParams) + kC;
@@ -655,7 +656,8 @@ __global__ void __launch_bounds__(kGlbThreads)
     grid_lift_bwd_kernel(const float* __restrict__ da0, const float* __restrict__ inputs, const float* __restrict__ mask,
                          const float* __restrict__ params, const float* __restrict__ gx, const float* __restrict__ gy,
                          const float* __restrict__ fc0_w, float* __restrict__ partial, float* __restrict__ d_inputs,
-                         float* __restrict__ d_params, const float* __restrict__ add, int batch, int p, int h, int wd) {
+                         float* __restrict__ d_params, const float* __restrict__ add,
+                         const unsigned char* __restrict__ gate, int batch, int p, int h, int wd) {
   __shared__ float sums[kC][6];
   __shared__ float accw[kC * (5 + kMaxCaseParams)];
   __shared__ float accb[kC];
@@ -723,6 +725,13 @@ __global__ void __launch_bounds__(kGlbThreads)
     }
     if (d_inputs) {
       const float* add_b = add != nullptr ? add + static_cast<size_t>(b) * 2 * hw : nullptr;
+      if (kHandOff && add_b != nullptr && gate != nullptr && gate[b] != 0) {   // a forced sample: the carry is add alone
+        for (int pix = tid; pix < hw; pix += kGlbThreads) {
+          d_inputs[(static_cast<size_t>(b) * 2 + 0) * hw + pix] = add_b[pix];
+          d_inputs[(static_cast<size_t>(b) * 2 + 1) * hw + pix] = add_b[hw + pix];
+        }
+        continue;
+      }
       for (int pix = tid; pix < hw; pix += kGlbThreads) {
         float du = 0.f, dv = 0.f;
 #pragma unroll 8
@@ -757,14 +766,14 @@ int grid_lift_bwd_row() { return kGlbRow; }
 cudaError_t launch_grid_lift_bwd(const float* da0, const float* inputs, const float* mask, const float* params,
                                  const float* gx, const float* gy, const float* fc0_w, float* partial, float* d_inputs,
                                  float* d_params, const float* add, int hand_off, int batch, int p, int h, int wd,
-                                 cudaStream_t stream) {
+                                 cudaStream_t stream, const unsigned char* gate) {
   if (p < 0 || p > kMaxCaseParams) return cudaErrorInvalidValue;
   if (hand_off)
     grid_lift_bwd_kernel<true><<<grid_lift_bwd_parts(batch), kGlbThreads, 0, stream>>>(
-        da0, inputs, mask, params, gx, gy, fc0_w, partial, d_inputs, d_params, add, batch, p, h, wd);
+        da0, inputs, mask, params, gx, gy, fc0_w, partial, d_inputs, d_params, add, gate, batch, p, h, wd);
   else
     grid_lift_bwd_kernel<false><<<grid_lift_bwd_parts(batch), kGlbThreads, 0, stream>>>(
-        da0, inputs, mask, params, gx, gy, fc0_w, partial, d_inputs, d_params, nullptr, batch, p, h, wd);
+        da0, inputs, mask, params, gx, gy, fc0_w, partial, d_inputs, d_params, nullptr, nullptr, batch, p, h, wd);
   return cudaGetLastError();
 }
 

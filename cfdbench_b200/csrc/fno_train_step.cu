@@ -578,21 +578,38 @@ __device__ __forceinline__ float4 noise_normals(unsigned long long seed, unsigne
 // The body of both noise kernels for sample b = blockIdx.y and quad q.  kInPlace (add_input_noise_kernel, out == in):
 // only the cells where mask != 0 are written.  Otherwise (input_noise_stream_kernel) out = in + noise where mask != 0 and
 // out = in elsewhere, so `out` is a whole frame; `out` may still equal `in`.
-template <bool kVec, bool kInPlace>
+// kSelect (the teacher-forced feed of a rollout step): sample b's frame is alt's where flags[b] != 0, in's otherwise -- a
+// choice of source, so the frame that is not chosen is never read and nothing of it (a NaN included) reaches out.
+// !kNoise: out = that frame, bit for bit (no noise drawn; idx, step_base and mask are not read).
+template <bool kVec, bool kInPlace, bool kSelect = false, bool kNoise = true>
 __device__ __forceinline__ void input_noise(const float* in, float* out, const float* __restrict__ mask,
                                             const long long* __restrict__ idx, int hw, float std, unsigned long long seed,
                                             const long long* __restrict__ step_base, const int* __restrict__ step_offset,
-                                            unsigned stream) {
+                                            unsigned stream, const float* alt = nullptr,
+                                            const unsigned char* __restrict__ flags = nullptr) {
+  static_assert(!(kInPlace && kSelect), "the select writes a whole frame");
   const int b = blockIdx.y;
   const int n_el = 2 * hw;
   const unsigned q = blockIdx.x * kNoiseThreads + threadIdx.x;
   if (4 * q >= static_cast<unsigned>(n_el)) return;
+  const float* src = in;
+  if constexpr (kSelect) src = flags[b] != 0 ? alt : in;
+  const float* x = src + static_cast<size_t>(b) * n_el;
+  float* y = out + static_cast<size_t>(b) * n_el;
+  if constexpr (!kNoise) {
+    if constexpr (kVec) {
+      *reinterpret_cast<float4*>(y + 4 * q) = *reinterpret_cast<const float4*>(x + 4 * q);
+    } else {
+#pragma unroll
+      for (int r = 0; r < 4; ++r)
+        if (static_cast<int>(4 * q) + r < n_el) y[4 * q + r] = x[4 * q + r];
+    }
+    return;
+  }
   const unsigned long long step =
       static_cast<unsigned long long>(*step_base) + (step_offset ? static_cast<long long>(*step_offset) : 0ll);
   const float4 z = noise_normals(seed, step, static_cast<unsigned>(idx[b]), q + (stream << 16));
   const float zs[4] = {z.x, z.y, z.z, z.w};
-  const float* x = in + static_cast<size_t>(b) * n_el;
-  float* y = out + static_cast<size_t>(b) * n_el;
   const float* m = mask + static_cast<size_t>(b) * hw;
   if constexpr (kVec) {   // hw % 4 == 0 and 16-byte aligned slices: the quad lies in one channel
     const int e = 4 * q, cell = e < hw ? e : e - hw;
@@ -641,13 +658,15 @@ __global__ void __launch_bounds__(kNoiseThreads)
   input_noise<kVec, true>(inputs, inputs, mask, idx, hw, std, seed, step_base, step_offset, 0u);
 }
 
-// out = in + noise of stream `stream` (input_noise's out-of-place form; in == out is allowed)
-template <bool kVec>
+// out = in + noise of stream `stream` (input_noise's out-of-place form; in == out is allowed).  kSelect / !kNoise: the
+// teacher-forced feed (launch_teacher_feed): out = (flags[b] ? alt : in) [+ noise].
+template <bool kVec, bool kSelect = false, bool kNoise = true>
 __global__ void __launch_bounds__(kNoiseThreads)
     input_noise_stream_kernel(const float* in, float* out, const float* __restrict__ mask, const long long* __restrict__ idx,
                               int hw, float std, unsigned long long seed, const long long* __restrict__ step_base,
-                              const int* __restrict__ step_offset, unsigned stream) {
-  input_noise<kVec, false>(in, out, mask, idx, hw, std, seed, step_base, step_offset, stream);
+                              const int* __restrict__ step_offset, unsigned stream, const float* alt,
+                              const unsigned char* __restrict__ flags) {
+  input_noise<kVec, false, kSelect, kNoise>(in, out, mask, idx, hw, std, seed, step_base, step_offset, stream, alt, flags);
 }
 
 cudaError_t launch_add_input_noise(float* inputs, const float* mask, const long long* idx, int n, int h, int w, float std,
@@ -675,10 +694,66 @@ cudaError_t launch_input_noise_stream(const float* in, float* out, const float* 
   const unsigned k = static_cast<unsigned>(noise_stream);
   if (vec)
     input_noise_stream_kernel<true><<<grid, kNoiseThreads, 0, stream>>>(in, out, mask, idx, hw, std, seed, step_base,
-                                                                         step_offset, k);
+                                                                         step_offset, k, nullptr, nullptr);
   else
     input_noise_stream_kernel<false><<<grid, kNoiseThreads, 0, stream>>>(in, out, mask, idx, hw, std, seed, step_base,
-                                                                          step_offset, k);
+                                                                          step_offset, k, nullptr, nullptr);
+  return cudaGetLastError();
+}
+
+// ------------------------------------------------------------------------------------------------ teacher forcing
+// The feed of a teacher-forced rollout step: out[b] = (flags[b] ? teacher[b] : pred[b]), plus the noise of stream
+// `noise_stream` where mask != 0 when `noise` is set (input_noise_stream_kernel's select forms).  One launch.
+cudaError_t launch_teacher_feed(const float* pred, const float* teacher, const unsigned char* flags, float* out,
+                                const float* mask, const long long* idx, int n, int h, int w, float std,
+                                unsigned long long seed, const long long* step_base, const int* step_offset, int noise_stream,
+                                bool noise, cudaStream_t stream) {
+  const int hw = h * w, quads = (2 * hw + 3) / 4;
+  const dim3 grid((quads + kNoiseThreads - 1) / kNoiseThreads, n);
+  const bool vec = hw % 4 == 0 && ((reinterpret_cast<uintptr_t>(pred) | reinterpret_cast<uintptr_t>(teacher) |
+                                    reinterpret_cast<uintptr_t>(out) | reinterpret_cast<uintptr_t>(mask)) & 15) == 0;
+  const unsigned k = static_cast<unsigned>(noise_stream);
+#define FNO_FEED(V, N)                                                                                                     \
+  input_noise_stream_kernel<V, true, N><<<grid, kNoiseThreads, 0, stream>>>(pred, out, mask, idx, hw, std, seed, step_base, \
+                                                                            step_offset, k, teacher, flags)
+  if (noise) {
+    if (vec) FNO_FEED(true, true);
+    else FNO_FEED(false, true);
+  } else {
+    if (vec) FNO_FEED(true, false);
+    else FNO_FEED(false, false);
+  }
+#undef FNO_FEED
+  return cudaGetLastError();
+}
+
+// flags[s - 1][i] = (u <= *prob) for rollout steps s = 1 .. steps - 1 and samples i < batch, u = the uniform in (0, 1] of
+// word x of Philox4x32-10(counter = (s, j, step_lo, step_hi), key = (seed_lo, seed_hi)), j = idx[i], step = *step_base
+// (+ *step_offset): a pure function of (seed, step, j, s), whatever the batch slot.  p = 0 never sets a flag (u > 0) and
+// p = 1 always does (u <= 1); p and the step are read on the device, so a captured launch sees each replay's.
+constexpr int kFlagThreads = 256;
+
+__global__ void __launch_bounds__(kFlagThreads)
+    teacher_flags_kernel(const long long* __restrict__ idx, int batch, int n, const float* __restrict__ prob,
+                         unsigned long long seed, const long long* __restrict__ step_base,
+                         const int* __restrict__ step_offset, unsigned char* __restrict__ flags) {
+  const int i = blockIdx.x * kFlagThreads + threadIdx.x;
+  if (i >= n) return;
+  const int s = i / batch + 1, b = i - (s - 1) * batch;
+  const unsigned long long step =
+      static_cast<unsigned long long>(*step_base) + (step_offset ? static_cast<long long>(*step_offset) : 0ll);
+  const uint4 x = philox4x32_10(make_uint4(static_cast<unsigned>(s), static_cast<unsigned>(idx[b]),
+                                           static_cast<unsigned>(step), static_cast<unsigned>(step >> 32)),
+                                make_uint2(static_cast<unsigned>(seed), static_cast<unsigned>(seed >> 32)));
+  flags[i] = noise_uniform(x.x) <= *prob ? 1 : 0;
+}
+
+cudaError_t launch_teacher_flags(const long long* idx, int batch, int steps, const float* prob, unsigned long long seed,
+                                 const long long* step_base, const int* step_offset, unsigned char* flags,
+                                 cudaStream_t stream) {
+  const int n = (steps - 1) * batch;
+  teacher_flags_kernel<<<(n + kFlagThreads - 1) / kFlagThreads, kFlagThreads, 0, stream>>>(idx, batch, n, prob, seed,
+                                                                                           step_base, step_offset, flags);
   return cudaGetLastError();
 }
 

@@ -346,6 +346,80 @@ def add_input_noise(frames: Tensor, mask: Tensor, ids: Tensor, std: float, seed:
     return _noise_out_of_place(frames.detach().contiguous(), *args)
 
 
+class TeacherForcing(NamedTuple):
+    """The teacher forcing of `Fno2d.rollout(teacher=...)` (scheduled sampling): `frames` ((steps - 1, B, 2, H, W)
+    float32 on the model's device) are the true frames and `flags` ((steps - 1, B) bool or uint8, same device) choose
+    them: rollout step s >= 1 of sample b is fed frames[s - 1][b] where flags[s - 1][b] is set, else the prediction of
+    step s - 1.  With `rollout_batch`'s window, frames = b["labels"][:steps - 1] (the masked targets) and flags from
+    `teacher_forcing_flags`."""
+    frames: Tensor
+    flags: Tensor
+
+
+def check_teacher_forcing(teacher, batch: int, steps, gh: int, gw: int) -> Optional[TeacherForcing]:
+    """Refuse a `Fno2d.rollout` teacher record the native drivers cannot take: not a TeacherForcing, steps < 2, frames
+    that are not a (steps - 1, batch, 2, gh, gw) float32 tensor or that require grad (the true frames are data), flags
+    that are not a (steps - 1, batch) bool or uint8 tensor, or the two on different devices.  Returns None for None,
+    else the record with contiguous frames and uint8 flags."""
+    if teacher is None:
+        return None
+    if not isinstance(teacher, TeacherForcing):
+        raise ValueError(f"teacher must be a TeacherForcing or None, got {type(teacher).__name__}")
+    if isinstance(steps, bool) or not isinstance(steps, int) or steps < 2:
+        raise ValueError(f"teacher forcing needs steps >= 2 (step 0 is always fed the start frame), got steps={steps!r}")
+    frames, flags = teacher.frames, teacher.flags
+    shape = (steps - 1, batch, 2, gh, gw)
+    if not isinstance(frames, Tensor) or frames.dtype != torch.float32 or tuple(frames.shape) != shape:
+        raise ValueError(f"teacher.frames must be a {shape} float32 tensor, got "
+                         f"{getattr(frames, 'dtype', type(frames).__name__)} {tuple(getattr(frames, 'shape', ()))}")
+    if frames.requires_grad:
+        raise ValueError("teacher.frames requires grad: the true frames are data, and no gradient flows into them")
+    if not isinstance(flags, Tensor) or flags.dtype not in (torch.bool, torch.uint8) or \
+            tuple(flags.shape) != (steps - 1, batch):
+        raise ValueError(f"teacher.flags must be a ({steps - 1}, {batch}) bool or uint8 tensor, got "
+                         f"{getattr(flags, 'dtype', type(flags).__name__)} {tuple(getattr(flags, 'shape', ()))}")
+    if flags.device != frames.device:
+        raise ValueError(f"teacher.frames is on {frames.device}, teacher.flags on {flags.device}")
+    return TeacherForcing(frames.contiguous(), flags.to(torch.uint8).contiguous())
+
+
+def check_teacher_prob(prob, name: str = "prob") -> float:
+    """A teacher-forcing probability: a real number in [0, 1].  Returns it as a float."""
+    if isinstance(prob, bool) or not isinstance(prob, (int, float, np.integer, np.floating)) \
+            or not np.isfinite(prob) or not 0 <= prob <= 1:
+        raise ValueError(f"{name} must be a real number in [0, 1], got {prob!r}")
+    return float(prob)
+
+
+def teacher_forcing_flags(ids: Tensor, steps: int, prob: float, seed: int, step: int) -> Tensor:
+    """The (steps - 1, B) uint8 teacher-forcing flags of windows that start at dataset indices `ids` ((B,) int64 on a
+    CUDA device): flags[s - 1][b] = 1 with probability `prob`, drawn from the counter-based RNG of `add_input_noise`
+    keyed by `seed` and counted by `step` (train_auto passes Adam's 1-based step), a pure function of (seed, step,
+    ids[b], s) whatever the batch slot.  prob = 0 sets no flag, prob = 1 every flag.  One launch
+    (`fno_teacher_flags`); train_auto(teacher_forcing=p, teacher_seed=seed) draws exactly these.  Raises ValueError for
+    steps < 2, a prob outside [0, 1], a seed outside [0, 2^64), a step outside [0, 2^63) or malformed ids."""
+    from . import _lib
+    if isinstance(steps, bool) or not isinstance(steps, (int, np.integer)) or not 2 <= steps <= 2 ** 16:
+        raise ValueError(f"steps must be an int in [2, 2^16], got {steps!r}")
+    prob = check_teacher_prob(prob)
+    for name, v, hi in (("seed", seed, 2 ** 64), ("step", step, 2 ** 63)):
+        if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or not 0 <= int(v) < hi:
+            raise ValueError(f"{name} must be an int in [0, 2^{hi.bit_length() - 1}), got {v!r}")
+    if not isinstance(ids, Tensor) or ids.dtype != torch.int64 or ids.dim() != 1 or ids.numel() < 1 \
+            or ids.device.type != "cuda":
+        raise ValueError("ids must be a non-empty (B,) int64 tensor on a CUDA device")
+    ids = ids.contiguous()
+    b = ids.numel()
+    out = torch.empty(int(steps) - 1, b, dtype=torch.uint8, device=ids.device)
+    with torch.cuda.device(ids.device):
+        step_dev = torch.full((1,), int(step), dtype=torch.int64, device=ids.device)   # fill kernels, no copies
+        prob_dev = torch.full((1,), prob, dtype=torch.float32, device=ids.device)
+        st = C.c_void_p(torch.cuda.current_stream(ids.device).cuda_stream)
+        _lib.check(_lib.load().fno_teacher_flags(ids.data_ptr(), b, int(steps), prob_dev.data_ptr(), int(seed),
+                                                 step_dev.data_ptr(), None, out.data_ptr(), st), "fno_teacher_flags")
+    return out
+
+
 def index_batches(n: int, batch_size: int, shuffle: bool = False, generator=None,
                   drop_last: bool = False) -> Iterator[List[int]]:
     """The index batches one iteration of `DataLoader(dataset_of_len_n, batch_size, shuffle, generator=generator,

@@ -32,7 +32,7 @@ from torch import Tensor
 
 from . import _lib
 from .base_model import AutoCfdModel
-from .data import check_rollout_noise
+from .data import check_rollout_noise, check_teacher_forcing
 
 H = W = 64
 HIDDEN = 32
@@ -182,29 +182,30 @@ class _RolloutFn(torch.autograd.Function):
     native sweep, s = K-1 .. 0, that recomputes step s's saved set from its stored input frame and runs step s's backward
     with the upstream gradient dpreds_s + carry (carry = dL/d(frame fed to step s+1)), accumulating the parameter and
     case-parameter gradients.  Memory: the K+1 frames and one saved set instead of K saved sets.  With `noise` (a
-    RolloutNoise) the perturbed frames the steps were fed are kept as well, one more frame per step, and the sweep
-    recomputes from them."""
+    RolloutNoise) or `teacher` (a TeacherForcing) the frames the steps were fed are kept as well, one more frame per
+    step, and the sweep recomputes from them; with `teacher` it also keeps the flags, which gate the hand-off."""
 
     @staticmethod
-    def forward(ctx, model: "Fno2d", inputs: Tensor, mask: Tensor, case_params: Tensor, steps: int, noise, *params: Tensor):
+    def forward(ctx, model: "Fno2d", inputs: Tensor, mask: Tensor, case_params: Tensor, steps: int, noise, teacher,
+                *params: Tensor):
         _refuse_mask_grad(mask)
-        seq, fed = model._native_rollout_train(inputs, mask, case_params, steps, noise)
+        seq, fed = model._native_rollout_train(inputs, mask, case_params, steps, noise, teacher)
         ctx.model, ctx.steps, ctx.noise = model, steps, noise
-        ctx.save_for_backward(inputs, mask, case_params, seq, fed)
+        ctx.save_for_backward(inputs, mask, case_params, seq, fed, None if teacher is None else teacher.flags)
         return seq
 
     @staticmethod
     def backward(ctx, dseq: Tensor):
-        inputs, mask, case_params, seq, fed = ctx.saved_tensors
+        inputs, mask, case_params, seq, fed, flags = ctx.saved_tensors
         model: "Fno2d" = ctx.model
-        need = ctx.needs_input_grad   # (model, inputs, mask, case_params, steps, noise, *params)
+        need = ctx.needs_input_grad   # (model, inputs, mask, case_params, steps, noise, teacher, *params)
         d_inputs = torch.empty_like(inputs) if need[1] else None
         d_cp = torch.empty_like(case_params) if need[3] else None
         grads = model._native_rollout_backward(inputs, mask, case_params, seq, _lib.aligned(dseq.float()), ctx.steps,
-                                               any(need[6:]), d_inputs, d_cp, ctx.noise, fed)
+                                               any(need[7:]), d_inputs, d_cp, ctx.noise, fed, flags)
         if grads is None:
-            grads = [None] * (len(need) - 6)
-        return (None, d_inputs, None, d_cp, None, None, *grads)
+            grads = [None] * (len(need) - 7)
+        return (None, d_inputs, None, d_cp, None, None, None, *grads)
 
 
 class Fno2d(AutoCfdModel):
@@ -659,11 +660,21 @@ class Fno2d(AutoCfdModel):
         nio["ids"].copy_(noise.ids)
         nio["step"].fill_(noise.step)   # a fill kernel: no host-to-device copy
 
-    def _native_rollout_train(self, inputs: Tensor, mask4: Tensor, case_params: Tensor, steps: int, noise=None):
+    @staticmethod
+    def _teacher_io(frames: Optional[Tensor], flags: Tensor) -> dict:
+        """Graph-owned copies of a teacher's frames (None for the sweep, which reads only the flags) and flags, and the
+        fno_teacher descriptor pointing at them."""
+        io = dict(frames=None if frames is None else _lib.aligned(frames.clone()), flags=flags.clone())
+        io["desc"] = _lib.FnoTeacher(_ptr(io["frames"]), io["flags"].data_ptr())
+        return io
+
+    def _native_rollout_train(self, inputs: Tensor, mask4: Tensor, case_params: Tensor, steps: int, noise=None,
+                              teacher=None):
         """(preds, fed): preds (steps, B, 2, H, W) from fno_[grid_]rollout_forward_train: the training forward's kernels,
         so the predictions equal those of chained `generate` calls under autograd bit for bit.  fed is None, or with
         `noise` (a RolloutNoise) the (steps, B, 2, H, W) frames the steps were fed (fno_[grid_]rollout_forward_train_noise:
-        slot s holds step s's perturbed input when its stream k0 + s is at least 1)."""
+        slot s holds step s's perturbed input when its stream k0 + s is at least 1).  With `teacher` (a TeacherForcing)
+        the call is fno_[grid_]rollout_forward_train_feed and slot s >= 1 of fed always holds step s's input."""
         b = inputs.shape[0]
         route = self._route(*inputs.shape[-2:])
         gh, gw = route.gh, route.gw
@@ -671,10 +682,15 @@ class Fno2d(AutoCfdModel):
         ws, ws_bufs = self._workspace(b, route)
         rs = self._rollout_state(b, route)
         seq = torch.empty(steps, b, self.out_chan, gh, gw, dtype=torch.float32, device=self.device)
-        fed = None if noise is None else torch.empty_like(seq)
+        fed = None if noise is None and teacher is None else torch.empty_like(seq)
 
-        def call(st, x, mk, cp, out, nio, fd):
-            if nio is None:
+        def call(st, x, mk, cp, out, nio, tio, fd):
+            if tio is not None:
+                route.call("rollout_forward_train_feed", C.byref(st), x.data_ptr(), mk.data_ptr(), cp.data_ptr(),
+                           out.data_ptr(), steps, C.byref(rs["sv"]), C.byref(ws),
+                           None if nio is None else C.byref(nio["desc"]), C.byref(tio["desc"]), fd.data_ptr(), b,
+                           self._stream())
+            elif nio is None:
                 route.call("rollout_forward_train", C.byref(st), x.data_ptr(), mk.data_ptr(), cp.data_ptr(),
                            out.data_ptr(), steps, C.byref(rs["sv"]), C.byref(ws), b, self._stream())
             else:
@@ -682,21 +698,30 @@ class Fno2d(AutoCfdModel):
                            out.data_ptr(), steps, C.byref(rs["sv"]), C.byref(ws), C.byref(nio["desc"]), fd.data_ptr(), b,
                            self._stream())
         if not self.graph_rollout:
+            tio = None
+            if teacher is not None:
+                tio = dict(frames=teacher.frames, flags=teacher.flags)
+                tio["desc"] = _lib.FnoTeacher(teacher.frames.data_ptr(), teacher.flags.data_ptr())
             call(self._coords(pk, gh, gw)[0], inputs, mask4, case_params, seq,
-                 None if noise is None else self._noise_io(noise), fed)
+                 None if noise is None else self._noise_io(noise), tio, fed)
             return seq, fed
         key = ("fwd", b, steps, gh, gw, route.grid, self.act_dtype,
-               None if noise is None else (noise.std, noise.seed, noise.k0))
+               None if noise is None else (noise.std, noise.seed, noise.k0), teacher is not None)
 
         def make_io():
             io = dict(x=inputs.clone(), mk=mask4.clone(), cp=case_params.clone(), seq=torch.empty_like(seq),
-                      noise=None, fed=None)
+                      noise=None, teacher=None, fed=None)
             if noise is not None:
-                io["noise"], io["fed"] = self._noise_io(noise), torch.empty_like(seq)
+                io["noise"] = self._noise_io(noise)
+            if teacher is not None:
+                io["teacher"] = self._teacher_io(teacher.frames, teacher.flags)
+            if fed is not None:
+                io["fed"] = torch.empty_like(seq)
             return io
         ent = self._train_graph(
             key, pk, route, make_io,
-            lambda sw, io: call(sw["struct"], io["x"], io["mk"], io["cp"], io["seq"], io["noise"], io["fed"]),
+            lambda sw, io: call(sw["struct"], io["x"], io["mk"], io["cp"], io["seq"], io["noise"], io["teacher"],
+                                io["fed"]),
             (ws_bufs, rs))
         io = ent["io"]
         io["x"].copy_(inputs)
@@ -704,19 +729,23 @@ class Fno2d(AutoCfdModel):
         io["cp"].copy_(case_params)
         if noise is not None:
             self._refill_noise_io(io["noise"], noise)
+        if teacher is not None:
+            io["teacher"]["frames"].copy_(teacher.frames)
+            io["teacher"]["flags"].copy_(teacher.flags)
         ent["graph"].replay()
         seq.copy_(io["seq"])
-        if noise is not None:
+        if fed is not None:
             fed.copy_(io["fed"])
         return seq, fed
 
     def _native_rollout_backward(self, inputs, mask4, case_params, seq, dseq, steps: int, want_params: bool,
                                  d_inputs: Optional[Tensor], d_cp: Optional[Tensor], noise=None,
-                                 fed: Optional[Tensor] = None):
+                                 fed: Optional[Tensor] = None, flags: Optional[Tensor] = None):
         """One native sweep (fno_[grid_]rollout_backward): parameter gradients in parameter order (None when
         `want_params` is false), dL/dinputs into `d_inputs` and dL/dcase_params into `d_cp` when given.  With data
         parallel enabled the flat parameter-gradient buffer is all-reduced once.  With `noise` the sweep
-        (fno_[grid_]rollout_backward_noise) recomputes each noisy step from its frame in `fed`."""
+        (fno_[grid_]rollout_backward_noise) recomputes each noisy step from its frame in `fed`; with teacher `flags`
+        (fno_[grid_]rollout_backward_feed) every step s >= 1 from fed[s], and the flags gate the hand-off."""
         if self.n_case_params == 0:
             d_cp = None
         if not want_params and d_inputs is None and d_cp is None:
@@ -729,9 +758,14 @@ class Fno2d(AutoCfdModel):
         rs = self._rollout_state(b, route)
         carry = rs["bufs"]["carry"]
 
-        def call(st, sb, x, mk, cp, sq, dsq, g, din, dcp, nio, fd):
+        def call(st, sb, x, mk, cp, sq, dsq, g, din, dcp, nio, tio, fd):
             g = C.byref(g) if g is not None else None
-            if nio is None:
+            if tio is not None:
+                route.call("rollout_backward_feed", C.byref(st), C.byref(sb), x.data_ptr(), mk.data_ptr(),
+                           cp.data_ptr(), sq.data_ptr(), dsq.data_ptr(), steps, C.byref(rs["sv"]), g, C.byref(rs["sc"]),
+                           C.byref(ws), None if nio is None else C.byref(nio["desc"]), C.byref(tio["desc"]),
+                           fd.data_ptr(), carry.data_ptr(), _ptr(din), _ptr(dcp), b, self._stream())
+            elif nio is None:
                 route.call("rollout_backward", C.byref(st), C.byref(sb), x.data_ptr(), mk.data_ptr(), cp.data_ptr(),
                            sq.data_ptr(), dsq.data_ptr(), steps, C.byref(rs["sv"]), g, C.byref(rs["sc"]), C.byref(ws),
                            carry.data_ptr(), _ptr(din), _ptr(dcp), b, self._stream())
@@ -745,32 +779,41 @@ class Fno2d(AutoCfdModel):
             g = None
             if want_params:
                 flat, views, g = self._grad_buffers()
+            tio = None
+            if flags is not None:
+                tio = dict(flags=flags, desc=_lib.FnoTeacher(None, flags.data_ptr()))
             call(self._coords(pk, gh, gw)[0], pk["struct_bwd"], inputs, mask4, case_params, seq, dseq, g, d_inputs,
-                 d_cp, None if noise is None else self._noise_io(noise), fed)
+                 d_cp, None if noise is None else self._noise_io(noise), tio, fed)
         else:
             def make_io():
                 io = dict(x=inputs.clone(), mk=mask4.clone(), cp=case_params.clone(), seq=torch.empty_like(seq),
                           dseq=torch.empty_like(dseq), g=None,
                           din=torch.empty_like(d_inputs) if d_inputs is not None else None,
-                          dcp=torch.empty_like(d_cp) if d_cp is not None else None, noise=None, fed=None)
+                          dcp=torch.empty_like(d_cp) if d_cp is not None else None, noise=None, teacher=None, fed=None)
                 if want_params:
                     io["flat"], _, io["g"] = self._grad_buffers()
                 if noise is not None:
-                    io["noise"], io["fed"] = self._noise_io(noise), torch.empty_like(fed)
+                    io["noise"] = self._noise_io(noise)
+                if flags is not None:
+                    io["teacher"] = self._teacher_io(None, flags)
+                if fed is not None:
+                    io["fed"] = torch.empty_like(fed)
                 return io
             # the sweep draws no noise: of the descriptor it reads only k0 (the other fields, from the capturing call,
             # are checked and never read), so std, seed, step and ids do not key the capture
             key = ("bwd", b, steps, gh, gw, route.grid, self.act_dtype, want_params, d_inputs is not None,
-                   d_cp is not None, None if noise is None else noise.k0)
+                   d_cp is not None, None if noise is None else noise.k0, flags is not None)
             ent = self._train_graph(
                 key, pk, route, make_io,
                 lambda sw, io: call(sw["struct"], sw["struct_bwd"], io["x"], io["mk"], io["cp"], io["seq"], io["dseq"],
-                                    io["g"], io["din"], io["dcp"], io["noise"], io["fed"]), (ws_bufs, rs))
+                                    io["g"], io["din"], io["dcp"], io["noise"], io["teacher"], io["fed"]), (ws_bufs, rs))
             io = ent["io"]
             for k, t in (("x", inputs), ("mk", mask4), ("cp", case_params), ("seq", seq), ("dseq", dseq)):
                 io[k].copy_(t)
-            if noise is not None:
+            if fed is not None:
                 io["fed"].copy_(fed)
+            if flags is not None:
+                io["teacher"]["flags"].copy_(flags)
             ent["graph"].replay()
             if d_inputs is not None:
                 d_inputs.copy_(io["din"])
@@ -834,7 +877,8 @@ class Fno2d(AutoCfdModel):
                 seq = self._rollout_device(inputs, case_params, mask4, steps)
         return [seq[s] for s in range(steps)]
 
-    def rollout(self, inputs: Tensor, case_params: Tensor, mask: Optional[Tensor], steps: int, noise=None) -> Tensor:
+    def rollout(self, inputs: Tensor, case_params: Tensor, mask: Optional[Tensor], steps: int, noise=None,
+                teacher=None) -> Tensor:
         """`steps` autoregressive steps as one (steps, B, 2, H, W) float32 tensor, trainable through the whole rollout.
         Arguments as `generate_many` ((c,h,w) / (p,) / (h,w) inputs get a batch axis); every grid and storage mode of
         `forward`.  Step s is fed the (masked) prediction of step s-1, computed with the training forward's kernels, so
@@ -854,8 +898,18 @@ class Fno2d(AutoCfdModel):
         perturbed frame is the identity, so they and the gradients equal those of the chain of one-step `rollout`
         calls on frames perturbed with `add_input_noise`.  It costs one launch and keeps one more frame per noisy step.
         noise=None, or std 0, runs exactly what runs without it.  Raises ValueError for a malformed record (see
-        `check_rollout_noise`)."""
-        noise = check_rollout_noise(noise, inputs.shape[0] if inputs.dim() == 4 else 1, steps)
+        `check_rollout_noise`).
+
+        teacher = TeacherForcing(frames, flags) is scheduled sampling: step s >= 1 of sample b is fed the true frame
+        frames[s - 1][b] where flags[s - 1][b] is set, else the prediction of step s - 1 (with `noise`, the noise of
+        stream k0 + s is added to whichever frame was chosen).  It is a choice of frame: a forced sample's input never
+        depends on its prediction.  The gradient w.r.t. prediction s - 1 of a forced sample is then exactly the
+        loss's own, and nothing flows into `frames` (a `frames` that requires grad is refused).  With all flags 0 the
+        predictions and every gradient equal those without a teacher bit for bit.  It costs one launch and keeps one
+        more frame per step s >= 1.  Raises ValueError for a malformed record (see `check_teacher_forcing`)."""
+        batch = inputs.shape[0] if inputs.dim() == 4 else 1
+        noise = check_rollout_noise(noise, batch, steps)
+        teacher = check_teacher_forcing(teacher, batch, steps, *inputs.shape[-2:])
         self._require_cuda()
         if isinstance(steps, bool) or not isinstance(steps, int) or steps < 1:
             raise ValueError(f"steps must be a positive int; got {steps!r}")
@@ -865,11 +919,13 @@ class Fno2d(AutoCfdModel):
         inputs, case_params, mask4 = self._prep_inputs(inputs, case_params, mask)
         if noise is not None and noise.ids.device != self.device:
             raise ValueError(f"noise.ids is on {noise.ids.device}, the model on {self.device}")
+        if teacher is not None and teacher.frames.device != self.device:
+            raise ValueError(f"teacher.frames is on {teacher.frames.device}, the model on {self.device}")
         with torch.cuda.device(self.device):
             if self._needs_grad(inputs, case_params, mask4):
-                return _RolloutFn.apply(self, inputs, mask4, case_params, steps, noise, *self.parameters())
+                return _RolloutFn.apply(self, inputs, mask4, case_params, steps, noise, teacher, *self.parameters())
             with torch.no_grad():
-                return self._native_rollout_train(inputs, mask4, case_params, steps, noise)[0]
+                return self._native_rollout_train(inputs, mask4, case_params, steps, noise, teacher)[0]
 
     def _rollout_device(self, inputs, case_params, mask4, steps) -> Tensor:
         b = inputs.shape[0]

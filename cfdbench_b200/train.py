@@ -18,6 +18,7 @@ synchronisation.  The result is bit-identical to the eager loop `DeviceFrames.lo
     train_auto(..., rollout_steps=4, rollout_grad_steps=1, random_unroll=True)   # ... 0 to 3 of them, drawn per step
     train_auto(..., input_noise_std=0.01, noise_seed=1)      # Gaussian noise on every step's input frame
     train_auto(..., rollout_steps=4, input_noise_std=0.01, noise_every_step=True)   # ... and on every rollout step's
+    train_auto(..., rollout_steps=4, teacher_forcing=[1 - e / 99 for e in range(100)], num_epochs=100)   # scheduled sampling
     train_auto(..., resumable=True)   # relaunching the same call continues an interrupted run bit for bit
 """
 from __future__ import annotations
@@ -35,7 +36,7 @@ import torch
 
 from . import _lib, resume
 from .data import (DeviceFrames, _check_chain, _check_split, _gather, _positive_int, as_device_frames, check_noise_args,
-                   index_batches, split_windows)
+                   check_teacher_prob, index_batches, split_windows)
 from .fno2d import capture_graph, side_stream
 from .metrics import _evaluate_rollout, evaluate_auto
 from .optim import FusedAdam
@@ -92,6 +93,7 @@ class _StepGraphs:
     uses the first r samples' worth of every buffer.  The parameters and the optimizer state are read and written in
     place; the packed weight images are rebuilt inside the graph from the parameters as the previous replay's Adam
     left them."""
+    teacher = False   # _RolloutStepGraphs with teacher forcing: flags drawn on the device from Adam's step
 
     def __init__(self, model, frames: DeviceFrames, batch_size: int, optimizer, n: Optional[int] = None,
                  noise_std: float = 0.0, noise_seed: int = 0):
@@ -131,7 +133,8 @@ class _StepGraphs:
         if self.ema_decay is not None:
             self.io["ema_d"] = torch.empty(self.steps, dtype=torch.float32, device=dev)
             self.ema_host = torch.empty(self.steps, dtype=torch.float32, pin_memory=True)
-        if noise_std > 0:   # the epoch's first Adam step; a step's noise step is this plus the cursor
+        self.uses_step = noise_std > 0 or self.teacher
+        if self.uses_step:   # the epoch's first Adam step; a step's noise (and flag) step is this plus the cursor
             self.io["step_base"] = torch.zeros(1, dtype=torch.int64, device=dev)
             self.step_base_host = torch.empty(1, dtype=torch.int64, pin_memory=True)
         self.perm_host = torch.empty(n, dtype=torch.int64, pin_memory=True)
@@ -267,7 +270,7 @@ class _StepGraphs:
             _lib.check(self.lib.fno_ema_decays(self.ema_decay, first_step, self.steps, self.ema_host.data_ptr()),
                        "fno_ema_decays")
             io["ema_d"].copy_(self.ema_host, non_blocking=True)
-        if self.noise_std > 0:
+        if self.uses_step:
             self.step_base_host[0] = first_step
             io["step_base"].copy_(self.step_base_host, non_blocking=True)
         io["cursor"].zero_()
@@ -309,15 +312,25 @@ class _RolloutStepGraphs(_StepGraphs):
     random_unroll (g < k): Adam's step t runs u_t = unroll_lengths(unroll_seed, t, 1, k - g)[0] prefix steps instead of
     k - g, and trains steps u_t .. u_t + g - 1 of the window (u_t = 0: no prefix launch, the start frame is trained).
     One step is captured per u in 0 .. k - g and batch size, every capture on the same buffers (the prefix buffer holds
-    the longest prefix); the epoch replays the graph of each step's u_t."""
+    the longest prefix); the epoch replays the graph of each step's u_t.
+
+    teacher (g = k, scheduled sampling): after the gather, fno_teacher_flags draws the (k - 1, b) flags of the step
+    from the epoch's probability (a device float uploaded with the epoch's tables) and step = step_base + cursor; the
+    training forward and the sweep are the *_feed drivers, fed the gathered targets 0 .. k - 2 as the true frames.  A
+    (k, bmax, ...) fed-frame buffer and one more launch per rollout step, as every-step noise."""
 
     def __init__(self, model, frames: DeviceFrames, batch_size: int, optimizer, n_windows: int, steps: int,
                  time_step_size: int, grad_steps: Optional[int] = None, noise_std: float = 0.0, noise_seed: int = 0,
-                 noise_every_step: bool = False, random_unroll: bool = False, unroll_seed: int = 0):
+                 noise_every_step: bool = False, random_unroll: bool = False, unroll_seed: int = 0,
+                 teacher: bool = False, teacher_seed: int = 0):
         self.k, self.tss = steps, time_step_size
         self.g = steps if grad_steps is None else grad_steps
         self.every = noise_every_step and noise_std > 0
         self.random_unroll, self.unroll_seed = random_unroll, unroll_seed
+        self.teacher, self.teacher_seed = teacher, teacher_seed
+        if teacher:
+            assert self.g == steps > 1 and not random_unroll
+            self.prob_host = torch.zeros(1, dtype=torch.float32, pin_memory=True)
         super().__init__(model, frames, batch_size, optimizer, n=n_windows, noise_std=noise_std, noise_seed=noise_seed)
 
     def _make_io(self, bmax: int, gh: int, gw: int, p: int) -> dict:
@@ -336,12 +349,27 @@ class _RolloutStepGraphs(_StepGraphs):
             coef=torch.empty(self.steps, 2, **f32), log=torch.empty(self.steps, len(LOG_COLUMNS), **f32))
         if g < k:
             io["prefix"] = torch.empty(k - g, bmax, 2, gh, gw, **f32)
-        if self.every:
+        if self.every or self.teacher:
             io["fed"] = torch.empty(g, bmax, 2, gh, gw, **f32)
-            if g < k:
-                io["fed_prefix"] = torch.empty(k - g, bmax, 2, gh, gw, **f32)
+        if self.every and g < k:
+            io["fed_prefix"] = torch.empty(k - g, bmax, 2, gh, gw, **f32)
+        if self.teacher:
+            io["flags"] = torch.zeros(k - 1, bmax, dtype=torch.uint8, device=dev)
+            io["prob"] = torch.zeros(1, **f32)
         io["gout"][3:].fill_(1.0)
         return io
+
+    def _teacher(self):
+        """The fno_teacher of the step: the gathered targets 0 .. k - 2 and the step's flags, [k - 1][b] blocks."""
+        io = self.io
+        return C.byref(_lib.FnoTeacher(io["labels"].data_ptr(), io["flags"].data_ptr()))
+
+    def epoch(self, perm: np.ndarray, lr: float, first_step: int, teacher_prob: float = 0.0) -> np.ndarray:
+        """_StepGraphs.epoch; with teacher forcing the epoch's flags are drawn with probability `teacher_prob`."""
+        if self.teacher:   # the previous epoch's upload completed before its log came back
+            self.prob_host[0] = teacher_prob
+            self.io["prob"].copy_(self.prob_host, non_blocking=True)
+        return super().epoch(perm, lr, first_step)
 
     def _noise(self, k0: int):
         """The fno_noise of the step's rollout calls whose first step is window step k0: step = step_base + cursor,
@@ -379,6 +407,10 @@ class _RolloutStepGraphs(_StepGraphs):
         _gather(self.frames, io["idx"], b, io["inputs"], None, io["mask"], io["cp"], st,
                 window=(k, self.tss, io["labels"]))
         self._add_noise(b, st)
+        if self.teacher:
+            _lib.check(lib.fno_teacher_flags(io["idx"].data_ptr(), b, k, io["prob"].data_ptr(), self.teacher_seed,
+                                             io["step_base"].data_ptr(), io["cursor"].data_ptr(), io["flags"].data_ptr(),
+                                             st), "fno_teacher_flags")
         self._repack(st)
         x, mk, cp = io["inputs"].data_ptr(), io["mask"].data_ptr(), io["cp"].data_ptr()
         preds, labels, dpreds = io["preds"].data_ptr(), io["labels"].data_ptr(), io["dpreds"].data_ptr()
@@ -393,7 +425,10 @@ class _RolloutStepGraphs(_StepGraphs):
                 route.call("rollout", C.byref(sw["struct"]), x, mk, cp, pre, u, C.byref(ws), b, st)
             x = pre + (u - 1) * n_el * 4
             labels += u * n_el * 4
-        if self.every:
+        if self.teacher:
+            route.call("rollout_forward_train_feed", C.byref(sw["struct"]), x, mk, cp, preds, g, C.byref(ts["sv"]),
+                       C.byref(ws), self._noise(u) if self.every else None, self._teacher(), io["fed"].data_ptr(), b, st)
+        elif self.every:
             route.call("rollout_forward_train_noise", C.byref(sw["struct"]), x, mk, cp, preds, g, C.byref(ts["sv"]),
                        C.byref(ws), self._noise(u), io["fed"].data_ptr(), b, st)
         else:
@@ -403,7 +438,12 @@ class _RolloutStepGraphs(_StepGraphs):
                    "fno_loss_seq_fwd")
         _lib.check(lib.fno_loss_seq_bwd(preds, labels, io["loss"].data_ptr(), io["gout"].data_ptr(), dpreds, n_el, g, st),
                    "fno_loss_seq_bwd")
-        if self.every:
+        if self.teacher:
+            route.call("rollout_backward_feed", C.byref(sw["struct"]), C.byref(sw["struct_bwd"]), x, mk, cp, preds,
+                       dpreds, g, C.byref(ts["sv"]), C.byref(self.grads), C.byref(ts["sc"]), C.byref(ws),
+                       self._noise(u) if self.every else None, self._teacher(), io["fed"].data_ptr(),
+                       io["carry"].data_ptr(), None, None, b, st)
+        elif self.every:
             route.call("rollout_backward_noise", C.byref(sw["struct"]), C.byref(sw["struct_bwd"]), x, mk, cp, preds,
                        dpreds, g, C.byref(ts["sv"]), C.byref(self.grads), C.byref(ts["sc"]), C.byref(ws),
                        self._noise(u), io["fed"].data_ptr(), io["carry"].data_ptr(), None, None, b, st)
@@ -416,6 +456,48 @@ class _RolloutStepGraphs(_StepGraphs):
 
 
 # ------------------------------------------------------------------------------------------------ train_auto
+def _teacher_record(teacher_forcing):
+    """teacher_forcing as plain Python values for the resume record: a float, or a list of floats."""
+    if isinstance(teacher_forcing, (int, float, np.integer, np.floating)):
+        return float(teacher_forcing)
+    return [float(v) for v in teacher_forcing]
+
+
+def teacher_schedule(teacher_forcing, num_epochs: int, teacher_seed, rollout_steps: int, grad_steps: int,
+                     random_unroll: bool) -> Optional[List[float]]:
+    """The per-epoch teacher-forcing probabilities of `train_auto(teacher_forcing=..., teacher_seed=...)`: None when
+    teacher forcing is off (None, or 0 in every epoch: the call runs what runs without it), else num_epochs floats.
+    ValueError, naming the argument, for a value that is not a real in [0, 1], a sequence shorter than num_epochs, a
+    teacher_seed that is not an int in [0, 2^64), or teacher forcing with rollout_steps = 1, pushforward
+    (rollout_grad_steps < rollout_steps) or random_unroll."""
+    if isinstance(teacher_seed, bool) or not isinstance(teacher_seed, (int, np.integer)) \
+            or not 0 <= int(teacher_seed) < 2 ** 64:
+        raise ValueError(f"teacher_seed must be an int in [0, 2^64), got {teacher_seed!r}")
+    if teacher_forcing is None:
+        return None
+    if isinstance(teacher_forcing, (bool, str, bytes)):
+        raise ValueError(f"teacher_forcing must be None, a real in [0, 1] or a sequence of them, got {teacher_forcing!r}")
+    if isinstance(teacher_forcing, (int, float, np.integer, np.floating)):
+        probs = [check_teacher_prob(teacher_forcing, "teacher_forcing")] * num_epochs
+    else:
+        try:
+            values = list(teacher_forcing)
+        except TypeError:
+            raise ValueError(f"teacher_forcing must be None, a real in [0, 1] or a sequence of them, got "
+                             f"{teacher_forcing!r}") from None
+        if len(values) < num_epochs:
+            raise ValueError(f"teacher_forcing has {len(values)} values, fewer than num_epochs={num_epochs} (one per "
+                             "epoch)")
+        probs = [check_teacher_prob(v, f"teacher_forcing[{i}]") for i, v in enumerate(values)][:num_epochs]
+    if rollout_steps < 2:
+        raise ValueError("teacher_forcing chooses what rollout steps 1 .. K - 1 are fed: it needs rollout_steps > 1")
+    if grad_steps < rollout_steps or random_unroll:
+        raise ValueError(f"teacher_forcing does not combine with pushforward training: it needs rollout_grad_steps = "
+                         f"rollout_steps and random_unroll=False, got rollout_grad_steps={grad_steps}, "
+                         f"random_unroll={random_unroll}")
+    return probs if any(p > 0 for p in probs) else None
+
+
 def _ema_shadow(model):
     """A Fno2d with `model`'s configuration, storage mode, device and kernel choices, holding a copy of its weights: the
     model the EMA weights are evaluated and saved through.  Built without drawing from the CPU RNG (the parameters'
@@ -438,7 +520,7 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
                rollout_grad_steps: Optional[int] = None, noise_every_step: bool = False,
                dev_rollout_steps: Optional[int] = None, max_grad_norm: Optional[float] = None,
                ema_decay: Optional[float] = None, resumable: bool = False, random_unroll: bool = False,
-               unroll_seed: int = 0) -> dict:
+               unroll_seed: int = 0, teacher_forcing=None, teacher_seed: int = 0) -> dict:
     """What the reference's `train(model, train_data, dev_data, output_dir, ...)` does (src/train_auto.py:181-313), with
     its argument names and defaults, every training step replayed from a CUDA graph and one synchronisation per epoch.
 
@@ -515,6 +597,24 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
           seq = model.rollout(x, b["case_params"], b["mask"], G, noise=RolloutNoise(sigma, noise_seed, t, ids, K - G))
           loss = sum(model.loss_fn(preds=seq[g], labels=b["labels"][K - G + g])["nmse"] for g in range(G)) / G
 
+    - teacher_forcing = p (a real in [0, 1], or a sequence of at least num_epochs of them, one per epoch) is scheduled
+      sampling (Bengio et al. 2015) over the K-step window (needs K > 1 and no pushforward): rollout step s >= 1 of a
+      window is fed the true frame, the masked target of step s - 1, with probability p, else the model's prediction
+      of step s - 1.  The flags are drawn on the device per window and step from `teacher_seed` and Adam's step
+      (`teacher_forcing_flags`); p reaches the device with each epoch's uploads.  The gradient through a forced step's
+      input is cut: prediction s - 1 of a forced window gets the loss's gradient alone.  With noise_every_step the
+      noise of stream s is added to whichever frame was chosen.  It costs one launch and one frame per sample per
+      rollout step.  None, or p = 0 in every epoch, runs exactly what runs without it.  One step is bit-identical to
+      the eager loop (p the epoch's value)
+
+          b = frames.rollout_batch(idx, K, noise_std=sigma, noise_seed=noise_seed, noise_step=t)
+          ids = torch.as_tensor(idx, device=b["inputs"].device)
+          flags = teacher_forcing_flags(ids, K, p, teacher_seed, t)
+          noise = RolloutNoise(sigma, noise_seed, t, ids, 0) if noise_every_step else None
+          seq = model.rollout(b["inputs"], b["case_params"], b["mask"], K, noise=noise,
+                              teacher=TeacherForcing(b["labels"][:K - 1], flags))
+          loss = sum(model.loss_fn(preds=seq[k], labels=b["labels"][k])["nmse"] for k in range(K)) / K
+
     - dev_rollout_steps = S selects checkpoints by rollout error: every evaluation also runs
       `evaluate_rollout_auto(model, <DeviceFrames of dev_data>, S, time_step_size)` -- every S-step window of the dev
       split rolled out from its start sample, step k against the frame k + 1 time steps on -- writes its result to
@@ -571,7 +671,9 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
     training_state.pt that does not load, has another format version or was written with another config (naming every
     differing field), or for an output_dir with ckpt-* directories and no training_state.pt; ValueError for a
     resumable that is not a bool; for a random_unroll that is not a bool, an unroll_seed that is not an int >= 0, or
-    random_unroll=True with rollout_steps = 1 or rollout_grad_steps = rollout_steps.
+    random_unroll=True with rollout_steps = 1 or rollout_grad_steps = rollout_steps; for a teacher_forcing that is not
+    None, a real in [0, 1] or a sequence of at least num_epochs of them, a teacher_seed that is not an int in
+    [0, 2^64), or teacher_forcing with rollout_steps = 1, rollout_grad_steps < rollout_steps or random_unroll.
     Frozen parameters (requires_grad=False) are not updated, as FusedAdam.step skips them.  Data parallel training in
     this loop is not supported."""
     from .fno2d import Fno2d
@@ -605,6 +707,7 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
         raise ValueError(f"random_unroll draws the pushforward prefix length: it needs rollout_steps > 1 and "
                          f"rollout_grad_steps < rollout_steps, got rollout_steps={rollout_steps}, "
                          f"rollout_grad_steps={rollout_grad_steps!r}")
+    teacher_probs = teacher_schedule(teacher_forcing, num_epochs, teacher_seed, rollout_steps, grad_steps, random_unroll)
     if model._dp_enabled:
         raise ValueError("train_auto does not run data parallel: its step graph has no all-reduce")
     if not any(p.requires_grad for p in model.parameters()):
@@ -634,6 +737,8 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
             ema_decay=ema_decay, generator=generator is not None)
         if random_unroll:   # recorded only when set: a fixed-prefix run's record is that of earlier versions
             config.update(random_unroll=True, unroll_seed=int(unroll_seed))
+        if teacher_forcing is not None:   # likewise
+            config.update(teacher_forcing=_teacher_record(teacher_forcing), teacher_seed=int(teacher_seed))
         state = resume.find_state(output_dir, config)
     model._require_cuda()
     output_dir = Path(output_dir)
@@ -669,7 +774,8 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
             else:
                 graphs = _RolloutStepGraphs(model, frames, batch_size, optimizer, windows.size, rollout_steps,
                                             tss, grad_steps, noise_every_step=noise_every_step,
-                                            random_unroll=random_unroll, unroll_seed=int(unroll_seed), **noise)
+                                            random_unroll=random_unroll, unroll_seed=int(unroll_seed),
+                                            teacher=teacher_probs is not None, teacher_seed=int(teacher_seed), **noise)
         print("====== Training ======")
         print(f"# batch: {batch_size}")
         print(f"# examples: {n}")
@@ -681,6 +787,9 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
                           f"steps (pushforward, unroll seed {int(unroll_seed)})")
                 else:
                     print(f"# trained steps: the last {grad_steps} (pushforward)")
+        if teacher_probs is not None:
+            print(f"# teacher forcing: p = {teacher_probs[0]} .. {teacher_probs[-1]} over the epochs, seed "
+                  f"{int(teacher_seed)}")
         if input_noise_std > 0:
             every = ", on every rollout step" if noise_every_step and windows is not None else ""
             print(f"# input noise std: {input_noise_std}, seed {int(noise_seed)}{every}")
@@ -704,7 +813,10 @@ def train_auto(model, train_data, dev_data, output_dir, num_epochs: int = 400, l
                     perm = epoch_permutation(n, batch_size, generator)
                 else:
                     perm = windows[epoch_permutation(windows.size, batch_size, generator)]
-                log = graphs.epoch(perm, lr_ep, global_step + 1)
+                if teacher_probs is not None:
+                    log = graphs.epoch(perm, lr_ep, global_step + 1, teacher_prob=teacher_probs[ep])
+                else:
+                    log = graphs.epoch(perm, lr_ep, global_step + 1)
                 ep_train_losses = [float(v) for v in log[:, 3]]
                 if max_grad_norm is not None:
                     grad_norms += [float(v) for v in graphs.norms]

@@ -418,6 +418,46 @@ int fno_rollout_backward_noise(const fno_weights* w, const fno_weights_bwd* wb, 
                                const fno_workspace* ws, const fno_noise* noise, const float* fed, float* carry,
                                float* d_inputs, float* d_case_params, int batch, int act_dtype, void* stream);
 
+/* ---- teacher forcing of a rollout (train_auto(teacher_forcing=...), Fno2d.rollout(teacher=...)) -------------------
+ * Scheduled sampling: rollout step s >= 1 of a window is fed the true frame of step s - 1 instead of the model's
+ * prediction where a per-sample flag is set.
+ * fno_teacher_flags: flags[s-1][i] = (u <= *prob) for s = 1 .. steps - 1 and i < batch (uint8 0 / 1), u = the uniform
+ * of fno_add_input_noise's RNG, x0 2^-32 + 2^-33 in float32, from word x0 of Philox4x32-10(counter = (s, j,
+ * step & 0xffffffff, step >> 32), key = (seed & 0xffffffff, seed >> 32)), j = idx[i]: a pure function of (seed, step, j,
+ * s).  u lies in (0, 1], so *prob = 0 sets no flag and *prob = 1 every flag.  prob (float32) and step = *step_base +
+ * *step_offset (step_offset may be NULL for 0) are read on the device when the kernel runs.  Status 1 for a null pointer
+ * (other than step_offset), batch <= 0, steps < 2 or steps > 2^16.
+ * The *_feed rollout drivers take a nullable noise descriptor (as the *_noise drivers) and a teacher descriptor:
+ * frames [steps-1][B][2][H][W] float32 (the true frames, typically the masked window targets of steps 0 .. steps - 2)
+ * and flags [steps-1][B].  The forward writes fed[s] = (flags[s-1][b] ? frames[s-1][b] : preds_seq[s-1][b]) for every
+ * s >= 1 with one launch (plus the noise of stream k0 + s with a noise descriptor, as the *_noise drivers; a step 0 with
+ * k0 >= 1 is fed as there) -- a choice of frame: a forced sample's fed frame never reads its prediction.  The backward
+ * recomputes step s >= 1 from fed[s] and hands prediction s - 1 of a forced sample exactly dpreds_seq[s-1] (bit for bit;
+ * nothing of step s's input gradient) and of any other sample fc0^T dL/da0 + dpreds_seq[s-1]; the parameter and
+ * case-parameter gradients take every step's share as without a teacher.  Of the descriptor the backward reads only
+ * flags (frames may be NULL there).  Every other argument and status code as the driver without a teacher; status 1
+ * (before any device work) for a null teacher descriptor, fed or flags, or null frames in a forward driver. */
+typedef struct fno_teacher {
+  const float* frames;   /* [steps-1][B][2][H][W] */
+  const uint8_t* flags;  /* [steps-1][B] */
+} fno_teacher;
+/* The status the teacher-forcing entry points return: 0, or the codes of the int-returning entry points above.  Their
+ * pointer arguments' alignment contract is tested in tests/test_teacher_forcing_host.py: idx and step_base 8 bytes,
+ * prob and step_offset 4; the *_feed drivers as the matching *_noise driver, teacher->frames 4 (float4 only where the
+ * frames of a feed are 16-byte aligned), flags 1. */
+typedef int fno_status;
+fno_status fno_teacher_flags(const int64_t* idx, int batch, int steps, const float* prob, uint64_t seed, const int64_t* step_base,
+                      const int32_t* step_offset, uint8_t* flags, void* stream);
+fno_status fno_rollout_forward_train_feed(const fno_weights* w, const float* inputs, const float* mask, const float* case_params,
+                                   float* preds_seq, int steps, const fno_train_saved* saved, const fno_workspace* ws,
+                                   const fno_noise* noise, const fno_teacher* teacher, float* fed, int batch, int act_dtype,
+                                   void* stream);
+fno_status fno_rollout_backward_feed(const fno_weights* w, const fno_weights_bwd* wb, const float* inputs, const float* mask,
+                              const float* case_params, const float* preds_seq, const float* dpreds_seq, int steps,
+                              const fno_train_saved* saved, const fno_grads* grads, const fno_bwd_scratch* scratch,
+                              const fno_workspace* ws, const fno_noise* noise, const fno_teacher* teacher, const float* fed,
+                              float* carry, float* d_inputs, float* d_case_params, int batch, int act_dtype, void* stream);
+
 /* ---------------------------------------------------------------------------------------------------
  * Grid-generic path: the same network on H x W frames with 24 <= H <= 128 and 24 <= W <= 128, e.g. CFDBench's
  * tube and dam problems (66 x 65, reference src/utils/autoregressive.py:24-26).  fp32 activation storage only (there is
@@ -488,6 +528,17 @@ int fno_grid_rollout_backward_noise(const fno_weights* w, const fno_weights_bwd*
                                     const fno_train_saved* saved, const fno_grads* grads, const fno_bwd_scratch* scratch,
                                     const fno_workspace* ws, const fno_noise* noise, const float* fed, float* carry,
                                     float* d_inputs, float* d_case_params, int batch, int h, int w_, void* stream);
+/* the *_feed rollout drivers (above) on an H x W grid */
+fno_status fno_grid_rollout_forward_train_feed(const fno_weights* w, const float* inputs, const float* mask,
+                                        const float* case_params, float* preds_seq, int steps, const fno_train_saved* saved,
+                                        const fno_workspace* ws, const fno_noise* noise, const fno_teacher* teacher, float* fed,
+                                        int batch, int h, int w_, void* stream);
+fno_status fno_grid_rollout_backward_feed(const fno_weights* w, const fno_weights_bwd* wb, const float* inputs, const float* mask,
+                                   const float* case_params, const float* preds_seq, const float* dpreds_seq, int steps,
+                                   const fno_train_saved* saved, const fno_grads* grads, const fno_bwd_scratch* scratch,
+                                   const fno_workspace* ws, const fno_noise* noise, const fno_teacher* teacher,
+                                   const float* fed, float* carry, float* d_inputs, float* d_case_params, int batch, int h,
+                                   int w_, void* stream);
 /* fno_multistep_metrics on an H x W grid: preds_seq [S][B][2][H][W], label_u and mask [S][B][H][W]; sums [S][B][3] as
  * there (sums over the H*W pixels).  One CTA per (step, case) plane, fixed-order reduction: bit-reproducible.
  * steps <= 65535. */
